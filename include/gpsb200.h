@@ -258,7 +258,9 @@ int gpsb200_codegen(int prn, uint8_t ca[GPSB200_CA_LEN]);
  * gps.c:1131-1505, satpos/computeRange/ionosphericDelay gps.c:508-611,1893-2026,
  * computeCodePhase gps.c:2033-2064, eph2sbf/generateNavMsg/computeChecksum gps.c:617-884,
  * 1008-1072,2066-2140, allocateChannel gps.c:2142-2235, the 10 Hz / 30 s loop gps.c:2703-2765,
- * 2870-2932). Almanac pages are not generated (reference run with its almanac disabled). */
+ * 2870-2932). With almanac_file set, the almanac of a SEM file goes into subframes 4 and 5 as the reference sends it
+ * by default (SEM reader almanac.c:73-184, pages gps.c:772-883, time check gps.c:2637-2651); without one, the pages
+ * are those of the reference run with --disable-almanac. */
 typedef struct gpsb200_scenario_config {
     const char *nav_file;          /* -e: RINEX v2 (or, with rinex3, v3) navigation file */
     const char *motion_file;       /* -m: ECEF motion csv "t,x,y,z" at 10 Hz, NULL = static */
@@ -274,6 +276,12 @@ typedef struct gpsb200_scenario_config {
      * [m] and bearing [deg] from the location, height offset [m]; ignored with a motion file, as in the reference */
     int32_t target_valid, reserved;
     double target_distance_m, target_bearing_deg, target_height_m;
+    /* SEM almanac file sent in subframe 4 pages 2-5/7-10 (PRN 25-32) and subframe 5 pages 1-25 (PRN 1-24, toa/WNa);
+     * NULL = no almanac (the reference's --disable-almanac). Read as the reference reads ./almanac.sem: at most 32
+     * records, records parsed before the end of the file are kept (a partly read last record too), any other parse
+     * error drops the whole almanac. A file that cannot be opened, or a record whose toa is more than 4 weeks from
+     * the scenario start (a file with the full week number instead of week modulo 1024), is an error. */
+    const char *almanac_file;
 } gpsb200_scenario_config_t;
 typedef struct gpsb200_scenario gpsb200_scenario_t;
 
@@ -285,6 +293,22 @@ int gpsb200_scenario_channels(const gpsb200_scenario_t *s);
 int gpsb200_scenario_nav_frames(const gpsb200_scenario_t *s);
 const gpsb200_chan_t *gpsb200_scenario_chans(const gpsb200_scenario_t *s);   /* [blocks][channels] */
 const uint32_t *gpsb200_scenario_nav(const gpsb200_scenario_t *s);           /* [frames][channels][60] */
+/* Time of applicability of the almanac in use as "yyyy/mm/dd,hh:mm:ss" (the last valid record's, gps.c:2644-2654), or
+ * NULL when no valid record was read (no almanac_file, or nothing usable in it). */
+const char *gpsb200_scenario_almanac_date(const gpsb200_scenario_t *s);
+
+/* One SEM almanac record as the scenario engine reads it (the reference's almanac_prn_t, almanac.h:21-38). */
+typedef struct gpsb200_almanac_record {
+    int32_t svid;          /* 1..32 (file id 0 reads as 1, above 32 as 32); 0 = no record */
+    int32_t svn, ura, health, config_code;   /* ura <= 15, health <= 63, config_code <= 15 */
+    int32_t valid;         /* 1 = all lines read; svid != 0 with valid == 0: the record the file ended in */
+    int32_t toa_week;      /* file week + 2048 */
+    int32_t reserved;
+    double e, delta_i, omegadot, sqrta, omega0, aop, m0, af0, af1, toa_sec;
+} gpsb200_almanac_record_t;
+/* Parse a SEM file into rec[0..31] (indexed by svid - 1); *valid = 1 when at least one record is complete. Returns
+ * GPSB200_ERR_ARG when the file cannot be opened. For tests (the parser against the reference's, field by field). */
+int gpsb200_almanac_read(const char *path, gpsb200_almanac_record_t rec[32], int32_t *valid);
 
 /* ---- FIFO / sink boundary: the reference's own API (fifo.h:19-62) --------------
  * Guarded by the reference header's own include guard (fifo.h:13-14), so that a translation unit of the reference

@@ -50,7 +50,15 @@ class ScenarioConfig(C.Structure):
                 ("start_year", C.c_int32), ("start_month", C.c_int32), ("start_day", C.c_int32),
                 ("start_hour", C.c_int32), ("start_min", C.c_int32), ("rinex3", C.c_int32),
                 ("start_sec", C.c_double), ("target_valid", C.c_int32), ("reserved", C.c_int32),
-                ("target_distance_m", C.c_double), ("target_bearing_deg", C.c_double), ("target_height_m", C.c_double)]
+                ("target_distance_m", C.c_double), ("target_bearing_deg", C.c_double), ("target_height_m", C.c_double),
+                ("almanac_file", C.c_char_p)]
+
+
+ALMANAC_RECORD_DTYPE = np.dtype([("svid", "<i4"), ("svn", "<i4"), ("ura", "<i4"), ("health", "<i4"), ("config_code", "<i4"),
+                                 ("valid", "<i4"), ("toa_week", "<i4"), ("reserved", "<i4"),
+                                 ("e", "<f8"), ("delta_i", "<f8"), ("omegadot", "<f8"), ("sqrta", "<f8"), ("omega0", "<f8"),
+                                 ("aop", "<f8"), ("m0", "<f8"), ("af0", "<f8"), ("af1", "<f8"), ("toa_sec", "<f8")])
+assert ALMANAC_RECORD_DTYPE.itemsize == 112          # gpsb200_almanac_record_t
 
 
 class SliceLink(C.Structure):
@@ -78,7 +86,7 @@ EXPORTS = ["gpsb200_create", "gpsb200_destroy", "gpsb200_last_error", "gpsb200_v
            "gpsb200_slice_finish", "gpsb200_slice_finish_cb", "gpsb200_slice_wait", "gpsb200_link_apply", "gpsb200_slice_link_host", "gpsb200_debug_corrupt_chain", "gpsb200_synth_kernel_name",
            "gpsb200_scenario_create", "gpsb200_scenario_destroy", "gpsb200_scenario_error",
            "gpsb200_scenario_blocks", "gpsb200_scenario_channels", "gpsb200_scenario_nav_frames",
-           "gpsb200_scenario_chans", "gpsb200_scenario_nav",
+           "gpsb200_scenario_chans", "gpsb200_scenario_nav", "gpsb200_scenario_almanac_date", "gpsb200_almanac_read",
            "fifo_create", "fifo_destroy", "fifo_wait_next", "fifo_wait_full", "fifo_halt", "fifo_acquire",
            "fifo_enqueue", "fifo_dequeue", "fifo_release", "fifo_set_compat_drop",
            "gpsb200_iqfile_start", "gpsb200_iqfile_stop", "gpsb200_fifo_push", "gpsb200_fifo_push_flush"]
@@ -114,6 +122,9 @@ def lib():
         L.gpsb200_scenario_chans.restype = C.c_void_p
         L.gpsb200_scenario_nav.argtypes = [C.c_void_p]
         L.gpsb200_scenario_nav.restype = C.c_void_p
+        L.gpsb200_scenario_almanac_date.argtypes = [C.c_void_p]
+        L.gpsb200_scenario_almanac_date.restype = C.c_char_p
+        L.gpsb200_almanac_read.argtypes = [C.c_char_p, C.c_void_p, C.POINTER(C.c_int32)]
         L.gpsb200_carrier_probe_fixup.argtypes = [C.c_double, C.c_double, C.c_double, C.c_int64, C.POINTER(C.c_double)]
         L.gpsb200_carrier_chain_device.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p]
         L.gpsb200_carrier_chain.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int]
@@ -217,10 +228,23 @@ def link_apply(link, nchan, prn_in=None, phase_in=None):
     return po, xo
 
 
+def almanac_read(path):
+    """gpsb200_almanac_read: parse a SEM almanac file as the scenario engine does.
+    -> (valid, records ALMANAC_RECORD_DTYPE[32] indexed by PRN - 1)"""
+    rec = np.zeros(32, ALMANAC_RECORD_DTYPE)
+    valid = C.c_int32(0)
+    rc = lib().gpsb200_almanac_read(os.fsencode(path), rec.ctypes.data, C.byref(valid))
+    if rc:
+        raise GpsB200Error(rc, "cannot open almanac file %s" % path)
+    return bool(valid.value), rec
+
+
 def scenario(nav_file, lat, lon, height, seconds, max_chan=12, motion_file=None, start=None,
-             ionosphere=True, pluto_gain=False, rinex3=False, target=None):
+             ionosphere=True, pluto_gain=False, rinex3=False, target=None, almanac_file=None, info=None):
     """Run the host scenario engine. -> (chans[nblk, max_chan] CHAN_DTYPE, nav[nframes, max_chan, 60] uint32).
-    start: (y, m, d, hh, mm, sec) or None for the first ephemeris epoch."""
+    start: (y, m, d, hh, mm, sec) or None for the first ephemeris epoch. almanac_file: SEM almanac to transmit in
+    subframes 4 and 5 (None: no almanac, the reference's --disable-almanac). info: optional dict that receives
+    "almanac_date" ("yyyy/mm/dd,hh:mm:ss", or None when no valid almanac record was read)."""
     cfg = ScenarioConfig()
     cfg.nav_file = os.fsencode(nav_file)
     cfg.motion_file = os.fsencode(motion_file) if motion_file else None
@@ -230,6 +254,7 @@ def scenario(nav_file, lat, lon, height, seconds, max_chan=12, motion_file=None,
     cfg.ionosphere_enable = 1 if ionosphere else 0
     cfg.pluto_gain = 1 if pluto_gain else 0
     cfg.rinex3 = 1 if rinex3 else 0
+    cfg.almanac_file = os.fsencode(almanac_file) if almanac_file else None
     if target is not None:          # -t distance,bearing,height
         cfg.target_valid = 1
         cfg.target_distance_m, cfg.target_bearing_deg, cfg.target_height_m = [float(v) for v in target]
@@ -246,6 +271,9 @@ def scenario(nav_file, lat, lon, height, seconds, max_chan=12, motion_file=None,
                           L.gpsb200_scenario_nav_frames(h))
         chans = np.frombuffer(C.string_at(L.gpsb200_scenario_chans(h), nblk * nch * 64), dtype=CHAN_DTYPE)
         nav = np.frombuffer(C.string_at(L.gpsb200_scenario_nav(h), nfr * nch * 60 * 4), dtype=np.uint32)
+        if info is not None:
+            d = L.gpsb200_scenario_almanac_date(h)
+            info["almanac_date"] = d.decode() if d else None
         return chans.reshape(nblk, nch).copy(), nav.reshape(nfr, nch, 60).copy()
     finally:
         if h:

@@ -6,18 +6,20 @@
 //   satellite position, range, Klobuchar delay (gps.c:508-611, 1893-2026)
 //   code phase / NAV position  (gps.c:2033-2064)
 //   subframes, parity, 30 s NAV frames (gps.c:617-884, 1008-1072, 2066-2140)
+//   SEM almanac reader + almanac pages (behaviour of almanac.c:73-184, gps.c:772-883, 2637-2657)
 //   visibility + channel allocation (gps.c:2142-2235), 10 Hz loop (gps.c:2703-2765, 2870-2932)
 // These are rows f1/f2/f4 of SURVEY.md section 8 ("next" after the sample loop). The
 // doubles feed the CUDA kernels bit for bit, so every expression keeps the reference's
 // evaluation order (no FMA contraction: -ffp-contract=off) and the same libm calls;
 // tests/test_scenario.py compares every field with the reference's own dumps.
 //
-// Scope notes: almanac pages are not generated (the reference run with its almanac
-// disabled, as in all BASELINE configs); downloads, interactive motion and
-// the HackRF/Pluto specifics (except the Pluto gain doubling) are out of scope.
+// Scope notes: the almanac comes from a SEM file the caller names (the reference reads ./almanac.sem implicitly;
+// without a file the pages are the reference's with --disable-almanac, as in all BASELINE configs); downloads,
+// interactive motion and the HackRF/Pluto specifics (except the Pluto gain doubling) are out of scope.
 #include <algorithm>
 #include <cmath>
 #include <cstdio>
+#include <cstddef>
 #include <cstdlib>
 #include <cstring>
 #include <functional>
@@ -45,6 +47,10 @@ constexpr double P2_5 = 0.03125, P2_19 = 1.907348632812500e-6, P2_29 = 1.8626451
                  P2_31 = 4.656612873077393e-10, P2_33 = 1.164153218269348e-10, P2_43 = 1.136868377216160e-13,
                  P2_55 = 2.775557561562891e-17, P2_50 = 8.881784197001252e-016, P2_30 = 9.313225746154785e-010,
                  P2_27 = 7.450580596923828e-009, P2_24 = 5.960464477539063e-008;
+// almanac scale factors (gps.h:79-84): P2_38 and P2_23 are not exact powers of two, P2p12 is an int
+constexpr double P2_21 = 4.76837158203125e-007, P2_38 = 3.63797880709171e-012, P2_11 = 0.00048828125,
+                 P2_23 = 1.19209289550781e-007, P2_20 = 9.5367431640625e-007;
+constexpr int P2p12 = 4096;
 // receiver antenna attenuation in dB per 5 deg of boresight angle (gps.c:215-220)
 const double kAntPatDb[37] = {0.00,  0.00,  0.22,  0.44,  0.67,  1.11,  1.56,  2.00,  2.44,  2.89,  3.56,  4.22,  4.89,
                               5.56,  6.22,  6.89,  7.56,  8.22,  8.89,  9.78,  10.67, 11.56, 12.44, 13.33, 14.44, 15.56,
@@ -116,6 +122,22 @@ GpsTime gps_add(const GpsTime &g0, double dt) {
         g.week--;
     }
     return g;
+}
+
+// gps.c:339-355
+Date gps_to_date(const GpsTime &g) {
+    const int c = (int) (7 * g.week + floor(g.sec / 86400.0) + 2444245.0) + 1537;
+    const int d = (int) ((c - 122.1) / 365.25);
+    const int e = 365 * d + d / 4;
+    const int f = (int) ((c - e) / 30.6001);
+    Date t;
+    t.d = c - e - (int) (30.6001 * f);
+    t.m = f - 1 - 12 * (f / 14);
+    t.y = d - 4715 - ((7 + t.m) / 10);
+    t.hh = ((int) (g.sec / 3600.0)) % 24;
+    t.mm = ((int) (g.sec / 60.0)) % 60;
+    t.sec = g.sec - 60.0 * floor(g.sec / 60.0);
+    return t;
 }
 
 // ---- coordinates (gps.c:361-499) ----------------------------------------------------------
@@ -305,8 +327,72 @@ uint32_t nav_word(uint32_t source, bool nib) {
     return D;
 }
 
-// ---- subframes 1-3 + dummy pages of 4/5 (gps.c:617-884, almanac absent) -----------------------------------
-void build_subframes(const Eph &e, const IonoUtc &io, uint32_t sbf[kSbfPages][kWordsPerSbf]) {
+// ---- SEM almanac (the reference's almanac_gps_t, almanac.h:21-43) ------------------------------------------------
+struct AlmRec {
+    unsigned char ura = 0, health = 0, config_code = 0;
+    unsigned short svid = 0, svn = 0;
+    unsigned valid = 0;
+    double e = 0, delta_i = 0, omegadot = 0, sqrta = 0, omega0 = 0, aop = 0, m0 = 0, af0 = 0, af1 = 0;
+    GpsTime toa;
+};
+struct Almanac {
+    bool valid = false;                             // at least one complete record
+    AlmRec sv[kMaxSat];
+};
+
+// Reads a SEM file with the reference's semantics: header "n title" and "week sec"; at most 32 records, each
+// optionally preceded by one blank line; id 0 reads as 1 and ids above 32 as 32 (a later record of the same id
+// overwrites the fields it reaches); the SVN line may be blank; ura, health and config code are clamped to 15, 63 and
+// 15; toa = (week + 2048, sec). Lines are read 99 characters at a time and the numbers with sscanf, as the reference
+// does. When the file ends early, what was read is kept -- including the fields of a record cut short, whose svid is
+// set while valid stays 0. Any other parse error empties the almanac. Returns false if the file cannot be opened.
+bool read_sem(const char *path, Almanac &alm) {
+    alm = Almanac();
+    FILE *fp = fopen(path, "rt");
+    if (!fp) return false;
+    char line[100];
+    auto next = [&]() { return fgets(line, sizeof line, fp) != nullptr; };
+    auto blank = [&]() { return line[0] == '\n' || line[0] == '\r'; };
+    unsigned n = 0, week = 0, sec = 0;
+    char title[32];
+    auto record = [&]() -> bool {
+        if (!next()) return false;
+        if (blank() && !next()) return false;
+        unsigned id = 0;
+        if (sscanf(line, "%u", &id) != 1) return false;
+        id = id == 0 ? 1 : (id > 32 ? 32 : id);
+        AlmRec &a = alm.sv[id - 1];
+        a.svid = (unsigned short) id;
+        if (!next()) return false;
+        if (blank()) a.svn = 0;
+        else if (sscanf(line, "%hu", &a.svn) != 1) return false;
+        if (!next() || sscanf(line, "%hhu", &a.ura) != 1) return false;
+        if (a.ura > 15) a.ura = 15;
+        if (!next() || sscanf(line, "%lf %lf %lf", &a.e, &a.delta_i, &a.omegadot) != 3) return false;
+        if (!next() || sscanf(line, "%lf %lf %lf", &a.sqrta, &a.omega0, &a.aop) != 3) return false;
+        if (!next() || sscanf(line, "%lf %lf %lf", &a.m0, &a.af0, &a.af1) != 3) return false;
+        if (!next() || sscanf(line, "%hhu", &a.health) != 1) return false;
+        if (a.health > 63) a.health = 63;
+        if (!next() || sscanf(line, "%hhu", &a.config_code) != 1) return false;
+        if (a.config_code > 15) a.config_code = 15;
+        a.toa.week = (int) week + 2048;             // the file holds the week modulo 1024 (Celestrak)
+        a.toa.sec = (double) sec;
+        a.valid = 1;
+        alm.valid = true;
+        return true;
+    };
+    bool ok = next() && sscanf(line, "%u %24s", &n, title) == 2 && next() && sscanf(line, "%u %u", &week, &sec) == 2;
+    if (ok) {
+        const unsigned count = n - 1u > 31u ? 32u : n;   // n = 0 wraps, as in the reference: 32 records
+        for (unsigned j = 0; j < count && ok; j++) ok = record();
+    }
+    if (!ok && !feof(fp)) alm = Almanac();
+    fclose(fp);
+    return true;
+}
+
+// ---- subframes 1-3, almanac / dummy pages of 4/5 (gps.c:617-884) ----------------------------------------------------
+void build_subframes(const Eph &e, const IonoUtc &io, const Almanac &alm, uint32_t sbf[kSbfPages][kWordsPerSbf]) {
     typedef unsigned long UL;    // the reference packs in (64-bit) long; only the low 32 bits survive
     const UL wn = 0, ura = 0, dataId = 1, EMPTY = 0xaaaaaaaaUL;
     const UL toe = (UL) (e.toe.sec / 16.0), toc = (UL) (e.toc.sec / 16.0);
@@ -369,6 +455,28 @@ void build_subframes(const Eph &e, const IonoUtc &io, uint32_t sbf[kSbfPages][kW
             for (int w = 3; w < 9; w++) put(page, w, (EMPTY & 0xFFFFFFUL) << 6);
             put(page, 9, (EMPTY & 0x3FFFFFUL) << 8);
         }
+    // almanac page of satellite sv (0-based) in subframe sfid; health written as 000 (all data OK)
+    auto put_alm = [&](int page, UL sfid, int sv) {
+        const AlmRec &a = alm.sv[sv];
+        const UL svId = (UL) (sv + 1);
+        const UL ecc = (UL) (a.e / P2_21), toa = (UL) (a.toa.sec / P2p12), sqrta = (UL) (a.sqrta / P2_11);
+        const long delta_i = (long) (a.delta_i / P2_19), omegadot = (long) (a.omegadot / P2_38),
+                   omega0 = (long) (a.omega0 / P2_23), aop = (long) (a.aop / P2_23), m0 = (long) (a.m0 / P2_23),
+                   af0 = (long) (a.af0 / P2_20), af1 = (long) (a.af1 / P2_38);
+        put(page, 0, TLM);
+        put(page, 1, sfid << 8);
+        put(page, 2, (dataId << 28) | (svId << 22) | ((ecc & 0xFFFFUL) << 6));
+        put(page, 3, ((toa & 0xFFUL) << 22) | ((delta_i & 0xFFFFUL) << 6));
+        put(page, 4, (omegadot & 0xFFFFUL) << 14);
+        put(page, 5, (sqrta & 0xFFFFFFUL) << 6);
+        put(page, 6, (omega0 & 0xFFFFFFUL) << 6);
+        put(page, 7, (aop & 0xFFFFFFUL) << 6);
+        put(page, 8, (m0 & 0xFFFFFFUL) << 6);
+        put(page, 9, ((af0 & 0x7F8UL) << 19) | ((af1 & 0x7FFUL) << 11) | ((af0 & 0x7UL) << 8));
+    };
+    // subframe 4 pages 2-5 and 7-10: PRN 25-28 and 29-32, complete records only (gps.c:773-803)
+    for (int sv = 24; sv < kMaxSat; sv++)
+        if (alm.sv[sv].valid) put_alm(3 + (sv <= 27 ? sv - 23 : sv - 22) * 2, 0x4UL, sv);
     if (io.valid) {                                    // subframe 4 page 18: ionosphere + UTC (SV id 56)
         const int p = 3 + 17 * 2;
         put(p, 0, TLM);
@@ -389,9 +497,18 @@ void build_subframes(const Eph &e, const IonoUtc &io, uint32_t sbf[kSbfPages][kW
         put(p, 2, (dataId << 28) | (63UL << 22));
         for (int w = 3; w < 10; w++) put(p, w, 0);
     }
+    // subframe 5 pages 1-24: PRN 1-24, every record with an svid -- a record cut short too (gps.c:832-859)
+    for (int sv = 0; sv < 24; sv++)
+        if (alm.sv[sv].svid != 0) put_alm(4 + sv * 2, 0x5UL, sv);
     {                                                   // subframe 5 page 25 (SV id 51): toa / wna
         const int p = 4 + 24 * 2;
-        const UL wna = (UL) (e.toe.week % 256), toa = (UL) (e.toe.sec / 4096.0);
+        UL wna = (UL) (e.toe.week % 256), toa = (UL) (e.toe.sec / 4096.0);
+        for (int sv = 0; sv < kMaxSat; sv++)            // the first record with an svid, else the ephemeris toe
+            if (alm.sv[sv].svid != 0) {
+                wna = (UL) (alm.sv[sv].toa.week % 256);
+                toa = (UL) (alm.sv[sv].toa.sec / 4096.0);
+                break;
+            }
         put(p, 0, TLM);
         put(p, 1, 0x5UL << 8);
         put(p, 2, (dataId << 28) | (51UL << 22) | ((toa & 0xFFUL) << 14) | ((wna & 0xFFUL) << 6));
@@ -660,6 +777,7 @@ struct gpsb200_scenario {
     std::vector<uint32_t> nav;                      // [nframes][nchan][60]
     int nframes = 0;
     std::string err;
+    std::string almanac_date;                       // empty: no valid almanac record
 };
 
 namespace {
@@ -679,6 +797,9 @@ int build(gpsb200_scenario *S) {
     io.enable = cfg.ionosphere_enable != 0;
     const int neph = cfg.rinex3 ? read_rinex3(cfg.nav_file, eph, io) : read_rinex2(cfg.nav_file, eph, io);
     if (neph <= 0) return fail(S, "cannot read the RINEX navigation file (wrong version flag, or no ephemeris in it)");
+    Almanac alm;                                    // empty unless a SEM file is named: the reference's almanac_init()
+    if (cfg.almanac_file && !read_sem(cfg.almanac_file, alm))
+        return fail(S, std::string("cannot open almanac file ") + cfg.almanac_file);
 
     // receiver positions per 0.1 s (gps.c:2331-2363, 2489-2500)
     int numd = cfg.duration_ds;
@@ -757,6 +878,24 @@ int build(gpsb200_scenario *S) {
                 }
             }
     if (ieph < 0) return fail(S, "no current set of ephemerides");
+    if (alm.valid) {                                // every complete record within 4 weeks of the start (gps.c:2637-2654)
+        GpsTime last;
+        for (int sv = 0; sv < kMaxSat; sv++)
+            if (alm.sv[sv].valid) {
+                last = alm.sv[sv].toa;
+                const double dt = gps_diff(alm.sv[sv].toa, g0);
+                if (dt < -4.0 * kSecWeek || dt > 4.0 * kSecWeek) {
+                    char m[160];
+                    snprintf(m, sizeof m, "invalid time of almanac: PRN %d toa (week %d, %.0f s) is more than 4 weeks from "
+                             "the start (the file should hold the week modulo 1024)", sv + 1, last.week, last.sec);
+                    return fail(S, m);
+                }
+            }
+        const Date t = gps_to_date(last);
+        char buf[64];
+        snprintf(buf, sizeof buf, "%4d/%02d/%02d,%02d:%02d:%02.0f", t.y, t.m, t.d, t.hh, t.mm, t.sec);
+        S->almanac_date = buf;
+    }
 
     std::vector<Channel> chan(C);
     std::vector<char> fresh(C, 0);                  // slot (re)allocated since the last epoch snapshot
@@ -791,7 +930,7 @@ int build(gpsb200_scenario *S) {
                             fresh[i] = 1;
                             // the reference never initialises channel_t.ipage (gps.c:2086 reads it);
                             // its -Og build sees zeroed stack there, which is what is reproduced here
-                            build_subframes(set[sv], io, ch.sbf);
+                            build_subframes(set[sv], io, alm, ch.sbf);
                             build_nav_frame(grx, ch, true);
                             const Range r = pseudo_range(set[sv], io, grx, p0);
                             ch.rho0 = r;
@@ -888,7 +1027,7 @@ int build(gpsb200_scenario *S) {
                         if (gps_diff(eph[ieph + 1][sv].toc, grx) < kSecHour) {
                             ieph++;
                             for (int i = 0; i < C; i++)
-                                if (chan[i].prn != 0) build_subframes(eph[ieph][chan[i].prn - 1], io, chan[i].sbf);
+                                if (chan[i].prn != 0) build_subframes(eph[ieph][chan[i].prn - 1], io, alm, chan[i].sbf);
                         }
                         break;
                     }
@@ -952,6 +1091,12 @@ int build(gpsb200_scenario *S) {
 
 }  // namespace
 
+// the Python mirror (api.py ScenarioConfig) and callers built against the header before almanac_file rely on these
+static_assert(offsetof(gpsb200_scenario_config_t, target_height_m) == 112, "gpsb200_scenario_config_t layout");
+static_assert(offsetof(gpsb200_scenario_config_t, almanac_file) == 120, "gpsb200_scenario_config_t layout");
+static_assert(sizeof(gpsb200_scenario_config_t) == 128, "gpsb200_scenario_config_t layout");
+static_assert(sizeof(gpsb200_almanac_record_t) == 112, "gpsb200_almanac_record_t layout");
+
 extern "C" {
 
 int gpsb200_scenario_create(const gpsb200_scenario_config_t *cfg, gpsb200_scenario_t **out) {
@@ -973,5 +1118,38 @@ int gpsb200_scenario_channels(const gpsb200_scenario_t *s) { return s ? s->nchan
 int gpsb200_scenario_nav_frames(const gpsb200_scenario_t *s) { return s ? s->nframes : 0; }
 const gpsb200_chan_t *gpsb200_scenario_chans(const gpsb200_scenario_t *s) { return s ? s->chans.data() : nullptr; }
 const uint32_t *gpsb200_scenario_nav(const gpsb200_scenario_t *s) { return s ? s->nav.data() : nullptr; }
+const char *gpsb200_scenario_almanac_date(const gpsb200_scenario_t *s) {
+    return s && !s->almanac_date.empty() ? s->almanac_date.c_str() : nullptr;
+}
+
+int gpsb200_almanac_read(const char *path, gpsb200_almanac_record_t rec[32], int32_t *valid) {
+    if (!path || !rec) return GPSB200_ERR_ARG;
+    Almanac alm;
+    if (!read_sem(path, alm)) return GPSB200_ERR_ARG;
+    for (int sv = 0; sv < kMaxSat; sv++) {
+        const AlmRec &a = alm.sv[sv];
+        gpsb200_almanac_record_t &r = rec[sv];
+        r = gpsb200_almanac_record_t{};
+        r.svid = a.svid;
+        r.svn = a.svn;
+        r.ura = a.ura;
+        r.health = a.health;
+        r.config_code = a.config_code;
+        r.valid = (int32_t) a.valid;
+        r.toa_week = a.toa.week;
+        r.e = a.e;
+        r.delta_i = a.delta_i;
+        r.omegadot = a.omegadot;
+        r.sqrta = a.sqrta;
+        r.omega0 = a.omega0;
+        r.aop = a.aop;
+        r.m0 = a.m0;
+        r.af0 = a.af0;
+        r.af1 = a.af1;
+        r.toa_sec = a.toa.sec;
+    }
+    if (valid) *valid = alm.valid ? 1 : 0;
+    return GPSB200_OK;
+}
 
 }  // extern "C"

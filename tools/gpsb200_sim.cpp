@@ -1,5 +1,6 @@
 // gpsb200-sim: file-sink driver with the reference's command-line vocabulary (help.h:20-53:
-// -e nav file, -l location, -t target, -d duration, -m motion file, -s start, --iq16, -I no ionosphere).
+// -e nav file, -l location, -t target, -d duration, -m motion file, -s start, --iq16, -I no ionosphere,
+// --disable-almanac; --almanac FILE names the SEM almanac the reference would read from ./almanac.sem).
 // RINEX + location -> scenario engine (host) -> CUDA synthesis -> reference-compatible FIFO ->
 // iqfile writer. Output is byte-identical to the reference's enqueue stream; --compat-drop
 // reproduces the stock program's iqdata.bin (which lacks blocks 1..6, fifo.c:163-168).
@@ -30,7 +31,8 @@
 static void usage() {
     fprintf(stderr,
             "gpsb200-sim -e NAV[.gz] [-3] -l lat,lon,h [-t dist,bearing,height] [-d SEC] [-m motion.csv] [-s y/m/d,h:m:s]\n"
-            "            [--iq16] [-I] [--pluto-gain] [--chan N] [--gpus N] [-o iqdata.bin] [--compat-drop]\n");
+            "            [--iq16] [-I] [--pluto-gain] [--chan N] [--gpus N] [-o iqdata.bin] [--compat-drop]\n"
+            "            [--almanac FILE.sem | --disable-almanac]\n");
     exit(2);
 }
 
@@ -81,6 +83,8 @@ int main(int argc, char **argv) {
         else if (a == "--gpus") gpus = atoi(need());
         else if (a == "-o") out = need();
         else if (a == "--compat-drop") compat = true;
+        else if (a == "--almanac") sc.almanac_file = need();
+        else if (a == "--disable-almanac") sc.almanac_file = nullptr;      // gps-sim.c:165-166; also the default here
         else usage();
     }
     if (!sc.nav_file || gpus < 1) usage();
@@ -93,8 +97,11 @@ int main(int argc, char **argv) {
     }
     const int nblk = gpsb200_scenario_blocks(scn), nchan = gpsb200_scenario_channels(scn);
     const int nframes = gpsb200_scenario_nav_frames(scn);
-    fprintf(stderr, "gpsb200-sim: note: no almanac pages are generated -- the stream equals the reference's with its almanac "
-                    "disabled (the reference enables it by default and downloads one)\n");
+    const char *alm_date = gpsb200_scenario_almanac_date(scn);             // gps.c:2652-2656
+    fprintf(stderr, "gpsb200-sim: almanac date: %s\n", alm_date ? alm_date : "disabled or invalid");
+    if (!sc.almanac_file)
+        fprintf(stderr, "gpsb200-sim: note: no almanac pages are generated -- the stream equals the reference's with its almanac "
+                        "disabled (the reference sends the one in ./almanac.sem by default; pass it with --almanac FILE)\n");
     const gpsb200_chan_t *chans = gpsb200_scenario_chans(scn);
     const uint32_t *nav = gpsb200_scenario_nav(scn);
     const size_t blk_bytes = (size_t) GPSB200_BLOCK_ELEMS * sample_size;
