@@ -126,8 +126,9 @@ int gpsb200_synth_blocks_scatter(gpsb200_ctx_t *ctx, const gpsb200_chan_t *chans
                                  int sample_size, void *const *dst_blocks, double *carr_phase_out,
                                  gpsb200_stats_t *stats);
 
-/* Same, but the output stays in device memory (dst_device: device pointer with room for
- * nblk * 600000 elements) and the synthesis is only ENQUEUED on `stream` (a cudaStream_t,
+/* Same, but the output stays in device memory (dst_device: 16-byte aligned device pointer with room for
+ * nblk * 600000 elements; the kernels store 16-byte words, a misaligned dst_device is GPSB200_ERR_ARG, as for
+ * gpsb200_slice_prepare and gpsb200_replay_device) and the synthesis is only ENQUEUED on `stream` (a cudaStream_t,
  * 0 = the context's own stream) -- the caller synchronizes before reading dst_device. The call itself returns when
  * the speculative pre-phase (block probes, span chaining), the host scan and the run checkpoints are done and the
  * device self-check of the carrier chain has been read (a failed check returns GPSB200_ERR_INTERNAL, and nothing of the
@@ -167,7 +168,7 @@ typedef struct gpsb200_slice_link {
     double first_phase[GPSB200_MAX_CHAN];   /* carr_phase of the first block (used when the slot does not continue) */
     double value[GPSB200_MAX_CHAN];         /* guessed phase after the slice (absolute), or the advance over the slice */
 } gpsb200_slice_link_t;
-/* dst_device and/or dst_host: with dst_host != NULL the synthesis is launched in chunks whose downloads into dst_host
+/* dst_device (16-byte aligned) and/or dst_host: with dst_host != NULL the synthesis is launched in chunks whose downloads into dst_host
  * (pinned memory) overlap later chunks, dst_device may then be NULL (a context-owned staging buffer is used);
  * gpsb200_slice_wait blocks until synthesis and downloads of the slice are complete and reports the self-check. */
 int gpsb200_slice_prepare(gpsb200_ctx_t *ctx, const gpsb200_chan_t *chans, int nblk, int nchan, int sample_size,
@@ -198,13 +199,14 @@ int gpsb200_link_apply(const gpsb200_slice_link_t *link, int nchan, const int32_
 int gpsb200_debug_corrupt_chain(gpsb200_ctx_t *ctx, int on);
 
 /* Name of the synthesis kernel a call with nchan channels launches on this context as it stands: "k_synth_lanes"
- * (lane = sample: run length a multiple of 96 up to 2400, every code rate seen so far within 1.0157 .. 1.0302 MHz, 16-byte aligned
- * destination, GPSB200_LANES != 0) or "k_synth" (lane = channel, no such conditions). Both are bit-exact; for reporting. */
+ * (lane = sample: run length a multiple of 96 up to 2400, every code rate seen so far within 1.0157 .. 1.0302 MHz,
+ * GPSB200_LANES != 0) or "k_synth" (lane = channel, no such conditions). Both are bit-exact; for reporting. */
 const char *gpsb200_synth_kernel_name(const gpsb200_ctx_t *ctx, int nchan);
 
 /* Re-run the device part of the previous gpsb200_synth_blocks_device call (parameters,
  * start phases and guesses already resident in HBM): used by bench.py to time the kernels
- * alone. kernel_mask bits: 8 = carrier tables, 4 = carrier probe, 1 = run checkpoints, 2 = synthesis. */
+ * alone. dst_device: 16-byte aligned, or NULL for the previous call's destination. kernel_mask bits: 8 = carrier
+ * tables, 4 = carrier probe, 1 = run checkpoints, 2 = synthesis. */
 int gpsb200_replay_device(gpsb200_ctx_t *ctx, void *dst_device, void *stream, int kernel_mask);
 
 /* Exact carrier phase after n samples of Doppler f_carr (the chain of gps.c:2821-2826

@@ -538,6 +538,15 @@ int check_call(gpsb200_ctx *ctx, const gpsb200_chan_t *chans, int nblk, int ncha
     return GPSB200_OK;
 }
 
+// Both synthesis kernels store whole 2- to 16-byte words at multiples of their width from the destination (k_synth_lanes
+// always 16 bytes, k_synth up to 32 bytes per lane as 16-byte vectors): a caller's device destination must be 16-byte
+// aligned. Checked before anything is enqueued; allocations of CUDA and torch are aligned to 256 bytes.
+int check_dst_aligned(gpsb200_ctx *ctx, const void *dst_device, const char *fn) {
+    if ((reinterpret_cast<uintptr_t>(dst_device) & 15u) != 0)
+        return fail(ctx, GPSB200_ERR_ARG, std::string(fn) + ": dst_device is not 16-byte aligned");
+    return GPSB200_OK;
+}
+
 // Wait for everything this context has in flight (error paths: the caller may free its buffers once it
 // sees the error code, so no copy into them may still be pending).
 void drain(gpsb200_ctx *ctx, cudaStream_t extra) {
@@ -1235,6 +1244,8 @@ int gpsb200_synth_blocks_device(gpsb200_ctx_t *ctx, const gpsb200_chan_t *chans,
                                 gpsb200_stats_t *stats) {
     int rc = check_call(ctx, chans, nblk, nchan, sample_size, dst_device);
     if (rc) return rc;
+    rc = check_dst_aligned(ctx, dst_device, "gpsb200_synth_blocks_device");
+    if (rc) return rc;
     cudaStream_t s = stream_ ? (cudaStream_t) stream_ : ctx->s_compute;
     return run_pipeline(ctx, chans, nblk, nchan, sample_size, dst_device, nullptr, s, nullptr, nullptr, nullptr,
                         carr_phase_out, stats);
@@ -1244,6 +1255,8 @@ int gpsb200_synth_blocks_device(gpsb200_ctx_t *ctx, const gpsb200_chan_t *chans,
 int gpsb200_slice_prepare(gpsb200_ctx_t *ctx, const gpsb200_chan_t *chans, int nblk, int nchan, int sample_size,
                           void *dst_device, void *dst_host, void *stream_, gpsb200_slice_link_t *link) {
     int rc = check_call(ctx, chans, nblk, nchan, sample_size, dst_device ? dst_device : dst_host);
+    if (rc) return rc;
+    rc = check_dst_aligned(ctx, dst_device, "gpsb200_slice_prepare");
     if (rc) return rc;
     if (!dst_device) {                          // host destination only: stage in the context's own device buffer
         const size_t need = (size_t) ctx->cfg.max_blocks * GPSB200_BLOCK_ELEMS * sample_size;
@@ -1569,6 +1582,8 @@ int gpsb200_carrier_chain_device(gpsb200_ctx_t *ctx, const gpsb200_chan_t *chans
 
 int gpsb200_replay_device(gpsb200_ctx_t *ctx, void *dst_device, void *stream_, int kernel_mask) {
     if (!ctx || !ctx->have_last) return GPSB200_ERR_ARG;
+    const int rc = check_dst_aligned(ctx, dst_device, "gpsb200_replay_device");
+    if (rc) return rc;
     CU(cudaSetDevice(ctx->cfg.device));
     cudaStream_t s = stream_ ? (cudaStream_t) stream_ : ctx->s_compute;
     SynthArgs a = ctx->last;

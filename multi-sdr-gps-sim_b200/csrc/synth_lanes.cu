@@ -256,8 +256,7 @@ __global__ void __launch_bounds__(kLaneWarps * 32, 2) k_synth_lanes(SynthArgs a)
 }  // namespace
 
 bool synth_lanes_applicable(const SynthArgs &a) {
-    return a.lanes && a.nchan <= 32 && a.run_samples % lanes::kWindow == 0 && a.run_samples <= lanes::kMaxRun &&
-           (reinterpret_cast<uintptr_t>(a.out) & 15u) == 0;                    // 16-byte stores
+    return a.lanes && a.nchan <= 32 && a.run_samples % lanes::kWindow == 0 && a.run_samples <= lanes::kMaxRun;
 }
 
 static int device_sms() {

@@ -11,7 +11,7 @@ from scenario import gps
 pytestmark = pytest.mark.gpu
 
 
-def run_golden(name, nblocks=None, run_samples=0):
+def run_golden(name, nblocks=None, run_samples=0, kernel=None):
     g = scenario.load_golden(name)
     ch, frames = scenario.golden_chans(g, nblocks)
     nblk, nchan = ch.shape
@@ -19,6 +19,8 @@ def run_golden(name, nblocks=None, run_samples=0):
     with gps.Context(nchan, nblk, max_nav_frames=len(frames), run_samples=run_samples) as ctx:
         ctx.set_nav_frames(frames)
         out, cp = ctx.synth_blocks(ch, ss)
+        if kernel is not None:
+            assert ctx.synth_kernel_name(nchan) == kernel, (name, run_samples)
     crc = scenario.crc_blocks(out)
     want = g["crcs"][:nblk, 0]
     bad = np.nonzero(crc != want)[0]
@@ -47,9 +49,32 @@ def test_nav_frame_roll_and_35s_chain_matches_reference_stream():
     run_golden("sky12_static_35s_i8")
 
 
-@pytest.mark.parametrize("run_samples", [800, 4000, 12000])
-def test_other_run_lengths_give_identical_output(run_samples):
-    run_golden("sky12_static_10s_i8", nblocks=12, run_samples=run_samples)
+RUN_LENGTHS = [32, 96, 160, 480, 800, 2400, 4000, 12000, 20000, 60000, 100000, 300000]   # every one gpsb200_create accepts
+LANES_RUN_LENGTHS = (96, 480, 2400)                                                        # multiples of 96 up to 2400
+
+
+def _run_length_cases():
+    cases = []
+    for nblocks in (2, 12):
+        for name in ("sky12_static_10s_i8", "sky12_circle_10s_i16"):
+            for run in RUN_LENGTHS:
+                # the first cases of this test (12 int8 blocks at 800, 4000, 12000) keep their ids
+                first = nblocks == 12 and name == "sky12_static_10s_i8" and run in (800, 4000, 12000)
+                cases.append(pytest.param(run, name, nblocks, id=str(run) if first else "%d-%s-%d" % (nblocks, name, run)))
+    return cases
+
+
+@pytest.mark.parametrize("run_samples,name,nblocks", _run_length_cases())
+def test_other_run_lengths_give_identical_output(run_samples, name, nblocks, monkeypatch):
+    """Every accepted run length (1 to 9375 runs per block: k_checkpoints, the host walk of small calls, the launch shapes
+    of both kernels), int8 and int16, a two-block call (host-resolved) and a twelve-block call (speculative chain),
+    against the reference's stream. The lengths k_synth_lanes takes run a second time on k_synth."""
+    passes = [("1", "k_synth_lanes" if run_samples in LANES_RUN_LENGTHS else "k_synth")]
+    if run_samples in LANES_RUN_LENGTHS:
+        passes.append(("0", "k_synth"))
+    for lanes, kernel in passes:
+        monkeypatch.setenv("GPSB200_LANES", lanes)
+        run_golden(name, nblocks=nblocks, run_samples=run_samples, kernel=kernel)
 
 
 @pytest.mark.parametrize("nchan,ss", [(1, 1), (5, 2), (8, 1), (9, 1), (16, 2), (17, 1), (32, 1), (32, 2)])

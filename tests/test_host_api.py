@@ -351,3 +351,24 @@ def test_lane_per_sample_model_adversarial_phases():
         walks += int(counters[3])
         rebuilt += int(counters[2])
     assert walks > 0 and rebuilt > 0, (walks, rebuilt)
+
+
+def test_lane_per_sample_model_engineered_repair_hits():
+    """The engineered hits of tests/repair_cases.py (carrier-index and chip boundaries at chosen block, run, window, lane,
+    residue and slot, from exact anchors of later runs and later blocks): each hit, alone in its block, makes the model
+    walk (carrier) or rebuild the window's chip signs exactly (code), and every block of every case equals the oracle.
+    The GPU test feeds the same cases to k_synth_lanes; its anchors are the exact walks the model takes here."""
+    import repair_cases as rc
+    for case in rc.CASES:
+        ch, nav, decisive = rc.build(case)
+        for h in case.hits:
+            row = rc.chained_row(ch, h.block)[[h.slot]]
+            _, _, counters = gps.lanes_model_block(row, nav[0][[h.slot]])
+            assert counters[3 if h.kind == "carr" else 2] > 0, (case.name, h, counters)
+            # the FP64 and the linear phase straddle the boundary: skipping the repair would change the sample
+            # (window 0, sample 0 of run 0 has no rounding behind it: its linear phase is the input phase itself)
+            assert decisive[h.slot] == (h.run + h.win + h.n + h.block > 0), (case.name, h)
+        want, _ = scenario.oracle_run(ch, nav, 2)
+        for b in range(case.nblk):
+            iq, _, counters = gps.lanes_model_block(rc.chained_row(ch, b), nav[0])
+            assert np.array_equal(iq, want[b * gps.BLOCK_ELEMS:(b + 1) * gps.BLOCK_ELEMS]), (case.name, b, counters)
