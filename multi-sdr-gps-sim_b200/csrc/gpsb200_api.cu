@@ -140,13 +140,8 @@ struct gpsb200_ctx {
     CarrierProbe *h_probe = nullptr, *d_probe_host = nullptr;   // ... and in mapped host memory (host fallback)
     CarrierProbe *h_span_sum = nullptr, *d_span_sum = nullptr;  // span summaries, mapped host memory
     SpanBlockState *d_spec = nullptr;                  // speculative block-start phases
-    double *d_run_x = nullptr;                         // run-start states of the block probes' variant trajectories
-    double *d_blk_shift = nullptr, *h_blk_shift = nullptr;     // host-resolved spans: per-block shift / variant pick
-    int32_t *d_blk_pick = nullptr, *h_blk_pick = nullptr;
-    int run_ld = 0;                                    // leading dimension (blocks, padded) of d_run_x
     bool lanes_on = true;                              // GPSB200_LANES=0: always k_synth (lane = channel)
     bool lanes_veto = false;                           // a channel record outside k_synth_lanes' range was seen
-    int check_stride = 8, check_phase = 0;             // sampled exact re-walk of the chain (GPSB200_CHECK_STRIDE)
     SpanRes *d_span_res = nullptr, *h_span_res = nullptr;
     int max_spans = 0, max_segs = 0;
     double *h_seg_end = nullptr, *d_seg_end = nullptr;   // mapped: device-walked end phases of every pipeline segment's last block
@@ -170,7 +165,6 @@ struct gpsb200_ctx {
     void *d_out = nullptr;
     size_t out_bytes = 0;
     bool nav_dirty = true;
-    bool graded_chunks = true;             // GPSB200_GRADED_CHUNKS=0: uniform 256-block chunks (A/B knob)
     std::unique_ptr<WorkerPool> pool;      // host passes (guesses, fix-up scan)
     SynthArgs last{};                      // replay state
     bool have_last = false;
@@ -379,11 +373,9 @@ void reanchor_guesses(gpsb200_ctx *ctx, int b0, int b1, int nchan, const std::ve
 }
 
 // One block of the chain, resolved on the host from its block probe (the first level of the speculation);
-// the exact sequential walk when the probe cannot be used. Returns 1 when it had to walk.
-inline int resolve_block(ChainState &st, const BlockChanDev &bc, const CarrierProbe &probe, double &start_out,
-                         int32_t &pick_out, double &shift_out) {
-    pick_out = -1;                       // -1: k_checkpoints walks the block exactly
-    shift_out = 0.0;
+// the exact sequential walk when the probe cannot be used. start_out: the block's exact start phase (k_checkpoints
+// walks the block from it). Returns 1 when it had to walk.
+inline int resolve_block(ChainState &st, const BlockChanDev &bc, const CarrierProbe &probe, double &start_out) {
     if (bc.prn <= 0) {
         st.prn = 0;
         start_out = 0.0;
@@ -392,12 +384,9 @@ inline int resolve_block(ChainState &st, const BlockChanDev &bc, const CarrierPr
     if (st.prn != bc.prn) st.phase = bc.carr_in;
     st.prn = bc.prn;
     start_out = st.phase;
-    double xe, d;
-    int v;
-    if (carrier_fixup(st.phase, bc.c_carr, probe, xe, &v, &d)) {
+    double xe;
+    if (carrier_fixup(st.phase, bc.c_carr, probe, xe)) {
         st.phase = xe;
-        pick_out = v;
-        shift_out = d;
         return 0;
     }
     int64_t dummy = 0;
@@ -409,10 +398,10 @@ inline int resolve_block(ChainState &st, const BlockChanDev &bc, const CarrierPr
 // carrier_fixup per SPAN from the span summaries k_chain left in mapped host memory; a span the device
 // could not chain speculatively (reallocation inside it, Doppler zero crossing, a rejected block probe)
 // or whose summary does not fit the true start phase is resolved block by block from the block probes.
-// Serial over spans per channel, parallel over channels. Returns the number of blocks walked sequentially.
-int64_t resolve_chain(gpsb200_ctx *ctx, int b0, int b1, int nchan, std::vector<ChainState> &chain,
-                      int64_t *spans_regular, int64_t *spans_slow) {
-    std::vector<int64_t> fallbacks(nchan, 0), reg(nchan, 0), slow(nchan, 0);
+// Serial over spans per channel, parallel over channels. Returns the number of blocks walked sequentially; adds the
+// number of spans resolved block by block to *spans_slow.
+int64_t resolve_chain(gpsb200_ctx *ctx, int b0, int b1, int nchan, std::vector<ChainState> &chain, int64_t *spans_slow) {
+    std::vector<int64_t> fallbacks(nchan, 0), slow(nchan, 0);
     const int K = kSpanBlocks;
     const int nspan = (b1 - b0 + K - 1) / K;
     ctx->pool->run(nchan, [&](int c_lo, int c_hi) {
@@ -443,7 +432,6 @@ int64_t resolve_chain(gpsb200_ctx *ctx, int b0, int b1, int nchan, std::vector<C
                         res.variant = v;
                         st.prn = first.prn;
                         st.phase = xe;
-                        ++reg[c];
                         continue;
                     }
                 }
@@ -452,24 +440,23 @@ int64_t resolve_chain(gpsb200_ctx *ctx, int b0, int b1, int nchan, std::vector<C
                 ++slow[c];
                 for (int b = s0; b < s1; b++) {
                     const size_t i = (size_t) b * nchan + c;
-                    fallbacks[c] += resolve_block(st, ctx->h_bc[i], ctx->h_probe[i], ctx->h_carr0[i], ctx->h_blk_pick[i],
-                                                  ctx->h_blk_shift[i]);
+                    fallbacks[c] += resolve_block(st, ctx->h_bc[i], ctx->h_probe[i], ctx->h_carr0[i]);
                 }
             }
             chain[c] = st;
         }
     });
-    // test hook of the device self-check (gpsb200_debug_corrupt_chain): corrupt the resolution of one span by
-    // one unit of the rounding grid; k_checkpoints must notice
+    // test hook of the device self-check (gpsb200_debug_corrupt_chain): corrupt the resolution of slot 0's first span
+    // by one unit of the rounding grid -- the span's shift, or the start phase of block b0 + 5 when the span was
+    // resolved block by block; k_checkpoints must notice
     if (ctx->fault_inject_chain && b1 - b0 > 6) {
         SpanRes &r = ctx->h_span_res[(size_t) (b0 / K) * nchan];
         if (r.mode == 0) r.shift += 0x1p-51;
-        else if (r.mode == 1) ctx->h_blk_shift[(size_t) (b0 + 5) * nchan] += 0x1p-51;
+        else if (r.mode == 1) ctx->h_carr0[(size_t) (b0 + 5) * nchan] += 0x1p-51;
     }
     int64_t n = 0;
     for (int c = 0; c < nchan; c++) {
         n += fallbacks[c];
-        if (spans_regular) *spans_regular += reg[c];
         if (spans_slow) *spans_slow += slow[c];
     }
     return n;
@@ -501,13 +488,6 @@ void fill_args(gpsb200_ctx *ctx, SynthArgs &a, int blk0, int nblk, int nchan, in
     a.nruns = ctx->nruns;
     a.run_samples = ctx->cfg.run_samples;
     a.iq16 = sample_size == GPSB200_SC16;
-    a.check_stride = ctx->check_stride;
-    a.check_phase = ctx->check_phase;
-    a.run_x = ctx->d_run_x;
-    a.run_b0 = blk0;
-    a.run_ld = ctx->run_ld;
-    a.blk_shift = ctx->d_blk_shift + off;
-    a.blk_pick = ctx->d_blk_pick + off;
     a.lanes = ctx->lanes_on && !ctx->lanes_veto ? 1 : 0;
     // lanes per run follow the channel count; a CTA takes up to 24 warps' worth of runs
     const int grp = nchan > 16 ? 32 : (nchan > 8 ? 16 : 8);
@@ -547,8 +527,21 @@ int check_dst_aligned(gpsb200_ctx *ctx, const void *dst_device, const char *fn) 
     return GPSB200_OK;
 }
 
+// Host destinations are staged in the context's own device buffer, sized for the context's largest call.
+int ensure_staging(gpsb200_ctx *ctx, int sample_size) {
+    const size_t need = (size_t) ctx->cfg.max_blocks * GPSB200_BLOCK_ELEMS * sample_size;
+    if (ctx->out_bytes < need) {
+        cudaFree(ctx->d_out);
+        ctx->d_out = nullptr;
+        ctx->out_bytes = 0;
+        CU(cudaMalloc(&ctx->d_out, need));
+        ctx->out_bytes = need;
+    }
+    return GPSB200_OK;
+}
+
 // Wait for everything this context has in flight (error paths: the caller may free its buffers once it
-// sees the error code, so no copy into them may still be pending).
+// sees the error code, so no copy into them may still be pending). Leaves ctx->err alone.
 void drain(gpsb200_ctx *ctx, cudaStream_t extra) {
     if (extra) cudaStreamSynchronize(extra);
     cudaStreamSynchronize(ctx->s_compute);
@@ -591,30 +584,22 @@ int segment_probe(gpsb200_ctx *ctx, int b0, int b1, int nchan, cudaStream_t sp, 
     return GPSB200_OK;
 }
 
-// Second half: wait for the span summaries, host scan from the chain state, resolutions up, exact run
-// checkpoints (+ device self-check). After it the segment's synthesis may be enqueued behind sp.
-int segment_checkpoints(gpsb200_ctx *ctx, int b0, int b1, int nchan, cudaStream_t sp, gpsb200_stats_t &st, bool first,
-                        const SynthArgs &a, int64_t slow);
-
-int segment_resolve(gpsb200_ctx *ctx, int b0, int b1, int nchan, cudaStream_t sp, std::vector<ChainState> &chain,
-                    gpsb200_stats_t &st, bool first, const SynthArgs &a, cudaEvent_t probes_done = nullptr,
-                    int64_t *slow_out = nullptr) {
-    // probes and span summaries must be in (mapped) host memory: wait for the segment's own probe event when the
-    // post-scan work runs on a stream of its own (slice path), else for the pre-phase stream
+// Host scan of a segment: wait until its probes and span summaries are in (mapped) host memory -- for the segment's
+// own probe event when there is one, else for the stream that ran them -- and resolve the chain from `chain` on.
+// slow: the number of spans resolved block by block (segment_checkpoints uploads their block start phases).
+int segment_scan(gpsb200_ctx *ctx, int b0, int b1, int nchan, cudaEvent_t probes_done, cudaStream_t sp,
+                 std::vector<ChainState> &chain, gpsb200_stats_t &st, int64_t &slow) {
     if (probes_done) CU(cudaEventSynchronize(probes_done));
     else CU(cudaStreamSynchronize(sp));
     const double t0 = now_ms();
-    int64_t reg = 0, slow = 0;
-    st.chain_fallbacks += (int32_t) resolve_chain(ctx, b0, b1, nchan, chain, &reg, &slow);
+    slow = 0;
+    st.chain_fallbacks += (int32_t) resolve_chain(ctx, b0, b1, nchan, chain, &slow);
     st.host_chain_ms += now_ms() - t0;
-    if (slow_out) {                 // scan only: the caller enqueues the device part later (segment_checkpoints)
-        *slow_out = slow;
-        return GPSB200_OK;
-    }
-    return segment_checkpoints(ctx, b0, b1, nchan, sp, st, first, a, slow);
+    return GPSB200_OK;
 }
 
-// Device part of a segment's resolution: resolutions up, exact run checkpoints (+ self-check).
+// Device part of a segment's resolution: resolutions up, exact run checkpoints (+ device self-check). After it the
+// segment's synthesis may be enqueued behind sp.
 int segment_checkpoints(gpsb200_ctx *ctx, int b0, int b1, int nchan, cudaStream_t sp, gpsb200_stats_t &st, bool first,
                         const SynthArgs &a, int64_t slow) {
     const size_t off = (size_t) b0 * nchan, cnt = (size_t) (b1 - b0) * nchan;
@@ -622,11 +607,9 @@ int segment_checkpoints(gpsb200_ctx *ctx, int b0, int b1, int nchan, cudaStream_
     if (first) CU(cudaEventRecord(ctx->ev[3], sp));
     CU(cudaMemcpyAsync(ctx->d_span_res + soff, ctx->h_span_res + soff, scnt * sizeof(SpanRes), cudaMemcpyHostToDevice, sp));
     st.h2d_bytes += (int64_t) (scnt * sizeof(SpanRes));
-    if (slow > 0) {                                  // rare: per-block resolutions of the host-resolved spans
+    if (slow > 0) {                                  // rare: block start phases of the host-resolved spans
         CU(cudaMemcpyAsync(ctx->d_carr0 + off, ctx->h_carr0 + off, cnt * sizeof(double), cudaMemcpyHostToDevice, sp));
-        CU(cudaMemcpyAsync(ctx->d_blk_shift + off, ctx->h_blk_shift + off, cnt * sizeof(double), cudaMemcpyHostToDevice, sp));
-        CU(cudaMemcpyAsync(ctx->d_blk_pick + off, ctx->h_blk_pick + off, cnt * sizeof(int32_t), cudaMemcpyHostToDevice, sp));
-        st.h2d_bytes += (int64_t) (cnt * (2 * sizeof(double) + sizeof(int32_t)));
+        st.h2d_bytes += (int64_t) (cnt * sizeof(double));
     }
     SynthArgs ack = a;
     ack.last_end_host = ctx->cur_seg < ctx->max_segs ? ctx->d_seg_end + (size_t) ctx->cur_seg * nchan : nullptr;
@@ -643,8 +626,7 @@ int synth_chunks(gpsb200_ctx *ctx, int b0, int b1, int nchan, int sample_size, v
     const size_t blk_bytes = (size_t) GPSB200_BLOCK_ELEMS * sample_size;
     // the very first chunks are short, so that the download (the long pole of this path) starts early
     for (int c0 = b0, nc = 0; c0 < b1; c0 += nc, ichunk++) {
-        nc = kSynthChunk;
-        if (ctx->graded_chunks) nc = c0 == 0 ? 32 : (c0 == 32 ? 96 : (c0 == 128 ? 128 : kSynthChunk));
+        nc = c0 == 0 ? 32 : (c0 == 32 ? 96 : (c0 == 128 ? 128 : kSynthChunk));
         nc = std::min(nc, b1 - c0);
         SynthArgs ac{};
         char *dout = (char *) dst_dev + (size_t) c0 * blk_bytes;
@@ -762,17 +744,16 @@ std::vector<std::pair<int, int>> segments_of(int nblk) {
     return v;
 }
 
-// After the checkpoint kernel of segment i: remember what the chain expects at the segment's end and fetch what the
-// device's exact walk of the segment's last block ended on (k_checkpoints -> carr_end); compared in verify_chain().
-// This extends the device self-check across pipeline-segment (and call) boundaries.
-int note_segment_end(gpsb200_ctx *ctx, int iseg, int b1, int nchan, cudaStream_t sp, const std::vector<ChainState> &chain) {
-    if (iseg >= ctx->max_segs) return GPSB200_OK;
+// After the checkpoint kernel of segment i: remember what the chain expects at the segment's end. The kernel itself
+// stores what the device's exact walk of the segment's last block ended on into h_seg_end (mapped memory: a
+// copy-engine transfer would queue behind the large result downloads); verify_chain() compares the two. This extends
+// the device self-check across pipeline-segment (and call) boundaries.
+void note_segment_end(gpsb200_ctx *ctx, int iseg, int b1, int nchan, const std::vector<ChainState> &chain) {
+    if (iseg >= ctx->max_segs) return;
     for (int c = 0; c < nchan; c++) {
         const bool live = chain[c].prn > 0 && ctx->h_bc[(size_t) (b1 - 1) * nchan + c].prn == chain[c].prn;
         ctx->seg_expect[(size_t) iseg * nchan + c] = live ? chain[c].phase : -1.0;       // -1: nothing to compare
     }
-    (void) sp;       // the checkpoint kernel of the segment stores its last block's end phases into h_seg_end itself
-    return GPSB200_OK;   // (mapped memory: a copy-engine transfer would queue behind the large result downloads)
 }
 
 // Verdict of the device self-check (all of sp's work must be complete): the per-block comparisons inside the
@@ -802,7 +783,6 @@ int run_pipeline_inner(gpsb200_ctx *ctx, const gpsb200_chan_t *chans, int nblk, 
     gpsb200_stats_t st{};
     std::vector<ChainState> chain(nchan);
     seed_chain(chain, nchan, prn_in, phase_in);
-    ctx->check_phase = (ctx->check_phase + 1) % ctx->check_stride;      // the sampled exact re-walk rotates
     ctx->trace_t0 = now_ms();
     trace(ctx, "call");
     if (nblk <= kHostChainBlocks && !ctx->fault_inject_chain)
@@ -813,7 +793,7 @@ int run_pipeline_inner(gpsb200_ctx *ctx, const gpsb200_chan_t *chans, int nblk, 
     int rc = upload_nav(ctx, sp);
     if (rc) return rc;
     CU(cudaMemsetAsync(ctx->d_chain_errors, 0, sizeof(int), sp));
-    int ichunk = 0, iseg = 0;
+    int iseg = 0;
     const auto segs = segments_of(nblk);
     if (!dst_host) {
         // Device destination: nothing has to leave early, so everything speculative goes first -- the host prepares
@@ -839,59 +819,44 @@ int run_pipeline_inner(gpsb200_ctx *ctx, const gpsb200_chan_t *chans, int nblk, 
         int64_t slow = 0;
         trace(ctx, "speculative work enqueued");
         for (size_t i = 0; i < segs.size(); i++) {
-            CU(cudaEventSynchronize(ctx->ev_seg[std::min((int) i, ctx->max_segs - 1)]));
-            const double t0 = now_ms();
-            int64_t reg = 0, sl = 0;
-            st.chain_fallbacks += (int32_t) resolve_chain(ctx, segs[i].first, segs[i].second, nchan, chain, &reg, &sl);
+            int64_t sl = 0;
+            rc = segment_scan(ctx, segs[i].first, segs[i].second, nchan, ctx->ev_seg[std::min((int) i, ctx->max_segs - 1)],
+                              nullptr, chain, st, sl);
+            if (rc) return rc;
             slow += sl;
-            st.host_chain_ms += now_ms() - t0;
         }
         CU(cudaStreamSynchronize(ctx->s_ck));           // (its last segment's event has been waited for; this orders the
         trace(ctx, "host scan done");                   //  checkpoint launch on sp behind everything on s_ck)
         SynthArgs all{};
         fill_args(ctx, all, 0, nblk, nchan, sample_size, dst_dev);
-        const size_t cnt = (size_t) nblk * nchan, scnt = (size_t) all.nspan * nchan;
-        CU(cudaEventRecord(ctx->ev[3], sp));
-        CU(cudaMemcpyAsync(ctx->d_span_res, ctx->h_span_res, scnt * sizeof(SpanRes), cudaMemcpyHostToDevice, sp));
-        if (slow > 0) {
-            CU(cudaMemcpyAsync(ctx->d_carr0, ctx->h_carr0, cnt * sizeof(double), cudaMemcpyHostToDevice, sp));
-            CU(cudaMemcpyAsync(ctx->d_blk_shift, ctx->h_blk_shift, cnt * sizeof(double), cudaMemcpyHostToDevice, sp));
-            CU(cudaMemcpyAsync(ctx->d_blk_pick, ctx->h_blk_pick, cnt * sizeof(int32_t), cudaMemcpyHostToDevice, sp));
-        }
-        SynthArgs ack = all;
-        ack.last_end_host = ctx->d_seg_end;
-        CU(launch_checkpoints(ack, sp));
-        CU(cudaEventRecord(ctx->ev[4], sp));
-        rc = note_segment_end(ctx, 0, nblk, nchan, sp, chain);
+        ctx->cur_seg = 0;
+        rc = segment_checkpoints(ctx, 0, nblk, nchan, sp, st, true, all, slow);
         if (rc) return rc;
-        iseg = 1;
+        note_segment_end(ctx, iseg++, nblk, nchan, chain);
         CU(cudaEventRecord(ctx->ev_done[0], sp));
         CU(cudaStreamWaitEvent(s, ctx->ev_done[0], 0));
         CU(launch_synth(all, s));
-        st.launches += 2;
-        st.h2d_bytes += (int64_t) (scnt * sizeof(SpanRes));
+        st.launches += 1;
         trace(ctx, "checkpoints + synthesis enqueued");
-    }
-    for (const auto &sg : segs) {
-        if (!dst_host) break;
-        const int b0 = sg.first, b1 = sg.second;
-        SynthArgs a{};
-        rc = segment_params(ctx, chans, b0, b1, nchan, sample_size, dst_dev, sp, chain, st, a, nullptr);
-        if (rc) return rc;
-        rc = segment_probe(ctx, b0, b1, nchan, sp, st, b0 == 0, a);
-        if (rc) return rc;
-        ctx->cur_seg = iseg;
-        rc = segment_resolve(ctx, b0, b1, nchan, sp, chain, st, b0 == 0, a);
-        if (rc) return rc;
-        rc = note_segment_end(ctx, iseg++, b1, nchan, sp, chain);
-        if (rc) return rc;
-        CU(cudaEventRecord(ctx->ev_done[ichunk], sp));   // synthesis of this segment waits for its checkpoints
-        CU(cudaStreamWaitEvent(s, ctx->ev_done[ichunk], 0));
-        ichunk++;
-        if (!dst_host) {
-            CU(launch_synth(a, s));
-            st.launches += 1;
-        } else {
+    } else {
+        int ichunk = 0;
+        for (const auto &sg : segs) {
+            const int b0 = sg.first, b1 = sg.second;
+            SynthArgs a{};
+            rc = segment_params(ctx, chans, b0, b1, nchan, sample_size, dst_dev, sp, chain, st, a, nullptr);
+            if (rc) return rc;
+            rc = segment_probe(ctx, b0, b1, nchan, sp, st, b0 == 0, a);
+            if (rc) return rc;
+            int64_t slow = 0;
+            rc = segment_scan(ctx, b0, b1, nchan, nullptr, sp, chain, st, slow);
+            if (rc) return rc;
+            ctx->cur_seg = iseg;
+            rc = segment_checkpoints(ctx, b0, b1, nchan, sp, st, b0 == 0, a, slow);
+            if (rc) return rc;
+            note_segment_end(ctx, iseg++, b1, nchan, chain);
+            CU(cudaEventRecord(ctx->ev_done[ichunk], sp));   // synthesis of this segment waits for its checkpoints
+            CU(cudaStreamWaitEvent(s, ctx->ev_done[ichunk], 0));
+            ichunk++;
             rc = synth_chunks(ctx, b0, b1, nchan, sample_size, dst_dev, dst_host, s, st, ichunk);
             if (rc) return rc;
         }
@@ -933,11 +898,7 @@ int run_pipeline(gpsb200_ctx *ctx, const gpsb200_chan_t *chans, int nblk, int nc
                  int32_t *prn_out, double *carr_phase_out, gpsb200_stats_t *stats) {
     const int rc = run_pipeline_inner(ctx, chans, nblk, nchan, sample_size, dst_dev, dst_host, s, prn_in, phase_in, prn_out,
                                       carr_phase_out, stats);
-    if (rc) {                       // nothing of this call may still be in flight when the caller sees the error
-        const std::string keep = ctx->err;
-        drain(ctx, s);
-        ctx->err = keep;
-    }
+    if (rc) drain(ctx, s);          // nothing of this call may still be in flight when the caller sees the error
     return rc;
 }
 
@@ -1094,7 +1055,6 @@ int gpsb200_create(const gpsb200_config_t *cfg, gpsb200_ctx_t **out) {
         return GPSB200_ERR_ARG;
     }
     ctx->nruns = GPSB200_BLOCK_SAMPLES / c.run_samples;
-    if (const char *ev = getenv("GPSB200_GRADED_CHUNKS")) ctx->graded_chunks = atoi(ev) != 0;
     ctx->pool.reset(new WorkerPool(std::min(c.host_threads, c.max_chan)));
     *out = ctx;   // from here on errors are reported through the context
     int ndev = 0;
@@ -1146,20 +1106,6 @@ int gpsb200_create(const gpsb200_config_t *cfg, gpsb200_ctx_t **out) {
     CU(cudaHostAlloc(&ctx->h_span_sum, nsc * sizeof(CarrierProbe), cudaHostAllocMapped));
     CU(cudaHostGetDevicePointer((void **) &ctx->d_span_sum, ctx->h_span_sum, 0));
     CU(cudaMalloc(&ctx->d_spec, nbc * sizeof(SpanBlockState)));
-    // Run-start carrier states taken from the probes' own trajectories (+ resolved shift) instead of a second exact
-    // walk: implemented and exact (GPU suite green with every block cross-checked), but it does not pay -- stopping the
-    // probe walks at the 125 run starts lengthens k_probe, while k_checkpoints is bound by the latency of its longest
-    // walk, which sampling does not shorten. Off unless
-    // GPSB200_DERIVED_ANCHORS=1 (then every 8th warp of blocks, rotating, is still re-walked: GPSB200_CHECK_STRIDE).
-    ctx->run_ld = (c.max_blocks + 31) & ~31;
-    if (const char *ev = getenv("GPSB200_DERIVED_ANCHORS"))
-        if (atoi(ev) != 0)
-            CU(cudaMalloc(&ctx->d_run_x, (size_t) ctx->run_ld * c.max_chan * ctx->nruns * 2 * sizeof(double)));
-    CU(cudaMalloc(&ctx->d_blk_shift, nbc * sizeof(double)));
-    CU(cudaHostAlloc(&ctx->h_blk_shift, nbc * sizeof(double), cudaHostAllocDefault));
-    CU(cudaMalloc(&ctx->d_blk_pick, nbc * sizeof(int32_t)));
-    CU(cudaHostAlloc(&ctx->h_blk_pick, nbc * sizeof(int32_t), cudaHostAllocDefault));
-    if (const char *ev = getenv("GPSB200_CHECK_STRIDE")) ctx->check_stride = std::max(1, atoi(ev));
     if (const char *ev = getenv("GPSB200_TRACE")) ctx->trace_on = atoi(ev) != 0;
     if (const char *ev = getenv("GPSB200_LANES")) ctx->lanes_on = atoi(ev) != 0;
     CU(cudaMalloc(&ctx->d_span_res, nsc * sizeof(SpanRes)));
@@ -1205,11 +1151,6 @@ void gpsb200_destroy(gpsb200_ctx_t *ctx) {
     cudaFree(ctx->d_probe);
     cudaFreeHost(ctx->h_span_sum);
     cudaFree(ctx->d_spec);
-    cudaFree(ctx->d_run_x);
-    cudaFree(ctx->d_blk_shift);
-    cudaFreeHost(ctx->h_blk_shift);
-    cudaFree(ctx->d_blk_pick);
-    cudaFreeHost(ctx->h_blk_pick);
     cudaFree(ctx->d_span_res);
     cudaFreeHost(ctx->h_span_res);
     cudaFree(ctx->d_nav);
@@ -1259,20 +1200,13 @@ int gpsb200_slice_prepare(gpsb200_ctx_t *ctx, const gpsb200_chan_t *chans, int n
     rc = check_dst_aligned(ctx, dst_device, "gpsb200_slice_prepare");
     if (rc) return rc;
     if (!dst_device) {                          // host destination only: stage in the context's own device buffer
-        const size_t need = (size_t) ctx->cfg.max_blocks * GPSB200_BLOCK_ELEMS * sample_size;
-        if (ctx->out_bytes < need) {
-            cudaFree(ctx->d_out);
-            ctx->d_out = nullptr;
-            ctx->out_bytes = 0;
-            CU(cudaMalloc(&ctx->d_out, need));
-            ctx->out_bytes = need;
-        }
+        rc = ensure_staging(ctx, sample_size);
+        if (rc) return rc;
         dst_device = ctx->d_out;
     }
     if (!link) return fail(ctx, GPSB200_ERR_ARG, "gpsb200_slice_prepare: link is NULL");
     cudaStream_t s = stream_ ? (cudaStream_t) stream_ : ctx->s_compute;
     cudaStream_t sp = ctx->s_pre;
-    ctx->check_phase = (ctx->check_phase + 1) % ctx->check_stride;      // the sampled exact re-walk rotates
     CU(cudaEventRecord(ctx->ev[0], s));
     CU(cudaStreamWaitEvent(sp, ctx->ev[0], 0));         // earlier work on s may still read the buffers rewritten now
     CU(cudaStreamWaitEvent(ctx->s_ck, ctx->ev[0], 0));
@@ -1285,9 +1219,7 @@ int gpsb200_slice_prepare(gpsb200_ctx_t *ctx, const gpsb200_chan_t *chans, int n
     memset(link, 0, sizeof *link);
     rc = segment_params(ctx, chans, 0, nblk, nchan, sample_size, dst_device, sp, none, st, a, link);
     if (rc) {
-        const std::string keep = ctx->err;
         drain(ctx, s);
-        ctx->err = keep;
         return rc;
     }
     ctx->last = a;
@@ -1332,9 +1264,7 @@ int gpsb200_slice_probe(gpsb200_ctx_t *ctx, const int32_t *prn_in, const double 
         if (!rc && cudaEventRecord(ctx->ev_seg[iseg++], ctx->s_pre) != cudaSuccess) rc = fail(ctx, GPSB200_ERR_CUDA, "cudaEventRecord");
     }
     if (rc) {
-        const std::string keep = ctx->err;
         drain(ctx, ctx->pending.stream);
-        ctx->err = keep;
         ctx->pending.active = false;
         return rc;
     }
@@ -1357,12 +1287,11 @@ int slice_finish_inner(gpsb200_ctx *ctx, std::vector<ChainState> &chain, gpsb200
         // A successor waits for the outgoing state: scan EVERYTHING first (all probes were submitted up front), hand
         // the exact state on, and only then enqueue the long kernels -- a message sent behind them would wait for them.
         for (size_t i = 0; i < segs.size(); i++) {
-            SynthArgs a{};
             if (i == 0) {
                 CU(cudaEventSynchronize(ctx->ev_seg[0]));
                 trace(ctx, "probes complete");
             }
-            int rc = segment_resolve(ctx, segs[i].first, segs[i].second, nchan, sk, chain, st, i == 0, a, ctx->ev_seg[i], &slow[i]);
+            int rc = segment_scan(ctx, segs[i].first, segs[i].second, nchan, ctx->ev_seg[i], sk, chain, st, slow[i]);
             if (rc) return rc;
             after[i] = chain;
         }
@@ -1376,19 +1305,16 @@ int slice_finish_inner(gpsb200_ctx *ctx, std::vector<ChainState> &chain, gpsb200
         const int b0 = segs[i].first, b1 = segs[i].second;
         SynthArgs a{};
         fill_args(ctx, a, b0, b1 - b0, nchan, sample_size, (char *) ctx->pending.dst + (size_t) b0 * blk_bytes);
-        ctx->cur_seg = iseg;
         int rc;
-        if (ctx->pending.eager) {
-            rc = segment_checkpoints(ctx, b0, b1, nchan, sk, st, b0 == 0, a, slow[i]);
-            if (rc) return rc;
-            rc = note_segment_end(ctx, iseg++, b1, nchan, sk, after[i]);
-        } else {
+        if (!ctx->pending.eager) {
             // lazy: host scan of this segment as soon as ITS probes are done; checkpoints on a stream of their own
-            rc = segment_resolve(ctx, b0, b1, nchan, sk, chain, st, b0 == 0, a, ctx->ev_seg[iseg]);
+            rc = segment_scan(ctx, b0, b1, nchan, ctx->ev_seg[iseg], sk, chain, st, slow[i]);
             if (rc) return rc;
-            rc = note_segment_end(ctx, iseg++, b1, nchan, sk, chain);
         }
+        ctx->cur_seg = iseg;
+        rc = segment_checkpoints(ctx, b0, b1, nchan, sk, st, b0 == 0, a, slow[i]);
         if (rc) return rc;
+        note_segment_end(ctx, iseg++, b1, nchan, ctx->pending.eager ? after[i] : chain);
         CU(cudaEventRecord(ctx->ev_done[ichunk], sk));
         CU(cudaStreamWaitEvent(s, ctx->ev_done[ichunk], 0));
         ichunk++;
@@ -1438,9 +1364,7 @@ int gpsb200_slice_finish_cb(gpsb200_ctx_t *ctx, const int32_t *prn_in, const dou
     std::vector<double> xo(nchan, 0.0);
     const int rc = slice_finish_inner(ctx, chain, st, po.data(), xo.data(), handoff, user);
     if (rc) {
-        const std::string keep = ctx->err;
         drain(ctx, ctx->pending.stream);
-        ctx->err = keep;
         return rc;
     }
     SynthArgs all{};
@@ -1573,7 +1497,7 @@ int gpsb200_carrier_chain_device(gpsb200_ctx_t *ctx, const gpsb200_chan_t *chans
         CU(launch_probe(a, s));
         CU(launch_chain(a, s));
         CU(cudaStreamSynchronize(s));
-        resolve_chain(ctx, 0, nw, nchan, chain, nullptr, nullptr);
+        resolve_chain(ctx, 0, nw, nchan, chain, nullptr);
     }
     ctx->have_last = false;
     for (int c = 0; c < nchan; c++) phase_out[c] = chain[c].prn > 0 ? chain[c].phase : 0.0;
@@ -1613,14 +1537,8 @@ int gpsb200_synth_blocks(gpsb200_ctx_t *ctx, const gpsb200_chan_t *chans, int nb
                          void *dst, double *carr_phase_out, gpsb200_stats_t *stats) {
     int rc = check_call(ctx, chans, nblk, nchan, sample_size, dst);
     if (rc) return rc;
-    const size_t need = (size_t) ctx->cfg.max_blocks * GPSB200_BLOCK_ELEMS * sample_size;
-    if (ctx->out_bytes < need) {
-        cudaFree(ctx->d_out);
-        ctx->d_out = nullptr;
-        ctx->out_bytes = 0;
-        CU(cudaMalloc(&ctx->d_out, need));
-        ctx->out_bytes = need;
-    }
+    rc = ensure_staging(ctx, sample_size);
+    if (rc) return rc;
     return run_pipeline(ctx, chans, nblk, nchan, sample_size, ctx->d_out, dst, ctx->s_compute, nullptr, nullptr, nullptr,
                         carr_phase_out, stats);
 }
