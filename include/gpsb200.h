@@ -195,8 +195,15 @@ int gpsb200_link_apply(const gpsb200_slice_link_t *link, int nchan, const int32_
                        int32_t *prn_out, double *phase_out);
 
 /* Test hook of the device self-check: corrupt the resolved carrier chain of the next calls by one unit of the
- * rounding grid (on != 0); every synth call must then fail with GPSB200_ERR_INTERNAL instead of returning samples. */
+ * rounding grid (on == 1), or the carrier state one block probe recorded at a checkpoint-segment start (on == 2: slot 0,
+ * sixth block of a pipeline segment, middle segment, both parity variants); every synth call must then fail with
+ * GPSB200_ERR_INTERNAL instead of returning samples. on == 0: off. */
 int gpsb200_debug_corrupt_chain(gpsb200_ctx_t *ctx, int on);
+
+/* Test hook: copy the run checkpoints of the previous synth call (nblk x 300000/run_samples x nchan records of 24 bytes:
+ * carrier phase, code phase, NAV position iword | ibit << 8 | icode << 16, pad) to host memory. Waits for the context's
+ * work to complete. */
+int gpsb200_debug_run_checkpoints(gpsb200_ctx_t *ctx, int nblk, int nchan, void *out);
 
 /* Name of the synthesis kernel a call with nchan channels launches on this context as it stands: "k_synth_lanes"
  * (lane = sample: run length a multiple of 96 up to 2400, every code rate seen so far within 1.0157 .. 1.0302 MHz,
@@ -241,6 +248,16 @@ int gpsb200_carrier_probe_fixup(double start, double guess, double f_carr, int64
  * (starts_out[nblk + 1]) when the span-level speculation is accepted, 0 when it is rejected (the pipeline then
  * resolves the span block by block). For tests. */
 int gpsb200_span_chain_host(const double *f_carr, int nblk, double start_true, double start_guess, double *starts_out);
+
+/* Host-only model of how the run-checkpoint kernel starts the J checkpoint segments of ONE block (J = min(8, runs per
+ * block); segment j starts at run floor(j * runs / J)): the block probe from start_guess records its trajectory at the
+ * segment starts, the fix-up with the true start picks its parity variant and shift, and segment j >= 1 starts from
+ * the recorded state plus the shift when it starts at or after the probe's first wrap. run_samples divides 300000.
+ * starts_out[8]: starts_out[0] = start_true, derived starts for j >= 1, NaN for segments that are walked from the
+ * block start instead (and past J). Returns 1 when the fix-up accepts the probe (every derived start then equals
+ * gpsb200_carrier_advance(start_true, f_carr, j-th segment start) bit for bit), 0 when it rejects it. For tests. */
+int gpsb200_checkpoint_segments_host(double start_true, double start_guess, double f_carr, int run_samples,
+                                     double *starts_out, int *nseg_out);
 
 /* Host model of the lane = sample synthesis kernel (csrc/synth_lanes.h) for ONE block: the same window / band / repair
  * logic, executed on the CPU, int16 I/Q out. force bits: 1 = repair every sample's index, 2 = exact chip signs for every

@@ -36,6 +36,10 @@ CHAN_DTYPE = np.dtype([("prn", "<i4"), ("iword", "<i4"), ("ibit", "<i4"), ("icod
                        ("code_phase", "<f8"), ("gain", "<f8")])
 assert CHAN_DTYPE.itemsize == C.sizeof(Chan) == 64
 
+# one run checkpoint (gpsb200_debug_run_checkpoints): NCO state at the first sample of a run
+RUN_CKPT_DTYPE = np.dtype([("x", "<f8"), ("y", "<f8"), ("nav", "<u4"), ("pad", "<u4")])
+assert RUN_CKPT_DTYPE.itemsize == 24
+
 
 class Config(C.Structure):
     _fields_ = [("device", C.c_int32), ("max_chan", C.c_int32), ("max_blocks", C.c_int32),
@@ -84,6 +88,7 @@ EXPORTS = ["gpsb200_create", "gpsb200_destroy", "gpsb200_last_error", "gpsb200_v
            "gpsb200_carrier_advance", "gpsb200_carrier_chain", "gpsb200_carrier_chain_device", "gpsb200_carrier_probe_fixup",
            "gpsb200_codegen", "gpsb200_bind_numa", "gpsb200_span_chain_host", "gpsb200_lanes_model_block", "gpsb200_slice_prepare", "gpsb200_slice_probe",
            "gpsb200_slice_finish", "gpsb200_slice_finish_cb", "gpsb200_slice_wait", "gpsb200_link_apply", "gpsb200_slice_link_host", "gpsb200_debug_corrupt_chain", "gpsb200_synth_kernel_name",
+           "gpsb200_debug_run_checkpoints", "gpsb200_checkpoint_segments_host",
            "gpsb200_scenario_create", "gpsb200_scenario_destroy", "gpsb200_scenario_error",
            "gpsb200_scenario_blocks", "gpsb200_scenario_channels", "gpsb200_scenario_nav_frames",
            "gpsb200_scenario_chans", "gpsb200_scenario_nav", "gpsb200_scenario_almanac_date", "gpsb200_almanac_read",
@@ -139,6 +144,9 @@ def lib():
         L.gpsb200_slice_finish.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(Stats)]
         L.gpsb200_link_apply.argtypes = [C.POINTER(SliceLink), C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
         L.gpsb200_debug_corrupt_chain.argtypes = [C.c_void_p, C.c_int]
+        L.gpsb200_debug_run_checkpoints.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p]
+        L.gpsb200_checkpoint_segments_host.argtypes = [C.c_double, C.c_double, C.c_double, C.c_int, C.c_void_p,
+                                                       C.POINTER(C.c_int)]
         L.gpsb200_synth_kernel_name.argtypes = [C.c_void_p, C.c_int]
         L.gpsb200_synth_kernel_name.restype = C.c_char_p
         _lib = L
@@ -204,6 +212,19 @@ def span_chain_host(f_carr, start_true, start_guess):
     if rc < 0:
         raise GpsB200Error(rc, "gpsb200_span_chain_host")
     return out if rc == 1 else None
+
+
+def checkpoint_segments_host(start_true, start_guess, f_carr, run_samples=2400):
+    """Host model of how the run-checkpoint kernel starts the checkpoint segments of one block.
+    -> (accepted, starts float64[J]): starts[0] = start_true, derived start phases of the later segments (NaN for
+    those walked from the block start; all NaN when the fix-up rejected the probe)."""
+    out = np.zeros(8)
+    nseg = C.c_int(0)
+    rc = lib().gpsb200_checkpoint_segments_host(float(start_true), float(start_guess), float(f_carr), int(run_samples),
+                                            out.ctypes.data, C.byref(nseg))
+    if rc < 0:
+        raise GpsB200Error(rc, "gpsb200_checkpoint_segments_host")
+    return rc == 1, out[:nseg.value]
 
 
 def slice_link_host(chans):
@@ -396,7 +417,15 @@ class Context:
         return lib().gpsb200_synth_kernel_name(self._h, int(nchan)).decode()
 
     def debug_corrupt_chain(self, on):
-        self._check(lib().gpsb200_debug_corrupt_chain(self._h, 1 if on else 0))
+        """on: False/0 off, True/1 corrupt the resolved chain, 2 corrupt a recorded checkpoint-segment state."""
+        self._check(lib().gpsb200_debug_corrupt_chain(self._h, int(on)))
+
+    def debug_run_checkpoints(self, nblk, nchan):
+        """The previous call's run checkpoints -> structured array [nblk, runs per block, nchan] (x, y, nav, pad)."""
+        nruns = BLOCK_SAMPLES // (self.cfg.run_samples or 2400)
+        out = np.zeros((nblk, nruns, nchan), RUN_CKPT_DTYPE)
+        self._check(lib().gpsb200_debug_run_checkpoints(self._h, nblk, nchan, out.ctypes.data))
+        return out
 
     def carrier_chain(self, chans, phase_in=None):
         """Exact carrier phases after all blocks of chans (device probe + host fix-up, no synthesis)."""

@@ -138,6 +138,7 @@ struct gpsb200_ctx {
     double *d_carr0 = nullptr, *h_carr0 = nullptr;     // exact block-start phases of host-resolved (irregular) spans
     CarrierProbe *d_probe = nullptr;                   // block probes in HBM (k_chain reads them)
     CarrierProbe *h_probe = nullptr, *d_probe_host = nullptr;   // ... and in mapped host memory (host fallback)
+    double *d_seg = nullptr;                           // [block][chan][kSegStates] probe states at checkpoint-segment starts
     CarrierProbe *h_span_sum = nullptr, *d_span_sum = nullptr;  // span summaries, mapped host memory
     SpanBlockState *d_spec = nullptr;                  // speculative block-start phases
     bool lanes_on = true;                              // GPSB200_LANES=0: always k_synth (lane = channel)
@@ -149,7 +150,7 @@ struct gpsb200_ctx {
     std::vector<double> seg_expect;        // what the chain says they must be
     std::vector<cudaEvent_t> ev_seg;       // slice path: probes of segment i complete
     void *const *scatter = nullptr;        // gpsb200_synth_blocks_scatter: one host destination per block
-    bool fault_inject_chain = false;
+    int fault_inject_chain = 0;            // gpsb200_debug_corrupt_chain(): 1 = resolution, 2 = segment state
     bool trace_on = false;
     double trace_t0 = 0.0;       // gpsb200_debug_corrupt_chain(): test hook of the device self-check
     // state of a begun, not yet finished call (gpsb200_synth_begin / _finish)
@@ -449,7 +450,7 @@ int64_t resolve_chain(gpsb200_ctx *ctx, int b0, int b1, int nchan, std::vector<C
     // test hook of the device self-check (gpsb200_debug_corrupt_chain): corrupt the resolution of slot 0's first span
     // by one unit of the rounding grid -- the span's shift, or the start phase of block b0 + 5 when the span was
     // resolved block by block; k_checkpoints must notice
-    if (ctx->fault_inject_chain && b1 - b0 > 6) {
+    if (ctx->fault_inject_chain == 1 && b1 - b0 > 6) {
         SpanRes &r = ctx->h_span_res[(size_t) (b0 / K) * nchan];
         if (r.mode == 0) r.shift += 0x1p-51;
         else if (r.mode == 1) ctx->h_carr0[(size_t) (b0 + 5) * nchan] += 0x1p-51;
@@ -470,6 +471,7 @@ void fill_args(gpsb200_ctx *ctx, SynthArgs &a, int blk0, int nblk, int nchan, in
     a.guess = ctx->d_guess + off;
     a.probe = ctx->d_probe + off;
     a.probe_host = ctx->d_probe_host + off;
+    a.seg = ctx->d_seg + off * kSegStates;
     a.spec = ctx->d_spec + off;
     a.span_blocks = kSpanBlocks;
     a.nspan = (nblk + kSpanBlocks - 1) / kSpanBlocks;
@@ -569,7 +571,8 @@ int segment_params(gpsb200_ctx *ctx, const gpsb200_chan_t *chans, int b0, int b1
     return GPSB200_OK;
 }
 
-// Second part: everything speculative -- guesses up, block probes, span chaining. Needs no true start phase.
+// Second part: everything that needs no true start phase -- guesses up, block probes (+ the code-NCO half of the run
+// checkpoints, which segment_checkpoints relies on), span chaining.
 int segment_probe(gpsb200_ctx *ctx, int b0, int b1, int nchan, cudaStream_t sp, gpsb200_stats_t &st, bool first,
                   const SynthArgs &a) {
     const size_t off = (size_t) b0 * nchan, cnt = (size_t) (b1 - b0) * nchan;
@@ -610,6 +613,19 @@ int segment_checkpoints(gpsb200_ctx *ctx, int b0, int b1, int nchan, cudaStream_
     if (slow > 0) {                                  // rare: block start phases of the host-resolved spans
         CU(cudaMemcpyAsync(ctx->d_carr0 + off, ctx->h_carr0 + off, cnt * sizeof(double), cudaMemcpyHostToDevice, sp));
         st.h2d_bytes += (int64_t) (cnt * sizeof(double));
+    }
+    // test hook of the device self-check (gpsb200_debug_corrupt_chain mode 2): move the state that block b0 + 5's probe
+    // recorded for slot 0 at the start of the middle checkpoint segment by one unit of the rounding grid (the probes
+    // are complete: the host scan waited for them); k_checkpoints must notice
+    const int jm = ckpt_segments(ctx->nruns) / 2;
+    if (ctx->fault_inject_chain == 2 && b1 - b0 > 6 && jm >= 1) {
+        double *p = ctx->d_seg + (size_t) (b0 + 5) * nchan * kSegStates, h[kSegStates];
+        CU(cudaMemcpyAsync(h, p, sizeof h, cudaMemcpyDeviceToHost, sp));
+        CU(cudaStreamSynchronize(sp));
+        h[jm - 1] += 0x1p-51;
+        h[kCkptSegs - 1 + jm - 1] += 0x1p-51;
+        CU(cudaMemcpyAsync(p, h, sizeof h, cudaMemcpyHostToDevice, sp));
+        CU(cudaStreamSynchronize(sp));
     }
     SynthArgs ack = a;
     ack.last_end_host = ctx->cur_seg < ctx->max_segs ? ctx->d_seg_end + (size_t) ctx->cur_seg * nchan : nullptr;
@@ -687,11 +703,12 @@ int small_call(gpsb200_ctx *ctx, const gpsb200_chan_t *chans, int nblk, int ncha
                 stc.prn = p.prn;
                 double x = stc.phase, y = p.code0;
                 int iword = p.nav0 & 0xFF, ibit = (p.nav0 >> 8) & 0xFF, icode = (p.nav0 >> 16) & 0xFF;
+                const WalkConst wx = walk_const(p.c_carr), wy = walk_const(p.c_code);
                 for (int r = 0; r < nruns; r++) {
                     ck[(size_t) r * nchan] = RunCkpt{x, y, (uint32_t) iword | ((uint32_t) ibit << 8) | ((uint32_t) icode << 16), 0u};
                     int64_t periods = 0, dummy = 0;
-                    nco_advance<NCO_CARRIER>(x, p.c_carr, run, dummy);
-                    nco_advance<NCO_CODE>(y, p.c_code, run, periods);
+                    nco_advance<NCO_CARRIER>(x, wx, run, dummy);
+                    nco_advance<NCO_CODE>(y, wy, run, periods);
                     nav_advance(iword, ibit, icode, periods);
                 }
                 stc.phase = x;
@@ -1006,6 +1023,28 @@ int gpsb200_span_chain_host(const double *f_carr, int nblk, double start_true, d
     return 1;
 }
 
+int gpsb200_checkpoint_segments_host(double start_true, double start_guess, double f_carr, int run_samples,
+                                     double *starts_out, int *nseg_out) {
+    // Host-only model of ONE block of k_probe (both variants, segment-start states) and of how k_checkpoints starts
+    // its segments from them
+    if (!starts_out || run_samples <= 0 || GPSB200_BLOCK_SAMPLES % run_samples != 0) return GPSB200_ERR_ARG;
+    const double c = f_carr * (1.0 / (double) GPSB200_SAMPLERATE);
+    const int nruns = GPSB200_BLOCK_SAMPLES / run_samples, nseg = ckpt_segments(nruns);
+    CarrierProbe p;
+    double seg[kSegStates];
+    for (int v = 0; v < 2; v++)
+        carrier_probe_variant(start_guess, c, GPSB200_BLOCK_SAMPLES, v, p, seg + v * (kCkptSegs - 1), nruns, run_samples);
+    if (nseg_out) *nseg_out = nseg;
+    starts_out[0] = start_true;
+    for (int j = 1; j < kCkptSegs; j++) starts_out[j] = NAN;
+    double xe, d;
+    int v;
+    if (!carrier_fixup(start_true, c, p, xe, &v, &d)) return 0;
+    for (int j = first_derived_segment(p, nseg, nruns, run_samples); j < nseg; j++)
+        starts_out[j] = seg[v * (kCkptSegs - 1) + j - 1] + d;
+    return 1;
+}
+
 int gpsb200_carrier_chain(const gpsb200_chan_t *chans, int nblk, int nchan, const double *phase_in,
                           double *phase_out, int threads) {
     if (!chans || !phase_out || nblk < 0 || nchan < 1) return GPSB200_ERR_ARG;
@@ -1101,6 +1140,7 @@ int gpsb200_create(const gpsb200_config_t *cfg, gpsb200_ctx_t **out) {
     CU(cudaMalloc(&ctx->d_probe, nbc * sizeof(CarrierProbe)));
     CU(cudaHostAlloc(&ctx->h_probe, nbc * sizeof(CarrierProbe), cudaHostAllocMapped));
     CU(cudaHostGetDevicePointer((void **) &ctx->d_probe_host, ctx->h_probe, 0));
+    CU(cudaMalloc(&ctx->d_seg, nbc * kSegStates * sizeof(double)));      // only k_checkpoints reads them: HBM only
     ctx->max_spans = (c.max_blocks + kSpanBlocks - 1) / kSpanBlocks + 1;
     const size_t nsc = (size_t) ctx->max_spans * c.max_chan;
     CU(cudaHostAlloc(&ctx->h_span_sum, nsc * sizeof(CarrierProbe), cudaHostAllocMapped));
@@ -1149,6 +1189,7 @@ void gpsb200_destroy(gpsb200_ctx_t *ctx) {
     cudaFreeHost(ctx->h_carr0);
     cudaFreeHost(ctx->h_probe);
     cudaFree(ctx->d_probe);
+    cudaFree(ctx->d_seg);
     cudaFreeHost(ctx->h_span_sum);
     cudaFree(ctx->d_spec);
     cudaFree(ctx->d_span_res);
@@ -1465,8 +1506,18 @@ const char *gpsb200_synth_kernel_name(const gpsb200_ctx_t *ctx, int nchan) {
 }
 
 int gpsb200_debug_corrupt_chain(gpsb200_ctx_t *ctx, int on) {
-    if (!ctx) return GPSB200_ERR_ARG;
-    ctx->fault_inject_chain = on != 0;
+    if (!ctx || on < 0 || on > 2) return GPSB200_ERR_ARG;
+    ctx->fault_inject_chain = on;
+    return GPSB200_OK;
+}
+
+int gpsb200_debug_run_checkpoints(gpsb200_ctx_t *ctx, int nblk, int nchan, void *out) {
+    if (!ctx || !out || nblk < 1 || nblk > ctx->cfg.max_blocks || nchan < 1 || nchan > ctx->cfg.max_chan)
+        return GPSB200_ERR_ARG;
+    if (!ctx->s_compute) return fail(ctx, GPSB200_ERR_CUDA, "context has no CUDA device");
+    CU(cudaSetDevice(ctx->cfg.device));
+    CU(cudaDeviceSynchronize());             // the call's streams may be the caller's
+    CU(cudaMemcpy(out, ctx->d_ck, (size_t) nblk * ctx->nruns * nchan * sizeof(RunCkpt), cudaMemcpyDeviceToHost));
     return GPSB200_OK;
 }
 
@@ -1494,6 +1545,7 @@ int gpsb200_carrier_chain_device(gpsb200_ctx_t *ctx, const gpsb200_chan_t *chans
         CU(cudaMemcpyAsync(ctx->d_guess, ctx->h_guess, cnt * sizeof(double), cudaMemcpyHostToDevice, s));
         SynthArgs a{};
         fill_args(ctx, a, 0, nw, nchan, GPSB200_SC08, nullptr);
+        a.ck = nullptr;                                // no run checkpoints: the probes need no code walk
         CU(launch_probe(a, s));
         CU(launch_chain(a, s));
         CU(cudaStreamSynchronize(s));

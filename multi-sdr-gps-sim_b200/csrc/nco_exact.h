@@ -241,13 +241,13 @@ GPSB_HD bool walk_iteration(double &x, const WalkConst &w, double &nd, int64_t &
     return wrapped;
 }
 
-// Advance x by exactly n reference steps of increment c (n < 2^31).
+// Advance x by exactly n reference steps of increment w.c (n < 2^31); w = walk_const(c), computed once by callers
+// that advance the same increment many times (one call per run).
 // Returns the number of loop iterations spent (diagnostics only).
 template <int KIND>
-GPSB_HD int nco_advance(double &x, double c, int64_t n, int64_t &periods) {
-    if (c == 0.0 || n <= 0) return 0;
-    const WalkConst w = walk_const(c);
-    if (!w.fast || (KIND == NCO_CODE && w.neg)) return nco_advance_generic<KIND>(x, c, n, periods);
+GPSB_HD int nco_advance(double &x, const WalkConst &w, int64_t n, int64_t &periods) {
+    if (w.c == 0.0 || n <= 0) return 0;
+    if (!w.fast || (KIND == NCO_CODE && w.neg)) return nco_advance_generic<KIND>(x, w.c, n, periods);
     int iters = 0;
     double nd = (double) n;
     while (nd > 0.0) {
@@ -255,6 +255,12 @@ GPSB_HD int nco_advance(double &x, double c, int64_t n, int64_t &periods) {
         walk_iteration<KIND>(x, w, nd, periods, nullptr);
     }
     return iters;
+}
+
+template <int KIND>
+GPSB_HD int nco_advance(double &x, double c, int64_t n, int64_t &periods) {
+    if (c == 0.0 || n <= 0) return 0;
+    return nco_advance<KIND>(x, walk_const(c), n, periods);
 }
 
 // ---------------------------------------------------------------------------------
@@ -341,32 +347,61 @@ GPSB_HD int64_t carrier_walk(double &x, double c, int64_t n, bool stop_at_wrap, 
     return carrier_walk_w(x, w, n, stop_at_wrap, wrapped, ok, m_pos, m_neg);
 }
 
+// Checkpoint segments: k_checkpoints walks the carrier of a block in J = ckpt_segments(nruns) segments of
+// consecutive runs, one thread each (125 runs: 15 or 16 per segment). Segment j starts at run seg_first_run(j);
+// seg_first_run(J) = nruns.
+constexpr int kCkptSegs = 8;
+constexpr int kSegStates = 2 * (kCkptSegs - 1);        // recorded states per (block, channel): [variant][j - 1]
+GPSB_HD int ckpt_segments(int nruns) { return nruns < kCkptSegs ? nruns : kCkptSegs; }
+GPSB_HD int seg_first_run(int j, int nseg, int nruns) { return j * nruns / nseg; }
+
 // One parity variant v of the probe (the device runs the two variants in different threads;
-// each repeats the short walk to the first wrap). Fills n_w/x_w (identical for both v) and
-// the v-th end state and margins.
-GPSB_HD void carrier_probe_variant(double guess, double c, int64_t n, int v, CarrierProbe &o) {
+// each repeats the short walk to the first wrap): n_w/x_w (identical for both v) and the v-th
+// end state and margins of CarrierProbe, as scalars.
+// seg (optional): variant v's state at the start s_j = seg_first_run(j) * run_samples of every interior checkpoint
+// segment j = 1 .. J-1 goes to seg[j-1], for s_j >= n_w (the others are not written). The walk stops at each s_j,
+// which only shortens a jump: the states, margins and end state are the same as without.
+GPSB_HD void carrier_probe_walk(double guess, double c, int64_t n, int v, int32_t &n_w, double &x_w, double &x_end,
+                                double &m_pos, double &m_neg, double *seg = nullptr, int nruns = 0,
+                                int run_samples = 0) {
+    const WalkConst w = walk_const(c);
     double x = guess;
     bool wrapped = false, ok = true;
-    const int64_t nw = carrier_walk(x, c, n, true, wrapped, ok, nullptr, nullptr);
-    o.pad = 0;
+    const int64_t nw = carrier_walk_w(x, w, n, true, wrapped, ok, nullptr, nullptr);
+    x_w = x;
     if (!wrapped || !ok) {
-        o.n_w = -1;
-        o.x_w = x;
-        o.x_end[v] = x;
-        o.m_pos[v] = o.m_neg[v] = 0.0;
+        n_w = -1;
+        x_end = x;
+        m_pos = m_neg = 0.0;
         return;
     }
-    o.n_w = (int32_t) nw;
-    o.x_w = x;
+    n_w = (int32_t) nw;
     double xv = x + (v ? carrier_grid(c) : 0.0);       // exact: x_w is a multiple of G
     double mp = 1.0, mn = 1.0;
     bool w2, ok2;
     // a parity partner that left [0,1) (x_w at the very edge) is simply unusable
-    if (!(xv >= 0.0 && xv < 1.0)) mp = mn = 0.0;
-    else carrier_walk(xv, c, n - nw, false, w2, ok2, &mp, &mn);
-    o.x_end[v] = xv;
-    o.m_pos[v] = mp;
-    o.m_neg[v] = mn;
+    if (!(xv >= 0.0 && xv < 1.0)) {
+        mp = mn = 0.0;
+    } else {
+        int64_t pos = nw;
+        const int nseg = seg ? ckpt_segments(nruns) : 1;
+        for (int j = 1; j <= nseg; j++) {               // to every segment start, then to the end of the block
+            const int64_t s = j < nseg ? seg_first_run(j, nseg, nruns) * run_samples : n;
+            if (s < pos) continue;                      // before the first wrap: not derivable
+            carrier_walk_w(xv, w, s - pos, false, w2, ok2, &mp, &mn);
+            pos = s;
+            if (j < nseg) seg[j - 1] = xv;
+        }
+    }
+    x_end = xv;
+    m_pos = mp;
+    m_neg = mn;
+}
+
+GPSB_HD void carrier_probe_variant(double guess, double c, int64_t n, int v, CarrierProbe &o, double *seg = nullptr,
+                                   int nruns = 0, int run_samples = 0) {
+    o.pad = 0;
+    carrier_probe_walk(guess, c, n, v, o.n_w, o.x_w, o.x_end[v], o.m_pos[v], o.m_neg[v], seg, nruns, run_samples);
 }
 
 GPSB_HD void carrier_probe(double guess, double c, int64_t n, CarrierProbe &o) {
@@ -405,6 +440,16 @@ GPSB_HD bool carrier_fixup(double s, double c, const CarrierProbe &p, double &x_
     if (v_out) *v_out = v;
     if (d_out) *d_out = d;
     return true;
+}
+
+// Once carrier_fixup() has accepted a block probe (variant v, shift d), the true state at the start of checkpoint
+// segment j is seg[v][j-1] + d -- exact for the same reason x_end[v] + d is: the margins cover every state of the
+// variant's trajectory after the first wrap -- for the segments that start at or after that wrap, i.e. from
+// first_derived_segment() on (J: none). The segments before it are walked from the block's start.
+GPSB_HD int first_derived_segment(const CarrierProbe &p, int nseg, int nruns, int run_samples) {
+    int j = 1;
+    while (j < nseg && seg_first_run(j, nseg, nruns) * run_samples < p.n_w) j++;
+    return j;
 }
 
 // ---------------------------------------------------------------------------------------------------

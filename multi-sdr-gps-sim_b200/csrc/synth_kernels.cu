@@ -6,15 +6,18 @@
 // Work decomposition
 //   block  = 0.1 s = 300000 samples (the reference's unit, sdr.h:26)
 //   run    = run_samples consecutive samples of one block (default 2400)
-//   k_probe       : one thread per (block, channel) walks the carrier NCO through the
-//                   block from a GUESSED start phase (speculative, parallel in time);
-//                   the host turns the probes into exact start phases (nco_exact.h).
+//   k_probe       : two threads per (block, channel) walk the carrier NCO through the
+//                   block from a GUESSED start phase (speculative, parallel in time) and
+//                   record its state at the checkpoint-segment starts; the host turns the
+//                   probes into exact start phases (nco_exact.h). A third thread walks the
+//                   code NCO (+ NAV position) and stores it at every run start.
 //   k_tables      : one thread per (block, carrier-table row < 256, lane column): the gain-scaled
 //                   carrier table of every block, written once to HBM; k_synth's CTAs (several
 //                   per block) fetch it with one TMA bulk copy each instead of recomputing it.
-//   k_checkpoints : two threads per (block, channel) walk the code and the carrier NCO
-//                   through the block with the exact O(#binade crossings) fast-forward
-//                   and store the state at every run start.
+//   k_checkpoints : one thread per (checkpoint segment, block, channel) walks the carrier
+//                   NCO through its segment's runs with the exact O(#binade crossings)
+//                   fast-forward, from a start state derived from the block probe, and
+//                   stores the phase at every run start.
 //   k_synth       : one warp per run (32 channels) or per 2/4 runs (<=16/<=8
 //                   channels). LANE = CHANNEL: every lane steps its channel's two
 //                   FP64 NCOs sample by sample with the reference's own rounding
@@ -84,26 +87,48 @@ __device__ __forceinline__ bool map_block_chan(const SynthArgs &a, int idx, int 
     return c < a.nchan && b < a.nblk;
 }
 
+// The code NCO (+ NAV position) of block b, channel c, walked exactly through the block; its state at every run start
+// goes to the run checkpoints (the carrier phase is k_checkpoints' part). Needs no carrier-chain result.
+__device__ __forceinline__ void code_walk(const SynthArgs &a, int b, int c) {
+    const BlockChanDev p = a.bc[(size_t) b * a.nchan + c];
+    RunCkpt *ck = a.ck + (size_t) b * a.nruns * a.nchan + c;
+    const WalkConst w = walk_const(p.c_code);
+    double y = p.code0;
+    int iword = p.nav0 & 0xFF, ibit = (p.nav0 >> 8) & 0xFF, icode = (p.nav0 >> 16) & 0xFF;
+    for (int r = 0; r < a.nruns; r++) {
+        RunCkpt *o = ck + (size_t) r * a.nchan;
+        o->y = y;
+        o->nav = (uint32_t) iword | ((uint32_t) ibit << 8) | ((uint32_t) icode << 16);
+        o->pad = 0;
+        if (p.prn <= 0) continue;
+        int64_t periods = 0;
+        nco_advance<NCO_CODE>(y, w, a.run_samples, periods);
+        nav_advance(iword, ibit, icode, periods);
+    }
+}
+
 __global__ void __launch_bounds__(128) k_probe(SynthArgs a) {
-    // two threads per (block, channel): one per parity variant (nco_exact.h); a warp is 32 consecutive
-    // blocks of one channel
+    // roles 0, 1: one thread per (block, channel) and parity variant v = role (nco_exact.h); role 2 (a.ck set): one
+    // thread per (block, channel) walks the code NCO -- in the shadow of the longer carrier walks, which come first in
+    // the grid. A warp is 32 consecutive blocks of one channel.
     const int nblk_pad = (a.nblk + 31) & ~31;
     const int per_v = nblk_pad * a.nchan;
     int idx = blockIdx.x * blockDim.x + threadIdx.x;
     const int v = idx / per_v;
     idx -= v * per_v;
     int b, c;
-    if (v > 1 || !map_block_chan(a, idx, b, c)) return;
+    if (v > 2 || !map_block_chan(a, idx, b, c)) return;
+    if (v == 2) {
+        if (a.ck) code_walk(a, b, c);
+        return;
+    }
     const size_t i = (size_t) b * a.nchan + c;
     const BlockChanDev p = a.bc[i];
-    CarrierProbe o;
-    if (p.prn > 0) {
-        carrier_probe_variant(a.guess[i], p.c_carr, kBlockSamples, v, o);
-    } else {
-        o.n_w = -1;
-        o.x_w = 0.0;
-        o.x_end[v] = o.m_pos[v] = o.m_neg[v] = 0.0;
-    }
+    int32_t n_w = -1;
+    double x_w = 0.0, x_end = 0.0, m_pos = 0.0, m_neg = 0.0;
+    if (p.prn > 0)
+        carrier_probe_walk(a.guess[i], p.c_carr, kBlockSamples, v, n_w, x_w, x_end, m_pos, m_neg,
+                           a.seg + i * kSegStates + v * (kCkptSegs - 1), a.nruns, a.run_samples);
     // two copies: HBM for k_chain, mapped host memory for the host's (rare) block-by-block fallback
     CarrierProbe *dsts[2] = {a.probe + i, a.probe_host ? a.probe_host + i : nullptr};
 #pragma unroll
@@ -111,13 +136,13 @@ __global__ void __launch_bounds__(128) k_probe(SynthArgs a) {
         CarrierProbe *dst = dsts[k];
         if (!dst) continue;
         if (v == 0) {
-            dst->x_w = o.x_w;
-            dst->n_w = o.n_w;
+            dst->x_w = x_w;
+            dst->n_w = n_w;
             dst->pad = 0;
         }
-        dst->x_end[v] = o.x_end[v];
-        dst->m_pos[v] = o.m_pos[v];
-        dst->m_neg[v] = o.m_neg[v];
+        dst->x_end[v] = x_end;
+        dst->m_pos[v] = m_pos;
+        dst->m_neg[v] = m_neg;
     }
 }
 
@@ -168,53 +193,57 @@ __device__ __forceinline__ double resolved_start(const SynthArgs &a, int b, int 
 }
 
 __global__ void __launch_bounds__(128) k_checkpoints(SynthArgs a) {
-    // role 0: one thread per (block, channel) walks the code NCO (+ NAV position) through the block;
-    // role 1: one thread per (block, channel) walks the carrier through the block from its resolved start
+    // one thread per (checkpoint segment j, block, channel); a warp is 32 consecutive blocks of one channel for one j
     const int nblk_pad = (a.nblk + 31) & ~31;
-    const int per_code = nblk_pad * a.nchan;
+    const int per_j = nblk_pad * a.nchan;
+    const int nseg = ckpt_segments(a.nruns);
     int idx = blockIdx.x * blockDim.x + threadIdx.x;
+    const int j = idx / per_j;
+    idx -= j * per_j;
     int b, c;
-    if (idx < per_code) {
-        if (!map_block_chan(a, idx, b, c)) return;
-        const BlockChanDev p = a.bc[(size_t) b * a.nchan + c];
-        RunCkpt *ck = a.ck + (size_t) b * a.nruns * a.nchan + c;
-        double y = p.code0;
-        int iword = p.nav0 & 0xFF, ibit = (p.nav0 >> 8) & 0xFF, icode = (p.nav0 >> 16) & 0xFF;
-        for (int r = 0; r < a.nruns; r++) {
-            RunCkpt *o = ck + (size_t) r * a.nchan;
-            o->y = y;
-            o->nav = (uint32_t) iword | ((uint32_t) ibit << 8) | ((uint32_t) icode << 16);
-            o->pad = 0;
-            if (p.prn <= 0) continue;
-            int64_t periods = 0;
-            nco_advance<NCO_CODE>(y, p.c_code, a.run_samples, periods);
-            nav_advance(iword, ibit, icode, periods);
-        }
-        return;
-    }
-    idx -= per_code;
-    if (!map_block_chan(a, idx, b, c)) return;
+    if (j >= nseg || !map_block_chan(a, idx, b, c)) return;
     const size_t i = (size_t) b * a.nchan + c;
     const BlockChanDev p = a.bc[i];
     RunCkpt *ck = a.ck + (size_t) b * a.nruns * a.nchan + c;
     if (p.prn <= 0) {
-        for (int r = 0; r < a.nruns; r++) ck[(size_t) r * a.nchan].x = 0.0;
-        if (a.carr_end) a.carr_end[i] = 0.0;
-        if (a.last_end_host && b == a.nblk - 1) a.last_end_host[c] = 0.0;
+        for (int r = seg_first_run(j, nseg, a.nruns); r < seg_first_run(j + 1, nseg, a.nruns); r++)
+            ck[(size_t) r * a.nchan].x = 0.0;
+        if (j == nseg - 1) {
+            if (a.carr_end) a.carr_end[i] = 0.0;
+            if (a.last_end_host && b == a.nblk - 1) a.last_end_host[c] = 0.0;
+        }
         return;
     }
-    // exact walk of the whole block from its resolved start
-    double x = resolved_start(a, b, c);
-    for (int r = 0; r < a.nruns; r++) {
+    // Where the segments start: from the block probe, when it fits the block's resolved start (variant v, shift d),
+    // for every segment from j_d = first_derived_segment() on. Thread 0 walks the segments before j_d (all of them
+    // when the probe does not fit) from the resolved start.
+    const double s = resolved_start(a, b, c);
+    const CarrierProbe &pr = a.probe[i];
+    int v = 0;
+    double d = 0.0, xe;
+    const int jd = carrier_fixup(s, p.c_carr, pr, xe, &v, &d) ? first_derived_segment(pr, nseg, a.nruns, a.run_samples)
+                                                               : nseg;
+    if (j > 0 && j < jd) return;
+    const double *seg = a.seg + i * kSegStates + v * (kCkptSegs - 1);
+    const int jn = j == 0 ? jd : j + 1;                          // the segment that follows this thread's walk
+    double x = j == 0 ? s : seg[j - 1] + d;                      // exact: see first_derived_segment()
+    const WalkConst w = walk_const(p.c_carr);
+    for (int r = seg_first_run(j, nseg, a.nruns); r < seg_first_run(jn, nseg, a.nruns); r++) {
         ck[(size_t) r * a.nchan].x = x;
         int64_t dummy = 0;
-        nco_advance<NCO_CARRIER>(x, p.c_carr, a.run_samples, dummy);
+        nco_advance<NCO_CARRIER>(x, w, a.run_samples, dummy);
     }
-    // ... whose end must BE the start phase resolved for the next block of the same satellite in this launch
-    const bool bad = b + 1 < a.nblk && a.bc[i + a.nchan].prn == p.prn && f64_bits(resolved_start(a, b + 1, c)) != f64_bits(x);
+    // The walked end must BE the derived start of the next segment, or after the last segment the start phase resolved
+    // for the next block of the same satellite in this launch
+    bool bad;
+    if (jn < nseg) {
+        bad = f64_bits(seg[jn - 1] + d) != f64_bits(x);
+    } else {
+        bad = b + 1 < a.nblk && a.bc[i + a.nchan].prn == p.prn && f64_bits(resolved_start(a, b + 1, c)) != f64_bits(x);
+        if (a.carr_end) a.carr_end[i] = x;
+        if (a.last_end_host && b == a.nblk - 1) a.last_end_host[c] = x;
+    }
     if (bad && a.chain_errors) atomicAdd(a.chain_errors, 1);
-    if (a.carr_end) a.carr_end[i] = x;
-    if (a.last_end_host && b == a.nblk - 1) a.last_end_host[c] = x;
 }
 
 // ---------------------------------------------------------------------------------
@@ -525,7 +554,7 @@ cudaError_t launch_tables(const SynthArgs &a, cudaStream_t s) {
 
 cudaError_t launch_checkpoints(const SynthArgs &a, cudaStream_t s) {
     const int nblk_pad = (a.nblk + 31) & ~31;
-    const long total = 2L * nblk_pad * a.nchan;
+    const long total = (long) ckpt_segments(a.nruns) * nblk_pad * a.nchan;
     const int threads = 128;
     k_checkpoints<<<(unsigned) ((total + threads - 1) / threads), threads, 0, s>>>(a);
     return cudaGetLastError();
@@ -533,7 +562,7 @@ cudaError_t launch_checkpoints(const SynthArgs &a, cudaStream_t s) {
 
 cudaError_t launch_probe(const SynthArgs &a, cudaStream_t s) {
     const int nblk_pad = (a.nblk + 31) & ~31;
-    const long total = 2L * nblk_pad * a.nchan;
+    const long total = (a.ck ? 3L : 2L) * nblk_pad * a.nchan;
     const int threads = 128;
     k_probe<<<(unsigned) ((total + threads - 1) / threads), threads, 0, s>>>(a);
     return cudaGetLastError();

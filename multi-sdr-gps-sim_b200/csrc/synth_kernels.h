@@ -51,11 +51,12 @@ struct SynthArgs {
     const double *guess;      // [nblk][nchan] guessed start phases for the speculative probe
     CarrierProbe *probe;      // [nblk][nchan] block probes (device copy, read by k_chain)
     CarrierProbe *probe_host; // same, mapped host memory: the host's block-by-block fallback reads them
+    double *seg;              // [nblk][nchan][kSegStates] the probes' states at the checkpoint-segment starts (nco_exact.h)
     CarrierProbe *span_sum;   // [nspan][nchan] span summaries (mapped host memory)
     SpanBlockState *spec;     // [nblk][nchan] speculative block-start phases per span variant
     const SpanRes *span_res;  // [nspan][nchan] the host scan's resolution of every span
     int span_blocks, nspan;
-    RunCkpt *ck;              // [nblk][nruns][nchan]
+    RunCkpt *ck;              // [nblk][nruns][nchan]; NULL for probes without checkpoints (no code walk)
     const uint32_t *nav;      // [frames][nav_stride][60]: rows are the context's channel slots (cfg.max_chan >= nchan)
     int nav_stride;
     const uint32_t *chipbits; // [33][33] packed C/A chips per PRN (bit n = ca[n mod 1023]), row 0 unused
@@ -71,11 +72,13 @@ struct SynthArgs {
 
 // Gain-scaled carrier tables of every block (gps.c:2781-2782), fetched by k_synth with TMA bulk copies.
 cudaError_t launch_tables(const SynthArgs &a, cudaStream_t s);
-// Speculative carrier walk of every (block, channel) from a guessed start phase (nco_exact.h).
+// Speculative carrier walk of every (block, channel) from a guessed start phase (nco_exact.h), plus (a.ck set) the
+// exact code-NCO walk that writes the code phase and NAV position of every run checkpoint.
 cudaError_t launch_probe(const SynthArgs &a, cudaStream_t s);
 // Speculative chaining of the block probes inside every span, both parity variants (nco_exact.h: span_chain).
 cudaError_t launch_chain(const SynthArgs &a, cudaStream_t s);
-// Run-start checkpoints for every (block, channel): exact walk, O(#binade crossings).
+// Run-start carrier phases for every (block, channel): exact walk, O(#binade crossings), one thread per checkpoint
+// segment. Needs the probes of the same blocks (launch_probe with a.ck set) and the host scan's resolution.
 cudaError_t launch_checkpoints(const SynthArgs &a, cudaStream_t s);
 // The per-sample synthesis (gps.c:2767-2857): lanes = channels, warp-sum over channels.
 cudaError_t launch_synth(const SynthArgs &a, cudaStream_t s);
