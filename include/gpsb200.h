@@ -41,7 +41,8 @@ enum {
     GPSB200_ERR_CUDA = -2,       /* CUDA runtime error; text via gpsb200_last_error() */
     GPSB200_ERR_RANGE = -3,      /* sum of channel amplitudes would overflow the int16 I/Q the reference stores */
     GPSB200_ERR_NOMEM = -4,
-    GPSB200_ERR_INTERNAL = -5    /* device self-check failed (would mean a bug; never returns wrong samples silently) */
+    GPSB200_ERR_INTERNAL = -5,   /* device self-check failed (would mean a bug; never returns wrong samples silently) */
+    GPSB200_ERR_END = -6         /* gpsb200_scenario_advance / _key: no block of the run left */
 };
 
 /* One channel for one 0.1 s block: the fields of the reference's channel_t
@@ -293,7 +294,10 @@ typedef struct gpsb200_scenario_config {
     double start_sec;
     /* -t distance,bearing,height (gps-sim.c:145-148, gps.c:2348-2357): static runs start at a point given by distance
      * [m] and bearing [deg] from the location, height offset [m]; ignored with a motion file, as in the reference */
-    int32_t target_valid, reserved;
+    int32_t target_valid;
+    /* -i: the receiver is steered by gpsb200_scenario_key between advances (gps.c:2714-2729); ignored with a motion
+     * file (gps-sim.c:297-301). Without keys the run equals the static one bit for bit. */
+    int32_t interactive;
     double target_distance_m, target_bearing_deg, target_height_m;
     /* SEM almanac file sent in subframe 4 pages 2-5/7-10 (PRN 25-32) and subframe 5 pages 1-25 (PRN 1-24, toa/WNa);
      * NULL = no almanac (the reference's --disable-almanac). Read as the reference reads ./almanac.sem: at most 32
@@ -315,6 +319,36 @@ const uint32_t *gpsb200_scenario_nav(const gpsb200_scenario_t *s);           /* 
 /* Time of applicability of the almanac in use as "yyyy/mm/dd,hh:mm:ss" (the last valid record's, gps.c:2644-2654), or
  * NULL when no valid record was read (no almanac_file, or nothing usable in it). */
 const char *gpsb200_scenario_almanac_date(const gpsb200_scenario_t *s);
+
+/* ---- incremental scenario: the same engine advanced block range by block range -------------------------------
+ * gpsb200_scenario_create == gpsb200_scenario_open + one advance over the whole run. An opened scenario keeps the
+ * reference producer's state between advances (channels, allocation, ephemeris set, receiver time, NAV frame table,
+ * previous ranges), so its memory is bounded by the largest advance and not by the duration; any cut of a run into
+ * advances gives the records and frames of the batch run. On failure *out is still set (read the error, then destroy).
+ *   advance  the next min(nblk, blocks left) blocks into chans_out[nblk][channels] (*got of them); nav_frame is the
+ *            global frame number. GPSB200_ERR_END when no block is left (also after key 'x').
+ *   frame    the [channels][60] NAV words of global frame f, valid for the frames the last advance referenced (and
+ *            until the next advance); NULL otherwise.
+ *   key      one key of the reference's interactive mode (gps-sim.c:363-401, gui.h:25-32), acting on the next block
+ *            advance produces: 'a'/'d' bearing -/+ 127 mdeg (below 0 -> 360000, above 360000 -> 0), 'w'/'s' vertical
+ *            speed +/- 1 m/s, 'e'/'q' speed +/- 0.01 m/s (clamped at 0), 't'/'g' SDR gain (no effect on the samples),
+ *            'x'/'X' end the run after the blocks already produced. GPSB200_ERR_ARG for any other key, for a scenario
+ *            opened without `interactive` (or with a motion file) and before block 1 (the reference reads keys only
+ *            once its producer has started); GPSB200_ERR_END when no block is left. */
+typedef struct gpsb200_steer_state {
+    double speed;            /* target_t.speed (gps-sim.h:36-46): key units of 0.01 m/s */
+    double velocity;         /* m/s = speed / 100 */
+    double bearing_mdeg;     /* millidegrees; starts at the -t bearing x 1000, else 0 */
+    double vertical_speed;   /* m/s */
+    double xyz[3];           /* ECEF [m] of the receiver in the last block produced (before any: the start point) */
+    int32_t next_block;      /* first block of the next advance */
+    int32_t end_block;       /* blocks of the run (fewer after 'x') */
+} gpsb200_steer_state_t;     /* 64 bytes */
+int gpsb200_scenario_open(const gpsb200_scenario_config_t *cfg, gpsb200_scenario_t **out);
+int gpsb200_scenario_advance(gpsb200_scenario_t *s, int nblk, gpsb200_chan_t *chans_out, int32_t *got);
+const uint32_t *gpsb200_scenario_frame(const gpsb200_scenario_t *s, int frame);
+int gpsb200_scenario_key(gpsb200_scenario_t *s, int key);
+int gpsb200_scenario_steer_state(const gpsb200_scenario_t *s, gpsb200_steer_state_t *out);
 
 /* One SEM almanac record as the scenario engine reads it (the reference's almanac_prn_t, almanac.h:21-38). */
 typedef struct gpsb200_almanac_record {

@@ -56,6 +56,23 @@ class ScenarioConfig(C.Structure):
                 ("start_sec", C.c_double), ("target_valid", C.c_int32), ("reserved", C.c_int32),
                 ("target_distance_m", C.c_double), ("target_bearing_deg", C.c_double), ("target_height_m", C.c_double),
                 ("almanac_file", C.c_char_p)]
+    # the header's `interactive` field (int32 at offset 92); _fields_ keeps its former name `reserved`, so that code
+    # written against the earlier mirror still runs
+    interactive = property(lambda self: self.reserved, lambda self, v: setattr(self, "reserved", v))
+
+
+class SteerState(C.Structure):
+    """gpsb200_steer_state_t."""
+    _fields_ = [("speed", C.c_double), ("velocity", C.c_double), ("bearing_mdeg", C.c_double),
+                ("vertical_speed", C.c_double), ("xyz", C.c_double * 3), ("next_block", C.c_int32),
+                ("end_block", C.c_int32)]
+
+
+assert C.sizeof(SteerState) == 64
+
+ERR_END = -6
+# the keys of the reference's interactive mode (gui.h:25-32, gps-sim.c:336-401)
+KEYS = "adwseqtgxX"
 
 
 ALMANAC_RECORD_DTYPE = np.dtype([("svid", "<i4"), ("svn", "<i4"), ("ura", "<i4"), ("health", "<i4"), ("config_code", "<i4"),
@@ -92,6 +109,8 @@ EXPORTS = ["gpsb200_create", "gpsb200_destroy", "gpsb200_last_error", "gpsb200_v
            "gpsb200_scenario_create", "gpsb200_scenario_destroy", "gpsb200_scenario_error",
            "gpsb200_scenario_blocks", "gpsb200_scenario_channels", "gpsb200_scenario_nav_frames",
            "gpsb200_scenario_chans", "gpsb200_scenario_nav", "gpsb200_scenario_almanac_date", "gpsb200_almanac_read",
+           "gpsb200_scenario_open", "gpsb200_scenario_advance", "gpsb200_scenario_frame", "gpsb200_scenario_key",
+           "gpsb200_scenario_steer_state",
            "fifo_create", "fifo_destroy", "fifo_wait_next", "fifo_wait_full", "fifo_halt", "fifo_acquire",
            "fifo_enqueue", "fifo_dequeue", "fifo_release", "fifo_set_compat_drop",
            "gpsb200_iqfile_start", "gpsb200_iqfile_stop", "gpsb200_fifo_push", "gpsb200_fifo_push_flush"]
@@ -130,6 +149,12 @@ def lib():
         L.gpsb200_scenario_almanac_date.argtypes = [C.c_void_p]
         L.gpsb200_scenario_almanac_date.restype = C.c_char_p
         L.gpsb200_almanac_read.argtypes = [C.c_char_p, C.c_void_p, C.POINTER(C.c_int32)]
+        L.gpsb200_scenario_open.argtypes = [C.POINTER(ScenarioConfig), C.POINTER(C.c_void_p)]
+        L.gpsb200_scenario_advance.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.POINTER(C.c_int32)]
+        L.gpsb200_scenario_frame.argtypes = [C.c_void_p, C.c_int]
+        L.gpsb200_scenario_frame.restype = C.c_void_p
+        L.gpsb200_scenario_key.argtypes = [C.c_void_p, C.c_int]
+        L.gpsb200_scenario_steer_state.argtypes = [C.c_void_p, C.POINTER(SteerState)]
         L.gpsb200_carrier_probe_fixup.argtypes = [C.c_double, C.c_double, C.c_double, C.c_int64, C.POINTER(C.c_double)]
         L.gpsb200_carrier_chain_device.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p]
         L.gpsb200_carrier_chain.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int]
@@ -260,12 +285,8 @@ def almanac_read(path):
     return bool(valid.value), rec
 
 
-def scenario(nav_file, lat, lon, height, seconds, max_chan=12, motion_file=None, start=None,
-             ionosphere=True, pluto_gain=False, rinex3=False, target=None, almanac_file=None, info=None):
-    """Run the host scenario engine. -> (chans[nblk, max_chan] CHAN_DTYPE, nav[nframes, max_chan, 60] uint32).
-    start: (y, m, d, hh, mm, sec) or None for the first ephemeris epoch. almanac_file: SEM almanac to transmit in
-    subframes 4 and 5 (None: no almanac, the reference's --disable-almanac). info: optional dict that receives
-    "almanac_date" ("yyyy/mm/dd,hh:mm:ss", or None when no valid almanac record was read)."""
+def _scenario_config(nav_file, lat, lon, height, seconds, max_chan=12, motion_file=None, start=None,
+                     ionosphere=True, pluto_gain=False, rinex3=False, target=None, almanac_file=None, interactive=False):
     cfg = ScenarioConfig()
     cfg.nav_file = os.fsencode(nav_file)
     cfg.motion_file = os.fsencode(motion_file) if motion_file else None
@@ -276,12 +297,33 @@ def scenario(nav_file, lat, lon, height, seconds, max_chan=12, motion_file=None,
     cfg.pluto_gain = 1 if pluto_gain else 0
     cfg.rinex3 = 1 if rinex3 else 0
     cfg.almanac_file = os.fsencode(almanac_file) if almanac_file else None
+    cfg.interactive = 1 if interactive else 0
     if target is not None:          # -t distance,bearing,height
         cfg.target_valid = 1
         cfg.target_distance_m, cfg.target_bearing_deg, cfg.target_height_m = [float(v) for v in target]
     if start:
         (cfg.start_year, cfg.start_month, cfg.start_day, cfg.start_hour, cfg.start_min) = [int(v) for v in start[:5]]
         cfg.start_sec = float(start[5])
+    return cfg
+
+
+def scenario(nav_file, lat, lon, height, seconds, max_chan=12, motion_file=None, start=None,
+             ionosphere=True, pluto_gain=False, rinex3=False, target=None, almanac_file=None, info=None, steer=None):
+    """Run the host scenario engine. -> (chans[nblk, max_chan] CHAN_DTYPE, nav[nframes, max_chan, 60] uint32).
+    start: (y, m, d, hh, mm, sec) or None for the first ephemeris epoch. almanac_file: SEM almanac to transmit in
+    subframes 4 and 5 (None: no almanac, the reference's --disable-almanac). info: optional dict that receives
+    "almanac_date" ("yyyy/mm/dd,hh:mm:ss", or None when no valid almanac record was read).
+    steer: interactive run, [(block, keys, repeat), ...]: the string `keys`, `repeat` times, before `block` (>= 1);
+    built on the incremental engine (LiveScenario). [] is an interactive run without keys."""
+    kw = dict(max_chan=max_chan, motion_file=motion_file, start=start, ionosphere=ionosphere, pluto_gain=pluto_gain,
+              rinex3=rinex3, target=target, almanac_file=almanac_file)
+    if steer is not None:
+        with LiveScenario(nav_file, lat, lon, height, seconds, interactive=True, **kw) as s:
+            chans, nav = s.run(steer)
+            if info is not None:
+                info["almanac_date"] = s.almanac_date
+            return chans, nav
+    cfg = _scenario_config(nav_file, lat, lon, height, seconds, **kw)
     h = C.c_void_p()
     L = lib()
     rc = L.gpsb200_scenario_create(C.byref(cfg), C.byref(h))
@@ -299,6 +341,102 @@ def scenario(nav_file, lat, lon, height, seconds, max_chan=12, motion_file=None,
     finally:
         if h:
             L.gpsb200_scenario_destroy(h)
+
+
+def parse_steer(text):
+    """The `B,KEYS[,REPEAT]` schedule format (one event per line, as gpsb200-sim --steer reads it) -> [(B, KEYS, REPEAT)]."""
+    out = []
+    for line in text.splitlines():
+        line = line.strip()
+        if not line or line.startswith("#"):
+            continue
+        f = line.split(",")
+        out.append((int(f[0]), f[1], int(f[2]) if len(f) > 2 else 1))
+    return out
+
+
+class LiveScenario:
+    """An opened scenario (gpsb200_scenario_open), advanced block range by block range and steered in between:
+    open -> advance(n) / key(k) / frame(f) / state() -> close."""
+
+    def __init__(self, nav_file, lat, lon, height, seconds, **kw):
+        self._h = C.c_void_p()
+        cfg = _scenario_config(nav_file, lat, lon, height, seconds, **kw)
+        L = lib()
+        rc = L.gpsb200_scenario_open(C.byref(cfg), C.byref(self._h))
+        if rc:
+            msg = L.gpsb200_scenario_error(self._h).decode() if self._h else "gpsb200_scenario_open"
+            self.close()
+            raise GpsB200Error(rc, msg)
+        self.blocks = L.gpsb200_scenario_blocks(self._h)
+        self.channels = L.gpsb200_scenario_channels(self._h)
+        d = L.gpsb200_scenario_almanac_date(self._h)
+        self.almanac_date = d.decode() if d else None
+
+    def close(self):
+        if self._h:
+            lib().gpsb200_scenario_destroy(self._h)
+            self._h = C.c_void_p()
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *a):
+        self.close()
+
+    def _check(self, rc):
+        if rc:
+            raise GpsB200Error(rc, lib().gpsb200_scenario_error(self._h).decode())
+
+    def advance(self, nblk):
+        """The next <= nblk blocks -> chans[got, channels] CHAN_DTYPE (nav_frame: global frame number)."""
+        out = np.zeros((nblk, self.channels), CHAN_DTYPE)
+        got = C.c_int32(0)
+        self._check(lib().gpsb200_scenario_advance(self._h, int(nblk), out.ctypes.data, C.byref(got)))
+        return out[:got.value]
+
+    def frame(self, f):
+        """NAV words uint32[channels, 60] of global frame f (one the last advance referenced)."""
+        p = lib().gpsb200_scenario_frame(self._h, int(f))
+        if not p:
+            raise GpsB200Error(-1, "NAV frame %d is not held (only those of the last advance are)" % f)
+        return np.frombuffer(C.string_at(p, self.channels * 60 * 4), dtype=np.uint32).reshape(self.channels, 60).copy()
+
+    def key(self, k):
+        """One key ('a', 'd', 'w', 's', 'e', 'q', 't', 'g', 'x'); acts on the next block advance produces."""
+        self._check(lib().gpsb200_scenario_key(self._h, ord(k) if isinstance(k, str) else int(k)))
+
+    def state(self):
+        st = SteerState()
+        self._check(lib().gpsb200_scenario_steer_state(self._h, C.byref(st)))
+        return st
+
+    def run(self, steer, chunk=None):
+        """Advance to the end of the run, pressing the keys of `steer` [(block, keys, repeat)] before their blocks.
+        chunk: largest advance (None: from key block to key block). -> (chans[nblk, C], nav[nframes, C, 60])."""
+        events = {}
+        for b, keys, rep in steer:
+            events[int(b)] = events.get(int(b), "") + keys * int(rep)
+        parts, frames = [], {}
+        b = 0
+        while True:
+            if b in events:
+                for k in events.pop(b):
+                    self.key(k)
+            st = self.state()
+            if st.next_block >= st.end_block:
+                break
+            nxt = min([e for e in events if e > b] + [st.end_block])
+            n = nxt - b if chunk is None else min(chunk, nxt - b)
+            ch = self.advance(n)
+            for f in np.unique(ch["nav_frame"]):
+                if f not in frames:
+                    frames[int(f)] = self.frame(int(f))
+            parts.append(ch)
+            b += ch.shape[0]
+        chans = np.concatenate(parts) if parts else np.zeros((0, self.channels), CHAN_DTYPE)
+        nav = np.stack([frames[f] for f in sorted(frames)]) if frames else np.zeros((0, self.channels, 60), np.uint32)
+        return chans, nav
 
 
 class Context:

@@ -8,14 +8,18 @@
 //   subframes, parity, 30 s NAV frames (gps.c:617-884, 1008-1072, 2066-2140)
 //   SEM almanac reader + almanac pages (behaviour of almanac.c:73-184, gps.c:772-883, 2637-2657)
 //   visibility + channel allocation (gps.c:2142-2235), 10 Hz loop (gps.c:2703-2765, 2870-2932)
+//   interactive steering: the key switch (gps-sim.c:363-393) and the per-block move (gps.c:2714-2729)
+// The engine is incremental: gpsb200_scenario_open does what the reference's producer does before its loop, and
+// gpsb200_scenario_advance runs the loop for the next range of blocks, keeping the producer's state in between (memory
+// bounded by the range, not the run); keys act between advances. gpsb200_scenario_create is open + one advance.
 // These are rows f1/f2/f4 of SURVEY.md section 8 ("next" after the sample loop). The
 // doubles feed the CUDA kernels bit for bit, so every expression keeps the reference's
 // evaluation order (no FMA contraction: -ffp-contract=off) and the same libm calls;
 // tests/test_scenario.py compares every field with the reference's own dumps.
 //
 // Scope notes: the almanac comes from a SEM file the caller names (the reference reads ./almanac.sem implicitly;
-// without a file the pages are the reference's with --disable-almanac, as in all BASELINE configs); downloads,
-// interactive motion and the HackRF/Pluto specifics (except the Pluto gain doubling) are out of scope.
+// without a file the pages are the reference's with --disable-almanac, as in all BASELINE configs); downloads, `-s now`
+// and the HackRF/Pluto specifics (except the Pluto gain doubling) are out of scope.
 #include <algorithm>
 #include <cmath>
 #include <cstdio>
@@ -770,14 +774,43 @@ int read_rinex3(const char *path, Eph eph[kEphSets][kMaxSat], IonoUtc &io) {
 }  // namespace
 
 // =====================================================================================================
+// The reference's producer keeps its state on its stack between 0.1 s blocks (gps.c:2282-2936). An opened scenario
+// keeps the same state between advances: the ephemeris table and the current set, the channels and the allocation,
+// the receiver time, the NAV frame table, the previous block's range of every slot and, in interactive mode, the
+// receiver position and the steering state. Memory is bounded by the largest advance, not by the run.
 struct gpsb200_scenario {
     gpsb200_scenario_config_t cfg{};
     int nchan = 12, nblocks = 0;
-    std::vector<gpsb200_chan_t> chans;              // [nblocks][nchan]
-    std::vector<uint32_t> nav;                      // [nframes][nchan][60]
-    int nframes = 0;
+    std::vector<gpsb200_chan_t> chans;              // gpsb200_scenario_create: [nblocks][nchan]
+    std::vector<uint32_t> nav;                      // frames [nav_base, nframes), [frame][nchan][60]
+    int nframes = 0, nav_base = 0;
     std::string err;
     std::string almanac_date;                       // empty: no valid almanac record
+
+    bool opened = false;
+    std::vector<Eph> eph;                           // [kEphSets][kMaxSat]
+    int ieph = 0;
+    IonoUtc io;
+    Almanac alm;
+    double ant_pat[37];
+    std::vector<Channel> chan;
+    std::vector<char> fresh;                        // slot (re)allocated since the last epoch snapshot
+    int allocated[kMaxSat];
+    GpsTime grx;                                    // receiver time of the next block
+    int next_block = 0, end_block = 0;              // end_block < nblocks after 'x'
+    std::vector<double> motion;                     // -m: xyz[iumd] of every row read (bounded by the file)
+    double xyz0[3] = {0, 0, 0};                     // xyz[0]: the location, or the -t start point
+    std::vector<uint32_t> cur, last;                // NAV words of every slot now / of the newest frame
+    bool words_may_have_changed = true;
+    std::vector<Range> prev_rho;                    // [nchan] range of the previous block (what chan[i].rho0 holds)
+    // interactive mode: the reference's target_t (gps-sim.h:36-46) and xyz[iumd - 1] (gps.c:2714-2729)
+    bool interactive = false;
+    double bearing = 0, speed = 0, velocity = 0, vertical_speed = 0;
+    double pos[3] = {0, 0, 0};
+    double tmat[3][3];                              // ltcmat of the -l location, never updated (gps.c:2341)
+
+    Eph (*table())[kMaxSat] { return reinterpret_cast<Eph (*)[kMaxSat]>(eph.data()); }
+    const double *pos_at(int iumd) const { return motion.empty() ? xyz0 : &motion[3 * (size_t) iumd]; }
 };
 
 namespace {
@@ -787,57 +820,107 @@ int fail(gpsb200_scenario *s, const std::string &m) {
     return GPSB200_ERR_ARG;
 }
 
-int build(gpsb200_scenario *S) {
+// visibility + channel allocation (gps.c:2142-2235); always evaluated at the INITIAL position xyz[0] (gps.c:2909)
+void allocate(gpsb200_scenario *S, const Eph *set, const GpsTime &grx) {
+    const int C = S->nchan;
+    const double *p0 = S->pos_at(0);
+    double llh0[3], tm[3][3];
+    ecef_to_llh(p0, llh0);
+    local_frame(llh0, tm);
+    for (int sv = 0; sv < kMaxSat; sv++) {
+        bool visible = false;
+        double az = 0, el = 0;
+        if (set[sv].valid) {
+            double pos[3], vel[3], clk[2], los[3];
+            sat_state(set[sv], grx, pos, vel, clk);
+            for (int k = 0; k < 3; k++) los[k] = pos[k] - p0[k];
+            az_el(los, tm, az, el);
+            visible = el * kR2D > 0.0;
+        }
+        if (visible) {
+            if (S->allocated[sv] == -1) {
+                int i = 0;
+                for (; i < C; i++)
+                    if (S->chan[i].prn == 0) {
+                        Channel &ch = S->chan[i];
+                        ch.prn = sv + 1;
+                        S->fresh[i] = 1;
+                        // the reference never initialises channel_t.ipage (gps.c:2086 reads it);
+                        // its -Og build sees zeroed stack there, which is what is reproduced here
+                        build_subframes(set[sv], S->io, S->alm, ch.sbf);
+                        build_nav_frame(grx, ch, true);
+                        const Range r = pseudo_range(set[sv], S->io, grx, p0);
+                        ch.rho0 = r;
+                        const double ref[3] = {0.0, 0.0, 0.0};
+                        const Range rr = pseudo_range(set[sv], S->io, grx, ref);
+                        const double phase_ini = (2.0 * rr.range - r.range) / kLambda;
+                        ch.carr_phase = phase_ini - floor(phase_ini);
+                        break;
+                    }
+                if (i < C) S->allocated[sv] = i;
+            }
+        } else if (S->allocated[sv] >= 0) {
+            S->chan[S->allocated[sv]].prn = 0;
+            S->allocated[sv] = -1;
+        }
+    }
+}
+
+// Everything the reference's producer does before its 10 Hz loop (gps.c:2282-2692): files, receiver position, start
+// time, ephemeris set, almanac, first allocation.
+int open_scenario(gpsb200_scenario *S) {
     const gpsb200_scenario_config_t &cfg = S->cfg;
     const int C = S->nchan;
-    static thread_local Eph eph[kEphSets][kMaxSat];
-    for (auto &set : eph)
-        for (auto &e : set) e = Eph();
-    IonoUtc io;
+    S->eph.assign((size_t) kEphSets * kMaxSat, Eph());
+    Eph (*eph)[kMaxSat] = S->table();
+    IonoUtc &io = S->io;
     io.enable = cfg.ionosphere_enable != 0;
     const int neph = cfg.rinex3 ? read_rinex3(cfg.nav_file, eph, io) : read_rinex2(cfg.nav_file, eph, io);
     if (neph <= 0) return fail(S, "cannot read the RINEX navigation file (wrong version flag, or no ephemeris in it)");
-    Almanac alm;                                    // empty unless a SEM file is named: the reference's almanac_init()
+    Almanac &alm = S->alm;                          // empty unless a SEM file is named: the reference's almanac_init()
     if (cfg.almanac_file && !read_sem(cfg.almanac_file, alm))
         return fail(S, std::string("cannot open almanac file ") + cfg.almanac_file);
 
     // receiver positions per 0.1 s (gps.c:2331-2363, 2489-2500)
     int numd = cfg.duration_ds;
     double llh[3] = {cfg.lat_deg / kR2D, cfg.lon_deg / kR2D, cfg.height_m};
-    std::vector<double> xyz;
+    local_frame(llh, S->tmat);
     if (cfg.motion_file && cfg.motion_file[0]) {
+        // a motion file switches interactive mode off (gps-sim.c:297-301)
         FILE *fp = fopen(cfg.motion_file, "rt");
         if (!fp) return fail(S, "cannot open motion file");
         char str[128];
         while (fgets(str, 100, fp)) {
             double t, x, y, z;
             if (sscanf(str, "%lf,%lf,%lf,%lf", &t, &x, &y, &z) == EOF) break;
-            xyz.push_back(x);
-            xyz.push_back(y);
-            xyz.push_back(z);
+            S->motion.push_back(x);
+            S->motion.push_back(y);
+            S->motion.push_back(z);
         }
         fclose(fp);
-        const int got = (int) (xyz.size() / 3);
+        const int got = (int) (S->motion.size() / 3);
         if (got <= 0) return fail(S, "empty motion file");
         numd = got > cfg.duration_ds ? cfg.duration_ds : got;
     } else {
-        xyz.resize(3);
-        llh_to_ecef(llh, xyz.data());
+        S->interactive = cfg.interactive != 0;
+        double *xyz = S->xyz0;
+        llh_to_ecef(llh, xyz);
+        // the CLI stores the bearing in millidegrees (gps-sim.c:148) and the producer divides it back: same round trip
+        // here; interactive steering starts from that bearing
+        if (cfg.target_valid) S->bearing = cfg.target_bearing_deg * 1000;
         if (cfg.target_valid) {
-            // -t distance,bearing,height: start at a point given relative to the location (gps.c:2348-2357). The CLI
-            // stores the bearing in millidegrees (gps-sim.c:148) and the producer divides it back: same round trip here.
-            double t[3][3], neu[3];
-            local_frame(llh, t);
-            const double bearing_milli = cfg.target_bearing_deg * 1000;
-            neu[0] = cfg.target_distance_m * cos((bearing_milli / 1000) / kR2D);
-            neu[1] = cfg.target_distance_m * sin((bearing_milli / 1000) / kR2D);
+            // -t distance,bearing,height: start at a point given relative to the location (gps.c:2348-2357)
+            double neu[3];
+            const double(*t)[3] = S->tmat;
+            neu[0] = cfg.target_distance_m * cos((S->bearing / 1000) / kR2D);
+            neu[1] = cfg.target_distance_m * sin((S->bearing / 1000) / kR2D);
             neu[2] = cfg.target_height_m;
             xyz[0] += t[0][0] * neu[0] + t[1][0] * neu[1] + t[2][0] * neu[2];
             xyz[1] += t[0][1] * neu[0] + t[1][1] * neu[1] + t[2][1] * neu[2];
             xyz[2] += t[0][2] * neu[0] + t[1][2] * neu[1] + t[2][2] * neu[2];
         }
+        memcpy(S->pos, xyz, sizeof S->pos);
     }
-    auto pos_at = [&](int i) -> const double * { return xyz.size() > 3 ? &xyz[3 * (size_t) i] : xyz.data(); };
     if (numd < 2) return fail(S, "duration too short");
 
     // scenario start (gps.c:2502-2577)
@@ -897,67 +980,42 @@ int build(gpsb200_scenario *S) {
         S->almanac_date = buf;
     }
 
-    std::vector<Channel> chan(C);
-    std::vector<char> fresh(C, 0);                  // slot (re)allocated since the last epoch snapshot
-    int allocated[kMaxSat];
-    for (int sv = 0; sv < kMaxSat; sv++) allocated[sv] = -1;
-    double ant_pat[37];
-    for (int i = 0; i < 37; i++) ant_pat[i] = pow(10.0, -kAntPatDb[i] / 20.0);
+    S->chan.assign(C, Channel());
+    S->fresh.assign(C, 0);
+    for (int sv = 0; sv < kMaxSat; sv++) S->allocated[sv] = -1;
+    for (int i = 0; i < 37; i++) S->ant_pat[i] = pow(10.0, -kAntPatDb[i] / 20.0);
+    S->ieph = ieph;
+    S->grx = gps_add(g0, 0.0);
+    allocate(S, eph[ieph], S->grx);
+    S->grx = gps_add(S->grx, 0.1);
+    S->nblocks = S->end_block = numd - 1;
+    S->next_block = 0;
+    S->cur.assign((size_t) C * GPSB200_NAV_WORDS, 0);
+    S->last.clear();
+    S->words_may_have_changed = true;
+    S->prev_rho.assign(C, Range());
+    S->nav.clear();
+    S->nframes = S->nav_base = 0;
+    S->opened = true;
+    return GPSB200_OK;
+}
 
-    // visibility + channel allocation (gps.c:2142-2235); always evaluated at the INITIAL position
-    auto allocate = [&](const Eph *set, const GpsTime &grx) {
-        const double *p0 = pos_at(0);
-        double llh0[3], tm[3][3];
-        ecef_to_llh(p0, llh0);
-        local_frame(llh0, tm);
-        for (int sv = 0; sv < kMaxSat; sv++) {
-            bool visible = false;
-            double az = 0, el = 0;
-            if (set[sv].valid) {
-                double pos[3], vel[3], clk[2], los[3];
-                sat_state(set[sv], grx, pos, vel, clk);
-                for (int k = 0; k < 3; k++) los[k] = pos[k] - p0[k];
-                az_el(los, tm, az, el);
-                visible = el * kR2D > 0.0;
-            }
-            if (visible) {
-                if (allocated[sv] == -1) {
-                    int i = 0;
-                    for (; i < C; i++)
-                        if (chan[i].prn == 0) {
-                            Channel &ch = chan[i];
-                            ch.prn = sv + 1;
-                            fresh[i] = 1;
-                            // the reference never initialises channel_t.ipage (gps.c:2086 reads it);
-                            // its -Og build sees zeroed stack there, which is what is reproduced here
-                            build_subframes(set[sv], io, alm, ch.sbf);
-                            build_nav_frame(grx, ch, true);
-                            const Range r = pseudo_range(set[sv], io, grx, p0);
-                            ch.rho0 = r;
-                            const double ref[3] = {0.0, 0.0, 0.0};
-                            const Range rr = pseudo_range(set[sv], io, grx, ref);
-                            const double phase_ini = (2.0 * rr.range - r.range) / kLambda;
-                            ch.carr_phase = phase_ini - floor(phase_ini);
-                            break;
-                        }
-                    if (i < C) allocated[sv] = i;
-                }
-            } else if (allocated[sv] >= 0) {
-                chan[allocated[sv]].prn = 0;
-                allocated[sv] = -1;
-            }
-        }
-    };
+// The next nb blocks of the reference's loop (gps.c:2703-2936) into out[nb][nchan]. Per 0.1 s block the loop does two
+// things: the per-channel range / code-phase / gain update, which depends only on this block's and the previous
+// block's range, and, every 30 s, the NAV frame roll / ephemeris roll / reallocation. Here: (A) one cheap sequential
+// pass moves the receiver, runs the 30 s events and records, per EPOCH (the blocks between two events), which
+// satellite sits in which slot, with which ephemeris set and NAV frame; (B) the ranges and (C) the block-start states
+// of the range are then computed block-parallel. Every number comes out of the same function with the same arguments
+// as in the sequential order, so the result is bit-identical for any cut of the run into advances
+// (tests/test_scenario.py, tests/test_interactive.py).
+void advance_blocks(gpsb200_scenario *S, int nb, gpsb200_chan_t *out) {
+    const gpsb200_scenario_config_t &cfg = S->cfg;
+    const int C = S->nchan, b0 = S->next_block;
+    Eph (*eph)[kMaxSat] = S->table();
+    std::vector<Channel> &chan = S->chan;
 
-    // The reference's loop (gps.c:2731-2930) does two things per 0.1 s block: the per-channel range /
-    // code-phase / gain update, which depends only on this block's and the previous block's range, and,
-    // every 30 s, the NAV frame roll / ephemeris roll / reallocation. Here: (A) one cheap sequential pass
-    // runs the 30 s events and records, per EPOCH (the blocks between two events), which satellite sits in
-    // which slot, with which ephemeris set and NAV frame; (B) all ranges and (C) all block-start states are
-    // then computed block-parallel. Every number comes out of the same function with the same arguments
-    // as in the sequential order, so the result is bit-identical (tests/test_scenario.py).
     struct Epoch {
-        int b_first = 0, ieph = 0;
+        int k_first = 0, ieph = 0;
         std::vector<int> prn;
         std::vector<char> fresh;
         std::vector<GpsTime> frame_g0;
@@ -965,12 +1023,12 @@ int build(gpsb200_scenario *S) {
         std::vector<double> carr_phase;
     };
     std::vector<Epoch> epochs;
-    auto snapshot = [&](int b_first, int ieph_now) {
+    auto snapshot = [&](int k_first) {
         Epoch e;
-        e.b_first = b_first;
-        e.ieph = ieph_now;
+        e.k_first = k_first;
+        e.ieph = S->ieph;
         e.prn.resize(C);
-        e.fresh = fresh;
+        e.fresh = S->fresh;
         e.frame_g0.resize(C);
         e.rho_alloc.resize(C);
         e.carr_phase.resize(C);
@@ -980,105 +1038,120 @@ int build(gpsb200_scenario *S) {
             e.rho_alloc[i] = chan[i].rho0;           // only read where fresh[i]
             e.carr_phase[i] = chan[i].carr_phase;
         }
-        std::fill(fresh.begin(), fresh.end(), 0);
+        std::fill(S->fresh.begin(), S->fresh.end(), 0);
         epochs.push_back(std::move(e));
     };
 
-    GpsTime grx = gps_add(g0, 0.0);
-    allocate(eph[ieph], grx);
-    grx = gps_add(grx, 0.1);
-
-    S->nblocks = numd - 1;
-    const int NB = S->nblocks;
-    S->chans.assign((size_t) NB * C, gpsb200_chan_t{});
-    S->nav.clear();
-    S->nframes = 0;
-    std::vector<GpsTime> grx_of(NB);
-    std::vector<int> epoch_of(NB), frame_of(NB);
-    std::vector<uint32_t> cur((size_t) C * GPSB200_NAV_WORDS, 0), last;
-    // ---- (A) sequential: times, 30 s events, NAV frame table ------------------------------------------------
-    snapshot(0, ieph);
-    bool words_may_have_changed = true;
-    for (int iumd = 1; iumd < numd; iumd++) {
-        const int b = iumd - 1;
-        grx_of[b] = grx;
-        epoch_of[b] = (int) epochs.size() - 1;
-        // NAV frame table: a new frame whenever any channel's words changed (every 30 s / reallocation)
-        if (words_may_have_changed) {
-            for (int i = 0; i < C; i++)
-                for (int k = 0; k < GPSB200_NAV_WORDS; k++)
-                    cur[(size_t) i * GPSB200_NAV_WORDS + k] = chan[i].prn > 0 ? chan[i].dwrd[k] : 0u;
-            if (cur != last) {
-                S->nav.insert(S->nav.end(), cur.begin(), cur.end());
-                S->nframes++;
-                last = cur;
-            }
-            words_may_have_changed = false;
+    // frames the previous advance referenced are dropped, except the newest: the next block may still use it
+    if (S->nframes > S->nav_base + 1) {
+        S->nav.erase(S->nav.begin(), S->nav.end() - (size_t) C * GPSB200_NAV_WORDS);
+        S->nav_base = S->nframes - 1;
+    }
+    std::vector<GpsTime> grx_of(nb);
+    std::vector<int> epoch_of(nb), frame_of(nb);
+    std::vector<double> steered(S->interactive ? 3 * (size_t) nb : 0);
+    // ---- (A) sequential: receiver motion, times, 30 s events, NAV frame table -----------------------------------
+    snapshot(0);
+    for (int k = 0; k < nb; k++) {
+        if (S->interactive) {
+            // xyz[iumd] = xyz[iumd - 1] + T^T neu, T of the -l location (gps.c:2714-2729)
+            double *xyz = S->pos, neu[3];
+            const double(*t)[3] = S->tmat;
+            const double dir = (S->bearing / 1000) / kR2D;
+            neu[0] = (S->velocity * cos(dir)) * 0.1;
+            neu[1] = (S->velocity * sin(dir)) * 0.1;
+            neu[2] = S->vertical_speed * 0.1;
+            xyz[0] += t[0][0] * neu[0] + t[1][0] * neu[1] + t[2][0] * neu[2];
+            xyz[1] += t[0][1] * neu[0] + t[1][1] * neu[1] + t[2][1] * neu[2];
+            xyz[2] += t[0][2] * neu[0] + t[1][2] * neu[1] + t[2][2] * neu[2];
+            memcpy(&steered[3 * (size_t) k], xyz, sizeof S->pos);
         }
-        frame_of[b] = S->nframes - 1;
+        const GpsTime grx = S->grx;
+        grx_of[k] = grx;
+        epoch_of[k] = (int) epochs.size() - 1;
+        // NAV frame table: a new frame whenever any channel's words changed (every 30 s / reallocation)
+        if (S->words_may_have_changed) {
+            for (int i = 0; i < C; i++)
+                for (int j = 0; j < GPSB200_NAV_WORDS; j++)
+                    S->cur[(size_t) i * GPSB200_NAV_WORDS + j] = chan[i].prn > 0 ? chan[i].dwrd[j] : 0u;
+            if (S->cur != S->last) {
+                S->nav.insert(S->nav.end(), S->cur.begin(), S->cur.end());
+                S->nframes++;
+                S->last = S->cur;
+            }
+            S->words_may_have_changed = false;
+        }
+        frame_of[k] = S->nframes - 1;
         // every 30 s: NAV frame roll, ephemeris set roll, reallocation (gps.c:2870-2930)
         const int igrx = (int) (grx.sec * 10.0 + 0.5);
         if (igrx % 300 == 0) {
             for (int i = 0; i < C; i++)
                 if (chan[i].prn > 0) build_nav_frame(grx, chan[i], false);
+            int &ieph = S->ieph;
             if (ieph + 1 < kEphSets)
                 for (int sv = 0; sv < kMaxSat; sv++)
                     if (eph[ieph + 1][sv].valid) {
                         if (gps_diff(eph[ieph + 1][sv].toc, grx) < kSecHour) {
                             ieph++;
                             for (int i = 0; i < C; i++)
-                                if (chan[i].prn != 0) build_subframes(eph[ieph][chan[i].prn - 1], io, alm, chan[i].sbf);
+                                if (chan[i].prn != 0) build_subframes(eph[ieph][chan[i].prn - 1], S->io, S->alm, chan[i].sbf);
                         }
                         break;
                     }
-            allocate(eph[ieph], grx);
-            if (iumd + 1 < numd) snapshot(b + 1, ieph);
-            words_may_have_changed = true;
+            allocate(S, eph[ieph], grx);
+            if (k + 1 < nb) snapshot(k + 1);        // else the next advance's first snapshot takes these flags
+            S->words_may_have_changed = true;
         }
-        grx = gps_add(grx, 0.1);
+        S->grx = gps_add(grx, 0.1);
     }
+    auto pos_of = [&](int k) -> const double * { return S->interactive ? &steered[3 * (size_t) k] : S->pos_at(b0 + k + 1); };
 
     // ---- (B) + (C) block-parallel ----------------------------------------------------------------------------
-    const Eph(*E)[kMaxSat] = eph;                   // `eph` is thread_local: hand the workers THIS thread's table
-    std::vector<Range> rho((size_t) NB * C);
+    const Eph(*E)[kMaxSat] = eph;
+    const IonoUtc &io = S->io;
+    std::vector<Range> rho((size_t) nb * C);
     int nthr = (int) std::thread::hardware_concurrency();
     if (const char *ev = getenv("GPSB200_SCENARIO_THREADS")) nthr = atoi(ev);
-    nthr = std::max(1, std::min(std::min(nthr, 16), NB / 64 + 1));
+    nthr = std::max(1, std::min(std::min(nthr, 16), nb / 64 + 1));
     auto parallel_blocks = [&](const std::function<void(int, int)> &job) {
         if (nthr == 1) {
-            job(0, NB);
+            job(0, nb);
             return;
         }
         std::vector<std::thread> th;
-        const int per = (NB + nthr - 1) / nthr;
+        const int per = (nb + nthr - 1) / nthr;
         for (int t = 0; t < nthr; t++) {
-            const int lo = t * per, hi = std::min(NB, lo + per);
+            const int lo = t * per, hi = std::min(nb, lo + per);
             if (lo < hi) th.emplace_back(job, lo, hi);
         }
         for (auto &t : th) t.join();
     };
     parallel_blocks([&](int lo, int hi) {            // (B) this block's pseudorange per channel (gps.c:2738)
-        for (int b = lo; b < hi; b++) {
-            const Epoch &ep = epochs[epoch_of[b]];
+        for (int k = lo; k < hi; k++) {
+            const Epoch &ep = epochs[epoch_of[k]];
             for (int i = 0; i < C; i++)
-                if (ep.prn[i] > 0) rho[(size_t) b * C + i] = pseudo_range(E[ep.ieph][ep.prn[i] - 1], io, grx_of[b], pos_at(b + 1));
+                if (ep.prn[i] > 0) rho[(size_t) k * C + i] = pseudo_range(E[ep.ieph][ep.prn[i] - 1], io, grx_of[k], pos_of(k));
         }
     });
+    const Range *prev = S->prev_rho.data();
     parallel_blocks([&](int lo, int hi) {            // (C) block-start state and gain (gps.c:2744-2763)
-        for (int b = lo; b < hi; b++) {
-            const Epoch &ep = epochs[epoch_of[b]];
+        for (int k = lo; k < hi; k++) {
+            const Epoch &ep = epochs[epoch_of[k]];
             for (int i = 0; i < C; i++) {
-                gpsb200_chan_t &o = S->chans[(size_t) b * C + i];
-                o.nav_frame = frame_of[b];
+                gpsb200_chan_t &o = out[(size_t) k * C + i];
+                o = gpsb200_chan_t{};
+                o.nav_frame = frame_of[k];
                 if (ep.prn[i] <= 0) continue;
-                const Range &r1 = rho[(size_t) b * C + i];
+                const Range &r1 = rho[(size_t) k * C + i];
                 // the range the reference still holds in chan[i].rho0: the allocation's for a slot's first
                 // block, else the previous block's (possibly computed with the previous ephemeris set)
-                const Range &r0 = (b == ep.b_first && ep.fresh[i]) ? ep.rho_alloc[i] : rho[(size_t) (b - 1) * C + i];
+                const Range &r0 = (k == ep.k_first && ep.fresh[i]) ? ep.rho_alloc[i]
+                                  : k == 0                        ? prev[i]
+                                                                  : rho[(size_t) (k - 1) * C + i];
                 block_start_pure(r0, ep.frame_g0[i], r1, 0.1, o);
                 const double path_loss = 20200000.0 / r1.d;                     // gps.c:2749
                 const int ibs = (int) ((90.0 - r1.el * kR2D) / 5.0);
-                double gain = (double) (path_loss * ant_pat[ibs]);
+                double gain = (double) (path_loss * S->ant_pat[ibs]);
                 if (cfg.pluto_gain) gain *= 2;                                  // gps.c:2759-2763
                 o.prn = ep.prn[i];
                 o.carr_phase = ep.carr_phase[i];   // meaningful for a slot's first block only
@@ -1086,7 +1159,10 @@ int build(gpsb200_scenario *S) {
             }
         }
     });
-    return GPSB200_OK;
+    const Epoch &tail = epochs[epoch_of[nb - 1]];
+    for (int i = 0; i < C; i++)
+        if (tail.prn[i] > 0) S->prev_rho[i] = rho[(size_t) (nb - 1) * C + i];
+    S->next_block = b0 + nb;
 }
 
 }  // namespace
@@ -1095,18 +1171,101 @@ int build(gpsb200_scenario *S) {
 static_assert(offsetof(gpsb200_scenario_config_t, target_height_m) == 112, "gpsb200_scenario_config_t layout");
 static_assert(offsetof(gpsb200_scenario_config_t, almanac_file) == 120, "gpsb200_scenario_config_t layout");
 static_assert(sizeof(gpsb200_scenario_config_t) == 128, "gpsb200_scenario_config_t layout");
+static_assert(offsetof(gpsb200_scenario_config_t, interactive) == 92, "gpsb200_scenario_config_t layout");
 static_assert(sizeof(gpsb200_almanac_record_t) == 112, "gpsb200_almanac_record_t layout");
+static_assert(sizeof(gpsb200_steer_state_t) == 64, "gpsb200_steer_state_t layout");
 
 extern "C" {
 
-int gpsb200_scenario_create(const gpsb200_scenario_config_t *cfg, gpsb200_scenario_t **out) {
+int gpsb200_scenario_open(const gpsb200_scenario_config_t *cfg, gpsb200_scenario_t **out) {
     if (!cfg || !out || !cfg->nav_file) return GPSB200_ERR_ARG;
     gpsb200_scenario *S = new gpsb200_scenario();
     S->cfg = *cfg;
     S->nchan = cfg->max_chan > 0 ? cfg->max_chan : 12;
     *out = S;
     if (S->nchan > GPSB200_MAX_CHAN) return fail(S, "max_chan > 32");
-    return build(S);
+    return open_scenario(S);
+}
+
+int gpsb200_scenario_create(const gpsb200_scenario_config_t *cfg, gpsb200_scenario_t **out) {
+    const int rc = gpsb200_scenario_open(cfg, out);
+    if (rc != GPSB200_OK) return rc;
+    gpsb200_scenario *S = *out;
+    S->chans.resize((size_t) S->nblocks * S->nchan);
+    advance_blocks(S, S->nblocks, S->chans.data());
+    return GPSB200_OK;
+}
+
+int gpsb200_scenario_advance(gpsb200_scenario_t *s, int nblk, gpsb200_chan_t *chans_out, int32_t *got) {
+    if (got) *got = 0;
+    if (!s || !s->opened || nblk < 1 || !chans_out) return GPSB200_ERR_ARG;
+    const int nb = std::min(nblk, s->end_block - s->next_block);
+    if (nb <= 0) {
+        s->err = "advance past the end of the run";
+        return GPSB200_ERR_END;
+    }
+    advance_blocks(s, nb, chans_out);
+    if (got) *got = nb;
+    return GPSB200_OK;
+}
+
+const uint32_t *gpsb200_scenario_frame(const gpsb200_scenario_t *s, int frame) {
+    if (!s || frame < s->nav_base || frame >= s->nframes) return nullptr;
+    return s->nav.data() + (size_t) (frame - s->nav_base) * s->nchan * GPSB200_NAV_WORDS;
+}
+
+// the reference's key switch (gps-sim.c:336-401, keys gui.h:25-32)
+int gpsb200_scenario_key(gpsb200_scenario_t *s, int key) {
+    if (!s || !s->opened) return GPSB200_ERR_ARG;
+    if (!strchr("adwseqtgxX", key) || key == 0) {
+        s->err = "unknown key";
+        return GPSB200_ERR_ARG;
+    }
+    if (!s->interactive) {
+        s->err = "key on a scenario without interactive mode";
+        return GPSB200_ERR_ARG;
+    }
+    if (s->next_block < 1) {        // the reference reads keys only once its producer runs (gps-sim.c:316-333)
+        s->err = "key before block 1";
+        return GPSB200_ERR_ARG;
+    }
+    if (s->next_block >= s->end_block) {
+        s->err = "key after the end of the run";
+        return GPSB200_ERR_END;
+    }
+    switch (key) {
+        case 'a':
+        case 'd':
+            s->bearing += key == 'a' ? -127.0 : 127.0;
+            if (s->bearing < 0) s->bearing = 360000.0;
+            if (s->bearing > 360000) s->bearing = 0;
+            break;
+        case 'w': s->vertical_speed += 1; break;
+        case 's': s->vertical_speed -= 1; break;
+        case 'e':
+        case 'q':
+            s->speed += key == 'e' ? 1.0 : -1.0;
+            if (s->speed < 0) s->speed = 0;
+            s->velocity = s->speed / 100.0;
+            break;
+        case 'x':
+        case 'X': s->end_block = s->next_block; break;
+        default: break;             // t / g: SDR gain, no effect on the samples
+    }
+    return GPSB200_OK;
+}
+
+int gpsb200_scenario_steer_state(const gpsb200_scenario_t *s, gpsb200_steer_state_t *out) {
+    if (!s || !s->opened || !out) return GPSB200_ERR_ARG;
+    *out = gpsb200_steer_state_t{};
+    out->speed = s->speed;
+    out->velocity = s->velocity;
+    out->bearing_mdeg = s->bearing;
+    out->vertical_speed = s->vertical_speed;
+    memcpy(out->xyz, s->interactive ? s->pos : s->pos_at(s->next_block), sizeof out->xyz);
+    out->next_block = s->next_block;
+    out->end_block = s->end_block;
+    return GPSB200_OK;
 }
 
 void gpsb200_scenario_destroy(gpsb200_scenario_t *s) { delete s; }

@@ -13,8 +13,16 @@
 // + gpsb200_link_apply), all workers probe speculatively in parallel, and the exact states travel worker to worker
 // (gpsb200_slice_prepare / _probe / _finish). Each worker downloads into a page-locked slice buffer; the main thread
 // feeds the slices to the FIFO in stream order as they complete.
+// -i / --steer FILE: the reference's interactive mode (gps-sim.c:363-393, gps.c:2714-2729) on one GPU. The scenario is
+// opened, not built up front, and advanced chunk by chunk; keys (from stdin, paced to real time, or replayed from a
+// schedule) are applied between advances. Each chunk is synthesized with gpsb200_synth_blocks_scatter, the carrier
+// chain continued across calls, the NAV frames kept in a ring of context slots (global frame f in slot f mod R).
 #include <algorithm>
+#include <atomic>
 #include <chrono>
+#include <csignal>
+#include <deque>
+#include <map>
 #include <condition_variable>
 #include <cstdio>
 #include <cstdlib>
@@ -24,6 +32,9 @@
 #include <thread>
 #include <vector>
 
+#include <termios.h>
+#include <unistd.h>
+
 #include <cuda_runtime_api.h>
 
 #include "../include/gpsb200.h"
@@ -32,7 +43,10 @@ static void usage() {
     fprintf(stderr,
             "gpsb200-sim -e NAV[.gz] [-3] -l lat,lon,h [-t dist,bearing,height] [-d SEC] [-m motion.csv] [-s y/m/d,h:m:s]\n"
             "            [--iq16] [-I] [--pluto-gain] [--chan N] [--gpus N] [-o iqdata.bin] [--compat-drop]\n"
-            "            [--almanac FILE.sem | --disable-almanac]\n");
+            "            [--almanac FILE.sem | --disable-almanac] [-i | --steer FILE] [--steer-log FILE]\n"
+            "  -i              interactive: keys from stdin (a/d heading, w/s climb, e/q speed, x end), paced to real time\n"
+            "  --steer FILE    replay a schedule, one line per event \"B,KEYS[,REPEAT]\": KEYS, REPEAT times, before block B\n"
+            "  --steer-log F   write the schedule that was applied (replays byte-identically with --steer)\n");
     exit(2);
 }
 
@@ -42,6 +56,185 @@ static double now_s() {
 }
 
 namespace {
+std::atomic<bool> g_stop{false};
+struct termios g_tty;
+bool g_tty_raw = false;
+
+void restore_tty() {
+    if (g_tty_raw) tcsetattr(0, TCSANOW, &g_tty);
+    g_tty_raw = false;
+}
+void on_sigint(int) { g_stop = true; }          // the block in progress is finished, then the file is closed
+
+bool read_schedule(const char *path, std::map<int, std::string> &keys) {
+    FILE *fp = fopen(path, "r");
+    if (!fp) return false;
+    char line[8192];
+    bool ok = true;
+    while (ok && fgets(line, sizeof line, fp)) {
+        if (line[0] == '#' || line[0] == '\n') continue;
+        int b = 0, rep = 1;
+        char k[8192];
+        const int n = sscanf(line, "%d,%8191[^,\n],%d", &b, k, &rep);
+        ok = n >= 2 && b >= 1 && rep >= 0;
+        for (int r = 0; ok && r < rep; r++) keys[b] += k;
+    }
+    fclose(fp);
+    return ok;
+}
+
+// -i / --steer: open the scenario, then advance / key / synthesize chunk by chunk on one GPU
+int run_steered(gpsb200_scenario_config_t sc, int sample_size, bool live, const char *steer_file, const char *log_file,
+                const std::string &out) {
+    std::map<int, std::string> sched;
+    if (steer_file && !read_schedule(steer_file, sched)) {
+        fprintf(stderr, "gpsb200-sim: cannot read schedule %s\n", steer_file);
+        return 1;
+    }
+    FILE *log = nullptr;
+    if (log_file && !(log = fopen(log_file, "w"))) {
+        fprintf(stderr, "gpsb200-sim: cannot write %s\n", log_file);
+        return 1;
+    }
+    sc.interactive = 1;
+    gpsb200_scenario_t *scn = nullptr;
+    if (gpsb200_scenario_open(&sc, &scn) != GPSB200_OK) {
+        fprintf(stderr, "scenario: %s\n", gpsb200_scenario_error(scn));
+        return 1;
+    }
+    const int nchan = gpsb200_scenario_channels(scn);
+    const bool motion = sc.motion_file && sc.motion_file[0];
+    if (motion) fprintf(stderr, "gpsb200-sim: user motion file supplied, interactive mode disabled (keys are ignored)\n");
+    const int batch = live ? 1 : 256, ring = 4;       // <= 2 frames per 256 blocks (one roll per 30 s)
+    const size_t blk_bytes = (size_t) GPSB200_BLOCK_ELEMS * sample_size;
+    gpsb200_ctx_t *ctx = nullptr;
+    gpsb200_bind_numa(0);
+    gpsb200_config_t cfg{};
+    cfg.max_chan = nchan;
+    cfg.max_blocks = batch;
+    cfg.max_nav_frames = ring;
+    if (gpsb200_create(&cfg, &ctx) != GPSB200_OK) {
+        fprintf(stderr, "gpsb200: %s\n", gpsb200_last_error(ctx));
+        return 1;
+    }
+    if (!fifo_create((unsigned) batch + 8, GPSB200_BLOCK_ELEMS, sample_size)) return 1;
+    // keys from stdin: a reader thread queues them; each applies to the first block not yet handed to the synthesis
+    std::mutex kmu;
+    std::deque<char> kq;
+    if (live) {
+        if (isatty(0) && tcgetattr(0, &g_tty) == 0) {
+            struct termios raw = g_tty;
+            raw.c_lflag &= ~(ICANON | ECHO);
+            raw.c_cc[VMIN] = 1;
+            raw.c_cc[VTIME] = 0;
+            if (tcsetattr(0, TCSANOW, &raw) == 0) g_tty_raw = true;
+            atexit(restore_tty);
+        }
+        std::thread([&kq, &kmu] {
+            char c;
+            while (read(0, &c, 1) == 1) {
+                std::lock_guard<std::mutex> lk(kmu);
+                kq.push_back(c);
+            }
+        }).detach();
+    }
+    signal(SIGINT, on_sigint);
+    bool writer = false;
+    int queued = 0, b = 0, uploaded = -1, rc = 0;
+    std::vector<gpsb200_chan_t> part((size_t) batch * nchan);
+    std::vector<int32_t> prev_prn(nchan, 0);
+    std::vector<double> carr(nchan, 0.0);
+    std::vector<void *> dsts(batch);
+    std::vector<struct iq_buf *> bufs(batch);
+    const double t0 = now_s();
+    while (!g_stop) {
+        std::string keys;
+        if (b >= 1) {
+            auto it = sched.find(b);
+            if (it != sched.end()) keys = it->second;
+            std::lock_guard<std::mutex> lk(kmu);
+            for (char c : kq)
+                if (strchr("adwseqtgxX", c)) keys += c;     // anything else (newlines, panels of the TUI) is ignored
+            kq.clear();
+        }
+        bool end = false;
+        for (char c : motion ? std::string() : keys) {
+            const int k = gpsb200_scenario_key(scn, c);
+            if (k == GPSB200_ERR_END) break;
+            if (k != GPSB200_OK) {
+                fprintf(stderr, "scenario: %s\n", gpsb200_scenario_error(scn));
+                end = true;
+                rc = 1;
+                break;
+            }
+        }
+        if (log && !keys.empty()) fprintf(log, "%d,%s\n", b, keys.c_str());
+        gpsb200_steer_state_t st;
+        gpsb200_scenario_steer_state(scn, &st);
+        if (end || st.next_block >= st.end_block) break;
+        int n = std::min(batch, st.end_block - b);
+        auto nx = sched.upper_bound(b);
+        if (nx != sched.end()) n = std::min(n, nx->first - b);
+        int32_t got = 0;
+        if (gpsb200_scenario_advance(scn, n, part.data(), &got) != GPSB200_OK) {
+            fprintf(stderr, "scenario: %s\n", gpsb200_scenario_error(scn));
+            rc = 1;
+            break;
+        }
+        for (int k = 0; k < got; k++)                    // NAV ring: upload a frame before the chunk that first uses it
+            for (int c = 0; c < nchan; c++) {
+                gpsb200_chan_t &p = part[(size_t) k * nchan + c];
+                if (p.nav_frame > uploaded) {
+                    const uint32_t *w = gpsb200_scenario_frame(scn, p.nav_frame);
+                    for (int cc = 0; cc < nchan; cc++)
+                        gpsb200_set_nav(ctx, p.nav_frame % ring, cc, w + (size_t) cc * GPSB200_NAV_WORDS);
+                    uploaded = p.nav_frame;
+                }
+                p.nav_frame %= ring;
+            }
+        for (int c = 0; c < nchan; c++)                  // continue the carrier chain across calls
+            if (part[c].prn > 0 && part[c].prn == prev_prn[c]) part[c].carr_phase = carr[c];
+        for (int c = 0; c < nchan; c++) prev_prn[c] = part[(size_t) (got - 1) * nchan + c].prn;
+        if (live) {                                      // real time, at most 8 blocks (the reference's FIFO) ahead
+            const double due = t0 + (b - 8) * 0.1 - now_s();
+            if (due > 0) std::this_thread::sleep_for(std::chrono::duration<double>(due));
+        }
+        for (int k = 0; k < got; k++) {
+            bufs[k] = fifo_acquire();
+            if (!bufs[k]) return 1;
+            dsts[k] = sample_size == GPSB200_SC16 ? (void *) bufs[k]->data16 : (void *) bufs[k]->data8;
+        }
+        if (gpsb200_synth_blocks_scatter(ctx, part.data(), got, nchan, sample_size, dsts.data(), carr.data(), nullptr) !=
+            GPSB200_OK) {
+            fprintf(stderr, "gpsb200: %s\n", gpsb200_last_error(ctx));
+            rc = 1;
+            break;
+        }
+        for (int k = 0; k < got; k++) {
+            if (!writer && queued >= 8) {
+                if (gpsb200_iqfile_start(out.c_str(), sample_size) != GPSB200_OK) return 1;
+                writer = true;
+            }
+            bufs[k]->validLength = GPSB200_BLOCK_ELEMS;
+            fifo_enqueue(bufs[k]);
+            queued++;
+        }
+        b += got;
+    }
+    if (!writer && gpsb200_iqfile_start(out.c_str(), sample_size) != GPSB200_OK) return 1;
+    gpsb200_iqfile_stop();
+    fifo_destroy();
+    gpsb200_destroy(ctx);
+    restore_tty();
+    if (log) fclose(log);
+    gpsb200_steer_state_t st;
+    gpsb200_scenario_steer_state(scn, &st);
+    fprintf(stderr, "gpsb200-sim: %d blocks (%d channels), steered%s -> %s; speed %.2f m/s, heading %.3f deg, climb %.0f m/s\n", b,
+            nchan, live ? " live" : "", out.c_str(), st.velocity, st.bearing_mdeg / 1000, st.vertical_speed);
+    gpsb200_scenario_destroy(scn);
+    return rc;
+}
+
 struct Handoff {                 // exact chain state after slice r, published by worker r
     std::mutex mu;
     std::condition_variable cv;
@@ -57,7 +250,8 @@ int main(int argc, char **argv) {
     sc.max_chan = 12;
     double dur = 300.0;
     int sample_size = GPSB200_SC08, gpus = 1;
-    bool compat = false;
+    bool compat = false, live = false, have_dur = false;
+    const char *steer_file = nullptr, *log_file = nullptr;
     std::string out = "iqdata.bin";
     for (int i = 1; i < argc; i++) {
         std::string a = argv[i];
@@ -70,7 +264,12 @@ int main(int argc, char **argv) {
         else if (a == "-t") {
             sc.target_valid = 1;                                    // gps-sim.c:145-148
             sscanf(need(), "%lf,%lf,%lf", &sc.target_distance_m, &sc.target_bearing_deg, &sc.target_height_m);
-        } else if (a == "-d") dur = atof(need());
+        } else if (a == "-d") {
+            dur = atof(need());
+            have_dur = true;
+        } else if (a == "-i") live = true;
+        else if (a == "--steer") steer_file = need();
+        else if (a == "--steer-log") log_file = need();
         else if (a == "-m") sc.motion_file = need();
         else if (a == "-s")
             sscanf(need(), "%d/%d/%d,%d:%d:%lf", &sc.start_year, &sc.start_month, &sc.start_day, &sc.start_hour,
@@ -88,7 +287,16 @@ int main(int argc, char **argv) {
         else usage();
     }
     if (!sc.nav_file || gpus < 1) usage();
+    if (live && !have_dur) dur = 86400.0;                         // the reference's default (gps-sim.c:190)
     sc.duration_ds = (int) (dur * 10.0 + 0.5);                  // gps-sim.c:140
+    if (live || steer_file) {
+        if (gpus != 1) {
+            fprintf(stderr, "gpsb200-sim: -i / --steer run on one GPU (time slices would need the keys of the future)\n");
+            return 2;
+        }
+        if (live && steer_file) usage();
+        return run_steered(sc, sample_size, live, steer_file, log_file, out);
+    }
 
     gpsb200_scenario_t *scn = nullptr;
     if (gpsb200_scenario_create(&sc, &scn) != GPSB200_OK) {
