@@ -289,7 +289,8 @@ typedef struct gpsb200_scenario_config {
     int32_t max_chan;              /* 12 as shipped (gps.h:36); up to 32 */
     int32_t ionosphere_enable;     /* 1 = reference default (-I clears it) */
     int32_t pluto_gain;            /* 1 = gain x 2 (gps.c:2759-2763) */
-    int32_t start_year, start_month, start_day, start_hour, start_min;   /* -s; year 0: first ephemeris epoch */
+    int32_t start_year, start_month, start_day, start_hour, start_min;   /* -s; year 0: first ephemeris epoch;
+                                                                             -s now: see gpsb200_scenario_create_now */
     int32_t rinex3;                /* -3: nav_file is RINEX v3 (gps.c:1512-1891) instead of v2 */
     double start_sec;
     /* -t distance,bearing,height (gps-sim.c:145-148, gps.c:2348-2357): static runs start at a point given by distance
@@ -319,6 +320,29 @@ const uint32_t *gpsb200_scenario_nav(const gpsb200_scenario_t *s);           /* 
 /* Time of applicability of the almanac in use as "yyyy/mm/dd,hh:mm:ss" (the last valid record's, gps.c:2644-2654), or
  * NULL when no valid record was read (no almanac_file, or nothing usable in it). */
 const char *gpsb200_scenario_almanac_date(const gpsb200_scenario_t *s);
+/* The resolved scenario start as "yyyy/mm/dd,hh:mm:ss" (seconds rounded as the reference prints them, gps.c:2580): the
+ * configured start, or the first ephemeris record's epoch when start_year is 0. NULL before the scenario is opened. */
+const char *gpsb200_scenario_start_date(const gpsb200_scenario_t *s);
+/* The same start as GPS week and second of week (the receiver time of the allocation, gps.c:2575-2584). */
+int gpsb200_scenario_start_time(const gpsb200_scenario_t *s, int32_t *week, double *sow);
+
+/* ---- `-s now`: the ephemeris time overwrite (gps-sim.c:89-102, gps.c:2531-2561) -------------------------------
+ * gpsb200_scenario_create_now / _open_now are _create / _open with the reference's time_overwrite set. cfg->start_* is
+ * the clock reading (the reference takes gmtime(time()) in whole seconds and uses UTC as GPS time, without the leap
+ * seconds; a caller that mirrors it passes the same). It is required and range-checked as the reference checks -s
+ * (gps-sim.c:106-114: year after 1980, month 1-12, day 1-31, 0-23 h, 0-59 min, 0 <= sec < 60), else GPSB200_ERR_ARG.
+ * Then, with gtmp = (start week, start second of week truncated to a multiple of 7200 s) and dsec = gtmp - toc of the
+ * first record of the file:
+ *   - every record's toc and toe move by dsec (week carry included), so the file may be of any date;
+ *   - the UTC reference becomes WNt = gtmp.week, tot = gtmp.sec; the iono/UTC valid flag stays as read, so subframe 4
+ *     page 18 carries tot / 4096 truncated and WNt mod 256;
+ *   - the ephemeris span check of an explicit start is skipped.
+ * Everything after that is the ordinary path on the moved times: the set within +-1 h of the start ("no current set
+ * of ephemerides" when there is none -- a one-set file and a start in the second hour of its 2-hour epoch), the
+ * 4-week almanac check against the start, the 30 s ephemeris roll. A moved toe second of week turns the constellation
+ * in longitude by OMEGA_E * (new toe.sec - old toe.sec) (gps.c:585), as in the reference. */
+int gpsb200_scenario_create_now(const gpsb200_scenario_config_t *cfg, gpsb200_scenario_t **out);
+int gpsb200_scenario_open_now(const gpsb200_scenario_config_t *cfg, gpsb200_scenario_t **out);
 
 /* ---- incremental scenario: the same engine advanced block range by block range -------------------------------
  * gpsb200_scenario_create == gpsb200_scenario_open + one advance over the whole run. An opened scenario keeps the

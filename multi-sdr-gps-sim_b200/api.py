@@ -110,7 +110,8 @@ EXPORTS = ["gpsb200_create", "gpsb200_destroy", "gpsb200_last_error", "gpsb200_v
            "gpsb200_scenario_blocks", "gpsb200_scenario_channels", "gpsb200_scenario_nav_frames",
            "gpsb200_scenario_chans", "gpsb200_scenario_nav", "gpsb200_scenario_almanac_date", "gpsb200_almanac_read",
            "gpsb200_scenario_open", "gpsb200_scenario_advance", "gpsb200_scenario_frame", "gpsb200_scenario_key",
-           "gpsb200_scenario_steer_state",
+           "gpsb200_scenario_steer_state", "gpsb200_scenario_open_now", "gpsb200_scenario_create_now",
+           "gpsb200_scenario_start_date", "gpsb200_scenario_start_time",
            "fifo_create", "fifo_destroy", "fifo_wait_next", "fifo_wait_full", "fifo_halt", "fifo_acquire",
            "fifo_enqueue", "fifo_dequeue", "fifo_release", "fifo_set_compat_drop",
            "gpsb200_iqfile_start", "gpsb200_iqfile_stop", "gpsb200_fifo_push", "gpsb200_fifo_push_flush"]
@@ -150,6 +151,11 @@ def lib():
         L.gpsb200_scenario_almanac_date.restype = C.c_char_p
         L.gpsb200_almanac_read.argtypes = [C.c_char_p, C.c_void_p, C.POINTER(C.c_int32)]
         L.gpsb200_scenario_open.argtypes = [C.POINTER(ScenarioConfig), C.POINTER(C.c_void_p)]
+        L.gpsb200_scenario_open_now.argtypes = [C.POINTER(ScenarioConfig), C.POINTER(C.c_void_p)]
+        L.gpsb200_scenario_create_now.argtypes = [C.POINTER(ScenarioConfig), C.POINTER(C.c_void_p)]
+        L.gpsb200_scenario_start_date.argtypes = [C.c_void_p]
+        L.gpsb200_scenario_start_date.restype = C.c_char_p
+        L.gpsb200_scenario_start_time.argtypes = [C.c_void_p, C.POINTER(C.c_int32), C.POINTER(C.c_double)]
         L.gpsb200_scenario_advance.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.POINTER(C.c_int32)]
         L.gpsb200_scenario_frame.argtypes = [C.c_void_p, C.c_int]
         L.gpsb200_scenario_frame.restype = C.c_void_p
@@ -308,25 +314,31 @@ def _scenario_config(nav_file, lat, lon, height, seconds, max_chan=12, motion_fi
 
 
 def scenario(nav_file, lat, lon, height, seconds, max_chan=12, motion_file=None, start=None,
-             ionosphere=True, pluto_gain=False, rinex3=False, target=None, almanac_file=None, info=None, steer=None):
+             ionosphere=True, pluto_gain=False, rinex3=False, target=None, almanac_file=None, info=None, steer=None,
+             time_overwrite=False):
     """Run the host scenario engine. -> (chans[nblk, max_chan] CHAN_DTYPE, nav[nframes, max_chan, 60] uint32).
     start: (y, m, d, hh, mm, sec) or None for the first ephemeris epoch. almanac_file: SEM almanac to transmit in
     subframes 4 and 5 (None: no almanac, the reference's --disable-almanac). info: optional dict that receives
-    "almanac_date" ("yyyy/mm/dd,hh:mm:ss", or None when no valid almanac record was read).
+    "almanac_date" ("yyyy/mm/dd,hh:mm:ss", or None when no valid almanac record was read) and "start_date" (the
+    resolved start, "yyyy/mm/dd,hh:mm:ss").
     steer: interactive run, [(block, keys, repeat), ...]: the string `keys`, `repeat` times, before `block` (>= 1);
-    built on the incremental engine (LiveScenario). [] is an interactive run without keys."""
+    built on the incremental engine (LiveScenario). [] is an interactive run without keys.
+    time_overwrite: the reference's `-s now` (gpsb200_scenario_create_now): `start` is the clock reading, and the
+    ephemeris and UTC reference times of the file are moved to it."""
     kw = dict(max_chan=max_chan, motion_file=motion_file, start=start, ionosphere=ionosphere, pluto_gain=pluto_gain,
               rinex3=rinex3, target=target, almanac_file=almanac_file)
     if steer is not None:
-        with LiveScenario(nav_file, lat, lon, height, seconds, interactive=True, **kw) as s:
+        with LiveScenario(nav_file, lat, lon, height, seconds, interactive=True, time_overwrite=time_overwrite, **kw) as s:
             chans, nav = s.run(steer)
             if info is not None:
                 info["almanac_date"] = s.almanac_date
+                info["start_date"] = s.start_date
             return chans, nav
     cfg = _scenario_config(nav_file, lat, lon, height, seconds, **kw)
     h = C.c_void_p()
     L = lib()
-    rc = L.gpsb200_scenario_create(C.byref(cfg), C.byref(h))
+    create = L.gpsb200_scenario_create_now if time_overwrite else L.gpsb200_scenario_create
+    rc = create(C.byref(cfg), C.byref(h))
     try:
         if rc:
             raise GpsB200Error(rc, L.gpsb200_scenario_error(h).decode() if h else "gpsb200_scenario_create")
@@ -337,6 +349,7 @@ def scenario(nav_file, lat, lon, height, seconds, max_chan=12, motion_file=None,
         if info is not None:
             d = L.gpsb200_scenario_almanac_date(h)
             info["almanac_date"] = d.decode() if d else None
+            info["start_date"] = L.gpsb200_scenario_start_date(h).decode()
         return chans.reshape(nblk, nch).copy(), nav.reshape(nfr, nch, 60).copy()
     finally:
         if h:
@@ -357,13 +370,15 @@ def parse_steer(text):
 
 class LiveScenario:
     """An opened scenario (gpsb200_scenario_open), advanced block range by block range and steered in between:
-    open -> advance(n) / key(k) / frame(f) / state() -> close."""
+    open -> advance(n) / key(k) / frame(f) / state() -> close. time_overwrite: the reference's `-s now`
+    (gpsb200_scenario_open_now), `start` being the clock reading."""
 
-    def __init__(self, nav_file, lat, lon, height, seconds, **kw):
+    def __init__(self, nav_file, lat, lon, height, seconds, time_overwrite=False, **kw):
         self._h = C.c_void_p()
         cfg = _scenario_config(nav_file, lat, lon, height, seconds, **kw)
         L = lib()
-        rc = L.gpsb200_scenario_open(C.byref(cfg), C.byref(self._h))
+        open_ = L.gpsb200_scenario_open_now if time_overwrite else L.gpsb200_scenario_open
+        rc = open_(C.byref(cfg), C.byref(self._h))
         if rc:
             msg = L.gpsb200_scenario_error(self._h).decode() if self._h else "gpsb200_scenario_open"
             self.close()
@@ -372,6 +387,7 @@ class LiveScenario:
         self.channels = L.gpsb200_scenario_channels(self._h)
         d = L.gpsb200_scenario_almanac_date(self._h)
         self.almanac_date = d.decode() if d else None
+        self.start_date = L.gpsb200_scenario_start_date(self._h).decode()
 
     def close(self):
         if self._h:

@@ -18,8 +18,9 @@
 // tests/test_scenario.py compares every field with the reference's own dumps.
 //
 // Scope notes: the almanac comes from a SEM file the caller names (the reference reads ./almanac.sem implicitly;
-// without a file the pages are the reference's with --disable-almanac, as in all BASELINE configs); downloads, `-s now`
-// and the HackRF/Pluto specifics (except the Pluto gain doubling) are out of scope.
+// without a file the pages are the reference's with --disable-almanac, as in all BASELINE configs); `-s now` is the
+// time overwrite of gpsb200_scenario_open_now / _create_now (gps.c:2531-2561), the clock reading being the caller's;
+// downloads and the HackRF/Pluto specifics (except the Pluto gain doubling) are out of scope.
 #include <algorithm>
 #include <cmath>
 #include <cstdio>
@@ -786,7 +787,10 @@ struct gpsb200_scenario {
     int nframes = 0, nav_base = 0;
     std::string err;
     std::string almanac_date;                       // empty: no valid almanac record
+    std::string start_date;                         // the resolved start, "yyyy/mm/dd,hh:mm:ss"
+    GpsTime g0;                                     // ... as GPS time
 
+    bool time_overwrite = false;                    // -s now (gps-sim.c:89-102): opened through _open_now
     bool opened = false;
     std::vector<Eph> eph;                           // [kEphSets][kMaxSat]
     int ieph = 0;
@@ -925,10 +929,12 @@ int open_scenario(gpsb200_scenario *S) {
 
     // scenario start (gps.c:2502-2577)
     GpsTime gmin, gmax, g0;
+    Date start;
     bool have = false;
     for (int sv = 0; sv < kMaxSat && !have; sv++)
         if (eph[0][sv].valid) {
             gmin = eph[0][sv].toc;
+            start = eph[0][sv].t;                   // tmin: the start when none is given
             have = true;
         }
     for (int sv = 0; sv < kMaxSat; sv++)
@@ -946,9 +952,35 @@ int open_scenario(gpsb200_scenario *S) {
         t.sec = cfg.start_sec;
         if (t.m < 1 || t.m > 12) return fail(S, "invalid start date");
         g0 = date_to_gps(t);
-        if (gps_diff(g0, gmin) < 0.0 || gps_diff(gmax, g0) < 0.0) return fail(S, "start time outside the ephemeris span");
+        start = t;
+        if (S->time_overwrite) {
+            // -s now: every record's toc and toe, and the UTC reference time, move by the distance from the first
+            // record's toc to the start's 2-hour epoch (gps.c:2533-2561). The iono/UTC valid flag stays as read, so
+            // subframe 4 page 18 carries tot / 4096 truncated. There is no span check: the file may be of any date.
+            GpsTime gtmp;
+            gtmp.week = g0.week;
+            gtmp.sec = (double) (((int) (g0.sec)) / 7200) * 7200.0;
+            const double dsec = gps_diff(gtmp, gmin);
+            io.wnt = gtmp.week;
+            io.tot = (int) gtmp.sec;
+            for (int sv = 0; sv < kMaxSat; sv++)
+                for (int i = 0; i < neph; i++)
+                    if (eph[i][sv].valid) {
+                        eph[i][sv].toc = gps_add(eph[i][sv].toc, dsec);
+                        eph[i][sv].t = gps_to_date(eph[i][sv].toc);
+                        eph[i][sv].toe = gps_add(eph[i][sv].toe, dsec);
+                    }
+        } else if (gps_diff(g0, gmin) < 0.0 || gps_diff(gmax, g0) < 0.0) {
+            return fail(S, "start time outside the ephemeris span");
+        }
     } else {
         g0 = gmin;
+    }
+    {
+        char buf[64];
+        snprintf(buf, sizeof buf, "%4d/%02d/%02d,%02d:%02d:%02.0f", start.y, start.m, start.d, start.hh, start.mm, start.sec);
+        S->start_date = buf;
+        S->g0 = g0;
     }
     int ieph = -1;
     for (int i = 0; i < neph && ieph < 0; i++)
@@ -1177,23 +1209,44 @@ static_assert(sizeof(gpsb200_steer_state_t) == 64, "gpsb200_steer_state_t layout
 
 extern "C" {
 
-int gpsb200_scenario_open(const gpsb200_scenario_config_t *cfg, gpsb200_scenario_t **out) {
+static int open_with(const gpsb200_scenario_config_t *cfg, gpsb200_scenario_t **out, bool time_overwrite) {
     if (!cfg || !out || !cfg->nav_file) return GPSB200_ERR_ARG;
     gpsb200_scenario *S = new gpsb200_scenario();
     S->cfg = *cfg;
     S->nchan = cfg->max_chan > 0 ? cfg->max_chan : 12;
+    S->time_overwrite = time_overwrite;
     *out = S;
     if (S->nchan > GPSB200_MAX_CHAN) return fail(S, "max_chan > 32");
+    if (time_overwrite) {                           // the clock reading passes the -s range check (gps-sim.c:106-114)
+        const gpsb200_scenario_config_t &c = *cfg;
+        if (c.start_year <= 1980 || c.start_month < 1 || c.start_month > 12 || c.start_day < 1 || c.start_day > 31 ||
+            c.start_hour < 0 || c.start_hour > 23 || c.start_min < 0 || c.start_min > 59 || !(c.start_sec >= 0.0) ||
+            c.start_sec >= 60.0)
+            return fail(S, "invalid date and time: the time overwrite needs the clock reading as start, after 1980");
+    }
     return open_scenario(S);
 }
 
-int gpsb200_scenario_create(const gpsb200_scenario_config_t *cfg, gpsb200_scenario_t **out) {
-    const int rc = gpsb200_scenario_open(cfg, out);
+static int create_with(const gpsb200_scenario_config_t *cfg, gpsb200_scenario_t **out, bool time_overwrite) {
+    const int rc = open_with(cfg, out, time_overwrite);
     if (rc != GPSB200_OK) return rc;
     gpsb200_scenario *S = *out;
     S->chans.resize((size_t) S->nblocks * S->nchan);
     advance_blocks(S, S->nblocks, S->chans.data());
     return GPSB200_OK;
+}
+
+int gpsb200_scenario_open(const gpsb200_scenario_config_t *cfg, gpsb200_scenario_t **out) {
+    return open_with(cfg, out, false);
+}
+int gpsb200_scenario_create(const gpsb200_scenario_config_t *cfg, gpsb200_scenario_t **out) {
+    return create_with(cfg, out, false);
+}
+int gpsb200_scenario_open_now(const gpsb200_scenario_config_t *cfg, gpsb200_scenario_t **out) {
+    return open_with(cfg, out, true);
+}
+int gpsb200_scenario_create_now(const gpsb200_scenario_config_t *cfg, gpsb200_scenario_t **out) {
+    return create_with(cfg, out, true);
 }
 
 int gpsb200_scenario_advance(gpsb200_scenario_t *s, int nblk, gpsb200_chan_t *chans_out, int32_t *got) {
@@ -1279,6 +1332,15 @@ const gpsb200_chan_t *gpsb200_scenario_chans(const gpsb200_scenario_t *s) { retu
 const uint32_t *gpsb200_scenario_nav(const gpsb200_scenario_t *s) { return s ? s->nav.data() : nullptr; }
 const char *gpsb200_scenario_almanac_date(const gpsb200_scenario_t *s) {
     return s && !s->almanac_date.empty() ? s->almanac_date.c_str() : nullptr;
+}
+const char *gpsb200_scenario_start_date(const gpsb200_scenario_t *s) {
+    return s && s->opened ? s->start_date.c_str() : nullptr;
+}
+int gpsb200_scenario_start_time(const gpsb200_scenario_t *s, int32_t *week, double *sow) {
+    if (!s || !s->opened) return GPSB200_ERR_ARG;
+    if (week) *week = s->g0.week;
+    if (sow) *sow = s->g0.sec;
+    return GPSB200_OK;
 }
 
 int gpsb200_almanac_read(const char *path, gpsb200_almanac_record_t rec[32], int32_t *valid) {

@@ -17,6 +17,9 @@
 // opened, not built up front, and advanced chunk by chunk; keys (from stdin, paced to real time, or replayed from a
 // schedule) are applied between advances. Each chunk is synthesized with gpsb200_synth_blocks_scatter, the carrier
 // chain continued across calls, the NAV frames kept in a ring of context slots (global frame f in slot f mod R).
+// -s now: the start is the UTC clock read while the arguments are parsed (gps-sim.c:89-102), and the scenario is opened
+// with the reference's ephemeris time overwrite (gpsb200_scenario_create_now / _open_now) on every path; --now DATE
+// replaces the clock reading (a session replayed, a test).
 #include <algorithm>
 #include <atomic>
 #include <chrono>
@@ -33,6 +36,7 @@
 #include <vector>
 
 #include <termios.h>
+#include <time.h>
 #include <unistd.h>
 
 #include <cuda_runtime_api.h>
@@ -41,9 +45,13 @@
 
 static void usage() {
     fprintf(stderr,
-            "gpsb200-sim -e NAV[.gz] [-3] -l lat,lon,h [-t dist,bearing,height] [-d SEC] [-m motion.csv] [-s y/m/d,h:m:s]\n"
-            "            [--iq16] [-I] [--pluto-gain] [--chan N] [--gpus N] [-o iqdata.bin] [--compat-drop]\n"
-            "            [--almanac FILE.sem | --disable-almanac] [-i | --steer FILE] [--steer-log FILE]\n"
+            "gpsb200-sim -e NAV[.gz] [-3] -l lat,lon,h [-t dist,bearing,height] [-d SEC] [-m motion.csv]\n"
+            "            [-s y/m/d,h:m:s | -s now [--now y/m/d,h:m:s]] [--iq16] [-I] [--pluto-gain] [--chan N] [--gpus N]\n"
+            "            [-o iqdata.bin] [--compat-drop] [--almanac FILE.sem | --disable-almanac] [-i | --steer FILE]\n"
+            "            [--steer-log FILE]\n"
+            "  -s now          start at the current time (UTC used as GPS time, as the reference does): the ephemeris and\n"
+            "                  UTC reference times of the file are moved to it, so a file of any date can be used\n"
+            "  --now DATE      with -s now: use DATE instead of the clock (replay a session)\n"
             "  -i              interactive: keys from stdin (a/d heading, w/s climb, e/q speed, x end), paced to real time\n"
             "  --steer FILE    replay a schedule, one line per event \"B,KEYS[,REPEAT]\": KEYS, REPEAT times, before block B\n"
             "  --steer-log F   write the schedule that was applied (replays byte-identically with --steer)\n");
@@ -83,9 +91,34 @@ bool read_schedule(const char *path, std::map<int, std::string> &keys) {
     return ok;
 }
 
+// "y/m/d,h:m:s" -> the start fields; all six are required
+bool parse_date(const char *s, gpsb200_scenario_config_t &sc) {
+    return sscanf(s, "%d/%d/%d,%d:%d:%lf", &sc.start_year, &sc.start_month, &sc.start_day, &sc.start_hour, &sc.start_min,
+                  &sc.start_sec) == 6;
+}
+
+// the -s range check (gps-sim.c:106-114)
+bool date_in_range(const gpsb200_scenario_config_t &sc) {
+    return !(sc.start_year <= 1980 || sc.start_month < 1 || sc.start_month > 12 || sc.start_day < 1 || sc.start_day > 31 ||
+             sc.start_hour < 0 || sc.start_hour > 23 || sc.start_min < 0 || sc.start_min > 59 || !(sc.start_sec >= 0.0) ||
+             sc.start_sec >= 60.0);
+}
+
+int open_scenario(const gpsb200_scenario_config_t &sc, bool now, bool build, gpsb200_scenario_t **scn) {
+    if (build) return now ? gpsb200_scenario_create_now(&sc, scn) : gpsb200_scenario_create(&sc, scn);
+    return now ? gpsb200_scenario_open_now(&sc, scn) : gpsb200_scenario_open(&sc, scn);
+}
+
+void print_start(const gpsb200_scenario_t *scn) {
+    int32_t week = 0;
+    double sow = 0;
+    gpsb200_scenario_start_time(scn, &week, &sow);
+    fprintf(stderr, "gpsb200-sim: start time: %s (week %d, sow %.10g)\n", gpsb200_scenario_start_date(scn), week, sow);
+}
+
 // -i / --steer: open the scenario, then advance / key / synthesize chunk by chunk on one GPU
-int run_steered(gpsb200_scenario_config_t sc, int sample_size, bool live, const char *steer_file, const char *log_file,
-                const std::string &out) {
+int run_steered(gpsb200_scenario_config_t sc, bool now, int sample_size, bool live, const char *steer_file,
+                const char *log_file, const std::string &out) {
     std::map<int, std::string> sched;
     if (steer_file && !read_schedule(steer_file, sched)) {
         fprintf(stderr, "gpsb200-sim: cannot read schedule %s\n", steer_file);
@@ -98,10 +131,11 @@ int run_steered(gpsb200_scenario_config_t sc, int sample_size, bool live, const 
     }
     sc.interactive = 1;
     gpsb200_scenario_t *scn = nullptr;
-    if (gpsb200_scenario_open(&sc, &scn) != GPSB200_OK) {
+    if (open_scenario(sc, now, false, &scn) != GPSB200_OK) {
         fprintf(stderr, "scenario: %s\n", gpsb200_scenario_error(scn));
         return 1;
     }
+    print_start(scn);
     const int nchan = gpsb200_scenario_channels(scn);
     const bool motion = sc.motion_file && sc.motion_file[0];
     if (motion) fprintf(stderr, "gpsb200-sim: user motion file supplied, interactive mode disabled (keys are ignored)\n");
@@ -250,8 +284,8 @@ int main(int argc, char **argv) {
     sc.max_chan = 12;
     double dur = 300.0;
     int sample_size = GPSB200_SC08, gpus = 1;
-    bool compat = false, live = false, have_dur = false;
-    const char *steer_file = nullptr, *log_file = nullptr;
+    bool compat = false, live = false, have_dur = false, have_start = false, now = false;
+    const char *steer_file = nullptr, *log_file = nullptr, *now_arg = nullptr;
     std::string out = "iqdata.bin";
     for (int i = 1; i < argc; i++) {
         std::string a = argv[i];
@@ -271,9 +305,25 @@ int main(int argc, char **argv) {
         else if (a == "--steer") steer_file = need();
         else if (a == "--steer-log") log_file = need();
         else if (a == "-m") sc.motion_file = need();
-        else if (a == "-s")
-            sscanf(need(), "%d/%d/%d,%d:%d:%lf", &sc.start_year, &sc.start_month, &sc.start_day, &sc.start_hour,
-                   &sc.start_min, &sc.start_sec);
+        else if (a == "-s") {
+            const char *v = need();
+            have_start = true;
+            if (strncmp(v, "now", 3) == 0) {                        // gps-sim.c:89-102: whole seconds of UTC
+                now = true;
+                const time_t t = time(nullptr);
+                struct tm g;
+                gmtime_r(&t, &g);
+                sc.start_year = g.tm_year + 1900;
+                sc.start_month = g.tm_mon + 1;
+                sc.start_day = g.tm_mday;
+                sc.start_hour = g.tm_hour;
+                sc.start_min = g.tm_min;
+                sc.start_sec = (double) g.tm_sec;
+            } else if (!parse_date(v, sc)) {
+                fprintf(stderr, "gpsb200-sim: -s %s: expected y/m/d,h:m:s or now\n", v);
+                return 2;
+            }
+        } else if (a == "--now") now_arg = need();
         else if (a == "--iq16") sample_size = GPSB200_SC16;
         else if (a == "-I") sc.ionosphere_enable = 0;
         else if (a == "-3") sc.rinex3 = 1;
@@ -287,6 +337,21 @@ int main(int argc, char **argv) {
         else usage();
     }
     if (!sc.nav_file || gpus < 1) usage();
+    if (now_arg) {
+        if (!now) {
+            fprintf(stderr, "gpsb200-sim: --now replaces the clock reading of -s now and needs it\n");
+            return 2;
+        }
+        if (!parse_date(now_arg, sc)) {
+            fprintf(stderr, "gpsb200-sim: --now %s: expected y/m/d,h:m:s\n", now_arg);
+            return 2;
+        }
+    }
+    if (have_start && !date_in_range(sc)) {
+        fprintf(stderr, "gpsb200-sim: invalid date and time: %d/%d/%d,%d:%d:%g\n", sc.start_year, sc.start_month,
+                sc.start_day, sc.start_hour, sc.start_min, sc.start_sec);
+        return 2;
+    }
     if (live && !have_dur) dur = 86400.0;                         // the reference's default (gps-sim.c:190)
     sc.duration_ds = (int) (dur * 10.0 + 0.5);                  // gps-sim.c:140
     if (live || steer_file) {
@@ -295,14 +360,15 @@ int main(int argc, char **argv) {
             return 2;
         }
         if (live && steer_file) usage();
-        return run_steered(sc, sample_size, live, steer_file, log_file, out);
+        return run_steered(sc, now, sample_size, live, steer_file, log_file, out);
     }
 
     gpsb200_scenario_t *scn = nullptr;
-    if (gpsb200_scenario_create(&sc, &scn) != GPSB200_OK) {
+    if (open_scenario(sc, now, true, &scn) != GPSB200_OK) {
         fprintf(stderr, "scenario: %s\n", gpsb200_scenario_error(scn));
         return 1;
     }
+    print_start(scn);
     const int nblk = gpsb200_scenario_blocks(scn), nchan = gpsb200_scenario_channels(scn);
     const int nframes = gpsb200_scenario_nav_frames(scn);
     const char *alm_date = gpsb200_scenario_almanac_date(scn);             // gps.c:2652-2656
