@@ -264,9 +264,11 @@ int gpsb200_checkpoint_segments_host(double start_true, double start_guess, doub
  * logic, executed on the CPU, int16 I/Q out. force bits: 1 = repair every sample's index, 2 = exact chip signs for every
  * window, 4 = every repair walks exactly from the run anchor, 8 = carry points of every window by the FP64 second
  * opinion instead of the 32-bit estimate. counters[4] = fast samples, repaired samples, exactly
- * rebuilt sign windows, exact walks. For tests (the algorithm against the oracle without a GPU); not a product path. */
+ * rebuilt sign windows, exact walks. signs (NULL: not wanted) [nchan][3125][3]: the sign words of every 96-sample
+ * window of the block as the synthesis reads them (word j, bit 11 (i mod 3) + i / 3: chip XOR data bit of sample
+ * 32 j + i; idle channels untouched). For tests (the algorithm against the oracle without a GPU); not a product path. */
 int gpsb200_lanes_model_block(const gpsb200_chan_t *chans, int nchan, const uint32_t *nav, int run_samples, int force,
-                              int16_t *iq, double *carr_out, int64_t *counters);
+                              int16_t *iq, double *carr_out, int64_t *counters, uint32_t *signs);
 
 /* C/A code of prn (1..32) as 0/1 chips (codegen, gps.c:272-309). */
 int gpsb200_codegen(int prn, uint8_t ca[GPSB200_CA_LEN]);

@@ -217,21 +217,24 @@ def carrier_chain(chans, phase_in=None, threads=16):
     return out
 
 
-def lanes_model_block(chans_row, nav_frame, run_samples=2400, force=0):
+def lanes_model_block(chans_row, nav_frame, run_samples=2400, force=0, want_signs=False):
     """Host model of the lane = sample kernel for one block. chans_row: CHAN_DTYPE[nchan]; nav_frame: uint32[nchan, 60].
-    -> (iq int16[600000], carr_out float64[nchan], counters int64[4])"""
+    -> (iq int16[600000], carr_out float64[nchan], counters int64[4]), and with want_signs the sign words of every window
+    (uint32[nchan, 3125, 3]; word j, bit 11 (i % 3) + i // 3: chip XOR data bit of sample 32 j + i of the window)"""
     a = np.ascontiguousarray(chans_row, dtype=CHAN_DTYPE)
     nv = np.ascontiguousarray(nav_frame, dtype=np.uint32)
     iq = np.zeros(BLOCK_ELEMS, np.int16)
     co = np.zeros(a.size, np.float64)
     cnt = np.zeros(4, np.int64)
+    signs = np.zeros((a.size, BLOCK_SAMPLES // 96, 3), np.uint32) if want_signs else None
     L = lib()
-    L.gpsb200_lanes_model_block.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
+    L.gpsb200_lanes_model_block.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
+                                            C.c_void_p]
     rc = L.gpsb200_lanes_model_block(a.ctypes.data, a.size, nv.ctypes.data, run_samples, force, iq.ctypes.data, co.ctypes.data,
-                                     cnt.ctypes.data)
+                                     cnt.ctypes.data, None if signs is None else signs.ctypes.data)
     if rc:
         raise GpsB200Error(rc, "gpsb200_lanes_model_block")
-    return iq, co, cnt
+    return (iq, co, cnt, signs) if want_signs else (iq, co, cnt)
 
 
 def span_chain_host(f_carr, start_true, start_guess):

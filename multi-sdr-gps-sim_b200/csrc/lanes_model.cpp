@@ -25,7 +25,8 @@ int sine512_host(int k) {
 
 extern "C" int gpsb200_lanes_model_block(const gpsb200_chan_t *chans, int nchan, const uint32_t *nav /* [nchan][60] */,
                                          int run_samples, int force, int16_t *iq /* [600000] */, double *carr_out,
-                                         int64_t *counters /* [4]: fast, repaired samples, slow windows, walks */) {
+                                         int64_t *counters /* [4]: fast, repaired samples, slow windows, walks */,
+                                         uint32_t *signs /* [nchan][3125][3] or NULL */) {
     if (!chans || !nav || !iq || nchan < 1 || nchan > 32 || run_samples % lanes::kWindow != 0 || run_samples > lanes::kMaxRun ||
         GPSB200_BLOCK_SAMPLES % run_samples != 0)
         return GPSB200_ERR_ARG;
@@ -81,10 +82,16 @@ extern "C" int gpsb200_lanes_model_block(const gpsb200_chan_t *chans, int nchan,
                 }
                 base[c] = lanes::fast_base(st[c]);
                 step[c] = lanes::fast_step(st[c]);
+                if (signs) {
+                    const size_t win = (size_t) r * nwin + (size_t) w;
+                    memcpy(signs + ((size_t) c * (GPSB200_BLOCK_SAMPLES / lanes::kWindow) + win) * 3, &S[3 * c], 3 * sizeof(uint32_t));
+                }
             }
             for (int n = 0; n < lanes::kWindow; n++) {
-                const int q = n / 3, rr = n - 3 * q;
-                int acc = 0;
+                // as the kernel: the table entry of the unsigned phase into acc_all and, for a negative chip x data bit,
+                // into acc_neg as well; the sample is acc_all - 2 acc_neg (modulo 2^32, as the packed I + (Q << 16) sums)
+                const uint32_t bit = 1u << lanes::sign_pos(n & 31);
+                uint32_t acc_all = 0, acc_neg = 0;
                 bool repaired = false;
                 for (int c = 0; c < nchan; c++) {
                     if (!st[c].active) continue;
@@ -97,9 +104,10 @@ extern "C" int gpsb200_lanes_model_block(const gpsb200_chan_t *chans, int nchan,
                         k = lanes::exact_index(st[c].P, st[c].D, an[c], w, n, (force & 4) != 0);
                         repaired = true;
                     }
-                    const int sign = (int) ((S[3 * c + rr] >> q) & 1u);
-                    acc += tab[c][k ^ (sign << 8)];                       // table[k ^ 256] = -table[k]
+                    acc_all += (uint32_t) tab[c][k];
+                    if (S[3 * c + (n >> 5)] & bit) acc_neg += (uint32_t) tab[c][k];      // table[k ^ 256] = -table[k]
                 }
+                const int acc = (int) (acc_all - 2u * acc_neg);
                 ++cnt[repaired ? 1 : 0];
                 const int iv = (int) (short) (acc & 0xFFFF), qv = (acc - iv) >> 16;
                 const size_t o = ((size_t) r * run_samples + (size_t) w * lanes::kWindow + n) * 2;

@@ -12,8 +12,10 @@
 //   channel side  up to 16 channels: lane = (half h, channel c), state of channel c at window w + h of the warp's run,
 //                 every trip produces the chip-sign words and the 32-bit phase base of TWO windows into shared memory;
 //                 17..32 channels: lane = channel, one window per trip
-//   sample side   lane q: samples 3q, 3q+1, 3q+2 of each window of the trip: per channel one broadcast read of the
-//                 window record, three table look-ups (index and sign from one 32-bit word), register accumulation
+//   sample side   lane i: samples i, 32 + i, 64 + i of each window of the trip: per channel one broadcast read of the
+//                 window record, three table look-ups at the unsigned phase (32 consecutive samples per look-up: at
+//                 most 27 entries at 5 kHz, in distinct banks or broadcast), the chip x data-bit sign applied after
+//                 the look-up through a second, predicated accumulator
 //   output        quantise + pack (gps.c:2833-2845), staged per warp, written with 16-byte stores
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -30,7 +32,7 @@ constexpr int kLaneWarps = 16;
 constexpr int kLaneChipWords = 36;      // 1023 chips periodically extended to 1152 bits (window_signs reads word j0/32 + 2)
 
 struct LaneWin {
-    uint32_t s0, s1, s2;                // chip-sign words of the residue classes (bit q: sample 3q + r)
+    uint32_t s0, s1, s2;                // sign words of samples 0..31, 32..63, 64..95 (bit lanes::sign_pos(i): sample 32 j + i)
     uint32_t base;                      // 32-bit carrier phase of sample 0, biased by -1 (fast_base)
 };
 
@@ -38,8 +40,10 @@ struct LaneWin {
 // prepare two consecutive windows per trip, with CH = 32 the warp prepares one.
 // The carrier tables ([channel][k]: I + (Q << 16), gain-scaled, gps.c:2781-2782; 2 KB per channel) sit in front of this
 // struct at a 2 KB-aligned shared address, so that "table base | byte offset of k" is one logic instruction. Entry k of
-// channel c is stored at k ^ swz(c) (swz(c) = c * 32 / CH): the transposing fill from k_tables' [k][channel] layout is then
-// free of bank conflicts, and the look-ups fold the swizzle into the same logic instruction ("^ (base | swz)").
+// channel c is stored at (k + swz(c)) mod 512 (swz(c) = c * 32 / CH): the transposing fill from k_tables' [k][channel]
+// layout is then free of bank conflicts, and the look-ups take the rotation from the phase itself: the channel side adds
+// swz(c) << 23 to the window's phase base, so that the top 9 bits of a sample's phase are its stored slot. Channel c's
+// table base is then a compile-time offset from the loop's base in the unrolled channel loop.
 template <int CH>
 struct LanesSmem {
     static constexpr int kWins = 32 / CH;
@@ -56,6 +60,14 @@ __device__ __forceinline__ uint64_t shfl64(uint64_t v, int src) {
     const uint32_t lo = __shfl_sync(0xFFFFFFFFu, (uint32_t) v, src);
     const uint32_t hi = __shfl_sync(0xFFFFFFFFu, (uint32_t) (v >> 32), src);
     return ((uint64_t) hi << 32) | lo;
+}
+
+// acc += e if (w & bit) != 0, as one logic instruction that sets a predicate and one predicated add: written as C++ the
+// compiler selects (SEL) and then adds, one instruction more per channel-sample.
+__device__ __forceinline__ void add_if(int &acc, uint32_t w, uint32_t bit, int e) {
+    asm("{\n\t.reg .pred p;\n\t.reg .b32 t;\n\tand.b32 t, %1, %2;\n\tsetp.ne.u32 p, t, 0;\n\t@p add.s32 %0, %0, %3;\n\t}"
+        : "+r"(acc)
+        : "r"(w), "r"(bit), "r"(e));
 }
 
 template <bool IQ16, int CH>
@@ -81,7 +93,7 @@ __global__ void __launch_bounds__(kLaneWarps * 32, 2) k_synth_lanes(SynthArgs a)
         const int32_t *src = a.atab + (size_t) b * kAtabRows * 32;             // [k][lane], column c = channel c
         for (int i = tid; i < 512 * CH; i += nthr) {
             const int k = i / CH, c = i - k * CH;
-            tab[c * 512 + (k ^ (c * SWZ))] = c < nchan ? src[k * 32 + c] : 0;
+            tab[c * 512 + ((k + c * SWZ) & 511)] = c < nchan ? src[k * 32 + c] : 0;
         }
         for (int i = tid; i < CH * kLaneChipWords; i += nthr) {
             const int c = i / kLaneChipWords, w = i - c * kLaneChipWords;
@@ -109,9 +121,8 @@ __global__ void __launch_bounds__(kLaneWarps * 32, 2) k_synth_lanes(SynthArgs a)
     const uint32_t *chip_row = &sm.chips[ch][0];
     auto navf = [nav_row](int iw) { return nav_row[iw]; };
     auto chipf = [chip_row](int i) { return chip_row[i]; };
-    const uint32_t lane3 = 3u * (uint32_t) lane;                                  // sample side
-    uint32_t pw;                             // bit lane -> bit 31 by a MULTIPLICATION (FMA pipe): opaque to the compiler,
-    asm volatile("mov.b32 %0, %1;" : "=r"(pw) : "r"(1u << (31 - lane)));          // which would turn it back into a shift
+    const uint32_t n0 = (uint32_t) lane, n1 = n0 + 32u, n2 = n0 + 64u;              // sample side: this lane's samples
+    const uint32_t sbit = 1u << lanes::sign_pos(lane);                            // and sign bit
     const int nwin = a.run_samples / lanes::kWindow;
     uint32_t *stage = &sm.stage[warp][0];
 
@@ -140,10 +151,10 @@ __global__ void __launch_bounds__(kLaneWarps * 32, 2) k_synth_lanes(SynthArgs a)
         for (int w = 0; w < nwin; w += WINS) {
             {
                 uint32_t S[3] = {0u, 0u, 0u};
-                uint32_t base = 0u;
+                uint32_t base = (uint32_t) (ch * SWZ) << 23;                        // rotation of the channel's table
                 if (chan_ok && w + half < nwin) {
                     if (!lanes::window_signs(s, chipf, navf, S)) lanes::exact_signs(an, w + half, chipf, navf, S);
-                    base = lanes::fast_base(s);
+                    base += lanes::fast_base(s);
                 }
                 *reinterpret_cast<uint4 *>(&sm.win[warp][half][ch]) = make_uint4(S[0], S[1], S[2], base);
             }
@@ -154,41 +165,47 @@ __global__ void __launch_bounds__(kLaneWarps * 32, 2) k_synth_lanes(SynthArgs a)
             for (int hh = 0; hh < WINS; hh++) {
                 if (w + hh >= nwin) break;
                 const LaneWin *wrow = &sm.win[warp][hh][0];
-                int acc0 = 0, acc1 = 0, acc2 = 0;
+                // all_j: every channel's entry at the unsigned phase; neg_j: those of the channels whose chip x data bit
+                // is negative. The sample is all_j - 2 neg_j: table[k ^ 256] = -table[k] entry by entry, and the packed
+                // I + (Q << 16) sums are linear modulo 2^32.
+                int all0 = 0, all1 = 0, all2 = 0, neg0 = 0, neg1 = 0, neg2 = 0;
                 uint32_t dmax = 0u;
-                // Two channels per trip (an odd count is padded with the next slot, which is all zeros). The integer work is
-                // split over both integer pipes on purpose (with shifts only, the ALU pipe limits while the FMA pipe idles):
-                // the sign bit reaches bit 31 through a multiplication by the lane's power of two.
+                // Two channels per trip (an odd count is padded with the next slot, which is all zeros).
+                const LaneWin *wp = wrow;
+                const uint32_t *sp = &sm.step[warp][0];
+                uint32_t ta = tab_base;                                        // table of channel c; c + 1 at + 2048
 #pragma unroll 4
-                for (int c = 0; c < nchan; c += 2) {
-                    const uint4 wa = *reinterpret_cast<const uint4 *>(&wrow[c]);      // broadcast
-                    const uint4 wb = *reinterpret_cast<const uint4 *>(&wrow[c + 1]);
-                    const uint2 st = *reinterpret_cast<const uint2 *>(&sm.step[warp][c]);
-                    const uint32_t a0 = wa.w + lane3 * st.x, a1 = a0 + st.x, a2 = a1 + st.x;
-                    const uint32_t b0 = wb.w + lane3 * st.y, b1 = b0 + st.y, b2 = b1 + st.y;
-                    // chip x data-bit sign = half a cycle: table[k ^ 256] = -table[k]
-                    const uint32_t qa0 = a0 ^ ((wa.x * pw) & 0x80000000u), qa1 = a1 ^ ((wa.y * pw) & 0x80000000u),
-                                   qa2 = a2 ^ ((wa.z * pw) & 0x80000000u);
-                    const uint32_t qb0 = b0 ^ ((wb.x * pw) & 0x80000000u), qb1 = b1 ^ ((wb.y * pw) & 0x80000000u),
-                                   qb2 = b2 ^ ((wb.z * pw) & 0x80000000u);
-                    // table base (low 11 bits zero) | swizzle of the channel as a byte offset (< 128): linear in c
-                    const uint32_t ta = tab_base + (uint32_t) c * (2048u + 4u * SWZ), tb = ta + (2048u + 4u * SWZ);
+                for (int c = 0; c < nchan; c += 2, wp += 2, sp += 2, ta += 2 * 2048u) {
+                    const uint4 wa = *reinterpret_cast<const uint4 *>(&wp[0]);       // broadcast
+                    const uint4 wb = *reinterpret_cast<const uint4 *>(&wp[1]);
+                    const uint2 st = *reinterpret_cast<const uint2 *>(sp);
+                    const uint32_t a0 = wa.w + n0 * st.x, a1 = wa.w + n1 * st.x, a2 = wa.w + n2 * st.x;
+                    const uint32_t b0 = wb.w + n0 * st.y, b1 = wb.w + n1 * st.y, b2 = wb.w + n2 * st.y;
+                    // table base (low 11 bits zero) | byte offset of the stored slot
                     int ea0, ea1, ea2, eb0, eb1, eb2;
-                    asm volatile("ld.shared.b32 %0, [%1];" : "=r"(ea0) : "r"(((qa0 >> 21) & 0x7FCu) ^ ta));
-                    asm volatile("ld.shared.b32 %0, [%1];" : "=r"(eb0) : "r"(((qb0 >> 21) & 0x7FCu) ^ tb));
-                    asm volatile("ld.shared.b32 %0, [%1];" : "=r"(ea1) : "r"(((qa1 >> 21) & 0x7FCu) ^ ta));
-                    asm volatile("ld.shared.b32 %0, [%1];" : "=r"(eb1) : "r"(((qb1 >> 21) & 0x7FCu) ^ tb));
-                    asm volatile("ld.shared.b32 %0, [%1];" : "=r"(ea2) : "r"(((qa2 >> 21) & 0x7FCu) ^ ta));
-                    asm volatile("ld.shared.b32 %0, [%1];" : "=r"(eb2) : "r"(((qb2 >> 21) & 0x7FCu) ^ tb));
-                    acc0 += ea0 + eb0;
-                    acc1 += ea1 + eb1;
-                    acc2 += ea2 + eb2;
+                    asm volatile("ld.shared.b32 %0, [%1];" : "=r"(ea0) : "r"(((a0 >> 21) & 0x7FCu) | ta));
+                    asm volatile("ld.shared.b32 %0, [%1+2048];" : "=r"(eb0) : "r"(((b0 >> 21) & 0x7FCu) | ta));
+                    asm volatile("ld.shared.b32 %0, [%1];" : "=r"(ea1) : "r"(((a1 >> 21) & 0x7FCu) | ta));
+                    asm volatile("ld.shared.b32 %0, [%1+2048];" : "=r"(eb1) : "r"(((b1 >> 21) & 0x7FCu) | ta));
+                    asm volatile("ld.shared.b32 %0, [%1];" : "=r"(ea2) : "r"(((a2 >> 21) & 0x7FCu) | ta));
+                    asm volatile("ld.shared.b32 %0, [%1+2048];" : "=r"(eb2) : "r"(((b2 >> 21) & 0x7FCu) | ta));
+                    all0 += ea0 + eb0;
+                    all1 += ea1 + eb1;
+                    all2 += ea2 + eb2;
+                    add_if(neg0, wa.x, sbit, ea0);
+                    add_if(neg0, wb.x, sbit, eb0);
+                    add_if(neg1, wa.y, sbit, ea1);
+                    add_if(neg1, wb.y, sbit, eb1);
+                    add_if(neg2, wa.z, sbit, ea2);
+                    add_if(neg2, wb.z, sbit, eb2);
                     // fast_risky(p) <=> (~p) << 9 < kBandFast << 9 <=> p << 9 > 0xFFFFFE00 - (kBandFast << 9): the largest
-                    // fraction below an index boundary over all channels and samples (the sign bit shifts out)
-                    dmax = __vimax3_u32(dmax, qa0 << 9, qb0 << 9);
-                    dmax = __vimax3_u32(dmax, qa1 << 9, qb1 << 9);
-                    dmax = __vimax3_u32(dmax, qa2 << 9, qb2 << 9);
+                    // fraction below an index boundary over all channels and samples
+                    dmax = __vimax3_u32(dmax, a0 << 9, b0 << 9);
+                    dmax = __vimax3_u32(dmax, a1 << 9, b1 << 9);
+                    dmax = __vimax3_u32(dmax, a2 << 9, b2 << 9);
                 }
+                int accs[3] = {(int) ((uint32_t) all0 - 2u * (uint32_t) neg0), (int) ((uint32_t) all1 - 2u * (uint32_t) neg1),
+                               (int) ((uint32_t) all2 - 2u * (uint32_t) neg2)};
                 if (__any_sync(kFull, dmax > 0xFFFFFE00u - (lanes::kBandFast << 9))) {
                     // ---- repair: some sample of this window sits within 2^-25 cycles below an index boundary for some
                     // channel. Find the channel(s), take the certain index of exactly those (channel, sample) pairs (64-bit
@@ -196,7 +213,7 @@ __global__ void __launch_bounds__(kLaneWarps * 32, 2) k_synth_lanes(SynthArgs a)
                     for (int c = 0; c < nchan; c++) {
                         const uint4 wv = *reinterpret_cast<const uint4 *>(&wrow[c]);
                         const uint32_t st = sm.step[warp][c];
-                        const uint32_t p0 = wv.w + lane3 * st, p1 = p0 + st, p2 = p1 + st;
+                        const uint32_t p0 = wv.w + n0 * st, p1 = wv.w + n1 * st, p2 = wv.w + n2 * st;
                         const bool risky = lanes::fast_risky(p0) | lanes::fast_risky(p1) | lanes::fast_risky(p2);
                         if (!__any_sync(kFull, risky)) continue;
                         const int src = hh * CH + c;
@@ -205,28 +222,23 @@ __global__ void __launch_bounds__(kLaneWarps * 32, 2) k_synth_lanes(SynthArgs a)
                         const RunCkpt k0 = a.ck[((size_t) b * a.nruns + r) * nchan + c];
                         const lanes::Anchor ac = {k0.x, k0.y, bc[c].c_carr, bc[c].c_code, k0.nav};
                         const uint32_t ps[3] = {p0, p1, p2}, sw[3] = {wv.x, wv.y, wv.z};
-                        int fix[3] = {0, 0, 0};
 #pragma unroll
-                        for (int rr = 0; rr < 3; rr++) {
-                            if (!lanes::fast_risky(ps[rr])) continue;
-                            const int kf = (int) (ps[rr] >> 23);
-                            const int k = lanes::exact_index(Pc, Dc, ac, w + hh, (int) lane3 + rr);
-                            const int flip = (int) ((sw[rr] >> lane) & 1u) << 8;
-                            fix[rr] = tab[c * 512 + ((k ^ flip) ^ (c * SWZ))] - tab[c * 512 + ((kf ^ flip) ^ (c * SWZ))];
+                        for (int j = 0; j < 3; j++) {
+                            if (!lanes::fast_risky(ps[j])) continue;
+                            const int kf = (int) (ps[j] >> 23);                      // stored slot (rotated)
+                            const int k = lanes::exact_index(Pc, Dc, ac, w + hh, 32 * j + lane);
+                            const int fix = tab[c * 512 + ((k + c * SWZ) & 511)] - tab[c * 512 + kf];
+                            accs[j] += (sw[j] & sbit) ? -fix : fix;
                         }
-                        acc0 += fix[0];
-                        acc1 += fix[1];
-                        acc2 += fix[2];
                     }
                 }
                 // ---- quantise + pack (gps.c:2833-2845) ---------------------------------------------------------------
-                const int accs[3] = {acc0, acc1, acc2};
 #pragma unroll
-                for (int rr = 0; rr < 3; rr++) {
-                    const int p = accs[rr];
+                for (int j = 0; j < 3; j++) {
+                    const int p = accs[j];
                     const int iv = (int) (short) (p & 0xFFFF);                 // (short) i_acc, gps.c:2834
                     const int qv = (p - iv) >> 16;                             // (short) q_acc, gps.c:2835
-                    const int n = hh * lanes::kWindow + (int) lane3 + rr;
+                    const int n = hh * lanes::kWindow + 32 * j + lane;
                     if (IQ16) {
                         stage[n] = ((uint32_t) iv & 0xFFFFu) | ((uint32_t) qv << 16);
                     } else {

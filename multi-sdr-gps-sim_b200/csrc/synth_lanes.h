@@ -20,7 +20,9 @@
 // residue class r = n mod 3: f_code / f_s = 0.341 chips per sample, so along a residue class the chip index advances
 // by 3 * 0.341 = 1 + delta3 (delta3 = 0.023): sample q of the class sits on chip J + q, plus one more after the single
 // point where the accumulated q * delta3 carries. A class word is therefore two shifted copies of the chip stream
-// spliced at that point.
+// spliced at that point. The lane = sample side runs lane i on samples 32 j + i (j = 0, 1, 2), so that the 32 table
+// look-ups of one instruction fall on 32 consecutive samples; sample_words() regroups the class words into three words,
+// one per 32 samples (see sign_pos).
 #pragma once
 #include <stdint.h>
 
@@ -106,7 +108,8 @@ GPSB_HD uint32_t mulhi32(uint32_t a, uint32_t b) {
 }
 
 // Second opinion on the carry points of a window, in FP64: used when the 32-bit estimate of window_signs() lands within
-// its own error of an integer. c_lo / c_hi: the 64 chip-sign bits from chip j0 on. Returns false when a sample's linear
+// its own error of an integer. c_lo / c_hi: the 64 chip-sign bits from chip j0 on; S: the class words (S[r] bit q:
+// sample 3q + r), which window_signs() regroups. Returns false when a sample's linear
 // code phase is within the band of a chip boundary or a carry point stays ambiguous.
 GPSB_HD bool window_signs_fp64(const ChanRun &s, uint32_t c_lo, uint32_t c_hi, int j0, uint32_t S[3]) {
     const uint64_t d3 = 3 * s.E - kOne54;
@@ -132,7 +135,21 @@ GPSB_HD bool window_signs_fp64(const ChanRun &s, uint32_t c_lo, uint32_t c_hi, i
     return certain;
 }
 
-// The chip-sign words of the current window: S[r] bit q = sign flag (chip XOR data bit) of sample 3q + r.
+// Sign words of a window as the lane = sample side reads them: word j holds the sign flags (chip XOR data bit) of samples
+// 32 j .. 32 j + 31, sample 32 j + i at bit sign_pos(i). The bits are grouped by i mod 3 (three fields of 11, 11 and 10
+// bits) rather than in sample order: a field is then a run of consecutive bits of ONE class word, and regrouping the class
+// words costs a few shifts and masks instead of a 3-way bit interleave. The position depends on the lane only, not on j.
+GPSB_HD int sign_pos(int i) { return 11 * (i % 3) + i / 3; }
+
+// Class words (S[r] bit q: sample 3q + r) -> sign words. Field t of word j starts at sample 32 j + t, which is sample
+// q0 = (32 j + t) / 3 of class (2 j + t) mod 3.
+GPSB_HD void sample_words(const uint32_t S[3], uint32_t W[3]) {
+    W[0] = (S[0] & 0x7FFu) | ((S[1] & 0x7FFu) << 11) | (S[2] << 22);
+    W[1] = ((S[2] >> 10) & 0x7FFu) | (((S[0] >> 11) & 0x7FFu) << 11) | ((S[1] >> 11) << 22);
+    W[2] = (S[1] >> 21) | ((S[2] >> 21) << 11) | ((S[0] >> 22) << 22);
+}
+
+// The sign words of the current window (layout: sign_pos), built from the class words of the construction above.
 // chips(w) = word w of the channel's packed, periodically extended C/A code (bit n = ca[n mod 1023]).
 // Returns false when some sample's linear code phase is too close to a chip boundary (or the carry point of a class is
 // ambiguous): the caller then builds the words with exact_signs().
@@ -143,7 +160,7 @@ GPSB_HD bool window_signs_fp64(const ChanRun &s, uint32_t c_lo, uint32_t c_hi, i
 // mulhi32(2^32 - fr - 3, inv32) = t * 2^25, short by less than 2^-22 (truncations of fr, inv32 and the product); when its
 // fraction keeps 2^-21 away from 0 and 1 the floor is certain and so is the band condition of the carry point (<= 2^-26).
 template <class ChipFn, class NavFn>
-GPSB_HD bool window_signs(const ChanRun &s, ChipFn chips, NavFn nav, uint32_t S[3], bool force_fp64 = false) {
+GPSB_HD bool window_signs(const ChanRun &s, ChipFn chips, NavFn nav, uint32_t W[3], bool force_fp64 = false) {
     const int j0 = (int) (s.Y >> 54);
     // 64 chips from chip j0 on, data bit folded in; chips of the NEXT code period (position >= 1023 - j0) take the
     // next NAV bit when this period is the 20th of its bit (gps.c:2793-2812)
@@ -173,6 +190,7 @@ GPSB_HD bool window_signs(const ChanRun &s, ChipFn chips, NavFn nav, uint32_t S[
     const uint32_t f0 = (uint32_t) (s.Y >> 22);
     const uint32_t sh1 = funnel_r(c_lo, c_hi, 1), sh2 = funnel_r(c_lo, c_hi, 2);
     bool certain = !force_fp64;
+    uint32_t S[3];
 #pragma unroll
     for (int r = 0; r < 3; r++) {
         const uint32_t fr = f0 + (uint32_t) r * s.e22;                        // r e22 < one chip: at most one wrap
@@ -185,8 +203,9 @@ GPSB_HD bool window_signs(const ChanRun &s, ChipFn chips, NavFn nav, uint32_t S[
         const uint32_t a = J ? sh1 : c_lo, b = J ? sh2 : sh1;
         S[r] = (a & lowm) | (b & ~lowm);
     }
-    if (certain) return true;
-    return window_signs_fp64(s, c_lo, c_hi, j0, S);
+    if (!certain && !window_signs_fp64(s, c_lo, c_hi, j0, S)) return false;
+    sample_words(S, W);
+    return true;
 }
 
 // Next window: 96 samples on.
@@ -208,23 +227,22 @@ GPSB_HD void advance_window(ChanRun &s, NavFn nav) {
     }
 }
 
-// Exact chip-sign words of window w of the run (repair path): the reference's own code recurrence, stepped sample by
-// sample from the exact state at the window start (nco_exact.h).
+// Exact sign words of window w of the run (repair path; layout: sign_pos): the reference's own code recurrence, stepped
+// sample by sample from the exact state at the window start (nco_exact.h).
 template <class ChipFn, class NavFn>
-GPSB_HD void exact_signs(const Anchor &an, int w, ChipFn chips, NavFn nav, uint32_t S[3]) {
+GPSB_HD void exact_signs(const Anchor &an, int w, ChipFn chips, NavFn nav, uint32_t W[3]) {
     double y = an.y0;
     int iword = (int) (an.navpos & 0xFF), ibit = (int) ((an.navpos >> 8) & 0xFF), icode = (int) ((an.navpos >> 16) & 0xFF);
     int64_t periods = 0;
     nco_advance<NCO_CODE>(y, an.d, (int64_t) w * kWindow, periods);
     nav_advance(iword, ibit, icode, periods);
     int dbit = nav_bit_at(nav, iword, ibit);
-    S[0] = S[1] = S[2] = 0;
+    W[0] = W[1] = W[2] = 0;
     for (int n = 0; n < kWindow; n++) {
         const int j = (int) y;                                              // gps.c:2817
         const uint32_t chip = (chips(j >> 5) >> (j & 31)) & 1u;
         const uint32_t flag = chip ^ (uint32_t) dbit;
-        const int q = n / 3, r = n - 3 * q;
-        S[r] |= flag << q;
+        W[n >> 5] |= flag << sign_pos(n & 31);
         int64_t p = 0;
         nco_step<NCO_CODE>(y, an.d, p);
         if (p) {
