@@ -206,6 +206,14 @@ int gpsb200_debug_corrupt_chain(gpsb200_ctx_t *ctx, int on);
  * work to complete. */
 int gpsb200_debug_run_checkpoints(gpsb200_ctx_t *ctx, int nblk, int nchan, void *out);
 
+/* Test hook: copy the carrier block probes of the previous synth call of more than two blocks to host memory:
+ * probes_out gets nblk x nchan records of 64 bytes (the layout gpsb200_carrier_probe_host writes), seg_out (NULL: not
+ * wanted) nblk x nchan x 14 doubles, the probes' states at the checkpoint-segment starts as gpsb200_carrier_probe_host
+ * orders them (entries the probe did not record hold whatever the buffer held), guess_out (NULL: not wanted) nblk x
+ * nchan doubles, the guessed start phases the probes walked from. Waits for the context's work to complete. */
+int gpsb200_debug_block_probes(gpsb200_ctx_t *ctx, int nblk, int nchan, void *probes_out, double *seg_out,
+                               double *guess_out);
+
 /* Name of the synthesis kernel a call with nchan channels launches on this context as it stands: "k_synth_lanes"
  * (lane = sample: run length a multiple of 96 up to 2400, every code rate seen so far within 1.0157 .. 1.0302 MHz,
  * GPSB200_LANES != 0) or "k_synth" (lane = channel, no such conditions). Both are bit-exact; for reporting. */
@@ -259,6 +267,16 @@ int gpsb200_span_chain_host(const double *f_carr, int nblk, double start_true, d
  * gpsb200_carrier_advance(start_true, f_carr, j-th segment start) bit for bit), 0 when it rejects it. For tests. */
 int gpsb200_checkpoint_segments_host(double start_true, double start_guess, double f_carr, int run_samples,
                                      double *starts_out, int *nseg_out);
+
+/* Host-only: the carrier block probe the probe kernel computes for a walk of nsamples (< 2^31) from the guessed phase
+ * `guess` at Doppler f_carr. mode 0: each parity variant walked on its own (the reference formulation); mode 1: both
+ * variants in lockstep (what the kernel runs). probe_out: 64 bytes, x_w, x_end[2], m_pos[2], m_neg[2] (doubles), n_w,
+ * pad (int32). seg_out (used when run_samples > 0, which must divide nsamples): 2 x 7 doubles, variant v's state at the
+ * start of checkpoint segment j = 1 .. J - 1 (J = min(8, nsamples / run_samples)) at seg_out[7 v + j - 1]; NaN where
+ * the walk records none (segments before the first wrap or past J - 1, an unusable variant). Both modes write the same
+ * bytes. For tests. */
+int gpsb200_carrier_probe_host(double guess, double f_carr, int64_t nsamples, int run_samples, int mode, void *probe_out,
+                               double *seg_out);
 
 /* Host model of the lane = sample synthesis kernel (csrc/synth_lanes.h) for ONE block: the same window / band / repair
  * logic, executed on the CPU, int16 I/Q out. force bits: 1 = repair every sample's index, 2 = exact chip signs for every

@@ -40,6 +40,11 @@ assert CHAN_DTYPE.itemsize == C.sizeof(Chan) == 64
 RUN_CKPT_DTYPE = np.dtype([("x", "<f8"), ("y", "<f8"), ("nav", "<u4"), ("pad", "<u4")])
 assert RUN_CKPT_DTYPE.itemsize == 24
 
+# one carrier block probe (gpsb200_carrier_probe_host, gpsb200_debug_block_probes)
+CARRIER_PROBE_DTYPE = np.dtype([("x_w", "<f8"), ("x_end", "<f8", 2), ("m_pos", "<f8", 2), ("m_neg", "<f8", 2),
+                                ("n_w", "<i4"), ("pad", "<i4")])
+assert CARRIER_PROBE_DTYPE.itemsize == 64
+
 
 class Config(C.Structure):
     _fields_ = [("device", C.c_int32), ("max_chan", C.c_int32), ("max_blocks", C.c_int32),
@@ -106,6 +111,7 @@ EXPORTS = ["gpsb200_create", "gpsb200_destroy", "gpsb200_last_error", "gpsb200_v
            "gpsb200_codegen", "gpsb200_bind_numa", "gpsb200_span_chain_host", "gpsb200_lanes_model_block", "gpsb200_slice_prepare", "gpsb200_slice_probe",
            "gpsb200_slice_finish", "gpsb200_slice_finish_cb", "gpsb200_slice_wait", "gpsb200_link_apply", "gpsb200_slice_link_host", "gpsb200_debug_corrupt_chain", "gpsb200_synth_kernel_name",
            "gpsb200_debug_run_checkpoints", "gpsb200_checkpoint_segments_host",
+           "gpsb200_carrier_probe_host", "gpsb200_debug_block_probes",
            "gpsb200_scenario_create", "gpsb200_scenario_destroy", "gpsb200_scenario_error",
            "gpsb200_scenario_blocks", "gpsb200_scenario_channels", "gpsb200_scenario_nav_frames",
            "gpsb200_scenario_chans", "gpsb200_scenario_nav", "gpsb200_scenario_almanac_date", "gpsb200_almanac_read",
@@ -178,6 +184,9 @@ def lib():
         L.gpsb200_debug_run_checkpoints.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p]
         L.gpsb200_checkpoint_segments_host.argtypes = [C.c_double, C.c_double, C.c_double, C.c_int, C.c_void_p,
                                                        C.POINTER(C.c_int)]
+        L.gpsb200_carrier_probe_host.argtypes = [C.c_double, C.c_double, C.c_int64, C.c_int, C.c_int, C.c_void_p,
+                                                 C.c_void_p]
+        L.gpsb200_debug_block_probes.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
         L.gpsb200_synth_kernel_name.argtypes = [C.c_void_p, C.c_int]
         L.gpsb200_synth_kernel_name.restype = C.c_char_p
         _lib = L
@@ -259,6 +268,18 @@ def checkpoint_segments_host(start_true, start_guess, f_carr, run_samples=2400):
     if rc < 0:
         raise GpsB200Error(rc, "gpsb200_checkpoint_segments_host")
     return rc == 1, out[:nseg.value]
+
+
+def carrier_probe_host(guess, f_carr, nsamples=BLOCK_SAMPLES, run_samples=2400, mode=1):
+    """Host model of one carrier block probe (mode 0: each parity variant on its own, 1: both in lockstep).
+    -> (probe CARRIER_PROBE_DTYPE scalar record, seg float64[2, 7] with NaN where no state is recorded)"""
+    probe = np.zeros(1, CARRIER_PROBE_DTYPE)
+    seg = np.zeros((2, 7))
+    rc = lib().gpsb200_carrier_probe_host(float(guess), float(f_carr), int(nsamples), int(run_samples), int(mode),
+                                          probe.ctypes.data, seg.ctypes.data)
+    if rc:
+        raise GpsB200Error(rc, "gpsb200_carrier_probe_host")
+    return probe[0], seg
 
 
 def slice_link_host(chans):
@@ -583,6 +604,17 @@ class Context:
         out = np.zeros((nblk, nruns, nchan), RUN_CKPT_DTYPE)
         self._check(lib().gpsb200_debug_run_checkpoints(self._h, nblk, nchan, out.ctypes.data))
         return out
+
+    def debug_block_probes(self, nblk, nchan):
+        """The previous call's carrier block probes -> (CARRIER_PROBE_DTYPE [nblk, nchan], seg float64[nblk, nchan, 2, 7]
+        as carrier_probe_host orders them (entries a probe did not record are undefined), guess float64[nblk, nchan]:
+        the start phases the probes walked from)."""
+        probes = np.zeros((nblk, nchan), CARRIER_PROBE_DTYPE)
+        seg = np.zeros((nblk, nchan, 2, 7))
+        guess = np.zeros((nblk, nchan))
+        self._check(lib().gpsb200_debug_block_probes(self._h, nblk, nchan, probes.ctypes.data, seg.ctypes.data,
+                                                     guess.ctypes.data))
+        return probes, seg, guess
 
     def carrier_chain(self, chans, phase_in=None):
         """Exact carrier phases after all blocks of chans (device probe + host fix-up, no synthesis)."""

@@ -1032,8 +1032,7 @@ int gpsb200_checkpoint_segments_host(double start_true, double start_guess, doub
     const int nruns = GPSB200_BLOCK_SAMPLES / run_samples, nseg = ckpt_segments(nruns);
     CarrierProbe p;
     double seg[kSegStates];
-    for (int v = 0; v < 2; v++)
-        carrier_probe_variant(start_guess, c, GPSB200_BLOCK_SAMPLES, v, p, seg + v * (kCkptSegs - 1), nruns, run_samples);
+    carrier_probe_walk2(start_guess, c, GPSB200_BLOCK_SAMPLES, p, seg, nruns, run_samples);
     if (nseg_out) *nseg_out = nseg;
     starts_out[0] = start_true;
     for (int j = 1; j < kCkptSegs; j++) starts_out[j] = NAN;
@@ -1043,6 +1042,28 @@ int gpsb200_checkpoint_segments_host(double start_true, double start_guess, doub
     for (int j = first_derived_segment(p, nseg, nruns, run_samples); j < nseg; j++)
         starts_out[j] = seg[v * (kCkptSegs - 1) + j - 1] + d;
     return 1;
+}
+
+int gpsb200_carrier_probe_host(double guess, double f_carr, int64_t nsamples, int run_samples, int mode, void *probe_out,
+                               double *seg_out) {
+    if (!probe_out || nsamples < 0 || nsamples >= ((int64_t) 1 << 31) || (mode != 0 && mode != 1) || run_samples < 0 ||
+        (run_samples > 0 && nsamples % run_samples != 0))
+        return GPSB200_ERR_ARG;
+    const double c = f_carr * (1.0 / (double) GPSB200_SAMPLERATE);
+    const int nruns = run_samples > 0 ? (int) (nsamples / run_samples) : 0;
+    double *seg = run_samples > 0 ? seg_out : nullptr;
+    if (seg)                                 // states a walk does not record stay NaN
+        for (int k = 0; k < kSegStates; k++) seg[k] = NAN;
+    CarrierProbe p{};
+    if (mode == 0) {
+        for (int v = 0; v < 2; v++)
+            carrier_probe_walk(guess, c, nsamples, v, p.n_w, p.x_w, p.x_end[v], p.m_pos[v], p.m_neg[v],
+                               seg ? seg + v * (kCkptSegs - 1) : nullptr, nruns, run_samples);
+    } else {
+        carrier_probe_walk2(guess, c, nsamples, p, seg, nruns, run_samples);
+    }
+    memcpy(probe_out, &p, sizeof p);
+    return GPSB200_OK;
 }
 
 int gpsb200_carrier_chain(const gpsb200_chan_t *chans, int nblk, int nchan, const double *phase_in,
@@ -1518,6 +1539,20 @@ int gpsb200_debug_run_checkpoints(gpsb200_ctx_t *ctx, int nblk, int nchan, void 
     CU(cudaSetDevice(ctx->cfg.device));
     CU(cudaDeviceSynchronize());             // the call's streams may be the caller's
     CU(cudaMemcpy(out, ctx->d_ck, (size_t) nblk * ctx->nruns * nchan * sizeof(RunCkpt), cudaMemcpyDeviceToHost));
+    return GPSB200_OK;
+}
+
+int gpsb200_debug_block_probes(gpsb200_ctx_t *ctx, int nblk, int nchan, void *probes_out, double *seg_out,
+                               double *guess_out) {
+    if (!ctx || !probes_out || nblk < 1 || nblk > ctx->cfg.max_blocks || nchan < 1 || nchan > ctx->cfg.max_chan)
+        return GPSB200_ERR_ARG;
+    if (!ctx->s_compute) return fail(ctx, GPSB200_ERR_CUDA, "context has no CUDA device");
+    CU(cudaSetDevice(ctx->cfg.device));
+    CU(cudaDeviceSynchronize());             // the call's streams may be the caller's
+    const size_t cnt = (size_t) nblk * nchan;
+    CU(cudaMemcpy(probes_out, ctx->d_probe, cnt * sizeof(CarrierProbe), cudaMemcpyDeviceToHost));
+    if (seg_out) CU(cudaMemcpy(seg_out, ctx->d_seg, cnt * kSegStates * sizeof(double), cudaMemcpyDeviceToHost));
+    if (guess_out) CU(cudaMemcpy(guess_out, ctx->d_guess, cnt * sizeof(double), cudaMemcpyDeviceToHost));
     return GPSB200_OK;
 }
 

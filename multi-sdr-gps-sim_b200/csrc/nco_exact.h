@@ -355,9 +355,9 @@ constexpr int kSegStates = 2 * (kCkptSegs - 1);        // recorded states per (b
 GPSB_HD int ckpt_segments(int nruns) { return nruns < kCkptSegs ? nruns : kCkptSegs; }
 GPSB_HD int seg_first_run(int j, int nseg, int nruns) { return j * nruns / nseg; }
 
-// One parity variant v of the probe (the device runs the two variants in different threads;
-// each repeats the short walk to the first wrap): n_w/x_w (identical for both v) and the v-th
-// end state and margins of CarrierProbe, as scalars.
+// One parity variant v of the probe, walked on its own: n_w/x_w (identical for both v) and the v-th
+// end state and margins of CarrierProbe, as scalars. The probes themselves come from carrier_probe_walk2()
+// (both variants in lockstep, the same bytes); this is the reference formulation the tests compare it with.
 // seg (optional): variant v's state at the start s_j = seg_first_run(j) * run_samples of every interior checkpoint
 // segment j = 1 .. J-1 goes to seg[j-1], for s_j >= n_w (the others are not written). The walk stops at each s_j,
 // which only shortens a jump: the states, margins and end state are the same as without.
@@ -398,16 +398,141 @@ GPSB_HD void carrier_probe_walk(double guess, double c, int64_t n, int v, int32_
     m_neg = mn;
 }
 
-GPSB_HD void carrier_probe_variant(double guess, double c, int64_t n, int v, CarrierProbe &o, double *seg = nullptr,
-                                   int nruns = 0, int run_samples = 0) {
-    o.pad = 0;
-    carrier_probe_walk(guess, c, n, v, o.n_w, o.x_w, o.x_end[v], o.m_pos[v], o.m_neg[v], seg, nruns, run_samples);
+// Both parity variants in lockstep: one iteration of the schedule of walk_iteration<NCO_CARRIER> for the two states
+// x[0], x[1] at the same step count, for an increment of sign NEG. The jump k = min(k_0, k_1) is the smaller of the
+// two variants' own jumps (zero when they are in different binades or either one is `special`, which walk_iteration
+// evaluates per state), so it stays strictly inside both binades and each trajectory is exactly the one its own walk
+// visits; then each variant does one real step. The binade quantities (lo, the in-binade step, the tie test, the
+// room) are computed once for both. e_tie: the one binade whose grid puts |c| on an exact tie (tie_binade()).
+// Margins: inside one binade visit the trajectory is monotone, so its smallest distance to the edge it walks away from
+// is at its first state -- the start of the walk or the state after a real step, i.e. the state an iteration starts
+// from -- and its smallest distance to the edge it walks towards at its last -- the state a real step starts from,
+// i.e. an after-jump state, or the end of the walk (folded by the caller). Each state folds just that one of the two
+// distances; the minima are those carrier_walk_w() folds from every visited state. (States after a first wrap are 0
+// or at least 2^-75 -- multiples of 2^-75 -- so the branch-free distances equal binade_margins()'.)
+template <bool NEG>
+GPSB_HD void walk_iteration2(double *x, const WalkConst &w, int e_tie, double &nd, double *mp, double *mn) {
+    const uint64_t b0 = f64_bits(x[0]), b1 = f64_bits(x[1]);
+    const int ex = (int) ((b0 >> 52) & 0x7FF);
+    const double lo[2] = {bits_f64((uint64_t) ex << 52), bits_f64(b1 & 0x7FF0000000000000ull)};
+    for (int v = 0; v < 2; v++) {                       // first state of a visit: the edge walked away from
+        if (NEG) {
+            const double up = (lo[v] + lo[v]) - x[v];
+            if (up < mp[v]) mp[v] = up;
+        } else {
+            const double dn = x[v] - lo[v];
+            if (dn < mn[v]) mn[v] = dn;
+        }
+    }
+    bool special = ((b0 ^ b1) >> 52) != 0 || !(x[0] >= w.ac) || !(x[1] >= w.ac);
+    special |= (ex == e_tie) & (((b0 | b1) & 1) != 0);  // an odd mantissa in the tie binade
+    double stepd = (lo[0] + w.ac) - lo[0];              // |c| rounded to the grid of [2^e, 2^(e+1))
+    if (ex == w.ec) stepd = w.ac;                       // own binade of c: steps are exact
+    // the variant nearer the edge walked towards has the smaller room (the rounding of the subtraction is monotone)
+    const double room = NEG ? (x[0] < x[1] ? x[0] : x[1]) - lo[0]
+                            : bits_f64(((uint64_t) (ex + 1) << 52) - 1) - (x[0] > x[1] ? x[0] : x[1]);
+    double kq = room * w.rinv;
+    if (kq > nd) kq = nd;
+    if (special) kq = 0.0;
+    const double k = floor_nonneg(kq);
+    const double adv = k * stepd;                       // exact: k*R < 2^53
+    nd -= k;
+    for (int v = 0; v < 2; v++) {
+        x[v] = NEG ? x[v] - adv : x[v] + adv;           // exact
+        if (NEG) {                                      // last state of a visit: the edge walked towards
+            const double dn = x[v] - lo[v];
+            if (dn < mn[v]) mn[v] = dn;
+        } else {
+            const double up = (lo[v] + lo[v]) - x[v];
+            if (up < mp[v]) mp[v] = up;
+        }
+    }
+    if (nd > 0.0) {                                     // the real step (nco_step<NCO_CARRIER> for this sign of c)
+        for (int v = 0; v < 2; v++) {
+#if defined(__CUDA_ARCH__)
+            x[v] = __dadd_rn(x[v], w.c);
+#else
+            x[v] = x[v] + w.c;
+#endif
+            if (!NEG) {
+                if (x[v] >= 1.0) x[v] -= 1.0;
+            } else if (x[v] < 0.0) {
+                x[v] += 1.0;
+                if (x[v] >= 1.0) x[v] = kBelowOne;
+            }
+        }
+        nd -= 1.0;
+    }
 }
 
-GPSB_HD void carrier_probe(double guess, double c, int64_t n, CarrierProbe &o) {
-    carrier_probe_variant(guess, c, n, 0, o);
-    carrier_probe_variant(guess, c, n, 1, o);
+// The binade exponent e_tie in whose grid |c| (fast range) lies exactly half-way between two neighbours: ulp/2 there
+// equals the lowest set bit of |c|. walk_iteration's tie test is true in that binade only.
+GPSB_HD int tie_binade(const WalkConst &w) {
+    const uint64_t m = (f64_bits(w.ac) & ((1ull << 52) - 1)) | (1ull << 52);
+    int tz = 0;
+    while (!((m >> tz) & 1)) tz++;
+    return w.ec + 1 + tz;
 }
+
+// n steps of both variants (carrier_walk_w() without stop at a wrap, for each of them), folding their margins
+template <bool NEG>
+GPSB_HD void carrier_walk2(double *x, const WalkConst &w, int e_tie, int64_t n, double *mp, double *mn) {
+    if (n <= 0) return;
+    for (int v = 0; v < 2; v++) binade_margins(x[v], mp[v], mn[v]);
+    double nd = (double) n;
+    while (nd > 0.0) walk_iteration2<NEG>(x, w, e_tie, nd, mp, mn);
+    for (int v = 0; v < 2; v++) binade_margins(x[v], mp[v], mn[v]);     // the end: maybe a visit's last state
+}
+
+// carrier_probe_walk() for v = 0 and v = 1 at once: the walk to the first wrap is done once, then x_w and x_w + G
+// are walked in lockstep (walk_iteration2) through the segment starts to the end of the block. Writes exactly what the
+// two carrier_probe_walk() calls write: the state after n steps does not depend on how the steps are grouped into
+// jumps, and the margins come from the first and last state of every binade visit, which both schedules visit.
+// seg (optional): variant v's segment states go to seg[v * (kCkptSegs - 1) + j - 1], as carrier_probe_walk() has them.
+GPSB_HD void carrier_probe_walk2(double guess, double c, int64_t n, CarrierProbe &o, double *seg = nullptr,
+                                 int nruns = 0, int run_samples = 0) {
+    const WalkConst w = walk_const(c);
+    double x = guess;
+    bool wrapped = false, ok = true;
+    const int64_t nw = carrier_walk_w(x, w, n, true, wrapped, ok, nullptr, nullptr);
+    o.x_w = x;
+    o.pad = 0;
+    if (!wrapped || !ok) {
+        o.n_w = -1;
+        o.x_end[0] = o.x_end[1] = x;
+        o.m_pos[0] = o.m_pos[1] = o.m_neg[0] = o.m_neg[1] = 0.0;
+        return;
+    }
+    o.n_w = (int32_t) nw;
+    const double xv[2] = {x + 0.0, x + carrier_grid(c)};     // exact: x_w is a multiple of G
+    // a parity partner that left [0,1) (x_w at the very edge) is simply unusable: it is not walked, and follows the
+    // other variant through the loop, its results discarded
+    const bool live[2] = {xv[0] >= 0.0 && xv[0] < 1.0, xv[1] >= 0.0 && xv[1] < 1.0};
+    double xs[2] = {live[0] ? xv[0] : xv[1], live[1] ? xv[1] : xv[0]};
+    double mp[2] = {1.0, 1.0}, mn[2] = {1.0, 1.0};
+    if (live[0] || live[1]) {
+        const int e_tie = tie_binade(w);
+        int64_t pos = nw;
+        const int nseg = seg ? ckpt_segments(nruns) : 1;
+        for (int j = 1; j <= nseg; j++) {               // to every segment start, then to the end of the block
+            const int64_t s = j < nseg ? seg_first_run(j, nseg, nruns) * run_samples : n;
+            if (s < pos) continue;                      // before the first wrap: not derivable
+            if (w.neg) carrier_walk2<true>(xs, w, e_tie, s - pos, mp, mn);
+            else carrier_walk2<false>(xs, w, e_tie, s - pos, mp, mn);
+            pos = s;
+            if (j < nseg)
+                for (int v = 0; v < 2; v++)
+                    if (live[v]) seg[v * (kCkptSegs - 1) + j - 1] = xs[v];
+        }
+    }
+    for (int v = 0; v < 2; v++) {
+        o.x_end[v] = live[v] ? xs[v] : xv[v];
+        o.m_pos[v] = live[v] ? mp[v] : 0.0;
+        o.m_neg[v] = live[v] ? mn[v] : 0.0;
+    }
+}
+
+GPSB_HD void carrier_probe(double guess, double c, int64_t n, CarrierProbe &o) { carrier_probe_walk2(guess, c, n, o); }
 
 // Exact end-of-block carrier phase from the true start s and the probe of a guessed start.
 // Returns false when the speculation cannot be used (caller then runs nco_advance).

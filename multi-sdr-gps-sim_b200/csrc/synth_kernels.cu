@@ -6,11 +6,12 @@
 // Work decomposition
 //   block  = 0.1 s = 300000 samples (the reference's unit, sdr.h:26)
 //   run    = run_samples consecutive samples of one block (default 2400)
-//   k_probe       : two threads per (block, channel) walk the carrier NCO through the
-//                   block from a GUESSED start phase (speculative, parallel in time) and
-//                   record its state at the checkpoint-segment starts; the host turns the
-//                   probes into exact start phases (nco_exact.h). A third thread walks the
-//                   code NCO (+ NAV position) and stores it at every run start.
+//   k_probe       : one thread per (block, channel) walks the carrier NCO through the
+//                   block from a GUESSED start phase (speculative, parallel in time), both
+//                   parity variants in lockstep, and records their states at the
+//                   checkpoint-segment starts; the host turns the probes into exact start
+//                   phases (nco_exact.h). A second thread walks the code NCO (+ NAV
+//                   position) and stores it at every run start.
 //   k_tables      : one thread per (block, carrier-table row < 256, lane column): the gain-scaled
 //                   carrier table of every block, written once to HBM; k_synth's CTAs (several
 //                   per block) fetch it with one TMA bulk copy each instead of recomputing it.
@@ -108,42 +109,29 @@ __device__ __forceinline__ void code_walk(const SynthArgs &a, int b, int c) {
 }
 
 __global__ void __launch_bounds__(128) k_probe(SynthArgs a) {
-    // roles 0, 1: one thread per (block, channel) and parity variant v = role (nco_exact.h); role 2 (a.ck set): one
-    // thread per (block, channel) walks the code NCO -- in the shadow of the longer carrier walks, which come first in
-    // the grid. A warp is 32 consecutive blocks of one channel.
+    // role 0: one thread per (block, channel) walks both parity variants of the carrier probe in lockstep
+    // (nco_exact.h: carrier_probe_walk2); role 1 (a.ck set): one thread per (block, channel) walks the code NCO, after
+    // the longer carrier walks in the grid (when not every warp of the call is resident, the code walks that wait for
+    // a free slot are the kernel's tail: DESIGN.md §5). A warp is 32 consecutive blocks of one channel.
     const int nblk_pad = (a.nblk + 31) & ~31;
-    const int per_v = nblk_pad * a.nchan;
+    const int per_role = nblk_pad * a.nchan;
     int idx = blockIdx.x * blockDim.x + threadIdx.x;
-    const int v = idx / per_v;
-    idx -= v * per_v;
+    const int role = idx / per_role;
+    idx -= role * per_role;
     int b, c;
-    if (v > 2 || !map_block_chan(a, idx, b, c)) return;
-    if (v == 2) {
+    if (role > 1 || !map_block_chan(a, idx, b, c)) return;
+    if (role == 1) {
         if (a.ck) code_walk(a, b, c);
         return;
     }
     const size_t i = (size_t) b * a.nchan + c;
     const BlockChanDev p = a.bc[i];
-    int32_t n_w = -1;
-    double x_w = 0.0, x_end = 0.0, m_pos = 0.0, m_neg = 0.0;
+    CarrierProbe pr{0.0, {0.0, 0.0}, {0.0, 0.0}, {0.0, 0.0}, -1, 0};
     if (p.prn > 0)
-        carrier_probe_walk(a.guess[i], p.c_carr, kBlockSamples, v, n_w, x_w, x_end, m_pos, m_neg,
-                           a.seg + i * kSegStates + v * (kCkptSegs - 1), a.nruns, a.run_samples);
+        carrier_probe_walk2(a.guess[i], p.c_carr, kBlockSamples, pr, a.seg + i * kSegStates, a.nruns, a.run_samples);
     // two copies: HBM for k_chain, mapped host memory for the host's (rare) block-by-block fallback
-    CarrierProbe *dsts[2] = {a.probe + i, a.probe_host ? a.probe_host + i : nullptr};
-#pragma unroll
-    for (int k = 0; k < 2; k++) {
-        CarrierProbe *dst = dsts[k];
-        if (!dst) continue;
-        if (v == 0) {
-            dst->x_w = x_w;
-            dst->n_w = n_w;
-            dst->pad = 0;
-        }
-        dst->x_end[v] = x_end;
-        dst->m_pos[v] = m_pos;
-        dst->m_neg[v] = m_neg;
-    }
+    a.probe[i] = pr;
+    if (a.probe_host) a.probe_host[i] = pr;
 }
 
 struct ColumnParams {
@@ -562,7 +550,7 @@ cudaError_t launch_checkpoints(const SynthArgs &a, cudaStream_t s) {
 
 cudaError_t launch_probe(const SynthArgs &a, cudaStream_t s) {
     const int nblk_pad = (a.nblk + 31) & ~31;
-    const long total = (a.ck ? 3L : 2L) * nblk_pad * a.nchan;
+    const long total = (a.ck ? 2L : 1L) * nblk_pad * a.nchan;
     const int threads = 128;
     k_probe<<<(unsigned) ((total + threads - 1) / threads), threads, 0, s>>>(a);
     return cudaGetLastError();
