@@ -160,8 +160,8 @@ int gpsb200_synth_blocks_device(gpsb200_ctx_t *ctx, const gpsb200_chan_t *chans,
  *                             (GPSB200_ERR_INTERNAL: the output must not be used).
  * A slot continues the incoming phase only when it still holds the same satellite (prn_in[c] == prn of its first
  * block, > 0); otherwise its first block takes carr_phase from chans, exactly as between the blocks of one call.
- * chans must stay valid until gpsb200_slice_prepare returns. gpsb200_synth_blocks_device == the three steps with
- * NULL incoming states. */
+ * chans must stay valid until gpsb200_slice_prepare returns. gpsb200_synth_blocks_device gives the same result as the
+ * three steps with NULL incoming states; the one-call path schedules its segments as DESIGN §6 describes. */
 typedef struct gpsb200_slice_link {
     int32_t prn_first[GPSB200_MAX_CHAN];    /* satellite of each slot in the slice's first block (0: idle) */
     int32_t prn_last[GPSB200_MAX_CHAN];     /* ... in its last block */

@@ -137,6 +137,8 @@ def lib():
         L.gpsb200_set_nav.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p]
         L.gpsb200_synth_blocks.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p,
                                            C.c_void_p, C.POINTER(Stats)]
+        L.gpsb200_synth_blocks_scatter.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p,
+                                                   C.c_void_p, C.POINTER(Stats)]
         L.gpsb200_synth_blocks_device.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p,
                                                   C.c_void_p, C.c_void_p, C.POINTER(Stats)]
         L.gpsb200_replay_device.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]
@@ -538,6 +540,20 @@ class Context:
         self._check(lib().gpsb200_synth_blocks(self._h, a.ctypes.data, nblk, nchan, sample_size,
                                                out.ctypes.data, cp.ctypes.data, C.byref(st)))
         return (out, cp, st) if want_stats else (out, cp)
+
+    def synth_blocks_scatter(self, chans, sample_size, blocks, want_stats=False):
+        """Host-destination path, block b into its own host buffer blocks[b] (BLOCK_ELEMS elements).
+        Returns carr_phase_out[, Stats]."""
+        a = self._chans(chans)
+        nblk, nchan = a.shape
+        dt = np.int16 if sample_size == SC16 else np.int8
+        assert len(blocks) == nblk and all(b.dtype == dt and b.size >= BLOCK_ELEMS and b.flags.c_contiguous for b in blocks)
+        ptrs = (C.c_void_p * nblk)(*[b.ctypes.data for b in blocks])
+        cp = np.zeros(nchan, np.float64)
+        st = Stats()
+        self._check(lib().gpsb200_synth_blocks_scatter(self._h, a.ctypes.data, nblk, nchan, sample_size,
+                                                       C.cast(ptrs, C.c_void_p), cp.ctypes.data, C.byref(st)))
+        return (cp, st) if want_stats else cp
 
     def synth_blocks_device(self, chans, sample_size, dst_ptr, stream=0, want_stats=False):
         """Device-destination path: dst_ptr is a raw device pointer (e.g. torch tensor .data_ptr())."""

@@ -117,13 +117,60 @@ private:
     bool stop_ = false;
 };
 
+// Pipeline segments of a call: a short first one (its chain resolution is the lead-in of everything), then long ones.
+std::vector<std::pair<int, int>> segments_of(int nblk) {
+    std::vector<std::pair<int, int>> v;
+    int len = kSegFirst;
+    for (int b0 = 0; b0 < nblk; len = kSegBlocks) {
+        const int b1 = std::min(nblk, b0 + len);
+        v.emplace_back(b0, b1);
+        b0 = b1;
+    }
+    return v;
+}
+
+// One synthesis call: what its steps (call_open, seg_params, seg_probe, seg_scan, seg_commit, call_close) share.
+struct Call {
+    const gpsb200_chan_t *chans = nullptr;      // the caller's records; read by seg_params only
+    int nblk = 0, nchan = 0, sample_size = 0;
+    void *dst = nullptr;                        // device destination (NULL: the carrier chain only, no synthesis)
+    void *dst_host = nullptr;                   // host destination: one contiguous buffer ...
+    void *const *scatter = nullptr;             // ... or one buffer per block
+    cudaStream_t stream = nullptr;              // the caller's stream: synthesis
+    std::vector<std::pair<int, int>> segs;      // pipeline segments
+    std::vector<ChainState> chain;              // exact chain state after the blocks scanned so far
+    std::vector<std::vector<ChainState>> after; // ... after each scanned segment
+    std::vector<int64_t> slow;                  // spans of each segment the host scan resolved block by block
+    int rows = 0;                               // rows of h_seg_end the committed ranges filled
+    int ichunk = 0;                             // next entry of ev_done
+    gpsb200_stats_t st{};
+    bool active = false, eager = false, probed = false, finished = false;   // slice calls
+
+    Call() = default;
+    Call(const gpsb200_chan_t *chans_, int nblk_, int nchan_, int sample_size_, void *dst_, void *dst_host_,
+         void *const *scatter_, cudaStream_t stream_)
+        : chans(chans_), nblk(nblk_), nchan(nchan_), sample_size(sample_size_), dst(dst_), dst_host(dst_host_),
+          scatter(scatter_), stream(stream_), chain(nchan_) {
+        plan(segments_of(nblk_));
+    }
+    void plan(std::vector<std::pair<int, int>> s) {
+        segs = std::move(s);
+        after.assign(segs.size(), {});
+        slow.assign(segs.size(), 0);
+    }
+    bool host() const { return dst_host || scatter; }
+};
+
+// Events a call records for its stats (the first segment's probe and checkpoint launches, the caller's stream).
+enum { kEvCallStart, kEvProbeStart, kEvProbeEnd, kEvCkptStart, kEvCkptEnd, kEvCallEnd, kCallEvents };
+
 }  // namespace
 
 struct gpsb200_ctx {
     gpsb200_config_t cfg{};
     int nruns = 0;
     cudaStream_t s_compute = nullptr, s_copy = nullptr, s_pre = nullptr, s_ck = nullptr;
-    cudaEvent_t ev[8]{};
+    cudaEvent_t ev[kCallEvents]{};
     std::vector<cudaEvent_t> ev_done;      // one per synthesis chunk
     BlockChanDev *d_bc = nullptr, *h_bc = nullptr;
     RunCkpt *d_ck = nullptr, *h_ck = nullptr;          // h_ck: run checkpoints of small calls, computed on the host
@@ -144,25 +191,14 @@ struct gpsb200_ctx {
     bool lanes_on = true;                              // GPSB200_LANES=0: always k_synth (lane = channel)
     bool lanes_veto = false;                           // a channel record outside k_synth_lanes' range was seen
     SpanRes *d_span_res = nullptr, *h_span_res = nullptr;
-    int max_spans = 0, max_segs = 0;
+    int max_spans = 0;
     double *h_seg_end = nullptr, *d_seg_end = nullptr;   // mapped: device-walked end phases of every pipeline segment's last block
-    int cur_seg = 0;                       // which row of h_seg_end the next checkpoint launch fills
     std::vector<double> seg_expect;        // what the chain says they must be
-    std::vector<cudaEvent_t> ev_seg;       // slice path: probes of segment i complete
-    void *const *scatter = nullptr;        // gpsb200_synth_blocks_scatter: one host destination per block
+    std::vector<cudaEvent_t> ev_seg;       // probes of segment i complete
     int fault_inject_chain = 0;            // gpsb200_debug_corrupt_chain(): 1 = resolution, 2 = segment state
     bool trace_on = false;
-    double trace_t0 = 0.0;       // gpsb200_debug_corrupt_chain(): test hook of the device self-check
-    // state of a begun, not yet finished call (gpsb200_synth_begin / _finish)
-    struct Pending {
-        bool active = false;
-        int nblk = 0, nchan = 0, sample_size = 0;
-        void *dst = nullptr, *dst_host = nullptr;
-        cudaStream_t stream = nullptr;
-        bool probed = false, finished = false, eager = false;
-        int nseg = 0;
-        gpsb200_stats_t st{};
-    } pending;
+    double trace_t0 = 0.0;
+    Call call;                             // a slice call begun with gpsb200_slice_prepare (active until finished)
     void *d_out = nullptr;
     size_t out_bytes = 0;
     bool nav_dirty = true;
@@ -210,15 +246,24 @@ void trace(gpsb200_ctx *ctx, const char *what) {
             ctx->pool ? ctx->pool->size() : 0);
 }
 
-// Host pre-pass: validate, fill the device-layout records and GUESS every block's start
-// carrier phase (closed form + expected rounding drift, long double accumulation).
-// Phases as 64-bit fixed point (cycles * 2^64, modulo one cycle) for the closed-form guesses.
+// The closed-form carrier-phase guess (the phase predicted for the end of a run of blocks) of prepare_blocks,
+// gpsb200_slice_link_host and gpsb200_span_chain_host: phases as 64-bit fixed point (cycles * 2^64, modulo 2^64 =
+// modulo one cycle: exact integer arithmetic), truncated to a double when read.
 inline uint64_t phase_to_fix(double p) { return (p >= 0.0 && p < 1.0) ? (uint64_t) (p * 0x1p64) : 0; }
 inline double fix_to_phase(uint64_t a) { return (double) (a >> 11) * 0x1p-53; }
 inline uint64_t step_to_fix(double c) {     // c in (-1, 1): c * 2^64 modulo 2^64 (exact for |c| >= 2^-12, else truncated)
     const uint64_t m = (uint64_t) (std::fabs(c) * 0x1p64);
     return c < 0.0 ? (uint64_t) 0 - m : m;
 }
+// One block: 300000 steps of c, plus the expected rounding drift of those steps. (The drift of a block is up to +-8e-12
+// cycles and depends on the low bits of c, i.e. it is uncorrelated from block to block: evaluating it for every 4th
+// block only was tried and made 50x more probes miss.)
+inline uint64_t guess_block(uint64_t acc, double c) {
+    acc += (uint64_t) GPSB200_BLOCK_SAMPLES * step_to_fix(c);
+    return acc + (uint64_t) (int64_t) ((double) GPSB200_BLOCK_SAMPLES * carrier_drift_per_step(c) * 0x1p64);
+}
+
+// Host pre-pass: validate, fill the device-layout records and GUESS every block's start carrier phase.
 
 // With link != NULL (time-slice hand-over, gpsb200_slice_prepare) the incoming chain state is not known yet:
 // guesses are accumulated RELATIVE to it (h_guess holds the advance since the slice start, h_guess_abs marks
@@ -298,11 +343,7 @@ int prepare_blocks(gpsb200_ctx *ctx, const gpsb200_chan_t *chans, int b0, int b1
                 o.nav0 = (uint32_t) in.iword | ((uint32_t) in.ibit << 8) | ((uint32_t) in.icode << 16);
                 o.frame = in.nav_frame;
                 ctx->h_guess[i] = fix_to_phase(acc);
-                // one block: 300000 steps of c, plus the expected rounding drift of those steps. (The drift of a block is
-                // up to +-8e-12 cycles and depends on the low bits of c, i.e. it is uncorrelated from block to block:
-                // evaluating it for every 4th block only was tried and made 50x more probes miss.)
-                acc += (uint64_t) GPSB200_BLOCK_SAMPLES * step_to_fix(o.c_carr);
-                acc += (uint64_t) (int64_t) ((double) GPSB200_BLOCK_SAMPLES * carrier_drift_per_step(o.c_carr) * 0x1p64);
+                acc = guess_block(acc, o.c_carr);
             }
             if (end_guess) {
                 (*end_guess)[c].prn = prev_prn > 0 ? prev_prn : 0;
@@ -463,8 +504,9 @@ int64_t resolve_chain(gpsb200_ctx *ctx, int b0, int b1, int nchan, std::vector<C
     return n;
 }
 
-void fill_args(gpsb200_ctx *ctx, SynthArgs &a, int blk0, int nblk, int nchan, int sample_size, void *out) {
+SynthArgs make_args(gpsb200_ctx *ctx, int blk0, int nblk, int nchan, int sample_size, void *out) {
     // blk0 is a multiple of kSpanBlocks whenever the chain kernels are launched with these arguments
+    SynthArgs a{};
     const size_t off = (size_t) blk0 * nchan;
     a.bc = ctx->d_bc + off;
     a.carr0 = ctx->d_carr0 + off;
@@ -499,6 +541,13 @@ void fill_args(gpsb200_ctx *ctx, SynthArgs &a, int blk0, int nblk, int nchan, in
     per_cta = (ctx->nruns + ctas - 1) / ctas;
     a.runs_per_cta = per_cta;
     a.ctas_per_block = ctas;
+    return a;
+}
+
+// Arguments of a call's kernels over blocks [b0, b0 + nb), synthesizing into the call's device destination.
+SynthArgs call_args(gpsb200_ctx *ctx, const Call &call, int b0, int nb) {
+    const size_t blk_bytes = (size_t) GPSB200_BLOCK_ELEMS * call.sample_size;
+    return make_args(ctx, b0, nb, call.nchan, call.sample_size, (char *) call.dst + (size_t) b0 * blk_bytes);
 }
 
 int upload_nav(gpsb200_ctx *ctx, cudaStream_t s) {
@@ -510,12 +559,11 @@ int upload_nav(gpsb200_ctx *ctx, cudaStream_t s) {
 }
 
 int check_call(gpsb200_ctx *ctx, const gpsb200_chan_t *chans, int nblk, int nchan, int sample_size, void *dst) {
-    if (!ctx) return GPSB200_ERR_ARG;
     if (!chans || !dst || nblk < 1 || nblk > ctx->cfg.max_blocks || nchan < 1 || nchan > ctx->cfg.max_chan ||
         (sample_size != GPSB200_SC08 && sample_size != GPSB200_SC16))
         return fail(ctx, GPSB200_ERR_ARG, "bad arguments (1 <= nchan <= cfg.max_chan; 1 <= nblk <= cfg.max_blocks)");
     if (!ctx->s_compute) return fail(ctx, GPSB200_ERR_CUDA, "context has no CUDA device");
-    if (ctx->pending.active) return fail(ctx, GPSB200_ERR_ARG, "a call begun with gpsb200_synth_begin has not been finished");
+    if (ctx->call.active) return fail(ctx, GPSB200_ERR_ARG, "a call begun with gpsb200_slice_prepare has not been finished");
     CU(cudaSetDevice(ctx->cfg.device));     // the caller may be a thread that never selected the context's device
     return GPSB200_OK;
 }
@@ -542,77 +590,119 @@ int ensure_staging(gpsb200_ctx *ctx, int sample_size) {
     return GPSB200_OK;
 }
 
-// Wait for everything this context has in flight (error paths: the caller may free its buffers once it
-// sees the error code, so no copy into them may still be pending). Leaves ctx->err alone.
-void drain(gpsb200_ctx *ctx, cudaStream_t extra) {
-    if (extra) cudaStreamSynchronize(extra);
+// The one error path of every entry point that enqueues work: on a non-OK return wait for everything this context
+// and the caller's stream have in flight (the caller may free its buffers once it sees the error code, so no copy into
+// them may still be pending) and drop the begun slice call; the context stays usable. Leaves ctx->err alone.
+int settle(gpsb200_ctx *ctx, cudaStream_t caller, int rc) {
+    if (rc == GPSB200_OK) return rc;
+    ctx->call.active = false;
+    if (!ctx->s_compute) return rc;
+    if (caller) cudaStreamSynchronize(caller);
     cudaStreamSynchronize(ctx->s_compute);
     cudaStreamSynchronize(ctx->s_pre);
-    if (ctx->s_ck) cudaStreamSynchronize(ctx->s_ck);
+    cudaStreamSynchronize(ctx->s_ck);
     cudaStreamSynchronize(ctx->s_copy);
+    return rc;
 }
 
-// First part of a pipeline segment [b0, b1): host records + guesses, parameters up, carrier tables.
-int segment_params(gpsb200_ctx *ctx, const gpsb200_chan_t *chans, int b0, int b1, int nchan, int sample_size,
-                   void *dst_dev, cudaStream_t sp, const std::vector<ChainState> &chain, gpsb200_stats_t &st,
-                   SynthArgs &a, gpsb200_slice_link_t *link, std::vector<ChainState> *end_guess = nullptr) {
-    const size_t blk_bytes = (size_t) GPSB200_BLOCK_ELEMS * sample_size;
-    const int nb = b1 - b0;
-    const size_t off = (size_t) b0 * nchan, cnt = (size_t) nb * nchan;
-    double t0 = now_ms();
-    int rc = prepare_blocks(ctx, chans, b0, b1, nchan, chain, link, end_guess);
+// ---- the steps of a call --------------------------------------------------------------------------------------------
+// A call's segments go through params -> probe -> scan -> commit; the schedules below (run_pipeline, the slice
+// entry points, gpsb200_carrier_chain_device) differ only in how they order and overlap these steps (DESIGN §6).
+
+// Start of a call's device work: the pre-phase streams wait for what the caller's stream holds so far (it may still read
+// the buffers rewritten now), then NAV words up and the self-check counter cleared on s_pre.
+int call_open(gpsb200_ctx *ctx, const Call &call) {
+    CU(cudaEventRecord(ctx->ev[kEvCallStart], call.stream));
+    CU(cudaStreamWaitEvent(ctx->s_pre, ctx->ev[kEvCallStart], 0));
+    CU(cudaStreamWaitEvent(ctx->s_ck, ctx->ev[kEvCallStart], 0));
+    const int rc = upload_nav(ctx, ctx->s_pre);
     if (rc) return rc;
-    st.host_chain_ms += now_ms() - t0;
-    CU(cudaMemcpyAsync(ctx->d_bc + off, ctx->h_bc + off, cnt * sizeof(BlockChanDev), cudaMemcpyHostToDevice, sp));
-    fill_args(ctx, a, b0, nb, nchan, sample_size, (char *) dst_dev + (size_t) b0 * blk_bytes);
-    CU(launch_tables(a, sp));                        // needs only the parameters: off the chain's critical path
-    st.launches += 1;
-    st.h2d_bytes += (int64_t) (cnt * sizeof(BlockChanDev));
+    CU(cudaMemsetAsync(ctx->d_chain_errors, 0, sizeof(int), ctx->s_pre));
     return GPSB200_OK;
 }
 
-// Second part: everything that needs no true start phase -- guesses up, block probes (+ the code-NCO half of the run
-// checkpoints, which segment_checkpoints relies on), span chaining.
-int segment_probe(gpsb200_ctx *ctx, int b0, int b1, int nchan, cudaStream_t sp, gpsb200_stats_t &st, bool first,
-                  const SynthArgs &a) {
-    const size_t off = (size_t) b0 * nchan, cnt = (size_t) (b1 - b0) * nchan;
+// Params of blocks [b0, b1) on sp: host records + guesses, parameters up, carrier tables (a call without a destination
+// computes the chain only and needs none). The guesses continue the call's exact chain state before b0, or with
+// `guessed` a GUESSED one (advanced in place to the guessed state after b1 - 1, so that the next segment can be
+// prepared before this one is resolved), or with `link` none at all (relative mode, see prepare_blocks).
+int seg_params(gpsb200_ctx *ctx, Call &call, int b0, int b1, cudaStream_t sp, std::vector<ChainState> *guessed,
+               gpsb200_slice_link_t *link) {
+    const size_t off = (size_t) b0 * call.nchan, cnt = (size_t) (b1 - b0) * call.nchan;
+    const double t0 = now_ms();
+    const int rc = prepare_blocks(ctx, call.chans, b0, b1, call.nchan, guessed ? *guessed : call.chain, link, guessed);
+    if (rc) return rc;
+    call.st.host_chain_ms += now_ms() - t0;
+    CU(cudaMemcpyAsync(ctx->d_bc + off, ctx->h_bc + off, cnt * sizeof(BlockChanDev), cudaMemcpyHostToDevice, sp));
+    call.st.h2d_bytes += (int64_t) (cnt * sizeof(BlockChanDev));
+    if (call.dst) {
+        CU(launch_tables(call_args(ctx, call, b0, b1 - b0), sp));     // needs only the parameters: off the critical path
+        call.st.launches += 1;
+    }
+    return GPSB200_OK;
+}
+
+// Probe of blocks [b0, b1) on sp: everything that needs no true start phase -- guesses up, block probes (+ the code-NCO
+// half of the run checkpoints, which seg_commit relies on; not for a call without a destination), span chaining.
+int seg_probe(gpsb200_ctx *ctx, Call &call, int b0, int b1, cudaStream_t sp) {
+    const size_t off = (size_t) b0 * call.nchan, cnt = (size_t) (b1 - b0) * call.nchan;
+    SynthArgs a = make_args(ctx, b0, b1 - b0, call.nchan, call.sample_size, nullptr);
+    if (!call.dst) a.ck = nullptr;
     CU(cudaMemcpyAsync(ctx->d_guess + off, ctx->h_guess + off, cnt * sizeof(double), cudaMemcpyHostToDevice, sp));
-    if (first) CU(cudaEventRecord(ctx->ev[1], sp));
+    if (b0 == 0) CU(cudaEventRecord(ctx->ev[kEvProbeStart], sp));
     CU(launch_probe(a, sp));
     CU(launch_chain(a, sp));
-    if (first) CU(cudaEventRecord(ctx->ev[2], sp));
-    st.launches += 2;
-    st.h2d_bytes += (int64_t) (cnt * sizeof(double));
-    st.d2h_bytes += (int64_t) (cnt * sizeof(CarrierProbe) + (size_t) a.nspan * nchan * sizeof(CarrierProbe));
+    if (b0 == 0) CU(cudaEventRecord(ctx->ev[kEvProbeEnd], sp));
+    call.st.launches += 2;
+    call.st.h2d_bytes += (int64_t) (cnt * sizeof(double));
+    call.st.d2h_bytes += (int64_t) (cnt * sizeof(CarrierProbe) + (size_t) a.nspan * call.nchan * sizeof(CarrierProbe));
     return GPSB200_OK;
 }
 
-// Host scan of a segment: wait until its probes and span summaries are in (mapped) host memory -- for the segment's
-// own probe event when there is one, else for the stream that ran them -- and resolve the chain from `chain` on.
-// slow: the number of spans resolved block by block (segment_checkpoints uploads their block start phases).
-int segment_scan(gpsb200_ctx *ctx, int b0, int b1, int nchan, cudaEvent_t probes_done, cudaStream_t sp,
-                 std::vector<ChainState> &chain, gpsb200_stats_t &st, int64_t &slow) {
+// Host scan of segment i: wait until its probes and span summaries are in (mapped) host memory -- for `probes_done`
+// when given, else for the stream that ran them -- and resolve the call's chain through the segment.
+int seg_scan(gpsb200_ctx *ctx, Call &call, int i, cudaEvent_t probes_done, cudaStream_t sp) {
     if (probes_done) CU(cudaEventSynchronize(probes_done));
     else CU(cudaStreamSynchronize(sp));
     const double t0 = now_ms();
-    slow = 0;
-    st.chain_fallbacks += (int32_t) resolve_chain(ctx, b0, b1, nchan, chain, &slow);
-    st.host_chain_ms += now_ms() - t0;
+    call.slow[i] = 0;
+    call.st.chain_fallbacks +=
+        (int32_t) resolve_chain(ctx, call.segs[i].first, call.segs[i].second, call.nchan, call.chain, &call.slow[i]);
+    call.st.host_chain_ms += now_ms() - t0;
+    call.after[i] = call.chain;
     return GPSB200_OK;
 }
 
-// Device part of a segment's resolution: resolutions up, exact run checkpoints (+ device self-check). After it the
-// segment's synthesis may be enqueued behind sp.
-int segment_checkpoints(gpsb200_ctx *ctx, int b0, int b1, int nchan, cudaStream_t sp, gpsb200_stats_t &st, bool first,
-                        const SynthArgs &a, int64_t slow) {
+// Blocks [b0, b1) of the call's device destination to its host destination, on stream s.
+int download(gpsb200_ctx *ctx, Call &call, int b0, int b1, cudaStream_t s) {
+    const size_t blk_bytes = (size_t) GPSB200_BLOCK_ELEMS * call.sample_size;
+    const char *src = (const char *) call.dst;
+    if (call.scatter) {          // every block straight into its own (FIFO) buffer
+        for (int b = b0; b < b1; b++)
+            CU(cudaMemcpyAsync(call.scatter[b], src + (size_t) b * blk_bytes, blk_bytes, cudaMemcpyDeviceToHost, s));
+    } else {
+        CU(cudaMemcpyAsync((char *) call.dst_host + (size_t) b0 * blk_bytes, src + (size_t) b0 * blk_bytes,
+                           (size_t) (b1 - b0) * blk_bytes, cudaMemcpyDeviceToHost, s));
+    }
+    call.st.d2h_bytes += (int64_t) (b1 - b0) * (int64_t) blk_bytes;
+    return GPSB200_OK;
+}
+
+// Commit of the scanned segments [i0, i1) as one range: resolutions up, exact run checkpoints (+ device self-check,
+// which stores the end phase of the range's last block into row i0 of h_seg_end) on sp, then -- behind them on the
+// caller's stream -- one synthesis launch, or with a host destination chunks each downloaded on s_copy behind it.
+int seg_commit(gpsb200_ctx *ctx, Call &call, int i0, int i1, cudaStream_t sp) {
+    const int b0 = call.segs[i0].first, b1 = call.segs[i1 - 1].second, nchan = call.nchan;
     const size_t off = (size_t) b0 * nchan, cnt = (size_t) (b1 - b0) * nchan;
+    int64_t slow = 0;
+    for (int i = i0; i < i1; i++) slow += call.slow[i];
+    SynthArgs a = call_args(ctx, call, b0, b1 - b0);
     const size_t soff = (size_t) (b0 / kSpanBlocks) * nchan, scnt = (size_t) a.nspan * nchan;
-    if (first) CU(cudaEventRecord(ctx->ev[3], sp));
+    if (b0 == 0) CU(cudaEventRecord(ctx->ev[kEvCkptStart], sp));
     CU(cudaMemcpyAsync(ctx->d_span_res + soff, ctx->h_span_res + soff, scnt * sizeof(SpanRes), cudaMemcpyHostToDevice, sp));
-    st.h2d_bytes += (int64_t) (scnt * sizeof(SpanRes));
+    call.st.h2d_bytes += (int64_t) (scnt * sizeof(SpanRes));
     if (slow > 0) {                                  // rare: block start phases of the host-resolved spans
         CU(cudaMemcpyAsync(ctx->d_carr0 + off, ctx->h_carr0 + off, cnt * sizeof(double), cudaMemcpyHostToDevice, sp));
-        st.h2d_bytes += (int64_t) (cnt * sizeof(double));
+        call.st.h2d_bytes += (int64_t) (cnt * sizeof(double));
     }
     // test hook of the device self-check (gpsb200_debug_corrupt_chain mode 2): move the state that block b0 + 5's probe
     // recorded for slot 0 at the start of the middle checkpoint segment by one unit of the rounding grid (the probes
@@ -628,39 +718,61 @@ int segment_checkpoints(gpsb200_ctx *ctx, int b0, int b1, int nchan, cudaStream_
         CU(cudaStreamSynchronize(sp));
     }
     SynthArgs ack = a;
-    ack.last_end_host = ctx->cur_seg < ctx->max_segs ? ctx->d_seg_end + (size_t) ctx->cur_seg * nchan : nullptr;
+    ack.last_end_host = ctx->d_seg_end + (size_t) i0 * nchan;
     CU(launch_checkpoints(ack, sp));
-    if (first) CU(cudaEventRecord(ctx->ev[4], sp));
-    st.launches += 1;
+    if (b0 == 0) CU(cudaEventRecord(ctx->ev[kEvCkptEnd], sp));
+    call.st.launches += 1;
+    // what the chain says the device's walk of the range's last block must end on (call_verdict compares the two):
+    // this extends the device self-check across pipeline-segment (and call) boundaries
+    for (int c = 0; c < nchan; c++) {
+        const ChainState &e = call.after[i1 - 1][c];
+        const bool live = e.prn > 0 && ctx->h_bc[(size_t) (b1 - 1) * nchan + c].prn == e.prn;
+        ctx->seg_expect[(size_t) i0 * nchan + c] = live ? e.phase : -1.0;       // -1: nothing to compare
+    }
+    call.rows = i0 + 1;
+    CU(cudaEventRecord(ctx->ev_done[call.ichunk], sp));           // the synthesis waits for the checkpoints
+    CU(cudaStreamWaitEvent(call.stream, ctx->ev_done[call.ichunk], 0));
+    call.ichunk++;
+    if (!call.host()) {
+        CU(launch_synth(a, call.stream));
+        call.st.launches += 1;
+        return GPSB200_OK;
+    }
+    // the very first chunks are short, so that the download (the long pole of this path) starts early
+    for (int c0 = b0, nc = 0; c0 < b1; c0 += nc, call.ichunk++) {
+        nc = c0 == 0 ? 32 : (c0 == 32 ? 96 : (c0 == 128 ? 128 : kSynthChunk));
+        nc = std::min(nc, b1 - c0);
+        CU(launch_synth(call_args(ctx, call, c0, nc), call.stream));
+        call.st.launches += 1;
+        CU(cudaEventRecord(ctx->ev_done[call.ichunk], call.stream));
+        CU(cudaStreamWaitEvent(ctx->s_copy, ctx->ev_done[call.ichunk], 0));
+        const int rc = download(ctx, call, c0, c0 + nc, ctx->s_copy);
+        if (rc) return rc;
+    }
     return GPSB200_OK;
 }
 
-// Synthesis of blocks [b0, b1) in chunks, each chunk's download to dst_host enqueued on s_copy behind it.
-// dst_host is either one contiguous buffer or, when ctx->scatter is set, ignored in favour of one host address per block.
-int synth_chunks(gpsb200_ctx *ctx, int b0, int b1, int nchan, int sample_size, void *dst_dev, void *dst_host,
-                 cudaStream_t s, gpsb200_stats_t &st, int &ichunk) {
-    const size_t blk_bytes = (size_t) GPSB200_BLOCK_ELEMS * sample_size;
-    // the very first chunks are short, so that the download (the long pole of this path) starts early
-    for (int c0 = b0, nc = 0; c0 < b1; c0 += nc, ichunk++) {
-        nc = c0 == 0 ? 32 : (c0 == 32 ? 96 : (c0 == 128 ? 128 : kSynthChunk));
-        nc = std::min(nc, b1 - c0);
-        SynthArgs ac{};
-        char *dout = (char *) dst_dev + (size_t) c0 * blk_bytes;
-        fill_args(ctx, ac, c0, nc, nchan, sample_size, dout);
-        CU(launch_synth(ac, s));
-        st.launches += 1;
-        CU(cudaEventRecord(ctx->ev_done[ichunk], s));
-        CU(cudaStreamWaitEvent(ctx->s_copy, ctx->ev_done[ichunk], 0));
-        if (ctx->scatter) {          // every block straight into its own (FIFO) buffer
-            for (int b = c0; b < c0 + nc; b++)
-                CU(cudaMemcpyAsync(ctx->scatter[b], dout + (size_t) (b - c0) * blk_bytes, blk_bytes, cudaMemcpyDeviceToHost,
-                                   ctx->s_copy));
-        } else {
-            CU(cudaMemcpyAsync((char *) dst_host + (size_t) c0 * blk_bytes, dout, (size_t) nc * blk_bytes,
-                               cudaMemcpyDeviceToHost, ctx->s_copy));
+// End of a call's enqueued work: end event on the caller's stream, the self-check counter read back behind the
+// checkpoint launches on sp; the call's device state stays resident for gpsb200_replay_device.
+int call_close(gpsb200_ctx *ctx, const Call &call, cudaStream_t sp) {
+    CU(cudaEventRecord(ctx->ev[kEvCallEnd], call.stream));
+    CU(cudaMemcpyAsync(ctx->h_chain_errors, ctx->d_chain_errors, sizeof(int), cudaMemcpyDeviceToHost, sp));
+    ctx->last = call_args(ctx, call, 0, call.nblk);
+    ctx->have_last = true;
+    return GPSB200_OK;
+}
+
+// Verdict of the device self-check (the counter read by call_close must have arrived): the per-block comparisons inside
+// the checkpoint launches plus the comparisons at the end of every committed range.
+int call_verdict(gpsb200_ctx *ctx, const Call &call) {
+    int bad = *ctx->h_chain_errors;
+    for (int i = 0; i < call.rows; i++)
+        for (int c = 0; c < call.nchan; c++) {
+            const double want = ctx->seg_expect[(size_t) i * call.nchan + c];
+            if (want >= 0.0 && f64_bits(want) != f64_bits(ctx->h_seg_end[(size_t) i * call.nchan + c])) ++bad;
         }
-        st.d2h_bytes += (int64_t) nc * (int64_t) blk_bytes;
-    }
+    if (bad != 0)
+        return fail(ctx, GPSB200_ERR_INTERNAL, "carrier chain self-check failed on " + std::to_string(bad) + " blocks");
     return GPSB200_OK;
 }
 
@@ -680,17 +792,16 @@ void export_chain(const std::vector<ChainState> &chain, int nchan, int32_t *prn_
 
 // A call of one or two blocks (the reference's cadence): the host walks every NCO chain exactly (nco_exact.h) and
 // hands the device ready-made run checkpoints; tables + synthesis are the only kernels. Exact by construction.
-int small_call(gpsb200_ctx *ctx, const gpsb200_chan_t *chans, int nblk, int nchan, int sample_size, void *dst_dev,
-               void *dst_host, cudaStream_t s, std::vector<ChainState> &chain, int32_t *prn_out, double *carr_phase_out,
-               gpsb200_stats_t *stats) {
-    gpsb200_stats_t st{};
+int small_call(gpsb200_ctx *ctx, Call &call, double *carr_phase_out, gpsb200_stats_t *stats) {
+    const int nblk = call.nblk, nchan = call.nchan;
+    cudaStream_t s = call.stream;
     double t0 = now_ms();
-    int rc = prepare_blocks(ctx, chans, 0, nblk, nchan, chain);
+    int rc = prepare_blocks(ctx, call.chans, 0, nblk, nchan, call.chain);
     if (rc) return rc;
     const int nruns = ctx->nruns, run = ctx->cfg.run_samples;
     ctx->pool->run(nchan, [&](int c_lo, int c_hi) {
         for (int c = c_lo; c < c_hi; c++) {
-            ChainState stc = chain[c];
+            ChainState stc = call.chain[c];
             for (int b = 0; b < nblk; b++) {
                 const BlockChanDev &p = ctx->h_bc[(size_t) b * nchan + c];
                 RunCkpt *ck = ctx->h_ck + (size_t) b * nruns * nchan + c;
@@ -713,210 +824,256 @@ int small_call(gpsb200_ctx *ctx, const gpsb200_chan_t *chans, int nblk, int ncha
                 }
                 stc.phase = x;
             }
-            chain[c] = stc;
+            call.chain[c] = stc;
         }
     });
-    st.host_chain_ms = now_ms() - t0;
+    call.st.host_chain_ms = now_ms() - t0;
     rc = upload_nav(ctx, s);
     if (rc) return rc;
     const size_t cnt = (size_t) nblk * nchan;
-    CU(cudaEventRecord(ctx->ev[0], s));
+    CU(cudaEventRecord(ctx->ev[kEvCallStart], s));
     CU(cudaMemcpyAsync(ctx->d_bc, ctx->h_bc, cnt * sizeof(BlockChanDev), cudaMemcpyHostToDevice, s));
     CU(cudaMemcpyAsync(ctx->d_ck, ctx->h_ck, cnt * nruns * sizeof(RunCkpt), cudaMemcpyHostToDevice, s));
-    SynthArgs a{};
-    fill_args(ctx, a, 0, nblk, nchan, sample_size, dst_dev);
+    const SynthArgs a = call_args(ctx, call, 0, nblk);
     CU(launch_tables(a, s));
     CU(launch_synth(a, s));
-    CU(cudaEventRecord(ctx->ev[5], s));
-    st.launches = 2;
-    st.h2d_bytes = (int64_t) (cnt * (sizeof(BlockChanDev) + nruns * sizeof(RunCkpt)));
-    const size_t bytes = (size_t) nblk * GPSB200_BLOCK_ELEMS * sample_size;
-    if (dst_host) {
-        if (ctx->scatter) {
-            for (int b = 0; b < nblk; b++)
-                CU(cudaMemcpyAsync(ctx->scatter[b], (char *) dst_dev + (size_t) b * (bytes / nblk), bytes / nblk,
-                                   cudaMemcpyDeviceToHost, s));
-        } else {
-            CU(cudaMemcpyAsync(dst_host, dst_dev, bytes, cudaMemcpyDeviceToHost, s));
-        }
-        st.d2h_bytes = (int64_t) bytes;
+    CU(cudaEventRecord(ctx->ev[kEvCallEnd], s));
+    call.st.launches = 2;
+    call.st.h2d_bytes = (int64_t) (cnt * (sizeof(BlockChanDev) + nruns * sizeof(RunCkpt)));
+    if (call.host()) {
+        rc = download(ctx, call, 0, nblk, s);
+        if (rc) return rc;
         CU(cudaStreamSynchronize(s));
     }
-    ctx->last = a;
     ctx->have_last = false;              // nothing to replay: there were no walk kernels
-    export_chain(chain, nchan, prn_out, carr_phase_out);
-    if (stats) *stats = st;
+    export_chain(call.chain, nchan, nullptr, carr_phase_out);
+    if (stats) *stats = call.st;
     return GPSB200_OK;
 }
 
-// Pipeline segments of a call: a short first one (its chain resolution is the lead-in of everything), then long ones.
-std::vector<std::pair<int, int>> segments_of(int nblk) {
-    std::vector<std::pair<int, int>> v;
-    int len = kSegFirst;
-    for (int b0 = 0; b0 < nblk; len = kSegBlocks) {
-        const int b1 = std::min(nblk, b0 + len);
-        v.emplace_back(b0, b1);
-        b0 = b1;
-    }
-    return v;
-}
-
-// After the checkpoint kernel of segment i: remember what the chain expects at the segment's end. The kernel itself
-// stores what the device's exact walk of the segment's last block ended on into h_seg_end (mapped memory: a
-// copy-engine transfer would queue behind the large result downloads); verify_chain() compares the two. This extends
-// the device self-check across pipeline-segment (and call) boundaries.
-void note_segment_end(gpsb200_ctx *ctx, int iseg, int b1, int nchan, const std::vector<ChainState> &chain) {
-    if (iseg >= ctx->max_segs) return;
-    for (int c = 0; c < nchan; c++) {
-        const bool live = chain[c].prn > 0 && ctx->h_bc[(size_t) (b1 - 1) * nchan + c].prn == chain[c].prn;
-        ctx->seg_expect[(size_t) iseg * nchan + c] = live ? chain[c].phase : -1.0;       // -1: nothing to compare
-    }
-}
-
-// Verdict of the device self-check (all of sp's work must be complete): the per-block comparisons inside the
-// checkpoint launches plus the segment-boundary comparisons.
-int verify_chain(gpsb200_ctx *ctx, int nseg, int nchan) {
-    int bad = *ctx->h_chain_errors;
-    for (int i = 0; i < std::min(nseg, ctx->max_segs); i++)
-        for (int c = 0; c < nchan; c++) {
-            const double want = ctx->seg_expect[(size_t) i * nchan + c];
-            if (want >= 0.0 && f64_bits(want) != f64_bits(ctx->h_seg_end[(size_t) i * nchan + c])) ++bad;
-        }
-    if (bad != 0)
-        return fail(ctx, GPSB200_ERR_INTERNAL, "carrier chain self-check failed on " + std::to_string(bad) + " blocks");
-    return GPSB200_OK;
-}
-
-// The whole path for nblk blocks, as a pipeline of segments: the carrier-chain resolution of a segment (parameters
-// up -> block probes -> span chaining -> host scan over the span summaries -> resolutions up -> run checkpoints)
-// runs on the context's high-priority pre-phase stream and therefore CONCURRENTLY with the synthesis kernels of
-// earlier segments on the caller's stream (the walk kernels are latency bound and fit beside k_synth's CTAs) and,
-// with a host destination, with the downloads of finished chunks. Only the first (short) segment's resolution is
-// a lead-in. dst_host == NULL: results stay at dst_dev and the call returns once everything is enqueued and the
-// chain self-check has been read.
-int run_pipeline_inner(gpsb200_ctx *ctx, const gpsb200_chan_t *chans, int nblk, int nchan, int sample_size,
-                       void *dst_dev, void *dst_host, cudaStream_t s, const int32_t *prn_in, const double *phase_in,
-                       int32_t *prn_out, double *carr_phase_out, gpsb200_stats_t *stats) {
-    gpsb200_stats_t st{};
-    std::vector<ChainState> chain(nchan);
-    seed_chain(chain, nchan, prn_in, phase_in);
+// A one-shot call, as a pipeline of segments: the carrier-chain resolution of a segment runs on the context's
+// high-priority pre-phase stream and therefore CONCURRENTLY with the synthesis kernels of earlier segments on the
+// caller's stream (the walk kernels are latency bound and fit beside k_synth's CTAs) and, with a host destination, with
+// the downloads of finished chunks. Only the first (short) segment's resolution is a lead-in. Without a host destination
+// the results stay at call.dst and the call returns once everything is enqueued and the chain self-check has been read.
+int run_pipeline(gpsb200_ctx *ctx, Call &call, double *carr_phase_out, gpsb200_stats_t *stats) {
     ctx->trace_t0 = now_ms();
     trace(ctx, "call");
-    if (nblk <= kHostChainBlocks && !ctx->fault_inject_chain)
-        return small_call(ctx, chans, nblk, nchan, sample_size, dst_dev, dst_host, s, chain, prn_out, carr_phase_out, stats);
+    if (call.nblk <= kHostChainBlocks && !ctx->fault_inject_chain) return small_call(ctx, call, carr_phase_out, stats);
     cudaStream_t sp = ctx->s_pre;                       // stream of the pre-phase
-    CU(cudaEventRecord(ctx->ev[0], s));
-    CU(cudaStreamWaitEvent(sp, ctx->ev[0], 0));         // earlier work on s may still read the buffers rewritten now
-    int rc = upload_nav(ctx, sp);
+    int rc = call_open(ctx, call);
     if (rc) return rc;
-    CU(cudaMemsetAsync(ctx->d_chain_errors, 0, sizeof(int), sp));
-    int iseg = 0;
-    const auto segs = segments_of(nblk);
-    if (!dst_host) {
-        // Device destination: nothing has to leave early, so everything speculative goes first -- the host prepares
-        // segment after segment (guesses continue from the GUESSED end of the previous segment) while the GPU already
-        // probes the earlier ones -- then the host scans the span summaries, and run checkpoints and synthesis are
-        // ONE launch each over the whole call.
-        std::vector<ChainState> guess = chain;
-        std::vector<SynthArgs> sa(segs.size());
-        CU(cudaStreamWaitEvent(ctx->s_ck, ctx->ev[0], 0));
-        for (size_t i = 0; i < segs.size(); i++) {
+    const auto &segs = call.segs;
+    const int nseg = (int) segs.size();
+    if (!call.host()) {
+        // Device destination (EAGER): nothing has to leave early, so everything speculative goes first -- the host
+        // prepares segment after segment (guesses continue from the GUESSED end of the previous segment) while the GPU
+        // already probes the earlier ones -- then the host scans the span summaries, and run checkpoints and synthesis
+        // are ONE launch each over the whole call.
+        std::vector<ChainState> guess = call.chain;
+        for (int i = 0; i < nseg; i++) {
             // the segments' walk kernels alternate between two streams: their long tails (walk lengths differ by
             // an order of magnitude between satellites) overlap instead of adding up
             cudaStream_t sw = (i & 1) ? ctx->s_ck : sp;
-            std::vector<ChainState> next(nchan);
-            rc = segment_params(ctx, chans, segs[i].first, segs[i].second, nchan, sample_size, dst_dev, sw, guess, st, sa[i], nullptr,
-                                &next);
+            rc = seg_params(ctx, call, segs[i].first, segs[i].second, sw, &guess, nullptr);
             if (rc) return rc;
-            rc = segment_probe(ctx, segs[i].first, segs[i].second, nchan, sw, st, i == 0, sa[i]);
+            rc = seg_probe(ctx, call, segs[i].first, segs[i].second, sw);
             if (rc) return rc;
-            CU(cudaEventRecord(ctx->ev_seg[std::min((int) i, ctx->max_segs - 1)], sw));
-            guess = next;
+            CU(cudaEventRecord(ctx->ev_seg[i], sw));
         }
-        int64_t slow = 0;
         trace(ctx, "speculative work enqueued");
-        for (size_t i = 0; i < segs.size(); i++) {
-            int64_t sl = 0;
-            rc = segment_scan(ctx, segs[i].first, segs[i].second, nchan, ctx->ev_seg[std::min((int) i, ctx->max_segs - 1)],
-                              nullptr, chain, st, sl);
+        for (int i = 0; i < nseg; i++) {
+            rc = seg_scan(ctx, call, i, ctx->ev_seg[i], nullptr);
             if (rc) return rc;
-            slow += sl;
         }
         CU(cudaStreamSynchronize(ctx->s_ck));           // (its last segment's event has been waited for; this orders the
         trace(ctx, "host scan done");                   //  checkpoint launch on sp behind everything on s_ck)
-        SynthArgs all{};
-        fill_args(ctx, all, 0, nblk, nchan, sample_size, dst_dev);
-        ctx->cur_seg = 0;
-        rc = segment_checkpoints(ctx, 0, nblk, nchan, sp, st, true, all, slow);
+        rc = seg_commit(ctx, call, 0, nseg, sp);
         if (rc) return rc;
-        note_segment_end(ctx, iseg++, nblk, nchan, chain);
-        CU(cudaEventRecord(ctx->ev_done[0], sp));
-        CU(cudaStreamWaitEvent(s, ctx->ev_done[0], 0));
-        CU(launch_synth(all, s));
-        st.launches += 1;
         trace(ctx, "checkpoints + synthesis enqueued");
     } else {
-        int ichunk = 0;
-        for (const auto &sg : segs) {
-            const int b0 = sg.first, b1 = sg.second;
-            SynthArgs a{};
-            rc = segment_params(ctx, chans, b0, b1, nchan, sample_size, dst_dev, sp, chain, st, a, nullptr);
+        // Host destination (LAZY): segment by segment from the exact chain, so that the first downloads start early
+        for (int i = 0; i < nseg; i++) {
+            rc = seg_params(ctx, call, segs[i].first, segs[i].second, sp, nullptr, nullptr);
             if (rc) return rc;
-            rc = segment_probe(ctx, b0, b1, nchan, sp, st, b0 == 0, a);
+            rc = seg_probe(ctx, call, segs[i].first, segs[i].second, sp);
             if (rc) return rc;
-            int64_t slow = 0;
-            rc = segment_scan(ctx, b0, b1, nchan, nullptr, sp, chain, st, slow);
+            rc = seg_scan(ctx, call, i, nullptr, sp);
             if (rc) return rc;
-            ctx->cur_seg = iseg;
-            rc = segment_checkpoints(ctx, b0, b1, nchan, sp, st, b0 == 0, a, slow);
-            if (rc) return rc;
-            note_segment_end(ctx, iseg++, b1, nchan, chain);
-            CU(cudaEventRecord(ctx->ev_done[ichunk], sp));   // synthesis of this segment waits for its checkpoints
-            CU(cudaStreamWaitEvent(s, ctx->ev_done[ichunk], 0));
-            ichunk++;
-            rc = synth_chunks(ctx, b0, b1, nchan, sample_size, dst_dev, dst_host, s, st, ichunk);
+            rc = seg_commit(ctx, call, i, i + 1, sp);
             if (rc) return rc;
         }
     }
-    CU(cudaEventRecord(ctx->ev[5], s));
-    SynthArgs all{};
-    fill_args(ctx, all, 0, nblk, nchan, sample_size, dst_dev);
-    ctx->last = all;
-    ctx->have_last = true;
-    export_chain(chain, nchan, prn_out, carr_phase_out);
+    rc = call_close(ctx, call, sp);
+    if (rc) return rc;
+    export_chain(call.chain, call.nchan, nullptr, carr_phase_out);
     // the device self-check of the carrier chain is never skipped: a wrong start phase must not produce samples silently
-    CU(cudaMemcpyAsync(ctx->h_chain_errors, ctx->d_chain_errors, sizeof(int), cudaMemcpyDeviceToHost, sp));
     CU(cudaStreamSynchronize(sp));
     trace(ctx, "pre-phase stream drained (self-check read)");
-    rc = verify_chain(ctx, iseg, nchan);
+    rc = call_verdict(ctx, call);
     if (rc) return rc;
-    if (dst_host) {
-        CU(cudaStreamSynchronize(s));
+    if (call.host()) {
+        CU(cudaStreamSynchronize(call.stream));
         CU(cudaStreamSynchronize(ctx->s_copy));
     }
     if (stats) {
         float ms = 0;
         // per-kernel times of the FIRST segment ...
-        cudaEventElapsedTime(&ms, ctx->ev[1], ctx->ev[2]);
-        st.probe_kernel_ms = ms;
-        cudaEventElapsedTime(&ms, ctx->ev[3], ctx->ev[4]);
-        st.checkpoint_kernel_ms = ms;
-        if (dst_host) {      // ... and the whole span of the call's stream (a device-destination call is still running)
-            cudaEventElapsedTime(&ms, ctx->ev[0], ctx->ev[5]);
-            st.kernel_ms = ms;
+        cudaEventElapsedTime(&ms, ctx->ev[kEvProbeStart], ctx->ev[kEvProbeEnd]);
+        call.st.probe_kernel_ms = ms;
+        cudaEventElapsedTime(&ms, ctx->ev[kEvCkptStart], ctx->ev[kEvCkptEnd]);
+        call.st.checkpoint_kernel_ms = ms;
+        if (call.host()) {      // ... and the whole span of the call's stream (a device-destination call is still running)
+            cudaEventElapsedTime(&ms, ctx->ev[kEvCallStart], ctx->ev[kEvCallEnd]);
+            call.st.kernel_ms = ms;
         }
-        *stats = st;
+        *stats = call.st;
     }
     return GPSB200_OK;
 }
 
-int run_pipeline(gpsb200_ctx *ctx, const gpsb200_chan_t *chans, int nblk, int nchan, int sample_size,
-                 void *dst_dev, void *dst_host, cudaStream_t s, const int32_t *prn_in, const double *phase_in,
-                 int32_t *prn_out, double *carr_phase_out, gpsb200_stats_t *stats) {
-    const int rc = run_pipeline_inner(ctx, chans, nblk, nchan, sample_size, dst_dev, dst_host, s, prn_in, phase_in, prn_out,
-                                      carr_phase_out, stats);
-    if (rc) drain(ctx, s);          // nothing of this call may still be in flight when the caller sees the error
-    return rc;
+// The three slice steps (include/gpsb200.h); the begun call lives in ctx->call between them.
+int slice_prepare(gpsb200_ctx *ctx, const gpsb200_chan_t *chans, int nblk, int nchan, int sample_size, void *dst_device,
+                  void *dst_host, cudaStream_t s, gpsb200_slice_link_t *link) {
+    int rc = check_call(ctx, chans, nblk, nchan, sample_size, dst_device ? dst_device : dst_host);
+    if (rc) return rc;
+    rc = check_dst_aligned(ctx, dst_device, "gpsb200_slice_prepare");
+    if (rc) return rc;
+    if (!dst_device) {                          // host destination only: stage in the context's own device buffer
+        rc = ensure_staging(ctx, sample_size);
+        if (rc) return rc;
+        dst_device = ctx->d_out;
+    }
+    if (!link) return fail(ctx, GPSB200_ERR_ARG, "gpsb200_slice_prepare: link is NULL");
+    Call &call = ctx->call = Call(chans, nblk, nchan, sample_size, dst_device, dst_host, nullptr, s);
+    call.active = true;
+    rc = call_open(ctx, call);
+    if (rc) return rc;
+    memset(link, 0, sizeof *link);
+    rc = seg_params(ctx, call, 0, nblk, ctx->s_pre, nullptr, link);
+    if (rc) return rc;
+    call.chans = nullptr;                       // the caller's records may go now
+    ctx->have_last = false;
+    return GPSB200_OK;
+}
+
+int slice_probe(gpsb200_ctx *ctx, const int32_t *prn_in, const double *phase_guess_in, int eager) {
+    Call &call = ctx->call;
+    if (!call.active || call.probed) return fail(ctx, GPSB200_ERR_ARG, "gpsb200_slice_probe: call gpsb200_slice_prepare first");
+    CU(cudaSetDevice(ctx->cfg.device));
+    const double t0 = now_ms();
+    finalize_guesses(ctx, 0, call.nblk, call.nchan, prn_in, phase_guess_in);
+    call.st.host_chain_ms += now_ms() - t0;
+    // EAGER: everything speculative at once, ONE probe and ONE chaining launch over the whole slice (no per-segment
+    // tails). LAZY: only the first segment's; the others follow one by one in slice_finish.
+    call.eager = eager != 0;
+    const int n = call.eager ? (int) call.segs.size() : 1;
+    int rc = seg_probe(ctx, call, 0, call.segs[n - 1].second, ctx->s_pre);
+    if (rc) return rc;
+    for (int i = 0; i < n; i++) CU(cudaEventRecord(ctx->ev_seg[i], ctx->s_pre));
+    call.probed = true;
+    return GPSB200_OK;
+}
+
+int slice_finish(gpsb200_ctx *ctx, const int32_t *prn_in, const double *phase_in, int32_t *prn_out, double *phase_out,
+                 gpsb200_stats_t *stats, gpsb200_handoff_fn handoff, void *user) {
+    Call &call = ctx->call;
+    if (!call.active || !call.probed)
+        return fail(ctx, GPSB200_ERR_ARG, "gpsb200_slice_finish: call gpsb200_slice_prepare and gpsb200_slice_probe first");
+    CU(cudaSetDevice(ctx->cfg.device));
+    const int nchan = call.nchan, nseg = (int) call.segs.size();
+    cudaStream_t sk = ctx->s_ck;
+    seed_chain(call.chain, nchan, prn_in, phase_in);
+    std::vector<int32_t> po(nchan, 0);
+    std::vector<double> xo(nchan, 0.0);
+    ctx->trace_t0 = now_ms();
+    trace(ctx, "slice_finish");
+    int rc;
+    if (call.eager) {
+        // A successor waits for the outgoing state: scan EVERYTHING first (all probes were submitted up front), hand
+        // the exact state on, and only then enqueue the long kernels -- a message sent behind them would wait for them.
+        for (int i = 0; i < nseg; i++) {
+            rc = seg_scan(ctx, call, i, ctx->ev_seg[i], sk);
+            if (rc) return rc;
+        }
+        trace(ctx, "host scan done");
+        export_chain(call.chain, nchan, po.data(), xo.data());
+        if (handoff) handoff(user, po.data(), xo.data());
+        trace(ctx, "handed over");
+    }
+    for (int i = 0; i < nseg; i++) {
+        if (!call.eager) {
+            // lazy: host scan of this segment as soon as ITS probes are done; checkpoints on a stream of their own
+            rc = seg_scan(ctx, call, i, ctx->ev_seg[i], sk);
+            if (rc) return rc;
+        }
+        rc = seg_commit(ctx, call, i, i + 1, sk);
+        if (rc) return rc;
+        if (!call.eager && i + 1 < nseg) {
+            // lazy: the next segment's speculative work is submitted only now, BEHIND this segment's synthesis, from
+            // guesses re-anchored on the exact state just resolved
+            const int b0 = call.segs[i + 1].first, b1 = call.segs[i + 1].second;
+            reanchor_guesses(ctx, b0, b1, nchan, call.chain);
+            rc = seg_probe(ctx, call, b0, b1, ctx->s_pre);
+            if (rc) return rc;
+            CU(cudaEventRecord(ctx->ev_seg[i + 1], ctx->s_pre));
+        }
+    }
+    if (!call.eager) {
+        export_chain(call.chain, nchan, po.data(), xo.data());
+        if (handoff) handoff(user, po.data(), xo.data());
+    }
+    rc = call_close(ctx, call, sk);
+    if (rc) return rc;
+    trace(ctx, "checkpoints + synthesis enqueued");
+    call.active = false;
+    call.finished = true;
+    for (int c = 0; c < nchan; c++) {
+        if (prn_out) prn_out[c] = po[c];
+        if (phase_out) phase_out[c] = xo[c];
+    }
+    if (stats) *stats = call.st;
+    return GPSB200_OK;
+}
+
+// gpsb200_synth_blocks and _scatter: staged in the context's own device buffer, downloaded to the host destination.
+int synth_host(gpsb200_ctx *ctx, const gpsb200_chan_t *chans, int nblk, int nchan, int sample_size, void *dst_host,
+               void *const *scatter, double *carr_phase_out, gpsb200_stats_t *stats) {
+    for (int b = 0; scatter && b < nblk; b++)
+        if (!scatter[b]) return fail(ctx, GPSB200_ERR_ARG, "gpsb200_synth_blocks_scatter: NULL block destination");
+    int rc = check_call(ctx, chans, nblk, nchan, sample_size, scatter ? scatter[0] : dst_host);
+    if (rc) return rc;
+    rc = ensure_staging(ctx, sample_size);
+    if (rc) return rc;
+    Call call(chans, nblk, nchan, sample_size, ctx->d_out, dst_host, scatter, ctx->s_compute);
+    return run_pipeline(ctx, call, carr_phase_out, stats);
+}
+
+// gpsb200_carrier_chain_device: windows of at most cfg.max_blocks, each params -> probe -> scan on the context's stream;
+// the call has no destination (no carrier tables, no code walk, no checkpoints).
+int carrier_chain_device(gpsb200_ctx *ctx, const gpsb200_chan_t *chans, int nblk, int nchan, const double *phase_in,
+                         double *phase_out) {
+    if (!ctx->s_compute) return fail(ctx, GPSB200_ERR_CUDA, "context has no CUDA device");
+    if (ctx->call.active) return fail(ctx, GPSB200_ERR_ARG, "a call begun with gpsb200_slice_prepare has not been finished");
+    CU(cudaSetDevice(ctx->cfg.device));
+    cudaStream_t s = ctx->s_compute;
+    Call call(chans, 0, nchan, GPSB200_SC08, nullptr, nullptr, nullptr, s);
+    if (phase_in && nblk > 0)
+        for (int c = 0; c < nchan; c++)
+            if (chans[c].prn > 0) call.chain[c] = ChainState{chans[c].prn, phase_in[c]};
+    for (int w0 = 0; w0 < nblk; w0 += ctx->cfg.max_blocks) {
+        const int nw = std::min(ctx->cfg.max_blocks, nblk - w0);
+        call.chans = chans + (size_t) w0 * nchan;
+        call.nblk = nw;
+        call.plan({std::make_pair(0, nw)});
+        int rc = seg_params(ctx, call, 0, nw, s, nullptr, nullptr);
+        if (!rc) rc = seg_probe(ctx, call, 0, nw, s);
+        if (!rc) rc = seg_scan(ctx, call, 0, nullptr, s);
+        if (rc) return rc;
+    }
+    ctx->have_last = false;
+    export_chain(call.chain, nchan, nullptr, phase_out);
+    return GPSB200_OK;
 }
 
 }  // namespace
@@ -993,19 +1150,17 @@ int gpsb200_span_chain_host(const double *f_carr, int nblk, double start_true, d
     std::vector<CarrierProbe> probes(nblk);
     std::vector<double> cc(nblk);
     std::vector<SpanBlockState> spec(nblk);
-    long double acc = start_guess;
+    uint64_t acc = phase_to_fix(start_guess);
+    const double guess0 = fix_to_phase(acc);        // the span is chained from its first block's guess, as k_chain does
     for (int j = 0; j < nblk; j++) {
         cc[j] = f_carr[j] * delt;
-        double g = (double) acc;
-        if (!(g >= 0.0 && g < 1.0)) g = 0.0;
-        carrier_probe(g, cc[j], GPSB200_BLOCK_SAMPLES, probes[j]);
-        acc += (long double) GPSB200_BLOCK_SAMPLES * ((long double) cc[j] + (long double) carrier_drift_per_step(cc[j]));
-        acc -= floorl(acc);
+        carrier_probe(fix_to_phase(acc), cc[j], GPSB200_BLOCK_SAMPLES, probes[j]);
+        acc = guess_block(acc, cc[j]);
     }
     CarrierProbe sum{}, part{};
     bool ok[2];
     for (int V = 0; V < 2; V++) {
-        span_chain(probes.data(), OneSatellite{cc.data()}, nblk, 1, start_guess, V, part, ok[V], spec.data());
+        span_chain(probes.data(), OneSatellite{cc.data()}, nblk, 1, guess0, V, part, ok[V], spec.data());
         if (V == 0) {
             sum.x_w = part.x_w;
             sum.n_w = part.n_w;
@@ -1133,12 +1288,12 @@ int gpsb200_create(const gpsb200_config_t *cfg, gpsb200_ctx_t **out) {
     const int nchunk = (c.max_blocks + kSynthChunk - 1) / kSynthChunk + (c.max_blocks + kSegBlocks - 1) / kSegBlocks + 5;
     ctx->ev_done.resize(nchunk);
     for (auto &e : ctx->ev_done) CU(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-    ctx->max_segs = (c.max_blocks + kSegBlocks - 1) / kSegBlocks + 2;
-    ctx->ev_seg.resize(ctx->max_segs);
+    const size_t max_segs = segments_of(c.max_blocks).size();     // every call's segments have their rows and events
+    ctx->ev_seg.resize(max_segs);
     for (auto &e : ctx->ev_seg) CU(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-    CU(cudaHostAlloc(&ctx->h_seg_end, (size_t) ctx->max_segs * c.max_chan * sizeof(double), cudaHostAllocMapped));
+    CU(cudaHostAlloc(&ctx->h_seg_end, max_segs * c.max_chan * sizeof(double), cudaHostAllocMapped));
     CU(cudaHostGetDevicePointer((void **) &ctx->d_seg_end, ctx->h_seg_end, 0));
-    ctx->seg_expect.assign((size_t) ctx->max_segs * c.max_chan, -1.0);
+    ctx->seg_expect.assign(max_segs * c.max_chan, -1.0);
     const size_t nbc = (size_t) c.max_blocks * c.max_chan;
     CU(cudaMalloc(&ctx->d_bc, nbc * sizeof(BlockChanDev)));
     CU(cudaHostAlloc(&ctx->h_bc, nbc * sizeof(BlockChanDev), cudaHostAllocDefault));
@@ -1245,201 +1400,36 @@ int gpsb200_set_nav(gpsb200_ctx_t *ctx, int frame, int chan, const uint32_t dwrd
 int gpsb200_synth_blocks_device(gpsb200_ctx_t *ctx, const gpsb200_chan_t *chans, int nblk, int nchan,
                                 int sample_size, void *dst_device, void *stream_, double *carr_phase_out,
                                 gpsb200_stats_t *stats) {
-    int rc = check_call(ctx, chans, nblk, nchan, sample_size, dst_device);
-    if (rc) return rc;
-    rc = check_dst_aligned(ctx, dst_device, "gpsb200_synth_blocks_device");
-    if (rc) return rc;
+    if (!ctx) return GPSB200_ERR_ARG;
     cudaStream_t s = stream_ ? (cudaStream_t) stream_ : ctx->s_compute;
-    return run_pipeline(ctx, chans, nblk, nchan, sample_size, dst_device, nullptr, s, nullptr, nullptr, nullptr,
-                        carr_phase_out, stats);
+    int rc = check_call(ctx, chans, nblk, nchan, sample_size, dst_device);
+    if (!rc) rc = check_dst_aligned(ctx, dst_device, "gpsb200_synth_blocks_device");
+    if (!rc) {
+        Call call(chans, nblk, nchan, sample_size, dst_device, nullptr, nullptr, s);
+        rc = run_pipeline(ctx, call, carr_phase_out, stats);
+    }
+    return settle(ctx, s, rc);
 }
 
 // ---- time-slice hand-over: one call in three steps (see include/gpsb200.h) --------------------------
 int gpsb200_slice_prepare(gpsb200_ctx_t *ctx, const gpsb200_chan_t *chans, int nblk, int nchan, int sample_size,
                           void *dst_device, void *dst_host, void *stream_, gpsb200_slice_link_t *link) {
-    int rc = check_call(ctx, chans, nblk, nchan, sample_size, dst_device ? dst_device : dst_host);
-    if (rc) return rc;
-    rc = check_dst_aligned(ctx, dst_device, "gpsb200_slice_prepare");
-    if (rc) return rc;
-    if (!dst_device) {                          // host destination only: stage in the context's own device buffer
-        rc = ensure_staging(ctx, sample_size);
-        if (rc) return rc;
-        dst_device = ctx->d_out;
-    }
-    if (!link) return fail(ctx, GPSB200_ERR_ARG, "gpsb200_slice_prepare: link is NULL");
+    if (!ctx) return GPSB200_ERR_ARG;
     cudaStream_t s = stream_ ? (cudaStream_t) stream_ : ctx->s_compute;
-    cudaStream_t sp = ctx->s_pre;
-    CU(cudaEventRecord(ctx->ev[0], s));
-    CU(cudaStreamWaitEvent(sp, ctx->ev[0], 0));         // earlier work on s may still read the buffers rewritten now
-    CU(cudaStreamWaitEvent(ctx->s_ck, ctx->ev[0], 0));
-    rc = upload_nav(ctx, sp);
-    if (rc) return rc;
-    CU(cudaMemsetAsync(ctx->d_chain_errors, 0, sizeof(int), sp));
-    std::vector<ChainState> none(nchan);
-    gpsb200_stats_t st{};
-    SynthArgs a{};
-    memset(link, 0, sizeof *link);
-    rc = segment_params(ctx, chans, 0, nblk, nchan, sample_size, dst_device, sp, none, st, a, link);
-    if (rc) {
-        drain(ctx, s);
-        return rc;
-    }
-    ctx->last = a;
-    ctx->have_last = false;
-    ctx->pending.active = true;
-    ctx->pending.probed = false;
-    ctx->pending.finished = false;
-    ctx->pending.nblk = nblk;
-    ctx->pending.nchan = nchan;
-    ctx->pending.sample_size = sample_size;
-    ctx->pending.dst = dst_device;
-    ctx->pending.dst_host = dst_host;
-    ctx->pending.stream = s;
-    ctx->pending.st = st;
-    return GPSB200_OK;
+    return settle(ctx, s, slice_prepare(ctx, chans, nblk, nchan, sample_size, dst_device, dst_host, s, link));
 }
 
 int gpsb200_slice_probe(gpsb200_ctx_t *ctx, const int32_t *prn_in, const double *phase_guess_in, int eager) {
     if (!ctx) return GPSB200_ERR_ARG;
-    if (!ctx->pending.active || ctx->pending.probed)
-        return fail(ctx, GPSB200_ERR_ARG, "gpsb200_slice_probe: call gpsb200_slice_prepare first");
-    CU(cudaSetDevice(ctx->cfg.device));
-    const int nblk = ctx->pending.nblk, nchan = ctx->pending.nchan;
-    const double t0 = now_ms();
-    finalize_guesses(ctx, 0, nblk, nchan, prn_in, phase_guess_in);
-    ctx->pending.st.host_chain_ms += now_ms() - t0;
-    int rc = GPSB200_OK, iseg = 0;
-    ctx->pending.eager = eager != 0;
-    const auto segs = segments_of(nblk);
-    if (ctx->pending.eager) {
-        // everything speculative at once: ONE probe and ONE chaining launch over the whole slice (no per-segment tails)
-        SynthArgs a{};
-        fill_args(ctx, a, 0, nblk, nchan, ctx->pending.sample_size, nullptr);
-        rc = segment_probe(ctx, 0, nblk, nchan, ctx->s_pre, ctx->pending.st, true, a);
-        for (size_t i = 0; !rc && i < segs.size(); i++)
-            if (cudaEventRecord(ctx->ev_seg[i], ctx->s_pre) != cudaSuccess) rc = fail(ctx, GPSB200_ERR_CUDA, "cudaEventRecord");
-    } else {
-        // only the first segment's; the others follow one by one in gpsb200_slice_finish
-        SynthArgs a{};
-        fill_args(ctx, a, segs[0].first, segs[0].second - segs[0].first, nchan, ctx->pending.sample_size, nullptr);
-        rc = segment_probe(ctx, segs[0].first, segs[0].second, nchan, ctx->s_pre, ctx->pending.st, true, a);
-        if (!rc && cudaEventRecord(ctx->ev_seg[iseg++], ctx->s_pre) != cudaSuccess) rc = fail(ctx, GPSB200_ERR_CUDA, "cudaEventRecord");
-    }
-    if (rc) {
-        drain(ctx, ctx->pending.stream);
-        ctx->pending.active = false;
-        return rc;
-    }
-    ctx->pending.probed = true;
-    return GPSB200_OK;
+    cudaStream_t s = ctx->call.active ? ctx->call.stream : nullptr;
+    return settle(ctx, s, slice_probe(ctx, prn_in, phase_guess_in, eager));
 }
-
-namespace {
-int slice_finish_inner(gpsb200_ctx *ctx, std::vector<ChainState> &chain, gpsb200_stats_t &st, int32_t *prn_out,
-                       double *phase_out, gpsb200_handoff_fn handoff, void *user) {
-    const int nblk = ctx->pending.nblk, nchan = ctx->pending.nchan, sample_size = ctx->pending.sample_size;
-    const size_t blk_bytes = (size_t) GPSB200_BLOCK_ELEMS * sample_size;
-    cudaStream_t s = ctx->pending.stream, sk = ctx->s_ck;
-    const auto segs = segments_of(nblk);
-    std::vector<int64_t> slow(segs.size(), 0);
-    std::vector<std::vector<ChainState>> after(segs.size());
-    ctx->trace_t0 = now_ms();
-    trace(ctx, "slice_finish");
-    if (ctx->pending.eager) {
-        // A successor waits for the outgoing state: scan EVERYTHING first (all probes were submitted up front), hand
-        // the exact state on, and only then enqueue the long kernels -- a message sent behind them would wait for them.
-        for (size_t i = 0; i < segs.size(); i++) {
-            if (i == 0) {
-                CU(cudaEventSynchronize(ctx->ev_seg[0]));
-                trace(ctx, "probes complete");
-            }
-            int rc = segment_scan(ctx, segs[i].first, segs[i].second, nchan, ctx->ev_seg[i], sk, chain, st, slow[i]);
-            if (rc) return rc;
-            after[i] = chain;
-        }
-        trace(ctx, "host scan done");
-        export_chain(chain, nchan, prn_out, phase_out);
-        if (handoff) handoff(user, prn_out, phase_out);
-        trace(ctx, "handed over");
-    }
-    int iseg = 0, ichunk = 0;
-    for (size_t i = 0; i < segs.size(); i++) {
-        const int b0 = segs[i].first, b1 = segs[i].second;
-        SynthArgs a{};
-        fill_args(ctx, a, b0, b1 - b0, nchan, sample_size, (char *) ctx->pending.dst + (size_t) b0 * blk_bytes);
-        int rc;
-        if (!ctx->pending.eager) {
-            // lazy: host scan of this segment as soon as ITS probes are done; checkpoints on a stream of their own
-            rc = segment_scan(ctx, b0, b1, nchan, ctx->ev_seg[iseg], sk, chain, st, slow[i]);
-            if (rc) return rc;
-        }
-        ctx->cur_seg = iseg;
-        rc = segment_checkpoints(ctx, b0, b1, nchan, sk, st, b0 == 0, a, slow[i]);
-        if (rc) return rc;
-        note_segment_end(ctx, iseg++, b1, nchan, ctx->pending.eager ? after[i] : chain);
-        CU(cudaEventRecord(ctx->ev_done[ichunk], sk));
-        CU(cudaStreamWaitEvent(s, ctx->ev_done[ichunk], 0));
-        ichunk++;
-        if (ctx->pending.dst_host) {
-            rc = synth_chunks(ctx, b0, b1, nchan, sample_size, ctx->pending.dst, ctx->pending.dst_host, s, st, ichunk);
-            if (rc) return rc;
-        } else {
-            CU(launch_synth(a, s));
-            st.launches += 1;
-        }
-        if (!ctx->pending.eager && b1 < nblk) {
-            // lazy: the next segment's speculative work is submitted only now, BEHIND this segment's synthesis, from
-            // guesses re-anchored on the exact state just resolved
-            const int n1 = std::min(nblk, b1 + kSegBlocks);
-            reanchor_guesses(ctx, b1, n1, nchan, chain);
-            SynthArgs an{};
-            fill_args(ctx, an, b1, n1 - b1, nchan, sample_size, nullptr);
-            rc = segment_probe(ctx, b1, n1, nchan, ctx->s_pre, st, false, an);
-            if (rc) return rc;
-            CU(cudaEventRecord(ctx->ev_seg[iseg], ctx->s_pre));
-        }
-    }
-    if (!ctx->pending.eager) {
-        export_chain(chain, nchan, prn_out, phase_out);
-        if (handoff) handoff(user, prn_out, phase_out);
-    }
-    ctx->pending.nseg = iseg;
-    CU(cudaEventRecord(ctx->ev[5], s));
-    CU(cudaMemcpyAsync(ctx->h_chain_errors, ctx->d_chain_errors, sizeof(int), cudaMemcpyDeviceToHost, sk));
-    trace(ctx, "checkpoints + synthesis enqueued");
-    return GPSB200_OK;
-}
-}  // namespace
 
 int gpsb200_slice_finish_cb(gpsb200_ctx_t *ctx, const int32_t *prn_in, const double *phase_in, int32_t *prn_out,
                             double *phase_out, gpsb200_stats_t *stats, gpsb200_handoff_fn handoff, void *user) {
     if (!ctx) return GPSB200_ERR_ARG;
-    if (!ctx->pending.active || !ctx->pending.probed)
-        return fail(ctx, GPSB200_ERR_ARG, "gpsb200_slice_finish: call gpsb200_slice_prepare and gpsb200_slice_probe first");
-    CU(cudaSetDevice(ctx->cfg.device));
-    const int nblk = ctx->pending.nblk, nchan = ctx->pending.nchan;
-    ctx->pending.active = false;
-    std::vector<ChainState> chain(nchan);
-    seed_chain(chain, nchan, prn_in, phase_in);
-    gpsb200_stats_t st = ctx->pending.st;
-    std::vector<int32_t> po(nchan, 0);
-    std::vector<double> xo(nchan, 0.0);
-    const int rc = slice_finish_inner(ctx, chain, st, po.data(), xo.data(), handoff, user);
-    if (rc) {
-        drain(ctx, ctx->pending.stream);
-        return rc;
-    }
-    SynthArgs all{};
-    fill_args(ctx, all, 0, nblk, nchan, ctx->pending.sample_size, ctx->pending.dst);
-    ctx->last = all;
-    ctx->have_last = true;
-    ctx->pending.finished = true;
-    for (int c = 0; c < nchan; c++) {
-        if (prn_out) prn_out[c] = po[c];
-        if (phase_out) phase_out[c] = xo[c];
-    }
-    if (stats) *stats = st;
-    return GPSB200_OK;
+    cudaStream_t s = ctx->call.active ? ctx->call.stream : nullptr;
+    return settle(ctx, s, slice_finish(ctx, prn_in, phase_in, prn_out, phase_out, stats, handoff, user));
 }
 
 int gpsb200_slice_finish(gpsb200_ctx_t *ctx, const int32_t *prn_in, const double *phase_in, int32_t *prn_out,
@@ -1452,22 +1442,22 @@ int gpsb200_slice_wait(gpsb200_ctx_t *ctx) {
     CU(cudaSetDevice(ctx->cfg.device));
     CU(cudaStreamSynchronize(ctx->s_pre));
     CU(cudaStreamSynchronize(ctx->s_ck));
-    if (ctx->pending.stream) CU(cudaStreamSynchronize(ctx->pending.stream));
+    if (ctx->call.stream) CU(cudaStreamSynchronize(ctx->call.stream));
     CU(cudaStreamSynchronize(ctx->s_copy));
-    if (ctx->pending.finished) {
-        ctx->pending.finished = false;
-        return verify_chain(ctx, ctx->pending.nseg, ctx->pending.nchan);
+    if (ctx->call.finished) {
+        ctx->call.finished = false;
+        return call_verdict(ctx, ctx->call);
     }
     return GPSB200_OK;
 }
 
 int gpsb200_slice_link_host(const gpsb200_chan_t *chans, int nblk, int nchan, gpsb200_slice_link_t *link) {
-    // the link of a slice from its parameters alone (what gpsb200_slice_prepare also returns); no device involved
+    // the link of a slice from its parameters alone (what prepare_blocks fills in relative mode); no device involved
     if (!chans || !link || nblk < 1 || nchan < 1 || nchan > GPSB200_MAX_CHAN) return GPSB200_ERR_ARG;
     const double delt = 1.0 / (double) GPSB200_SAMPLERATE;
     memset(link, 0, sizeof *link);
     for (int c = 0; c < nchan; c++) {
-        long double acc = 0.0L;
+        uint64_t acc = 0;
         int prev = chans[c].prn;
         bool absolute = false;
         link->prn_first[c] = prev;
@@ -1480,18 +1470,15 @@ int gpsb200_slice_link_host(const gpsb200_chan_t *chans, int nblk, int nchan, gp
                 continue;
             }
             if (in.prn != prev) {
-                acc = in.carr_phase;
+                acc = phase_to_fix(in.carr_phase);
                 absolute = true;
             }
             prev = in.prn;
-            const double cc = in.f_carr * delt;
-            acc += (long double) GPSB200_BLOCK_SAMPLES * ((long double) cc + (long double) carrier_drift_per_step(cc));
-            acc -= floorl(acc);
+            acc = guess_block(acc, in.f_carr * delt);
         }
         link->prn_last[c] = prev > 0 ? prev : 0;
         link->reset_inside[c] = absolute ? 1 : 0;
-        const double g = (double) acc;
-        link->value[c] = (g >= 0.0 && g < 1.0) ? g : 0.0;
+        link->value[c] = fix_to_phase(acc);
     }
     return GPSB200_OK;
 }
@@ -1559,36 +1546,7 @@ int gpsb200_debug_block_probes(gpsb200_ctx_t *ctx, int nblk, int nchan, void *pr
 int gpsb200_carrier_chain_device(gpsb200_ctx_t *ctx, const gpsb200_chan_t *chans, int nblk, int nchan,
                                  const double *phase_in, double *phase_out) {
     if (!ctx || !chans || !phase_out || nblk < 0 || nchan < 1 || nchan > ctx->cfg.max_chan) return GPSB200_ERR_ARG;
-    if (!ctx->s_compute) return fail(ctx, GPSB200_ERR_CUDA, "context has no CUDA device");
-    if (ctx->pending.active) return fail(ctx, GPSB200_ERR_ARG, "a call begun with gpsb200_synth_begin has not been finished");
-    CU(cudaSetDevice(ctx->cfg.device));
-    cudaStream_t s = ctx->s_compute;
-    std::vector<ChainState> chain(nchan);
-    if (phase_in && nblk > 0)
-        for (int c = 0; c < nchan; c++)
-            if (chans[c].prn > 0) {
-                chain[c].prn = chans[c].prn;
-                chain[c].phase = phase_in[c];
-            }
-    for (int w0 = 0; w0 < nblk; w0 += ctx->cfg.max_blocks) {
-        const int nw = std::min(ctx->cfg.max_blocks, nblk - w0);
-        const gpsb200_chan_t *cw = chans + (size_t) w0 * nchan;
-        int rc = prepare_blocks(ctx, cw, 0, nw, nchan, chain);
-        if (rc) return rc;
-        const size_t cnt = (size_t) nw * nchan;
-        CU(cudaMemcpyAsync(ctx->d_bc, ctx->h_bc, cnt * sizeof(BlockChanDev), cudaMemcpyHostToDevice, s));
-        CU(cudaMemcpyAsync(ctx->d_guess, ctx->h_guess, cnt * sizeof(double), cudaMemcpyHostToDevice, s));
-        SynthArgs a{};
-        fill_args(ctx, a, 0, nw, nchan, GPSB200_SC08, nullptr);
-        a.ck = nullptr;                                // no run checkpoints: the probes need no code walk
-        CU(launch_probe(a, s));
-        CU(launch_chain(a, s));
-        CU(cudaStreamSynchronize(s));
-        resolve_chain(ctx, 0, nw, nchan, chain, nullptr);
-    }
-    ctx->have_last = false;
-    for (int c = 0; c < nchan; c++) phase_out[c] = chain[c].prn > 0 ? chain[c].phase : 0.0;
-    return GPSB200_OK;
+    return settle(ctx, nullptr, carrier_chain_device(ctx, chans, nblk, nchan, phase_in, phase_out));
 }
 
 int gpsb200_replay_device(gpsb200_ctx_t *ctx, void *dst_device, void *stream_, int kernel_mask) {
@@ -1612,22 +1570,13 @@ int gpsb200_replay_device(gpsb200_ctx_t *ctx, void *dst_device, void *stream_, i
 int gpsb200_synth_blocks_scatter(gpsb200_ctx_t *ctx, const gpsb200_chan_t *chans, int nblk, int nchan, int sample_size,
                                  void *const *dst_blocks, double *carr_phase_out, gpsb200_stats_t *stats) {
     if (!ctx || !dst_blocks) return GPSB200_ERR_ARG;
-    for (int b = 0; b < nblk; b++)
-        if (!dst_blocks[b]) return fail(ctx, GPSB200_ERR_ARG, "gpsb200_synth_blocks_scatter: NULL block destination");
-    ctx->scatter = dst_blocks;
-    const int rc = gpsb200_synth_blocks(ctx, chans, nblk, nchan, sample_size, dst_blocks[0], carr_phase_out, stats);
-    ctx->scatter = nullptr;
-    return rc;
+    return settle(ctx, nullptr, synth_host(ctx, chans, nblk, nchan, sample_size, nullptr, dst_blocks, carr_phase_out, stats));
 }
 
 int gpsb200_synth_blocks(gpsb200_ctx_t *ctx, const gpsb200_chan_t *chans, int nblk, int nchan, int sample_size,
                          void *dst, double *carr_phase_out, gpsb200_stats_t *stats) {
-    int rc = check_call(ctx, chans, nblk, nchan, sample_size, dst);
-    if (rc) return rc;
-    rc = ensure_staging(ctx, sample_size);
-    if (rc) return rc;
-    return run_pipeline(ctx, chans, nblk, nchan, sample_size, ctx->d_out, dst, ctx->s_compute, nullptr, nullptr, nullptr,
-                        carr_phase_out, stats);
+    if (!ctx) return GPSB200_ERR_ARG;
+    return settle(ctx, nullptr, synth_host(ctx, chans, nblk, nchan, sample_size, dst, nullptr, carr_phase_out, stats));
 }
 
 }  // extern "C"
