@@ -291,6 +291,59 @@ int gpsb200_lanes_model_block(const gpsb200_chan_t *chans, int nchan, const uint
 /* C/A code of prn (1..32) as 0/1 chips (codegen, gps.c:272-309). */
 int gpsb200_codegen(int prn, uint8_t ca[GPSB200_CA_LEN]);
 
+/* ---- acquisition search: which satellites does an I/Q stream contain? ------------------------------------------------
+ * The first step of a GPS receiver, for interleaved I/Q at 3 Msps (one C/A period = 3000 samples): for each requested PRN
+ * a search over code delay tau (0..2999 samples) x Doppler bin j (f_j = f_lo_hz + j * step_hz), over K coherent 1 ms
+ * periods summed non-coherently. Not a receiver: no tracking, bit sync or navigation solution. Exact integer
+ * arithmetic, deterministic (DESIGN §9; tests/acq_model.py states it in numpy):
+ *   samples    int8 as is; int16 reduced to clamp(x >> 4, -128, 127) (the int8 stream's scale, saturated where the int8
+ *              stream wraps)
+ *   window     samples s0 .. s0 + 3000 K + 2998 (3000 K + 2999 of them) of a buffer of nsamples; m = sample - s0
+ *   carrier    u_j = (uint32) llround(f_j * 2^32 / 3e6), phase (uint32)(m * u_j), index phase >> 23 into the
+ *              synthesizer's 512-entry cos/sin tables (|entry| <= 250)
+ *   wipe-off   I_d = I cos + Q sin, Q_d = Q cos - I sin (int32, |.| <= 64000): the stream's e^{+j phi} is removed, so the
+ *              peak is at f_j ~ f_carr of the channel record
+ *   replica    c_p[n] = 2 ca_p[(n * 1023) / 3000] - 1, n < 3000 (ca_p: gpsb200_codegen)
+ *   correlate  C_I(k, tau) = sum_{n<3000} c_p[n] I_d[3000 k + tau + n], C_Q likewise (int32, |.| <= 1.92e8)
+ *   power      P(j, tau) = sum_{k<K} C_I^2 + C_Q^2 (uint64, <= K * 7.4e16: hence K <= 100)
+ *   result     (j1, tau1) = argmax P, ties to the lowest j, then the lowest tau; p1 = P(j1, tau1); p2 = the largest
+ *              P(j1, tau) with circular distance |tau - tau1| (period 3000) > 3 samples, outside the +-1-chip
+ *              correlation triangle; ratio = p1 / p2 (infinity when p2 is 0). */
+#define GPSB200_ACQ_MAX_MS    100
+#define GPSB200_ACQ_MAX_BINS  1024
+#define GPSB200_ACQ_CODE_SAMPLES 3000
+typedef struct gpsb200_acq_config {
+    int64_t s0;            /* first sample of the window (sample = one I,Q pair) */
+    int32_t ms;            /* K, coherent 1 ms periods: 1..GPSB200_ACQ_MAX_MS */
+    int32_t nprn;          /* 1..32 entries of prn[] */
+    int32_t prn[32];       /* 1..32 each */
+    double f_lo_hz;        /* first Doppler bin */
+    double step_hz;        /* bin spacing (> 0 when nbins > 1); every bin within +-1.5 MHz */
+    int32_t nbins;         /* 1..GPSB200_ACQ_MAX_BINS */
+    int32_t reserved;
+} gpsb200_acq_config_t;    /* 168 bytes */
+typedef struct gpsb200_acq_result {
+    int32_t prn;
+    int32_t bin;           /* j1 */
+    int32_t delay;         /* tau1: samples from s0 to where the code's chip 0 starts, modulo 3000 */
+    int32_t reserved;
+    double doppler_hz;     /* f_j1 */
+    double delay_chips;    /* tau1 * 1023 / 3000 */
+    uint64_t p1, p2;
+    double ratio;          /* p1 / p2: a receiver counts the PRN as acquired above a threshold (gpsb200-acq: 2.5) */
+} gpsb200_acq_result_t;    /* 56 bytes */
+/* Search nsamples samples of host memory (int8 or int16 I,Q interleaved, sample_size GPSB200_SC08 / GPSB200_SC16); only
+ * the window is copied to the device. res: [cfg->nprn] in the order of cfg->prn. grid (NULL: not wanted): host
+ * [nprn][nbins][3000] uint64, the whole P. Every argument is checked before anything is enqueued (GPSB200_ERR_ARG).
+ * Blocking; scratch is allocated on the context's device as needed. */
+int gpsb200_acquire(gpsb200_ctx_t *ctx, const void *iq, int64_t nsamples, int sample_size, const gpsb200_acq_config_t *cfg,
+                    gpsb200_acq_result_t *res, uint64_t *grid);
+/* Same for a source in device memory (16-byte aligned, as gpsb200_synth_blocks_device's dst_device, else GPSB200_ERR_ARG),
+ * searched in place: the search is enqueued on `stream` (0 = the context's own stream) behind whatever it holds -- e.g.
+ * the synthesis of that buffer -- and the call returns when the results (and grid, in host memory) are in. */
+int gpsb200_acquire_device(gpsb200_ctx_t *ctx, const void *iq_device, int64_t nsamples, int sample_size,
+                           const gpsb200_acq_config_t *cfg, gpsb200_acq_result_t *res, uint64_t *grid, void *stream);
+
 /* ---- scenario engine: the reference's host path outside the sample loop -------------
  * RINEX-2/3 navigation file (plain or gzip-compressed, read through zlib like the reference, gps.c:1147) +
  * location/motion -> the gpsb200_chan_t records and NAV frames the

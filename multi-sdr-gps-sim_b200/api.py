@@ -101,6 +101,26 @@ class Stats(C.Structure):
                 ("chain_fallbacks", C.c_int32)]
 
 
+class AcqConfig(C.Structure):
+    """gpsb200_acq_config_t (168 bytes)."""
+    _fields_ = [("s0", C.c_int64), ("ms", C.c_int32), ("nprn", C.c_int32), ("prn", C.c_int32 * 32),
+                ("f_lo_hz", C.c_double), ("step_hz", C.c_double), ("nbins", C.c_int32), ("reserved", C.c_int32)]
+
+
+assert C.sizeof(AcqConfig) == 168
+
+# gpsb200_acq_result_t: one row per searched PRN
+ACQ_RESULT_DTYPE = np.dtype([("prn", "<i4"), ("bin", "<i4"), ("delay", "<i4"), ("reserved", "<i4"),
+                             ("doppler_hz", "<f8"), ("delay_chips", "<f8"), ("p1", "<u8"), ("p2", "<u8"), ("ratio", "<f8")])
+assert ACQ_RESULT_DTYPE.itemsize == 56
+ACQ_CODE_SAMPLES = 3000
+
+
+def acq_window_samples(ms):
+    """Samples an acquisition search over `ms` coherent 1 ms periods reads from s0 on: 3000 ms + 2999."""
+    return ACQ_CODE_SAMPLES * int(ms) + ACQ_CODE_SAMPLES - 1
+
+
 HANDOFF_FN = C.CFUNCTYPE(None, C.c_void_p, C.POINTER(C.c_int32), C.POINTER(C.c_double))     # gpsb200_handoff_fn
 
 _lib = None
@@ -108,7 +128,7 @@ _lib = None
 EXPORTS = ["gpsb200_create", "gpsb200_destroy", "gpsb200_last_error", "gpsb200_version", "gpsb200_set_nav",
            "gpsb200_synth_blocks", "gpsb200_synth_blocks_scatter", "gpsb200_synth_blocks_device", "gpsb200_replay_device",
            "gpsb200_carrier_advance", "gpsb200_carrier_chain", "gpsb200_carrier_chain_device", "gpsb200_carrier_probe_fixup",
-           "gpsb200_codegen", "gpsb200_bind_numa", "gpsb200_span_chain_host", "gpsb200_lanes_model_block", "gpsb200_slice_prepare", "gpsb200_slice_probe",
+           "gpsb200_codegen", "gpsb200_acquire", "gpsb200_acquire_device", "gpsb200_bind_numa", "gpsb200_span_chain_host", "gpsb200_lanes_model_block", "gpsb200_slice_prepare", "gpsb200_slice_probe",
            "gpsb200_slice_finish", "gpsb200_slice_finish_cb", "gpsb200_slice_wait", "gpsb200_link_apply", "gpsb200_slice_link_host", "gpsb200_debug_corrupt_chain", "gpsb200_synth_kernel_name",
            "gpsb200_debug_run_checkpoints", "gpsb200_checkpoint_segments_host",
            "gpsb200_carrier_probe_host", "gpsb200_debug_block_probes",
@@ -191,6 +211,10 @@ def lib():
         L.gpsb200_debug_block_probes.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
         L.gpsb200_synth_kernel_name.argtypes = [C.c_void_p, C.c_int]
         L.gpsb200_synth_kernel_name.restype = C.c_char_p
+        L.gpsb200_acquire.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.POINTER(AcqConfig), C.c_void_p,
+                                      C.c_void_p]
+        L.gpsb200_acquire_device.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.POINTER(AcqConfig),
+                                             C.c_void_p, C.c_void_p, C.c_void_p]
         _lib = L
     return _lib
 
@@ -641,6 +665,36 @@ class Context:
         self._check(lib().gpsb200_carrier_chain_device(self._h, a.ctypes.data, nblk, nchan,
                                                        None if pin is None else pin.ctypes.data, out.ctypes.data))
         return out
+
+    def acquire(self, iq=None, sample_size=SC08, prns=range(1, 33), ms=10, s0=0, f_lo=-5000.0, step=250.0, nbins=41,
+                want_grid=False, device_ptr=None, nsamples=None, stream=0):
+        """GPS L1 C/A acquisition search (gpsb200_acquire; DESIGN §9) over code delay x Doppler bin f_lo + j * step,
+        `ms` coherent 1 ms periods from sample s0, for each PRN of `prns`.
+        Source: iq, a numpy array of interleaved I,Q (int8 for SC08, int16 for SC16), or device_ptr (a raw 16-byte
+        aligned device pointer, e.g. the buffer synth_blocks_device filled) holding nsamples samples, searched in place
+        on `stream` behind the work it holds.
+        -> results ACQ_RESULT_DTYPE[nprn] (prn, bin, delay, doppler_hz, delay_chips, p1, p2, ratio), and with want_grid
+        also the whole power grid uint64[nprn, nbins, 3000]."""
+        prns = [int(p) for p in prns]
+        cfg = AcqConfig()
+        cfg.s0, cfg.ms, cfg.nprn = int(s0), int(ms), len(prns)
+        for i, p in enumerate(prns[:32]):   # more than 32 is rejected by the library with the other argument checks
+            cfg.prn[i] = p
+        cfg.f_lo_hz, cfg.step_hz, cfg.nbins = float(f_lo), float(step), int(nbins)
+        res = np.zeros(max(1, min(len(prns), 32)), ACQ_RESULT_DTYPE)
+        grid = np.zeros((max(1, len(prns)), max(1, int(nbins)), ACQ_CODE_SAMPLES), np.uint64) if want_grid else None
+        gp = None if grid is None else grid.ctypes.data
+        if device_ptr is not None:
+            assert iq is None and nsamples is not None
+            rc = lib().gpsb200_acquire_device(self._h, C.c_void_p(device_ptr), int(nsamples), int(sample_size), C.byref(cfg),
+                                              res.ctypes.data, gp, C.c_void_p(stream))
+        else:
+            a = np.ascontiguousarray(iq)
+            n = a.size // 2 if nsamples is None else int(nsamples)
+            assert n <= a.size // 2
+            rc = lib().gpsb200_acquire(self._h, a.ctypes.data, n, int(sample_size), C.byref(cfg), res.ctypes.data, gp)
+        self._check(rc)
+        return (res, grid) if want_grid else res
 
     def replay_device(self, dst_ptr=0, stream=0, kernel_mask=15):
         self._check(lib().gpsb200_replay_device(self._h, C.c_void_p(dst_ptr), C.c_void_p(stream), kernel_mask))

@@ -1,0 +1,53 @@
+// GPS L1 C/A acquisition search at 3 Msps (include/gpsb200.h: gpsb200_acquire): C/A code delay x Doppler grid over K
+// coherent 1 ms periods, non-coherently summed, reduced per PRN. Exact integer arithmetic (DESIGN §9, tests/acq_model.py).
+#pragma once
+#include <cuda_runtime.h>
+#include <stdint.h>
+
+#include <string>
+
+#include "../../include/gpsb200.h"
+
+namespace gpsb200 {
+namespace acq {
+
+constexpr int kCode = 3000;                    // samples per C/A period at 3 Msps
+constexpr int kThreads = 256;                  // threads of k_acq_grid
+constexpr int kTausPerThread = 12;             // delays per thread: 256 x 12 = 3072 >= 3000 (the last 72 are discarded)
+constexpr int kTaus = kThreads * kTausPerThread;
+constexpr int kPrefix = 6144;                  // prefix sums S[0..6144] of one window (needs 3072 + 3000 - 1 <= 6143)
+constexpr int kMaxEdges = 1024;                // sign changes of a sampled C/A replica (<= 1022), padded to a multiple of 8
+constexpr int kExclude = 3;                    // P2 excludes delays within +-3 samples (one chip) of the peak
+
+// Device scratch of the searches of one context, grown as needed.
+struct Scratch {
+    int16_t *d_edges = nullptr;        // [33][kMaxEdges] sign-change positions of every PRN's replica, row 0 unused
+    int32_t *d_nedges = nullptr;       // [33]
+    void *d_window = nullptr;          // the searched samples of a host source
+    size_t window_bytes = 0;
+    uint64_t *d_grid = nullptr;        // [nprn][nbins][3000] when the caller wants the grid
+    size_t grid_bytes = 0;
+    uint64_t *d_rows = nullptr;        // [nprn][nbins][3]: P1, P2, tau1 of every row
+    gpsb200_acq_result_t *d_res = nullptr, *h_res = nullptr;   // [32]
+    uint32_t *d_u = nullptr;           // [nbins] phase steps
+    int32_t *d_prn = nullptr;          // [32]
+    int max_bins = 0;
+};
+
+// Empty when the search is well-formed: PRNs 1..32, 1 <= K <= 100, 1 <= nbins <= GPSB200_ACQ_MAX_BINS, every bin within
+// +-1.5 MHz, sample size SC08/SC16, a window [s0, s0 + 3000 K + 2999) inside a buffer of nsamples samples.
+std::string check(const gpsb200_acq_config_t *cfg, int64_t nsamples, int sample_size);
+// Samples the search reads from s0 on: 3000 K + 2999.
+int64_t window_samples(const gpsb200_acq_config_t *cfg);
+// Phase step of bin j: (uint32) llround(f_j * 2^32 / 3e6).
+uint32_t phase_step(double f_hz);
+
+cudaError_t scratch_reserve(Scratch &sc, const gpsb200_acq_config_t *cfg, bool want_grid);
+void scratch_free(Scratch &sc);
+// Enqueue the search of the samples at `window` (the first sample is s0) on s; results land in sc.h_res after a
+// synchronize of s, the grid (want_grid) in sc.d_grid.
+cudaError_t launch(Scratch &sc, const void *window, int sample_size, const gpsb200_acq_config_t *cfg, bool want_grid,
+                   cudaStream_t s);
+
+}  // namespace acq
+}  // namespace gpsb200

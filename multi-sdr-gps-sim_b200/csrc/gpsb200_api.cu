@@ -28,6 +28,7 @@
 #include <vector>
 
 #include "../../include/gpsb200.h"
+#include "acquire.h"
 #include "nco_exact.h"
 #include "synth_kernels.h"
 #include "synth_lanes.h"
@@ -205,6 +206,7 @@ struct gpsb200_ctx {
     std::unique_ptr<WorkerPool> pool;      // host passes (guesses, fix-up scan)
     SynthArgs last{};                      // replay state
     bool have_last = false;
+    acq::Scratch acq;                      // acquisition searches (acquire.cu), allocated by the first one
     std::string err;
 };
 
@@ -1076,6 +1078,43 @@ int carrier_chain_device(gpsb200_ctx *ctx, const gpsb200_chan_t *chans, int nblk
     return GPSB200_OK;
 }
 
+
+// The acquisition search of both entry points (acquire.cu). Everything is checked before anything is enqueued; a device
+// source is searched in place on the caller's stream, a host source's window is copied up first.
+int acquire(gpsb200_ctx *ctx, const void *iq, int64_t nsamples, int sample_size, const gpsb200_acq_config_t *cfg,
+            gpsb200_acq_result_t *res, uint64_t *grid, bool device, cudaStream_t s) {
+    if (!iq || !res) return fail(ctx, GPSB200_ERR_ARG, "gpsb200_acquire: NULL source or result array");
+    const std::string bad = acq::check(cfg, nsamples, sample_size);
+    if (!bad.empty()) return fail(ctx, GPSB200_ERR_ARG, "gpsb200_acquire: " + bad);
+    if (device && (reinterpret_cast<uintptr_t>(iq) & 15u) != 0)
+        return fail(ctx, GPSB200_ERR_ARG, "gpsb200_acquire_device: iq_device is not 16-byte aligned");
+    if (!ctx->s_compute) return fail(ctx, GPSB200_ERR_CUDA, "context has no CUDA device");
+    if (ctx->call.active) return fail(ctx, GPSB200_ERR_ARG, "a call begun with gpsb200_slice_prepare has not been finished");
+    CU(cudaSetDevice(ctx->cfg.device));
+    CU(acq::scratch_reserve(ctx->acq, cfg, grid != nullptr));
+    const size_t elem = sample_size == GPSB200_SC16 ? 2 : 1;
+    const char *src = static_cast<const char *>(iq) + (size_t) cfg->s0 * 2 * elem;
+    const void *window = src;
+    if (!device) {
+        const size_t wb = (size_t) acq::window_samples(cfg) * 2 * elem;
+        if (wb > ctx->acq.window_bytes) {
+            cudaFree(ctx->acq.d_window);
+            ctx->acq.d_window = nullptr;
+            ctx->acq.window_bytes = 0;
+            CU(cudaMalloc(&ctx->acq.d_window, wb));
+            ctx->acq.window_bytes = wb;
+        }
+        CU(cudaMemcpyAsync(ctx->acq.d_window, src, wb, cudaMemcpyHostToDevice, s));
+        window = ctx->acq.d_window;
+    }
+    CU(acq::launch(ctx->acq, window, sample_size, cfg, grid != nullptr, s));
+    if (grid)
+        CU(cudaMemcpy(grid, ctx->acq.d_grid, (size_t) cfg->nprn * cfg->nbins * acq::kCode * sizeof(uint64_t),
+                      cudaMemcpyDeviceToHost));
+    memcpy(res, ctx->acq.h_res, (size_t) cfg->nprn * sizeof(gpsb200_acq_result_t));
+    return GPSB200_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -1381,6 +1420,7 @@ void gpsb200_destroy(gpsb200_ctx_t *ctx) {
     for (auto &e : ctx->ev_seg)
         if (e) cudaEventDestroy(e);
     cudaFreeHost(ctx->h_seg_end);
+    acq::scratch_free(ctx->acq);
     if (ctx->s_compute) cudaStreamDestroy(ctx->s_compute);
     if (ctx->s_copy) cudaStreamDestroy(ctx->s_copy);
     if (ctx->s_pre) cudaStreamDestroy(ctx->s_pre);
@@ -1577,6 +1617,19 @@ int gpsb200_synth_blocks(gpsb200_ctx_t *ctx, const gpsb200_chan_t *chans, int nb
                          void *dst, double *carr_phase_out, gpsb200_stats_t *stats) {
     if (!ctx) return GPSB200_ERR_ARG;
     return settle(ctx, nullptr, synth_host(ctx, chans, nblk, nchan, sample_size, dst, nullptr, carr_phase_out, stats));
+}
+
+int gpsb200_acquire(gpsb200_ctx_t *ctx, const void *iq, int64_t nsamples, int sample_size, const gpsb200_acq_config_t *cfg,
+                    gpsb200_acq_result_t *res, uint64_t *grid) {
+    if (!ctx) return GPSB200_ERR_ARG;
+    return settle(ctx, nullptr, acquire(ctx, iq, nsamples, sample_size, cfg, res, grid, false, ctx->s_compute));
+}
+
+int gpsb200_acquire_device(gpsb200_ctx_t *ctx, const void *iq_device, int64_t nsamples, int sample_size,
+                           const gpsb200_acq_config_t *cfg, gpsb200_acq_result_t *res, uint64_t *grid, void *stream_) {
+    if (!ctx) return GPSB200_ERR_ARG;
+    cudaStream_t s = stream_ ? (cudaStream_t) stream_ : ctx->s_compute;
+    return settle(ctx, s, acquire(ctx, iq_device, nsamples, sample_size, cfg, res, grid, true, s));
 }
 
 }  // extern "C"
