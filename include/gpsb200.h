@@ -288,6 +288,12 @@ int gpsb200_carrier_probe_host(double guess, double f_carr, int64_t nsamples, in
 int gpsb200_lanes_model_block(const gpsb200_chan_t *chans, int nchan, const uint32_t *nav, int run_samples, int force,
                               int16_t *iq, double *carr_out, int64_t *counters, uint32_t *signs);
 
+/* The window band certification of the lane = sample synthesis (csrc/synth_lanes.h), for n (step, base) pairs: out[i] = 1
+ * when some sample m < 96 of a window with 32-bit carrier phase base bases[i] and increment steps[i] has a phase
+ * bases[i] + m * steps[i] (mod 2^32) whose low 23 bits are 2^23 - 128 or more, else 0; what the kernel decides per
+ * (channel, window) from the sorted residues of the step. Consecutive equal steps share one residue list. For tests. */
+int gpsb200_lanes_window_band_host(const uint32_t *steps, const uint32_t *bases, int64_t n, uint8_t *out);
+
 /* C/A code of prn (1..32) as 0/1 chips (codegen, gps.c:272-309). */
 int gpsb200_codegen(int prn, uint8_t ca[GPSB200_CA_LEN]);
 

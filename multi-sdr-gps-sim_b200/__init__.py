@@ -9,7 +9,7 @@ Import it with importlib (the directory name is not a Python identifier):
 """
 from .api import (  # noqa: F401
     BLOCK_ELEMS, BLOCK_SAMPLES, SC08, SC16, Chan, Config, Context, GpsB200Error, Stats,
-    bind_numa, carrier_advance, span_chain_host, lanes_model_block, link_apply, slice_link_host, SliceLink, carrier_chain, codegen, scenario, lib, lib_path, CHAN_DTYPE,
+    bind_numa, carrier_advance, span_chain_host, lanes_model_block, lanes_window_band, link_apply, slice_link_host, SliceLink, carrier_chain, codegen, scenario, lib, lib_path, CHAN_DTYPE,
     ScenarioConfig, LiveScenario, SteerState, parse_steer, KEYS, ERR_END, almanac_read, ALMANAC_RECORD_DTYPE, checkpoint_segments_host, RUN_CKPT_DTYPE,
     carrier_probe_host, CARRIER_PROBE_DTYPE, AcqConfig, ACQ_RESULT_DTYPE, ACQ_CODE_SAMPLES, acq_window_samples,
 )

@@ -128,7 +128,8 @@ _lib = None
 EXPORTS = ["gpsb200_create", "gpsb200_destroy", "gpsb200_last_error", "gpsb200_version", "gpsb200_set_nav",
            "gpsb200_synth_blocks", "gpsb200_synth_blocks_scatter", "gpsb200_synth_blocks_device", "gpsb200_replay_device",
            "gpsb200_carrier_advance", "gpsb200_carrier_chain", "gpsb200_carrier_chain_device", "gpsb200_carrier_probe_fixup",
-           "gpsb200_codegen", "gpsb200_acquire", "gpsb200_acquire_device", "gpsb200_bind_numa", "gpsb200_span_chain_host", "gpsb200_lanes_model_block", "gpsb200_slice_prepare", "gpsb200_slice_probe",
+           "gpsb200_codegen", "gpsb200_acquire", "gpsb200_acquire_device", "gpsb200_bind_numa", "gpsb200_span_chain_host", "gpsb200_lanes_model_block",
+           "gpsb200_lanes_window_band_host", "gpsb200_slice_prepare", "gpsb200_slice_probe",
            "gpsb200_slice_finish", "gpsb200_slice_finish_cb", "gpsb200_slice_wait", "gpsb200_link_apply", "gpsb200_slice_link_host", "gpsb200_debug_corrupt_chain", "gpsb200_synth_kernel_name",
            "gpsb200_debug_run_checkpoints", "gpsb200_checkpoint_segments_host",
            "gpsb200_carrier_probe_host", "gpsb200_debug_block_probes",
@@ -270,6 +271,21 @@ def lanes_model_block(chans_row, nav_frame, run_samples=2400, force=0, want_sign
     if rc:
         raise GpsB200Error(rc, "gpsb200_lanes_model_block")
     return (iq, co, cnt, signs) if want_signs else (iq, co, cnt)
+
+
+def lanes_window_band(steps, bases):
+    """Window band certification of the lane = sample kernel for (step, base) pairs of uint32. -> bool array: some
+    sample m < 96 of the window has a phase base + m * step whose low 23 bits are 2^23 - 128 or more."""
+    st, bs = np.broadcast_arrays(np.asarray(steps, np.uint32), np.asarray(bases, np.uint32))
+    st = np.ascontiguousarray(st.ravel())
+    bs = np.ascontiguousarray(bs.ravel())
+    out = np.zeros(st.size, np.uint8)
+    L = lib()
+    L.gpsb200_lanes_window_band_host.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]
+    rc = L.gpsb200_lanes_window_band_host(st.ctypes.data, bs.ctypes.data, st.size, out.ctypes.data)
+    if rc:
+        raise GpsB200Error(rc, "gpsb200_lanes_window_band_host")
+    return out.astype(bool)
 
 
 def span_chain_host(f_carr, start_true, start_guess):

@@ -59,6 +59,11 @@ extern "C" int gpsb200_lanes_model_block(const gpsb200_chan_t *chans, int nchan,
     }
     std::vector<lanes::ChanRun> st(nchan);
     std::vector<lanes::Anchor> an(nchan);
+    // residue lists of the carrier steps, as each CTA of the kernel builds them
+    std::vector<std::vector<uint32_t>> band(nchan, std::vector<uint32_t>(lanes::kBandList));
+    for (int c = 0; c < nchan; c++)
+        lanes::band_residues(chans[c].prn > 0 ? (uint32_t) (lanes::carr_step_fix(chans[c].f_carr * delt) >> 32) : 0u,
+                             band[c].data());
     for (int r = 0; r < nruns; r++) {
         for (int c = 0; c < nchan; c++) {
             const uint32_t *nv = nav + (size_t) c * 60;
@@ -69,6 +74,7 @@ extern "C" int gpsb200_lanes_model_block(const gpsb200_chan_t *chans, int nchan,
         }
         for (int w = 0; w < nwin; w++) {
             std::vector<uint32_t> S(3 * nchan, 0), base(nchan, 0), step(nchan, 0);
+            std::vector<char> flagged(nchan, 0);        // the window has a fast_risky sample of the channel
             for (int c = 0; c < nchan; c++) {
                 if (!st[c].active) continue;
                 const uint32_t *nv = nav + (size_t) c * 60;
@@ -82,6 +88,7 @@ extern "C" int gpsb200_lanes_model_block(const gpsb200_chan_t *chans, int nchan,
                 }
                 base[c] = lanes::fast_base(st[c]);
                 step[c] = lanes::fast_step(st[c]);
+                flagged[c] = lanes::window_band_risky(band[c].data(), base[c]);
                 if (signs) {
                     const size_t win = (size_t) r * nwin + (size_t) w;
                     memcpy(signs + ((size_t) c * (GPSB200_BLOCK_SAMPLES / lanes::kWindow) + win) * 3, &S[3 * c], 3 * sizeof(uint32_t));
@@ -97,7 +104,7 @@ extern "C" int gpsb200_lanes_model_block(const gpsb200_chan_t *chans, int nchan,
                     if (!st[c].active) continue;
                     const uint32_t p = base[c] + (uint32_t) n * step[c];
                     int k = (int) (p >> 23);
-                    if (lanes::fast_risky(p) || (force & 1)) {
+                    if ((flagged[c] && lanes::fast_risky(p)) || (force & 1)) {
                         const uint64_t m = st[c].P + (uint64_t) n * st[c].D;
                         const uint64_t frac = m & ((1ull << 55) - 1);
                         if ((force & 4) || frac < lanes::kBandCarr || frac > (1ull << 55) - lanes::kBandCarr) ++cnt[3];
@@ -132,5 +139,15 @@ extern "C" int gpsb200_lanes_model_block(const gpsb200_chan_t *chans, int nchan,
     if (carr_out)
         for (int c = 0; c < nchan; c++) carr_out[c] = chans[c].prn > 0 ? x[c] : 0.0;
     if (counters) memcpy(counters, cnt, sizeof cnt);
+    return GPSB200_OK;
+}
+
+extern "C" int gpsb200_lanes_window_band_host(const uint32_t *steps, const uint32_t *bases, int64_t n, uint8_t *out) {
+    if (n < 0 || (n > 0 && (!steps || !bases || !out))) return GPSB200_ERR_ARG;
+    uint32_t R[lanes::kBandList];
+    for (int64_t i = 0; i < n; i++) {
+        if (i == 0 || steps[i] != steps[i - 1]) lanes::band_residues(steps[i], R);
+        out[i] = lanes::window_band_risky(R, bases[i]) ? 1 : 0;
+    }
     return GPSB200_OK;
 }

@@ -52,6 +52,7 @@ struct LanesSmem {
     alignas(16) LaneWin win[kLaneWarps][kWins][CH];     // per warp: the window(s) in flight
     alignas(16) uint32_t step[kLaneWarps][CH];          // per warp: 32-bit carrier increment per sample (fast_step)
     alignas(16) uint32_t stage[kLaneWarps][kWins * lanes::kWindow];   // packed output of the window(s)
+    uint32_t band[CH][lanes::kBandList + 1];            // band_residues() of each channel's step; rows skewed by one bank
 };
 template <int CH>
 constexpr size_t lanes_smem_bytes() { return sizeof(LanesSmem<CH>) + (size_t) CH * 2048 + 2048; }
@@ -111,6 +112,11 @@ __global__ void __launch_bounds__(kLaneWarps * 32, 2) k_synth_lanes(SynthArgs a)
             if (c < nchan && bc[c].prn > 0) v = a.nav[((size_t) bc[c].frame * a.nav_stride + c) * kNavWords + w];
             sm.nav[c][w] = v;
         }
+        // residue lists of the channels' steps (fast_step() of the run state), one lane per channel of the last warp
+        if (warp == kLaneWarps - 1 && lane < CH) {
+            const bool ok = lane < nchan && bc[lane].prn > 0;
+            lanes::band_residues(ok ? (uint32_t) (lanes::carr_step_fix(bc[lane].c_carr) >> 32) : 0u, &sm.band[lane][0]);
+        }
     }
     __syncthreads();
 
@@ -119,6 +125,7 @@ __global__ void __launch_bounds__(kLaneWarps * 32, 2) k_synth_lanes(SynthArgs a)
     const bool chan_ok = ch < nchan && bc[ch < nchan ? ch : 0].prn > 0;
     const uint32_t *nav_row = &sm.nav[ch][0];
     const uint32_t *chip_row = &sm.chips[ch][0];
+    const uint32_t *band_row = &sm.band[ch][0];
     auto navf = [nav_row](int iw) { return nav_row[iw]; };
     auto chipf = [chip_row](int i) { return chip_row[i]; };
     const uint32_t n0 = (uint32_t) lane, n1 = n0 + 32u, n2 = n0 + 64u;              // sample side: this lane's samples
@@ -149,14 +156,18 @@ __global__ void __launch_bounds__(kLaneWarps * 32, 2) k_synth_lanes(SynthArgs a)
 
 #pragma unroll 1
         for (int w = 0; w < nwin; w += WINS) {
+            uint32_t flagged;                           // bit half * CH + c: channel c has a fast_risky sample in window w + half
             {
                 uint32_t S[3] = {0u, 0u, 0u};
                 uint32_t base = (uint32_t) (ch * SWZ) << 23;                        // rotation of the channel's table
+                bool band = false;
                 if (chan_ok && w + half < nwin) {
-                    if (!lanes::window_signs(s, chipf, navf, S)) lanes::exact_signs(an, w + half, chipf, navf, S);
                     base += lanes::fast_base(s);
+                    band = lanes::window_band_risky(band_row, base);                 // the rotation keeps the low 23 bits
+                    if (!lanes::window_signs(s, chipf, navf, S)) lanes::exact_signs(an, w + half, chipf, navf, S);
                 }
                 *reinterpret_cast<uint4 *>(&sm.win[warp][half][ch]) = make_uint4(S[0], S[1], S[2], base);
+                flagged = __ballot_sync(kFull, band);
             }
             __syncwarp();
 
@@ -169,7 +180,6 @@ __global__ void __launch_bounds__(kLaneWarps * 32, 2) k_synth_lanes(SynthArgs a)
                 // is negative. The sample is all_j - 2 neg_j: table[k ^ 256] = -table[k] entry by entry, and the packed
                 // I + (Q << 16) sums are linear modulo 2^32.
                 int all0 = 0, all1 = 0, all2 = 0, neg0 = 0, neg1 = 0, neg2 = 0;
-                uint32_t dmax = 0u;
                 // Two channels per trip (an odd count is padded with the next slot, which is all zeros).
                 const LaneWin *wp = wrow;
                 const uint32_t *sp = &sm.step[warp][0];
@@ -198,38 +208,31 @@ __global__ void __launch_bounds__(kLaneWarps * 32, 2) k_synth_lanes(SynthArgs a)
                     add_if(neg1, wb.y, sbit, eb1);
                     add_if(neg2, wa.z, sbit, ea2);
                     add_if(neg2, wb.z, sbit, eb2);
-                    // fast_risky(p) <=> (~p) << 9 < kBandFast << 9 <=> p << 9 > 0xFFFFFE00 - (kBandFast << 9): the largest
-                    // fraction below an index boundary over all channels and samples
-                    dmax = __vimax3_u32(dmax, a0 << 9, b0 << 9);
-                    dmax = __vimax3_u32(dmax, a1 << 9, b1 << 9);
-                    dmax = __vimax3_u32(dmax, a2 << 9, b2 << 9);
                 }
                 int accs[3] = {(int) ((uint32_t) all0 - 2u * (uint32_t) neg0), (int) ((uint32_t) all1 - 2u * (uint32_t) neg1),
                                (int) ((uint32_t) all2 - 2u * (uint32_t) neg2)};
-                if (__any_sync(kFull, dmax > 0xFFFFFE00u - (lanes::kBandFast << 9))) {
-                    // ---- repair: some sample of this window sits within 2^-25 cycles below an index boundary for some
-                    // channel. Find the channel(s), take the certain index of exactly those (channel, sample) pairs (64-bit
-                    // linear phase; exact walk from the run anchor inside the 2^-41 band) and patch the sums.
-                    for (int c = 0; c < nchan; c++) {
-                        const uint4 wv = *reinterpret_cast<const uint4 *>(&wrow[c]);
-                        const uint32_t st = sm.step[warp][c];
-                        const uint32_t p0 = wv.w + n0 * st, p1 = wv.w + n1 * st, p2 = wv.w + n2 * st;
-                        const bool risky = lanes::fast_risky(p0) | lanes::fast_risky(p1) | lanes::fast_risky(p2);
-                        if (!__any_sync(kFull, risky)) continue;
-                        const int src = hh * CH + c;
-                        const uint64_t Pc = shfl64(s.P, src), Dc = shfl64(s.D, src);
-                        if (!risky || bc[c].prn <= 0) continue;
-                        const RunCkpt k0 = a.ck[((size_t) b * a.nruns + r) * nchan + c];
-                        const lanes::Anchor ac = {k0.x, k0.y, bc[c].c_carr, bc[c].c_code, k0.nav};
-                        const uint32_t ps[3] = {p0, p1, p2}, sw[3] = {wv.x, wv.y, wv.z};
+                // ---- repair: the channel side flagged the channels with a sample of this window within 2^-25 cycles below
+                // an index boundary (warp-uniform). Take the certain index of exactly those (channel, sample) pairs (64-bit
+                // linear phase; exact walk from the run anchor inside the 2^-41 band) and patch the sums.
+                for (uint32_t m = WINS == 1 ? flagged : (flagged >> (hh * CH)) & 0xFFFFu; m != 0u; m &= m - 1u) {
+                    const int c = __ffs((int) m) - 1;
+                    const uint4 wv = *reinterpret_cast<const uint4 *>(&wrow[c]);
+                    const uint32_t st = sm.step[warp][c];
+                    const uint32_t p0 = wv.w + n0 * st, p1 = wv.w + n1 * st, p2 = wv.w + n2 * st;
+                    const bool risky = lanes::fast_risky(p0) | lanes::fast_risky(p1) | lanes::fast_risky(p2);
+                    const int src = hh * CH + c;
+                    const uint64_t Pc = shfl64(s.P, src), Dc = shfl64(s.D, src);
+                    if (!risky) continue;
+                    const RunCkpt k0 = a.ck[((size_t) b * a.nruns + r) * nchan + c];
+                    const lanes::Anchor ac = {k0.x, k0.y, bc[c].c_carr, bc[c].c_code, k0.nav};
+                    const uint32_t ps[3] = {p0, p1, p2}, sw[3] = {wv.x, wv.y, wv.z};
 #pragma unroll
-                        for (int j = 0; j < 3; j++) {
-                            if (!lanes::fast_risky(ps[j])) continue;
-                            const int kf = (int) (ps[j] >> 23);                      // stored slot (rotated)
-                            const int k = lanes::exact_index(Pc, Dc, ac, w + hh, 32 * j + lane);
-                            const int fix = tab[c * 512 + ((k + c * SWZ) & 511)] - tab[c * 512 + kf];
-                            accs[j] += (sw[j] & sbit) ? -fix : fix;
-                        }
+                    for (int j = 0; j < 3; j++) {
+                        if (!lanes::fast_risky(ps[j])) continue;
+                        const int kf = (int) (ps[j] >> 23);                          // stored slot (rotated)
+                        const int k = lanes::exact_index(Pc, Dc, ac, w + hh, 32 * j + lane);
+                        const int fix = tab[c * 512 + ((k + c * SWZ) & 511)] - tab[c * 512 + kf];
+                        accs[j] += (sw[j] & sbit) ? -fix : fix;
                     }
                 }
                 // ---- quantise + pack (gps.c:2833-2845) ---------------------------------------------------------------

@@ -283,5 +283,73 @@ GPSB_HD uint32_t fast_base(const ChanRun &s) { return (uint32_t) (s.P >> 32) - 1
 GPSB_HD uint32_t fast_step(const ChanRun &s) { return (uint32_t) (s.D >> 32); }
 GPSB_HD bool fast_risky(uint32_t p) { return (((~p) << 9) < (kBandFast << 9)); }
 
+// fast_risky() for all 96 samples of a window at once. Sample n's phase is base + n * step, so its low 23 bits are
+// (b + n u) mod 2^23 with b, u the low 23 bits of base and step: some sample is risky exactly when some residue n u mod
+// 2^23, n < 96, lies in the circular interval [t, t + kBandFast), t = (2^23 - kBandFast - b) mod 2^23. The residues
+// depend on the step alone, which is fixed per (block, channel): band_residues() lists them once in ascending order, and
+// window_band_risky() answers for a window with a fixed 7-step search of that list.
+constexpr uint32_t kMod23 = 1u << 23;
+constexpr int kBandList = 128;                     // entries of a residue list: the residues, then kBandPad
+constexpr uint32_t kBandPad = kMod23;              // R[0] + 2^23 (R[0] = 0): the first residue once more, past the wrap
+
+// Number of distinct residues n u mod 2^23 over n < 96: they repeat with period 2^23 / (lowest set bit of u).
+GPSB_HD int band_distinct(uint32_t u) {
+    if (u == 0) return 1;
+    const uint32_t period = kMod23 / (u & (0u - u));
+    return period < (uint32_t) kWindow ? (int) period : kWindow;
+}
+
+// R[0 .. kBandList): the distinct residues n * step mod 2^23 (n < 96) in ascending order, then kBandPad. Built along the
+// successor rule of the three-distance theorem (Sos; Swierczkowski): for m distinct points n u (n < m), let a be the n
+// with the smallest residue above 0 and b the n with the largest; the point after n in ascending order is n + a if
+// n + a < m, else n - b if n >= b, else n + a - b, and the residue grows by r_a, 2^23 - r_b or their sum.
+GPSB_HD void band_residues(uint32_t step, uint32_t *R) {
+    const uint32_t u = step & (kMod23 - 1);
+    const int m = band_distinct(u);
+    int a = 0, b = 0;
+    uint32_t ra = kMod23, rb = 0;
+    for (int n = 1; n < m; n++) {
+        const uint32_t r = ((uint32_t) n * u) & (kMod23 - 1);
+        if (r < ra) ra = r, a = n;
+        if (r > rb) rb = r, b = n;
+    }
+    const uint32_t db = kMod23 - rb;
+    int n = 0;
+    uint32_t r = 0;
+    for (int k = 0; k < m; k++) {
+        R[k] = r;
+        if (n + a < m) {
+            n += a;
+            r += ra;
+        } else if (n >= b) {
+            n -= b;
+            r += db;
+        } else {
+            n += a - b;
+            r += ra + db;
+        }
+    }
+    for (int k = m; k < kBandList; k++) R[k] = kBandPad;
+}
+
+// True when some sample of a window with this phase base (only the low 23 bits count) is fast_risky(); R: the
+// band_residues() of its step. lo = the largest entry below t + kBandFast (R[0] = 0 always is one): a residue lies in
+// [t, t + kBandFast) exactly when lo >= t. When the interval passes 2^23, kBandPad is below its end and stands for R[0]
+// past the wrap.
+GPSB_HD bool window_band_risky(const uint32_t *R, uint32_t base) {
+    const uint32_t t = (0u - kBandFast - base) & (kMod23 - 1);
+    const uint32_t te = t + kBandFast;
+    uint32_t i = 0, lo = 0;
+#pragma unroll
+    for (uint32_t s = kBandList / 2; s > 0; s >>= 1) {
+        const uint32_t v = R[i + s - 1];
+        if (v < te) {
+            i += s;
+            lo = v;
+        }
+    }
+    return lo >= t;
+}
+
 }  // namespace lanes
 }  // namespace gpsb200
