@@ -36,6 +36,13 @@ struct LaneWin {
     uint32_t base;                      // 32-bit carrier phase of sample 0, biased by -1 (fast_base)
 };
 
+// The per-(block, channel) constants of the channel side's window state (lanes::init_steps). They are read from shared
+// memory at every trip rather than kept in registers across the sample side.
+struct LaneSteps {
+    uint64_t D96, E96;
+    uint32_t inv32, e22;
+};
+
 // CH = channel capacity of the variant (16 or 32). The channel side uses all 32 lanes: with CH = 16 the two half-warps
 // prepare two consecutive windows per trip, with CH = 32 the warp prepares one.
 // The carrier tables ([channel][k]: I + (Q << 16), gain-scaled, gps.c:2781-2782; 2 KB per channel) sit in front of this
@@ -50,17 +57,43 @@ struct LanesSmem {
     uint32_t chips[CH][kLaneChipWords];                 // packed C/A chips, bit n = ca[n mod 1023]
     uint32_t nav[CH][kNavWords];                        // NAV words of this block's frame
     alignas(16) LaneWin win[kLaneWarps][kWins][CH];     // per warp: the window(s) in flight
-    alignas(16) uint32_t step[kLaneWarps][CH];          // per warp: 32-bit carrier increment per sample (fast_step)
+    alignas(16) uint32_t step[CH];                      // 32-bit carrier increment per sample (fast_step)
+    LaneSteps steps[CH];
     alignas(16) uint32_t stage[kLaneWarps][kWins * lanes::kWindow];   // packed output of the window(s)
     uint32_t band[CH][lanes::kBandList + 1];            // band_residues() of each channel's step; rows skewed by one bank
 };
 template <int CH>
 constexpr size_t lanes_smem_bytes() { return sizeof(LanesSmem<CH>) + (size_t) CH * 2048 + 2048; }
 
-__device__ __forceinline__ uint64_t shfl64(uint64_t v, int src) {
-    const uint32_t lo = __shfl_sync(0xFFFFFFFFu, (uint32_t) v, src);
-    const uint32_t hi = __shfl_sync(0xFFFFFFFFu, (uint32_t) (v >> 32), src);
-    return ((uint64_t) hi << 32) | lo;
+// Entry of the carrier table at byte address ta + OFF (low 11 bits zero) for the 32-bit phase p: the stored slot is p >> 23,
+// its address slot * 4 + ta. Written as a shift and a multiply-add so that the address takes one ALU and one FMA-pipe
+// instruction: the shift-and-mask form ((p >> 21) & 0x7FC) | ta puts both on the integer ALU pipe, which the sign tests
+// and sums of the loop already keep close to saturation.
+template <int OFF>
+__device__ __forceinline__ int table_at(uint32_t p, uint32_t ta) {
+    int e;
+    asm volatile("{\n\t.reg .b32 i, ad;\n\tshr.b32 i, %1, 23;\n\tmad.lo.u32 ad, i, 4, %2;\n\tld.shared.b32 %0, [ad+%3];\n\t}"
+                 : "=r"(e)
+                 : "r"(p), "r"(ta), "n"(OFF));
+    return e;
+}
+
+// The rare paths that walk from the exact run anchor (nco_exact.h), out of line: inlined, their FP64 walks raise the
+// register pressure of the whole run loop, and at 64 registers more of the window state is then kept in local memory on
+// the common path as well.
+template <class ChipFn, class NavFn>
+__device__ __noinline__ uint3 exact_signs_call(lanes::Anchor an, int w, ChipFn chips, NavFn nav) {
+    uint32_t W[3];
+    lanes::exact_signs(an, w, chips, nav, W);
+    return make_uint3(W[0], W[1], W[2]);
+}
+
+// Certain carrier table index of sample n of window w of the run.
+__device__ __noinline__ int exact_index_call(lanes::Anchor an, int w, int n) {
+    // linear carrier phase at the window start, as init_run() + advance_window() make it (sums modulo 2^64: exact)
+    const uint64_t D = lanes::carr_step_fix(an.c);
+    const uint64_t P = lanes::carr_fix(an.x0) + (uint64_t) w * ((uint64_t) lanes::kWindow * D);
+    return lanes::exact_index(P, D, an, w, n);
 }
 
 // acc += e if (w & bit) != 0, as one logic instruction that sets a predicate and one predicated add: written as C++ the
@@ -112,10 +145,14 @@ __global__ void __launch_bounds__(kLaneWarps * 32, 2) k_synth_lanes(SynthArgs a)
             if (c < nchan && bc[c].prn > 0) v = a.nav[((size_t) bc[c].frame * a.nav_stride + c) * kNavWords + w];
             sm.nav[c][w] = v;
         }
-        // residue lists of the channels' steps (fast_step() of the run state), one lane per channel of the last warp
+        // step constants and residue lists of the channels' steps, one lane per channel of the last warp
         if (warp == kLaneWarps - 1 && lane < CH) {
             const bool ok = lane < nchan && bc[lane].prn > 0;
-            lanes::band_residues(ok ? (uint32_t) (lanes::carr_step_fix(bc[lane].c_carr) >> 32) : 0u, &sm.band[lane][0]);
+            lanes::ChanRun k;
+            lanes::init_steps(k, ok, ok ? bc[lane].c_carr : 0.0, ok ? bc[lane].c_code : 0.0);
+            sm.steps[lane] = LaneSteps{k.D96, k.E96, k.inv32, k.e22};
+            sm.step[lane] = lanes::fast_step(k);
+            lanes::band_residues(lanes::fast_step(k), &sm.band[lane][0]);
         }
     }
     __syncthreads();
@@ -138,20 +175,28 @@ __global__ void __launch_bounds__(kLaneWarps * 32, 2) k_synth_lanes(SynthArgs a)
 #pragma unroll 1
     for (int r = run_first + warp; r < run_last; r += kLaneWarps) {
         // ---- channel side: exact anchor of (run, channel), window state of window 0 + half -------------------------
+        // The anchor is read again from global memory (L1/L2-resident) on the rare paths that walk from it rather than
+        // held in registers across the sample side, where at 64 registers it pushed the window state to local memory.
+        auto anchor = [&](int c) {
+            const RunCkpt k0 = a.ck[((size_t) b * a.nruns + r) * nchan + c];
+            return lanes::Anchor{k0.x, k0.y, bc[c].c_carr, bc[c].c_code, k0.nav};
+        };
         lanes::ChanRun s;
-        lanes::Anchor an = {0.0, 0.0, 0.0, 0.0, 0u};
-        if (chan_ok) {
-            const RunCkpt k0 = a.ck[((size_t) b * a.nruns + r) * nchan + ch];
-            an.x0 = k0.x;
-            an.y0 = k0.y;
-            an.navpos = k0.nav;
-            an.c = bc[ch].c_carr;
-            an.d = bc[ch].c_code;
+        auto load_steps = [&]() {
+            const LaneSteps k = sm.steps[ch];
+            s.D96 = k.D96;
+            s.E96 = k.E96;
+            s.inv32 = k.inv32;
+            s.e22 = k.e22;
+        };
+        {
+            const lanes::Anchor an = chan_ok ? anchor(ch) : lanes::Anchor{0.0, 0.0, 0.0, 0.0, 0u};
+            lanes::init_run(s, chan_ok, an.x0, an.y0, an.navpos, an.c, an.d, navf);     // all zero when !chan_ok
         }
-        lanes::init_run(s, chan_ok, an.x0, an.y0, an.navpos, an.c, an.d, navf);
-        if (!chan_ok) s.P = s.D = s.Y = s.E = 0;
-        if (half == 0) sm.step[warp][ch] = chan_ok ? lanes::fast_step(s) : 0u;
-        if (WINS == 2 && chan_ok && half == 1) lanes::advance_window(s, navf);
+        if (WINS == 2 && chan_ok && half == 1) {
+            load_steps();
+            lanes::advance_window(s, navf);
+        }
         const size_t samp0 = (size_t) b * kBlockSamples + (size_t) r * a.run_samples;
 
 #pragma unroll 1
@@ -161,10 +206,20 @@ __global__ void __launch_bounds__(kLaneWarps * 32, 2) k_synth_lanes(SynthArgs a)
                 uint32_t S[3] = {0u, 0u, 0u};
                 uint32_t base = (uint32_t) (ch * SWZ) << 23;                        // rotation of the channel's table
                 bool band = false;
+                if (chan_ok) load_steps();
+                if (chan_ok && w > 0) {
+#pragma unroll
+                    for (int i = 0; i < WINS; i++) lanes::advance_window(s, navf);
+                }
                 if (chan_ok && w + half < nwin) {
                     base += lanes::fast_base(s);
                     band = lanes::window_band_risky(band_row, base);                 // the rotation keeps the low 23 bits
-                    if (!lanes::window_signs(s, chipf, navf, S)) lanes::exact_signs(an, w + half, chipf, navf, S);
+                    if (!lanes::window_signs(s, chipf, navf, S)) {
+                        const uint3 e = exact_signs_call(anchor(ch), w + half, chipf, navf);
+                        S[0] = e.x;
+                        S[1] = e.y;
+                        S[2] = e.z;
+                    }
                 }
                 *reinterpret_cast<uint4 *>(&sm.win[warp][half][ch]) = make_uint4(S[0], S[1], S[2], base);
                 flagged = __ballot_sync(kFull, band);
@@ -182,7 +237,7 @@ __global__ void __launch_bounds__(kLaneWarps * 32, 2) k_synth_lanes(SynthArgs a)
                 int all0 = 0, all1 = 0, all2 = 0, neg0 = 0, neg1 = 0, neg2 = 0;
                 // Two channels per trip (an odd count is padded with the next slot, which is all zeros).
                 const LaneWin *wp = wrow;
-                const uint32_t *sp = &sm.step[warp][0];
+                const uint32_t *sp = &sm.step[0];
                 uint32_t ta = tab_base;                                        // table of channel c; c + 1 at + 2048
 #pragma unroll 4
                 for (int c = 0; c < nchan; c += 2, wp += 2, sp += 2, ta += 2 * 2048u) {
@@ -191,14 +246,9 @@ __global__ void __launch_bounds__(kLaneWarps * 32, 2) k_synth_lanes(SynthArgs a)
                     const uint2 st = *reinterpret_cast<const uint2 *>(sp);
                     const uint32_t a0 = wa.w + n0 * st.x, a1 = wa.w + n1 * st.x, a2 = wa.w + n2 * st.x;
                     const uint32_t b0 = wb.w + n0 * st.y, b1 = wb.w + n1 * st.y, b2 = wb.w + n2 * st.y;
-                    // table base (low 11 bits zero) | byte offset of the stored slot
-                    int ea0, ea1, ea2, eb0, eb1, eb2;
-                    asm volatile("ld.shared.b32 %0, [%1];" : "=r"(ea0) : "r"(((a0 >> 21) & 0x7FCu) | ta));
-                    asm volatile("ld.shared.b32 %0, [%1+2048];" : "=r"(eb0) : "r"(((b0 >> 21) & 0x7FCu) | ta));
-                    asm volatile("ld.shared.b32 %0, [%1];" : "=r"(ea1) : "r"(((a1 >> 21) & 0x7FCu) | ta));
-                    asm volatile("ld.shared.b32 %0, [%1+2048];" : "=r"(eb1) : "r"(((b1 >> 21) & 0x7FCu) | ta));
-                    asm volatile("ld.shared.b32 %0, [%1];" : "=r"(ea2) : "r"(((a2 >> 21) & 0x7FCu) | ta));
-                    asm volatile("ld.shared.b32 %0, [%1+2048];" : "=r"(eb2) : "r"(((b2 >> 21) & 0x7FCu) | ta));
+                    const int ea0 = table_at<0>(a0, ta), eb0 = table_at<2048>(b0, ta);
+                    const int ea1 = table_at<0>(a1, ta), eb1 = table_at<2048>(b1, ta);
+                    const int ea2 = table_at<0>(a2, ta), eb2 = table_at<2048>(b2, ta);
                     all0 += ea0 + eb0;
                     all1 += ea1 + eb1;
                     all2 += ea2 + eb2;
@@ -217,20 +267,17 @@ __global__ void __launch_bounds__(kLaneWarps * 32, 2) k_synth_lanes(SynthArgs a)
                 for (uint32_t m = WINS == 1 ? flagged : (flagged >> (hh * CH)) & 0xFFFFu; m != 0u; m &= m - 1u) {
                     const int c = __ffs((int) m) - 1;
                     const uint4 wv = *reinterpret_cast<const uint4 *>(&wrow[c]);
-                    const uint32_t st = sm.step[warp][c];
+                    const uint32_t st = sm.step[c];
                     const uint32_t p0 = wv.w + n0 * st, p1 = wv.w + n1 * st, p2 = wv.w + n2 * st;
                     const bool risky = lanes::fast_risky(p0) | lanes::fast_risky(p1) | lanes::fast_risky(p2);
-                    const int src = hh * CH + c;
-                    const uint64_t Pc = shfl64(s.P, src), Dc = shfl64(s.D, src);
                     if (!risky) continue;
-                    const RunCkpt k0 = a.ck[((size_t) b * a.nruns + r) * nchan + c];
-                    const lanes::Anchor ac = {k0.x, k0.y, bc[c].c_carr, bc[c].c_code, k0.nav};
+                    const lanes::Anchor ac = anchor(c);
                     const uint32_t ps[3] = {p0, p1, p2}, sw[3] = {wv.x, wv.y, wv.z};
 #pragma unroll
                     for (int j = 0; j < 3; j++) {
                         if (!lanes::fast_risky(ps[j])) continue;
                         const int kf = (int) (ps[j] >> 23);                          // stored slot (rotated)
-                        const int k = lanes::exact_index(Pc, Dc, ac, w + hh, 32 * j + lane);
+                        const int k = exact_index_call(ac, w + hh, 32 * j + lane);
                         const int fix = tab[c * 512 + ((k + c * SWZ) & 511)] - tab[c * 512 + kf];
                         accs[j] += (sw[j] & sbit) ? -fix : fix;
                     }
@@ -259,10 +306,6 @@ __global__ void __launch_bounds__(kLaneWarps * 32, 2) k_synth_lanes(SynthArgs a)
                                                        (samp0 + (size_t) w * lanes::kWindow) * (IQ16 ? 4 : 2));
                 const uint4 *srcv = reinterpret_cast<const uint4 *>(stage);
                 for (int i = lane; i < nvec; i += 32) dst[i] = srcv[i];
-            }
-            if (chan_ok) {
-#pragma unroll
-                for (int i = 0; i < WINS; i++) lanes::advance_window(s, navf);
             }
         }
     }

@@ -65,6 +65,7 @@ GPSB_HD uint32_t funnel_r(uint32_t lo, uint32_t hi, int sh) {               // (
 struct ChanRun {
     uint64_t P, D;          // carrier: linear phase at the current window start, increment per sample
     uint64_t Y, E;          // code: linear phase at the current window start (chips * 2^54, < 1023 * 2^54), increment
+    uint64_t D96, E96;      // kWindow * D, kWindow * E: the advance of one window (the only increments the window loop needs)
     uint32_t inv32;         // floor(2^79 / delta3), delta3 = 3 E - 2^54 in [2^48, 2^49): the carry-point division as a multiply
     uint32_t e22;           // E >> 22: code increment in units of 2^-32 chips (truncated)
     int iword, ibit, icode, dbit;
@@ -83,6 +84,17 @@ GPSB_HD int nav_bit_at(NavFn nav, int iw, int ib) {
     return (int) ((w >> (29 - ib)) & 1u);                                   // gps.c:2812
 }
 
+// The increments of a ChanRun and what is derived from them: fixed per (block, channel), the same for every run.
+GPSB_HD void init_steps(ChanRun &s, bool active, double c, double d) {
+    s.D = carr_step_fix(c);
+    s.E = code_fix(d);
+    s.D96 = (uint64_t) kWindow * s.D;
+    s.E96 = (uint64_t) kWindow * s.E;
+    const uint64_t d3 = 3 * s.E - kOne54;
+    s.inv32 = active ? (uint32_t) (0x1p79 / (double) d3) : 0u;                // in (2^30, 2^31]
+    s.e22 = (uint32_t) (s.E >> 22);
+}
+
 template <class NavFn>
 GPSB_HD void init_run(ChanRun &s, bool active, double x, double y, uint32_t navpos, double c, double d, NavFn nav) {
     s.active = active;
@@ -90,12 +102,8 @@ GPSB_HD void init_run(ChanRun &s, bool active, double x, double y, uint32_t navp
     s.ibit = (int) ((navpos >> 8) & 0xFF);
     s.icode = (int) ((navpos >> 16) & 0xFF);
     s.P = carr_fix(x);
-    s.D = carr_step_fix(c);
     s.Y = code_fix(y);
-    s.E = code_fix(d);
-    const uint64_t d3 = 3 * s.E - kOne54;
-    s.inv32 = active ? (uint32_t) (0x1p79 / (double) d3) : 0u;                // in (2^30, 2^31]
-    s.e22 = (uint32_t) (s.E >> 22);
+    init_steps(s, active, c, d);
     s.dbit = active ? nav_bit_at(nav, s.iword, s.ibit) : 0;
 }
 
@@ -112,7 +120,7 @@ GPSB_HD uint32_t mulhi32(uint32_t a, uint32_t b) {
 // sample 3q + r), which window_signs() regroups. Returns false when a sample's linear
 // code phase is within the band of a chip boundary or a carry point stays ambiguous.
 GPSB_HD bool window_signs_fp64(const ChanRun &s, uint32_t c_lo, uint32_t c_hi, int j0, uint32_t S[3]) {
-    const uint64_t d3 = 3 * s.E - kOne54;
+    const uint64_t d3 = (s.E96 >> 5) - kOne54;                              // 3 E = 96 E / 32 (E96 < 2^64 holds 96 E exactly)
     const double rinv = 1.0 / (double) d3;
     const double tband = (double) kBandCode * rinv + 0x1p-40;                // band of the carry-point test, in units of q
     bool certain = true;
@@ -211,9 +219,9 @@ GPSB_HD bool window_signs(const ChanRun &s, ChipFn chips, NavFn nav, uint32_t W[
 // Next window: 96 samples on.
 template <class NavFn>
 GPSB_HD void advance_window(ChanRun &s, NavFn nav) {
-    s.P += (uint64_t) kWindow * s.D;
+    s.P += s.D96;
     const uint64_t y_old = s.Y;
-    s.Y += (uint64_t) kWindow * s.E;                                          // 1023 + 33 chips passes 2^64: modular
+    s.Y += s.E96;                                                             // 1023 + 33 chips passes 2^64: modular
     if (s.Y < y_old || s.Y >= kCodeWrap54) {
         s.Y -= kCodeWrap54;
         if (++s.icode >= 20) {
