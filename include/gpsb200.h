@@ -214,6 +214,14 @@ int gpsb200_debug_run_checkpoints(gpsb200_ctx_t *ctx, int nblk, int nchan, void 
 int gpsb200_debug_block_probes(gpsb200_ctx_t *ctx, int nblk, int nchan, void *probes_out, double *seg_out,
                                double *guess_out);
 
+/* Test hook: the shape of ONE synthesis launch over nblk blocks of nchan channels on this context's device as it stands
+ * (nblk may exceed cfg.max_blocks): *kernel = "k_synth_lanes" or "k_synth" (as gpsb200_synth_kernel_name), how many CTAs
+ * share a block and how many runs each CTA takes (the last CTA of a block may take fewer). Which launches a call makes
+ * depends on its path: a host-destination call launches per chunk of at most 256 blocks, a call of at most two blocks
+ * and a slice call per segment, an eager device-destination call once over the whole call. Enqueues nothing. */
+int gpsb200_debug_synth_shape(gpsb200_ctx_t *ctx, int nblk, int nchan, int sample_size, const char **kernel,
+                              int *ctas_per_block, int *runs_per_cta);
+
 /* Name of the synthesis kernel a call with nchan channels launches on this context as it stands: "k_synth_lanes"
  * (lane = sample: run length a multiple of 96 up to 2400, every code rate seen so far within 1.0157 .. 1.0302 MHz,
  * GPSB200_LANES != 0) or "k_synth" (lane = channel, no such conditions). Both are bit-exact; for reporting. */

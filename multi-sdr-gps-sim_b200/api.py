@@ -132,7 +132,7 @@ EXPORTS = ["gpsb200_create", "gpsb200_destroy", "gpsb200_last_error", "gpsb200_v
            "gpsb200_lanes_window_band_host", "gpsb200_slice_prepare", "gpsb200_slice_probe",
            "gpsb200_slice_finish", "gpsb200_slice_finish_cb", "gpsb200_slice_wait", "gpsb200_link_apply", "gpsb200_slice_link_host", "gpsb200_debug_corrupt_chain", "gpsb200_synth_kernel_name",
            "gpsb200_debug_run_checkpoints", "gpsb200_checkpoint_segments_host",
-           "gpsb200_carrier_probe_host", "gpsb200_debug_block_probes",
+           "gpsb200_carrier_probe_host", "gpsb200_debug_block_probes", "gpsb200_debug_synth_shape",
            "gpsb200_scenario_create", "gpsb200_scenario_destroy", "gpsb200_scenario_error",
            "gpsb200_scenario_blocks", "gpsb200_scenario_channels", "gpsb200_scenario_nav_frames",
            "gpsb200_scenario_chans", "gpsb200_scenario_nav", "gpsb200_scenario_almanac_date", "gpsb200_almanac_read",
@@ -210,6 +210,8 @@ def lib():
         L.gpsb200_carrier_probe_host.argtypes = [C.c_double, C.c_double, C.c_int64, C.c_int, C.c_int, C.c_void_p,
                                                  C.c_void_p]
         L.gpsb200_debug_block_probes.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
+        L.gpsb200_debug_synth_shape.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_char_p),
+                                                C.POINTER(C.c_int), C.POINTER(C.c_int)]
         L.gpsb200_synth_kernel_name.argtypes = [C.c_void_p, C.c_int]
         L.gpsb200_synth_kernel_name.restype = C.c_char_p
         L.gpsb200_acquire.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.POINTER(AcqConfig), C.c_void_p,
@@ -671,6 +673,14 @@ class Context:
         self._check(lib().gpsb200_debug_block_probes(self._h, nblk, nchan, probes.ctypes.data, seg.ctypes.data,
                                                      guess.ctypes.data))
         return probes, seg, guess
+
+    def debug_synth_shape(self, nblk, nchan, sample_size=SC08):
+        """Shape of one synthesis launch over nblk blocks on this context's device -> (kernel name, CTAs per block,
+        runs per CTA)."""
+        name, per_block, per_cta = C.c_char_p(), C.c_int(0), C.c_int(0)
+        self._check(lib().gpsb200_debug_synth_shape(self._h, int(nblk), int(nchan), int(sample_size), C.byref(name),
+                                                    C.byref(per_block), C.byref(per_cta)))
+        return name.value.decode(), per_block.value, per_cta.value
 
     def carrier_chain(self, chans, phase_in=None):
         """Exact carrier phases after all blocks of chans (device probe + host fix-up, no synthesis)."""

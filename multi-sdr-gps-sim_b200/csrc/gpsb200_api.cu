@@ -1583,6 +1583,21 @@ int gpsb200_debug_block_probes(gpsb200_ctx_t *ctx, int nblk, int nchan, void *pr
     return GPSB200_OK;
 }
 
+int gpsb200_debug_synth_shape(gpsb200_ctx_t *ctx, int nblk, int nchan, int sample_size, const char **kernel,
+                              int *ctas_per_block, int *runs_per_cta) {
+    if (!ctx || !kernel || !ctas_per_block || !runs_per_cta || nblk < 1 || nchan < 1 || nchan > ctx->cfg.max_chan ||
+        (sample_size != GPSB200_SC08 && sample_size != GPSB200_SC16))
+        return GPSB200_ERR_ARG;
+    if (!ctx->s_compute) return fail(ctx, GPSB200_ERR_CUDA, "context has no CUDA device");
+    CU(cudaSetDevice(ctx->cfg.device));      // the shape depends on the SM count of the context's device
+    const SynthArgs a = make_args(ctx, 0, nblk, nchan, sample_size, nullptr);   // the arguments of such a launch
+    int ctas = 0, threads = 0;
+    size_t smem = 0;
+    synth_launch_shape(a, &ctas, &threads, &smem, ctas_per_block, runs_per_cta);
+    *kernel = synth_lanes_applicable(a) ? "k_synth_lanes" : "k_synth";
+    return GPSB200_OK;
+}
+
 int gpsb200_carrier_chain_device(gpsb200_ctx_t *ctx, const gpsb200_chan_t *chans, int nblk, int nchan,
                                  const double *phase_in, double *phase_out) {
     if (!ctx || !chans || !phase_out || nblk < 0 || nchan < 1 || nchan > ctx->cfg.max_chan) return GPSB200_ERR_ARG;

@@ -526,10 +526,12 @@ cudaError_t launch_synth(const SynthArgs &a, cudaStream_t s) {
     }
 }
 
-void synth_launch_shape(const SynthArgs &a, int *ctas, int *threads, size_t *smem) {
-    if (synth_lanes_applicable(a)) return synth_lanes_launch_shape(a, ctas, threads, smem);
+void synth_launch_shape(const SynthArgs &a, int *ctas, int *threads, size_t *smem, int *ctas_per_block, int *runs_per_cta) {
+    if (synth_lanes_applicable(a)) return synth_lanes_launch_shape(a, ctas, threads, smem, ctas_per_block, runs_per_cta);
     const int grp = group_for(a.nchan), rpw = 32 / grp;
     *ctas = a.nblk * a.ctas_per_block;
+    *ctas_per_block = a.ctas_per_block;
+    *runs_per_cta = a.runs_per_cta;
     *threads = ((a.runs_per_cta + rpw - 1) / rpw) * 32;
     *smem = grp == 32 ? sizeof(SynthSmem<32>) : (grp == 16 ? sizeof(SynthSmem<16>) : sizeof(SynthSmem<8>));
 }

@@ -85,8 +85,10 @@ cudaError_t launch_synth(const SynthArgs &a, cudaStream_t s);
 // The lane = sample variant for at most 16 channels (synth_lanes.cu); launch_synth() dispatches to it when applicable.
 bool synth_lanes_applicable(const SynthArgs &a);
 cudaError_t launch_synth_lanes(const SynthArgs &a, cudaStream_t s);
-void synth_lanes_launch_shape(const SynthArgs &a, int *ctas, int *threads, size_t *smem);
-// Threads per CTA and dynamic shared memory the synthesis launch will use (for reporting).
-void synth_launch_shape(const SynthArgs &a, int *ctas, int *threads, size_t *smem);
+void synth_lanes_launch_shape(const SynthArgs &a, int *ctas, int *threads, size_t *smem, int *ctas_per_block,
+                              int *runs_per_cta);
+// CTAs, threads per CTA, dynamic shared memory, CTAs per block and runs per CTA the synthesis launch will use (for
+// reporting and tests).
+void synth_launch_shape(const SynthArgs &a, int *ctas, int *threads, size_t *smem, int *ctas_per_block, int *runs_per_cta);
 
 }  // namespace gpsb200

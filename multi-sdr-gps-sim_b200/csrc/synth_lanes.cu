@@ -354,12 +354,15 @@ cudaError_t launch_synth_lanes(const SynthArgs &a_in, cudaStream_t s) {
     return a.iq16 ? launch_lanes_t<true, 32>(a, s) : launch_lanes_t<false, 32>(a, s);
 }
 
-void synth_lanes_launch_shape(const SynthArgs &a, int *ctas, int *threads, size_t *smem) {
+void synth_lanes_launch_shape(const SynthArgs &a, int *ctas, int *threads, size_t *smem, int *ctas_per_block,
+                              int *runs_per_cta) {
     int per_block, per_cta;
     lanes_shape(a, &per_block, &per_cta);
     *ctas = a.nblk * per_block;
     *threads = kLaneWarps * 32;
     *smem = a.nchan <= 16 ? lanes_smem_bytes<16>() : lanes_smem_bytes<32>();
+    *ctas_per_block = per_block;
+    *runs_per_cta = per_cta;
 }
 
 }  // namespace gpsb200
