@@ -308,7 +308,8 @@ int gpsb200_codegen(int prn, uint8_t ca[GPSB200_CA_LEN]);
 /* ---- acquisition search: which satellites does an I/Q stream contain? ------------------------------------------------
  * The first step of a GPS receiver, for interleaved I/Q at 3 Msps (one C/A period = 3000 samples): for each requested PRN
  * a search over code delay tau (0..2999 samples) x Doppler bin j (f_j = f_lo_hz + j * step_hz), over K coherent 1 ms
- * periods summed non-coherently. Not a receiver: no tracking, bit sync or navigation solution. Exact integer
+ * periods summed non-coherently. Its results seed the tracking loops below (gpsb200_track_start); no navigation
+ * solution. Exact integer
  * arithmetic, deterministic (DESIGN §9; tests/acq_model.py states it in numpy):
  *   samples    int8 as is; int16 reduced to clamp(x >> 4, -128, 127) (the int8 stream's scale, saturated where the int8
  *              stream wraps)
@@ -357,6 +358,125 @@ int gpsb200_acquire(gpsb200_ctx_t *ctx, const void *iq, int64_t nsamples, int sa
  * the synthesis of that buffer -- and the call returns when the results (and grid, in host memory) are in. */
 int gpsb200_acquire_device(gpsb200_ctx_t *ctx, const void *iq_device, int64_t nsamples, int sample_size,
                            const gpsb200_acq_config_t *cfg, gpsb200_acq_result_t *res, uint64_t *grid, void *stream);
+
+/* ---- tracking: code and carrier loops over an I/Q stream, one coherent period per C/A code epoch ---------------------
+ * A closed loop per channel, sequential in time, in exact integer arithmetic so that it is reproducible bit for bit
+ * (DESIGN §10; tests/track_model.py states it in numpy). Samples are reduced as for the acquisition search (int8 as is,
+ * int16 to clamp(x >> 4, -128, 127)), and the carrier tables are the synthesizer's. ">>" is an arithmetic shift (floor),
+ * "/" a division truncating toward zero, M = 1023 * 2^32, H = 2^31 (half a chip).
+ *   period     starts at sample s, where the local prompt code wraps; its code phase there is phi (2^-32 chip units,
+ *              phi < GPSB200_TRK_CODE_STEP_MAX) and its code step u (GPSB200_TRK_CODE_STEP_MIN..MAX per sample), so it
+ *              holds L = ceil((M - phi) / u) samples, 2999 <= L <= 3001 (u >= M / 3001 gives L <= 3001;
+ *              phi < u_max <= M / 2999 gives L >= 2999); the next one starts at s + L with phi' = phi + L u - M < u.
+ *   carrier    theta_m = theta + m * w (uint32, w the int32 carrier step in 3e6/2^32 Hz), index theta_m >> 23;
+ *              I_d = I cos + Q sin, Q_d = Q cos - I sin (the stream is code * e^{+j phase}, so a locked w ~ f_carr)
+ *   replicas   c(x) = 2 ca[x >> 32] - 1; prompt at phi_m = phi + m u, early at (phi_m + H) mod M, late at (phi_m - H) mod M
+ *   sums       E_I = sum_{m<L} c(early) I_d, E_Q, P_I, P_Q, L_I, L_Q likewise: int32 (|.| <= 3001 * 64000 < 2^31)
+ *   angle(x,y) for x >= 0: both shifted right by max(0, bitlen(max(|x|, |y|)) - 30), then 24 CORDIC vectoring steps
+ *              i = 0..23: y > 0 ? (x + (y >> i), y - (x >> i), z + A_i) : (x - (y >> i), y + (x >> i), z - A_i) from
+ *              z = 0; A_i = round(atan(2^-i) / 2 pi * 2^32) (listed in csrc/track.h); z in 2^-32 turns
+ *   PLL        (x, y) = (P_I, P_Q), negated when P_I < 0 (Costas: data bits do not matter); e = angle(x, y)
+ *   FLL        for 1 <= epochs < GPSB200_TRK_FLL_EPOCHS: cross = I' P_Q - Q' P_I, dot = I' P_I + Q' P_Q (int64, I', Q'
+ *              the previous prompt), both negated when dot < 0; d = angle(dot, cross); F += (64 d) / 3000
+ *   filter     F += e >> 12, clamped to +-2^34 (F: int64, 2^-10 carrier step units); w' = (F >> 10) + (e >> 16)
+ *   DLL        E = E_I^2 + E_Q^2, L = L_I^2 + L_Q^2 (int64), both shifted right by max(0, bitlen(E + L) - 40);
+ *              D = ((E - L) << 14) / (E + L) (0 when E + L = 0); u' = clamp(GPSB200_TRK_CODE_STEP_NOM + w' / 1540 +
+ *              (2048 D) / 3000, GPSB200_TRK_CODE_STEP_MIN, GPSB200_TRK_CODE_STEP_MAX) (carrier aiding: f_code =
+ *              1.023 MHz + f_carr / 1540)
+ *   lock       A_I += (|P_I| - A_I) >> 4, A_Q += (|P_Q| - A_Q) >> 4; locked when 3 A_Q < A_I (phase error below
+ *              about 18 degrees, the narrow-band indicator as a ratio of integers)
+ * The next period runs with theta' = theta + L w, phi', w', u'. A call runs each channel's periods while the period lies
+ * inside the buffer and fewer than max_epochs were written; the state out continues the run, so any cut of a run into
+ * calls gives the epochs of one call, bit for bit. */
+#define GPSB200_TRK_CODE_STEP_NOM 1464583848u   /* round(1.023e6 / 3e6 * 2^32) */
+#define GPSB200_TRK_CODE_STEP_MIN 1464095816u   /* ceil(M / 3001) */
+#define GPSB200_TRK_CODE_STEP_MAX 1465072205u   /* floor(M / 2999) */
+#define GPSB200_TRK_FLL_EPOCHS    200
+#define GPSB200_TRK_MAX_CHAN      32
+typedef struct gpsb200_track_state {
+    int32_t prn;           /* 1..32 */
+    int32_t epochs;        /* periods tracked so far, >= 0 */
+    int64_t sample;        /* first sample of the next period (absolute: the stream's sample index) */
+    uint64_t code_phase;   /* prompt code phase at `sample`, 2^-32 chips, < GPSB200_TRK_CODE_STEP_MAX */
+    int64_t carr_freq;     /* F: loop-filter frequency in 2^-10 carrier step units, |F| <= 2^34 */
+    uint32_t carr_phase;   /* theta at `sample` */
+    int32_t carr_step;     /* w of the next period: 3e6 / 2^32 Hz units */
+    uint32_t code_step;    /* u of the next period: 2^-32 chips per sample */
+    int32_t prev_i, prev_q;/* prompt sums of the last period (FLL) */
+    int32_t lock_i, lock_q;/* A_I, A_Q, >= 0 */
+    int32_t lock;          /* 1 when locked after the last period */
+} gpsb200_track_state_t;   /* 64 bytes */
+typedef struct gpsb200_track_epoch {
+    int64_t sample;        /* first sample of the period */
+    int32_t e_i, e_q, p_i, p_q, l_i, l_q;
+    uint32_t carr_phase;   /* theta' at the next period's first sample */
+    int32_t carr_step;     /* w' */
+    uint32_t code_phase;   /* phi' */
+    uint32_t code_step;    /* u' */
+    int32_t lock;
+    int32_t reserved;
+} gpsb200_track_epoch_t;   /* 56 bytes */
+/* The start of a channel from an acquisition: prn, Doppler (|doppler_hz| <= 10 kHz) and the sample where the code's chip 0
+ * starts (s0 + gpsb200_acq_result_t.delay): w = (int32) llround(doppler_hz * 2^32 / 3e6), F = 1024 w, u = clamp(NOM +
+ * w / 1540), phi = theta = 0, everything else 0. GPSB200_ERR_ARG on a bad argument. Host only. */
+int gpsb200_track_start(int prn, double doppler_hz, int64_t sample, gpsb200_track_state_t *state);
+/* Track nchan (1..GPSB200_TRK_MAX_CHAN) channels over nsamples samples of host memory (int8 / int16 I,Q interleaved) whose
+ * first sample is the stream's sample `base`; every state's sample must be >= base. state: [nchan], in and out.
+ * epochs: [nchan][max_epochs] (max_epochs >= 1), nepochs: [nchan] written. Every argument is checked before anything is
+ * enqueued (GPSB200_ERR_ARG). Blocking. */
+int gpsb200_track(gpsb200_ctx_t *ctx, const void *iq, int64_t nsamples, int sample_size, int64_t base,
+                  gpsb200_track_state_t *state, int nchan, int max_epochs, gpsb200_track_epoch_t *epochs,
+                  int32_t *nepochs);
+/* Same for a source in device memory (16-byte aligned), tracked in place on `stream` (0 = the context's own stream)
+ * behind whatever it holds; returns when the epochs and states are in host memory. */
+int gpsb200_track_device(gpsb200_ctx_t *ctx, const void *iq_device, int64_t nsamples, int sample_size, int64_t base,
+                         gpsb200_track_state_t *state, int nchan, int max_epochs, gpsb200_track_epoch_t *epochs,
+                         int32_t *nepochs, void *stream);
+
+/* ---- navigation message from the epochs of one tracked channel (host; csrc/navdecode.cpp) ----------------------------
+ *   bit sync   histogram over the 20 epoch positions (index mod 20) of prompt-I sign changes between consecutive locked
+ *              epochs; the edge is the position with most changes (the lowest on ties; none: no bits)
+ *   bits       bit k = the sum of the 20 prompt I's from epoch edge + 20 k on; value (sum > 0)
+ *   frame sync the first bit index i >= 2 where bits i..i+7 are the preamble 10001011 or its complement (the Costas
+ *              180 degree ambiguity, resolved by inverting every bit), and, so inverted, the TLM word (bits i..i+29) and
+ *              the HOW (i+30..i+59) pass IS-GPS-200 parity with D29*, D30* of the bits before each, and the HOW's
+ *              subframe id is 1..5
+ *   words      every complete 30-bit word from i on: the bits as transmitted (what the synthesizer's NAV word holds in
+ *              bits 29..0), the 24 data bits with D30* undone, the parity verdict; subframe id and TOW of HOW words */
+typedef struct gpsb200_nav_bit {
+    int64_t sample;        /* first sample of the bit's first epoch */
+    int64_t sum;           /* the 20 prompt I's */
+    int32_t value;         /* (sum > 0), inverted when the frame sync found the inverted preamble */
+    int32_t locked;        /* 1 when all 20 epochs were locked */
+} gpsb200_nav_bit_t;       /* 24 bytes */
+typedef struct gpsb200_nav_word {
+    int64_t sample;        /* first sample of the word's first bit */
+    uint32_t raw;          /* the 30 bits as transmitted, first bit in bit 29 */
+    uint32_t data;         /* the 24 data bits, D30* undone */
+    int32_t parity_ok;
+    int32_t subframe;      /* HOW (second word of a subframe): subframe id, else 0 */
+    int32_t tow;           /* HOW: the 17-bit TOW count (the next subframe's start, in 6 s units), else -1 */
+    int32_t index;         /* words since frame sync: 0 is the first TLM */
+} gpsb200_nav_word_t;      /* 32 bytes */
+typedef struct gpsb200_nav_sync {
+    int32_t bit_edge;      /* epoch index of the first bit (0..19), -1: no bit sync */
+    int32_t nbits;
+    int32_t frame_bit;     /* bit index of the first TLM, -1: no frame sync */
+    int32_t inverted;
+    int32_t nwords;
+    int32_t words_ok;      /* with good parity */
+    int32_t subframes;     /* HOW words with good parity */
+    int32_t first_tow;     /* TOW of the first good HOW, -1: none */
+} gpsb200_nav_sync_t;      /* 32 bytes */
+/* Decode the n epochs of one channel (in time order). bits: [max_bits >= n / 20], words: [max_words >= n / 600]; either
+ * may be NULL when its count is 0. GPSB200_ERR_ARG on a bad argument. */
+int gpsb200_nav_decode(const gpsb200_track_epoch_t *epochs, int64_t n, gpsb200_nav_bit_t *bits, int64_t max_bits,
+                       gpsb200_nav_word_t *words, int64_t max_words, gpsb200_nav_sync_t *sync);
+/* IS-GPS-200 parity of a received word: word and prev are 30-bit words as transmitted (prev supplies D29*, D30*).
+ * Returns 1 when the 6 parity bits check, 0 if not; *data (may be NULL) gets the 24 data bits with D30* undone. */
+int gpsb200_nav_word_check(uint32_t word, uint32_t prev, uint32_t *data);
+/* The 6 parity bits of 24 data bits given D29*, D30* (computeChecksum, gps.c:1008-1072, without the D29/D30 solving). */
+uint32_t gpsb200_nav_parity(uint32_t data24, int d29, int d30);
 
 /* ---- scenario engine: the reference's host path outside the sample loop -------------
  * RINEX-2/3 navigation file (plain or gzip-compressed, read through zlib like the reference, gps.c:1147) +

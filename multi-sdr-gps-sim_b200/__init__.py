@@ -12,6 +12,8 @@ from .api import (  # noqa: F401
     bind_numa, carrier_advance, span_chain_host, lanes_model_block, lanes_window_band, link_apply, slice_link_host, SliceLink, carrier_chain, codegen, scenario, lib, lib_path, CHAN_DTYPE,
     ScenarioConfig, LiveScenario, SteerState, parse_steer, KEYS, ERR_END, almanac_read, ALMANAC_RECORD_DTYPE, checkpoint_segments_host, RUN_CKPT_DTYPE,
     carrier_probe_host, CARRIER_PROBE_DTYPE, AcqConfig, ACQ_RESULT_DTYPE, ACQ_CODE_SAMPLES, acq_window_samples,
+    TRACK_STATE_DTYPE, TRACK_EPOCH_DTYPE, NAV_BIT_DTYPE, NAV_WORD_DTYPE, NAV_SYNC_DTYPE, track_start, nav_decode, nav_word_check,
+    nav_parity,
 )
 from .synthetic import synthetic_chans  # noqa: F401,E402
 from . import sharding  # noqa: F401,E402

@@ -121,6 +121,61 @@ def acq_window_samples(ms):
     return ACQ_CODE_SAMPLES * int(ms) + ACQ_CODE_SAMPLES - 1
 
 
+# gpsb200_track_state_t / gpsb200_track_epoch_t (DESIGN §10)
+TRACK_STATE_DTYPE = np.dtype([("prn", "<i4"), ("epochs", "<i4"), ("sample", "<i8"), ("code_phase", "<u8"),
+                              ("carr_freq", "<i8"), ("carr_phase", "<u4"), ("carr_step", "<i4"), ("code_step", "<u4"),
+                              ("prev_i", "<i4"), ("prev_q", "<i4"), ("lock_i", "<i4"), ("lock_q", "<i4"), ("lock", "<i4")])
+assert TRACK_STATE_DTYPE.itemsize == 64
+TRACK_EPOCH_DTYPE = np.dtype([("sample", "<i8"), ("e_i", "<i4"), ("e_q", "<i4"), ("p_i", "<i4"), ("p_q", "<i4"),
+                              ("l_i", "<i4"), ("l_q", "<i4"), ("carr_phase", "<u4"), ("carr_step", "<i4"),
+                              ("code_phase", "<u4"), ("code_step", "<u4"), ("lock", "<i4"), ("reserved", "<i4")])
+assert TRACK_EPOCH_DTYPE.itemsize == 56
+NAV_BIT_DTYPE = np.dtype([("sample", "<i8"), ("sum", "<i8"), ("value", "<i4"), ("locked", "<i4")])
+NAV_WORD_DTYPE = np.dtype([("sample", "<i8"), ("raw", "<u4"), ("data", "<u4"), ("parity_ok", "<i4"), ("subframe", "<i4"),
+                           ("tow", "<i4"), ("index", "<i4")])
+NAV_SYNC_DTYPE = np.dtype([("bit_edge", "<i4"), ("nbits", "<i4"), ("frame_bit", "<i4"), ("inverted", "<i4"),
+                           ("nwords", "<i4"), ("words_ok", "<i4"), ("subframes", "<i4"), ("first_tow", "<i4")])
+assert NAV_BIT_DTYPE.itemsize == 24 and NAV_WORD_DTYPE.itemsize == 32 and NAV_SYNC_DTYPE.itemsize == 32
+
+
+def track_start(prn, doppler_hz, sample):
+    """gpsb200_track_start: the tracking state of a channel from an acquisition (prn, Doppler, the sample where the
+    code's chip 0 starts: s0 + delay). -> TRACK_STATE_DTYPE record."""
+    st = np.zeros(1, TRACK_STATE_DTYPE)
+    rc = lib().gpsb200_track_start(int(prn), float(doppler_hz), int(sample), st.ctypes.data)
+    if rc:
+        raise GpsB200Error(rc, "gpsb200_track_start(%d, %r, %d)" % (prn, doppler_hz, sample))
+    return st[0]
+
+
+def nav_decode(epochs):
+    """gpsb200_nav_decode: bit sync, frame sync and words from the epochs of one channel (TRACK_EPOCH_DTYPE, time order).
+    -> (bits NAV_BIT_DTYPE[], words NAV_WORD_DTYPE[], sync NAV_SYNC_DTYPE record)."""
+    e = np.ascontiguousarray(epochs, dtype=TRACK_EPOCH_DTYPE)
+    n = e.size
+    bits = np.zeros(max(1, n // 20), NAV_BIT_DTYPE)
+    words = np.zeros(max(1, n // 600), NAV_WORD_DTYPE)
+    sync = np.zeros(1, NAV_SYNC_DTYPE)
+    rc = lib().gpsb200_nav_decode(e.ctypes.data if n else None, n, bits.ctypes.data, bits.size, words.ctypes.data,
+                                  words.size, sync.ctypes.data)
+    if rc:
+        raise GpsB200Error(rc, "gpsb200_nav_decode")
+    s = sync[0]
+    return bits[:max(0, int(s["nbits"]))], words[:max(0, int(s["nwords"]))], s
+
+
+def nav_word_check(word, prev):
+    """gpsb200_nav_word_check: (parity ok, 24 data bits with D30* undone) of a received 30-bit word after `prev`."""
+    d = C.c_uint32(0)
+    ok = lib().gpsb200_nav_word_check(int(word) & 0x3FFFFFFF, int(prev) & 0x3FFFFFFF, C.byref(d))
+    return bool(ok), int(d.value)
+
+
+def nav_parity(data24, d29, d30):
+    """gpsb200_nav_parity: the 6 IS-GPS-200 parity bits of 24 data bits after D29*, D30*."""
+    return int(lib().gpsb200_nav_parity(int(data24) & 0xFFFFFF, int(d29), int(d30)))
+
+
 HANDOFF_FN = C.CFUNCTYPE(None, C.c_void_p, C.POINTER(C.c_int32), C.POINTER(C.c_double))     # gpsb200_handoff_fn
 
 _lib = None
@@ -128,7 +183,8 @@ _lib = None
 EXPORTS = ["gpsb200_create", "gpsb200_destroy", "gpsb200_last_error", "gpsb200_version", "gpsb200_set_nav",
            "gpsb200_synth_blocks", "gpsb200_synth_blocks_scatter", "gpsb200_synth_blocks_device", "gpsb200_replay_device",
            "gpsb200_carrier_advance", "gpsb200_carrier_chain", "gpsb200_carrier_chain_device", "gpsb200_carrier_probe_fixup",
-           "gpsb200_codegen", "gpsb200_acquire", "gpsb200_acquire_device", "gpsb200_bind_numa", "gpsb200_span_chain_host", "gpsb200_lanes_model_block",
+           "gpsb200_codegen", "gpsb200_acquire", "gpsb200_acquire_device", "gpsb200_track_start", "gpsb200_track",
+           "gpsb200_track_device", "gpsb200_nav_decode", "gpsb200_nav_word_check", "gpsb200_nav_parity", "gpsb200_bind_numa", "gpsb200_span_chain_host", "gpsb200_lanes_model_block",
            "gpsb200_lanes_window_band_host", "gpsb200_slice_prepare", "gpsb200_slice_probe",
            "gpsb200_slice_finish", "gpsb200_slice_finish_cb", "gpsb200_slice_wait", "gpsb200_link_apply", "gpsb200_slice_link_host", "gpsb200_debug_corrupt_chain", "gpsb200_synth_kernel_name",
            "gpsb200_debug_run_checkpoints", "gpsb200_checkpoint_segments_host",
@@ -218,6 +274,15 @@ def lib():
                                       C.c_void_p]
         L.gpsb200_acquire_device.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.POINTER(AcqConfig),
                                              C.c_void_p, C.c_void_p, C.c_void_p]
+        L.gpsb200_track_start.argtypes = [C.c_int, C.c_double, C.c_int64, C.c_void_p]
+        L.gpsb200_track.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_int64, C.c_void_p, C.c_int, C.c_int,
+                                    C.c_void_p, C.c_void_p]
+        L.gpsb200_track_device.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_int64, C.c_void_p, C.c_int,
+                                           C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
+        L.gpsb200_nav_decode.argtypes = [C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p]
+        L.gpsb200_nav_word_check.argtypes = [C.c_uint32, C.c_uint32, C.POINTER(C.c_uint32)]
+        L.gpsb200_nav_parity.argtypes = [C.c_uint32, C.c_int, C.c_int]
+        L.gpsb200_nav_parity.restype = C.c_uint32
         _lib = L
     return _lib
 
@@ -721,6 +786,33 @@ class Context:
             rc = lib().gpsb200_acquire(self._h, a.ctypes.data, n, int(sample_size), C.byref(cfg), res.ctypes.data, gp)
         self._check(rc)
         return (res, grid) if want_grid else res
+
+    def track(self, states, iq=None, sample_size=SC08, base=0, max_epochs=None, device_ptr=None, nsamples=None, stream=0):
+        """Code and carrier tracking (gpsb200_track; DESIGN §10) of the channels `states` (TRACK_STATE_DTYPE[nchan], e.g.
+        from track_start) over a buffer whose first sample is the stream's sample `base`.
+        Source: iq, a numpy array of interleaved I,Q (int8 for SC08, int16 for SC16), or device_ptr (a raw 16-byte
+        aligned device pointer) holding nsamples samples, tracked in place on `stream` behind the work it holds.
+        -> (epochs: a list of TRACK_EPOCH_DTYPE arrays, one per channel, states after the call)."""
+        st = np.array(states, dtype=TRACK_STATE_DTYPE).reshape(-1).copy()
+        nchan = st.size
+        if device_ptr is not None:
+            assert iq is None and nsamples is not None
+            n = int(nsamples)
+        else:
+            a = np.ascontiguousarray(iq)
+            n = a.size // 2 if nsamples is None else int(nsamples)
+            assert n <= a.size // 2
+        me = int(max_epochs) if max_epochs is not None else n // 2999 + 1
+        out = np.zeros((max(1, nchan), max(1, me)), TRACK_EPOCH_DTYPE)
+        cnt = np.zeros(max(1, nchan), np.int32)
+        if device_ptr is not None:
+            rc = lib().gpsb200_track_device(self._h, C.c_void_p(device_ptr), n, int(sample_size), int(base),
+                                            st.ctypes.data, nchan, me, out.ctypes.data, cnt.ctypes.data, C.c_void_p(stream))
+        else:
+            rc = lib().gpsb200_track(self._h, a.ctypes.data, n, int(sample_size), int(base), st.ctypes.data, nchan, me,
+                                     out.ctypes.data, cnt.ctypes.data)
+        self._check(rc)
+        return [out[c, :cnt[c]].copy() for c in range(nchan)], st
 
     def replay_device(self, dst_ptr=0, stream=0, kernel_mask=15):
         self._check(lib().gpsb200_replay_device(self._h, C.c_void_p(dst_ptr), C.c_void_p(stream), kernel_mask))

@@ -29,6 +29,7 @@
 
 #include "../../include/gpsb200.h"
 #include "acquire.h"
+#include "track.h"
 #include "nco_exact.h"
 #include "synth_kernels.h"
 #include "synth_lanes.h"
@@ -207,6 +208,7 @@ struct gpsb200_ctx {
     SynthArgs last{};                      // replay state
     bool have_last = false;
     acq::Scratch acq;                      // acquisition searches (acquire.cu), allocated by the first one
+    trk::Scratch trk;                      // tracking calls (track.cu), allocated by the first one
     std::string err;
 };
 
@@ -1115,6 +1117,29 @@ int acquire(gpsb200_ctx *ctx, const void *iq, int64_t nsamples, int sample_size,
     return GPSB200_OK;
 }
 
+// The tracking of both entry points (track.cu). Everything is checked before anything is enqueued; a device source is
+// tracked in place on the caller's stream, a host source is copied up first.
+int track(gpsb200_ctx *ctx, const void *iq, int64_t nsamples, int sample_size, int64_t base, gpsb200_track_state_t *state,
+          int nchan, int max_epochs, gpsb200_track_epoch_t *epochs, int32_t *nepochs, bool device, cudaStream_t s) {
+    if (!iq || !epochs || !nepochs) return fail(ctx, GPSB200_ERR_ARG, "gpsb200_track: NULL source, epochs or nepochs");
+    const std::string bad = trk::check(state, nchan, max_epochs, nsamples, base, sample_size);
+    if (!bad.empty()) return fail(ctx, GPSB200_ERR_ARG, "gpsb200_track: " + bad);
+    if (device && (reinterpret_cast<uintptr_t>(iq) & 15u) != 0)
+        return fail(ctx, GPSB200_ERR_ARG, "gpsb200_track_device: iq_device is not 16-byte aligned");
+    if (!ctx->s_compute) return fail(ctx, GPSB200_ERR_CUDA, "context has no CUDA device");
+    if (ctx->call.active) return fail(ctx, GPSB200_ERR_ARG, "a call begun with gpsb200_slice_prepare has not been finished");
+    CU(cudaSetDevice(ctx->cfg.device));
+    const size_t bytes = (size_t) nsamples * 2 * (sample_size == GPSB200_SC16 ? 2 : 1);
+    CU(trk::scratch_reserve(ctx->trk, nchan, max_epochs, device ? 0 : bytes));
+    const void *src = iq;
+    if (!device) {
+        if (bytes) CU(cudaMemcpyAsync(ctx->trk.d_src, iq, bytes, cudaMemcpyHostToDevice, s));
+        src = ctx->trk.d_src;
+    }
+    CU(trk::launch(ctx->trk, src, nsamples, sample_size, base, state, nchan, max_epochs, epochs, nepochs, s));
+    return GPSB200_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -1421,6 +1446,7 @@ void gpsb200_destroy(gpsb200_ctx_t *ctx) {
         if (e) cudaEventDestroy(e);
     cudaFreeHost(ctx->h_seg_end);
     acq::scratch_free(ctx->acq);
+    trk::scratch_free(ctx->trk);
     if (ctx->s_compute) cudaStreamDestroy(ctx->s_compute);
     if (ctx->s_copy) cudaStreamDestroy(ctx->s_copy);
     if (ctx->s_pre) cudaStreamDestroy(ctx->s_pre);
@@ -1645,6 +1671,36 @@ int gpsb200_acquire_device(gpsb200_ctx_t *ctx, const void *iq_device, int64_t ns
     if (!ctx) return GPSB200_ERR_ARG;
     cudaStream_t s = stream_ ? (cudaStream_t) stream_ : ctx->s_compute;
     return settle(ctx, s, acquire(ctx, iq_device, nsamples, sample_size, cfg, res, grid, true, s));
+}
+
+int gpsb200_track_start(int prn, double doppler_hz, int64_t sample, gpsb200_track_state_t *st) {
+    if (!st || prn < 1 || prn > 32 || !(std::fabs(doppler_hz) <= 10000.0) || sample < 0) return GPSB200_ERR_ARG;
+    memset(st, 0, sizeof *st);
+    st->prn = prn;
+    st->sample = sample;
+    st->carr_step = (int32_t) acq::phase_step(doppler_hz);
+    st->carr_freq = (int64_t) st->carr_step * 1024;
+    int64_t u = (int64_t) GPSB200_TRK_CODE_STEP_NOM + trk::tdiv(st->carr_step, 1540);
+    u = std::min<int64_t>(std::max<int64_t>(u, GPSB200_TRK_CODE_STEP_MIN), GPSB200_TRK_CODE_STEP_MAX);
+    st->code_step = (uint32_t) u;
+    return GPSB200_OK;
+}
+
+int gpsb200_track(gpsb200_ctx_t *ctx, const void *iq, int64_t nsamples, int sample_size, int64_t base,
+                  gpsb200_track_state_t *state, int nchan, int max_epochs, gpsb200_track_epoch_t *epochs,
+                  int32_t *nepochs) {
+    if (!ctx) return GPSB200_ERR_ARG;
+    return settle(ctx, nullptr, track(ctx, iq, nsamples, sample_size, base, state, nchan, max_epochs, epochs, nepochs,
+                                      false, ctx->s_compute));
+}
+
+int gpsb200_track_device(gpsb200_ctx_t *ctx, const void *iq_device, int64_t nsamples, int sample_size, int64_t base,
+                         gpsb200_track_state_t *state, int nchan, int max_epochs, gpsb200_track_epoch_t *epochs,
+                         int32_t *nepochs, void *stream_) {
+    if (!ctx) return GPSB200_ERR_ARG;
+    cudaStream_t s = stream_ ? (cudaStream_t) stream_ : ctx->s_compute;
+    return settle(ctx, s, track(ctx, iq_device, nsamples, sample_size, base, state, nchan, max_epochs, epochs, nepochs,
+                                true, s));
 }
 
 }  // extern "C"

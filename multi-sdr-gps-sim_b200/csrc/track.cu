@@ -1,0 +1,219 @@
+// Code and carrier tracking (include/gpsb200.h: gpsb200_track; DESIGN §10).
+//
+// k_track: one CTA per channel, 256 threads, looping over the channel's periods. Per period every thread wipes off and
+// correlates samples m = tid + 256 r (r < 12, m < L) against the early, prompt and late replicas, the six int32 sums are
+// reduced in a fixed order (warp shuffles, then warp 0 over the 8 warp partials), and thread 0 runs the loop update of
+// track.h and publishes the next period's NCO state through shared memory. The loop is sequential in time: the figure
+// of merit is the latency of one period, not bandwidth (every channel reads the same samples, which hit in L2).
+#include <cstring>
+#include <vector>
+
+#include "rx_samples.cuh"
+#include "synth_tables.h"
+#include "track.h"
+
+namespace gpsb200 {
+namespace trk {
+
+namespace {
+
+using rx::load_iq;
+using rx::sine512;
+
+constexpr int kWarps = kThreads / 32;
+
+struct Smem {
+    int2 tab[512];                  // (cos, sin)
+    int8_t ca[1024];                // the channel's chips as +-1
+    int32_t part[kWarps][6];        // warp partial sums
+    gpsb200_track_state_t st;       // the loop state, owned by thread 0
+    int L;                          // samples of the current period, 0: stop
+};
+
+template <typename T>
+__global__ void __launch_bounds__(kThreads)
+k_track(const T *__restrict__ iq, int64_t nsamples, int64_t base, const int8_t *__restrict__ codes,
+        gpsb200_track_state_t *__restrict__ states, int max_epochs, gpsb200_track_epoch_t *__restrict__ epochs,
+        int32_t *__restrict__ nepochs) {
+    __shared__ Smem sm;
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int ch = blockIdx.x;
+    for (int i = tid; i < 512; i += kThreads) sm.tab[i] = make_int2(sine512(i + 128), sine512(i));
+    if (tid == 0) sm.st = states[ch];
+    __syncthreads();
+    for (int i = tid; i < GPSB200_CA_LEN; i += kThreads) sm.ca[i] = codes[sm.st.prn * GPSB200_CA_LEN + i];
+    const int64_t end = base + nsamples;
+    gpsb200_track_epoch_t *out = epochs + (size_t) ch * max_epochs;
+    int k = 0;
+    for (;;) {
+        if (tid == 0) {
+            const int L = period_len(sm.st.code_phase, sm.st.code_step);
+            sm.L = (k < max_epochs && sm.st.sample + L <= end) ? L : 0;
+        }
+        __syncthreads();   // L and the NCO state published (and, at k = 0, the chips)
+        const int L = sm.L;
+        if (L == 0) break;
+        const int64_t s = sm.st.sample - base;
+        const uint64_t phi = sm.st.code_phase;
+        const uint32_t u = sm.st.code_step, theta = sm.st.carr_phase, w = (uint32_t) sm.st.carr_step;
+        int a[6] = {0, 0, 0, 0, 0, 0};
+#pragma unroll
+        for (int r = 0; r < kPerThread; r++) {
+            const int m = tid + kThreads * r;
+            if (m < L) {
+                int I, Q;
+                load_iq<T>(iq, s + m, I, Q);
+                const int2 cs = sm.tab[(theta + (uint32_t) m * w) >> 23];
+                const int dI = I * cs.x + Q * cs.y, dQ = Q * cs.x - I * cs.y;
+                const uint64_t p = phi + (uint64_t) m * u;
+                uint64_t e = p + kHalf;
+                if (e >= kM) e -= kM;
+                const uint64_t l = p >= kHalf ? p - kHalf : p + kM - kHalf;
+                const int ce = sm.ca[e >> 32], cp = sm.ca[p >> 32], cl = sm.ca[l >> 32];
+                a[0] += ce * dI;
+                a[1] += ce * dQ;
+                a[2] += cp * dI;
+                a[3] += cp * dQ;
+                a[4] += cl * dI;
+                a[5] += cl * dQ;
+            }
+        }
+#pragma unroll
+        for (int j = 0; j < 6; j++)
+#pragma unroll
+            for (int o = 16; o > 0; o >>= 1) a[j] += __shfl_xor_sync(0xffffffffu, a[j], o);
+        if (lane == 0)
+#pragma unroll
+            for (int j = 0; j < 6; j++) sm.part[warp][j] = a[j];
+        __syncthreads();
+        if (tid == 0) {
+            int32_t c[6];
+            for (int j = 0; j < 6; j++) {
+                int v = 0;
+                for (int q = 0; q < kWarps; q++) v += sm.part[q][j];
+                c[j] = v;
+            }
+            gpsb200_track_state_t st = sm.st;
+            const int64_t s_abs = st.sample;
+            st.sample += L;
+            st.carr_phase = theta + (uint32_t) L * w;
+            st.code_phase = phi + (uint64_t) L * u - kM;
+            loop_update(st, c);
+            gpsb200_track_epoch_t ep;
+            ep.sample = s_abs;
+            ep.e_i = c[0];
+            ep.e_q = c[1];
+            ep.p_i = c[2];
+            ep.p_q = c[3];
+            ep.l_i = c[4];
+            ep.l_q = c[5];
+            ep.carr_phase = st.carr_phase;
+            ep.carr_step = st.carr_step;
+            ep.code_phase = (uint32_t) st.code_phase;
+            ep.code_step = st.code_step;
+            ep.lock = st.lock;
+            ep.reserved = 0;
+            out[k] = ep;
+            sm.st = st;
+        }
+        k++;
+    }
+    if (tid == 0) {
+        states[ch] = sm.st;
+        nepochs[ch] = k;
+    }
+}
+
+}  // namespace
+
+std::string check(const gpsb200_track_state_t *st, int nchan, int max_epochs, int64_t nsamples, int64_t base,
+                  int sample_size) {
+    if (!st) return "state is NULL";
+    if (sample_size != GPSB200_SC08 && sample_size != GPSB200_SC16) return "sample_size must be GPSB200_SC08 or GPSB200_SC16";
+    if (nchan < 1 || nchan > GPSB200_TRK_MAX_CHAN) return "nchan must be 1..32";
+    if (max_epochs < 1) return "max_epochs must be >= 1";
+    if (nsamples < 0 || base < 0) return "nsamples and base must be >= 0";
+    for (int c = 0; c < nchan; c++) {
+        const gpsb200_track_state_t &s = st[c];
+        const std::string at = "channel " + std::to_string(c) + ": ";
+        if (s.prn < 1 || s.prn > 32) return at + "PRN outside 1..32";
+        if (s.epochs < 0 || s.lock < 0 || s.lock > 1 || s.lock_i < 0 || s.lock_q < 0) return at + "bad loop state";
+        if (s.code_step < GPSB200_TRK_CODE_STEP_MIN || s.code_step > GPSB200_TRK_CODE_STEP_MAX)
+            return at + "code_step outside GPSB200_TRK_CODE_STEP_MIN..MAX";
+        if (s.code_phase >= GPSB200_TRK_CODE_STEP_MAX) return at + "code_phase must be below GPSB200_TRK_CODE_STEP_MAX";
+        if (s.carr_freq > kFreqClamp || s.carr_freq < -kFreqClamp) return at + "|carr_freq| above 2^34";
+        if (s.sample < base) return at + "the next period starts before the buffer's first sample";
+    }
+    return std::string();
+}
+
+#define TRK_CU(call)                      \
+    do {                                  \
+        cudaError_t e_ = (call);          \
+        if (e_ != cudaSuccess) return e_; \
+    } while (0)
+
+cudaError_t scratch_reserve(Scratch &sc, int nchan, int max_epochs, size_t src_bytes) {
+    if (!sc.d_codes) {
+        std::vector<int8_t> c((size_t) 33 * GPSB200_CA_LEN, 0);
+        for (int prn = 1; prn <= 32; prn++) {
+            uint8_t ca[GPSB200_CA_LEN];
+            ca_code(prn, ca);
+            for (int i = 0; i < GPSB200_CA_LEN; i++) c[(size_t) prn * GPSB200_CA_LEN + i] = (int8_t) (2 * ca[i] - 1);
+        }
+        TRK_CU(cudaMalloc(&sc.d_codes, c.size()));
+        TRK_CU(cudaMemcpy(sc.d_codes, c.data(), c.size(), cudaMemcpyHostToDevice));
+        TRK_CU(cudaMalloc(&sc.d_state, GPSB200_TRK_MAX_CHAN * sizeof(gpsb200_track_state_t)));
+        TRK_CU(cudaMalloc(&sc.d_n, GPSB200_TRK_MAX_CHAN * sizeof(int32_t)));
+    }
+    const size_t cap = (size_t) nchan * max_epochs;
+    if (cap > sc.epoch_cap) {
+        cudaFree(sc.d_epochs);
+        sc.d_epochs = nullptr;
+        sc.epoch_cap = 0;
+        TRK_CU(cudaMalloc(&sc.d_epochs, cap * sizeof(gpsb200_track_epoch_t)));
+        sc.epoch_cap = cap;
+    }
+    if (src_bytes > sc.src_bytes) {
+        cudaFree(sc.d_src);
+        sc.d_src = nullptr;
+        sc.src_bytes = 0;
+        TRK_CU(cudaMalloc(&sc.d_src, src_bytes));
+        sc.src_bytes = src_bytes;
+    }
+    return cudaSuccess;
+}
+
+void scratch_free(Scratch &sc) {
+    cudaFree(sc.d_codes);
+    cudaFree(sc.d_src);
+    cudaFree(sc.d_state);
+    cudaFree(sc.d_epochs);
+    cudaFree(sc.d_n);
+    sc = Scratch();
+}
+
+cudaError_t launch(Scratch &sc, const void *src, int64_t nsamples, int sample_size, int64_t base,
+                   gpsb200_track_state_t *state, int nchan, int max_epochs, gpsb200_track_epoch_t *epochs,
+                   int32_t *nepochs, cudaStream_t s) {
+    TRK_CU(cudaMemcpyAsync(sc.d_state, state, nchan * sizeof(gpsb200_track_state_t), cudaMemcpyHostToDevice, s));
+    if (sample_size == GPSB200_SC08)
+        k_track<int8_t><<<nchan, kThreads, 0, s>>>(static_cast<const int8_t *>(src), nsamples, base, sc.d_codes,
+                                                   sc.d_state, max_epochs, sc.d_epochs, sc.d_n);
+    else
+        k_track<int16_t><<<nchan, kThreads, 0, s>>>(static_cast<const int16_t *>(src), nsamples, base, sc.d_codes,
+                                                    sc.d_state, max_epochs, sc.d_epochs, sc.d_n);
+    TRK_CU(cudaGetLastError());
+    TRK_CU(cudaMemcpyAsync(nepochs, sc.d_n, nchan * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+    TRK_CU(cudaMemcpyAsync(state, sc.d_state, nchan * sizeof(gpsb200_track_state_t), cudaMemcpyDeviceToHost, s));
+    TRK_CU(cudaStreamSynchronize(s));
+    // the epochs of channel c sit at c * max_epochs; copy only the written ones
+    for (int c = 0; c < nchan; c++)
+        if (nepochs[c] > 0)
+            TRK_CU(cudaMemcpyAsync(epochs + (size_t) c * max_epochs, sc.d_epochs + (size_t) c * max_epochs,
+                                   (size_t) nepochs[c] * sizeof(gpsb200_track_epoch_t), cudaMemcpyDeviceToHost, s));
+    return cudaStreamSynchronize(s);
+}
+
+}  // namespace trk
+}  // namespace gpsb200

@@ -1,0 +1,131 @@
+// Code and carrier tracking loops (include/gpsb200.h: gpsb200_track; DESIGN §10). One coherent period per local C/A code
+// epoch, exact integer arithmetic; the loop update below is the contract's, shared by the kernel and the host checks.
+#pragma once
+#include <cuda_runtime.h>
+#include <stdint.h>
+
+#include <string>
+
+#include "../../include/gpsb200.h"
+
+namespace gpsb200 {
+namespace trk {
+
+constexpr uint64_t kM = 1023ull << 32;          // code phase modulus: 1023 chips in 2^-32 chip units
+constexpr uint64_t kHalf = 1ull << 31;          // early / late offset: half a chip
+constexpr int kMaxPeriod = 3001;                // samples of a period at most (header: 2999..3001)
+constexpr int kThreads = 256;                   // threads of k_track
+constexpr int kPerThread = (kMaxPeriod + kThreads - 1) / kThreads;   // 12 samples per thread and period
+constexpr int64_t kFreqClamp = 1ll << 34;       // |F| bound, 2^-10 carrier step units (+-2^24 steps = +-11.7 kHz)
+constexpr int kCordicSteps = 24;
+
+// round(atan(2^-i) / (2 pi) * 2^32), i = 0..23 (tests/track_model.py checks the same list against the formula).
+#define GPSB200_TRK_ATAN                                                                                     \
+    536870912, 316933406, 167458907, 85004756, 42667331, 21354465, 10679838, 5340245, 2670163, 1335087, 667544, \
+        333772, 166886, 83443, 41722, 20861, 10430, 5215, 2608, 1304, 652, 326, 163, 81
+
+__host__ __device__ inline int64_t tdiv(int64_t a, int64_t b) { return a / b; }   // C++: truncation toward zero
+
+__host__ __device__ inline int bitlen64(uint64_t v) {
+#ifdef __CUDA_ARCH__
+    return 64 - __clzll((long long) v);
+#else
+    return v ? 64 - __builtin_clzll(v) : 0;
+#endif
+}
+
+// Angle of (x, y), x >= 0, in 2^-32 turns: normalised to 30 bits, then 24 CORDIC vectoring steps.
+__host__ __device__ inline int32_t angle(int64_t x, int64_t y) {
+    const int32_t A[kCordicSteps] = {GPSB200_TRK_ATAN};
+    const uint64_t ay = y < 0 ? (uint64_t) (-y) : (uint64_t) y;
+    const uint64_t mx = (uint64_t) x > ay ? (uint64_t) x : ay;
+    const int s = bitlen64(mx) > 30 ? bitlen64(mx) - 30 : 0;
+    x >>= s;
+    y >>= s;
+    int64_t z = 0;
+    for (int i = 0; i < kCordicSteps; i++) {
+        const int64_t xs = x >> i, ys = y >> i;
+        if (y > 0) {
+            x += ys;
+            y -= xs;
+            z += A[i];
+        } else {
+            x -= ys;
+            y += xs;
+            z -= A[i];
+        }
+    }
+    return (int32_t) z;
+}
+
+// One loop update after a period with sums c[6] = E_I, E_Q, P_I, P_Q, L_I, L_Q. Updates carr_freq, carr_step, code_step,
+// prev_*, lock_*, lock and epochs of st (the phases and sample are advanced by the caller).
+__host__ __device__ inline void loop_update(gpsb200_track_state_t &st, const int32_t c[6]) {
+    const int64_t pi = c[2], pq = c[3];
+    // PLL: Costas discriminator
+    const int32_t e = pi < 0 ? angle(-pi, -pq) : angle(pi, pq);
+    int64_t F = st.carr_freq;
+    // FLL assist during pull-in
+    if (st.epochs >= 1 && st.epochs < GPSB200_TRK_FLL_EPOCHS) {
+        int64_t cross = (int64_t) st.prev_i * pq - (int64_t) st.prev_q * pi;
+        int64_t dot = (int64_t) st.prev_i * pi + (int64_t) st.prev_q * pq;
+        if (dot < 0) {
+            dot = -dot;
+            cross = -cross;
+        }
+        F += tdiv(64 * (int64_t) angle(dot, cross), 3000);
+    }
+    F += (int64_t) (e >> 12);
+    F = F > kFreqClamp ? kFreqClamp : (F < -kFreqClamp ? -kFreqClamp : F);
+    st.carr_freq = F;
+    const int32_t w = (int32_t) ((F >> 10) + (int64_t) (e >> 16));
+    st.carr_step = w;
+    // DLL: normalised early-minus-late power, carrier aided
+    int64_t E = (int64_t) c[0] * c[0] + (int64_t) c[1] * c[1];
+    int64_t L = (int64_t) c[4] * c[4] + (int64_t) c[5] * c[5];
+    const int bl = bitlen64((uint64_t) (E + L));
+    const int s = bl > 40 ? bl - 40 : 0;
+    E >>= s;
+    L >>= s;
+    const int64_t D = (E + L) == 0 ? 0 : tdiv((E - L) * 16384, E + L);
+    int64_t u = (int64_t) GPSB200_TRK_CODE_STEP_NOM + tdiv(w, 1540) + tdiv(2048 * D, 3000);
+    u = u < (int64_t) GPSB200_TRK_CODE_STEP_MIN ? (int64_t) GPSB200_TRK_CODE_STEP_MIN
+                                                 : (u > (int64_t) GPSB200_TRK_CODE_STEP_MAX ? (int64_t) GPSB200_TRK_CODE_STEP_MAX : u);
+    st.code_step = (uint32_t) u;
+    // narrow-band lock indicator
+    const int32_t api = (int32_t) (pi < 0 ? -pi : pi), apq = (int32_t) (pq < 0 ? -pq : pq);
+    st.lock_i += (api - st.lock_i) >> 4;
+    st.lock_q += (apq - st.lock_q) >> 4;
+    st.lock = (int64_t) 3 * st.lock_q < (int64_t) st.lock_i ? 1 : 0;
+    st.prev_i = (int32_t) pi;
+    st.prev_q = (int32_t) pq;
+    st.epochs += 1;
+}
+
+// Samples of the period that starts with code phase phi at code step u: ceil((M - phi) / u).
+__host__ __device__ inline int period_len(uint64_t phi, uint32_t u) { return (int) ((kM - phi + u - 1) / u); }
+
+// Empty when the states and call shape are well-formed (see the header); nsamples / base describe the buffer.
+std::string check(const gpsb200_track_state_t *st, int nchan, int max_epochs, int64_t nsamples, int64_t base,
+                  int sample_size);
+
+// Device scratch of the tracking calls of one context, grown as needed.
+struct Scratch {
+    int8_t *d_codes = nullptr;                   // [33][1023] chips as +-1, row 0 unused
+    void *d_src = nullptr;                       // a host source's samples
+    size_t src_bytes = 0;
+    gpsb200_track_state_t *d_state = nullptr;    // [GPSB200_TRK_MAX_CHAN]
+    gpsb200_track_epoch_t *d_epochs = nullptr;   // [nchan][max_epochs]
+    size_t epoch_cap = 0;
+    int32_t *d_n = nullptr;                      // [GPSB200_TRK_MAX_CHAN]
+};
+
+cudaError_t scratch_reserve(Scratch &sc, int nchan, int max_epochs, size_t src_bytes);
+void scratch_free(Scratch &sc);
+// Enqueue the tracking of the samples at `src` (stream sample `base` first) on s and wait for the results.
+cudaError_t launch(Scratch &sc, const void *src, int64_t nsamples, int sample_size, int64_t base,
+                   gpsb200_track_state_t *state, int nchan, int max_epochs, gpsb200_track_epoch_t *epochs,
+                   int32_t *nepochs, cudaStream_t s);
+
+}  // namespace trk
+}  // namespace gpsb200

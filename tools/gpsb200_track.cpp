@@ -1,0 +1,180 @@
+// gpsb200-track: acquire, track and decode the navigation messages of a 3 Msps I/Q file (gpsb200-sim's output, the
+// reference's iqdata.bin, any capture in these formats: int8 or, with --iq16, int16 I,Q interleaved). The acquisition
+// is gpsb200_acquire at the start offset (10 coherent periods, bins of 100 Hz over +-5 kHz, so that the loops start
+// within their pull-in range); every PRN whose P1/P2 reaches the threshold is tracked with gpsb200_track over the file,
+// read in chunks of one second, and decoded with gpsb200_nav_decode. Prints one line per tracked PRN: locked at the
+// end or not, the Doppler at the end, subframes found, words with good parity and the first TOW (DESIGN §10).
+#include <sys/stat.h>
+
+#include <algorithm>
+#include <cmath>
+#include <cstdio>
+#include <cstdlib>
+#include <cstring>
+#include <string>
+#include <vector>
+
+#include "../include/gpsb200.h"
+
+static const double kDefaultThreshold = 2.5;      // as gpsb200-acq
+static const int kAcqMs = 10;
+static const double kAcqLo = -5000.0, kAcqHi = 5000.0, kAcqStep = 100.0;
+static const long long kChunk = 3000000;          // samples per tracking call: 1 s
+
+static void usage() {
+    fprintf(stderr,
+            "gpsb200-track FILE [--iq16] [--block B] [--offset-ms N] [--ms K] [--prn LIST] [--threshold R] [--device D]\n"
+            "  FILE              interleaved I,Q at 3 Msps, int8 (default) or int16 (--iq16)\n"
+            "  --block B         start at 0.1 s block B (sample 300000 B); --offset-ms N adds N ms (3000 N samples)\n"
+            "  --ms K            track K ms of signal from the start (default: to the end of the file)\n"
+            "  --prn LIST        PRNs searched, e.g. 1-32 (default), 3,7,12-15\n"
+            "  --threshold R     P1/P2 at or above R counts as acquired and is tracked (default %.1f)\n",
+            kDefaultThreshold);
+    exit(2);
+}
+
+static bool parse_prns(const char *s, gpsb200_acq_config_t *cfg) {
+    cfg->nprn = 0;
+    std::string t(s);
+    size_t pos = 0;
+    while (pos <= t.size()) {
+        size_t end = t.find(',', pos);
+        if (end == std::string::npos) end = t.size();
+        const std::string item = t.substr(pos, end - pos);
+        int a = 0, b = 0;
+        if (sscanf(item.c_str(), "%d-%d", &a, &b) == 2) {
+        } else if (sscanf(item.c_str(), "%d", &a) == 1) {
+            b = a;
+        } else {
+            return false;
+        }
+        for (int p = a; p <= b; p++) {
+            if (cfg->nprn >= 32 || p < 1 || p > 32) return false;
+            cfg->prn[cfg->nprn++] = p;
+        }
+        pos = end + 1;
+    }
+    return cfg->nprn > 0;
+}
+
+static bool read_at(FILE *f, long long s0, long long n, size_t elem, std::vector<char> &buf) {
+    buf.resize((size_t) n * 2 * elem);
+    return fseeko(f, (off_t) (s0 * 2 * (long long) elem), SEEK_SET) == 0 && fread(buf.data(), 1, buf.size(), f) == buf.size();
+}
+
+int main(int argc, char **argv) {
+    const char *path = nullptr;
+    int ss = GPSB200_SC08, device = 0;
+    long long block = 0, offset_ms = 0, ms = -1;
+    double threshold = kDefaultThreshold;
+    gpsb200_acq_config_t cfg;
+    memset(&cfg, 0, sizeof cfg);
+    cfg.ms = kAcqMs;
+    parse_prns("1-32", &cfg);
+    for (int i = 1; i < argc; i++) {
+        std::string a = argv[i];
+        auto val = [&]() -> const char * {
+            if (i + 1 >= argc) usage();
+            return argv[++i];
+        };
+        if (a == "--iq16") ss = GPSB200_SC16;
+        else if (a == "--block") block = atoll(val());
+        else if (a == "--offset-ms") offset_ms = atoll(val());
+        else if (a == "--ms") ms = atoll(val());
+        else if (a == "--prn") {
+            if (!parse_prns(val(), &cfg)) usage();
+        } else if (a == "--threshold") threshold = atof(val());
+        else if (a == "--device") device = atoi(val());
+        else if (a[0] != '-' && !path) path = argv[i];
+        else usage();
+    }
+    if (!path || block < 0 || offset_ms < 0 || ms == 0 || ms < -1) usage();
+    cfg.f_lo_hz = kAcqLo;
+    cfg.step_hz = kAcqStep;
+    cfg.nbins = (int) std::floor((kAcqHi - kAcqLo) / kAcqStep + 1e-9) + 1;
+
+    const size_t elem = ss == GPSB200_SC16 ? 2 : 1;
+    const long long s0 = block * GPSB200_BLOCK_SAMPLES + offset_ms * GPSB200_ACQ_CODE_SAMPLES;
+    const long long need = (long long) GPSB200_ACQ_CODE_SAMPLES * cfg.ms + GPSB200_ACQ_CODE_SAMPLES - 1;
+    struct stat st;
+    if (stat(path, &st) != 0) {
+        fprintf(stderr, "gpsb200-track: cannot open %s\n", path);
+        return 1;
+    }
+    const long long have = (long long) st.st_size / (long long) (2 * elem);
+    if (s0 + need > have) {
+        fprintf(stderr, "gpsb200-track: the acquisition window (sample %lld, %lld samples) is not inside %s (%lld samples)\n",
+                s0, need, path, have);
+        return 1;
+    }
+    const long long end = ms > 0 ? std::min(have, s0 + ms * GPSB200_ACQ_CODE_SAMPLES) : have;
+    FILE *f = fopen(path, "rb");
+    std::vector<char> buf;
+    if (!f || !read_at(f, s0, need, elem, buf)) {
+        fprintf(stderr, "gpsb200-track: cannot read the acquisition window of %s\n", path);
+        if (f) fclose(f);
+        return 1;
+    }
+
+    gpsb200_config_t cc;
+    memset(&cc, 0, sizeof cc);
+    cc.device = device;
+    cc.max_chan = 1;
+    cc.max_blocks = 1;
+    gpsb200_ctx_t *ctx = nullptr;
+    int rc = gpsb200_create(&cc, &ctx);
+    std::vector<gpsb200_acq_result_t> res(cfg.nprn);
+    if (rc == GPSB200_OK) rc = gpsb200_acquire(ctx, buf.data(), need, ss, &cfg, res.data(), nullptr);
+    std::vector<gpsb200_track_state_t> state;
+    for (const auto &r : res)
+        if (rc == GPSB200_OK && r.ratio >= threshold) {
+            gpsb200_track_state_t t;
+            if (gpsb200_track_start(r.prn, r.doppler_hz, s0 + r.delay, &t) == GPSB200_OK) state.push_back(t);
+        }
+    const int nch = (int) state.size();
+    std::vector<std::vector<gpsb200_track_epoch_t>> eps(nch);
+    const int max_ep = (int) (kChunk / 2999 + 1);
+    std::vector<gpsb200_track_epoch_t> out((size_t) std::max(nch, 1) * max_ep);
+    std::vector<int32_t> n(std::max(nch, 1));
+    while (rc == GPSB200_OK && nch > 0) {
+        long long base = state[0].sample;
+        for (const auto &t : state) base = std::min(base, (long long) t.sample);
+        const long long cnt = std::min(kChunk, end - base);
+        if (cnt <= 0) break;
+        if (!read_at(f, base, cnt, elem, buf)) {
+            fprintf(stderr, "gpsb200-track: cannot read %s at sample %lld\n", path, base);
+            rc = GPSB200_ERR_ARG;
+            break;
+        }
+        rc = gpsb200_track(ctx, buf.data(), cnt, ss, base, state.data(), nch, max_ep, out.data(), n.data());
+        long long got = 0;
+        for (int c = 0; c < nch && rc == GPSB200_OK; c++) {
+            eps[c].insert(eps[c].end(), out.begin() + (size_t) c * max_ep, out.begin() + (size_t) c * max_ep + n[c]);
+            got += n[c];
+        }
+        if (got == 0) break;
+    }
+    fclose(f);
+    if (rc != GPSB200_OK) {
+        fprintf(stderr, "gpsb200-track: %s\n", ctx ? gpsb200_last_error(ctx) : "cannot create a context");
+        gpsb200_destroy(ctx);
+        return 1;
+    }
+    gpsb200_destroy(ctx);
+    printf("# %s: sample %lld to %lld, %d of %d PRNs acquired (P1/P2 >= %.2f) and tracked\n", path, s0, end, nch, cfg.nprn,
+           threshold);
+    printf("# PRN  locked  doppler_hz  subframes  words_ok  words  first_tow\n");
+    for (int c = 0; c < nch; c++) {
+        const auto &e = eps[c];
+        const int64_t ne = (int64_t) e.size();
+        std::vector<gpsb200_nav_bit_t> bits((size_t) (ne / 20 + 1));
+        std::vector<gpsb200_nav_word_t> words((size_t) (ne / 600 + 1));
+        gpsb200_nav_sync_t sy;
+        gpsb200_nav_decode(e.data(), ne, bits.data(), (int64_t) bits.size(), words.data(), (int64_t) words.size(), &sy);
+        const bool locked = ne > 0 && e.back().lock;
+        const double dopp = ne > 0 ? e.back().carr_step * 3e6 / 4294967296.0 : 0.0;
+        printf("%5d  %6s  %10.1f  %9d  %8d  %5d  %9d\n", state[c].prn, locked ? "yes" : "no", dopp, sy.subframes,
+               sy.words_ok, sy.nwords, sy.first_tow);
+    }
+    return 0;
+}
