@@ -478,6 +478,123 @@ int gpsb200_nav_word_check(uint32_t word, uint32_t prev, uint32_t *data);
 /* The 6 parity bits of 24 data bits given D29*, D30* (computeChecksum, gps.c:1008-1072, without the D29/D30 solving). */
 uint32_t gpsb200_nav_parity(uint32_t data24, int d29, int d30);
 
+/* ---- broadcast ephemeris, ionosphere and time anchor from decoded words (host; csrc/navdecode.cpp) -------------------
+ * Input: the word records of one channel in order, words[i].index == words[0].index + i (what gpsb200_nav_decode
+ * returns; a NAV frame slot of the scenario, 60 words with index 0..59, turned into records with
+ * gpsb200_nav_word_check, reads the same way). A subframe starts at a word whose index is a multiple of 10; its id is
+ * bits 4..2 of the HOW's data. Each term is the IS-GPS-200 integer field (two's complement where signed; M0, e, sqrt A,
+ * OMEGA0, i0 and omega split 8 + 24 bits over two words) times its scale, x pi for semicircles (pi = 3.1415926535898,
+ * as gps.h:91): the inverse of the reference's eph2sbf (gps.c:662-684, 706-740).
+ *   ephemeris  from the LAST subframe 1, 2, 3 sequence (consecutive subframes) whose 30 words all pass parity and where
+ *              IODE of subframe 2 == IODE of subframe 3 == IODC & 0xFF; valid = 0 when there is none
+ *   iono       the Klobuchar alpha0..3 / beta0..3 of the last subframe 4 page 18 (data id 1, SV id 56) whose 10 words
+ *              pass parity; valid = 0 when there is none */
+typedef struct gpsb200_ephemeris {
+    int32_t valid;         /* 1: decoded from a complete, consistent set; 0: the rest is undefined */
+    int32_t week;          /* WN, the transmission week modulo 1024 (10 bits) */
+    int32_t iodc, iode;
+    int32_t health;        /* 6 bits; 0 = all data OK */
+    int32_t ura;           /* 4 bits */
+    int32_t reserved[2];
+    double toc;            /* s of week (x 16) */
+    double af0, af1, af2;  /* s, s/s, s/s^2 (2^-31, 2^-43, 2^-55) */
+    double tgd;            /* s (2^-31) */
+    double toe;            /* s of week (x 16) */
+    double m0, deltan;     /* rad, rad/s */
+    double ecc, sqrta;     /* -, m^1/2 */
+    double omg0, inc0, aop;/* rad */
+    double omgdot, idot;   /* rad/s */
+    double cuc, cus;       /* rad */
+    double crc, crs;       /* m */
+    double cic, cis;       /* rad */
+} gpsb200_ephemeris_t;     /* 200 bytes */
+typedef struct gpsb200_iono {
+    int32_t valid;
+    int32_t reserved;
+    double alpha[4];       /* s, s/semicircle, s/semicircle^2, s/semicircle^3 (2^-30, 2^-27, 2^-24, 2^-24) */
+    double beta[4];        /* s, ... (2^11, 2^14, 2^16, 2^16) */
+} gpsb200_iono_t;          /* 72 bytes */
+/* iono may be NULL. GPSB200_ERR_ARG on a bad argument (NULL eph, n < 0, words NULL with n > 0). */
+int gpsb200_nav_ephemeris(const gpsb200_nav_word_t *words, int64_t n, gpsb200_ephemeris_t *eph, gpsb200_iono_t *iono);
+/* The transmit-time anchor of a tracked channel from its first HOW with good parity (words and sync as
+ * gpsb200_nav_decode returned them for the channel's epochs): *anchor_epoch = bit_edge + 20 (frame_bit + 30 index), the
+ * epoch whose code period starts at the HOW's first bit, and *anchor_ms = ((6 TOW - 6) 1000 + 600) mod 604800000, the
+ * transmit time of that code period's start in ms of week. *anchor_epoch = -1 when there is no such HOW. */
+int gpsb200_nav_time_anchor(const gpsb200_nav_word_t *words, int64_t n, const gpsb200_nav_sync_t *sync,
+                            int32_t *anchor_epoch, int64_t *anchor_ms);
+
+/* ---- position, velocity and time from tracked channels (DESIGN §11; tests/pvt_model.py states it in numpy) -----------
+ * Fix instants: samples s = s0 + i step, i < nfix. Per channel c (epochs[c][0 .. nepochs[c]), in time order):
+ *   period     the k >= 1 with epochs[k].sample <= s < epochs[k + 1].sample (none: the channel is not used); its code
+ *              phase and step are phi_k = epochs[k-1].code_phase, u_k = epochs[k-1].code_step, its carrier step
+ *              w_k = epochs[k-1].carr_step
+ *   integers   phi = phi_k + (s - epochs[k].sample) u_k (2^-32 chips, uint64); T = (anchor_ms + k - anchor_epoch) mod
+ *              604800000 (whole ms of week); transmit time t_sv = T / 1000 + phi / (1023 2^32) / 1000 s of week
+ *   used       epochs[k-1].lock and epochs[k].lock, eph.valid, eph.health == 0 and |t_sv - toe| <= 7200 s (week-wrapped)
+ * Nominal receive time: the reference channel r is the lowest c with eph.valid and health 0; A = its anchor_ms,
+ * s_A = epochs[r][anchor_epoch].sample; t_nom(s) = A + 75 ms + (s - s_A) / 3e6 s. Pseudorange
+ * rho = c ((A + 75 + q - T) ms + (m / 3000 - phi / (1023 2^32)) ms) with s - s_A = 3000 q + m (0 <= m < 3000) and the
+ * whole-ms difference wrapped into half a week, so FP64 adds nothing above ~1 um. Range rate -lambda_L1 w_k 3e6 / 2^32.
+ * Per used channel (FP64, IS-GPS-200 20.3.3.3.3 / 20.3.3.4.3, the constants of gps.h:87-102): t = t_sv - dt, dt the
+ * af0..af2 polynomial at t_sv (t - toc week-wrapped); Kepler's equation by Newton from E = M until |dE| <= 1e-14 (at most
+ * 10 steps); satellite position and velocity (ECEF, at t); clock dt_sv = af0 + af1 d + af2 d^2 + F e sqrtA sin E - TGD
+ * (d = t - toc, F = -4.442807633e-10), clock drift af1 + 2 af2 d. Then Gauss-Newton on (x, y, z, b) from (0, 0, 0, 0),
+ * iteration j = 0 .. GPSB200_PVT_MAX_ITER - 1 at the estimate X_j:
+ *   flight time tau = |p - x_j| / c, p the satellite position; p rotated about z by -OMEGA_E tau (exact rotation);
+ *   model rho = |p_rot - x_j| + b_j - c dt_sv + I, I the Klobuchar delay (the reference's ionosphericDelay, gps.c:1893-1964,
+ *   with the config's alpha / beta, at the WGS-84 latitude / longitude of x_j, the azimuth / elevation of p_rot seen from
+ *   there, and the receive time t_nom - b_j / c) when cfg.iono and |x_j| >= 6e6 m, else 0;
+ *   rows (-(p_rot - x_j) / |p_rot - x_j|, 1); normal equations from the used channels; X_{j+1} = X_j + solve.
+ *   Status 2 as soon as |x_{j+1}| > 1e8 m (a diverging estimate: from the Earth's centre, Gauss-Newton on exactly four
+ *   satellites of poor geometry can run away) or the normal matrix is not positive definite. Otherwise converged after
+ *   the first j with |dx| < 1e-4 m: the fix is X_{j+1}; none after GPSB200_PVT_MAX_ITER: status 2.
+ * Velocity and clock drift: least squares with the same rows (at the last X_j) on rate + c drift_sv - e . v_sat, v_sat the
+ * satellite velocity rotated like p. Residuals (post-fit, m): rho - model - row . dX of the last iteration. PDOP:
+ * sqrt of the trace of the position block of (H^T H)^-1. Fewer than 4 used channels: status 1. */
+#define GPSB200_PVT_MAX_ITER 12
+enum { GPSB200_FIX_OK = 0, GPSB200_FIX_FEW = 1, GPSB200_FIX_NO_CONVERGENCE = 2 };
+typedef struct gpsb200_pvt_chan {
+    gpsb200_ephemeris_t eph;
+    int32_t prn;           /* for the caller's reference only */
+    int32_t anchor_epoch;  /* 0 <= anchor_epoch < nepochs[c] (gpsb200_nav_time_anchor) when eph.valid */
+    int64_t anchor_ms;     /* 0 <= anchor_ms < 604800000 when eph.valid */
+} gpsb200_pvt_chan_t;      /* 216 bytes */
+typedef struct gpsb200_pvt_config {
+    int64_t s0;            /* first fix instant (stream sample) */
+    int64_t step;          /* samples between fix instants, >= 1 */
+    int32_t nfix;          /* >= 1 */
+    int32_t iono;          /* 1: apply the Klobuchar delay with alpha / beta; 0: none */
+    double alpha[4], beta[4];
+} gpsb200_pvt_config_t;    /* 88 bytes */
+typedef struct gpsb200_fix {
+    int64_t sample;        /* the fix instant */
+    int32_t status;        /* GPSB200_FIX_*; the doubles below are NaN unless GPSB200_FIX_OK */
+    int32_t nused;         /* channels used */
+    uint32_t mask;         /* bit c: channel c used */
+    int32_t iterations;    /* Gauss-Newton iterations run */
+    double x, y, z;        /* ECEF, m */
+    double clock_m;        /* receiver clock bias b, m */
+    double t_rx;           /* receive time t_nom - b / c, s of week */
+    double vx, vy, vz;     /* ECEF, m/s */
+    double drift;          /* receiver clock drift, m/s */
+    double lat_deg, lon_deg, height;   /* WGS-84 */
+    double pdop;
+    double rms;            /* post-fit residual RMS over the used channels, m */
+} gpsb200_fix_t;           /* 136 bytes */
+/* Fixes at cfg->nfix instants from nchan (1..GPSB200_TRK_MAX_CHAN) channels: chans [nchan], epochs [nchan][max_epochs]
+ * host memory (row c holds nepochs[c] <= max_epochs records), fixes [nfix] out, residuals (NULL: not wanted)
+ * [nfix][nchan] out (NaN for channels not used). One ephemeris per channel per call. A channel with eph.valid == 0 is
+ * never used and its anchor is not checked, so a channel that has no ephemeris or no anchor yet (anchor_epoch -1) can
+ * keep its slot: bit c of every mask then stays channel c. Every argument is checked before
+ * anything is enqueued (GPSB200_ERR_ARG). Blocking: the epochs and channels go up once, the fixes come back in one
+ * download. */
+int gpsb200_pvt(gpsb200_ctx_t *ctx, const gpsb200_pvt_chan_t *chans, int nchan, const gpsb200_track_epoch_t *epochs,
+                const int32_t *nepochs, int max_epochs, const gpsb200_pvt_config_t *cfg, gpsb200_fix_t *fixes,
+                double *residuals);
+/* Re-run the fix kernel of the previous gpsb200_pvt call on its device-resident inputs, enqueued on `stream` (0 = the
+ * context's own stream), without transfers: for timing the kernel alone. GPSB200_ERR_ARG when there was no such call. */
+int gpsb200_pvt_replay(gpsb200_ctx_t *ctx, void *stream);
+
 /* ---- scenario engine: the reference's host path outside the sample loop -------------
  * RINEX-2/3 navigation file (plain or gzip-compressed, read through zlib like the reference, gps.c:1147) +
  * location/motion -> the gpsb200_chan_t records and NAV frames the

@@ -13,7 +13,8 @@ from .api import (  # noqa: F401
     ScenarioConfig, LiveScenario, SteerState, parse_steer, KEYS, ERR_END, almanac_read, ALMANAC_RECORD_DTYPE, checkpoint_segments_host, RUN_CKPT_DTYPE,
     carrier_probe_host, CARRIER_PROBE_DTYPE, AcqConfig, ACQ_RESULT_DTYPE, ACQ_CODE_SAMPLES, acq_window_samples,
     TRACK_STATE_DTYPE, TRACK_EPOCH_DTYPE, NAV_BIT_DTYPE, NAV_WORD_DTYPE, NAV_SYNC_DTYPE, track_start, nav_decode, nav_word_check,
-    nav_parity,
+    nav_parity, EPHEMERIS_DTYPE, IONO_DTYPE, PVT_CHAN_DTYPE, PVT_CONFIG_DTYPE, FIX_DTYPE, FIX_OK, FIX_FEW,
+    FIX_NO_CONVERGENCE, PVT_MAX_ITER, nav_words_of_frame, nav_ephemeris, nav_time_anchor, pvt_config,
 )
 from .synthetic import synthetic_chans  # noqa: F401,E402
 from . import sharding  # noqa: F401,E402

@@ -176,6 +176,77 @@ def nav_parity(data24, d29, d30):
     return int(lib().gpsb200_nav_parity(int(data24) & 0xFFFFFF, int(d29), int(d30)))
 
 
+# gpsb200_ephemeris_t / gpsb200_iono_t / gpsb200_pvt_chan_t / gpsb200_pvt_config_t / gpsb200_fix_t (DESIGN §11)
+EPHEMERIS_DTYPE = np.dtype([("valid", "<i4"), ("week", "<i4"), ("iodc", "<i4"), ("iode", "<i4"), ("health", "<i4"),
+                            ("ura", "<i4"), ("reserved", "<i4", 2), ("toc", "<f8"), ("af0", "<f8"), ("af1", "<f8"),
+                            ("af2", "<f8"), ("tgd", "<f8"), ("toe", "<f8"), ("m0", "<f8"), ("deltan", "<f8"), ("ecc", "<f8"),
+                            ("sqrta", "<f8"), ("omg0", "<f8"), ("inc0", "<f8"), ("aop", "<f8"), ("omgdot", "<f8"),
+                            ("idot", "<f8"), ("cuc", "<f8"), ("cus", "<f8"), ("crc", "<f8"), ("crs", "<f8"), ("cic", "<f8"),
+                            ("cis", "<f8")])
+IONO_DTYPE = np.dtype([("valid", "<i4"), ("reserved", "<i4"), ("alpha", "<f8", 4), ("beta", "<f8", 4)])
+PVT_CHAN_DTYPE = np.dtype([("eph", EPHEMERIS_DTYPE), ("prn", "<i4"), ("anchor_epoch", "<i4"), ("anchor_ms", "<i8")])
+PVT_CONFIG_DTYPE = np.dtype([("s0", "<i8"), ("step", "<i8"), ("nfix", "<i4"), ("iono", "<i4"), ("alpha", "<f8", 4),
+                             ("beta", "<f8", 4)])
+FIX_DTYPE = np.dtype([("sample", "<i8"), ("status", "<i4"), ("nused", "<i4"), ("mask", "<u4"), ("iterations", "<i4"),
+                      ("x", "<f8"), ("y", "<f8"), ("z", "<f8"), ("clock_m", "<f8"), ("t_rx", "<f8"), ("vx", "<f8"),
+                      ("vy", "<f8"), ("vz", "<f8"), ("drift", "<f8"), ("lat_deg", "<f8"), ("lon_deg", "<f8"),
+                      ("height", "<f8"), ("pdop", "<f8"), ("rms", "<f8")])
+assert (EPHEMERIS_DTYPE.itemsize, IONO_DTYPE.itemsize, PVT_CHAN_DTYPE.itemsize, PVT_CONFIG_DTYPE.itemsize,
+        FIX_DTYPE.itemsize) == (200, 72, 216, 88, 136)
+FIX_OK, FIX_FEW, FIX_NO_CONVERGENCE = 0, 1, 2
+PVT_MAX_ITER = 12
+
+
+def nav_words_of_frame(words60):
+    """The 60 NAV words of a frame slot as the scenario sends them (bits 29..0 used) -> NAV_WORD_DTYPE[60] records with
+    index 0..59, the parity verdict and data of gpsb200_nav_word_check, subframe id and TOW on HOW words (index % 10 == 1):
+    what gpsb200_nav_decode would return for a receiver that read the frame (sample = 0)."""
+    w = np.asarray(words60, np.uint32) & 0x3FFFFFFF
+    out = np.zeros(w.size, NAV_WORD_DTYPE)
+    prev = 0
+    for i, raw in enumerate(w):
+        ok, data = nav_word_check(int(raw), prev)
+        out[i]["raw"], out[i]["data"], out[i]["parity_ok"], out[i]["index"] = int(raw), data, int(ok), i
+        out[i]["subframe"], out[i]["tow"] = ((data >> 2) & 7, (data >> 7) & 0x1FFFF) if i % 10 == 1 else (0, -1)
+        prev = int(raw)
+    return out
+
+
+def nav_ephemeris(words):
+    """gpsb200_nav_ephemeris: the ephemeris of the last complete, consistent subframe 1-3 set and the Klobuchar terms of
+    the last subframe 4 page 18 in the word records (NAV_WORD_DTYPE, in order). -> (EPHEMERIS_DTYPE record, IONO_DTYPE
+    record); check their `valid`."""
+    w = np.ascontiguousarray(words, dtype=NAV_WORD_DTYPE)
+    eph, iono = np.zeros(1, EPHEMERIS_DTYPE), np.zeros(1, IONO_DTYPE)
+    rc = lib().gpsb200_nav_ephemeris(w.ctypes.data if w.size else None, w.size, eph.ctypes.data, iono.ctypes.data)
+    if rc:
+        raise GpsB200Error(rc, "gpsb200_nav_ephemeris")
+    return eph[0], iono[0]
+
+
+def nav_time_anchor(words, sync):
+    """gpsb200_nav_time_anchor: (anchor_epoch, anchor_ms) of a tracked channel from the words and sync nav_decode
+    returned for its epochs; anchor_epoch is -1 when no HOW passed parity."""
+    w = np.ascontiguousarray(words, dtype=NAV_WORD_DTYPE)
+    sy = np.array(sync, dtype=NAV_SYNC_DTYPE).reshape(1)
+    ep, ms = C.c_int32(0), C.c_int64(0)
+    rc = lib().gpsb200_nav_time_anchor(w.ctypes.data if w.size else None, w.size, sy.ctypes.data, C.byref(ep), C.byref(ms))
+    if rc:
+        raise GpsB200Error(rc, "gpsb200_nav_time_anchor")
+    return int(ep.value), int(ms.value)
+
+
+def pvt_config(s0, step, nfix, iono=None):
+    """A PVT_CONFIG_DTYPE record: fixes at samples s0 + i step, i < nfix; iono: (alpha[4], beta[4]) to apply the
+    Klobuchar delay with, or None for none."""
+    c = np.zeros(1, PVT_CONFIG_DTYPE)[0]
+    c["s0"], c["step"], c["nfix"] = int(s0), int(step), int(nfix)
+    if iono is not None:
+        c["iono"] = 1
+        c["alpha"], c["beta"] = np.asarray(iono[0], np.float64), np.asarray(iono[1], np.float64)
+    return c
+
+
 HANDOFF_FN = C.CFUNCTYPE(None, C.c_void_p, C.POINTER(C.c_int32), C.POINTER(C.c_double))     # gpsb200_handoff_fn
 
 _lib = None
@@ -184,7 +255,8 @@ EXPORTS = ["gpsb200_create", "gpsb200_destroy", "gpsb200_last_error", "gpsb200_v
            "gpsb200_synth_blocks", "gpsb200_synth_blocks_scatter", "gpsb200_synth_blocks_device", "gpsb200_replay_device",
            "gpsb200_carrier_advance", "gpsb200_carrier_chain", "gpsb200_carrier_chain_device", "gpsb200_carrier_probe_fixup",
            "gpsb200_codegen", "gpsb200_acquire", "gpsb200_acquire_device", "gpsb200_track_start", "gpsb200_track",
-           "gpsb200_track_device", "gpsb200_nav_decode", "gpsb200_nav_word_check", "gpsb200_nav_parity", "gpsb200_bind_numa", "gpsb200_span_chain_host", "gpsb200_lanes_model_block",
+           "gpsb200_track_device", "gpsb200_nav_decode", "gpsb200_nav_word_check", "gpsb200_nav_parity",
+           "gpsb200_nav_ephemeris", "gpsb200_nav_time_anchor", "gpsb200_pvt", "gpsb200_pvt_replay", "gpsb200_bind_numa", "gpsb200_span_chain_host", "gpsb200_lanes_model_block",
            "gpsb200_lanes_window_band_host", "gpsb200_slice_prepare", "gpsb200_slice_probe",
            "gpsb200_slice_finish", "gpsb200_slice_finish_cb", "gpsb200_slice_wait", "gpsb200_link_apply", "gpsb200_slice_link_host", "gpsb200_debug_corrupt_chain", "gpsb200_synth_kernel_name",
            "gpsb200_debug_run_checkpoints", "gpsb200_checkpoint_segments_host",
@@ -283,6 +355,12 @@ def lib():
         L.gpsb200_nav_word_check.argtypes = [C.c_uint32, C.c_uint32, C.POINTER(C.c_uint32)]
         L.gpsb200_nav_parity.argtypes = [C.c_uint32, C.c_int, C.c_int]
         L.gpsb200_nav_parity.restype = C.c_uint32
+        L.gpsb200_nav_ephemeris.argtypes = [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]
+        L.gpsb200_nav_time_anchor.argtypes = [C.c_void_p, C.c_int64, C.c_void_p, C.POINTER(C.c_int32),
+                                              C.POINTER(C.c_int64)]
+        L.gpsb200_pvt.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p,
+                                  C.c_void_p]
+        L.gpsb200_pvt_replay.argtypes = [C.c_void_p, C.c_void_p]
         _lib = L
     return _lib
 
@@ -813,6 +891,39 @@ class Context:
                                      out.ctypes.data, cnt.ctypes.data)
         self._check(rc)
         return [out[c, :cnt[c]].copy() for c in range(nchan)], st
+
+    def pvt(self, chans, epochs, cfg, want_residuals=False, nepochs=None):
+        """Position, velocity and time fixes (gpsb200_pvt; DESIGN §11). chans: PVT_CHAN_DTYPE[nchan] (ephemeris and time
+        anchor of each channel); epochs: a list of TRACK_EPOCH_DTYPE arrays, one per channel, in time order (as track
+        returns them, concatenated over calls), or, with nepochs (int32[nchan]), the [nchan, max_epochs] array as the C
+        call takes it; cfg: PVT_CONFIG_DTYPE record (pvt_config).
+        -> fixes FIX_DTYPE[nfix], and with want_residuals also the post-fit residuals float64[nfix, nchan] (NaN where a
+        channel is not used)."""
+        ch = np.ascontiguousarray(chans, dtype=PVT_CHAN_DTYPE).reshape(-1)
+        nchan = ch.size
+        if nepochs is not None:
+            ep = np.ascontiguousarray(epochs, dtype=TRACK_EPOCH_DTYPE)
+            n = np.ascontiguousarray(nepochs, dtype=np.int32)
+            assert ep.ndim == 2 and ep.shape[0] == n.size == nchan
+            me = ep.shape[1]
+        else:
+            n = np.array([len(e) for e in epochs], np.int32)
+            assert n.size == nchan
+            me = max(1, int(n.max()) if n.size else 1)
+            ep = np.zeros((max(1, nchan), me), TRACK_EPOCH_DTYPE)
+            for c, e in enumerate(epochs):
+                ep[c, :len(e)] = e
+        cf = np.array(cfg, dtype=PVT_CONFIG_DTYPE).reshape(1)
+        nfix = max(1, int(cf[0]["nfix"]))
+        fixes = np.zeros(nfix, FIX_DTYPE)
+        res = np.zeros((nfix, max(1, nchan))) if want_residuals else None
+        self._check(lib().gpsb200_pvt(self._h, ch.ctypes.data, nchan, ep.ctypes.data, n.ctypes.data, me, cf.ctypes.data,
+                                      fixes.ctypes.data, None if res is None else res.ctypes.data))
+        return (fixes, res) if want_residuals else fixes
+
+    def pvt_replay(self, stream=0):
+        """Enqueue the fix kernel of the previous pvt call again on `stream`, on its device-resident inputs (timing)."""
+        self._check(lib().gpsb200_pvt_replay(self._h, C.c_void_p(stream)))
 
     def replay_device(self, dst_ptr=0, stream=0, kernel_mask=15):
         self._check(lib().gpsb200_replay_device(self._h, C.c_void_p(dst_ptr), C.c_void_p(stream), kernel_mask))

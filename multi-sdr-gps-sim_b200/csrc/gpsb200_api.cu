@@ -30,6 +30,7 @@
 #include "../../include/gpsb200.h"
 #include "acquire.h"
 #include "track.h"
+#include "pvt.h"
 #include "nco_exact.h"
 #include "synth_kernels.h"
 #include "synth_lanes.h"
@@ -209,6 +210,7 @@ struct gpsb200_ctx {
     bool have_last = false;
     acq::Scratch acq;                      // acquisition searches (acquire.cu), allocated by the first one
     trk::Scratch trk;                      // tracking calls (track.cu), allocated by the first one
+    pvt::Scratch pvt;                      // position fixes (pvt.cu), allocated by the first one
     std::string err;
 };
 
@@ -1140,6 +1142,27 @@ int track(gpsb200_ctx *ctx, const void *iq, int64_t nsamples, int sample_size, i
     return GPSB200_OK;
 }
 
+// Position fixes (pvt.cu). Everything is checked before anything is enqueued.
+int pvt_fix(gpsb200_ctx *ctx, const gpsb200_pvt_chan_t *chans, int nchan, const gpsb200_track_epoch_t *epochs,
+            const int32_t *nepochs, int max_epochs, const gpsb200_pvt_config_t *cfg, gpsb200_fix_t *fixes,
+            double *residuals) {
+    if (!fixes) return fail(ctx, GPSB200_ERR_ARG, "gpsb200_pvt: NULL fixes");
+    const std::string bad = pvt::check(chans, nchan, epochs, nepochs, max_epochs, cfg);
+    if (!bad.empty()) return fail(ctx, GPSB200_ERR_ARG, "gpsb200_pvt: " + bad);
+    if (!ctx->s_compute) return fail(ctx, GPSB200_ERR_CUDA, "context has no CUDA device");
+    if (ctx->call.active) return fail(ctx, GPSB200_ERR_ARG, "a call begun with gpsb200_slice_prepare has not been finished");
+    CU(cudaSetDevice(ctx->cfg.device));
+    CU(pvt::run(ctx->pvt, chans, nchan, epochs, nepochs, max_epochs, cfg, fixes, residuals, ctx->s_compute));
+    return GPSB200_OK;
+}
+
+int pvt_replay(gpsb200_ctx *ctx, cudaStream_t s) {
+    if (!ctx->pvt.have_last) return fail(ctx, GPSB200_ERR_ARG, "gpsb200_pvt_replay: no previous gpsb200_pvt call");
+    CU(cudaSetDevice(ctx->cfg.device));
+    CU(pvt::replay(ctx->pvt, s));
+    return GPSB200_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -1447,6 +1470,7 @@ void gpsb200_destroy(gpsb200_ctx_t *ctx) {
     cudaFreeHost(ctx->h_seg_end);
     acq::scratch_free(ctx->acq);
     trk::scratch_free(ctx->trk);
+    pvt::scratch_free(ctx->pvt);
     if (ctx->s_compute) cudaStreamDestroy(ctx->s_compute);
     if (ctx->s_copy) cudaStreamDestroy(ctx->s_copy);
     if (ctx->s_pre) cudaStreamDestroy(ctx->s_pre);
@@ -1701,6 +1725,19 @@ int gpsb200_track_device(gpsb200_ctx_t *ctx, const void *iq_device, int64_t nsam
     cudaStream_t s = stream_ ? (cudaStream_t) stream_ : ctx->s_compute;
     return settle(ctx, s, track(ctx, iq_device, nsamples, sample_size, base, state, nchan, max_epochs, epochs, nepochs,
                                 true, s));
+}
+
+int gpsb200_pvt(gpsb200_ctx_t *ctx, const gpsb200_pvt_chan_t *chans, int nchan, const gpsb200_track_epoch_t *epochs,
+                const int32_t *nepochs, int max_epochs, const gpsb200_pvt_config_t *cfg, gpsb200_fix_t *fixes,
+                double *residuals) {
+    if (!ctx) return GPSB200_ERR_ARG;
+    return settle(ctx, nullptr, pvt_fix(ctx, chans, nchan, epochs, nepochs, max_epochs, cfg, fixes, residuals));
+}
+
+int gpsb200_pvt_replay(gpsb200_ctx_t *ctx, void *stream_) {
+    if (!ctx) return GPSB200_ERR_ARG;
+    cudaStream_t s = stream_ ? (cudaStream_t) stream_ : ctx->s_compute;
+    return settle(ctx, s, pvt_replay(ctx, s));
 }
 
 }  // extern "C"

@@ -1,7 +1,11 @@
 // Bit sync, frame sync and word decoding of the 50 bit/s navigation message from the epochs of one tracked channel
-// (include/gpsb200.h: gpsb200_nav_decode; DESIGN §10). Cheap and sequential: host code, shared by the CLI and Python.
+// (include/gpsb200.h: gpsb200_nav_decode; DESIGN §10), and the ephemeris, Klobuchar terms and transmit-time anchor the
+// words carry (gpsb200_nav_ephemeris, gpsb200_nav_time_anchor; DESIGN §11). Cheap and sequential: host code, shared by
+// the CLI and Python.
 #include <stdint.h>
 
+#include <cmath>
+#include <cstring>
 #include <vector>
 
 #include "../../include/gpsb200.h"
@@ -36,6 +40,20 @@ uint32_t bits_word(const std::vector<int> &v, int64_t i, int n) {
     for (int k = 0; k < n; k++) w = (w << 1) | (uint32_t) v[i + k];
     return w;
 }
+
+// The low `bits` bits of v as a two's complement integer.
+double sext(uint32_t v, int bits) {
+    const int64_t m = (int64_t) v & ((1ll << bits) - 1);
+    return (double) (m >= (1ll << (bits - 1)) ? m - (1ll << bits) : m);
+}
+
+// A 32-bit field split 8 + 24 over two words: the low 8 data bits of `hi`, all 24 of `lo`.
+int32_t split32(uint32_t hi, uint32_t lo) { return (int32_t) (((hi & 0xFFu) << 24) | (lo & 0xFFFFFFu)); }
+
+// IS-GPS-200 scale factors; semicircles are turned into radians with the reference's pi (gps.h:91).
+const double kPi = 3.1415926535898;
+const double kP2m5 = 0.03125, kP2m19 = 1.0 / 524288.0, kP2m29 = 1.0 / 536870912.0, kP2m31 = 1.0 / 2147483648.0,
+             kP2m33 = 1.0 / 8589934592.0, kP2m43 = 1.0 / 8796093022208.0, kP2m55 = 1.0 / 36028797018963968.0;
 
 }  // namespace
 
@@ -125,6 +143,91 @@ int gpsb200_nav_decode(const gpsb200_track_epoch_t *ep, int64_t n, gpsb200_nav_b
         }
     }
     *sync = sy;
+    return GPSB200_OK;
+}
+
+int gpsb200_nav_ephemeris(const gpsb200_nav_word_t *words, int64_t n, gpsb200_ephemeris_t *eph, gpsb200_iono_t *iono) {
+    if (!eph || n < 0 || (n > 0 && !words)) return GPSB200_ERR_ARG;
+    memset(eph, 0, sizeof *eph);
+    if (iono) memset(iono, 0, sizeof *iono);
+    // subframe starts: a TLM (index a multiple of 10) with its 9 successors in sequence and all 10 with good parity
+    auto good_subframe = [&](int64_t i) -> int {
+        if (i < 0 || i + 10 > n || words[i].index % 10 != 0) return 0;
+        for (int j = 0; j < 10; j++)
+            if (words[i + j].index != words[i].index + j || !words[i + j].parity_ok) return 0;
+        return (int) ((words[i + 1].data >> 2) & 7u);
+    };
+    for (int64_t i = n - 30; i >= 0; i--) {
+        if (good_subframe(i) != 1 || good_subframe(i + 10) != 2 || good_subframe(i + 20) != 3) continue;
+        const gpsb200_nav_word_t *s1 = words + i, *s2 = words + i + 10, *s3 = words + i + 20;
+        const int32_t iodc = (int32_t) (((s1[2].data & 3u) << 8) | ((s1[7].data >> 16) & 0xFFu));
+        const int32_t iode2 = (int32_t) ((s2[2].data >> 16) & 0xFFu), iode3 = (int32_t) ((s3[9].data >> 16) & 0xFFu);
+        if (iode2 != iode3 || iode2 != (iodc & 0xFF)) continue;
+        gpsb200_ephemeris_t &e = *eph;
+        e.week = (int32_t) ((s1[2].data >> 14) & 0x3FFu);
+        e.ura = (int32_t) ((s1[2].data >> 8) & 0xFu);
+        e.health = (int32_t) ((s1[2].data >> 2) & 0x3Fu);
+        e.iodc = iodc;
+        e.iode = iode2;
+        e.tgd = sext(s1[6].data, 8) * kP2m31;
+        e.toc = (double) (s1[7].data & 0xFFFFu) * 16.0;
+        e.af2 = sext(s1[8].data >> 16, 8) * kP2m55;
+        e.af1 = sext(s1[8].data, 16) * kP2m43;
+        e.af0 = sext(s1[9].data >> 2, 22) * kP2m31;
+        e.crs = sext(s2[2].data, 16) * kP2m5;
+        e.deltan = sext(s2[3].data >> 8, 16) * kP2m43 * kPi;
+        e.m0 = (double) split32(s2[3].data, s2[4].data) * kP2m31 * kPi;
+        e.cuc = sext(s2[5].data >> 8, 16) * kP2m29;
+        e.ecc = (double) (uint32_t) split32(s2[5].data, s2[6].data) * kP2m33;
+        e.cus = sext(s2[7].data >> 8, 16) * kP2m29;
+        e.sqrta = (double) (uint32_t) split32(s2[7].data, s2[8].data) * kP2m19;
+        e.toe = (double) ((s2[9].data >> 8) & 0xFFFFu) * 16.0;
+        e.cic = sext(s3[2].data >> 8, 16) * kP2m29;
+        e.omg0 = (double) split32(s3[2].data, s3[3].data) * kP2m31 * kPi;
+        e.cis = sext(s3[4].data >> 8, 16) * kP2m29;
+        e.inc0 = (double) split32(s3[4].data, s3[5].data) * kP2m31 * kPi;
+        e.crc = sext(s3[6].data >> 8, 16) * kP2m5;
+        e.aop = (double) split32(s3[6].data, s3[7].data) * kP2m31 * kPi;
+        e.omgdot = sext(s3[8].data, 24) * kP2m43 * kPi;
+        e.idot = sext(s3[9].data >> 2, 14) * kP2m43 * kPi;
+        e.valid = 1;
+        break;
+    }
+    if (iono)
+        for (int64_t i = n - 10; i >= 0; i--) {
+            if (good_subframe(i) != 4) continue;
+            const gpsb200_nav_word_t *s = words + i;
+            if (((s[2].data >> 22) & 3u) != 1u || ((s[2].data >> 16) & 0x3Fu) != 56u) continue;
+            iono->alpha[0] = sext(s[2].data >> 8, 8) * std::ldexp(1.0, -30);
+            iono->alpha[1] = sext(s[2].data, 8) * std::ldexp(1.0, -27);
+            iono->alpha[2] = sext(s[3].data >> 16, 8) * std::ldexp(1.0, -24);
+            iono->alpha[3] = sext(s[3].data >> 8, 8) * std::ldexp(1.0, -24);
+            iono->beta[0] = sext(s[3].data, 8) * 2048.0;
+            iono->beta[1] = sext(s[4].data >> 16, 8) * 16384.0;
+            iono->beta[2] = sext(s[4].data >> 8, 8) * 65536.0;
+            iono->beta[3] = sext(s[4].data, 8) * 65536.0;
+            iono->valid = 1;
+            break;
+        }
+    return GPSB200_OK;
+}
+
+int gpsb200_nav_time_anchor(const gpsb200_nav_word_t *words, int64_t n, const gpsb200_nav_sync_t *sync,
+                            int32_t *anchor_epoch, int64_t *anchor_ms) {
+    if (!sync || !anchor_epoch || !anchor_ms || n < 0 || (n > 0 && !words)) return GPSB200_ERR_ARG;
+    *anchor_epoch = -1;
+    *anchor_ms = 0;
+    if (sync->bit_edge < 0 || sync->frame_bit < 0) return GPSB200_OK;
+    for (int64_t i = 0; i < n; i++) {
+        const gpsb200_nav_word_t &w = words[i];
+        if (w.index % 10 != 1 || !w.parity_ok || w.tow < 0) continue;
+        const int64_t ep = (int64_t) sync->bit_edge + 20 * ((int64_t) sync->frame_bit + 30 * (int64_t) w.index);
+        if (ep > INT32_MAX) return GPSB200_OK;
+        const int64_t week_ms = 604800000;
+        *anchor_epoch = (int32_t) ep;
+        *anchor_ms = (((6 * (int64_t) w.tow - 6) * 1000 + 600) % week_ms + week_ms) % week_ms;
+        return GPSB200_OK;
+    }
     return GPSB200_OK;
 }
 

@@ -1,0 +1,46 @@
+// Position, velocity and time from tracked channels (include/gpsb200.h: gpsb200_pvt; DESIGN §11).
+#pragma once
+#include <cuda_runtime.h>
+#include <stdint.h>
+
+#include <string>
+
+#include "../../include/gpsb200.h"
+
+namespace gpsb200 {
+namespace pvt {
+
+constexpr int kWarps = 4;                // fixes per CTA of k_pvt (one warp each)
+constexpr int64_t kWeekMs = 604800000;   // ms of a GPS week
+
+// Empty when the call is well-formed (see the header).
+std::string check(const gpsb200_pvt_chan_t *chans, int nchan, const gpsb200_track_epoch_t *epochs, const int32_t *nepochs,
+                  int max_epochs, const gpsb200_pvt_config_t *cfg);
+
+// Device scratch of the fix calls of one context, grown as needed, and what gpsb200_pvt_replay re-runs.
+struct Scratch {
+    gpsb200_track_epoch_t *d_epochs = nullptr;   // [nchan][max_epochs]
+    size_t epoch_cap = 0;
+    gpsb200_pvt_chan_t *d_chans = nullptr;       // [GPSB200_TRK_MAX_CHAN]
+    int32_t *d_n = nullptr;                      // [GPSB200_TRK_MAX_CHAN]
+    gpsb200_fix_t *d_fixes = nullptr;            // [nfix]
+    size_t fix_cap = 0;
+    double *d_res = nullptr;                     // [nfix][nchan]
+    size_t res_cap = 0;
+    bool have_last = false;                      // the arguments of the previous call, for replay
+    int nchan = 0, max_epochs = 0, ref = -1;
+    int64_t ref_sample = 0, ref_ms = 0;
+    gpsb200_pvt_config_t cfg{};
+    bool want_res = false;
+};
+
+void scratch_free(Scratch &sc);
+// Upload, run k_pvt on s and download the fixes (and residuals when not NULL); waits for the results.
+cudaError_t run(Scratch &sc, const gpsb200_pvt_chan_t *chans, int nchan, const gpsb200_track_epoch_t *epochs,
+                const int32_t *nepochs, int max_epochs, const gpsb200_pvt_config_t *cfg, gpsb200_fix_t *fixes,
+                double *residuals, cudaStream_t s);
+// Enqueue k_pvt again on the previous call's device-resident inputs.
+cudaError_t replay(Scratch &sc, cudaStream_t s);
+
+}  // namespace pvt
+}  // namespace gpsb200

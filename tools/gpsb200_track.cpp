@@ -4,6 +4,10 @@
 // within their pull-in range); every PRN whose P1/P2 reaches the threshold is tracked with gpsb200_track over the file,
 // read in chunks of one second, and decoded with gpsb200_nav_decode. Prints one line per tracked PRN: locked at the
 // end or not, the Doppler at the end, subframes found, words with good parity and the first TOW (DESIGN §10).
+// With --fix it then computes position fixes with gpsb200_pvt from what it decoded alone: each channel's ephemeris
+// (gpsb200_nav_ephemeris) and time anchor (gpsb200_nav_time_anchor); channels without both are left out. The fixes
+// start 0.5 s after the acquisition window (the loops have pulled in by then) and follow every --fix-every ms; one line
+// per fix with status GPSB200_FIX_OK (DESIGN §11).
 #include <sys/stat.h>
 
 #include <algorithm>
@@ -20,16 +24,21 @@ static const double kDefaultThreshold = 2.5;      // as gpsb200-acq
 static const int kAcqMs = 10;
 static const double kAcqLo = -5000.0, kAcqHi = 5000.0, kAcqStep = 100.0;
 static const long long kChunk = 3000000;          // samples per tracking call: 1 s
+static const int kDefaultFixEvery = 1000;         // ms between fixes
+static const long long kFixLead = 1500000;        // samples from the start to the first fix: 0.5 s of pull-in
 
 static void usage() {
     fprintf(stderr,
             "gpsb200-track FILE [--iq16] [--block B] [--offset-ms N] [--ms K] [--prn LIST] [--threshold R] [--device D]\n"
+            "              [--fix [--fix-every MS] [--iono a0,a1,a2,a3,b0,b1,b2,b3]]\n"
             "  FILE              interleaved I,Q at 3 Msps, int8 (default) or int16 (--iq16)\n"
             "  --block B         start at 0.1 s block B (sample 300000 B); --offset-ms N adds N ms (3000 N samples)\n"
             "  --ms K            track K ms of signal from the start (default: to the end of the file)\n"
             "  --prn LIST        PRNs searched, e.g. 1-32 (default), 3,7,12-15\n"
-            "  --threshold R     P1/P2 at or above R counts as acquired and is tracked (default %.1f)\n",
-            kDefaultThreshold);
+            "  --threshold R     P1/P2 at or above R counts as acquired and is tracked (default %.1f)\n"
+            "  --fix             position, velocity and time from the decoded ephemeris and TOW, every --fix-every ms\n"
+            "                    (default %d) from 0.5 s after the start; --iono: the Klobuchar alpha / beta to apply\n",
+            kDefaultThreshold, kDefaultFixEvery);
     exit(2);
 }
 
@@ -62,11 +71,49 @@ static bool read_at(FILE *f, long long s0, long long n, size_t elem, std::vector
     return fseeko(f, (off_t) (s0 * 2 * (long long) elem), SEEK_SET) == 0 && fread(buf.data(), 1, buf.size(), f) == buf.size();
 }
 
+// Fixes from `first` every `step` samples to the last epoch of the channels, one line per fix with status OK.
+static int print_fixes(gpsb200_ctx_t *ctx, const std::vector<gpsb200_pvt_chan_t> &chans, const std::vector<int> &of,
+                       const std::vector<std::vector<gpsb200_track_epoch_t>> &eps, long long first, long long step,
+                       gpsb200_pvt_config_t cfg) {
+    const int n = (int) chans.size();
+    printf("# fixes: %d channel(s) with an ephemeris and a time anchor decoded, Klobuchar %s\n", n, cfg.iono ? "on" : "off");
+    if (n == 0) return GPSB200_OK;
+    size_t me = 1;
+    long long end = 0;
+    for (int c : of) {
+        me = std::max(me, eps[c].size());
+        if (!eps[c].empty()) end = std::max(end, (long long) eps[c].back().sample);
+    }
+    if (end < first) return GPSB200_OK;
+    std::vector<gpsb200_track_epoch_t> all((size_t) n * me);
+    std::vector<int32_t> cnt(n);
+    for (int k = 0; k < n; k++) {
+        std::copy(eps[of[k]].begin(), eps[of[k]].end(), all.begin() + (size_t) k * me);
+        cnt[k] = (int32_t) eps[of[k]].size();
+    }
+    cfg.s0 = first;
+    cfg.step = step;
+    cfg.nfix = (int32_t) ((end - first) / step + 1);
+    std::vector<gpsb200_fix_t> fx(cfg.nfix);
+    const int rc = gpsb200_pvt(ctx, chans.data(), n, all.data(), cnt.data(), (int) me, &cfg, fx.data(), nullptr);
+    if (rc != GPSB200_OK) return rc;
+    printf("# sample  tow_s  lat_deg  lon_deg  height_m  clock_m  vx  vy  vz (ECEF m/s)  channels  pdop\n");
+    for (const auto &f : fx)
+        if (f.status == GPSB200_FIX_OK)
+            printf("%lld  %.9f  %.8f  %.8f  %.3f  %.3f  %.3f  %.3f  %.3f  %d  %.2f\n", (long long) f.sample, f.t_rx,
+                   f.lat_deg, f.lon_deg, f.height, f.clock_m, f.vx, f.vy, f.vz, f.nused, f.pdop);
+    return GPSB200_OK;
+}
+
 int main(int argc, char **argv) {
     const char *path = nullptr;
     int ss = GPSB200_SC08, device = 0;
     long long block = 0, offset_ms = 0, ms = -1;
     double threshold = kDefaultThreshold;
+    bool fix = false;
+    long long fix_every = kDefaultFixEvery;
+    gpsb200_pvt_config_t pcfg;
+    memset(&pcfg, 0, sizeof pcfg);
     gpsb200_acq_config_t cfg;
     memset(&cfg, 0, sizeof cfg);
     cfg.ms = kAcqMs;
@@ -85,10 +132,18 @@ int main(int argc, char **argv) {
             if (!parse_prns(val(), &cfg)) usage();
         } else if (a == "--threshold") threshold = atof(val());
         else if (a == "--device") device = atoi(val());
+        else if (a == "--fix") fix = true;
+        else if (a == "--fix-every") fix_every = atoll(val());
+        else if (a == "--iono") {
+            double *v[8] = {&pcfg.alpha[0], &pcfg.alpha[1], &pcfg.alpha[2], &pcfg.alpha[3],
+                            &pcfg.beta[0], &pcfg.beta[1], &pcfg.beta[2], &pcfg.beta[3]};
+            if (sscanf(val(), "%lf,%lf,%lf,%lf,%lf,%lf,%lf,%lf", v[0], v[1], v[2], v[3], v[4], v[5], v[6], v[7]) != 8) usage();
+            pcfg.iono = 1;
+        }
         else if (a[0] != '-' && !path) path = argv[i];
         else usage();
     }
-    if (!path || block < 0 || offset_ms < 0 || ms == 0 || ms < -1) usage();
+    if (!path || block < 0 || offset_ms < 0 || ms == 0 || ms < -1 || fix_every < 1) usage();
     cfg.f_lo_hz = kAcqLo;
     cfg.step_hz = kAcqStep;
     cfg.nbins = (int) std::floor((kAcqHi - kAcqLo) / kAcqStep + 1e-9) + 1;
@@ -160,10 +215,11 @@ int main(int argc, char **argv) {
         gpsb200_destroy(ctx);
         return 1;
     }
-    gpsb200_destroy(ctx);
     printf("# %s: sample %lld to %lld, %d of %d PRNs acquired (P1/P2 >= %.2f) and tracked\n", path, s0, end, nch, cfg.nprn,
            threshold);
     printf("# PRN  locked  doppler_hz  subframes  words_ok  words  first_tow\n");
+    std::vector<gpsb200_pvt_chan_t> fix_chans;
+    std::vector<int> fix_of;
     for (int c = 0; c < nch; c++) {
         const auto &e = eps[c];
         const int64_t ne = (int64_t) e.size();
@@ -175,6 +231,20 @@ int main(int argc, char **argv) {
         const double dopp = ne > 0 ? e.back().carr_step * 3e6 / 4294967296.0 : 0.0;
         printf("%5d  %6s  %10.1f  %9d  %8d  %5d  %9d\n", state[c].prn, locked ? "yes" : "no", dopp, sy.subframes,
                sy.words_ok, sy.nwords, sy.first_tow);
+        if (fix) {
+            gpsb200_pvt_chan_t pc;
+            memset(&pc, 0, sizeof pc);
+            gpsb200_nav_ephemeris(words.data(), sy.nwords, &pc.eph, nullptr);
+            gpsb200_nav_time_anchor(words.data(), sy.nwords, &sy, &pc.anchor_epoch, &pc.anchor_ms);
+            pc.prn = state[c].prn;
+            if (pc.eph.valid && pc.anchor_epoch >= 0) {
+                fix_chans.push_back(pc);
+                fix_of.push_back(c);
+            }
+        }
     }
-    return 0;
+    if (fix) rc = print_fixes(ctx, fix_chans, fix_of, eps, s0 + kFixLead, fix_every * GPSB200_ACQ_CODE_SAMPLES, pcfg);
+    if (rc != GPSB200_OK) fprintf(stderr, "gpsb200-track: %s\n", gpsb200_last_error(ctx));
+    gpsb200_destroy(ctx);
+    return rc == GPSB200_OK ? 0 : 1;
 }

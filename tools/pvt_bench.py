@@ -1,0 +1,123 @@
+"""Time the position fix on one GPU and print one JSON line.
+
+Workload: 32 channels, 600 s of ideal epochs (tests/pvt_truth.py: what a perfect loop would record, built from the
+scenario engine's records of the 32-satellite sky at the fixtures' Tokyo location), the ephemeris from the scenario's
+NAV frames, a fix every 1 ms: 600 000 fixes in one gpsb200_pvt call. The epochs (32 x 600 001 records of 56 B, 1.08 GB)
+go up in that call, from pinned host memory.
+
+Reported: device-event time of the whole call (uploads, kernel, download; median over --iters after --warmup) and of
+the kernel alone (gpsb200_pvt_replay, median over --iters), fixes per second of kernel time, the fixes' status counts,
+and the largest difference from the numpy model (tests/pvt_model.py) over a seeded sample of --check fix instants. The
+card's name, power limit and maximum SM clock are read in the same run (nvidia-smi). Writes nothing; needs a GPU.
+
+    python tools/pvt_bench.py [--iters 5] [--warmup 1] [--check 64] [--seconds 600]
+"""
+import argparse
+import importlib
+import json
+import os
+import subprocess
+import sys
+import tempfile
+
+import numpy as np
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.join(ROOT, "tests"))
+gps = importlib.import_module("multi-sdr-gps-sim_b200")
+import pvt_model as PM   # noqa: E402
+import pvt_truth as PT   # noqa: E402
+
+LOC = (35.681298, 139.766247, 10.0)
+START = (2024, 1, 7, 2, 0, 0.0)
+
+
+def card():
+    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader,nounits",
+                        "-i", "0"], capture_output=True, text=True, check=True).stdout.strip().split(",")
+    return q[0].strip(), float(q[1]), float(q[2])
+
+
+def workload(seconds):
+    with tempfile.TemporaryDirectory() as d:
+        nav = os.path.join(d, "sky32.nav")
+        subprocess.check_call([sys.executable, os.path.join(ROOT, "oracle", "gen_rinex.py"), "--nsat", "32", "--out", nav])
+        ch, frames = gps.scenario(nav, *LOC, seconds=seconds + 0.2, max_chan=32, start=START)
+        _, alpha, beta = PT.read_rinex(nav)
+    fob = ch["nav_frame"][:, 0]
+    prns = sorted({int(p) for p in np.unique(ch["prn"]) if p > 0})
+    chans = np.zeros(len(prns), gps.PVT_CHAN_DTYPE)
+    eps = []
+    for c, prn in enumerate(prns):
+        e, ae, ams = PT.ideal_epochs(ch, prn, frames, fob)
+        eps.append(e)
+        b = int(np.nonzero((ch["prn"] == prn).any(1))[0][0])
+        slot = int(np.nonzero(ch[b]["prn"] == prn)[0][0])
+        chans[c]["eph"] = gps.nav_ephemeris(gps.nav_words_of_frame(frames[int(fob[b])][slot]))[0]
+        chans[c]["prn"], chans[c]["anchor_epoch"], chans[c]["anchor_ms"] = prn, ae, ams
+    return chans, eps, PT.klobuchar_broadcast(alpha, beta)
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--iters", type=int, default=5)
+    ap.add_argument("--warmup", type=int, default=1)
+    ap.add_argument("--check", type=int, default=64)
+    ap.add_argument("--seconds", type=int, default=600)
+    args = ap.parse_args()
+    import torch
+    if not torch.cuda.is_available():
+        raise SystemExit("pvt_bench: no CUDA device (this measurement has no CPU fallback)")
+    name, power_w, clk_mhz = card()
+    chans, eps, iono = workload(args.seconds)
+    nfix = args.seconds * 1000
+    cfg = gps.pvt_config(3000, 3000, nfix, iono)
+    # the epochs packed once as the C call takes them, in pinned memory
+    n = np.array([len(e) for e in eps], np.int32)
+    host = torch.empty(len(eps) * int(n.max()) * gps.TRACK_EPOCH_DTYPE.itemsize, dtype=torch.uint8, pin_memory=True)
+    packed = host.numpy().view(gps.TRACK_EPOCH_DTYPE).reshape(len(eps), int(n.max()))
+    for c, e in enumerate(eps):
+        packed[c, :len(e)] = e
+    stream = torch.cuda.Stream()
+    call, kern = [], []
+    with gps.Context(1, 1) as ctx:
+        for _ in range(args.warmup):
+            fix = ctx.pvt(chans, packed, cfg, nepochs=n)
+        for _ in range(args.iters):
+            a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            a.record(stream)
+            fix = ctx.pvt(chans, packed, cfg, nepochs=n)
+            b.record(stream)
+            b.synchronize()
+            call.append(a.elapsed_time(b))
+        ctx.pvt_replay(stream.cuda_stream)
+        for _ in range(args.iters):
+            a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            a.record(stream)
+            ctx.pvt_replay(stream.cuda_stream)
+            b.record(stream)
+            b.synchronize()
+            kern.append(a.elapsed_time(b))
+    rng = np.random.default_rng(1)
+    worst = {f: 0.0 for f in ("x", "y", "z", "clock_m", "vx", "vy", "vz")}
+    for i in rng.choice(nfix, size=min(args.check, nfix), replace=False):
+        one = gps.pvt_config(int(cfg["s0"]) + int(i) * int(cfg["step"]), 1, 1, iono)
+        want, _, _ = PM.pvt(chans, eps, one)
+        assert int(want["status"][0]) == int(fix["status"][i]) and int(want["mask"][0]) == int(fix["mask"][i])
+        for f in worst:
+            if fix["status"][i] == gps.FIX_OK:
+                worst[f] = max(worst[f], abs(float(fix[f][i]) - float(want[f][0])))
+    t_call, t_kern = float(np.median(call)), float(np.median(kern))
+    st = {int(k): int(v) for k, v in zip(*np.unique(fix["status"], return_counts=True))}
+    print(json.dumps({"tool": "pvt_bench", "gpu": name, "power_limit_w": power_w, "sm_clock_max_mhz": clk_mhz,
+                      "channels": len(eps), "seconds": args.seconds, "fixes": nfix, "epochs_per_channel": max(map(len, eps)),
+                      "call_ms_median": round(t_call, 3), "call_ms_min": round(float(np.min(call)), 3),
+                      "kernel_ms_median": round(t_kern, 3), "kernel_ms_min": round(float(np.min(kern)), 3),
+                      "iters": args.iters, "fixes_per_s_kernel": round(nfix / (t_kern * 1e-3)),
+                      "status_counts": st, "checked": min(args.check, nfix),
+                      "max_abs_diff_vs_model": {k: float("%.3g" % v) for k, v in worst.items()}}), flush=True)
+
+
+if __name__ == "__main__":
+    main()
