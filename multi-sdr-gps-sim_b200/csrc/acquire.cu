@@ -15,6 +15,7 @@
 #include <vector>
 
 #include "acquire.h"
+#include "device_buffer.h"
 #include "rx_samples.cuh"
 #include "synth_tables.h"
 
@@ -255,52 +256,30 @@ std::string check(const gpsb200_acq_config_t *cfg, int64_t nsamples, int sample_
     return std::string();
 }
 
-#define ACQ_CU(call)                              \
-    do {                                          \
-        cudaError_t e_ = (call);                  \
-        if (e_ != cudaSuccess) return e_;         \
-    } while (0)
-
 cudaError_t scratch_reserve(Scratch &sc, const gpsb200_acq_config_t *cfg, bool want_grid) {
     if (!sc.d_edges) {
         std::vector<int16_t> e((size_t) 33 * kMaxEdges, 0);
         std::vector<int32_t> n(33, 0);
         for (int prn = 1; prn <= 32; prn++) n[prn] = replica_edges(prn, e.data() + (size_t) prn * kMaxEdges);
-        ACQ_CU(cudaMalloc(&sc.d_edges, e.size() * sizeof(int16_t)));
-        ACQ_CU(cudaMemcpy(sc.d_edges, e.data(), e.size() * sizeof(int16_t), cudaMemcpyHostToDevice));
-        ACQ_CU(cudaMalloc(&sc.d_nedges, n.size() * sizeof(int32_t)));
-        ACQ_CU(cudaMemcpy(sc.d_nedges, n.data(), n.size() * sizeof(int32_t), cudaMemcpyHostToDevice));
-        ACQ_CU(cudaMalloc(&sc.d_res, 32 * sizeof(gpsb200_acq_result_t)));
-        ACQ_CU(cudaHostAlloc(&sc.h_res, 32 * sizeof(gpsb200_acq_result_t), cudaHostAllocDefault));
-        ACQ_CU(cudaMalloc(&sc.d_prn, 32 * sizeof(int32_t)));
-        ACQ_CU(cudaFuncSetAttribute(k_acq_grid<int8_t>, cudaFuncAttributeMaxDynamicSharedMemorySize, sizeof(Smem)));
-        ACQ_CU(cudaFuncSetAttribute(k_acq_grid<int16_t>, cudaFuncAttributeMaxDynamicSharedMemorySize, sizeof(Smem)));
+        CU_RET(cudaMalloc(&sc.d_edges, e.size() * sizeof(int16_t)));
+        CU_RET(cudaMemcpy(sc.d_edges, e.data(), e.size() * sizeof(int16_t), cudaMemcpyHostToDevice));
+        CU_RET(cudaMalloc(&sc.d_nedges, n.size() * sizeof(int32_t)));
+        CU_RET(cudaMemcpy(sc.d_nedges, n.data(), n.size() * sizeof(int32_t), cudaMemcpyHostToDevice));
+        CU_RET(cudaMalloc(&sc.d_res, 32 * sizeof(gpsb200_acq_result_t)));
+        CU_RET(cudaHostAlloc(&sc.h_res, 32 * sizeof(gpsb200_acq_result_t), cudaHostAllocDefault));
+        CU_RET(cudaMalloc(&sc.d_prn, 32 * sizeof(int32_t)));
+        CU_RET(cudaFuncSetAttribute(k_acq_grid<int8_t>, cudaFuncAttributeMaxDynamicSharedMemorySize, sizeof(Smem)));
+        CU_RET(cudaFuncSetAttribute(k_acq_grid<int16_t>, cudaFuncAttributeMaxDynamicSharedMemorySize, sizeof(Smem)));
     }
-    if (cfg->nbins > sc.max_bins) {
-        cudaFree(sc.d_rows);
-        cudaFree(sc.d_u);
-        sc.d_rows = nullptr;
-        sc.d_u = nullptr;
-        sc.max_bins = 0;
-        ACQ_CU(cudaMalloc(&sc.d_rows, (size_t) 32 * cfg->nbins * 3 * sizeof(uint64_t)));
-        ACQ_CU(cudaMalloc(&sc.d_u, (size_t) cfg->nbins * sizeof(uint32_t)));
-        sc.max_bins = cfg->nbins;
-    }
-    const size_t gb = want_grid ? (size_t) cfg->nprn * cfg->nbins * kCode * sizeof(uint64_t) : 0;
-    if (gb > sc.grid_bytes) {
-        cudaFree(sc.d_grid);
-        sc.d_grid = nullptr;
-        sc.grid_bytes = 0;
-        ACQ_CU(cudaMalloc(&sc.d_grid, gb));
-        sc.grid_bytes = gb;
-    }
+    CU_RET(grow(sc.d_rows, sc.rows_cap, (size_t) 32 * cfg->nbins * 3));
+    CU_RET(grow(sc.d_u, sc.u_cap, (size_t) cfg->nbins));
+    if (want_grid) CU_RET(grow(sc.d_grid, sc.grid_cap, (size_t) cfg->nprn * cfg->nbins * kCode));
     return cudaSuccess;
 }
 
 void scratch_free(Scratch &sc) {
     cudaFree(sc.d_edges);
     cudaFree(sc.d_nedges);
-    cudaFree(sc.d_window);
     cudaFree(sc.d_grid);
     cudaFree(sc.d_rows);
     cudaFree(sc.d_res);
@@ -315,8 +294,8 @@ cudaError_t launch(Scratch &sc, const void *window, int sample_size, const gpsb2
     // the small parameter arrays go up by value in the stream order (the host copies are on this call's stack)
     std::vector<uint32_t> u(cfg->nbins);
     for (int j = 0; j < cfg->nbins; j++) u[j] = phase_step(cfg->f_lo_hz + (double) j * cfg->step_hz);
-    ACQ_CU(cudaMemcpyAsync(sc.d_u, u.data(), u.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, s));
-    ACQ_CU(cudaMemcpyAsync(sc.d_prn, cfg->prn, cfg->nprn * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+    CU_RET(cudaMemcpyAsync(sc.d_u, u.data(), u.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, s));
+    CU_RET(cudaMemcpyAsync(sc.d_prn, cfg->prn, cfg->nprn * sizeof(int32_t), cudaMemcpyHostToDevice, s));
     const dim3 grid(cfg->nbins, cfg->nprn);
     uint64_t *g = want_grid ? sc.d_grid : nullptr;
     if (sample_size == GPSB200_SC08)
@@ -326,10 +305,10 @@ cudaError_t launch(Scratch &sc, const void *window, int sample_size, const gpsb2
         k_acq_grid<int16_t><<<grid, kThreads, sizeof(Smem), s>>>(static_cast<const int16_t *>(window), sc.d_edges,
                                                                  sc.d_nedges, sc.d_prn, sc.d_u, cfg->ms, cfg->nbins, g,
                                                                  sc.d_rows);
-    ACQ_CU(cudaGetLastError());
+    CU_RET(cudaGetLastError());
     k_acq_pick<<<cfg->nprn, 32, 0, s>>>(sc.d_rows, sc.d_prn, cfg->nbins, cfg->f_lo_hz, cfg->step_hz, sc.d_res);
-    ACQ_CU(cudaGetLastError());
-    ACQ_CU(cudaMemcpyAsync(sc.h_res, sc.d_res, cfg->nprn * sizeof(gpsb200_acq_result_t), cudaMemcpyDeviceToHost, s));
+    CU_RET(cudaGetLastError());
+    CU_RET(cudaMemcpyAsync(sc.h_res, sc.d_res, cfg->nprn * sizeof(gpsb200_acq_result_t), cudaMemcpyDeviceToHost, s));
     // pageable sources of the two uploads must outlive them: wait here (the search is blocking anyway)
     return cudaStreamSynchronize(s);
 }

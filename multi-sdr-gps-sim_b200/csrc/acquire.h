@@ -23,15 +23,14 @@ constexpr int kExclude = 3;                    // P2 excludes delays within +-3 
 struct Scratch {
     int16_t *d_edges = nullptr;        // [33][kMaxEdges] sign-change positions of every PRN's replica, row 0 unused
     int32_t *d_nedges = nullptr;       // [33]
-    void *d_window = nullptr;          // the searched samples of a host source
-    size_t window_bytes = 0;
     uint64_t *d_grid = nullptr;        // [nprn][nbins][3000] when the caller wants the grid
-    size_t grid_bytes = 0;
+    size_t grid_cap = 0;
     uint64_t *d_rows = nullptr;        // [nprn][nbins][3]: P1, P2, tau1 of every row
+    size_t rows_cap = 0;
     gpsb200_acq_result_t *d_res = nullptr, *h_res = nullptr;   // [32]
     uint32_t *d_u = nullptr;           // [nbins] phase steps
+    size_t u_cap = 0;
     int32_t *d_prn = nullptr;          // [32]
-    int max_bins = 0;
 };
 
 // Empty when the search is well-formed: PRNs 1..32, 1 <= K <= 100, 1 <= nbins <= GPSB200_ACQ_MAX_BINS, every bin within

@@ -29,6 +29,7 @@
 
 #include "../../include/gpsb200.h"
 #include "acquire.h"
+#include "device_buffer.h"
 #include "track.h"
 #include "pvt.h"
 #include "nco_exact.h"
@@ -202,8 +203,10 @@ struct gpsb200_ctx {
     bool trace_on = false;
     double trace_t0 = 0.0;
     Call call;                             // a slice call begun with gpsb200_slice_prepare (active until finished)
-    void *d_out = nullptr;
+    uint8_t *d_out = nullptr;              // synthesis staging of host destinations
     size_t out_bytes = 0;
+    uint8_t *d_rx = nullptr;               // receiver staging of host sources (acquisition window, tracking buffer)
+    size_t rx_bytes = 0;
     bool nav_dirty = true;
     std::unique_ptr<WorkerPool> pool;      // host passes (guesses, fix-up scan)
     SynthArgs last{};                      // replay state
@@ -564,35 +567,44 @@ int upload_nav(gpsb200_ctx *ctx, cudaStream_t s) {
     return GPSB200_OK;
 }
 
-int check_call(gpsb200_ctx *ctx, const gpsb200_chan_t *chans, int nblk, int nchan, int sample_size, void *dst) {
-    if (!chans || !dst || nblk < 1 || nblk > ctx->cfg.max_blocks || nchan < 1 || nchan > ctx->cfg.max_chan ||
-        (sample_size != GPSB200_SC08 && sample_size != GPSB200_SC16))
-        return fail(ctx, GPSB200_ERR_ARG, "bad arguments (1 <= nchan <= cfg.max_chan; 1 <= nblk <= cfg.max_blocks)");
+// The checks of every entry point that enqueues work, after its own argument checks: the context has a device and no
+// slice call is open. Then selects the context's device.
+int check_entry(gpsb200_ctx *ctx) {
     if (!ctx->s_compute) return fail(ctx, GPSB200_ERR_CUDA, "context has no CUDA device");
     if (ctx->call.active) return fail(ctx, GPSB200_ERR_ARG, "a call begun with gpsb200_slice_prepare has not been finished");
     CU(cudaSetDevice(ctx->cfg.device));     // the caller may be a thread that never selected the context's device
     return GPSB200_OK;
 }
 
-// Both synthesis kernels store whole 2- to 16-byte words at multiples of their width from the destination (k_synth_lanes
-// always 16 bytes, k_synth up to 32 bytes per lane as 16-byte vectors): a caller's device destination must be 16-byte
-// aligned. Checked before anything is enqueued; allocations of CUDA and torch are aligned to 256 bytes.
-int check_dst_aligned(gpsb200_ctx *ctx, const void *dst_device, const char *fn) {
-    if ((reinterpret_cast<uintptr_t>(dst_device) & 15u) != 0)
-        return fail(ctx, GPSB200_ERR_ARG, std::string(fn) + ": dst_device is not 16-byte aligned");
+int check_call(gpsb200_ctx *ctx, const gpsb200_chan_t *chans, int nblk, int nchan, int sample_size, void *dst) {
+    if (!chans || !dst || nblk < 1 || nblk > ctx->cfg.max_blocks || nchan < 1 || nchan > ctx->cfg.max_chan ||
+        (sample_size != GPSB200_SC08 && sample_size != GPSB200_SC16))
+        return fail(ctx, GPSB200_ERR_ARG, "bad arguments (1 <= nchan <= cfg.max_chan; 1 <= nblk <= cfg.max_blocks)");
+    return check_entry(ctx);
+}
+
+// A caller's device buffer must be 16-byte aligned. Both synthesis kernels store whole 2- to 16-byte words at multiples
+// of their width from the destination (k_synth_lanes always 16 bytes, k_synth up to 32 bytes per lane as 16-byte
+// vectors); the receiver calls' device sources are held to the same rule. Checked before anything is enqueued;
+// allocations of CUDA and torch are aligned to 256 bytes.
+int check_aligned(gpsb200_ctx *ctx, const void *p, const char *fn, const char *arg) {
+    if ((reinterpret_cast<uintptr_t>(p) & 15u) != 0)
+        return fail(ctx, GPSB200_ERR_ARG, std::string(fn) + ": " + arg + " is not 16-byte aligned");
     return GPSB200_OK;
 }
 
 // Host destinations are staged in the context's own device buffer, sized for the context's largest call.
 int ensure_staging(gpsb200_ctx *ctx, int sample_size) {
-    const size_t need = (size_t) ctx->cfg.max_blocks * GPSB200_BLOCK_ELEMS * sample_size;
-    if (ctx->out_bytes < need) {
-        cudaFree(ctx->d_out);
-        ctx->d_out = nullptr;
-        ctx->out_bytes = 0;
-        CU(cudaMalloc(&ctx->d_out, need));
-        ctx->out_bytes = need;
-    }
+    CU(grow(ctx->d_out, ctx->out_bytes, (size_t) ctx->cfg.max_blocks * GPSB200_BLOCK_ELEMS * sample_size));
+    return GPSB200_OK;
+}
+
+// A receiver call's host source is copied up on s into the context's receiver staging buffer, *dev points there.
+// Acquisition and tracking both wait for their results, so they never hold the buffer at the same time.
+int stage_rx_source(gpsb200_ctx *ctx, const void *src, size_t bytes, cudaStream_t s, const void **dev) {
+    CU(grow(ctx->d_rx, ctx->rx_bytes, bytes));
+    if (bytes) CU(cudaMemcpyAsync(ctx->d_rx, src, bytes, cudaMemcpyHostToDevice, s));
+    *dev = ctx->d_rx;
     return GPSB200_OK;
 }
 
@@ -943,7 +955,7 @@ int slice_prepare(gpsb200_ctx *ctx, const gpsb200_chan_t *chans, int nblk, int n
                   void *dst_host, cudaStream_t s, gpsb200_slice_link_t *link) {
     int rc = check_call(ctx, chans, nblk, nchan, sample_size, dst_device ? dst_device : dst_host);
     if (rc) return rc;
-    rc = check_dst_aligned(ctx, dst_device, "gpsb200_slice_prepare");
+    rc = check_aligned(ctx, dst_device, "gpsb200_slice_prepare", "dst_device");
     if (rc) return rc;
     if (!dst_device) {                          // host destination only: stage in the context's own device buffer
         rc = ensure_staging(ctx, sample_size);
@@ -1059,9 +1071,8 @@ int synth_host(gpsb200_ctx *ctx, const gpsb200_chan_t *chans, int nblk, int ncha
 // the call has no destination (no carrier tables, no code walk, no checkpoints).
 int carrier_chain_device(gpsb200_ctx *ctx, const gpsb200_chan_t *chans, int nblk, int nchan, const double *phase_in,
                          double *phase_out) {
-    if (!ctx->s_compute) return fail(ctx, GPSB200_ERR_CUDA, "context has no CUDA device");
-    if (ctx->call.active) return fail(ctx, GPSB200_ERR_ARG, "a call begun with gpsb200_slice_prepare has not been finished");
-    CU(cudaSetDevice(ctx->cfg.device));
+    int rc = check_entry(ctx);
+    if (rc) return rc;
     cudaStream_t s = ctx->s_compute;
     Call call(chans, 0, nchan, GPSB200_SC08, nullptr, nullptr, nullptr, s);
     if (phase_in && nblk > 0)
@@ -1072,7 +1083,7 @@ int carrier_chain_device(gpsb200_ctx *ctx, const gpsb200_chan_t *chans, int nblk
         call.chans = chans + (size_t) w0 * nchan;
         call.nblk = nw;
         call.plan({std::make_pair(0, nw)});
-        int rc = seg_params(ctx, call, 0, nw, s, nullptr, nullptr);
+        rc = seg_params(ctx, call, 0, nw, s, nullptr, nullptr);
         if (!rc) rc = seg_probe(ctx, call, 0, nw, s);
         if (!rc) rc = seg_scan(ctx, call, 0, nullptr, s);
         if (rc) return rc;
@@ -1090,26 +1101,15 @@ int acquire(gpsb200_ctx *ctx, const void *iq, int64_t nsamples, int sample_size,
     if (!iq || !res) return fail(ctx, GPSB200_ERR_ARG, "gpsb200_acquire: NULL source or result array");
     const std::string bad = acq::check(cfg, nsamples, sample_size);
     if (!bad.empty()) return fail(ctx, GPSB200_ERR_ARG, "gpsb200_acquire: " + bad);
-    if (device && (reinterpret_cast<uintptr_t>(iq) & 15u) != 0)
-        return fail(ctx, GPSB200_ERR_ARG, "gpsb200_acquire_device: iq_device is not 16-byte aligned");
-    if (!ctx->s_compute) return fail(ctx, GPSB200_ERR_CUDA, "context has no CUDA device");
-    if (ctx->call.active) return fail(ctx, GPSB200_ERR_ARG, "a call begun with gpsb200_slice_prepare has not been finished");
-    CU(cudaSetDevice(ctx->cfg.device));
+    int rc = device ? check_aligned(ctx, iq, "gpsb200_acquire_device", "iq_device") : GPSB200_OK;
+    if (!rc) rc = check_entry(ctx);
+    if (rc) return rc;
     CU(acq::scratch_reserve(ctx->acq, cfg, grid != nullptr));
     const size_t elem = sample_size == GPSB200_SC16 ? 2 : 1;
-    const char *src = static_cast<const char *>(iq) + (size_t) cfg->s0 * 2 * elem;
-    const void *window = src;
+    const void *window = static_cast<const char *>(iq) + (size_t) cfg->s0 * 2 * elem;
     if (!device) {
-        const size_t wb = (size_t) acq::window_samples(cfg) * 2 * elem;
-        if (wb > ctx->acq.window_bytes) {
-            cudaFree(ctx->acq.d_window);
-            ctx->acq.d_window = nullptr;
-            ctx->acq.window_bytes = 0;
-            CU(cudaMalloc(&ctx->acq.d_window, wb));
-            ctx->acq.window_bytes = wb;
-        }
-        CU(cudaMemcpyAsync(ctx->acq.d_window, src, wb, cudaMemcpyHostToDevice, s));
-        window = ctx->acq.d_window;
+        rc = stage_rx_source(ctx, window, (size_t) acq::window_samples(cfg) * 2 * elem, s, &window);
+        if (rc) return rc;
     }
     CU(acq::launch(ctx->acq, window, sample_size, cfg, grid != nullptr, s));
     if (grid)
@@ -1126,17 +1126,14 @@ int track(gpsb200_ctx *ctx, const void *iq, int64_t nsamples, int sample_size, i
     if (!iq || !epochs || !nepochs) return fail(ctx, GPSB200_ERR_ARG, "gpsb200_track: NULL source, epochs or nepochs");
     const std::string bad = trk::check(state, nchan, max_epochs, nsamples, base, sample_size);
     if (!bad.empty()) return fail(ctx, GPSB200_ERR_ARG, "gpsb200_track: " + bad);
-    if (device && (reinterpret_cast<uintptr_t>(iq) & 15u) != 0)
-        return fail(ctx, GPSB200_ERR_ARG, "gpsb200_track_device: iq_device is not 16-byte aligned");
-    if (!ctx->s_compute) return fail(ctx, GPSB200_ERR_CUDA, "context has no CUDA device");
-    if (ctx->call.active) return fail(ctx, GPSB200_ERR_ARG, "a call begun with gpsb200_slice_prepare has not been finished");
-    CU(cudaSetDevice(ctx->cfg.device));
-    const size_t bytes = (size_t) nsamples * 2 * (sample_size == GPSB200_SC16 ? 2 : 1);
-    CU(trk::scratch_reserve(ctx->trk, nchan, max_epochs, device ? 0 : bytes));
+    int rc = device ? check_aligned(ctx, iq, "gpsb200_track_device", "iq_device") : GPSB200_OK;
+    if (!rc) rc = check_entry(ctx);
+    if (rc) return rc;
+    CU(trk::scratch_reserve(ctx->trk, nchan, max_epochs));
     const void *src = iq;
     if (!device) {
-        if (bytes) CU(cudaMemcpyAsync(ctx->trk.d_src, iq, bytes, cudaMemcpyHostToDevice, s));
-        src = ctx->trk.d_src;
+        rc = stage_rx_source(ctx, iq, (size_t) nsamples * 2 * (sample_size == GPSB200_SC16 ? 2 : 1), s, &src);
+        if (rc) return rc;
     }
     CU(trk::launch(ctx->trk, src, nsamples, sample_size, base, state, nchan, max_epochs, epochs, nepochs, s));
     return GPSB200_OK;
@@ -1149,9 +1146,8 @@ int pvt_fix(gpsb200_ctx *ctx, const gpsb200_pvt_chan_t *chans, int nchan, const 
     if (!fixes) return fail(ctx, GPSB200_ERR_ARG, "gpsb200_pvt: NULL fixes");
     const std::string bad = pvt::check(chans, nchan, epochs, nepochs, max_epochs, cfg);
     if (!bad.empty()) return fail(ctx, GPSB200_ERR_ARG, "gpsb200_pvt: " + bad);
-    if (!ctx->s_compute) return fail(ctx, GPSB200_ERR_CUDA, "context has no CUDA device");
-    if (ctx->call.active) return fail(ctx, GPSB200_ERR_ARG, "a call begun with gpsb200_slice_prepare has not been finished");
-    CU(cudaSetDevice(ctx->cfg.device));
+    const int rc = check_entry(ctx);
+    if (rc) return rc;
     CU(pvt::run(ctx->pvt, chans, nchan, epochs, nepochs, max_epochs, cfg, fixes, residuals, ctx->s_compute));
     return GPSB200_OK;
 }
@@ -1461,6 +1457,7 @@ void gpsb200_destroy(gpsb200_ctx_t *ctx) {
     cudaFreeHost(ctx->h_nav);
     cudaFree(ctx->d_chips);
     cudaFree(ctx->d_out);
+    cudaFree(ctx->d_rx);
     for (auto &e : ctx->ev)
         if (e) cudaEventDestroy(e);
     for (auto &e : ctx->ev_done)
@@ -1493,7 +1490,7 @@ int gpsb200_synth_blocks_device(gpsb200_ctx_t *ctx, const gpsb200_chan_t *chans,
     if (!ctx) return GPSB200_ERR_ARG;
     cudaStream_t s = stream_ ? (cudaStream_t) stream_ : ctx->s_compute;
     int rc = check_call(ctx, chans, nblk, nchan, sample_size, dst_device);
-    if (!rc) rc = check_dst_aligned(ctx, dst_device, "gpsb200_synth_blocks_device");
+    if (!rc) rc = check_aligned(ctx, dst_device, "gpsb200_synth_blocks_device", "dst_device");
     if (!rc) {
         Call call(chans, nblk, nchan, sample_size, dst_device, nullptr, nullptr, s);
         rc = run_pipeline(ctx, call, carr_phase_out, stats);
@@ -1656,7 +1653,7 @@ int gpsb200_carrier_chain_device(gpsb200_ctx_t *ctx, const gpsb200_chan_t *chans
 
 int gpsb200_replay_device(gpsb200_ctx_t *ctx, void *dst_device, void *stream_, int kernel_mask) {
     if (!ctx || !ctx->have_last) return GPSB200_ERR_ARG;
-    const int rc = check_dst_aligned(ctx, dst_device, "gpsb200_replay_device");
+    const int rc = check_aligned(ctx, dst_device, "gpsb200_replay_device", "dst_device");
     if (rc) return rc;
     CU(cudaSetDevice(ctx->cfg.device));
     cudaStream_t s = stream_ ? (cudaStream_t) stream_ : ctx->s_compute;

@@ -1,5 +1,6 @@
 // Device helpers of the receiver-side kernels (acquire.cu, track.cu): the sample reduction and the carrier tables they
-// share (include/gpsb200.h: acquisition and tracking contracts).
+// share (include/gpsb200.h: acquisition and tracking contracts). The sine table also builds the synthesis's carrier
+// tables (k_tables, synth_kernels.cu).
 #pragma once
 #include <stdint.h>
 

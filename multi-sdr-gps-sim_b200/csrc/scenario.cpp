@@ -39,11 +39,11 @@
 
 namespace {
 
+using namespace gpsb200;   // the reference's physical constants and the NAV parity (synth_tables.h)
+
 // ---- constants of the reference (gps.h:60-118) --------------------------------------
 constexpr double kSecWeek = 604800.0, kSecHalfWeek = 302400.0, kSecDay = 86400.0, kSecHour = 3600.0;
-constexpr double kGM = 3.986005e14, kOmegaE = 7.2921151467e-5, kPi = 3.1415926535898;
-constexpr double kWgsA = 6378137.0, kWgsE = 0.0818191908426, kR2D = 57.2957795131;
-constexpr double kC = 2.99792458e8, kLambda = 0.190293672798365;
+constexpr double kR2D = 57.2957795131;
 constexpr double kCodeFreq = 1.023e6, kCarrToCode = 1.0 / 1540.0;
 constexpr int kMaxSat = 32, kEphSets = 13, kSbfPages = 3 + 2 * 25, kWordsPerSbf = 10;
 // 2^-n scale factors exactly as spelled in gps.h:66-83 (the literals, not ldexp: a few of
@@ -307,26 +307,18 @@ Range pseudo_range(const Eph &e, const IonoUtc &io, const GpsTime &g, const doub
 }
 
 // ---- NAV words (gps.c:890-905, 1008-1072) -------------------------------------------------------------
-unsigned parity_of(uint32_t v) { return (unsigned) __builtin_popcount(v) & 1u; }
-
 // 30-bit word with parity from {D29*, D30*, 24 data bits << 6}; nib: solve bits 23/24 so that
 // D29 = D30 = 0 (words 2 and 10 of a subframe)
 uint32_t nav_word(uint32_t source, bool nib) {
-    static const uint32_t mask[6] = {0x3B1F3480u, 0x1D8F9A40u, 0x2EC7CD00u, 0x1763E680u, 0x2BB1F340u, 0x0B7A89C0u};
     uint32_t d = source & 0x3FFFFFC0u;
     const unsigned D29 = (source >> 31) & 1u, D30 = (source >> 30) & 1u;
     if (nib) {
-        if ((D30 + parity_of(mask[4] & d)) % 2) d ^= (1u << 6);
-        if ((D29 + parity_of(mask[5] & d)) % 2) d ^= (1u << 7);
+        if ((D30 + parity_of(kParityMask[4] & d)) % 2) d ^= (1u << 6);
+        if ((D29 + parity_of(kParityMask[5] & d)) % 2) d ^= (1u << 7);
     }
     uint32_t D = d;
     if (D30) D ^= 0x3FFFFFC0u;
-    D |= ((D29 + parity_of(mask[0] & d)) % 2) << 5;
-    D |= ((D30 + parity_of(mask[1] & d)) % 2) << 4;
-    D |= ((D29 + parity_of(mask[2] & d)) % 2) << 3;
-    D |= ((D30 + parity_of(mask[3] & d)) % 2) << 2;
-    D |= ((D30 + parity_of(mask[4] & d)) % 2) << 1;
-    D |= ((D29 + parity_of(mask[5] & d)) % 2);
+    D |= parity6(d >> 6, D29, D30);
     D &= 0x3FFFFFFFu;
     D |= (source & 0xC0000000u);
     return D;

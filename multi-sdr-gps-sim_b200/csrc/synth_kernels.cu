@@ -33,19 +33,13 @@
 #include <type_traits>
 
 #include "nco_exact.h"
+#include "rx_samples.cuh"
 #include "synth_kernels.h"
 #include "synth_tables.h"
 
 namespace gpsb200 {
 
-__constant__ uint8_t c_quarter_sine[128] = {GPSB200_QUARTER_SINE};
-
-__device__ __forceinline__ int sine512(int k) {
-    k &= 511;
-    const int q = k & 255;
-    const int v = c_quarter_sine[q < 128 ? q : 255 - q];
-    return k < 256 ? v : -v;
-}
+using rx::sine512;
 
 static int group_for(int nchan) { return nchan > 16 ? 32 : (nchan > 8 ? 16 : 8); }
 

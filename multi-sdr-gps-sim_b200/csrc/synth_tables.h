@@ -44,4 +44,29 @@ inline int ca_code(int prn, uint8_t *ca /*[1023]*/) {
     return 0;
 }
 
+// Physical constants of the reference, spelled as gps.h:87-102 spells them: the scenario, the NAV decoder and k_pvt
+// all compute with these doubles.
+constexpr double kGM = 3.986005e14;               // GM_EARTH
+constexpr double kOmegaE = 7.2921151467e-5;       // OMEGA_EARTH
+constexpr double kPi = 3.1415926535898;           // PI
+constexpr double kWgsA = 6378137.0;               // WGS84_RADIUS
+constexpr double kWgsE = 0.0818191908426;         // WGS84_ECCENTRICITY
+constexpr double kC = 2.99792458e8;               // SPEED_OF_LIGHT
+constexpr double kLambda = 0.190293672798365;     // LAMBDA_L1
+
+inline unsigned parity_of(uint32_t v) { return (unsigned) __builtin_popcount(v) & 1u; }
+
+// IS-GPS-200 parity equations over data bits d1..d24 (word bits 29..6): bit masks of the data bits each parity bit sums.
+constexpr uint32_t kParityMask[6] = {0x3B1F3480u, 0x1D8F9A40u, 0x2EC7CD00u, 0x1763E680u, 0x2BB1F340u, 0x0B7A89C0u};
+
+// The six parity bits D25..D30 (D25 in bit 5) of data bits d1..d24 (bits 23..0, before the D30* complement), given
+// D29*, D30* of the previous word (computeChecksum, gps.c:1008-1072).
+inline uint32_t parity6(uint32_t data24, unsigned d29, unsigned d30) {
+    const uint32_t d = (data24 & 0xFFFFFFu) << 6;
+    const unsigned star[6] = {d29, d30, d29, d30, d30, d29};
+    uint32_t p = 0;
+    for (int k = 0; k < 6; k++) p = (p << 1) | ((star[k] + parity_of(kParityMask[k] & d)) & 1u);
+    return p;
+}
+
 }  // namespace gpsb200

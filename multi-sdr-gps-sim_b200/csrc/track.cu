@@ -8,6 +8,7 @@
 #include <cstring>
 #include <vector>
 
+#include "device_buffer.h"
 #include "rx_samples.cuh"
 #include "synth_tables.h"
 #include "track.h"
@@ -147,13 +148,7 @@ std::string check(const gpsb200_track_state_t *st, int nchan, int max_epochs, in
     return std::string();
 }
 
-#define TRK_CU(call)                      \
-    do {                                  \
-        cudaError_t e_ = (call);          \
-        if (e_ != cudaSuccess) return e_; \
-    } while (0)
-
-cudaError_t scratch_reserve(Scratch &sc, int nchan, int max_epochs, size_t src_bytes) {
+cudaError_t scratch_reserve(Scratch &sc, int nchan, int max_epochs) {
     if (!sc.d_codes) {
         std::vector<int8_t> c((size_t) 33 * GPSB200_CA_LEN, 0);
         for (int prn = 1; prn <= 32; prn++) {
@@ -161,32 +156,16 @@ cudaError_t scratch_reserve(Scratch &sc, int nchan, int max_epochs, size_t src_b
             ca_code(prn, ca);
             for (int i = 0; i < GPSB200_CA_LEN; i++) c[(size_t) prn * GPSB200_CA_LEN + i] = (int8_t) (2 * ca[i] - 1);
         }
-        TRK_CU(cudaMalloc(&sc.d_codes, c.size()));
-        TRK_CU(cudaMemcpy(sc.d_codes, c.data(), c.size(), cudaMemcpyHostToDevice));
-        TRK_CU(cudaMalloc(&sc.d_state, GPSB200_TRK_MAX_CHAN * sizeof(gpsb200_track_state_t)));
-        TRK_CU(cudaMalloc(&sc.d_n, GPSB200_TRK_MAX_CHAN * sizeof(int32_t)));
+        CU_RET(cudaMalloc(&sc.d_codes, c.size()));
+        CU_RET(cudaMemcpy(sc.d_codes, c.data(), c.size(), cudaMemcpyHostToDevice));
+        CU_RET(cudaMalloc(&sc.d_state, GPSB200_TRK_MAX_CHAN * sizeof(gpsb200_track_state_t)));
+        CU_RET(cudaMalloc(&sc.d_n, GPSB200_TRK_MAX_CHAN * sizeof(int32_t)));
     }
-    const size_t cap = (size_t) nchan * max_epochs;
-    if (cap > sc.epoch_cap) {
-        cudaFree(sc.d_epochs);
-        sc.d_epochs = nullptr;
-        sc.epoch_cap = 0;
-        TRK_CU(cudaMalloc(&sc.d_epochs, cap * sizeof(gpsb200_track_epoch_t)));
-        sc.epoch_cap = cap;
-    }
-    if (src_bytes > sc.src_bytes) {
-        cudaFree(sc.d_src);
-        sc.d_src = nullptr;
-        sc.src_bytes = 0;
-        TRK_CU(cudaMalloc(&sc.d_src, src_bytes));
-        sc.src_bytes = src_bytes;
-    }
-    return cudaSuccess;
+    return grow(sc.d_epochs, sc.epoch_cap, (size_t) nchan * max_epochs);
 }
 
 void scratch_free(Scratch &sc) {
     cudaFree(sc.d_codes);
-    cudaFree(sc.d_src);
     cudaFree(sc.d_state);
     cudaFree(sc.d_epochs);
     cudaFree(sc.d_n);
@@ -196,21 +175,21 @@ void scratch_free(Scratch &sc) {
 cudaError_t launch(Scratch &sc, const void *src, int64_t nsamples, int sample_size, int64_t base,
                    gpsb200_track_state_t *state, int nchan, int max_epochs, gpsb200_track_epoch_t *epochs,
                    int32_t *nepochs, cudaStream_t s) {
-    TRK_CU(cudaMemcpyAsync(sc.d_state, state, nchan * sizeof(gpsb200_track_state_t), cudaMemcpyHostToDevice, s));
+    CU_RET(cudaMemcpyAsync(sc.d_state, state, nchan * sizeof(gpsb200_track_state_t), cudaMemcpyHostToDevice, s));
     if (sample_size == GPSB200_SC08)
         k_track<int8_t><<<nchan, kThreads, 0, s>>>(static_cast<const int8_t *>(src), nsamples, base, sc.d_codes,
                                                    sc.d_state, max_epochs, sc.d_epochs, sc.d_n);
     else
         k_track<int16_t><<<nchan, kThreads, 0, s>>>(static_cast<const int16_t *>(src), nsamples, base, sc.d_codes,
                                                     sc.d_state, max_epochs, sc.d_epochs, sc.d_n);
-    TRK_CU(cudaGetLastError());
-    TRK_CU(cudaMemcpyAsync(nepochs, sc.d_n, nchan * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
-    TRK_CU(cudaMemcpyAsync(state, sc.d_state, nchan * sizeof(gpsb200_track_state_t), cudaMemcpyDeviceToHost, s));
-    TRK_CU(cudaStreamSynchronize(s));
+    CU_RET(cudaGetLastError());
+    CU_RET(cudaMemcpyAsync(nepochs, sc.d_n, nchan * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+    CU_RET(cudaMemcpyAsync(state, sc.d_state, nchan * sizeof(gpsb200_track_state_t), cudaMemcpyDeviceToHost, s));
+    CU_RET(cudaStreamSynchronize(s));
     // the epochs of channel c sit at c * max_epochs; copy only the written ones
     for (int c = 0; c < nchan; c++)
         if (nepochs[c] > 0)
-            TRK_CU(cudaMemcpyAsync(epochs + (size_t) c * max_epochs, sc.d_epochs + (size_t) c * max_epochs,
+            CU_RET(cudaMemcpyAsync(epochs + (size_t) c * max_epochs, sc.d_epochs + (size_t) c * max_epochs,
                                    (size_t) nepochs[c] * sizeof(gpsb200_track_epoch_t), cudaMemcpyDeviceToHost, s));
     return cudaStreamSynchronize(s);
 }

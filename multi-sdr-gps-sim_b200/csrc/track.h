@@ -112,15 +112,13 @@ std::string check(const gpsb200_track_state_t *st, int nchan, int max_epochs, in
 // Device scratch of the tracking calls of one context, grown as needed.
 struct Scratch {
     int8_t *d_codes = nullptr;                   // [33][1023] chips as +-1, row 0 unused
-    void *d_src = nullptr;                       // a host source's samples
-    size_t src_bytes = 0;
     gpsb200_track_state_t *d_state = nullptr;    // [GPSB200_TRK_MAX_CHAN]
     gpsb200_track_epoch_t *d_epochs = nullptr;   // [nchan][max_epochs]
     size_t epoch_cap = 0;
     int32_t *d_n = nullptr;                      // [GPSB200_TRK_MAX_CHAN]
 };
 
-cudaError_t scratch_reserve(Scratch &sc, int nchan, int max_epochs, size_t src_bytes);
+cudaError_t scratch_reserve(Scratch &sc, int nchan, int max_epochs);
 void scratch_free(Scratch &sc);
 // Enqueue the tracking of the samples at `src` (stream sample `base` first) on s and wait for the results.
 cudaError_t launch(Scratch &sc, const void *src, int64_t nsamples, int sample_size, int64_t base,

@@ -3,8 +3,6 @@
 // 3000 K + 2999 samples from the start offset -- and runs gpsb200_acquire on it; prints one line per PRN: best Doppler
 // bin, code delay (samples from the window start to the code's chip 0, and in chips), P1/P2 and whether P1/P2 reaches
 // the threshold. The search and its arithmetic are those of include/gpsb200.h (DESIGN §9).
-#include <sys/stat.h>
-
 #include <cmath>
 #include <cstdio>
 #include <cstdlib>
@@ -13,6 +11,7 @@
 #include <vector>
 
 #include "../include/gpsb200.h"
+#include "rx_cli.h"
 
 // P1/P2 at or above which a PRN counts as acquired. Without noise, absent PRNs of the project's streams stay below 1.6
 // and present ones are far above 3 (tests/test_acquire.py fixes the bounds of both from the model).
@@ -30,30 +29,6 @@ static void usage() {
             "  --threshold R     P1/P2 at or above R counts as acquired (default %.1f)\n",
             kDefaultThreshold);
     exit(2);
-}
-
-static bool parse_prns(const char *s, gpsb200_acq_config_t *cfg) {
-    cfg->nprn = 0;
-    std::string t(s);
-    size_t pos = 0;
-    while (pos <= t.size()) {
-        size_t end = t.find(',', pos);
-        if (end == std::string::npos) end = t.size();
-        const std::string item = t.substr(pos, end - pos);
-        int a = 0, b = 0;
-        if (sscanf(item.c_str(), "%d-%d", &a, &b) == 2) {
-        } else if (sscanf(item.c_str(), "%d", &a) == 1) {
-            b = a;
-        } else {
-            return false;
-        }
-        for (int p = a; p <= b; p++) {
-            if (cfg->nprn >= 32 || p < 1 || p > 32) return false;
-            cfg->prn[cfg->nprn++] = p;
-        }
-        pos = end + 1;
-    }
-    return cfg->nprn > 0;
 }
 
 int main(int argc, char **argv) {
@@ -92,32 +67,26 @@ int main(int argc, char **argv) {
     const size_t elem = ss == GPSB200_SC16 ? 2 : 1;
     const long long s0 = block * GPSB200_BLOCK_SAMPLES + offset_ms * GPSB200_ACQ_CODE_SAMPLES;
     const long long need = (long long) GPSB200_ACQ_CODE_SAMPLES * cfg.ms + GPSB200_ACQ_CODE_SAMPLES - 1;
-    struct stat st;
-    if (stat(path, &st) != 0) {
+    const long long have = file_samples(path, elem);
+    if (have < 0) {
         fprintf(stderr, "gpsb200-acq: cannot open %s\n", path);
         return 1;
     }
-    const long long have = (long long) st.st_size / (long long) (2 * elem);
     if (cfg.ms < 1 || cfg.ms > GPSB200_ACQ_MAX_MS || s0 + need > have) {
         fprintf(stderr, "gpsb200-acq: the window (sample %lld, %lld samples) is not inside %s (%lld samples)\n", s0, need,
                 path, have);
         return 1;
     }
-    std::vector<char> buf((size_t) need * 2 * elem);
+    std::vector<char> buf;
     FILE *f = fopen(path, "rb");
-    if (!f || fseeko(f, (off_t) (s0 * 2 * (long long) elem), SEEK_SET) != 0 || fread(buf.data(), 1, buf.size(), f) != buf.size()) {
+    if (!f || !read_at(f, s0, need, elem, buf)) {
         fprintf(stderr, "gpsb200-acq: cannot read the window of %s\n", path);
         return 1;
     }
     fclose(f);
 
-    gpsb200_config_t cc;
-    memset(&cc, 0, sizeof cc);
-    cc.device = device;
-    cc.max_chan = 1;
-    cc.max_blocks = 1;
     gpsb200_ctx_t *ctx = nullptr;
-    int rc = gpsb200_create(&cc, &ctx);
+    int rc = create_rx_context(device, &ctx);
     std::vector<gpsb200_acq_result_t> res(cfg.nprn);
     if (rc == GPSB200_OK) rc = gpsb200_acquire(ctx, buf.data(), need, ss, &cfg, res.data(), nullptr);
     if (rc != GPSB200_OK) {

@@ -8,8 +8,6 @@
 // (gpsb200_nav_ephemeris) and time anchor (gpsb200_nav_time_anchor); channels without both are left out. The fixes
 // start 0.5 s after the acquisition window (the loops have pulled in by then) and follow every --fix-every ms; one line
 // per fix with status GPSB200_FIX_OK (DESIGN §11).
-#include <sys/stat.h>
-
 #include <algorithm>
 #include <cmath>
 #include <cstdio>
@@ -19,6 +17,7 @@
 #include <vector>
 
 #include "../include/gpsb200.h"
+#include "rx_cli.h"
 
 static const double kDefaultThreshold = 2.5;      // as gpsb200-acq
 static const int kAcqMs = 10;
@@ -40,35 +39,6 @@ static void usage() {
             "                    (default %d) from 0.5 s after the start; --iono: the Klobuchar alpha / beta to apply\n",
             kDefaultThreshold, kDefaultFixEvery);
     exit(2);
-}
-
-static bool parse_prns(const char *s, gpsb200_acq_config_t *cfg) {
-    cfg->nprn = 0;
-    std::string t(s);
-    size_t pos = 0;
-    while (pos <= t.size()) {
-        size_t end = t.find(',', pos);
-        if (end == std::string::npos) end = t.size();
-        const std::string item = t.substr(pos, end - pos);
-        int a = 0, b = 0;
-        if (sscanf(item.c_str(), "%d-%d", &a, &b) == 2) {
-        } else if (sscanf(item.c_str(), "%d", &a) == 1) {
-            b = a;
-        } else {
-            return false;
-        }
-        for (int p = a; p <= b; p++) {
-            if (cfg->nprn >= 32 || p < 1 || p > 32) return false;
-            cfg->prn[cfg->nprn++] = p;
-        }
-        pos = end + 1;
-    }
-    return cfg->nprn > 0;
-}
-
-static bool read_at(FILE *f, long long s0, long long n, size_t elem, std::vector<char> &buf) {
-    buf.resize((size_t) n * 2 * elem);
-    return fseeko(f, (off_t) (s0 * 2 * (long long) elem), SEEK_SET) == 0 && fread(buf.data(), 1, buf.size(), f) == buf.size();
 }
 
 // Fixes from `first` every `step` samples to the last epoch of the channels, one line per fix with status OK.
@@ -151,12 +121,11 @@ int main(int argc, char **argv) {
     const size_t elem = ss == GPSB200_SC16 ? 2 : 1;
     const long long s0 = block * GPSB200_BLOCK_SAMPLES + offset_ms * GPSB200_ACQ_CODE_SAMPLES;
     const long long need = (long long) GPSB200_ACQ_CODE_SAMPLES * cfg.ms + GPSB200_ACQ_CODE_SAMPLES - 1;
-    struct stat st;
-    if (stat(path, &st) != 0) {
+    const long long have = file_samples(path, elem);
+    if (have < 0) {
         fprintf(stderr, "gpsb200-track: cannot open %s\n", path);
         return 1;
     }
-    const long long have = (long long) st.st_size / (long long) (2 * elem);
     if (s0 + need > have) {
         fprintf(stderr, "gpsb200-track: the acquisition window (sample %lld, %lld samples) is not inside %s (%lld samples)\n",
                 s0, need, path, have);
@@ -171,13 +140,8 @@ int main(int argc, char **argv) {
         return 1;
     }
 
-    gpsb200_config_t cc;
-    memset(&cc, 0, sizeof cc);
-    cc.device = device;
-    cc.max_chan = 1;
-    cc.max_blocks = 1;
     gpsb200_ctx_t *ctx = nullptr;
-    int rc = gpsb200_create(&cc, &ctx);
+    int rc = create_rx_context(device, &ctx);
     std::vector<gpsb200_acq_result_t> res(cfg.nprn);
     if (rc == GPSB200_OK) rc = gpsb200_acquire(ctx, buf.data(), need, ss, &cfg, res.data(), nullptr);
     std::vector<gpsb200_track_state_t> state;
