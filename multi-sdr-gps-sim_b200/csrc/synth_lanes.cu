@@ -28,7 +28,11 @@ namespace gpsb200 {
 
 namespace {
 
+// 16 warps per CTA, 2 CTAs per SM at 64 registers. Fewer resident warps with the registers to hold all of the window
+// state (1 CTA of 16, 20 or 24 warps at 93 / 93 / 80 registers, no spills on the common path) measured slower: the
+// kernel is bound by integer issue and needs the warps more than it loses to the spills.
 constexpr int kLaneWarps = 16;
+constexpr int kLaneCtas = 2;
 constexpr int kLaneChipWords = 36;      // 1023 chips periodically extended to 1152 bits (window_signs reads word j0/32 + 2)
 
 struct LaneWin {
@@ -46,7 +50,9 @@ struct LaneSteps {
 // CH = channel capacity of the variant (16 or 32). The channel side uses all 32 lanes: with CH = 16 the two half-warps
 // prepare two consecutive windows per trip, with CH = 32 the warp prepares one.
 // The carrier tables ([channel][k]: I + (Q << 16), gain-scaled, gps.c:2781-2782; 2 KB per channel) sit in front of this
-// struct at a 2 KB-aligned shared address, so that "table base | byte offset of k" is one logic instruction. Entry k of
+// struct at the start of the dynamic shared memory. The look-ups address an entry as slot * 4 + table base (table_at),
+// which needs no alignment of the base, so the layout has no alignment slack and the kernel no rounded-up base to
+// rebuild or keep. Entry k of
 // channel c is stored at (k + swz(c)) mod 512 (swz(c) = c * 32 / CH): the transposing fill from k_tables' [k][channel]
 // layout is then free of bank conflicts, and the look-ups take the rotation from the phase itself: the channel side adds
 // swz(c) << 23 to the window's phase base, so that the top 9 bits of a sample's phase are its stored slot. Channel c's
@@ -63,9 +69,9 @@ struct LanesSmem {
     uint32_t band[CH][lanes::kBandList + 1];            // band_residues() of each channel's step; rows skewed by one bank
 };
 template <int CH>
-constexpr size_t lanes_smem_bytes() { return sizeof(LanesSmem<CH>) + (size_t) CH * 2048 + 2048; }
+constexpr size_t lanes_smem_bytes() { return sizeof(LanesSmem<CH>) + (size_t) CH * 2048; }
 
-// Entry of the carrier table at byte address ta + OFF (low 11 bits zero) for the 32-bit phase p: the stored slot is p >> 23,
+// Entry of the carrier table at byte address ta + OFF for the 32-bit phase p: the stored slot is p >> 23,
 // its address slot * 4 + ta. Written as a shift and a multiply-add so that the address takes one ALU and one FMA-pipe
 // instruction: the shift-and-mask form ((p >> 21) & 0x7FC) | ta puts both on the integer ALU pipe, which the sign tests
 // and sums of the loop already keep close to saturation.
@@ -104,15 +110,52 @@ __device__ __forceinline__ void add_if(int &acc, uint32_t w, uint32_t bit, int e
         : "r"(w), "r"(bit), "r"(e));
 }
 
+// The sums over the channels of one window for this lane's samples n0, n0 + 32, n0 + 64. NC > 0: the call has NC
+// channels, known at compile time (the full-capacity case), so the loop has a fixed trip count and no remainder; NC = 0:
+// nchan channels. all_j: every channel's entry at the unsigned phase; neg_j: those of the channels whose chip x data bit
+// is negative. The sample is all_j - 2 neg_j: table[k ^ 256] = -table[k] entry by entry, and the packed I + (Q << 16)
+// sums are linear modulo 2^32. Two channels per trip (an odd count is padded with the next slot, which is all zeros).
+template <int NC>
+__device__ __forceinline__ void window_sums(const LaneWin *wp, const uint32_t *sp, uint32_t ta, int nchan, uint32_t n0,
+                                            uint32_t sbit, int accs[3]) {
+    const int nc = NC > 0 ? NC : nchan;
+    const uint32_t n1 = n0 + 32u, n2 = n0 + 64u;
+    int all0 = 0, all1 = 0, all2 = 0, neg0 = 0, neg1 = 0, neg2 = 0;
+#pragma unroll 4
+    for (int c = 0; c < nc; c += 2, wp += 2, sp += 2, ta += 2 * 2048u) {     // table of channel c; c + 1 at + 2048
+        const uint4 wa = *reinterpret_cast<const uint4 *>(&wp[0]);           // broadcast
+        const uint4 wb = *reinterpret_cast<const uint4 *>(&wp[1]);
+        const uint2 st = *reinterpret_cast<const uint2 *>(sp);
+        const uint32_t a0 = wa.w + n0 * st.x, a1 = wa.w + n1 * st.x, a2 = wa.w + n2 * st.x;
+        const uint32_t b0 = wb.w + n0 * st.y, b1 = wb.w + n1 * st.y, b2 = wb.w + n2 * st.y;
+        const int ea0 = table_at<0>(a0, ta), eb0 = table_at<2048>(b0, ta);
+        const int ea1 = table_at<0>(a1, ta), eb1 = table_at<2048>(b1, ta);
+        const int ea2 = table_at<0>(a2, ta), eb2 = table_at<2048>(b2, ta);
+        all0 += ea0 + eb0;
+        all1 += ea1 + eb1;
+        all2 += ea2 + eb2;
+        add_if(neg0, wa.x, sbit, ea0);
+        add_if(neg0, wb.x, sbit, eb0);
+        add_if(neg1, wa.y, sbit, ea1);
+        add_if(neg1, wb.y, sbit, eb1);
+        add_if(neg2, wa.z, sbit, ea2);
+        add_if(neg2, wb.z, sbit, eb2);
+    }
+    accs[0] = (int) ((uint32_t) all0 - 2u * (uint32_t) neg0);
+    accs[1] = (int) ((uint32_t) all1 - 2u * (uint32_t) neg1);
+    accs[2] = (int) ((uint32_t) all2 - 2u * (uint32_t) neg2);
+}
+
 template <bool IQ16, int CH>
-__global__ void __launch_bounds__(kLaneWarps * 32, 2) k_synth_lanes(SynthArgs a) {
+__global__ void __launch_bounds__(kLaneWarps * 32, kLaneCtas) k_synth_lanes(SynthArgs a) {
     constexpr int WINS = 32 / CH;                     // windows per trip
     constexpr int SWZ = 32 / CH;                      // swz(c) = c * SWZ
+    constexpr int BYTES = IQ16 ? 4 : 2;               // output bytes per sample
     extern __shared__ __align__(16) unsigned char smem_raw[];
-    const uint32_t raw_base = (uint32_t) __cvta_generic_to_shared(smem_raw);
-    const uint32_t tab_base = (raw_base + 2047u) & ~2047u;
-    int32_t *tab = reinterpret_cast<int32_t *>(smem_raw + (tab_base - raw_base));                 // [channel][512]
-    LanesSmem<CH> &sm = *reinterpret_cast<LanesSmem<CH> *>(smem_raw + (tab_base - raw_base) + CH * 2048);
+    int32_t *tab = reinterpret_cast<int32_t *>(smem_raw);                                            // [channel][512]
+    LanesSmem<CH> &sm = *reinterpret_cast<LanesSmem<CH> *>(smem_raw + CH * 2048);
+    // 32-bit shared address of the tables, for the look-ups' address arithmetic (table_at)
+    const uint32_t tab_base = (uint32_t) __cvta_generic_to_shared(smem_raw);
     constexpr uint32_t kFull = 0xFFFFFFFFu;
 
     const int b = blockIdx.x / a.ctas_per_block;
@@ -197,7 +240,9 @@ __global__ void __launch_bounds__(kLaneWarps * 32, 2) k_synth_lanes(SynthArgs a)
             load_steps();
             lanes::advance_window(s, navf);
         }
-        const size_t samp0 = (size_t) b * kBlockSamples + (size_t) r * a.run_samples;
+        // output of the trip's first window: derived once per run, advanced per trip
+        uint4 *dst = reinterpret_cast<uint4 *>(reinterpret_cast<char *>(a.out) +
+                                               ((size_t) b * kBlockSamples + (size_t) r * a.run_samples) * BYTES);
 
 #pragma unroll 1
         for (int w = 0; w < nwin; w += WINS) {
@@ -231,36 +276,13 @@ __global__ void __launch_bounds__(kLaneWarps * 32, 2) k_synth_lanes(SynthArgs a)
             for (int hh = 0; hh < WINS; hh++) {
                 if (w + hh >= nwin) break;
                 const LaneWin *wrow = &sm.win[warp][hh][0];
-                // all_j: every channel's entry at the unsigned phase; neg_j: those of the channels whose chip x data bit
-                // is negative. The sample is all_j - 2 neg_j: table[k ^ 256] = -table[k] entry by entry, and the packed
-                // I + (Q << 16) sums are linear modulo 2^32.
-                int all0 = 0, all1 = 0, all2 = 0, neg0 = 0, neg1 = 0, neg2 = 0;
-                // Two channels per trip (an odd count is padded with the next slot, which is all zeros).
-                const LaneWin *wp = wrow;
-                const uint32_t *sp = &sm.step[0];
-                uint32_t ta = tab_base;                                        // table of channel c; c + 1 at + 2048
-#pragma unroll 4
-                for (int c = 0; c < nchan; c += 2, wp += 2, sp += 2, ta += 2 * 2048u) {
-                    const uint4 wa = *reinterpret_cast<const uint4 *>(&wp[0]);       // broadcast
-                    const uint4 wb = *reinterpret_cast<const uint4 *>(&wp[1]);
-                    const uint2 st = *reinterpret_cast<const uint2 *>(sp);
-                    const uint32_t a0 = wa.w + n0 * st.x, a1 = wa.w + n1 * st.x, a2 = wa.w + n2 * st.x;
-                    const uint32_t b0 = wb.w + n0 * st.y, b1 = wb.w + n1 * st.y, b2 = wb.w + n2 * st.y;
-                    const int ea0 = table_at<0>(a0, ta), eb0 = table_at<2048>(b0, ta);
-                    const int ea1 = table_at<0>(a1, ta), eb1 = table_at<2048>(b1, ta);
-                    const int ea2 = table_at<0>(a2, ta), eb2 = table_at<2048>(b2, ta);
-                    all0 += ea0 + eb0;
-                    all1 += ea1 + eb1;
-                    all2 += ea2 + eb2;
-                    add_if(neg0, wa.x, sbit, ea0);
-                    add_if(neg0, wb.x, sbit, eb0);
-                    add_if(neg1, wa.y, sbit, ea1);
-                    add_if(neg1, wb.y, sbit, eb1);
-                    add_if(neg2, wa.z, sbit, ea2);
-                    add_if(neg2, wb.z, sbit, eb2);
-                }
-                int accs[3] = {(int) ((uint32_t) all0 - 2u * (uint32_t) neg0), (int) ((uint32_t) all1 - 2u * (uint32_t) neg1),
-                               (int) ((uint32_t) all2 - 2u * (uint32_t) neg2)};
+                int accs[3];
+                // The fixed-count loop for the full 32-channel call only: in the 16-channel variant the sample side
+                // runs once per window of the trip, and a second copy of the loop for each was slower at 12 channels.
+                if (CH == 32 && nchan == CH)                                      // warp-uniform
+                    window_sums<CH>(wrow, &sm.step[0], tab_base, nchan, n0, sbit, accs);
+                else
+                    window_sums<0>(wrow, &sm.step[0], tab_base, nchan, n0, sbit, accs);
                 // ---- repair: the channel side flagged the channels with a sample of this window within 2^-25 cycles below
                 // an index boundary (warp-uniform). Take the certain index of exactly those (channel, sample) pairs (64-bit
                 // linear phase; exact walk from the run anchor inside the 2^-41 band) and patch the sums.
@@ -283,29 +305,31 @@ __global__ void __launch_bounds__(kLaneWarps * 32, 2) k_synth_lanes(SynthArgs a)
                     }
                 }
                 // ---- quantise + pack (gps.c:2833-2845) ---------------------------------------------------------------
+                // i = (short) i_acc is the low half of the packed sum p, q = (short) q_acc its high half after the
+                // borrow that sign-extending i took (gps.c:2834-2835): q << 16 = p - i = the high half of
+                // x = p + ((p & 0x8000) << 1). So x is the int16 pair (i, q) as stored, and the int8 pair
+                // (i >> 4, q >> 4) (gps.c:2844) is bits 4..11 of p and bits 20..27 of x.
 #pragma unroll
                 for (int j = 0; j < 3; j++) {
-                    const int p = accs[j];
-                    const int iv = (int) (short) (p & 0xFFFF);                 // (short) i_acc, gps.c:2834
-                    const int qv = (p - iv) >> 16;                             // (short) q_acc, gps.c:2835
+                    const uint32_t p = (uint32_t) accs[j];
+                    const uint32_t x = p + ((p & 0x8000u) << 1);
                     const int n = hh * lanes::kWindow + 32 * j + lane;
-                    if (IQ16) {
-                        stage[n] = ((uint32_t) iv & 0xFFFFu) | ((uint32_t) qv << 16);
-                    } else {
-                        reinterpret_cast<uint16_t *>(stage)[n] =
-                            (uint16_t) ((((uint32_t) (iv >> 4)) & 0xFFu) | ((((uint32_t) (qv >> 4)) & 0xFFu) << 8));  // gps.c:2844
-                    }
+                    if (IQ16)
+                        stage[n] = x;
+                    else
+                        reinterpret_cast<uint16_t *>(stage)[n] = (uint16_t) (((p >> 4) & 0xFFu) | ((x >> 12) & 0xFF00u));
                 }
             }
             __syncwarp();
             // ---- 16-byte stores of the window(s) of this trip ------------------------------------------------------------
             {
-                const int nsamp = (nwin - w >= WINS ? WINS : 1) * lanes::kWindow;
-                const int nvec = nsamp * (IQ16 ? 4 : 2) / 16;
-                uint4 *dst = reinterpret_cast<uint4 *>(reinterpret_cast<char *>(a.out) +
-                                                       (samp0 + (size_t) w * lanes::kWindow) * (IQ16 ? 4 : 2));
+                constexpr int kVec = WINS * lanes::kWindow * BYTES / 16;       // 16-byte vectors of a full trip
+                const int nvec = WINS == 1 || nwin - w >= WINS ? kVec : kVec / WINS;
                 const uint4 *srcv = reinterpret_cast<const uint4 *>(stage);
-                for (int i = lane; i < nvec; i += 32) dst[i] = srcv[i];
+#pragma unroll
+                for (int i = lane; i < ((kVec + 31) & ~31); i += 32)
+                    if (i < nvec) dst[i] = srcv[i];
+                dst += kVec;
             }
         }
     }
@@ -328,7 +352,7 @@ static void lanes_shape(const SynthArgs &a, int *ctas_per_block, int *runs_per_c
     // CTAs all take about the same time and 2 per SM are resident (2 x 132 on an H100 SXM): aim at 40 or more waves so
     // that the last, partly filled one costs little (2999 blocks as ONE CTA each are 11.4 waves -> 12: 5 % lost), in
     // steps of one run per warp of a CTA
-    int per_block = (40 * 2 * device_sms() + a.nblk - 1) / a.nblk;
+    int per_block = (40 * kLaneCtas * device_sms() + a.nblk - 1) / a.nblk;
     if (per_block > 16) per_block = 16;
     if (per_block < 1) per_block = 1;
     int per_cta = (a.nruns + per_block - 1) / per_block;

@@ -68,9 +68,16 @@ struct ChanRun {
     uint64_t D96, E96;      // kWindow * D, kWindow * E: the advance of one window (the only increments the window loop needs)
     uint32_t inv32;         // floor(2^79 / delta3), delta3 = 3 E - 2^54 in [2^48, 2^49): the carry-point division as a multiply
     uint32_t e22;           // E >> 22: code increment in units of 2^-32 chips (truncated)
-    int iword, ibit, icode, dbit;
+    uint32_t nav;           // NAV position and data bit: iword | ibit << 8 | icode << 16 | dbit << 24 (Anchor::navpos + bit)
     bool active;
 };
+
+// Fields of ChanRun::nav. One word rather than four, so that the window state the kernel carries across its sample side
+// stays small enough for registers.
+GPSB_HD int nav_iword(uint32_t nav) { return (int) (nav & 0xFF); }
+GPSB_HD int nav_ibit(uint32_t nav) { return (int) ((nav >> 8) & 0xFF); }
+GPSB_HD int nav_icode(uint32_t nav) { return (int) ((nav >> 16) & 0xFF); }
+GPSB_HD uint32_t nav_dbit(uint32_t nav) { return nav >> 24; }
 
 // The exact NCO state at the run start (RunCkpt) and the increments: what the repair paths walk from.
 struct Anchor {
@@ -98,13 +105,11 @@ GPSB_HD void init_steps(ChanRun &s, bool active, double c, double d) {
 template <class NavFn>
 GPSB_HD void init_run(ChanRun &s, bool active, double x, double y, uint32_t navpos, double c, double d, NavFn nav) {
     s.active = active;
-    s.iword = (int) (navpos & 0xFF);
-    s.ibit = (int) ((navpos >> 8) & 0xFF);
-    s.icode = (int) ((navpos >> 16) & 0xFF);
+    s.nav = navpos & 0xFFFFFFu;
     s.P = carr_fix(x);
     s.Y = code_fix(y);
     init_steps(s, active, c, d);
-    s.dbit = active ? nav_bit_at(nav, s.iword, s.ibit) : 0;
+    if (active) s.nav |= (uint32_t) nav_bit_at(nav, nav_iword(s.nav), nav_ibit(s.nav)) << 24;
 }
 
 GPSB_HD uint32_t mulhi32(uint32_t a, uint32_t b) {
@@ -175,18 +180,19 @@ GPSB_HD bool window_signs(const ChanRun &s, ChipFn chips, NavFn nav, uint32_t W[
     const int wi = j0 >> 5, sh = j0 & 31;
     const uint32_t w0 = chips(wi), w1 = chips(wi + 1), w2 = chips(wi + 2);
     uint32_t c_lo = funnel_r(w0, w1, sh), c_hi = funnel_r(w1, w2, sh);
-    if (s.dbit) {
+    const int dbit = (int) nav_dbit(s.nav);
+    if (dbit) {
         c_lo = ~c_lo;
         c_hi = ~c_hi;
     }
     const int pw = 1023 - j0;
-    if (pw < 64 && s.icode == 19) {
-        int ib = s.ibit + 1, iw = s.iword;
+    if (pw < 64 && nav_icode(s.nav) == 19) {
+        int ib = nav_ibit(s.nav) + 1, iw = nav_iword(s.nav);
         if (ib >= 30) {
             ib = 0;
             ++iw;
         }
-        if (nav_bit_at(nav, iw, ib) != s.dbit) {
+        if (nav_bit_at(nav, iw, ib) != dbit) {
             if (pw < 32) {
                 c_lo ^= 0xFFFFFFFFu << pw;
                 c_hi = ~c_hi;
@@ -224,14 +230,17 @@ GPSB_HD void advance_window(ChanRun &s, NavFn nav) {
     s.Y += s.E96;                                                             // 1023 + 33 chips passes 2^64: modular
     if (s.Y < y_old || s.Y >= kCodeWrap54) {
         s.Y -= kCodeWrap54;
-        if (++s.icode >= 20) {
-            s.icode = 0;
-            if (++s.ibit >= 30) {
-                s.ibit = 0;
-                ++s.iword;
+        int icode = nav_icode(s.nav) + 1, ibit = nav_ibit(s.nav), iword = nav_iword(s.nav);
+        uint32_t dbit = nav_dbit(s.nav);
+        if (icode >= 20) {
+            icode = 0;
+            if (++ibit >= 30) {
+                ibit = 0;
+                ++iword;
             }
-            s.dbit = nav_bit_at(nav, s.iword, s.ibit);
+            dbit = (uint32_t) nav_bit_at(nav, iword, ibit);
         }
+        s.nav = (uint32_t) iword | ((uint32_t) ibit << 8) | ((uint32_t) icode << 16) | (dbit << 24);
     }
 }
 
