@@ -591,9 +591,63 @@ typedef struct gpsb200_fix {
 int gpsb200_pvt(gpsb200_ctx_t *ctx, const gpsb200_pvt_chan_t *chans, int nchan, const gpsb200_track_epoch_t *epochs,
                 const int32_t *nepochs, int max_epochs, const gpsb200_pvt_config_t *cfg, gpsb200_fix_t *fixes,
                 double *residuals);
-/* Re-run the fix kernel of the previous gpsb200_pvt call on its device-resident inputs, enqueued on `stream` (0 = the
- * context's own stream), without transfers: for timing the kernel alone. GPSB200_ERR_ARG when there was no such call. */
+/* Re-run the fix kernel of the previous gpsb200_pvt or gpsb200_pvt_raim call (whichever ran last) on its device-resident
+ * inputs, enqueued on `stream` (0 = the context's own stream), without transfers: for timing the kernel alone.
+ * GPSB200_ERR_ARG when there was no such call. */
 int gpsb200_pvt_replay(gpsb200_ctx_t *ctx, void *stream);
+
+/* ---- integrity of the fixes: RAIM fault detection, exclusion and protection levels (DESIGN §11.1; tests/raim_model.py)
+ * Per fix instant, with sigma, T_d and lambda_d below (d = degrees of freedom):
+ *   1. Solve exactly as gpsb200_pvt does (the set S = the channels it uses).
+ *   2. If the fix is OK and n = |S| >= 5: stat = sum over S of e_j^2 / sigma^2, e_j the post-fit residual of
+ *      gpsb200_pvt; dof = n - 4. A fault is detected when stat > T_dof.
+ *   3. If detected, n >= 6 and fewer than max_exclude channels have been excluded: exclude the channel j of S with the
+ *      largest e_j^2 / (1 - h_jj), the lowest channel on ties; h_jj = g_j . N^-1 g_j, g_j = (row of j, 1), N the normal
+ *      matrix of the last Gauss-Newton iteration. Channels with 1 - h_jj <= 1e-9 are never candidates.
+ *   4. Gauss-Newton again on S without j, from the fix of step 1 (or of the previous step 4), with the same rules.
+ *   5. Back to step 2's test on the new set.
+ * Verdicts: PASS the test passed and nothing was excluded; EXCLUDED the final set passes after exclusions; ALERT a fault
+ * is detected and not removed (dof 1, where every normalized residual is equal; max_exclude reached; no candidate; or a
+ * re-solve that did not converge); UNAVAILABLE fewer than 5 used channels or the first solve not OK.
+ * The fix record describes the final set (mask, nused, status, position, velocity, rms); iterations counts every pass.
+ * stat, dof and threshold are those of the last test run (NaN, 0, NaN when none ran). Protection levels (Brown's slope
+ * method) over the final set when its fix is OK and the verdict is not UNAVAILABLE, NaN otherwise:
+ *   x_j = N^-1 g_j rotated to east / north / up at the final fix's WGS-84 latitude and longitude,
+ *   Hslope_j = sqrt(x_jE^2 + x_jN^2) / sqrt(1 - h_jj), Vslope_j = |x_jU| / sqrt(1 - h_jj),
+ *   HPL = max_j Hslope_j sigma sqrt(lambda_dof), VPL = max_j Vslope_j sigma sqrt(lambda_dof); +inf when some channel of
+ *   the set has 1 - h_jj <= 1e-9.
+ * residuals (NULL: not wanted) [nfix][nchan]: the set's channels as gpsb200_pvt reports them; excluded channels their
+ * residual against the final fix (rho - model - row . dX of the final set's last iteration: the fault's size); every
+ * other channel NaN (all NaN when the final fix is not OK). */
+enum { GPSB200_RAIM_PASS = 0, GPSB200_RAIM_EXCLUDED = 1, GPSB200_RAIM_ALERT = 2, GPSB200_RAIM_UNAVAILABLE = 3 };
+#define GPSB200_RAIM_MAX_DOF 28          /* dof 1..28: 5..32 channels */
+#define GPSB200_RAIM_MAX_EXCLUDE 4
+typedef struct gpsb200_raim_config {
+    double sigma;          /* pseudorange sigma, m: finite, > 0 */
+    double p_fa;           /* false-alarm probability of the test, 1e-12..0.5 */
+    double p_md;           /* missed-detection probability of the protection levels, 1e-12..0.5 */
+    int32_t max_exclude;   /* 0..GPSB200_RAIM_MAX_EXCLUDE; 0 = detection only */
+    int32_t reserved;      /* 0 */
+} gpsb200_raim_config_t;   /* 32 bytes */
+typedef struct gpsb200_raim {
+    int32_t verdict;       /* GPSB200_RAIM_* */
+    uint32_t excluded;     /* bit c: channel c excluded */
+    int32_t dof;           /* of the last test; 0 when none ran */
+    int32_t reserved;
+    double stat;           /* sum e^2 / sigma^2 of the last test */
+    double threshold;      /* T_dof of the last test */
+    double hpl, vpl;       /* m */
+} gpsb200_raim_t;          /* 48 bytes */
+/* Host: for d = 1..28, T[d-1] = the chi^2(d) value whose upper tail is p_fa, lambda[d-1] = the noncentrality at which
+ * the noncentral chi^2(d, lambda) has P(<= T_d) = p_md (regularized incomplete gamma, a Poisson mixture for the
+ * noncentral CDF, bisection; 1e-10 relative or better). GPSB200_ERR_ARG when p_fa or p_md is outside 1e-12..0.5 or an
+ * array is NULL. */
+int gpsb200_raim_thresholds(double p_fa, double p_md, double T[GPSB200_RAIM_MAX_DOF], double lambda[GPSB200_RAIM_MAX_DOF]);
+/* gpsb200_pvt with the RAIM stage above: the same arguments and checks, plus the RAIM config (GPSB200_ERR_ARG outside its
+ * ranges) and out [nfix], one record per fix. The tables of gpsb200_raim_thresholds go up with the kernel's arguments. */
+int gpsb200_pvt_raim(gpsb200_ctx_t *ctx, const gpsb200_pvt_chan_t *chans, int nchan, const gpsb200_track_epoch_t *epochs,
+                     const int32_t *nepochs, int max_epochs, const gpsb200_pvt_config_t *cfg,
+                     const gpsb200_raim_config_t *raim, gpsb200_fix_t *fixes, double *residuals, gpsb200_raim_t *out);
 
 /* ---- scenario engine: the reference's host path outside the sample loop -------------
  * RINEX-2/3 navigation file (plain or gzip-compressed, read through zlib like the reference, gps.c:1147) +

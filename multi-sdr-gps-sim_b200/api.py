@@ -196,6 +196,34 @@ assert (EPHEMERIS_DTYPE.itemsize, IONO_DTYPE.itemsize, PVT_CHAN_DTYPE.itemsize, 
 FIX_OK, FIX_FEW, FIX_NO_CONVERGENCE = 0, 1, 2
 PVT_MAX_ITER = 12
 
+# gpsb200_raim_config_t / gpsb200_raim_t (DESIGN §11.1)
+RAIM_CONFIG_DTYPE = np.dtype([("sigma", "<f8"), ("p_fa", "<f8"), ("p_md", "<f8"), ("max_exclude", "<i4"),
+                              ("reserved", "<i4")])
+RAIM_DTYPE = np.dtype([("verdict", "<i4"), ("excluded", "<u4"), ("dof", "<i4"), ("reserved", "<i4"), ("stat", "<f8"),
+                       ("threshold", "<f8"), ("hpl", "<f8"), ("vpl", "<f8")])
+assert (RAIM_CONFIG_DTYPE.itemsize, RAIM_DTYPE.itemsize) == (32, 48)
+RAIM_PASS, RAIM_EXCLUDED, RAIM_ALERT, RAIM_UNAVAILABLE = 0, 1, 2, 3
+RAIM_MAX_DOF = 28
+RAIM_MAX_EXCLUDE = 4
+
+
+def raim_config(sigma, p_fa=1e-5, p_md=1e-3, max_exclude=1):
+    """A RAIM_CONFIG_DTYPE record: pseudorange sigma (m), false-alarm and missed-detection probabilities, and how many
+    channels a fix may exclude (0: detection only)."""
+    c = np.zeros(1, RAIM_CONFIG_DTYPE)[0]
+    c["sigma"], c["p_fa"], c["p_md"], c["max_exclude"] = float(sigma), float(p_fa), float(p_md), int(max_exclude)
+    return c
+
+
+def raim_thresholds(p_fa, p_md):
+    """gpsb200_raim_thresholds: (T[28], lambda[28]) for dof 1..28; T[d - 1] is the chi^2(d) value with upper tail p_fa,
+    lambda[d - 1] the noncentrality whose noncentral chi^2(d) CDF at T[d - 1] is p_md."""
+    T, lam = np.zeros(RAIM_MAX_DOF), np.zeros(RAIM_MAX_DOF)
+    rc = lib().gpsb200_raim_thresholds(float(p_fa), float(p_md), T.ctypes.data, lam.ctypes.data)
+    if rc:
+        raise GpsB200Error(rc, "gpsb200_raim_thresholds")
+    return T, lam
+
 
 def nav_words_of_frame(words60):
     """The 60 NAV words of a frame slot as the scenario sends them (bits 29..0 used) -> NAV_WORD_DTYPE[60] records with
@@ -256,7 +284,8 @@ EXPORTS = ["gpsb200_create", "gpsb200_destroy", "gpsb200_last_error", "gpsb200_v
            "gpsb200_carrier_advance", "gpsb200_carrier_chain", "gpsb200_carrier_chain_device", "gpsb200_carrier_probe_fixup",
            "gpsb200_codegen", "gpsb200_acquire", "gpsb200_acquire_device", "gpsb200_track_start", "gpsb200_track",
            "gpsb200_track_device", "gpsb200_nav_decode", "gpsb200_nav_word_check", "gpsb200_nav_parity",
-           "gpsb200_nav_ephemeris", "gpsb200_nav_time_anchor", "gpsb200_pvt", "gpsb200_pvt_replay", "gpsb200_bind_numa", "gpsb200_span_chain_host", "gpsb200_lanes_model_block",
+           "gpsb200_nav_ephemeris", "gpsb200_nav_time_anchor", "gpsb200_pvt", "gpsb200_pvt_replay",
+           "gpsb200_pvt_raim", "gpsb200_raim_thresholds", "gpsb200_bind_numa", "gpsb200_span_chain_host", "gpsb200_lanes_model_block",
            "gpsb200_lanes_window_band_host", "gpsb200_slice_prepare", "gpsb200_slice_probe",
            "gpsb200_slice_finish", "gpsb200_slice_finish_cb", "gpsb200_slice_wait", "gpsb200_link_apply", "gpsb200_slice_link_host", "gpsb200_debug_corrupt_chain", "gpsb200_synth_kernel_name",
            "gpsb200_debug_run_checkpoints", "gpsb200_checkpoint_segments_host",
@@ -361,6 +390,9 @@ def lib():
         L.gpsb200_pvt.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p,
                                   C.c_void_p]
         L.gpsb200_pvt_replay.argtypes = [C.c_void_p, C.c_void_p]
+        L.gpsb200_pvt_raim.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p,
+                                       C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+        L.gpsb200_raim_thresholds.argtypes = [C.c_double, C.c_double, C.c_void_p, C.c_void_p]
         _lib = L
     return _lib
 
@@ -899,6 +931,28 @@ class Context:
         call takes it; cfg: PVT_CONFIG_DTYPE record (pvt_config).
         -> fixes FIX_DTYPE[nfix], and with want_residuals also the post-fit residuals float64[nfix, nchan] (NaN where a
         channel is not used)."""
+        ch, nchan, ep, n, me, cf, fixes, res = self._pvt_args(chans, epochs, cfg, want_residuals, nepochs)
+        self._check(lib().gpsb200_pvt(self._h, ch.ctypes.data, nchan, ep.ctypes.data, n.ctypes.data, me, cf.ctypes.data,
+                                      fixes.ctypes.data, None if res is None else res.ctypes.data))
+        return (fixes, res) if want_residuals else fixes
+
+    def pvt_raim(self, chans, epochs, cfg, raim, want_residuals=False, nepochs=None):
+        """Fixes with RAIM fault detection, exclusion and protection levels (gpsb200_pvt_raim; DESIGN §11.1). The
+        arguments of pvt, plus raim: RAIM_CONFIG_DTYPE record (raim_config).
+        -> (fixes FIX_DTYPE[nfix] of each fix's final channel set, RAIM_DTYPE[nfix]), and with want_residuals also the
+        residuals float64[nfix, nchan]: the final set's post-fit residuals, an excluded channel's residual against the
+        final fix, NaN elsewhere."""
+        ch, nchan, ep, n, me, cf, fixes, res = self._pvt_args(chans, epochs, cfg, want_residuals, nepochs)
+        rc = np.array(raim, dtype=RAIM_CONFIG_DTYPE).reshape(1)
+        out = np.zeros(fixes.size, RAIM_DTYPE)
+        self._check(lib().gpsb200_pvt_raim(self._h, ch.ctypes.data, nchan, ep.ctypes.data, n.ctypes.data, me,
+                                           cf.ctypes.data, rc.ctypes.data, fixes.ctypes.data,
+                                           None if res is None else res.ctypes.data, out.ctypes.data))
+        return (fixes, out, res) if want_residuals else (fixes, out)
+
+    @staticmethod
+    def _pvt_args(chans, epochs, cfg, want_residuals, nepochs):
+        """The C call's arrays for pvt / pvt_raim: the epochs packed [nchan, max_epochs] unless they already are."""
         ch = np.ascontiguousarray(chans, dtype=PVT_CHAN_DTYPE).reshape(-1)
         nchan = ch.size
         if nepochs is not None:
@@ -917,9 +971,7 @@ class Context:
         nfix = max(1, int(cf[0]["nfix"]))
         fixes = np.zeros(nfix, FIX_DTYPE)
         res = np.zeros((nfix, max(1, nchan))) if want_residuals else None
-        self._check(lib().gpsb200_pvt(self._h, ch.ctypes.data, nchan, ep.ctypes.data, n.ctypes.data, me, cf.ctypes.data,
-                                      fixes.ctypes.data, None if res is None else res.ctypes.data))
-        return (fixes, res) if want_residuals else fixes
+        return ch, nchan, ep, n, me, cf, fixes, res
 
     def pvt_replay(self, stream=0):
         """Enqueue the fix kernel of the previous pvt call again on `stream`, on its device-resident inputs (timing)."""

@@ -1139,16 +1139,17 @@ int track(gpsb200_ctx *ctx, const void *iq, int64_t nsamples, int sample_size, i
     return GPSB200_OK;
 }
 
-// Position fixes (pvt.cu). Everything is checked before anything is enqueued.
-int pvt_fix(gpsb200_ctx *ctx, const gpsb200_pvt_chan_t *chans, int nchan, const gpsb200_track_epoch_t *epochs,
-            const int32_t *nepochs, int max_epochs, const gpsb200_pvt_config_t *cfg, gpsb200_fix_t *fixes,
-            double *residuals) {
-    if (!fixes) return fail(ctx, GPSB200_ERR_ARG, "gpsb200_pvt: NULL fixes");
-    const std::string bad = pvt::check(chans, nchan, epochs, nepochs, max_epochs, cfg);
-    if (!bad.empty()) return fail(ctx, GPSB200_ERR_ARG, "gpsb200_pvt: " + bad);
+// Position fixes (pvt.cu), with the RAIM stage when raim is not NULL. Everything is checked before anything is enqueued.
+int pvt_fix(gpsb200_ctx *ctx, const char *fn, const gpsb200_pvt_chan_t *chans, int nchan,
+            const gpsb200_track_epoch_t *epochs, const int32_t *nepochs, int max_epochs, const gpsb200_pvt_config_t *cfg,
+            const gpsb200_raim_config_t *raim, gpsb200_fix_t *fixes, double *residuals, gpsb200_raim_t *out) {
+    const std::string at = std::string(fn) + ": ";
+    if (!fixes) return fail(ctx, GPSB200_ERR_ARG, at + "NULL fixes");
+    const std::string bad = pvt::check(chans, nchan, epochs, nepochs, max_epochs, cfg, raim);
+    if (!bad.empty()) return fail(ctx, GPSB200_ERR_ARG, at + bad);
     const int rc = check_entry(ctx);
     if (rc) return rc;
-    CU(pvt::run(ctx->pvt, chans, nchan, epochs, nepochs, max_epochs, cfg, fixes, residuals, ctx->s_compute));
+    CU(pvt::run(ctx->pvt, chans, nchan, epochs, nepochs, max_epochs, cfg, raim, fixes, residuals, out, ctx->s_compute));
     return GPSB200_OK;
 }
 
@@ -1728,7 +1729,22 @@ int gpsb200_pvt(gpsb200_ctx_t *ctx, const gpsb200_pvt_chan_t *chans, int nchan, 
                 const int32_t *nepochs, int max_epochs, const gpsb200_pvt_config_t *cfg, gpsb200_fix_t *fixes,
                 double *residuals) {
     if (!ctx) return GPSB200_ERR_ARG;
-    return settle(ctx, nullptr, pvt_fix(ctx, chans, nchan, epochs, nepochs, max_epochs, cfg, fixes, residuals));
+    return settle(ctx, nullptr, pvt_fix(ctx, "gpsb200_pvt", chans, nchan, epochs, nepochs, max_epochs, cfg, nullptr, fixes,
+                                        residuals, nullptr));
+}
+
+int gpsb200_pvt_raim(gpsb200_ctx_t *ctx, const gpsb200_pvt_chan_t *chans, int nchan, const gpsb200_track_epoch_t *epochs,
+                     const int32_t *nepochs, int max_epochs, const gpsb200_pvt_config_t *cfg,
+                     const gpsb200_raim_config_t *raim, gpsb200_fix_t *fixes, double *residuals, gpsb200_raim_t *out) {
+    if (!ctx) return GPSB200_ERR_ARG;
+    if (!raim || !out) return settle(ctx, nullptr, fail(ctx, GPSB200_ERR_ARG, "gpsb200_pvt_raim: NULL raim or out"));
+    return settle(ctx, nullptr, pvt_fix(ctx, "gpsb200_pvt_raim", chans, nchan, epochs, nepochs, max_epochs, cfg, raim,
+                                        fixes, residuals, out));
+}
+
+int gpsb200_raim_thresholds(double p_fa, double p_md, double *T, double *lambda) {
+    if (!T || !lambda) return GPSB200_ERR_ARG;
+    return pvt::raim_thresholds(p_fa, p_md, T, lambda) ? GPSB200_OK : GPSB200_ERR_ARG;
 }
 
 int gpsb200_pvt_replay(gpsb200_ctx_t *ctx, void *stream_) {

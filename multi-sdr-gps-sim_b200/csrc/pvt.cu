@@ -8,6 +8,7 @@
 // atomics, no shared memory; the kernel is bound by FP64 arithmetic (the trigonometry of the orbit and the iterations).
 #include <cmath>
 #include <cstring>
+#include <type_traits>
 #include <vector>
 
 #include "device_buffer.h"
@@ -39,6 +40,15 @@ struct Args {
     double *res;
 };
 
+// The RAIM instantiation's arguments: the tables go up with the launch. Args comes first, so the fields the plain
+// instantiation reads sit at the same parameter offsets in both.
+struct RaimArgs : Args {
+    gpsb200_raim_config_t raim;
+    double T[GPSB200_RAIM_MAX_DOF], lambda[GPSB200_RAIM_MAX_DOF];
+    gpsb200_raim_t *out;
+};
+template <bool kRaim> using KernelArgs = typename std::conditional<kRaim, RaimArgs, Args>::type;
+
 __device__ inline double wrap_half_week(double d) { return d > 302400.0 ? d - 604800.0 : (d < -302400.0 ? d + 604800.0 : d); }
 
 __device__ inline int64_t floor_div(int64_t a, int64_t b) {
@@ -50,6 +60,25 @@ __device__ inline double warp_sum(double v) {
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(kFull, v, o);
     return v;
+}
+
+__device__ inline double warp_max(double v) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) v = fmax(v, __shfl_xor_sync(kFull, v, o));
+    return v;
+}
+
+// The largest v over the warp and its lane j, the lowest lane on ties; every lane ends with the same pair.
+__device__ inline void warp_argmax(double &v, int &j) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+        const double ov = __shfl_xor_sync(kFull, v, o);
+        const int oj = __shfl_xor_sync(kFull, j, o);
+        if (ov > v || (ov == v && oj < j)) {
+            v = ov;
+            j = oj;
+        }
+    }
 }
 
 // Cholesky solve of the symmetric 4 x 4 system N x = b, N packed as n00 n01 n02 n03 n11 n12 n13 n22 n23 n33.
@@ -212,7 +241,13 @@ __device__ int find_period(const gpsb200_track_epoch_t *e, int n, int64_t s) {
     return -1;
 }
 
-__global__ void __launch_bounds__(kWarps * 32) k_pvt(Args a) {
+// kRaim: the RAIM stage of gpsb200_pvt_raim after the solve (DESIGN §11.1). Each lane keeps two flags: `has` (a
+// measurement) and `use` (in the solve). An excluded lane still evaluates its row every iteration, with weight 0, so the
+// same warp sums serve every pass, and its residual against the final fix comes out of the same formula. The RAIM
+// instantiation is held to 128 registers (4 CTAs per SM, as the plain one) at the price of some spills: at its natural
+// 160 it ran 3 CTAs per SM and 15 % slower. The plain one keeps its bounds and instructions (DESIGN §11.1).
+template <bool kRaim>
+__global__ void __launch_bounds__(kWarps * 32, kRaim ? 4 : 0) k_pvt(const KernelArgs<kRaim> a) {
     const int lane = threadIdx.x & 31;
     const int64_t fi = (int64_t) blockIdx.x * kWarps + (threadIdx.x >> 5);
     if (fi >= a.cfg.nfix) return;   // the whole warp leaves together
@@ -247,8 +282,9 @@ __global__ void __launch_bounds__(kWarps * 32) k_pvt(Args a) {
             }
         }
     }
-    const unsigned mask = __ballot_sync(kFull, use);
-    const int nused = __popc(mask);
+    const bool has = use;
+    unsigned mask = __ballot_sync(kFull, use);
+    int nused = __popc(mask);
     gpsb200_fix_t f;
     f.sample = s;
     f.nused = nused;
@@ -258,12 +294,19 @@ __global__ void __launch_bounds__(kWarps * 32) k_pvt(Args a) {
     f.x = f.y = f.z = f.clock_m = f.t_rx = f.vx = f.vy = f.vz = f.drift = nan;
     f.lat_deg = f.lon_deg = f.height = f.pdop = f.rms = nan;
     double resid = nan;
+    // RAIM: the record, and this lane's N^-1 g (position part) and 1 - h_jj of the last pass
+    int verdict = GPSB200_RAIM_UNAVAILABLE, dof = 0;
+    unsigned excluded = 0;
+    double stat = nan, thr = nan, hpl = nan, vpl = nan, xg[3] = {0, 0, 0}, omh = 0.0;
     if (nused >= 4) {
         double X[4] = {0.0, 0.0, 0.0, 0.0};
         double h[3] = {0, 0, 0}, r = 0.0, pr_v[3] = {0, 0, 0};
         Chol ch;
         bool ok = false;
         double dX[4] = {0, 0, 0, 0};
+        int it0 = 0;   // iterations of the earlier passes
+#pragma unroll 1
+        for (;;) {     // Gauss-Newton passes: one, or (RAIM) one more per exclusion, from the previous pass's fix
 #pragma unroll 1
         for (int j = 0; j < GPSB200_PVT_MAX_ITER; j++) {
             const double rad = sqrt(X[0] * X[0] + X[1] * X[1] + X[2] * X[2]);
@@ -276,7 +319,7 @@ __global__ void __launch_bounds__(kWarps * 32) k_pvt(Args a) {
             }
             h[0] = h[1] = h[2] = 0.0;
             r = 0.0;
-            if (use) {
+            if (has) {
                 const double g0 = p[0] - X[0], g1 = p[1] - X[1], g2 = p[2] - X[2];
                 const double tau = sqrt(g0 * g0 + g1 * g1 + g2 * g2) / kC;
                 double sth, cth;
@@ -303,11 +346,13 @@ __global__ void __launch_bounds__(kWarps * 32) k_pvt(Args a) {
                 h[1] = -l1 / R;
                 h[2] = -l2 / R;
             }
-            const double N[10] = {warp_sum(h[0] * h[0]), warp_sum(h[0] * h[1]), warp_sum(h[0] * h[2]), warp_sum(h[0]),
-                                  warp_sum(h[1] * h[1]), warp_sum(h[1] * h[2]), warp_sum(h[1]),
-                                  warp_sum(h[2] * h[2]), warp_sum(h[2]), (double) nused};
-            const double b[4] = {warp_sum(h[0] * r), warp_sum(h[1] * r), warp_sum(h[2] * r), warp_sum(use ? r : 0.0)};
-            f.iterations = j + 1;
+            // an excluded lane's row enters with weight 0
+            const double w0 = kRaim && !use ? 0.0 : h[0], w1 = kRaim && !use ? 0.0 : h[1], w2 = kRaim && !use ? 0.0 : h[2];
+            const double N[10] = {warp_sum(w0 * w0), warp_sum(w0 * w1), warp_sum(w0 * w2), warp_sum(w0),
+                                  warp_sum(w1 * w1), warp_sum(w1 * w2), warp_sum(w1),
+                                  warp_sum(w2 * w2), warp_sum(w2), (double) nused};
+            const double b[4] = {warp_sum(w0 * r), warp_sum(w1 * r), warp_sum(w2 * r), warp_sum(use ? r : 0.0)};
+            f.iterations = it0 + j + 1;
             if (!ch.factor(N)) break;
             ch.solve(b, dX);
 #pragma unroll
@@ -318,9 +363,49 @@ __global__ void __launch_bounds__(kWarps * 32) k_pvt(Args a) {
                 break;
             }
         }
+        if constexpr (!kRaim) {
+            break;
+        } else {
+            // the test of the set just solved; an exclusion goes round again
+            if (!ok) {
+                if (excluded) verdict = GPSB200_RAIM_ALERT;   // a re-solve that failed; else the first: UNAVAILABLE
+                break;
+            }
+            if (nused < 5) break;                          // UNAVAILABLE (only the first set can be this small)
+            const double e = r - (h[0] * dX[0] + h[1] * dX[1] + h[2] * dX[2] + dX[3]);
+            const double g[4] = {h[0], h[1], h[2], 1.0};
+            double x[4];
+            ch.solve(g, x);
+            omh = 1.0 - (g[0] * x[0] + g[1] * x[1] + g[2] * x[2] + g[3] * x[3]);
+            xg[0] = x[0];
+            xg[1] = x[1];
+            xg[2] = x[2];
+            stat = warp_sum(use ? e * e : 0.0) / (a.raim.sigma * a.raim.sigma);
+            dof = nused - 4;
+            thr = a.T[dof - 1];
+            if (!(stat > thr)) {
+                verdict = excluded ? GPSB200_RAIM_EXCLUDED : GPSB200_RAIM_PASS;
+                break;
+            }
+            verdict = GPSB200_RAIM_ALERT;
+            if (nused < 6 || __popc(excluded) >= a.raim.max_exclude) break;
+            double key = use && omh > 1e-9 ? e * e / omh : -1.0;
+            int worst = lane;
+            warp_argmax(key, worst);
+            if (key < 0.0) break;                          // no candidate
+            excluded |= 1u << worst;
+            if (lane == worst) use = false;
+            mask = __ballot_sync(kFull, use);
+            nused = __popc(mask);
+            f.mask = mask;
+            f.nused = nused;
+            it0 = f.iterations;
+            ok = false;
+        }
+        }   // passes (the iteration loop inside keeps its indentation)
         if (ok) {
             // post-fit residuals of the last iteration, velocity and drift on the same rows
-            if (use) resid = r - (h[0] * dX[0] + h[1] * dX[1] + h[2] * dX[2] + dX[3]);
+            if (has) resid = r - (h[0] * dX[0] + h[1] * dX[1] + h[2] * dX[2] + dX[3]);
             const double y = use ? rate + kC * ddtsv + (h[0] * pr_v[0] + h[1] * pr_v[1] + h[2] * pr_v[2]) : 0.0;
             const double bv[4] = {warp_sum(h[0] * y), warp_sum(h[1] * y), warp_sum(h[2] * y), warp_sum(y)};
             double V[4];
@@ -352,14 +437,46 @@ __global__ void __launch_bounds__(kWarps * 32) k_pvt(Args a) {
             f.height = hgt;
             f.pdop = sqrt(Q[0] + Q[1] + Q[2]);
             f.rms = sqrt(ss / (double) nused);
+            if constexpr (kRaim) {
+                if (verdict != GPSB200_RAIM_UNAVAILABLE) {
+                    // Brown's slopes: N^-1 g in east / north / up at the fix
+                    double sla, cla, slo, clo;
+                    sincos(lat, &sla, &cla);
+                    sincos(lon, &slo, &clo);
+                    const double xe = -slo * xg[0] + clo * xg[1];
+                    const double xn = -sla * clo * xg[0] - sla * slo * xg[1] + cla * xg[2];
+                    const double xu = cla * clo * xg[0] + cla * slo * xg[1] + sla * xg[2];
+                    const double inf = __longlong_as_double(0x7ff0000000000000ll);
+                    const bool flat = !(omh > 1e-9);
+                    const double hs = use ? (flat ? inf : sqrt(xe * xe + xn * xn) / sqrt(omh)) : 0.0;
+                    const double vs = use ? (flat ? inf : fabs(xu) / sqrt(omh)) : 0.0;
+                    const double k = a.raim.sigma * sqrt(a.lambda[dof - 1]);
+                    hpl = warp_max(hs) * k;
+                    vpl = warp_max(vs) * k;
+                }
+            }
         }
     }
     if (lane == 0) a.fixes[fi] = f;
-    if (a.res && lane < a.nchan) a.res[fi * a.nchan + lane] = use ? resid : nan;
+    if (a.res && lane < a.nchan) a.res[fi * a.nchan + lane] = has ? resid : nan;
+    if constexpr (kRaim) {
+        if (lane == 0) {
+            gpsb200_raim_t o;
+            o.verdict = verdict;
+            o.excluded = excluded;
+            o.dof = dof;
+            o.reserved = 0;
+            o.stat = stat;
+            o.threshold = thr;
+            o.hpl = hpl;
+            o.vpl = vpl;
+            a.out[fi] = o;
+        }
+    }
 }
 
-cudaError_t launch(Scratch &sc, cudaStream_t s) {
-    Args a;
+template <bool kRaim> void fill(KernelArgs<kRaim> &a, const Scratch &sc);
+template <> void fill<false>(Args &a, const Scratch &sc) {
     a.ep = sc.d_epochs;
     a.ch = sc.d_chans;
     a.n = sc.d_n;
@@ -371,16 +488,39 @@ cudaError_t launch(Scratch &sc, cudaStream_t s) {
     a.cfg = sc.cfg;
     a.fixes = sc.d_fixes;
     a.res = sc.want_res ? sc.d_res : nullptr;
+}
+template <> void fill<true>(RaimArgs &a, const Scratch &sc) {
+    fill<false>(a, sc);
+    a.raim = sc.raim_cfg;
+    memcpy(a.T, sc.tab_T, sizeof a.T);
+    memcpy(a.lambda, sc.tab_lambda, sizeof a.lambda);
+    a.out = sc.d_raim;
+}
+
+template <bool kRaim> cudaError_t launch_as(const Scratch &sc, cudaStream_t s) {
+    KernelArgs<kRaim> a;
+    fill<kRaim>(a, sc);
     const int64_t blocks = ((int64_t) sc.cfg.nfix + kWarps - 1) / kWarps;
-    k_pvt<<<(unsigned) blocks, kWarps * 32, 0, s>>>(a);
+    k_pvt<kRaim><<<(unsigned) blocks, kWarps * 32, 0, s>>>(a);
     return cudaGetLastError();
+}
+
+cudaError_t launch(const Scratch &sc, cudaStream_t s) {
+    return sc.raim ? launch_as<true>(sc, s) : launch_as<false>(sc, s);
 }
 
 }  // namespace
 
 std::string check(const gpsb200_pvt_chan_t *chans, int nchan, const gpsb200_track_epoch_t *epochs, const int32_t *nepochs,
-                  int max_epochs, const gpsb200_pvt_config_t *cfg) {
+                  int max_epochs, const gpsb200_pvt_config_t *cfg, const gpsb200_raim_config_t *raim) {
     if (!chans || !epochs || !nepochs || !cfg) return "NULL chans, epochs, nepochs or cfg";
+    if (raim) {
+        if (!std::isfinite(raim->sigma) || !(raim->sigma > 0.0)) return "raim sigma must be finite and > 0";
+        if (!(raim->p_fa >= 1e-12 && raim->p_fa <= 0.5) || !(raim->p_md >= 1e-12 && raim->p_md <= 0.5))
+            return "raim p_fa and p_md must lie in 1e-12..0.5";
+        if (raim->max_exclude < 0 || raim->max_exclude > GPSB200_RAIM_MAX_EXCLUDE) return "raim max_exclude must be 0..4";
+        if (raim->reserved != 0) return "raim reserved must be 0";
+    }
     if (nchan < 1 || nchan > GPSB200_TRK_MAX_CHAN) return "nchan must be 1..32";
     if (max_epochs < 1) return "max_epochs must be >= 1";
     if (cfg->nfix < 1) return "nfix must be >= 1";
@@ -409,12 +549,14 @@ void scratch_free(Scratch &sc) {
     cudaFree(sc.d_n);
     cudaFree(sc.d_fixes);
     cudaFree(sc.d_res);
+    cudaFree(sc.d_raim);
     sc = Scratch();
 }
 
 cudaError_t run(Scratch &sc, const gpsb200_pvt_chan_t *chans, int nchan, const gpsb200_track_epoch_t *epochs,
-                const int32_t *nepochs, int max_epochs, const gpsb200_pvt_config_t *cfg, gpsb200_fix_t *fixes,
-                double *residuals, cudaStream_t s) {
+                const int32_t *nepochs, int max_epochs, const gpsb200_pvt_config_t *cfg,
+                const gpsb200_raim_config_t *raim, gpsb200_fix_t *fixes, double *residuals, gpsb200_raim_t *out,
+                cudaStream_t s) {
     sc.have_last = false;
     if (!sc.d_chans) {
         CU_RET(cudaMalloc(&sc.d_chans, GPSB200_TRK_MAX_CHAN * sizeof(gpsb200_pvt_chan_t)));
@@ -423,6 +565,16 @@ cudaError_t run(Scratch &sc, const gpsb200_pvt_chan_t *chans, int nchan, const g
     CU_RET(grow(sc.d_epochs, sc.epoch_cap, (size_t) nchan * max_epochs));
     CU_RET(grow(sc.d_fixes, sc.fix_cap, (size_t) cfg->nfix));
     if (residuals) CU_RET(grow(sc.d_res, sc.res_cap, (size_t) cfg->nfix * nchan));
+    sc.raim = raim != nullptr;
+    if (raim) {
+        CU_RET(grow(sc.d_raim, sc.raim_cap, (size_t) cfg->nfix));
+        sc.raim_cfg = *raim;
+        if (raim->p_fa != sc.tab_p_fa || raim->p_md != sc.tab_p_md) {   // the tables take 20-80 ms of host time
+            raim_thresholds(raim->p_fa, raim->p_md, sc.tab_T, sc.tab_lambda);
+            sc.tab_p_fa = raim->p_fa;
+            sc.tab_p_md = raim->p_md;
+        }
+    }
     // the reference channel of the nominal receive time: the lowest with a valid, healthy ephemeris
     sc.ref = -1;
     for (int c = 0; c < nchan && sc.ref < 0; c++)
@@ -441,6 +593,8 @@ cudaError_t run(Scratch &sc, const gpsb200_pvt_chan_t *chans, int nchan, const g
     CU_RET(cudaMemcpyAsync(fixes, sc.d_fixes, (size_t) cfg->nfix * sizeof(gpsb200_fix_t), cudaMemcpyDeviceToHost, s));
     if (residuals)
         CU_RET(cudaMemcpyAsync(residuals, sc.d_res, (size_t) cfg->nfix * nchan * sizeof(double), cudaMemcpyDeviceToHost, s));
+    if (raim)
+        CU_RET(cudaMemcpyAsync(out, sc.d_raim, (size_t) cfg->nfix * sizeof(gpsb200_raim_t), cudaMemcpyDeviceToHost, s));
     CU_RET(cudaStreamSynchronize(s));
     sc.have_last = true;
     return cudaSuccess;

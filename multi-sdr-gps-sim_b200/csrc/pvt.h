@@ -13,9 +13,15 @@ namespace pvt {
 constexpr int kWarps = 4;                // fixes per CTA of k_pvt (one warp each)
 constexpr int64_t kWeekMs = 604800000;   // ms of a GPS week
 
-// Empty when the call is well-formed (see the header).
+static_assert(sizeof(gpsb200_raim_config_t) == 32, "gpsb200_raim_config_t layout");
+static_assert(sizeof(gpsb200_raim_t) == 48, "gpsb200_raim_t layout");
+
+// Empty when the call is well-formed (see the header). raim may be NULL (gpsb200_pvt).
 std::string check(const gpsb200_pvt_chan_t *chans, int nchan, const gpsb200_track_epoch_t *epochs, const int32_t *nepochs,
-                  int max_epochs, const gpsb200_pvt_config_t *cfg);
+                  int max_epochs, const gpsb200_pvt_config_t *cfg, const gpsb200_raim_config_t *raim);
+
+// The RAIM tables of gpsb200_raim_thresholds (raim_thresholds.cpp); false when p_fa or p_md is outside 1e-12..0.5.
+bool raim_thresholds(double p_fa, double p_md, double *T, double *lambda);
 
 // Device scratch of the fix calls of one context, grown as needed, and what gpsb200_pvt_replay re-runs.
 struct Scratch {
@@ -32,13 +38,22 @@ struct Scratch {
     int64_t ref_sample = 0, ref_ms = 0;
     gpsb200_pvt_config_t cfg{};
     bool want_res = false;
+    // the RAIM stage of the previous call (gpsb200_pvt_raim), and the tables of the last p_fa / p_md seen
+    bool raim = false;
+    gpsb200_raim_config_t raim_cfg{};
+    gpsb200_raim_t *d_raim = nullptr;            // [nfix]
+    size_t raim_cap = 0;
+    double tab_p_fa = 0.0, tab_p_md = 0.0;       // 0: no tables yet
+    double tab_T[GPSB200_RAIM_MAX_DOF] = {}, tab_lambda[GPSB200_RAIM_MAX_DOF] = {};
 };
 
 void scratch_free(Scratch &sc);
-// Upload, run k_pvt on s and download the fixes (and residuals when not NULL); waits for the results.
+// Upload, run k_pvt on s and download the fixes (and residuals when not NULL); waits for the results. With raim
+// (not NULL) the kernel's RAIM instantiation runs and out [nfix] receives its records.
 cudaError_t run(Scratch &sc, const gpsb200_pvt_chan_t *chans, int nchan, const gpsb200_track_epoch_t *epochs,
-                const int32_t *nepochs, int max_epochs, const gpsb200_pvt_config_t *cfg, gpsb200_fix_t *fixes,
-                double *residuals, cudaStream_t s);
+                const int32_t *nepochs, int max_epochs, const gpsb200_pvt_config_t *cfg,
+                const gpsb200_raim_config_t *raim, gpsb200_fix_t *fixes, double *residuals, gpsb200_raim_t *out,
+                cudaStream_t s);
 // Enqueue k_pvt again on the previous call's device-resident inputs.
 cudaError_t replay(Scratch &sc, cudaStream_t s);
 

@@ -7,7 +7,8 @@
 // With --fix it then computes position fixes with gpsb200_pvt from what it decoded alone: each channel's ephemeris
 // (gpsb200_nav_ephemeris) and time anchor (gpsb200_nav_time_anchor); channels without both are left out. The fixes
 // start 0.5 s after the acquisition window (the loops have pulled in by then) and follow every --fix-every ms; one line
-// per fix with status GPSB200_FIX_OK (DESIGN §11).
+// per fix with status GPSB200_FIX_OK (DESIGN §11). With --raim the fixes come from gpsb200_pvt_raim and each line gains
+// the RAIM verdict, the PRNs it excluded ("-" for none) and HPL/VPL in metres (DESIGN §11.1).
 #include <algorithm>
 #include <cmath>
 #include <cstdio>
@@ -29,22 +30,27 @@ static const long long kFixLead = 1500000;        // samples from the start to t
 static void usage() {
     fprintf(stderr,
             "gpsb200-track FILE [--iq16] [--block B] [--offset-ms N] [--ms K] [--prn LIST] [--threshold R] [--device D]\n"
-            "              [--fix [--fix-every MS] [--iono a0,a1,a2,a3,b0,b1,b2,b3]]\n"
+            "              [--fix [--fix-every MS] [--iono a0,a1,a2,a3,b0,b1,b2,b3] [--raim SIGMA[,P_FA,P_MD[,MAX_EXCLUDE]]]]\n"
             "  FILE              interleaved I,Q at 3 Msps, int8 (default) or int16 (--iq16)\n"
             "  --block B         start at 0.1 s block B (sample 300000 B); --offset-ms N adds N ms (3000 N samples)\n"
             "  --ms K            track K ms of signal from the start (default: to the end of the file)\n"
             "  --prn LIST        PRNs searched, e.g. 1-32 (default), 3,7,12-15\n"
             "  --threshold R     P1/P2 at or above R counts as acquired and is tracked (default %.1f)\n"
             "  --fix             position, velocity and time from the decoded ephemeris and TOW, every --fix-every ms\n"
-            "                    (default %d) from 0.5 s after the start; --iono: the Klobuchar alpha / beta to apply\n",
+            "                    (default %d) from 0.5 s after the start; --iono: the Klobuchar alpha / beta to apply\n"
+            "  --raim            fault detection and exclusion with pseudorange sigma SIGMA m (P_FA 1e-5, P_MD 1e-3,\n"
+            "                    MAX_EXCLUDE 1 by default): adds the verdict, the excluded PRNs and HPL/VPL to each fix\n",
             kDefaultThreshold, kDefaultFixEvery);
     exit(2);
 }
 
-// Fixes from `first` every `step` samples to the last epoch of the channels, one line per fix with status OK.
+static const char *const kVerdict[] = {"PASS", "EXCLUDED", "ALERT", "UNAVAILABLE"};
+
+// Fixes from `first` every `step` samples to the last epoch of the channels, one line per fix with status OK; with
+// raim (not NULL) from gpsb200_pvt_raim, with its three columns.
 static int print_fixes(gpsb200_ctx_t *ctx, const std::vector<gpsb200_pvt_chan_t> &chans, const std::vector<int> &of,
                        const std::vector<std::vector<gpsb200_track_epoch_t>> &eps, long long first, long long step,
-                       gpsb200_pvt_config_t cfg) {
+                       gpsb200_pvt_config_t cfg, const gpsb200_raim_config_t *raim) {
     const int n = (int) chans.size();
     printf("# fixes: %d channel(s) with an ephemeris and a time anchor decoded, Klobuchar %s\n", n, cfg.iono ? "on" : "off");
     if (n == 0) return GPSB200_OK;
@@ -65,13 +71,26 @@ static int print_fixes(gpsb200_ctx_t *ctx, const std::vector<gpsb200_pvt_chan_t>
     cfg.step = step;
     cfg.nfix = (int32_t) ((end - first) / step + 1);
     std::vector<gpsb200_fix_t> fx(cfg.nfix);
-    const int rc = gpsb200_pvt(ctx, chans.data(), n, all.data(), cnt.data(), (int) me, &cfg, fx.data(), nullptr);
+    std::vector<gpsb200_raim_t> rm(raim ? cfg.nfix : 0);
+    const int rc = raim ? gpsb200_pvt_raim(ctx, chans.data(), n, all.data(), cnt.data(), (int) me, &cfg, raim, fx.data(),
+                                           nullptr, rm.data())
+                        : gpsb200_pvt(ctx, chans.data(), n, all.data(), cnt.data(), (int) me, &cfg, fx.data(), nullptr);
     if (rc != GPSB200_OK) return rc;
-    printf("# sample  tow_s  lat_deg  lon_deg  height_m  clock_m  vx  vy  vz (ECEF m/s)  channels  pdop\n");
-    for (const auto &f : fx)
-        if (f.status == GPSB200_FIX_OK)
-            printf("%lld  %.9f  %.8f  %.8f  %.3f  %.3f  %.3f  %.3f  %.3f  %d  %.2f\n", (long long) f.sample, f.t_rx,
-                   f.lat_deg, f.lon_deg, f.height, f.clock_m, f.vx, f.vy, f.vz, f.nused, f.pdop);
+    printf("# sample  tow_s  lat_deg  lon_deg  height_m  clock_m  vx  vy  vz (ECEF m/s)  channels  pdop%s\n",
+           raim ? "  raim  excluded_prns  hpl/vpl_m" : "");
+    for (int i = 0; i < cfg.nfix; i++) {
+        const gpsb200_fix_t &f = fx[i];
+        if (f.status != GPSB200_FIX_OK) continue;
+        printf("%lld  %.9f  %.8f  %.8f  %.3f  %.3f  %.3f  %.3f  %.3f  %d  %.2f", (long long) f.sample, f.t_rx, f.lat_deg,
+               f.lon_deg, f.height, f.clock_m, f.vx, f.vy, f.vz, f.nused, f.pdop);
+        if (raim) {
+            std::string ex;
+            for (int k = 0; k < n; k++)
+                if (rm[i].excluded >> k & 1u) ex += (ex.empty() ? "" : ",") + std::to_string(chans[k].prn);
+            printf("  %s  %s  %.2f/%.2f", kVerdict[rm[i].verdict], ex.empty() ? "-" : ex.c_str(), rm[i].hpl, rm[i].vpl);
+        }
+        printf("\n");
+    }
     return GPSB200_OK;
 }
 
@@ -84,6 +103,9 @@ int main(int argc, char **argv) {
     long long fix_every = kDefaultFixEvery;
     gpsb200_pvt_config_t pcfg;
     memset(&pcfg, 0, sizeof pcfg);
+    bool raim = false;
+    gpsb200_raim_config_t rcfg;
+    memset(&rcfg, 0, sizeof rcfg);
     gpsb200_acq_config_t cfg;
     memset(&cfg, 0, sizeof cfg);
     cfg.ms = kAcqMs;
@@ -109,11 +131,18 @@ int main(int argc, char **argv) {
                             &pcfg.beta[0], &pcfg.beta[1], &pcfg.beta[2], &pcfg.beta[3]};
             if (sscanf(val(), "%lf,%lf,%lf,%lf,%lf,%lf,%lf,%lf", v[0], v[1], v[2], v[3], v[4], v[5], v[6], v[7]) != 8) usage();
             pcfg.iono = 1;
+        } else if (a == "--raim") {
+            rcfg.p_fa = 1e-5;
+            rcfg.p_md = 1e-3;
+            rcfg.max_exclude = 1;
+            const int got = sscanf(val(), "%lf,%lf,%lf,%d", &rcfg.sigma, &rcfg.p_fa, &rcfg.p_md, &rcfg.max_exclude);
+            if (got != 1 && got != 3 && got != 4) usage();
+            raim = true;
         }
         else if (a[0] != '-' && !path) path = argv[i];
         else usage();
     }
-    if (!path || block < 0 || offset_ms < 0 || ms == 0 || ms < -1 || fix_every < 1) usage();
+    if (!path || block < 0 || offset_ms < 0 || ms == 0 || ms < -1 || fix_every < 1 || (raim && !fix)) usage();
     cfg.f_lo_hz = kAcqLo;
     cfg.step_hz = kAcqStep;
     cfg.nbins = (int) std::floor((kAcqHi - kAcqLo) / kAcqStep + 1e-9) + 1;
@@ -207,7 +236,8 @@ int main(int argc, char **argv) {
             }
         }
     }
-    if (fix) rc = print_fixes(ctx, fix_chans, fix_of, eps, s0 + kFixLead, fix_every * GPSB200_ACQ_CODE_SAMPLES, pcfg);
+    if (fix) rc = print_fixes(ctx, fix_chans, fix_of, eps, s0 + kFixLead, fix_every * GPSB200_ACQ_CODE_SAMPLES, pcfg,
+                              raim ? &rcfg : nullptr);
     if (rc != GPSB200_OK) fprintf(stderr, "gpsb200-track: %s\n", gpsb200_last_error(ctx));
     gpsb200_destroy(ctx);
     return rc == GPSB200_OK ? 0 : 1;

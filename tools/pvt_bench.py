@@ -10,7 +10,12 @@ the kernel alone (gpsb200_pvt_replay, median over --iters), fixes per second of 
 and the largest difference from the numpy model (tests/pvt_model.py) over a seeded sample of --check fix instants. The
 card's name, power limit and maximum SM clock are read in the same run (nvidia-smi). Writes nothing; needs a GPU.
 
-    python tools/pvt_bench.py [--iters 5] [--warmup 1] [--check 64] [--seconds 600]
+With --raim SIGMA the same run also times the RAIM stage (gpsb200_pvt_raim, DESIGN §11.1) in three arms, alternating
+--rounds times: the kernel without RAIM, with RAIM on the fault-free epochs, and with RAIM on epochs whose channel
+--fault carries a 0.1-chip code-phase bias (about 29 m), so that every fix excludes once. Each arm's kernel time is the
+median of its replays over all rounds; its verdict counts come from the call that set it up.
+
+    python tools/pvt_bench.py [--iters 5] [--warmup 1] [--check 64] [--seconds 600] [--raim SIGMA [--fault C]]
 """
 import argparse
 import importlib
@@ -59,12 +64,59 @@ def workload(seconds):
     return chans, eps, PT.klobuchar_broadcast(alpha, beta)
 
 
+def replay_ms(ctx, stream, iters):
+    import torch
+    out = []
+    ctx.pvt_replay(stream.cuda_stream)
+    for _ in range(iters):
+        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        a.record(stream)
+        ctx.pvt_replay(stream.cuda_stream)
+        b.record(stream)
+        b.synchronize()
+        out.append(a.elapsed_time(b))
+    return out
+
+
+def raim_arms(ctx, stream, chans, packed, n, cfg, args):
+    """Kernel time of the three arms, alternating, and the verdict counts of each."""
+    bad = packed.copy()
+    add = int(round(0.1 * 2.0 ** 32))
+    assert int(bad[args.fault, :n[args.fault]]["code_phase"].max()) + add < 2 ** 32
+    bad[args.fault, :n[args.fault]]["code_phase"] += np.uint32(add)
+    rcfg = gps.raim_config(args.raim)
+    arms = {"plain": lambda: ctx.pvt(chans, packed, cfg, nepochs=n),
+            "raim": lambda: ctx.pvt_raim(chans, packed, cfg, rcfg, nepochs=n),
+            "raim_fault": lambda: ctx.pvt_raim(chans, bad, cfg, rcfg, nepochs=n)}
+    times = {k: [] for k in arms}
+    verdicts = {}
+    for _ in range(args.rounds):
+        for k, call in arms.items():
+            got = call()
+            if k != "plain":
+                v, c = np.unique(got[1]["verdict"], return_counts=True)
+                verdicts[k] = {int(a): int(b) for a, b in zip(v, c)}
+                if k == "raim_fault":
+                    tested = got[1]["verdict"] != gps.RAIM_UNAVAILABLE
+                    verdicts["raim_fault_excluded_only_channel"] = bool(np.all(got[1]["excluded"][tested] ==
+                                                                               1 << args.fault))
+            times[k] += replay_ms(ctx, stream, args.iters)
+    out = {"sigma": args.raim, "fault_channel": args.fault, "rounds": args.rounds, "verdicts": verdicts}
+    for k, t in times.items():
+        out[k + "_kernel_ms_median"] = round(float(np.median(t)), 3)
+        out[k + "_kernel_ms_min"] = round(float(np.min(t)), 3)
+    return out
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--iters", type=int, default=5)
     ap.add_argument("--warmup", type=int, default=1)
     ap.add_argument("--check", type=int, default=64)
     ap.add_argument("--seconds", type=int, default=600)
+    ap.add_argument("--raim", type=float, default=None)
+    ap.add_argument("--fault", type=int, default=0)
+    ap.add_argument("--rounds", type=int, default=3)
     args = ap.parse_args()
     import torch
     if not torch.cuda.is_available():
@@ -99,6 +151,7 @@ def main():
             b.record(stream)
             b.synchronize()
             kern.append(a.elapsed_time(b))
+        raim = raim_arms(ctx, stream, chans, packed, n, cfg, args) if args.raim is not None else None
     rng = np.random.default_rng(1)
     worst = {f: 0.0 for f in ("x", "y", "z", "clock_m", "vx", "vy", "vz")}
     for i in rng.choice(nfix, size=min(args.check, nfix), replace=False):
@@ -116,7 +169,8 @@ def main():
                       "kernel_ms_median": round(t_kern, 3), "kernel_ms_min": round(float(np.min(kern)), 3),
                       "iters": args.iters, "fixes_per_s_kernel": round(nfix / (t_kern * 1e-3)),
                       "status_counts": st, "checked": min(args.check, nfix),
-                      "max_abs_diff_vs_model": {k: float("%.3g" % v) for k, v in worst.items()}}), flush=True)
+                      "max_abs_diff_vs_model": {k: float("%.3g" % v) for k, v in worst.items()},
+                      **({"raim": raim} if raim is not None else {})}), flush=True)
 
 
 if __name__ == "__main__":
