@@ -124,8 +124,8 @@ def llh_ecef(lat_deg, lon_deg, h):
                      (N * (1.0 - WGS_E ** 2) + h) * np.sin(lat)])
 
 
-def klobuchar(alpha, beta, lat, lon, az, el, t):
-    """IS-GPS-200 20.3.3.5.2.5 as the reference evaluates it (gps.c:1893-1964), in metres."""
+def klobuchar(alpha, beta, lat, lon, az, el, t, trace=None):
+    """IS-GPS-200 20.3.3.5.2.5 as the reference evaluates it (gps.c:1893-1964), in metres. trace: see pvt()."""
     E, phi_u, lam_u = el / PI, lat / PI, lon / PI
     F = 1.0 + 16.0 * (0.53 - E) ** 3
     psi = 0.0137 / (E + 0.11) - 0.022
@@ -136,11 +136,16 @@ def klobuchar(alpha, beta, lat, lon, az, el, t):
     per = np.maximum(beta[0] + beta[1] * phi_m + beta[2] * phi_m ** 2 + beta[3] * phi_m ** 3, 72000.0)
     tl = np.mod(43200.0 * lam_i + t, 86400.0)
     X = 2.0 * PI * (tl - 50400.0) / per
+    if trace is not None:
+        trace["klobuchar_x"].append(np.ravel(X))
     return np.where(np.abs(X) < 1.57, F * (5.0e-9 + amp * (1.0 - X * X / 2.0 + X ** 4 / 24.0)) * C, F * 5.0e-9 * C)
 
 
-def pvt(chans, epochs, cfg):
+def pvt(chans, epochs, cfg, trace=None):
     """The fixes of the contract. chans: PVT_CHAN records; epochs: list of TRACK_EPOCH arrays; cfg: PVT_CONFIG record.
+    trace: None, or a dict whose lists "radius", "runaway", "step" and "klobuchar_x" receive, per iteration, the values
+    the model compares with IONO_MIN_RADIUS, RUNAWAY, CONVERGED and the Klobuchar |X| < 1.57 branch (so that a caller can
+    check that no decision sits on its threshold).
     -> (fix dict of arrays [F] with the FIX_DTYPE field names, residuals [F, C], measurement dict of measure())."""
     nf, nc = int(cfg["nfix"]), len(epochs)
     s = int(cfg["s0"]) + np.arange(nf, dtype=np.int64) * int(cfg["step"])
@@ -191,7 +196,8 @@ def pvt(chans, epochs, cfg):
         los = pr - x[:, None, :3]
         R = np.linalg.norm(los, axis=-1)
         I = np.zeros(R.shape)
-        iono = bool(cfg["iono"]) & (np.linalg.norm(x[:, :3], axis=-1) >= IONO_MIN_RADIUS)
+        rad = np.linalg.norm(x[:, :3], axis=-1)
+        iono = bool(cfg["iono"]) & (rad >= IONO_MIN_RADIUS)
         if iono.any():
             lat, lon, _ = ecef_llh(x[:, :3])
             sla, cla, slo, clo = (f(v)[:, None] for f, v in ((np.sin, lat), (np.cos, lat), (np.sin, lon), (np.cos, lon)))
@@ -202,7 +208,8 @@ def pvt(chans, epochs, cfg):
             az = np.where(az < 0.0, az + 2.0 * PI, az)
             el = np.arctan2(uu, np.hypot(nn, ee))
             trx = (nom_ms[a] * 1e-3 + m[a] / 3e6 - x[:, 3] / C)[:, None]
-            I = np.where(iono[:, None], klobuchar(cfg["alpha"], cfg["beta"], lat[:, None], lon[:, None], az, el, trx), 0.0)
+            I = np.where(iono[:, None], klobuchar(cfg["alpha"], cfg["beta"], lat[:, None], lon[:, None], az, el, trx,
+                                                      trace), 0.0)
         ra = (rho[a] - (R + x[:, 3:4] - C * dtsv[a] + I)) * w[a]
         Ha = np.concatenate([-los / R[..., None], np.ones(R.shape + (1,))], -1) * w[a][..., None]
         H[a], r[a] = Ha, ra
@@ -217,9 +224,13 @@ def pvt(chans, epochs, cfg):
         X[a] += d
         dX[a] = d
         Nmat[a] = N
-        away = np.linalg.norm(X[a, :3], axis=-1) > RUNAWAY
+        out, step = np.linalg.norm(X[a, :3], axis=-1), np.linalg.norm(d[:, :3], axis=-1)
+        if trace is not None:
+            for k, v in (("radius", rad), ("runaway", out), ("step", step)):
+                trace[k].append(v)
+        away = out > RUNAWAY
         active[a[away]] = False
-        conv = (np.linalg.norm(d[:, :3], axis=-1) < CONVERGED) & ~away
+        conv = (step < CONVERGED) & ~away
         status[a[conv]] = FIX_OK
         active[a[conv]] = False
     fix = {f: np.full(nf, np.nan) for f in ("x", "y", "z", "clock_m", "t_rx", "vx", "vy", "vz", "drift", "lat_deg",
