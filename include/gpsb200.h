@@ -649,6 +649,95 @@ int gpsb200_pvt_raim(gpsb200_ctx_t *ctx, const gpsb200_pvt_chan_t *chans, int nc
                      const int32_t *nepochs, int max_epochs, const gpsb200_pvt_config_t *cfg,
                      const gpsb200_raim_config_t *raim, gpsb200_fix_t *fixes, double *residuals, gpsb200_raim_t *out);
 
+/* ---- advanced RAIM: weighted fix, elevation mask, solution separation and ARAIM protection levels (DESIGN §11.2;
+ * tests/araim_model.py states it in numpy). GPS L1 C/A only, single-satellite faults, at most one exclusion, no
+ * constellation faults and no wrong-exclusion term (where this differs from the EU-US ARAIM Airborne Algorithm
+ * Description: DESIGN §11.2). Per fix instant:
+ *   1. Channel set. Channel i can enter the set S when gpsb200_pvt would use it and its broadcast eph.ura < 15.
+ *      sigma_URA,i = max(cfg.sigma_ura, URA_nom(eph.ura)), URA_nom = 2.0, 2.8, 4, 5.7, 8, 11.3, 16, 32, 64, 128, 256, 512,
+ *      1024, 2048, 4096 m (IS-GPS-200 20.3.3.3.1.3); sigma_URE,i = sigma_URA,i sigma_ure / sigma_ura.
+ *   2. Weights, at the elevation el of the channel's line of sight (the rotated satellite position, as in gpsb200_pvt)
+ *      from the current estimate X_j, in every Gauss-Newton iteration; el = 90 deg while |x_j| < 6e6 m:
+ *        sigma_int,i^2 = sigma_URA,i^2 + sigma_tropo^2 + sigma_air^2 + sigma_iono^2, sigma_acc,i^2 the same with
+ *        sigma_URE,i; sigma_tropo = 0.12 1.001 / sqrt(0.002001 + sin^2 el); sigma_air^2 = sigma_noise^2 +
+ *        (0.13 + 0.53 exp(-el / 10 deg))^2; sigma_iono = max(I / 5, F tau(|phi_m|)) when cfg.iono and |x_j| >= 6e6 m,
+ *        else 0, with I, F and phi_m the Klobuchar delay, obliquity factor and geomagnetic latitude of gpsb200_pvt's
+ *        Klobuchar term and tau = 9 m for |phi_m| <= 20 deg, 4.5 m for <= 55 deg, 6 m above (DO-229 J.2.3).
+ *   3. Weighted Gauss-Newton: gpsb200_pvt's solve (from the Earth's centre, the same convergence, runaway and
+ *      positive-definiteness rules) with each row and residual scaled by 1 / sigma_int,i.
+ *   4. Elevation mask: after the first converged solve, the channels with el (of the last iteration) < mask_deg leave
+ *      S (bit c of `masked`). If any left, Gauss-Newton again from that fix (status 1 when fewer than 4 remain).
+ *   5. Solution separation at the final fix, n = |S| >= 5 (else UNAVAILABLE). G = the last iteration's rows (g_i, 1),
+ *      W = diag(1 / sigma_int,i^2), y = its prefit residuals, positions in east / north / up at the fix's WGS-84
+ *      latitude and longitude. S0 = (G^T W G)^-1 G^T W; S(k) the same without row k (column k zero), for each k in S.
+ *      dx(k) = (S(k) - S0) y; sigma_q(k)^2 = (S(k) C_int S(k)^T)_qq; sigma_ss,q(k)^2 = ((S(k) - S0) C_acc
+ *      (S(k) - S0)^T)_qq; b_q(k) = sum_i |S(k)_qi| b_nom, and b_q0, sigma_q0 the same for S0; C = diag(sigma^2).
+ *      UNAVAILABLE when some G^T W(k) G is not positive definite.
+ *   6. Test: T_k,q = K_fa,q sigma_ss,q(k), K_fa,H = Q^-1(p_fa_horz / (4 n)) for east and north, K_fa,V =
+ *      Q^-1(p_fa_vert / (2 n)) for up (Q the standard normal upper tail; gpsb200_araim_kfa). Passes when
+ *      |dx_q(k)| <= T_k,q for every k and q; test_ratio = max |dx_q(k)| / T_k,q.
+ *   7. Exclusion, when the test fails, max_exclude is 1 and n >= 6: the k with the largest max_q |dx_q(k)| / T_k,q
+ *      (the lowest channel on ties) leaves S; Gauss-Newton again from the current fix, then 5-6 on the new set:
+ *      EXCLUDED when it passes, else ALERT (also when that solve fails). Otherwise a failed test is ALERT.
+ *   8. Protection levels over the final set: P_NM = 1 - (1 - p_sat)^n - n p_sat (1 - p_sat)^(n-1) (UNAVAILABLE when
+ *      P_NM >= p_hmi_vert + p_hmi_horz); VPL the smallest L with
+ *        2 Q((L - b_U0) / sigma_U0) + sum_k p_sat Q((L - T_k,U - b_U(k)) / sigma_U(k)) <= p_hmi_vert (1 - P_NM /
+ *        (p_hmi_vert + p_hmi_horz)),
+ *      HPL_E and HPL_N the same in east and north with p_hmi_horz / 2 in place of p_hmi_vert, HPL = sqrt(HPL_E^2 +
+ *      HPL_N^2). Each by bisection (Q^-1(p) = sqrt(2) erfcinv(2 p) on the device): lo = the largest single-term
+ *      solution (b0 + sigma0 Q^-1(rhs / 2); for each k, when rhs < p_sat, T + b + sigma Q^-1(rhs / p_sat)), hi = the
+ *      same with rhs / (n + 1); halve until hi - lo <= 1e-3 m; the level is hi. EMT = max_k T_k,U, sigma_acc_v =
+ *      sqrt((S0 C_acc S0^T)_UU).
+ * The fix record describes the final set: mask, nused, status, position and clock; iterations counts every pass;
+ * velocity and drift come from the weighted rows, and pdop = sqrt of the trace of the position block of
+ * (G^T W G)^-1, in metres (the weighted solution's position sigma). residuals: every measured channel's post-fit
+ * residual against the final fix (masked and excluded channels included), NaN for the others. Record fields that
+ * no step computed are NaN (n, excluded, masked 0). */
+typedef struct gpsb200_araim_config {
+    double mask_deg;       /* elevation mask, deg: 0..90 */
+    double sigma_ura;      /* floor of the integrity sigma, m: 0 < sigma_ura <= 100 */
+    double sigma_ure;      /* accuracy sigma at sigma_ura, m: 0 < sigma_ure <= sigma_ura */
+    double sigma_noise;    /* receiver noise sigma, m: 0..100 */
+    double b_nom;          /* nominal bias, m: 0..100 */
+    double p_sat;          /* prior probability of a satellite fault: 1e-12..1e-2 */
+    double p_hmi_vert, p_hmi_horz;   /* integrity budgets: 1e-12..0.5 each */
+    double p_fa_vert, p_fa_horz;     /* false-alarm budgets: 1e-12..0.5 each */
+    int32_t max_exclude;   /* 0 or 1 */
+    int32_t reserved[3];   /* 0 */
+} gpsb200_araim_config_t;  /* 96 bytes */
+/* Documented defaults (LPV-200 allocations; araim_config() in Python): */
+#define GPSB200_ARAIM_MASK_DEG 5.0
+#define GPSB200_ARAIM_SIGMA_URA 1.0
+#define GPSB200_ARAIM_SIGMA_URE (2.0 / 3.0)
+#define GPSB200_ARAIM_SIGMA_NOISE 0.36
+#define GPSB200_ARAIM_B_NOM 0.75
+#define GPSB200_ARAIM_P_SAT 1e-5
+#define GPSB200_ARAIM_P_HMI_VERT 9.8e-8
+#define GPSB200_ARAIM_P_HMI_HORZ 2e-9
+#define GPSB200_ARAIM_P_FA_VERT 3.9e-6
+#define GPSB200_ARAIM_P_FA_HORZ 9e-8
+typedef struct gpsb200_araim {
+    int32_t verdict;       /* GPSB200_RAIM_* */
+    uint32_t excluded;     /* bit c: channel c excluded (at most one) */
+    uint32_t masked;       /* bit c: channel c below the elevation mask */
+    int32_t n;             /* channels in the final set */
+    double test_ratio;     /* max |dx| / T of the last test */
+    double hpl, vpl;       /* m */
+    double emt;            /* max_k T_k,U of the last test, m */
+    double sigma_acc_v;    /* m */
+    double p_nm;           /* the unmonitored fault probability of the final set */
+} gpsb200_araim_t;         /* 64 bytes */
+/* Host: K_fa,H[n - 5] and K_fa,V[n - 5] of step 6 for n = 5..32 (1e-13 relative or better). GPSB200_ERR_ARG when a
+ * probability is outside 1e-12..0.5 or an array is NULL. */
+int gpsb200_araim_kfa(double p_fa_vert, double p_fa_horz, double kfa_h[GPSB200_RAIM_MAX_DOF],
+                      double kfa_v[GPSB200_RAIM_MAX_DOF]);
+/* gpsb200_pvt with the ARAIM stage above: the same arguments and checks, plus the ARAIM config (GPSB200_ERR_ARG outside
+ * its ranges) and out [nfix]. gpsb200_pvt_replay re-runs it when it ran last. */
+int gpsb200_pvt_araim(gpsb200_ctx_t *ctx, const gpsb200_pvt_chan_t *chans, int nchan, const gpsb200_track_epoch_t *epochs,
+                      const int32_t *nepochs, int max_epochs, const gpsb200_pvt_config_t *cfg,
+                      const gpsb200_araim_config_t *araim, gpsb200_fix_t *fixes, double *residuals,
+                      gpsb200_araim_t *out);
+
 /* ---- scenario engine: the reference's host path outside the sample loop -------------
  * RINEX-2/3 navigation file (plain or gzip-compressed, read through zlib like the reference, gps.c:1147) +
  * location/motion -> the gpsb200_chan_t records and NAV frames the

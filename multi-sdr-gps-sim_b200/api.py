@@ -215,6 +215,38 @@ def raim_config(sigma, p_fa=1e-5, p_md=1e-3, max_exclude=1):
     return c
 
 
+# gpsb200_araim_config_t / gpsb200_araim_t (DESIGN §11.2)
+ARAIM_CONFIG_DTYPE = np.dtype([("mask_deg", "<f8"), ("sigma_ura", "<f8"), ("sigma_ure", "<f8"), ("sigma_noise", "<f8"),
+                               ("b_nom", "<f8"), ("p_sat", "<f8"), ("p_hmi_vert", "<f8"), ("p_hmi_horz", "<f8"),
+                               ("p_fa_vert", "<f8"), ("p_fa_horz", "<f8"), ("max_exclude", "<i4"),
+                               ("reserved", "<i4", (3,))])
+ARAIM_DTYPE = np.dtype([("verdict", "<i4"), ("excluded", "<u4"), ("masked", "<u4"), ("n", "<i4"),
+                        ("test_ratio", "<f8"), ("hpl", "<f8"), ("vpl", "<f8"), ("emt", "<f8"), ("sigma_acc_v", "<f8"),
+                        ("p_nm", "<f8")])
+assert (ARAIM_CONFIG_DTYPE.itemsize, ARAIM_DTYPE.itemsize) == (96, 64)
+
+
+def araim_config(mask_deg=5.0, sigma_ura=1.0, sigma_ure=2.0 / 3.0, sigma_noise=0.36, b_nom=0.75, p_sat=1e-5,
+                 p_hmi_vert=9.8e-8, p_hmi_horz=2e-9, p_fa_vert=3.9e-6, p_fa_horz=9e-8, max_exclude=1):
+    """An ARAIM_CONFIG_DTYPE record; the defaults are the header's (LPV-200 allocations)."""
+    c = np.zeros(1, ARAIM_CONFIG_DTYPE)[0]
+    for k, v in (("mask_deg", mask_deg), ("sigma_ura", sigma_ura), ("sigma_ure", sigma_ure),
+                 ("sigma_noise", sigma_noise), ("b_nom", b_nom), ("p_sat", p_sat), ("p_hmi_vert", p_hmi_vert),
+                 ("p_hmi_horz", p_hmi_horz), ("p_fa_vert", p_fa_vert), ("p_fa_horz", p_fa_horz)):
+        c[k] = float(v)
+    c["max_exclude"] = int(max_exclude)
+    return c
+
+
+def araim_kfa(p_fa_vert, p_fa_horz):
+    """gpsb200_araim_kfa: (K_fa,H[28], K_fa,V[28]) for n = 5..32 channels in the set."""
+    kh, kv = np.zeros(RAIM_MAX_DOF), np.zeros(RAIM_MAX_DOF)
+    rc = lib().gpsb200_araim_kfa(float(p_fa_vert), float(p_fa_horz), kh.ctypes.data, kv.ctypes.data)
+    if rc:
+        raise GpsB200Error(rc, "gpsb200_araim_kfa")
+    return kh, kv
+
+
 def raim_thresholds(p_fa, p_md):
     """gpsb200_raim_thresholds: (T[28], lambda[28]) for dof 1..28; T[d - 1] is the chi^2(d) value with upper tail p_fa,
     lambda[d - 1] the noncentrality whose noncentral chi^2(d) CDF at T[d - 1] is p_md."""
@@ -285,7 +317,7 @@ EXPORTS = ["gpsb200_create", "gpsb200_destroy", "gpsb200_last_error", "gpsb200_v
            "gpsb200_codegen", "gpsb200_acquire", "gpsb200_acquire_device", "gpsb200_track_start", "gpsb200_track",
            "gpsb200_track_device", "gpsb200_nav_decode", "gpsb200_nav_word_check", "gpsb200_nav_parity",
            "gpsb200_nav_ephemeris", "gpsb200_nav_time_anchor", "gpsb200_pvt", "gpsb200_pvt_replay",
-           "gpsb200_pvt_raim", "gpsb200_raim_thresholds", "gpsb200_bind_numa", "gpsb200_span_chain_host", "gpsb200_lanes_model_block",
+           "gpsb200_pvt_raim", "gpsb200_raim_thresholds", "gpsb200_pvt_araim", "gpsb200_araim_kfa", "gpsb200_bind_numa", "gpsb200_span_chain_host", "gpsb200_lanes_model_block",
            "gpsb200_lanes_window_band_host", "gpsb200_slice_prepare", "gpsb200_slice_probe",
            "gpsb200_slice_finish", "gpsb200_slice_finish_cb", "gpsb200_slice_wait", "gpsb200_link_apply", "gpsb200_slice_link_host", "gpsb200_debug_corrupt_chain", "gpsb200_synth_kernel_name",
            "gpsb200_debug_run_checkpoints", "gpsb200_checkpoint_segments_host",
@@ -393,6 +425,8 @@ def lib():
         L.gpsb200_pvt_raim.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p,
                                        C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
         L.gpsb200_raim_thresholds.argtypes = [C.c_double, C.c_double, C.c_void_p, C.c_void_p]
+        L.gpsb200_pvt_araim.argtypes = L.gpsb200_pvt_raim.argtypes
+        L.gpsb200_araim_kfa.argtypes = [C.c_double, C.c_double, C.c_void_p, C.c_void_p]
         _lib = L
     return _lib
 
@@ -948,6 +982,19 @@ class Context:
         self._check(lib().gpsb200_pvt_raim(self._h, ch.ctypes.data, nchan, ep.ctypes.data, n.ctypes.data, me,
                                            cf.ctypes.data, rc.ctypes.data, fixes.ctypes.data,
                                            None if res is None else res.ctypes.data, out.ctypes.data))
+        return (fixes, out, res) if want_residuals else (fixes, out)
+
+    def pvt_araim(self, chans, epochs, cfg, araim, want_residuals=False, nepochs=None):
+        """Fixes with advanced RAIM: weighted solve, elevation mask, solution-separation test and protection levels
+        (gpsb200_pvt_araim; DESIGN §11.2). The arguments of pvt, plus araim: ARAIM_CONFIG_DTYPE record (araim_config).
+        -> (fixes FIX_DTYPE[nfix] of each fix's final set, ARAIM_DTYPE[nfix]), and with want_residuals also the
+        residuals float64[nfix, nchan]: every measured channel's post-fit residual against the final fix."""
+        ch, nchan, ep, n, me, cf, fixes, res = self._pvt_args(chans, epochs, cfg, want_residuals, nepochs)
+        ac = np.array(araim, dtype=ARAIM_CONFIG_DTYPE).reshape(1)
+        out = np.zeros(fixes.size, ARAIM_DTYPE)
+        self._check(lib().gpsb200_pvt_araim(self._h, ch.ctypes.data, nchan, ep.ctypes.data, n.ctypes.data, me,
+                                            cf.ctypes.data, ac.ctypes.data, fixes.ctypes.data,
+                                            None if res is None else res.ctypes.data, out.ctypes.data))
         return (fixes, out, res) if want_residuals else (fixes, out)
 
     @staticmethod

@@ -47,7 +47,17 @@ struct RaimArgs : Args {
     double T[GPSB200_RAIM_MAX_DOF], lambda[GPSB200_RAIM_MAX_DOF];
     gpsb200_raim_t *out;
 };
+// The ARAIM instantiation's: K_fa,H / K_fa,V for n = 5..32 go up with the launch, as the chi^2 tables do.
+struct AraimArgs : Args {
+    gpsb200_araim_config_t araim;
+    double kh[GPSB200_RAIM_MAX_DOF], kv[GPSB200_RAIM_MAX_DOF];
+    gpsb200_araim_t *out;
+};
 template <bool kRaim> using KernelArgs = typename std::conditional<kRaim, RaimArgs, Args>::type;
+
+__constant__ double kUraNom[15] = {2.0, 2.8, 4.0, 5.7, 8.0, 11.3, 16.0, 32.0, 64.0, 128.0, 256.0, 512.0, 1024.0, 2048.0,
+                                   4096.0};
+constexpr double kTenDeg = 10.0 * M_PI / 180.0;
 
 __device__ inline double wrap_half_week(double d) { return d > 302400.0 ? d - 604800.0 : (d < -302400.0 ? d + 604800.0 : d); }
 
@@ -144,7 +154,9 @@ __device__ void ecef_llh(const double *x, double &lat, double &lon, double &h) {
 }
 
 // The Klobuchar delay in metres (the reference's ionosphericDelay, gps.c:1893-1964, with a valid alpha / beta set).
-__device__ double klobuchar(const gpsb200_pvt_config_t &cfg, double lat, double lon, double az, double el, double t) {
+// Fm (not NULL): receives the obliquity factor F and the geomagnetic latitude phi_m (semicircles) as well.
+__device__ double klobuchar(const gpsb200_pvt_config_t &cfg, double lat, double lon, double az, double el, double t,
+                            double *Fm = nullptr) {
     const double E = el / kPi, phi_u = lat / kPi, lam_u = lon / kPi;
     const double om = 0.53 - E;
     const double F = 1.0 + 16.0 * om * om * om;
@@ -153,6 +165,10 @@ __device__ double klobuchar(const gpsb200_pvt_config_t &cfg, double lat, double 
     phi_i = phi_i > 0.416 ? 0.416 : (phi_i < -0.416 ? -0.416 : phi_i);
     const double lam_i = lam_u + psi * sin(az) / cos(phi_i * kPi);
     const double phi_m = phi_i + 0.064 * cos((lam_i - 1.617) * kPi);
+    if (Fm) {
+        Fm[0] = F;
+        Fm[1] = phi_m;
+    }
     const double pm2 = phi_m * phi_m, pm3 = pm2 * phi_m;
     double amp = cfg.alpha[0] + cfg.alpha[1] * phi_m + cfg.alpha[2] * pm2 + cfg.alpha[3] * pm3;
     if (amp < 0.0) amp = 0.0;
@@ -239,6 +255,118 @@ __device__ int find_period(const gpsb200_track_epoch_t *e, int n, int64_t s) {
         hi = n - 2;
     }
     return -1;
+}
+
+// ---- ARAIM (DESIGN §11.2) --------------------------------------------------------------------------------------------
+__device__ inline double q_tail(double x) { return 0.5 * erfc(x / M_SQRT2); }          // the standard normal upper tail
+__device__ inline double q_inv(double p) { return M_SQRT2 * erfcinv(2.0 * p); }
+
+// One solution-separation pass at a fix (header, step 5-6): this lane's fault hypothesis k and hypothesis 0.
+struct Ss {
+    double dx[3], T[3], b[3], s[3];   // east, north, up of hypothesis k (this lane's channel, when in the set)
+    double b0[3], s0[3];              // hypothesis 0 (the same on every lane)
+    double ratio;                     // max_q |dx_q| / T_q; -1 outside the set
+    bool pass;                        // |dx_q| <= T_q for every q (true outside the set)
+    bool pd;                          // G^T W(k) G positive definite (true outside the set)
+};
+
+// use: this lane's channel is in the set; h, sw (= 1 / sigma_int), r: its row, weight and prefit residual of the last
+// Gauss-Newton iteration, acc2 = sigma_acc^2; N, ch: that iteration's normal matrix and its factor; X: the fix. The
+// subset solutions come from N_k = N - w_k g_k g_k^T, which each lane factors itself; the sums over the other channels'
+// rows run in one loop over the lanes (__shfl_sync), O(n^2) per fix. Returns sigma_acc,U.
+__device__ double mhss(const AraimArgs &a, bool use, int n, const double *h, double sw, double r, double acc2,
+                       const double *N, const Chol &ch, const double *X, Ss &o) {
+    const int lane = threadIdx.x & 31;
+    double lat, lon, hgt, sla, cla, slo, clo;
+    ecef_llh(X, lat, lon, hgt);
+    sincos(lat, &sla, &cla);
+    sincos(lon, &slo, &clo);
+    const double u[3][3] = {{-slo, clo, 0.0}, {-sla * clo, -sla * slo, cla}, {cla * clo, cla * slo, sla}};
+    // the normal matrix less this lane's row
+    const double w0 = use ? h[0] * sw : 0.0, w1 = use ? h[1] * sw : 0.0, w2 = use ? h[2] * sw : 0.0, wc = use ? sw : 0.0;
+    const double Nk[10] = {N[0] - w0 * w0, N[1] - w0 * w1, N[2] - w0 * w2, N[3] - w0 * wc, N[4] - w1 * w1,
+                           N[5] - w1 * w2, N[6] - w1 * wc, N[7] - w2 * w2, N[8] - w2 * wc, N[9] - wc * wc};
+    Chol ck;
+    const bool fk = use && ck.factor(Nk);
+    o.pd = !use || fk;
+    double z[3][4], z0[3][4];   // N_k^-1 u_q and N^-1 u_q
+#pragma unroll
+    for (int q = 0; q < 3; q++) {
+        const double e[4] = {u[q][0], u[q][1], u[q][2], 0.0};
+        ch.solve(e, z0[q]);
+        o.s0[q] = sqrt(e[0] * z0[q][0] + e[1] * z0[q][1] + e[2] * z0[q][2]);
+        if (fk) {
+            ck.solve(e, z[q]);
+            o.s[q] = sqrt(e[0] * z[q][0] + e[1] * z[q][1] + e[2] * z[q][2]);
+        } else {
+            z[q][0] = z[q][1] = z[q][2] = z[q][3] = 0.0;
+            o.s[q] = 0.0;
+        }
+    }
+    // S(k)_qi = w_i z_q . g_i (i != k), S0_qi = w_i z0_q . g_i, summed over the set's channels i
+    const double wself = use ? sw * sw : 0.0;
+    double bb[3] = {0, 0, 0}, ss[3] = {0, 0, 0}, dx[3] = {0, 0, 0};
+#pragma unroll 1
+    for (int i = 0; i < a.nchan; i++) {
+        const double g0 = __shfl_sync(kFull, h[0], i), g1 = __shfl_sync(kFull, h[1], i), g2 = __shfl_sync(kFull, h[2], i);
+        const double wi = __shfl_sync(kFull, wself, i), yi = __shfl_sync(kFull, r, i), ai = __shfl_sync(kFull, acc2, i);
+#pragma unroll
+        for (int q = 0; q < 3; q++) {
+            const double Sk = i == lane ? 0.0 : wi * (z[q][0] * g0 + z[q][1] * g1 + z[q][2] * g2 + z[q][3]);
+            const double dS = Sk - wi * (z0[q][0] * g0 + z0[q][1] * g1 + z0[q][2] * g2 + z0[q][3]);
+            bb[q] += fabs(Sk);
+            ss[q] += dS * dS * ai;
+            dx[q] += dS * yi;
+        }
+    }
+    const double kfa[3] = {a.kh[n - 5], a.kh[n - 5], a.kv[n - 5]};
+    o.pass = true;
+    o.ratio = -1.0;
+    double sacc = 0.0;
+#pragma unroll
+    for (int q = 0; q < 3; q++) {
+        const double S0 = wself * (z0[q][0] * h[0] + z0[q][1] * h[1] + z0[q][2] * h[2] + z0[q][3]);
+        o.b0[q] = a.araim.b_nom * warp_sum(fabs(S0));
+        if (q == 2) sacc = sqrt(warp_sum(S0 * S0 * acc2));
+        o.dx[q] = dx[q];
+        o.b[q] = a.araim.b_nom * bb[q];
+        o.T[q] = kfa[q] * sqrt(ss[q]);
+        if (use) {
+            o.pass = o.pass && fabs(dx[q]) <= o.T[q];
+            o.ratio = fmax(o.ratio, fabs(dx[q]) / o.T[q]);
+        }
+    }
+    return sacc;
+}
+
+// The smallest level L with 2 Q((L - b0) / s0) + sum over the set's lanes of p_sat Q((L - T - b) / s) <= rhs, by
+// bisection to 1e-3 m (header, step 8). Every lane takes the same branches: the sums are butterflies.
+__device__ double protection_level(double rhs, double b0, double s0, bool use, double T, double b, double s,
+                                   double p_sat, int n) {
+    const double m = (double) (n + 1);
+    double lo = b0 + s0 * q_inv(rhs / 2.0), hi = b0 + s0 * q_inv(rhs / m / 2.0);
+    lo = fmax(lo, warp_max(use && rhs < p_sat ? T + b + s * q_inv(rhs / p_sat) : -HUGE_VAL));
+    hi = fmax(hi, warp_max(use && rhs / m < p_sat ? T + b + s * q_inv(rhs / m / p_sat) : -HUGE_VAL));
+#pragma unroll 1
+    for (int it = 0; it < 200 && hi - lo > 1e-3; it++) {
+        const double mid = 0.5 * (lo + hi);
+        const double lhs = 2.0 * q_tail((mid - b0) / s0) + warp_sum(use ? p_sat * q_tail((mid - T - b) / s) : 0.0);
+        if (lhs <= rhs) hi = mid;
+        else lo = mid;
+    }
+    return hi;
+}
+
+// P_NM = 1 - (1 - p)^n - n p (1 - p)^(n-1), summed as the binomial tail sum_{j >= 2} C(n, j) p^j (1 - p)^(n-j), which
+// has no cancellation.
+__device__ double p_not_monitored(double p, int n) {
+    double t = 0.5 * n * (n - 1) * p * p * pow(1.0 - p, (double) (n - 2)), sum = 0.0;
+#pragma unroll 1
+    for (int j = 2; j <= n; j++) {
+        sum += t;
+        t *= (double) (n - j) / (double) (j + 1) * (p / (1.0 - p));
+    }
+    return sum;
 }
 
 // kRaim: the RAIM stage of gpsb200_pvt_raim after the solve (DESIGN §11.1). Each lane keeps two flags: `has` (a
@@ -475,6 +603,270 @@ __global__ void __launch_bounds__(kWarps * 32, kRaim ? 4 : 0) k_pvt(const Kernel
     }
 }
 
+// k_pvt_araim: gpsb200_pvt_araim (DESIGN §11.2). The measurement and the Gauss-Newton pass are k_pvt's, restated here
+// with the weights so that k_pvt's two instantiations keep their instructions; `use` is the set, so a masked or
+// excluded lane's row enters with weight 0. Rows and residuals are scaled by sw = 1 / sigma_int, computed per iteration
+// at the estimate's elevation. Solution separation and the protection levels run where the test of a set is final,
+// inside the pass loop, so that nothing of them stays live across a re-solve. kAraimMinBlocks: DESIGN §11.2.
+constexpr int kAraimMinBlocks = 4;
+__global__ void __launch_bounds__(kWarps * 32, kAraimMinBlocks) k_pvt_araim(const AraimArgs a) {
+    const int lane = threadIdx.x & 31;
+    const int64_t fi = (int64_t) blockIdx.x * kWarps + (threadIdx.x >> 5);
+    if (fi >= a.cfg.nfix) return;   // the whole warp leaves together
+    const int64_t s = a.cfg.s0 + fi * a.cfg.step;
+    const double nan = __longlong_as_double(0x7ff8000000000000ll);
+
+    // ---- the measurement of this lane's channel (integers), its satellite (FP64), its URA sigmas ----
+    bool use = false;
+    double rho = 0.0, rate = 0.0, dtsv = 0.0, ddtsv = 0.0, p[3] = {0, 0, 0}, v[3] = {0, 0, 0};
+    double sura2 = 0.0, sure2 = 0.0;
+    const int64_t ds = s - a.ref_sample;
+    const int64_t q = floor_div(ds, 3000), m = ds - 3000 * q;
+    const int64_t nom_ms = (((a.ref_ms + 75 + q) % kWeekMs) + kWeekMs) % kWeekMs;
+    if (lane < a.nchan && a.ref >= 0) {
+        const gpsb200_pvt_chan_t &c = a.ch[lane];
+        const gpsb200_track_epoch_t *e = a.ep + (size_t) lane * a.max_epochs;
+        const bool ura_ok = c.eph.ura >= 0 && c.eph.ura < 15;   // header step 1: URA index 15 never enters the set
+        const int k = ura_ok && c.eph.valid && c.eph.health == 0 ? find_period(e, a.n[lane], s) : -1;
+        if (k >= 1 && e[k - 1].lock && e[k].lock) {
+            const uint64_t phi = (uint64_t) e[k - 1].code_phase + (uint64_t) (s - e[k].sample) * e[k - 1].code_step;
+            const int64_t T = (((c.anchor_ms + k - c.anchor_epoch) % kWeekMs) + kWeekMs) % kWeekMs;
+            const double frac = (double) phi / kCodeMod;
+            const double tsv = (double) T * 1e-3 + frac * 1e-3;
+            if (fabs(wrap_half_week(tsv - c.eph.toe)) <= 7200.0) {
+                use = true;
+                int64_t D = (a.ref_ms + 75 + q - T) % kWeekMs;
+                D = D >= kWeekMs / 2 ? D - kWeekMs : (D < -kWeekMs / 2 ? D + kWeekMs : D);
+                rho = (double) D * kCms + ((double) m / 3000.0 - frac) * kCms;
+                rate = -kLambda * ((double) e[k - 1].carr_step * kStepHz);
+                const double d0 = wrap_half_week(tsv - c.eph.toc);
+                const double tt = tsv - (c.eph.af0 + d0 * (c.eph.af1 + d0 * c.eph.af2));
+                satellite(c.eph, tt, p, v, dtsv, ddtsv);
+                const double sura = fmax(a.araim.sigma_ura, kUraNom[c.eph.ura]);
+                const double sure = sura * a.araim.sigma_ure / a.araim.sigma_ura;
+                sura2 = sura * sura;
+                sure2 = sure * sure;
+            }
+        }
+    }
+    const bool has = use;
+    unsigned mask = __ballot_sync(kFull, use);
+    int nused = __popc(mask);
+    gpsb200_fix_t f;
+    f.sample = s;
+    f.nused = nused;
+    f.mask = mask;
+    f.iterations = 0;
+    f.status = nused < 4 ? GPSB200_FIX_FEW : GPSB200_FIX_NO_CONVERGENCE;
+    f.x = f.y = f.z = f.clock_m = f.t_rx = f.vx = f.vy = f.vz = f.drift = nan;
+    f.lat_deg = f.lon_deg = f.height = f.pdop = f.rms = nan;
+    double resid = nan;
+    // the record; this lane's 1 / sigma_int, elevation and sigma^2 other than URA / URE of the last iteration
+    int verdict = GPSB200_RAIM_UNAVAILABLE;
+    unsigned excluded = 0, masked = 0;
+    bool mask_done = false;
+    double hpl = nan, vpl = nan, ratio = nan, emt = nan, sacc_v = nan, pnm = nan;
+    double sw = 1.0, el = 0.5 * M_PI, rest2 = 0.0;
+    if (nused >= 4) {
+        double X[4] = {0.0, 0.0, 0.0, 0.0};
+        double h[3] = {0, 0, 0}, r = 0.0, pr_v[3] = {0, 0, 0};
+        double N[10];   // the weighted normal matrix of the last iteration
+        Chol ch;
+        bool ok = false;
+        double dX[4] = {0, 0, 0, 0};
+        int it0 = 0;   // iterations of the earlier passes
+#pragma unroll 1
+        for (;;) {     // Gauss-Newton passes: the first, one after the mask, one after an exclusion
+#pragma unroll 1
+            for (int j = 0; j < GPSB200_PVT_MAX_ITER; j++) {
+                const double rad = sqrt(X[0] * X[0] + X[1] * X[1] + X[2] * X[2]);
+                const bool near = rad >= kIonoMinRadius, iono = a.cfg.iono && near;
+                double lat = 0.0, lon = 0.0, hgt = 0.0, sla = 0.0, cla = 0.0, slo = 0.0, clo = 0.0;
+                if (near) {   // the elevation weighs with or without the Klobuchar term
+                    ecef_llh(X, lat, lon, hgt);
+                    sincos(lat, &sla, &cla);
+                    sincos(lon, &slo, &clo);
+                }
+                h[0] = h[1] = h[2] = 0.0;
+                r = 0.0;
+                if (has) {
+                    const double g0 = p[0] - X[0], g1 = p[1] - X[1], g2 = p[2] - X[2];
+                    const double tau = sqrt(g0 * g0 + g1 * g1 + g2 * g2) / kC;
+                    double sth, cth;
+                    sincos(kOmegaE * tau, &sth, &cth);
+                    const double px = p[0] * cth + p[1] * sth, py = p[1] * cth - p[0] * sth;
+                    pr_v[0] = v[0] * cth + v[1] * sth;
+                    pr_v[1] = v[1] * cth - v[0] * sth;
+                    pr_v[2] = v[2];
+                    const double l0 = px - X[0], l1 = py - X[1], l2 = p[2] - X[2];
+                    const double R = sqrt(l0 * l0 + l1 * l1 + l2 * l2);
+                    double I = 0.0, Fm[2] = {1.0, 0.0};
+                    el = 0.5 * M_PI;
+                    if (near) {
+                        const double nn = -sla * clo * l0 - sla * slo * l1 + cla * l2;
+                        const double ee = -slo * l0 + clo * l1;
+                        const double uu = cla * clo * l0 + cla * slo * l1 + sla * l2;
+                        double az = atan2(ee, nn);
+                        if (az < 0.0) az += 2.0 * kPi;
+                        el = atan2(uu, sqrt(nn * nn + ee * ee));
+                        if (iono) {
+                            const double trx = (double) nom_ms * 1e-3 + (double) m / 3e6 - X[3] / kC;
+                            I = klobuchar(a.cfg, lat, lon, az, el, trx, Fm);
+                        }
+                    }
+                    r = rho - (R + X[3] - kC * dtsv + I);
+                    h[0] = -l0 / R;
+                    h[1] = -l1 / R;
+                    h[2] = -l2 / R;
+                    // header step 2
+                    const double se = sin(el);
+                    const double st = 0.12 * 1.001 / sqrt(0.002001 + se * se);
+                    const double mp = 0.13 + 0.53 * exp(-el / kTenDeg);
+                    const double pm = fabs(Fm[1]) * 180.0;   // semicircles -> deg
+                    const double si = iono ? fmax(I / 5.0, Fm[0] * (pm <= 20.0 ? 9.0 : (pm <= 55.0 ? 4.5 : 6.0))) : 0.0;
+                    rest2 = st * st + (a.araim.sigma_noise * a.araim.sigma_noise + mp * mp) + si * si;
+                    sw = 1.0 / sqrt(sura2 + rest2);
+                }
+                // rows and residuals scaled by 1 / sigma_int; a lane outside the set weighs 0
+                const double w0 = use ? h[0] * sw : 0.0, w1 = use ? h[1] * sw : 0.0, w2 = use ? h[2] * sw : 0.0;
+                const double wc = use ? sw : 0.0, wr = use ? r * sw : 0.0;
+                N[0] = warp_sum(w0 * w0);
+                N[1] = warp_sum(w0 * w1);
+                N[2] = warp_sum(w0 * w2);
+                N[3] = warp_sum(w0 * wc);
+                N[4] = warp_sum(w1 * w1);
+                N[5] = warp_sum(w1 * w2);
+                N[6] = warp_sum(w1 * wc);
+                N[7] = warp_sum(w2 * w2);
+                N[8] = warp_sum(w2 * wc);
+                N[9] = warp_sum(wc * wc);
+                const double b[4] = {warp_sum(w0 * wr), warp_sum(w1 * wr), warp_sum(w2 * wr), warp_sum(wc * wr)};
+                f.iterations = it0 + j + 1;
+                if (!ch.factor(N)) break;
+                ch.solve(b, dX);
+#pragma unroll
+                for (int i = 0; i < 4; i++) X[i] += dX[i];
+                if (sqrt(X[0] * X[0] + X[1] * X[1] + X[2] * X[2]) > kRunaway) break;
+                if (sqrt(dX[0] * dX[0] + dX[1] * dX[1] + dX[2] * dX[2]) < kConverged) {
+                    ok = true;
+                    break;
+                }
+            }
+            // the test of the set just solved; the mask or an exclusion goes round again
+            if (!ok) {
+                if (excluded) verdict = GPSB200_RAIM_ALERT;   // a re-solve after an exclusion that failed
+                break;
+            }
+            if (!mask_done) {                              // header step 4, once, after the first converged solve
+                mask_done = true;
+                const bool low = use && el < a.araim.mask_deg * (M_PI / 180.0);
+                masked = __ballot_sync(kFull, low);
+                if (masked) {
+                    if (low) use = false;
+                    mask = __ballot_sync(kFull, use);
+                    nused = __popc(mask);
+                    f.mask = mask;
+                    f.nused = nused;
+                    it0 = f.iterations;
+                    ok = false;
+                    if (nused < 4) {
+                        f.status = GPSB200_FIX_FEW;
+                        break;
+                    }
+                    continue;
+                }
+            }
+            if (nused < 5) break;                          // UNAVAILABLE
+            Ss o;
+            const double sacc = mhss(a, use, nused, h, sw, r, sure2 + rest2, N, ch, X, o);
+            if (__any_sync(kFull, !o.pd)) break;           // UNAVAILABLE
+            double key = o.ratio;
+            int worst = lane;
+            warp_argmax(key, worst);
+            ratio = key;
+            emt = warp_max(use ? o.T[2] : 0.0);
+            sacc_v = sacc;
+            const bool pass = __all_sync(kFull, o.pass);
+            if (!pass && !excluded && a.araim.max_exclude == 1 && nused >= 6) {   // header step 7
+                excluded = 1u << worst;
+                if (lane == worst) use = false;
+                mask = __ballot_sync(kFull, use);
+                nused = __popc(mask);
+                f.mask = mask;
+                f.nused = nused;
+                it0 = f.iterations;
+                ok = false;
+                continue;
+            }
+            verdict = pass ? (excluded ? GPSB200_RAIM_EXCLUDED : GPSB200_RAIM_PASS) : GPSB200_RAIM_ALERT;
+            // header step 8, over this final set
+            const double ps = a.araim.p_sat, pv = a.araim.p_hmi_vert, ph = a.araim.p_hmi_horz;
+            pnm = p_not_monitored(ps, nused);
+            if (!(pnm < pv + ph)) {
+                verdict = GPSB200_RAIM_UNAVAILABLE;
+                break;
+            }
+            const double sc = 1.0 - pnm / (pv + ph);
+            vpl = protection_level(pv * sc, o.b0[2], o.s0[2], use, o.T[2], o.b[2], o.s[2], ps, nused);
+            const double he = protection_level(ph / 2.0 * sc, o.b0[0], o.s0[0], use, o.T[0], o.b[0], o.s[0], ps, nused);
+            const double hn = protection_level(ph / 2.0 * sc, o.b0[1], o.s0[1], use, o.T[1], o.b[1], o.s[1], ps, nused);
+            hpl = sqrt(he * he + hn * hn);
+            break;
+        }
+        if (ok) {
+            // post-fit residuals of the last iteration; velocity and drift on its weighted rows
+            if (has) resid = r - (h[0] * dX[0] + h[1] * dX[1] + h[2] * dX[2] + dX[3]);
+            const double y = use ? (rate + kC * ddtsv + (h[0] * pr_v[0] + h[1] * pr_v[1] + h[2] * pr_v[2])) * (sw * sw) : 0.0;
+            const double bv[4] = {warp_sum(h[0] * y), warp_sum(h[1] * y), warp_sum(h[2] * y), warp_sum(y)};
+            double V[4];
+            ch.solve(bv, V);
+            const double ss = warp_sum(use ? resid * resid : 0.0);
+            double Q[3];
+#pragma unroll
+            for (int i = 0; i < 3; i++) {
+                double ei[4] = {0, 0, 0, 0}, xi[4];
+                ei[i] = 1.0;
+                ch.solve(ei, xi);
+                Q[i] = xi[i];
+            }
+            f.status = GPSB200_FIX_OK;
+            f.x = X[0];
+            f.y = X[1];
+            f.z = X[2];
+            f.clock_m = X[3];
+            double trx = (double) nom_ms * 1e-3 + ((double) m / 3e6 - X[3] / kC);
+            f.t_rx = trx < 0.0 ? trx + 604800.0 : (trx >= 604800.0 ? trx - 604800.0 : trx);
+            f.vx = V[0];
+            f.vy = V[1];
+            f.vz = V[2];
+            f.drift = V[3];
+            double lat, lon, hgt;
+            ecef_llh(X, lat, lon, hgt);
+            f.lat_deg = lat * (180.0 / M_PI);
+            f.lon_deg = lon * (180.0 / M_PI);
+            f.height = hgt;
+            f.pdop = sqrt(Q[0] + Q[1] + Q[2]);
+            f.rms = sqrt(ss / (double) nused);
+        }
+    }
+    if (lane == 0) {
+        a.fixes[fi] = f;
+        gpsb200_araim_t o;
+        o.verdict = verdict;
+        o.excluded = excluded;
+        o.masked = masked;
+        o.n = nused;
+        o.test_ratio = ratio;
+        o.hpl = hpl;
+        o.vpl = vpl;
+        o.emt = emt;
+        o.sigma_acc_v = sacc_v;
+        o.p_nm = pnm;
+        a.out[fi] = o;
+    }
+    if (a.res && lane < a.nchan) a.res[fi * a.nchan + lane] = has ? resid : nan;
+}
+
 template <bool kRaim> void fill(KernelArgs<kRaim> &a, const Scratch &sc);
 template <> void fill<false>(Args &a, const Scratch &sc) {
     a.ep = sc.d_epochs;
@@ -506,14 +898,40 @@ template <bool kRaim> cudaError_t launch_as(const Scratch &sc, cudaStream_t s) {
 }
 
 cudaError_t launch(const Scratch &sc, cudaStream_t s) {
+    if (sc.araim) {
+        AraimArgs a;
+        fill<false>(a, sc);
+        a.araim = sc.araim_cfg;
+        memcpy(a.kh, sc.kfa_h, sizeof a.kh);
+        memcpy(a.kv, sc.kfa_v, sizeof a.kv);
+        a.out = sc.d_araim;
+        const int64_t blocks = ((int64_t) sc.cfg.nfix + kWarps - 1) / kWarps;
+        k_pvt_araim<<<(unsigned) blocks, kWarps * 32, 0, s>>>(a);
+        return cudaGetLastError();
+    }
     return sc.raim ? launch_as<true>(sc, s) : launch_as<false>(sc, s);
 }
 
 }  // namespace
 
 std::string check(const gpsb200_pvt_chan_t *chans, int nchan, const gpsb200_track_epoch_t *epochs, const int32_t *nepochs,
-                  int max_epochs, const gpsb200_pvt_config_t *cfg, const gpsb200_raim_config_t *raim) {
+                  int max_epochs, const gpsb200_pvt_config_t *cfg, const gpsb200_raim_config_t *raim,
+                  const gpsb200_araim_config_t *araim) {
     if (!chans || !epochs || !nepochs || !cfg) return "NULL chans, epochs, nepochs or cfg";
+    if (araim) {
+        const gpsb200_araim_config_t &r = *araim;
+        const auto in = [](double v, double lo, double hi) { return v >= lo && v <= hi; };   // false for NaN
+        if (!in(r.mask_deg, 0.0, 90.0)) return "araim mask_deg must lie in 0..90";
+        if (!in(r.sigma_ura, 0.0, 100.0) || !(r.sigma_ura > 0.0)) return "araim sigma_ura must lie in (0, 100]";
+        if (!in(r.sigma_ure, 0.0, r.sigma_ura) || !(r.sigma_ure > 0.0)) return "araim sigma_ure must lie in (0, sigma_ura]";
+        if (!in(r.sigma_noise, 0.0, 100.0) || !in(r.b_nom, 0.0, 100.0)) return "araim sigma_noise and b_nom must lie in 0..100";
+        if (!in(r.p_sat, 1e-12, 1e-2)) return "araim p_sat must lie in 1e-12..1e-2";
+        if (!in(r.p_hmi_vert, 1e-12, 0.5) || !in(r.p_hmi_horz, 1e-12, 0.5) || !in(r.p_fa_vert, 1e-12, 0.5) ||
+            !in(r.p_fa_horz, 1e-12, 0.5))
+            return "araim p_hmi_vert, p_hmi_horz, p_fa_vert and p_fa_horz must lie in 1e-12..0.5";
+        if (r.max_exclude != 0 && r.max_exclude != 1) return "araim max_exclude must be 0 or 1";
+        if (r.reserved[0] || r.reserved[1] || r.reserved[2]) return "araim reserved must be 0";
+    }
     if (raim) {
         if (!std::isfinite(raim->sigma) || !(raim->sigma > 0.0)) return "raim sigma must be finite and > 0";
         if (!(raim->p_fa >= 1e-12 && raim->p_fa <= 0.5) || !(raim->p_md >= 1e-12 && raim->p_md <= 0.5))
@@ -539,6 +957,7 @@ std::string check(const gpsb200_pvt_chan_t *chans, int nchan, const gpsb200_trac
         if (!ch.eph.valid) continue;   // never used: its anchor is not read
         if (ch.anchor_epoch < 0 || ch.anchor_epoch >= nepochs[c]) return at + "anchor_epoch outside the channel's epochs";
         if (ch.anchor_ms < 0 || ch.anchor_ms >= kWeekMs) return at + "anchor_ms outside 0..604799999";
+        if (araim && (ch.eph.ura < 0 || ch.eph.ura > 15)) return at + "eph.ura outside 0..15";
     }
     return std::string();
 }
@@ -550,13 +969,14 @@ void scratch_free(Scratch &sc) {
     cudaFree(sc.d_fixes);
     cudaFree(sc.d_res);
     cudaFree(sc.d_raim);
+    cudaFree(sc.d_araim);
     sc = Scratch();
 }
 
 cudaError_t run(Scratch &sc, const gpsb200_pvt_chan_t *chans, int nchan, const gpsb200_track_epoch_t *epochs,
                 const int32_t *nepochs, int max_epochs, const gpsb200_pvt_config_t *cfg,
                 const gpsb200_raim_config_t *raim, gpsb200_fix_t *fixes, double *residuals, gpsb200_raim_t *out,
-                cudaStream_t s) {
+                cudaStream_t s, const gpsb200_araim_config_t *araim, gpsb200_araim_t *aout) {
     sc.have_last = false;
     if (!sc.d_chans) {
         CU_RET(cudaMalloc(&sc.d_chans, GPSB200_TRK_MAX_CHAN * sizeof(gpsb200_pvt_chan_t)));
@@ -574,6 +994,12 @@ cudaError_t run(Scratch &sc, const gpsb200_pvt_chan_t *chans, int nchan, const g
             sc.tab_p_fa = raim->p_fa;
             sc.tab_p_md = raim->p_md;
         }
+    }
+    sc.araim = araim != nullptr;
+    if (araim) {
+        CU_RET(grow(sc.d_araim, sc.araim_cap, (size_t) cfg->nfix));
+        sc.araim_cfg = *araim;
+        araim_kfa(araim->p_fa_vert, araim->p_fa_horz, sc.kfa_h, sc.kfa_v);
     }
     // the reference channel of the nominal receive time: the lowest with a valid, healthy ephemeris
     sc.ref = -1;
@@ -595,6 +1021,9 @@ cudaError_t run(Scratch &sc, const gpsb200_pvt_chan_t *chans, int nchan, const g
         CU_RET(cudaMemcpyAsync(residuals, sc.d_res, (size_t) cfg->nfix * nchan * sizeof(double), cudaMemcpyDeviceToHost, s));
     if (raim)
         CU_RET(cudaMemcpyAsync(out, sc.d_raim, (size_t) cfg->nfix * sizeof(gpsb200_raim_t), cudaMemcpyDeviceToHost, s));
+    if (araim)
+        CU_RET(cudaMemcpyAsync(aout, sc.d_araim, (size_t) cfg->nfix * sizeof(gpsb200_araim_t), cudaMemcpyDeviceToHost,
+                               s));
     CU_RET(cudaStreamSynchronize(s));
     sc.have_last = true;
     return cudaSuccess;

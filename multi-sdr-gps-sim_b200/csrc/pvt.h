@@ -15,13 +15,18 @@ constexpr int64_t kWeekMs = 604800000;   // ms of a GPS week
 
 static_assert(sizeof(gpsb200_raim_config_t) == 32, "gpsb200_raim_config_t layout");
 static_assert(sizeof(gpsb200_raim_t) == 48, "gpsb200_raim_t layout");
+static_assert(sizeof(gpsb200_araim_config_t) == 96, "gpsb200_araim_config_t layout");
+static_assert(sizeof(gpsb200_araim_t) == 64, "gpsb200_araim_t layout");
 
-// Empty when the call is well-formed (see the header). raim may be NULL (gpsb200_pvt).
+// Empty when the call is well-formed (see the header). raim and araim may be NULL; at most one is not.
 std::string check(const gpsb200_pvt_chan_t *chans, int nchan, const gpsb200_track_epoch_t *epochs, const int32_t *nepochs,
-                  int max_epochs, const gpsb200_pvt_config_t *cfg, const gpsb200_raim_config_t *raim);
+                  int max_epochs, const gpsb200_pvt_config_t *cfg, const gpsb200_raim_config_t *raim,
+                  const gpsb200_araim_config_t *araim);
 
 // The RAIM tables of gpsb200_raim_thresholds (raim_thresholds.cpp); false when p_fa or p_md is outside 1e-12..0.5.
 bool raim_thresholds(double p_fa, double p_md, double *T, double *lambda);
+// The ARAIM test multipliers of gpsb200_araim_kfa (raim_thresholds.cpp); false when a probability is outside 1e-12..0.5.
+bool araim_kfa(double p_fa_vert, double p_fa_horz, double *kh, double *kv);
 
 // Device scratch of the fix calls of one context, grown as needed, and what gpsb200_pvt_replay re-runs.
 struct Scratch {
@@ -45,15 +50,22 @@ struct Scratch {
     size_t raim_cap = 0;
     double tab_p_fa = 0.0, tab_p_md = 0.0;       // 0: no tables yet
     double tab_T[GPSB200_RAIM_MAX_DOF] = {}, tab_lambda[GPSB200_RAIM_MAX_DOF] = {};
+    // the ARAIM stage of the previous call (gpsb200_pvt_araim)
+    bool araim = false;
+    gpsb200_araim_config_t araim_cfg{};
+    gpsb200_araim_t *d_araim = nullptr;          // [nfix]
+    size_t araim_cap = 0;
+    double kfa_h[GPSB200_RAIM_MAX_DOF] = {}, kfa_v[GPSB200_RAIM_MAX_DOF] = {};
 };
 
 void scratch_free(Scratch &sc);
 // Upload, run k_pvt on s and download the fixes (and residuals when not NULL); waits for the results. With raim
-// (not NULL) the kernel's RAIM instantiation runs and out [nfix] receives its records.
+// (not NULL) the kernel's RAIM instantiation runs and out [nfix] receives its records; with araim (not NULL) the ARAIM
+// instantiation and aout [nfix]. At most one of raim and araim is not NULL.
 cudaError_t run(Scratch &sc, const gpsb200_pvt_chan_t *chans, int nchan, const gpsb200_track_epoch_t *epochs,
                 const int32_t *nepochs, int max_epochs, const gpsb200_pvt_config_t *cfg,
                 const gpsb200_raim_config_t *raim, gpsb200_fix_t *fixes, double *residuals, gpsb200_raim_t *out,
-                cudaStream_t s);
+                cudaStream_t s, const gpsb200_araim_config_t *araim = nullptr, gpsb200_araim_t *aout = nullptr);
 // Enqueue k_pvt again on the previous call's device-resident inputs.
 cudaError_t replay(Scratch &sc, cudaStream_t s);
 

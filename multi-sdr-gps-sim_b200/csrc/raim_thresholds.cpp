@@ -1,4 +1,5 @@
-// The chi^2 tables of the RAIM stage (include/gpsb200.h: gpsb200_raim_thresholds; DESIGN §11.1), on the host.
+// The chi^2 tables of the RAIM stage (include/gpsb200.h: gpsb200_raim_thresholds; DESIGN §11.1) and the test
+// multipliers K_fa of the ARAIM stage (gpsb200_araim_kfa; DESIGN §11.2), on the host.
 //
 // P(a, x), the regularized lower incomplete gamma function, by its power series below x = a + 1 and as 1 - Q(a, x)
 // from the continued fraction of Q above; the chi^2(d) CDF at t is P(d / 2, t / 2). The noncentral chi^2(d, lambda)
@@ -88,7 +89,32 @@ template <typename F> double solve_decreasing(F f, double target) {
     return 0.5 * (lo + hi);
 }
 
+// Q^-1(p) for 0 < p <= 0.5, Q the standard normal upper tail 0.5 erfc(x / sqrt 2): Newton on log Q(x) - log p from
+// sqrt(-2 ln p), above the root (Q(x) <= exp(-x^2 / 2) / 2). log Q is concave and decreasing, so from above the steps
+// approach the root monotonically and never overshoot.
+double q_inv(double p) {
+    const double lp = std::log(p);
+    double x = std::sqrt(-2.0 * lp);
+    for (int i = 0; i < 100; i++) {
+        const double q = 0.5 * std::erfc(x / std::sqrt(2.0));
+        const double phi = std::exp(-0.5 * x * x) / std::sqrt(2.0 * M_PI);
+        const double dx = (std::log(q) - lp) * q / phi;
+        x += dx;
+        if (std::fabs(dx) <= 1e-16 * (1.0 + x)) break;
+    }
+    return x;
+}
+
 }  // namespace
+
+bool araim_kfa(double p_fa_vert, double p_fa_horz, double *kh, double *kv) {
+    if (!(p_fa_vert >= 1e-12 && p_fa_vert <= 0.5) || !(p_fa_horz >= 1e-12 && p_fa_horz <= 0.5)) return false;
+    for (int n = 5; n < 5 + GPSB200_RAIM_MAX_DOF; n++) {
+        kh[n - 5] = q_inv(p_fa_horz / (4.0 * n));
+        kv[n - 5] = q_inv(p_fa_vert / (2.0 * n));
+    }
+    return true;
+}
 
 bool raim_thresholds(double p_fa, double p_md, double *T, double *lambda) {
     if (!(p_fa >= 1e-12 && p_fa <= 0.5) || !(p_md >= 1e-12 && p_md <= 0.5)) return false;

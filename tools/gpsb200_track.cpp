@@ -8,7 +8,9 @@
 // (gpsb200_nav_ephemeris) and time anchor (gpsb200_nav_time_anchor); channels without both are left out. The fixes
 // start 0.5 s after the acquisition window (the loops have pulled in by then) and follow every --fix-every ms; one line
 // per fix with status GPSB200_FIX_OK (DESIGN §11). With --raim the fixes come from gpsb200_pvt_raim and each line gains
-// the RAIM verdict, the PRNs it excluded ("-" for none) and HPL/VPL in metres (DESIGN §11.1).
+// the RAIM verdict, the PRNs it excluded ("-" for none) and HPL/VPL in metres (DESIGN §11.1). With --araim they come
+// from gpsb200_pvt_araim and each line gains the ARAIM verdict, the excluded PRN, the PRNs below the elevation mask
+// ("-" for none), HPL/VPL and the EMT in metres (DESIGN §11.2).
 #include <algorithm>
 #include <cmath>
 #include <cstdio>
@@ -30,7 +32,8 @@ static const long long kFixLead = 1500000;        // samples from the start to t
 static void usage() {
     fprintf(stderr,
             "gpsb200-track FILE [--iq16] [--block B] [--offset-ms N] [--ms K] [--prn LIST] [--threshold R] [--device D]\n"
-            "              [--fix [--fix-every MS] [--iono a0,a1,a2,a3,b0,b1,b2,b3] [--raim SIGMA[,P_FA,P_MD[,MAX_EXCLUDE]]]]\n"
+            "              [--fix [--fix-every MS] [--iono a0,a1,a2,a3,b0,b1,b2,b3] [--raim SIGMA[,P_FA,P_MD[,MAX_EXCLUDE]]]\n"
+            "               [--araim MASK_DEG[,SIGMA_URA,SIGMA_URE,B_NOM,P_SAT]]]\n"
             "  FILE              interleaved I,Q at 3 Msps, int8 (default) or int16 (--iq16)\n"
             "  --block B         start at 0.1 s block B (sample 300000 B); --offset-ms N adds N ms (3000 N samples)\n"
             "  --ms K            track K ms of signal from the start (default: to the end of the file)\n"
@@ -39,7 +42,9 @@ static void usage() {
             "  --fix             position, velocity and time from the decoded ephemeris and TOW, every --fix-every ms\n"
             "                    (default %d) from 0.5 s after the start; --iono: the Klobuchar alpha / beta to apply\n"
             "  --raim            fault detection and exclusion with pseudorange sigma SIGMA m (P_FA 1e-5, P_MD 1e-3,\n"
-            "                    MAX_EXCLUDE 1 by default): adds the verdict, the excluded PRNs and HPL/VPL to each fix\n",
+            "                    MAX_EXCLUDE 1 by default): adds the verdict, the excluded PRNs and HPL/VPL to each fix\n"
+            "  --araim           advanced RAIM with elevation mask MASK_DEG (the other fields: the header's defaults): adds\n"
+            "                    the verdict, the excluded PRN, the masked PRNs, HPL/VPL and the EMT to each fix\n",
             kDefaultThreshold, kDefaultFixEvery);
     exit(2);
 }
@@ -47,10 +52,11 @@ static void usage() {
 static const char *const kVerdict[] = {"PASS", "EXCLUDED", "ALERT", "UNAVAILABLE"};
 
 // Fixes from `first` every `step` samples to the last epoch of the channels, one line per fix with status OK; with
-// raim (not NULL) from gpsb200_pvt_raim, with its three columns.
+// raim (not NULL) from gpsb200_pvt_raim, with its three columns; with araim (not NULL) from gpsb200_pvt_araim, with its five.
 static int print_fixes(gpsb200_ctx_t *ctx, const std::vector<gpsb200_pvt_chan_t> &chans, const std::vector<int> &of,
                        const std::vector<std::vector<gpsb200_track_epoch_t>> &eps, long long first, long long step,
-                       gpsb200_pvt_config_t cfg, const gpsb200_raim_config_t *raim) {
+                       gpsb200_pvt_config_t cfg, const gpsb200_raim_config_t *raim,
+                       const gpsb200_araim_config_t *araim) {
     const int n = (int) chans.size();
     printf("# fixes: %d channel(s) with an ephemeris and a time anchor decoded, Klobuchar %s\n", n, cfg.iono ? "on" : "off");
     if (n == 0) return GPSB200_OK;
@@ -72,12 +78,15 @@ static int print_fixes(gpsb200_ctx_t *ctx, const std::vector<gpsb200_pvt_chan_t>
     cfg.nfix = (int32_t) ((end - first) / step + 1);
     std::vector<gpsb200_fix_t> fx(cfg.nfix);
     std::vector<gpsb200_raim_t> rm(raim ? cfg.nfix : 0);
-    const int rc = raim ? gpsb200_pvt_raim(ctx, chans.data(), n, all.data(), cnt.data(), (int) me, &cfg, raim, fx.data(),
-                                           nullptr, rm.data())
-                        : gpsb200_pvt(ctx, chans.data(), n, all.data(), cnt.data(), (int) me, &cfg, fx.data(), nullptr);
+    std::vector<gpsb200_araim_t> am(araim ? cfg.nfix : 0);
+    const int rc = araim ? gpsb200_pvt_araim(ctx, chans.data(), n, all.data(), cnt.data(), (int) me, &cfg, araim,
+                                             fx.data(), nullptr, am.data())
+                   : raim ? gpsb200_pvt_raim(ctx, chans.data(), n, all.data(), cnt.data(), (int) me, &cfg, raim, fx.data(),
+                                             nullptr, rm.data())
+                          : gpsb200_pvt(ctx, chans.data(), n, all.data(), cnt.data(), (int) me, &cfg, fx.data(), nullptr);
     if (rc != GPSB200_OK) return rc;
     printf("# sample  tow_s  lat_deg  lon_deg  height_m  clock_m  vx  vy  vz (ECEF m/s)  channels  pdop%s\n",
-           raim ? "  raim  excluded_prns  hpl/vpl_m" : "");
+           raim ? "  raim  excluded_prns  hpl/vpl_m" : (araim ? "  araim  excluded_prn  masked_prns  hpl/vpl_m  emt_m" : ""));
     for (int i = 0; i < cfg.nfix; i++) {
         const gpsb200_fix_t &f = fx[i];
         if (f.status != GPSB200_FIX_OK) continue;
@@ -88,6 +97,15 @@ static int print_fixes(gpsb200_ctx_t *ctx, const std::vector<gpsb200_pvt_chan_t>
             for (int k = 0; k < n; k++)
                 if (rm[i].excluded >> k & 1u) ex += (ex.empty() ? "" : ",") + std::to_string(chans[k].prn);
             printf("  %s  %s  %.2f/%.2f", kVerdict[rm[i].verdict], ex.empty() ? "-" : ex.c_str(), rm[i].hpl, rm[i].vpl);
+        }
+        if (araim) {
+            std::string ex, mk;
+            for (int k = 0; k < n; k++) {
+                if (am[i].excluded >> k & 1u) ex += (ex.empty() ? "" : ",") + std::to_string(chans[k].prn);
+                if (am[i].masked >> k & 1u) mk += (mk.empty() ? "" : ",") + std::to_string(chans[k].prn);
+            }
+            printf("  %s  %s  %s  %.2f/%.2f  %.2f", kVerdict[am[i].verdict], ex.empty() ? "-" : ex.c_str(),
+                   mk.empty() ? "-" : mk.c_str(), am[i].hpl, am[i].vpl, am[i].emt);
         }
         printf("\n");
     }
@@ -106,6 +124,9 @@ int main(int argc, char **argv) {
     bool raim = false;
     gpsb200_raim_config_t rcfg;
     memset(&rcfg, 0, sizeof rcfg);
+    bool araim = false;
+    gpsb200_araim_config_t acfg;
+    memset(&acfg, 0, sizeof acfg);
     gpsb200_acq_config_t cfg;
     memset(&cfg, 0, sizeof cfg);
     cfg.ms = kAcqMs;
@@ -138,11 +159,28 @@ int main(int argc, char **argv) {
             const int got = sscanf(val(), "%lf,%lf,%lf,%d", &rcfg.sigma, &rcfg.p_fa, &rcfg.p_md, &rcfg.max_exclude);
             if (got != 1 && got != 3 && got != 4) usage();
             raim = true;
+        } else if (a == "--araim") {
+            acfg.sigma_ura = GPSB200_ARAIM_SIGMA_URA;
+            acfg.sigma_ure = GPSB200_ARAIM_SIGMA_URE;
+            acfg.sigma_noise = GPSB200_ARAIM_SIGMA_NOISE;
+            acfg.b_nom = GPSB200_ARAIM_B_NOM;
+            acfg.p_sat = GPSB200_ARAIM_P_SAT;
+            acfg.p_hmi_vert = GPSB200_ARAIM_P_HMI_VERT;
+            acfg.p_hmi_horz = GPSB200_ARAIM_P_HMI_HORZ;
+            acfg.p_fa_vert = GPSB200_ARAIM_P_FA_VERT;
+            acfg.p_fa_horz = GPSB200_ARAIM_P_FA_HORZ;
+            acfg.max_exclude = 1;
+            const int got = sscanf(val(), "%lf,%lf,%lf,%lf,%lf", &acfg.mask_deg, &acfg.sigma_ura, &acfg.sigma_ure,
+                                   &acfg.b_nom, &acfg.p_sat);
+            if (got != 1 && got != 5) usage();
+            araim = true;
         }
         else if (a[0] != '-' && !path) path = argv[i];
         else usage();
     }
-    if (!path || block < 0 || offset_ms < 0 || ms == 0 || ms < -1 || fix_every < 1 || (raim && !fix)) usage();
+    if (!path || block < 0 || offset_ms < 0 || ms == 0 || ms < -1 || fix_every < 1 || ((raim || araim) && !fix) ||
+        (raim && araim))
+        usage();
     cfg.f_lo_hz = kAcqLo;
     cfg.step_hz = kAcqStep;
     cfg.nbins = (int) std::floor((kAcqHi - kAcqLo) / kAcqStep + 1e-9) + 1;
@@ -237,7 +275,7 @@ int main(int argc, char **argv) {
         }
     }
     if (fix) rc = print_fixes(ctx, fix_chans, fix_of, eps, s0 + kFixLead, fix_every * GPSB200_ACQ_CODE_SAMPLES, pcfg,
-                              raim ? &rcfg : nullptr);
+                              raim ? &rcfg : nullptr, araim ? &acfg : nullptr);
     if (rc != GPSB200_OK) fprintf(stderr, "gpsb200-track: %s\n", gpsb200_last_error(ctx));
     gpsb200_destroy(ctx);
     return rc == GPSB200_OK ? 0 : 1;

@@ -13,9 +13,13 @@ card's name, power limit and maximum SM clock are read in the same run (nvidia-s
 With --raim SIGMA the same run also times the RAIM stage (gpsb200_pvt_raim, DESIGN §11.1) in three arms, alternating
 --rounds times: the kernel without RAIM, with RAIM on the fault-free epochs, and with RAIM on epochs whose channel
 --fault carries a 0.1-chip code-phase bias (about 29 m), so that every fix excludes once. Each arm's kernel time is the
-median of its replays over all rounds; its verdict counts come from the call that set it up.
+median of its replays over all rounds; its verdict counts come from the call that set it up. With --araim MASK_DEG
+two more arms alternate with them: the ARAIM stage (gpsb200_pvt_araim, DESIGN §11.2, the header's default allocations)
+on the fault-free epochs, and with channel --fault's satellite clock (af0) off by twice the smallest bias that the
+channel's own hypothesis detects (from the numpy model at the fix 1 s into the run), so that every fix excludes once.
 
     python tools/pvt_bench.py [--iters 5] [--warmup 1] [--check 64] [--seconds 600] [--raim SIGMA [--fault C]]
+                              [--araim MASK_DEG]
 """
 import argparse
 import importlib
@@ -78,6 +82,20 @@ def replay_ms(ctx, stream, iters):
     return out
 
 
+def araim_bias(chans, packed, n, cfg, acfg, c):
+    """Twice the smallest bias on channel c that its own hypothesis detects at the fix 1 s into the run: the bias moves
+    the all-in-view fix by S0_qc b and the subset without c not at all, so it is detected once |S0_qc| b > T_c,q for some
+    q (tests/araim_model.py)."""
+    import araim_model as AM
+    eps = [packed[k, :n[k]] for k in range(len(n))]
+    one = gps.pvt_config(int(cfg["s0"]) + 1000 * int(cfg["step"]), 1, 1, (cfg["alpha"], cfg["beta"]))
+    kh, kv = gps.araim_kfa(float(acfg["p_fa_vert"]), float(acfg["p_fa_horz"]))
+    _, _, rec, extra = AM.araim(chans, eps, one, acfg, kh, kv)
+    o = extra[0][0]
+    kk = int(np.nonzero(o["idx"] == c)[0][0])
+    return 2.0 * float(np.min(o["T"][kk] / np.abs(o["S0"][:, kk])))
+
+
 def raim_arms(ctx, stream, chans, packed, n, cfg, args):
     """Kernel time of the three arms, alternating, and the verdict counts of each."""
     bad = packed.copy()
@@ -88,6 +106,13 @@ def raim_arms(ctx, stream, chans, packed, n, cfg, args):
     arms = {"plain": lambda: ctx.pvt(chans, packed, cfg, nepochs=n),
             "raim": lambda: ctx.pvt_raim(chans, packed, cfg, rcfg, nepochs=n),
             "raim_fault": lambda: ctx.pvt_raim(chans, bad, cfg, rcfg, nepochs=n)}
+    if args.araim is not None:
+        acfg = gps.araim_config(mask_deg=args.araim)
+        arms["araim"] = lambda: ctx.pvt_araim(chans, packed, cfg, acfg, nepochs=n)
+        bias = araim_bias(chans, packed, n, cfg, acfg, args.fault)
+        achans = chans.copy()
+        achans[args.fault]["eph"]["af0"] += bias / PM.C
+        arms["araim_fault"] = lambda: ctx.pvt_araim(achans, packed, cfg, acfg, nepochs=n)
     times = {k: [] for k in arms}
     verdicts = {}
     for _ in range(args.rounds):
@@ -96,12 +121,12 @@ def raim_arms(ctx, stream, chans, packed, n, cfg, args):
             if k != "plain":
                 v, c = np.unique(got[1]["verdict"], return_counts=True)
                 verdicts[k] = {int(a): int(b) for a, b in zip(v, c)}
-                if k == "raim_fault":
+                if k.endswith("_fault"):
                     tested = got[1]["verdict"] != gps.RAIM_UNAVAILABLE
-                    verdicts["raim_fault_excluded_only_channel"] = bool(np.all(got[1]["excluded"][tested] ==
+                    verdicts[k + "_excluded_only_channel"] = bool(np.all(got[1]["excluded"][tested] ==
                                                                                1 << args.fault))
             times[k] += replay_ms(ctx, stream, args.iters)
-    out = {"sigma": args.raim, "fault_channel": args.fault, "rounds": args.rounds, "verdicts": verdicts}
+    out = {"sigma": args.raim, "araim_mask_deg": args.araim, "araim_fault_bias_m": round(bias, 3) if args.araim is not None else None, "fault_channel": args.fault, "rounds": args.rounds, "verdicts": verdicts}
     for k, t in times.items():
         out[k + "_kernel_ms_median"] = round(float(np.median(t)), 3)
         out[k + "_kernel_ms_min"] = round(float(np.min(t)), 3)
@@ -117,6 +142,7 @@ def main():
     ap.add_argument("--raim", type=float, default=None)
     ap.add_argument("--fault", type=int, default=0)
     ap.add_argument("--rounds", type=int, default=3)
+    ap.add_argument("--araim", type=float, default=None)
     args = ap.parse_args()
     import torch
     if not torch.cuda.is_available():
