@@ -738,6 +738,76 @@ int gpsb200_pvt_araim(gpsb200_ctx_t *ctx, const gpsb200_pvt_chan_t *chans, int n
                       const gpsb200_araim_config_t *araim, gpsb200_fix_t *fixes, double *residuals,
                       gpsb200_araim_t *out);
 
+/* ---- coarse-time fixes: position without the time anchor (DESIGN §11.3; tests/coarse_model.py states it in numpy) --
+ * Assistance: the ephemeris (as for gpsb200_pvt), an a-priori position x_a and an a-priori GPS time t_a (s of week,
+ * week `week`) at stream sample s_a. The tracked code phase gives each channel's transmit time modulo 1 ms; the whole
+ * ms come from a prediction at x_a, and the a-priori time error delta becomes a fifth unknown. Per fix instant s
+ * (s0 + i step, as gpsb200_pvt):
+ *   1. A-priori time. ds = s - s_a = 3000 q + m (0 <= m < 3000); u = t_a + ds / 3e6 (float64), kw = floor(u / 604800),
+ *      t_a(s) = u - 604800 kw. W = floor(t_a), F = t_a - W (exact).
+ *   2. Measurement: gpsb200_pvt's period k, phi and carrier step; frac = phi / (1023 2^32) ms. anchor_epoch / anchor_ms
+ *      are neither read nor checked. Used: epochs[k-1].lock and epochs[k].lock, eph.valid, eph.health == 0 and
+ *      |t_a(s) - toe| <= 7200 s (week-wrapped, as gpsb200_pvt wraps t_sv - toe).
+ *   3. Prediction of a used channel's transmit time at a position x and receive time t (here x_a and t_a(s)): tau_0 =
+ *      0.075 s; three fixed-point steps i = 0, 1, 2: p, dt_sv = gpsb200_pvt's satellite position and clock at GPS time
+ *      t - tau_i, p rotated about z by -OMEGA_E tau_i, tau_{i+1} = |p_rot - x| / c. pred = 1000 (t - tau_3 + dt_sv) ms,
+ *      dt_sv that of step i = 2 (satellite time; TGD and the relativistic term included, no ionosphere).
+ *   4. Reference channel r: the used channel with the largest sin(elevation) of p_rot (step i = 2) seen from x_a
+ *      (up vector at x_a's WGS-84 latitude / longitude, gpsb200_pvt's six-step conversion); the lowest channel on ties.
+ *   5. Whole ms, with round(v) = floor(v + 0.5) (exact halves go up): N_r = round(pred_r - frac_r),
+ *      N_c = N_r + round((pred_c - pred_r) - (frac_c - frac_r)). The resolved ms of week is N_c mod 604800000 and the
+ *      transmit time t_sv,c = (N_c mod 604800000) / 1000 + frac_c / 1000 s.
+ *   6. Pseudorange rho_c = c ((1000 W + q - N_c) ms + (1000 F + m / 3000 - frac_c) ms), the whole-ms difference taken mod
+ *      604800000 and wrapped into half a week (as gpsb200_pvt). It equals c (t_a(s) - t_sv,c).
+ *   7. Gauss-Newton on X = (x, y, z, b, delta) from (x_a, 0, 0), iteration j = 0 .. GPSB200_PVT_MAX_ITER - 1: each used
+ *      channel's satellite at satellite time t_sv,c + delta_j (GPS time by gpsb200_pvt's af0..af2 correction), then
+ *      gpsb200_pvt's flight time, rotation, Klobuchar term (receive time t_a(s) + delta_j - b_j / c) and model
+ *      rho = |p_rot - x_j| + b_j - c dt_sv + I; rows (-(p_rot - x_j) / R, 1, e . v_rot - c drift_sv), e = (p_rot - x_j) / R
+ *      and v_rot the rotated satellite velocity; 5 x 5 normal equations; the convergence (|dx| < 1e-4 m), runaway
+ *      (|x| > 1e8 m) and positive-definiteness rules of gpsb200_pvt. Fewer than 5 used channels: status 1.
+ *   8. Ambiguity check after convergence: steps 3 and 5 again at the fix (x_{j+1}, t_a(s) + delta - b / c) with the
+ *      same reference channel. The status is GPSB200_FIX_AMBIGUOUS (only this call returns it) if any N'_c - N'_r
+ *      differs from N_c - N_r (bit c of `changed`; N_r itself moves with delta by design), or if some used channel's
+ *      post-fit residual (step 9) exceeds GPSB200_COARSE_MAX_RESIDUAL in magnitude. Wrong integers usually fit a wrong
+ *      position well enough that re-resolving at it gives them back; they show instead as residuals of kilometres,
+ *      where right integers leave centimetres (ideal epochs) to tens of metres (tracked). With exactly 5 channels the
+ *      solve fits any integers exactly, so a wrong integer cannot be seen.
+ *   9. Post-fit residuals: rho - model - row . dX of the last iteration. Velocity and clock drift: gpsb200_pvt's least
+ *      squares on the rows' first four columns (at the last x_j).
+ *      t_rx = t_a(s) + delta - b / c, brought into 0..604800 with the week carried into the record's week.
+ * The integers are right when, for every used channel, the prediction error of its transmit time differs from the
+ * reference channel's by less than 0.5 ms (about 150 km). That holds for any geometry when x_a is within 50 km of the
+ * truth and t_a within 10 s: the line-of-sight projections of the position error differ by at most 2 x 50 km, the range
+ * rates by at most about 1.9 km/s (x 10 s = 19 km), well below 150 km.
+ * The fix record: status, mask, nused, iterations as gpsb200_pvt; position, clock, velocity, drift, t_rx, rms and pdop
+ * (the 5-state PDOP: sqrt of the trace of the position block of the 5 x 5 (H^T H)^-1) NaN unless GPSB200_FIX_OK.
+ * residuals (NULL: not wanted) [nfix][nchan]: post-fit residuals of the used channels when OK, NaN otherwise.
+ * ms (NULL: not wanted) [nfix][nchan]: the resolved ms of week of each used channel, -1 for the others. */
+enum { GPSB200_FIX_AMBIGUOUS = 3 };
+#define GPSB200_COARSE_MAX_RESIDUAL 1000.0   /* m */
+typedef struct gpsb200_coarse_config {
+    double x_a[3];         /* a-priori ECEF position, m: finite */
+    double t_a;            /* a-priori GPS time at sample s_a, s of week: 0 <= t_a < 604800 */
+    int64_t s_a;           /* stream sample of t_a: 0..2^62 */
+    int32_t week;          /* GPS week of t_a: >= 0 */
+    int32_t reserved;      /* 0 */
+} gpsb200_coarse_config_t; /* 48 bytes */
+typedef struct gpsb200_coarse {
+    double delta;          /* the solved a-priori time error, s; NaN unless GPSB200_FIX_OK */
+    double pdop;           /* the 5-state PDOP (as the fix record's); NaN unless GPSB200_FIX_OK */
+    int32_t ref;           /* the reference channel r; -1 when no channel is used */
+    int32_t week;          /* GPS week of t_rx; -1 unless GPSB200_FIX_OK */
+    uint32_t changed;      /* bit c: channel c's integer changed in the ambiguity check */
+    int32_t reserved;
+} gpsb200_coarse_t;        /* 32 bytes */
+/* Coarse-time fixes: gpsb200_pvt's arguments (the same checks, except that anchors are neither read nor checked), the
+ * a-priori config (GPSB200_ERR_ARG unless x_a is finite, 0 <= t_a < 604800, 0 <= s_a <= 2^62, week >= 0 and reserved
+ * is 0), out [nfix] records, and ms [nfix][nchan] (NULL: not wanted). gpsb200_pvt_replay re-runs it when it ran last. */
+int gpsb200_pvt_coarse(gpsb200_ctx_t *ctx, const gpsb200_pvt_chan_t *chans, int nchan,
+                       const gpsb200_track_epoch_t *epochs, const int32_t *nepochs, int max_epochs,
+                       const gpsb200_pvt_config_t *cfg, const gpsb200_coarse_config_t *apriori, gpsb200_fix_t *fixes,
+                       double *residuals, gpsb200_coarse_t *out, int64_t *ms);
+
 /* ---- scenario engine: the reference's host path outside the sample loop -------------
  * RINEX-2/3 navigation file (plain or gzip-compressed, read through zlib like the reference, gps.c:1147) +
  * location/motion -> the gpsb200_chan_t records and NAV frames the
@@ -853,6 +923,13 @@ typedef struct gpsb200_almanac_record {
 /* Parse a SEM file into rec[0..31] (indexed by svid - 1); *valid = 1 when at least one record is complete. Returns
  * GPSB200_ERR_ARG when the file cannot be opened. For tests (the parser against the reference's, field by field). */
 int gpsb200_almanac_read(const char *path, gpsb200_almanac_record_t rec[32], int32_t *valid);
+/* Assistance data for gpsb200_pvt_coarse: the ephemeris of a RINEX-2 (rinex3 = 0) or RINEX-3 (rinex3 = 1) navigation
+ * file, read by the scenario engine's readers. eph[prn - 1] is the PRN's record whose toe (week and second) is nearest
+ * to GPS time (week, sow), the first such record on ties, among those within 7200 s; valid = 0 where there is none. The
+ * fields are the file's values as read (not quantised as the broadcast message would carry them); week is the toe week
+ * modulo 1024, health the SV health as the engine reads it, ura 0 (the readers keep no URA). GPSB200_ERR_ARG when the
+ * file cannot be read, or for a NULL argument, week < 0 or sow outside 0..604800. */
+int gpsb200_rinex_ephemeris(const char *path, int rinex3, int32_t week, double sow, gpsb200_ephemeris_t eph[32]);
 
 /* ---- FIFO / sink boundary: the reference's own API (fifo.h:19-62) --------------
  * Guarded by the reference header's own include guard (fifo.h:13-14), so that a translation unit of the reference

@@ -17,6 +17,7 @@ from .api import (  # noqa: F401
     FIX_NO_CONVERGENCE, PVT_MAX_ITER, nav_words_of_frame, nav_ephemeris, nav_time_anchor, pvt_config,
     RAIM_CONFIG_DTYPE, RAIM_DTYPE, RAIM_PASS, RAIM_EXCLUDED, RAIM_ALERT, RAIM_UNAVAILABLE, RAIM_MAX_DOF,
     RAIM_MAX_EXCLUDE, raim_config, raim_thresholds, ARAIM_CONFIG_DTYPE, ARAIM_DTYPE, araim_config, araim_kfa,
+    COARSE_CONFIG_DTYPE, COARSE_DTYPE, FIX_AMBIGUOUS, coarse_config, rinex_ephemeris,
 )
 from .synthetic import synthetic_chans  # noqa: F401,E402
 from . import sharding  # noqa: F401,E402

@@ -247,6 +247,32 @@ def araim_kfa(p_fa_vert, p_fa_horz):
     return kh, kv
 
 
+# gpsb200_coarse_config_t / gpsb200_coarse_t (DESIGN §11.3)
+COARSE_CONFIG_DTYPE = np.dtype([("x_a", "<f8", 3), ("t_a", "<f8"), ("s_a", "<i8"), ("week", "<i4"), ("reserved", "<i4")])
+COARSE_DTYPE = np.dtype([("delta", "<f8"), ("pdop", "<f8"), ("ref", "<i4"), ("week", "<i4"), ("changed", "<u4"),
+                         ("reserved", "<i4")])
+assert (COARSE_CONFIG_DTYPE.itemsize, COARSE_DTYPE.itemsize) == (48, 32)
+FIX_AMBIGUOUS = 3
+
+
+def coarse_config(x_a, t_a, s_a=0, week=0):
+    """A COARSE_CONFIG_DTYPE record: a-priori ECEF position x_a (m) and GPS time t_a (s of week `week`) at stream sample
+    s_a."""
+    c = np.zeros(1, COARSE_CONFIG_DTYPE)[0]
+    c["x_a"], c["t_a"], c["s_a"], c["week"] = np.asarray(x_a, np.float64), float(t_a), int(s_a), int(week)
+    return c
+
+
+def rinex_ephemeris(path, week, sow, rinex3=False):
+    """gpsb200_rinex_ephemeris: EPHEMERIS_DTYPE[32], entry prn - 1 the PRN's record of the RINEX navigation file whose
+    toe is nearest to GPS time (week, sow), within 2 h (valid 0 where there is none)."""
+    eph = np.zeros(32, EPHEMERIS_DTYPE)
+    rc = lib().gpsb200_rinex_ephemeris(os.fsencode(str(path)), int(bool(rinex3)), int(week), float(sow), eph.ctypes.data)
+    if rc:
+        raise GpsB200Error(rc, "gpsb200_rinex_ephemeris")
+    return eph
+
+
 def raim_thresholds(p_fa, p_md):
     """gpsb200_raim_thresholds: (T[28], lambda[28]) for dof 1..28; T[d - 1] is the chi^2(d) value with upper tail p_fa,
     lambda[d - 1] the noncentrality whose noncentral chi^2(d) CDF at T[d - 1] is p_md."""
@@ -317,7 +343,7 @@ EXPORTS = ["gpsb200_create", "gpsb200_destroy", "gpsb200_last_error", "gpsb200_v
            "gpsb200_codegen", "gpsb200_acquire", "gpsb200_acquire_device", "gpsb200_track_start", "gpsb200_track",
            "gpsb200_track_device", "gpsb200_nav_decode", "gpsb200_nav_word_check", "gpsb200_nav_parity",
            "gpsb200_nav_ephemeris", "gpsb200_nav_time_anchor", "gpsb200_pvt", "gpsb200_pvt_replay",
-           "gpsb200_pvt_raim", "gpsb200_raim_thresholds", "gpsb200_pvt_araim", "gpsb200_araim_kfa", "gpsb200_bind_numa", "gpsb200_span_chain_host", "gpsb200_lanes_model_block",
+           "gpsb200_pvt_raim", "gpsb200_raim_thresholds", "gpsb200_pvt_araim", "gpsb200_araim_kfa", "gpsb200_pvt_coarse", "gpsb200_rinex_ephemeris", "gpsb200_bind_numa", "gpsb200_span_chain_host", "gpsb200_lanes_model_block",
            "gpsb200_lanes_window_band_host", "gpsb200_slice_prepare", "gpsb200_slice_probe",
            "gpsb200_slice_finish", "gpsb200_slice_finish_cb", "gpsb200_slice_wait", "gpsb200_link_apply", "gpsb200_slice_link_host", "gpsb200_debug_corrupt_chain", "gpsb200_synth_kernel_name",
            "gpsb200_debug_run_checkpoints", "gpsb200_checkpoint_segments_host",
@@ -427,6 +453,8 @@ def lib():
         L.gpsb200_raim_thresholds.argtypes = [C.c_double, C.c_double, C.c_void_p, C.c_void_p]
         L.gpsb200_pvt_araim.argtypes = L.gpsb200_pvt_raim.argtypes
         L.gpsb200_araim_kfa.argtypes = [C.c_double, C.c_double, C.c_void_p, C.c_void_p]
+        L.gpsb200_pvt_coarse.argtypes = L.gpsb200_pvt_raim.argtypes + [C.c_void_p]
+        L.gpsb200_rinex_ephemeris.argtypes = [C.c_char_p, C.c_int, C.c_int32, C.c_double, C.c_void_p]
         _lib = L
     return _lib
 
@@ -996,6 +1024,21 @@ class Context:
                                             cf.ctypes.data, ac.ctypes.data, fixes.ctypes.data,
                                             None if res is None else res.ctypes.data, out.ctypes.data))
         return (fixes, out, res) if want_residuals else (fixes, out)
+
+    def pvt_coarse(self, chans, epochs, cfg, apriori, want_residuals=False, want_ms=False, nepochs=None):
+        """Coarse-time fixes without time anchors (gpsb200_pvt_coarse; DESIGN §11.3). The arguments of pvt (anchors
+        unread), plus apriori: COARSE_CONFIG_DTYPE record (coarse_config).
+        -> (fixes FIX_DTYPE[nfix], COARSE_DTYPE[nfix]), then the residuals float64[nfix, nchan] with want_residuals and
+        the resolved ms of week int64[nfix, nchan] (-1 where not used) with want_ms."""
+        ch, nchan, ep, n, me, cf, fixes, res = self._pvt_args(chans, epochs, cfg, want_residuals, nepochs)
+        ap = np.array(apriori, dtype=COARSE_CONFIG_DTYPE).reshape(1)
+        out = np.zeros(fixes.size, COARSE_DTYPE)
+        ms = np.zeros((fixes.size, max(1, nchan)), np.int64) if want_ms else None
+        self._check(lib().gpsb200_pvt_coarse(self._h, ch.ctypes.data, nchan, ep.ctypes.data, n.ctypes.data, me,
+                                             cf.ctypes.data, ap.ctypes.data, fixes.ctypes.data,
+                                             None if res is None else res.ctypes.data, out.ctypes.data,
+                                             None if ms is None else ms.ctypes.data))
+        return (fixes, out) + ((res,) if want_residuals else ()) + ((ms,) if want_ms else ())
 
     @staticmethod
     def _pvt_args(chans, epochs, cfg, want_residuals, nepochs):

@@ -1139,19 +1139,21 @@ int track(gpsb200_ctx *ctx, const void *iq, int64_t nsamples, int sample_size, i
     return GPSB200_OK;
 }
 
-// Position fixes (pvt.cu), with the RAIM stage when raim is not NULL, the ARAIM stage when araim is not NULL. Everything is checked before anything is enqueued.
+// Position fixes (pvt.cu), with the RAIM stage when raim is not NULL, the ARAIM stage when araim is not NULL, coarse-time
+// fixes when coarse is not NULL. Everything is checked before anything is enqueued.
 int pvt_fix(gpsb200_ctx *ctx, const char *fn, const gpsb200_pvt_chan_t *chans, int nchan,
             const gpsb200_track_epoch_t *epochs, const int32_t *nepochs, int max_epochs, const gpsb200_pvt_config_t *cfg,
             const gpsb200_raim_config_t *raim, gpsb200_fix_t *fixes, double *residuals, gpsb200_raim_t *out,
-            const gpsb200_araim_config_t *araim = nullptr, gpsb200_araim_t *aout = nullptr) {
+            const gpsb200_araim_config_t *araim = nullptr, gpsb200_araim_t *aout = nullptr,
+            const gpsb200_coarse_config_t *coarse = nullptr, gpsb200_coarse_t *cout = nullptr, int64_t *ms = nullptr) {
     const std::string at = std::string(fn) + ": ";
     if (!fixes) return fail(ctx, GPSB200_ERR_ARG, at + "NULL fixes");
-    const std::string bad = pvt::check(chans, nchan, epochs, nepochs, max_epochs, cfg, raim, araim);
+    const std::string bad = pvt::check(chans, nchan, epochs, nepochs, max_epochs, cfg, raim, araim, coarse);
     if (!bad.empty()) return fail(ctx, GPSB200_ERR_ARG, at + bad);
     const int rc = check_entry(ctx);
     if (rc) return rc;
     CU(pvt::run(ctx->pvt, chans, nchan, epochs, nepochs, max_epochs, cfg, raim, fixes, residuals, out, ctx->s_compute,
-                araim, aout));
+                araim, aout, coarse, cout, ms));
     return GPSB200_OK;
 }
 
@@ -1752,6 +1754,17 @@ int gpsb200_pvt_araim(gpsb200_ctx_t *ctx, const gpsb200_pvt_chan_t *chans, int n
     if (!araim || !out) return settle(ctx, nullptr, fail(ctx, GPSB200_ERR_ARG, "gpsb200_pvt_araim: NULL araim or out"));
     return settle(ctx, nullptr, pvt_fix(ctx, "gpsb200_pvt_araim", chans, nchan, epochs, nepochs, max_epochs, cfg, nullptr,
                                         fixes, residuals, nullptr, araim, out));
+}
+
+int gpsb200_pvt_coarse(gpsb200_ctx_t *ctx, const gpsb200_pvt_chan_t *chans, int nchan,
+                       const gpsb200_track_epoch_t *epochs, const int32_t *nepochs, int max_epochs,
+                       const gpsb200_pvt_config_t *cfg, const gpsb200_coarse_config_t *apriori, gpsb200_fix_t *fixes,
+                       double *residuals, gpsb200_coarse_t *out, int64_t *ms) {
+    if (!ctx) return GPSB200_ERR_ARG;
+    if (!apriori || !out)
+        return settle(ctx, nullptr, fail(ctx, GPSB200_ERR_ARG, "gpsb200_pvt_coarse: NULL apriori or out"));
+    return settle(ctx, nullptr, pvt_fix(ctx, "gpsb200_pvt_coarse", chans, nchan, epochs, nepochs, max_epochs, cfg, nullptr,
+                                        fixes, residuals, nullptr, nullptr, nullptr, apriori, out, ms));
 }
 
 int gpsb200_araim_kfa(double p_fa_vert, double p_fa_horz, double *kfa_h, double *kfa_v) {

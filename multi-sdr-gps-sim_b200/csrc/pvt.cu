@@ -867,6 +867,300 @@ __global__ void __launch_bounds__(kWarps * 32, kAraimMinBlocks) k_pvt_araim(cons
     if (a.res && lane < a.nchan) a.res[fi * a.nchan + lane] = has ? resid : nan;
 }
 
+// ---- coarse-time fixes (DESIGN §11.3) -------------------------------------------------------------------------------
+struct CoarseArgs : Args {
+    gpsb200_coarse_config_t ap;
+    gpsb200_coarse_t *out;
+    int64_t *ms;
+};
+
+// Cholesky solve of the symmetric 5 x 5 system, N packed as its upper triangle row by row (15 values). solve<n> uses
+// the leading n x n block, whose factor is the leading block of the whole factor.
+struct Chol5 {
+    double l[5][5];
+    __device__ bool factor(const double *N) {
+        double a[5][5];
+        int t = 0;
+#pragma unroll
+        for (int i = 0; i < 5; i++)
+#pragma unroll
+            for (int j = i; j < 5; j++) a[i][j] = a[j][i] = N[t++];
+#pragma unroll
+        for (int j = 0; j < 5; j++) {
+            double d = a[j][j];
+#pragma unroll
+            for (int k = 0; k < j; k++) d -= l[j][k] * l[j][k];
+            if (!(d > 0.0)) return false;
+            l[j][j] = sqrt(d);
+#pragma unroll
+            for (int i = j + 1; i < 5; i++) {
+                double v = a[i][j];
+#pragma unroll
+                for (int k = 0; k < j; k++) v -= l[i][k] * l[j][k];
+                l[i][j] = v / l[j][j];
+            }
+        }
+        return true;
+    }
+    template <int n> __device__ void solve(const double *b, double *x) const {
+        double y[n];
+#pragma unroll
+        for (int i = 0; i < n; i++) {
+            double v = b[i];
+#pragma unroll
+            for (int k = 0; k < i; k++) v -= l[i][k] * y[k];
+            y[i] = v / l[i][i];
+        }
+#pragma unroll
+        for (int i = n - 1; i >= 0; i--) {
+            double v = y[i];
+#pragma unroll
+            for (int k = i + 1; k < n; k++) v -= l[k][i] * x[k];
+            x[i] = v / l[i][i];
+        }
+    }
+};
+
+// Header step 3: the predicted transmit time (ms, satellite time) of a satellite at position x and receive time t, and
+// sin(elevation) seen along the up vector `up` (unit, ECEF).
+__device__ double predict(const gpsb200_ephemeris_t &e, const double *x, double t, const double *up, double &sel) {
+    double tau = 0.075, p[3], v[3], dt = 0.0, ddt;
+    double l0 = 0.0, l1 = 0.0, l2 = 0.0;
+#pragma unroll 1
+    for (int i = 0; i < 3; i++) {
+        satellite(e, t - tau, p, v, dt, ddt);
+        double sth, cth;
+        sincos(kOmegaE * tau, &sth, &cth);
+        l0 = p[0] * cth + p[1] * sth - x[0];
+        l1 = p[1] * cth - p[0] * sth - x[1];
+        l2 = p[2] - x[2];
+        tau = sqrt(l0 * l0 + l1 * l1 + l2 * l2) / kC;
+    }
+    sel = (up[0] * l0 + up[1] * l1 + up[2] * l2) / (tau * kC);
+    return 1000.0 * (t - tau + dt);
+}
+
+__device__ inline double round_half_up(double v) { return floor(v + 0.5); }
+
+// k_pvt_coarse: gpsb200_pvt_coarse (DESIGN §11.3). One warp per fix, lane = channel, as k_pvt; a kernel of its own so
+// that k_pvt's and k_pvt_araim's instructions stay as they are. The satellite is evaluated in every iteration, at the
+// transmit time moved by the current delta. kCoarseMinBlocks: held to 128 registers (some spills) it ran 10 % faster
+// than at its natural 168 with 3 CTAs per SM (DESIGN §11.3).
+constexpr int kCoarseMinBlocks = 4;
+__global__ void __launch_bounds__(kWarps * 32, kCoarseMinBlocks) k_pvt_coarse(const CoarseArgs a) {
+    const int lane = threadIdx.x & 31;
+    const int64_t fi = (int64_t) blockIdx.x * kWarps + (threadIdx.x >> 5);
+    if (fi >= a.cfg.nfix) return;   // the whole warp leaves together
+    const int64_t s = a.cfg.s0 + fi * a.cfg.step;
+    const double nan = __longlong_as_double(0x7ff8000000000000ll);
+
+    // header step 1
+    const int64_t ds = s - a.ap.s_a;
+    const int64_t q = floor_div(ds, 3000), m = ds - 3000 * q;
+    const double u = a.ap.t_a + (double) ds / 3e6;
+    const double kw = floor(u / 604800.0);
+    const double tas = u - 604800.0 * kw;
+    const double W = floor(a.ap.t_a), F = a.ap.t_a - W;
+    const double sub = F * 1000.0 + (double) m / 3000.0;   // ms
+
+    // header steps 2-4: measurement, prediction at x_a, reference channel
+    bool use = false;
+    double frac = 0.0, pred = 0.0, sel = -2.0;
+    const gpsb200_ephemeris_t *eph = nullptr;
+    double up[3];
+    {
+        double lat, lon, hgt, sla, cla, slo, clo;
+        ecef_llh(a.ap.x_a, lat, lon, hgt);
+        sincos(lat, &sla, &cla);
+        sincos(lon, &slo, &clo);
+        up[0] = cla * clo;
+        up[1] = cla * slo;
+        up[2] = sla;
+    }
+    double rate = 0.0;
+    if (lane < a.nchan) {
+        const gpsb200_pvt_chan_t &c = a.ch[lane];
+        const gpsb200_track_epoch_t *e = a.ep + (size_t) lane * a.max_epochs;
+        const int k = c.eph.valid && c.eph.health == 0 ? find_period(e, a.n[lane], s) : -1;
+        if (k >= 1 && e[k - 1].lock && e[k].lock && fabs(wrap_half_week(tas - c.eph.toe)) <= 7200.0) {
+            use = true;
+            eph = &c.eph;
+            const uint64_t phi = (uint64_t) e[k - 1].code_phase + (uint64_t) (s - e[k].sample) * e[k - 1].code_step;
+            frac = (double) phi / kCodeMod;
+            rate = -kLambda * ((double) e[k - 1].carr_step * kStepHz);
+            pred = predict(*eph, a.ap.x_a, tas, up, sel);
+        }
+    }
+    const bool has = use;
+    const unsigned mask = __ballot_sync(kFull, use);
+    const int nused = __popc(mask);
+    double key = use ? sel : -2.0;
+    int r = lane;
+    warp_argmax(key, r);
+    const int ref = nused ? r : -1;
+    const double pred_r = __shfl_sync(kFull, pred, r), frac_r = __shfl_sync(kFull, frac, r);
+    // header step 5
+    const int64_t Nr = (int64_t) round_half_up(pred_r - frac_r);
+    const int64_t dN = (int64_t) round_half_up((pred - pred_r) - (frac - frac_r));
+    const int64_t Nw = (((Nr + dN) % kWeekMs) + kWeekMs) % kWeekMs;
+    // header step 6
+    double rho = 0.0, tsv = 0.0;
+    if (has) {
+        int64_t D = ((int64_t) W * 1000 + q - Nw) % kWeekMs;
+        D = D >= kWeekMs / 2 ? D - kWeekMs : (D < -kWeekMs / 2 ? D + kWeekMs : D);
+        rho = (double) D * kCms + (sub - frac) * kCms;
+        tsv = (double) Nw * 1e-3 + frac * 1e-3;
+    }
+
+    gpsb200_fix_t f;
+    f.sample = s;
+    f.nused = nused;
+    f.mask = mask;
+    f.iterations = 0;
+    f.status = nused < 5 ? GPSB200_FIX_FEW : GPSB200_FIX_NO_CONVERGENCE;
+    f.x = f.y = f.z = f.clock_m = f.t_rx = f.vx = f.vy = f.vz = f.drift = nan;
+    f.lat_deg = f.lon_deg = f.height = f.pdop = f.rms = nan;
+    gpsb200_coarse_t o;
+    o.delta = o.pdop = nan;
+    o.ref = ref;
+    o.week = -1;
+    o.changed = 0;
+    o.reserved = 0;
+    double resid = nan;
+    if (nused >= 5) {
+        double X[5] = {a.ap.x_a[0], a.ap.x_a[1], a.ap.x_a[2], 0.0, 0.0};
+        double h[4] = {0, 0, 0, 0}, rr = 0.0, pr_v[3] = {0, 0, 0}, ddtsv = 0.0;
+        Chol5 ch;
+        bool ok = false;
+        double dX[5] = {0, 0, 0, 0, 0};
+#pragma unroll 1
+        for (int j = 0; j < GPSB200_PVT_MAX_ITER; j++) {
+            const double rad = sqrt(X[0] * X[0] + X[1] * X[1] + X[2] * X[2]);
+            const bool iono = a.cfg.iono && rad >= kIonoMinRadius;
+            double lat = 0.0, lon = 0.0, hgt = 0.0, sla = 0.0, cla = 0.0, slo = 0.0, clo = 0.0;
+            if (iono) {
+                ecef_llh(X, lat, lon, hgt);
+                sincos(lat, &sla, &cla);
+                sincos(lon, &slo, &clo);
+            }
+            h[0] = h[1] = h[2] = h[3] = 0.0;
+            rr = 0.0;
+            if (has) {
+                const gpsb200_ephemeris_t &e = *eph;
+                const double t = tsv + X[4];
+                const double d0 = wrap_half_week(t - e.toc);
+                const double tt = t - (e.af0 + d0 * (e.af1 + d0 * e.af2));
+                double p[3], v[3], dtsv;
+                satellite(e, tt, p, v, dtsv, ddtsv);
+                const double g0 = p[0] - X[0], g1 = p[1] - X[1], g2 = p[2] - X[2];
+                const double tau = sqrt(g0 * g0 + g1 * g1 + g2 * g2) / kC;
+                double sth, cth;
+                sincos(kOmegaE * tau, &sth, &cth);
+                const double px = p[0] * cth + p[1] * sth, py = p[1] * cth - p[0] * sth;
+                pr_v[0] = v[0] * cth + v[1] * sth;
+                pr_v[1] = v[1] * cth - v[0] * sth;
+                pr_v[2] = v[2];
+                const double l0 = px - X[0], l1 = py - X[1], l2 = p[2] - X[2];
+                const double R = sqrt(l0 * l0 + l1 * l1 + l2 * l2);
+                double I = 0.0;
+                if (iono) {
+                    const double nn = -sla * clo * l0 - sla * slo * l1 + cla * l2;
+                    const double ee = -slo * l0 + clo * l1;
+                    const double uu = cla * clo * l0 + cla * slo * l1 + sla * l2;
+                    double az = atan2(ee, nn);
+                    if (az < 0.0) az += 2.0 * kPi;
+                    const double el = atan2(uu, sqrt(nn * nn + ee * ee));
+                    I = klobuchar(a.cfg, lat, lon, az, el, tas + X[4] - X[3] / kC);
+                }
+                rr = rho - (R + X[3] - kC * dtsv + I);
+                h[0] = -l0 / R;
+                h[1] = -l1 / R;
+                h[2] = -l2 / R;
+                h[3] = (l0 * pr_v[0] + l1 * pr_v[1] + l2 * pr_v[2]) / R - kC * ddtsv;
+            }
+            const double N[15] = {warp_sum(h[0] * h[0]), warp_sum(h[0] * h[1]), warp_sum(h[0] * h[2]), warp_sum(h[0]),
+                                  warp_sum(h[0] * h[3]), warp_sum(h[1] * h[1]), warp_sum(h[1] * h[2]), warp_sum(h[1]),
+                                  warp_sum(h[1] * h[3]), warp_sum(h[2] * h[2]), warp_sum(h[2]), warp_sum(h[2] * h[3]),
+                                  (double) nused, warp_sum(h[3]), warp_sum(h[3] * h[3])};
+            const double b[5] = {warp_sum(h[0] * rr), warp_sum(h[1] * rr), warp_sum(h[2] * rr), warp_sum(rr),
+                                 warp_sum(h[3] * rr)};
+            f.iterations = j + 1;
+            if (!ch.factor(N)) break;
+            ch.solve<5>(b, dX);
+#pragma unroll
+            for (int i = 0; i < 5; i++) X[i] += dX[i];
+            if (sqrt(X[0] * X[0] + X[1] * X[1] + X[2] * X[2]) > kRunaway) break;
+            if (sqrt(dX[0] * dX[0] + dX[1] * dX[1] + dX[2] * dX[2]) < kConverged) {
+                ok = true;
+                break;
+            }
+        }
+        if (ok) {
+            // header step 8, at the fix, with the same reference channel
+            const double trx = tas + X[4] - X[3] / kC;
+            double dummy, pred2 = 0.0;
+            if (has) pred2 = predict(*eph, X, trx, up, dummy);
+            const double pred2_r = __shfl_sync(kFull, pred2, r);
+            const bool moved = has && (int64_t) round_half_up((pred2 - pred2_r) - (frac - frac_r)) != dN;
+            o.changed = __ballot_sync(kFull, moved);
+            if (has) resid = rr - (h[0] * dX[0] + h[1] * dX[1] + h[2] * dX[2] + dX[3] + h[3] * dX[4]);
+            if (o.changed || __any_sync(kFull, has && !(fabs(resid) <= GPSB200_COARSE_MAX_RESIDUAL))) {
+                f.status = GPSB200_FIX_AMBIGUOUS;
+                resid = nan;
+            } else {
+                // velocity and drift on the rows' first four columns, 5-state PDOP
+                const double y = has ? rate + kC * ddtsv + (h[0] * pr_v[0] + h[1] * pr_v[1] + h[2] * pr_v[2]) : 0.0;
+                const double bv[4] = {warp_sum(h[0] * y), warp_sum(h[1] * y), warp_sum(h[2] * y), warp_sum(y)};
+                double V[4];
+                ch.solve<4>(bv, V);
+                const double ss = warp_sum(has ? resid * resid : 0.0);
+                double Q[3];
+#pragma unroll
+                for (int i = 0; i < 3; i++) {
+                    double ei[5] = {0, 0, 0, 0, 0}, xi[5];
+                    ei[i] = 1.0;
+                    ch.solve<5>(ei, xi);
+                    Q[i] = xi[i];
+                }
+                f.status = GPSB200_FIX_OK;
+                f.x = X[0];
+                f.y = X[1];
+                f.z = X[2];
+                f.clock_m = X[3];
+                double t = trx, wk = kw;
+                if (t < 0.0) {
+                    t += 604800.0;
+                    wk -= 1.0;
+                } else if (t >= 604800.0) {
+                    t -= 604800.0;
+                    wk += 1.0;
+                }
+                f.t_rx = t;
+                f.vx = V[0];
+                f.vy = V[1];
+                f.vz = V[2];
+                f.drift = V[3];
+                double lat, lon, hgt;
+                ecef_llh(X, lat, lon, hgt);
+                f.lat_deg = lat * (180.0 / M_PI);
+                f.lon_deg = lon * (180.0 / M_PI);
+                f.height = hgt;
+                f.pdop = sqrt(Q[0] + Q[1] + Q[2]);
+                f.rms = sqrt(ss / (double) nused);
+                o.delta = X[4];
+                o.pdop = f.pdop;
+                o.week = a.ap.week + (int) wk;
+            }
+        }
+    }
+    if (lane == 0) {
+        a.fixes[fi] = f;
+        a.out[fi] = o;
+    }
+    if (a.res && lane < a.nchan) a.res[fi * a.nchan + lane] = has ? resid : nan;
+    if (a.ms && lane < a.nchan) a.ms[fi * a.nchan + lane] = has ? Nw : -1;
+}
+
 template <bool kRaim> void fill(KernelArgs<kRaim> &a, const Scratch &sc);
 template <> void fill<false>(Args &a, const Scratch &sc) {
     a.ep = sc.d_epochs;
@@ -898,6 +1192,16 @@ template <bool kRaim> cudaError_t launch_as(const Scratch &sc, cudaStream_t s) {
 }
 
 cudaError_t launch(const Scratch &sc, cudaStream_t s) {
+    if (sc.coarse) {
+        CoarseArgs a;
+        fill<false>(a, sc);
+        a.ap = sc.coarse_cfg;
+        a.out = sc.d_coarse;
+        a.ms = sc.want_ms ? sc.d_ms : nullptr;
+        const int64_t blocks = ((int64_t) sc.cfg.nfix + kWarps - 1) / kWarps;
+        k_pvt_coarse<<<(unsigned) blocks, kWarps * 32, 0, s>>>(a);
+        return cudaGetLastError();
+    }
     if (sc.araim) {
         AraimArgs a;
         fill<false>(a, sc);
@@ -916,8 +1220,17 @@ cudaError_t launch(const Scratch &sc, cudaStream_t s) {
 
 std::string check(const gpsb200_pvt_chan_t *chans, int nchan, const gpsb200_track_epoch_t *epochs, const int32_t *nepochs,
                   int max_epochs, const gpsb200_pvt_config_t *cfg, const gpsb200_raim_config_t *raim,
-                  const gpsb200_araim_config_t *araim) {
+                  const gpsb200_araim_config_t *araim, const gpsb200_coarse_config_t *coarse) {
     if (!chans || !epochs || !nepochs || !cfg) return "NULL chans, epochs, nepochs or cfg";
+    if (coarse) {
+        const gpsb200_coarse_config_t &c = *coarse;
+        for (int i = 0; i < 3; i++)
+            if (!std::isfinite(c.x_a[i])) return "coarse x_a must be finite";
+        if (!(c.t_a >= 0.0 && c.t_a < 604800.0)) return "coarse t_a must lie in 0 <= t_a < 604800";
+        if (c.s_a < 0 || c.s_a > (1ll << 62)) return "coarse s_a outside 0..2^62";
+        if (c.week < 0) return "coarse week must be >= 0";
+        if (c.reserved != 0) return "coarse reserved must be 0";
+    }
     if (araim) {
         const gpsb200_araim_config_t &r = *araim;
         const auto in = [](double v, double lo, double hi) { return v >= lo && v <= hi; };   // false for NaN
@@ -954,7 +1267,7 @@ std::string check(const gpsb200_pvt_chan_t *chans, int nchan, const gpsb200_trac
         const std::string at = "channel " + std::to_string(c) + ": ";
         if (nepochs[c] < 0 || nepochs[c] > max_epochs) return at + "nepochs outside 0..max_epochs";
         if (ch.eph.valid != 0 && ch.eph.valid != 1) return at + "eph.valid must be 0 or 1";
-        if (!ch.eph.valid) continue;   // never used: its anchor is not read
+        if (!ch.eph.valid || coarse) continue;   // never used, or a coarse-time call: its anchor is not read
         if (ch.anchor_epoch < 0 || ch.anchor_epoch >= nepochs[c]) return at + "anchor_epoch outside the channel's epochs";
         if (ch.anchor_ms < 0 || ch.anchor_ms >= kWeekMs) return at + "anchor_ms outside 0..604799999";
         if (araim && (ch.eph.ura < 0 || ch.eph.ura > 15)) return at + "eph.ura outside 0..15";
@@ -970,13 +1283,16 @@ void scratch_free(Scratch &sc) {
     cudaFree(sc.d_res);
     cudaFree(sc.d_raim);
     cudaFree(sc.d_araim);
+    cudaFree(sc.d_coarse);
+    cudaFree(sc.d_ms);
     sc = Scratch();
 }
 
 cudaError_t run(Scratch &sc, const gpsb200_pvt_chan_t *chans, int nchan, const gpsb200_track_epoch_t *epochs,
                 const int32_t *nepochs, int max_epochs, const gpsb200_pvt_config_t *cfg,
                 const gpsb200_raim_config_t *raim, gpsb200_fix_t *fixes, double *residuals, gpsb200_raim_t *out,
-                cudaStream_t s, const gpsb200_araim_config_t *araim, gpsb200_araim_t *aout) {
+                cudaStream_t s, const gpsb200_araim_config_t *araim, gpsb200_araim_t *aout,
+                const gpsb200_coarse_config_t *coarse, gpsb200_coarse_t *cout, int64_t *ms) {
     sc.have_last = false;
     if (!sc.d_chans) {
         CU_RET(cudaMalloc(&sc.d_chans, GPSB200_TRK_MAX_CHAN * sizeof(gpsb200_pvt_chan_t)));
@@ -1001,9 +1317,17 @@ cudaError_t run(Scratch &sc, const gpsb200_pvt_chan_t *chans, int nchan, const g
         sc.araim_cfg = *araim;
         araim_kfa(araim->p_fa_vert, araim->p_fa_horz, sc.kfa_h, sc.kfa_v);
     }
-    // the reference channel of the nominal receive time: the lowest with a valid, healthy ephemeris
+    sc.coarse = coarse != nullptr;
+    sc.want_ms = ms != nullptr;
+    if (coarse) {
+        CU_RET(grow(sc.d_coarse, sc.coarse_cap, (size_t) cfg->nfix));
+        if (ms) CU_RET(grow(sc.d_ms, sc.ms_cap, (size_t) cfg->nfix * nchan));
+        sc.coarse_cfg = *coarse;
+    }
+    // the reference channel of the nominal receive time: the lowest with a valid, healthy ephemeris (a coarse-time call
+    // has no anchors and no nominal receive time)
     sc.ref = -1;
-    for (int c = 0; c < nchan && sc.ref < 0; c++)
+    for (int c = 0; c < nchan && sc.ref < 0 && !coarse; c++)
         if (chans[c].eph.valid && chans[c].eph.health == 0) sc.ref = c;
     sc.ref_sample = sc.ref >= 0 ? epochs[(size_t) sc.ref * max_epochs + chans[sc.ref].anchor_epoch].sample : 0;
     sc.ref_ms = sc.ref >= 0 ? chans[sc.ref].anchor_ms : 0;
@@ -1024,6 +1348,12 @@ cudaError_t run(Scratch &sc, const gpsb200_pvt_chan_t *chans, int nchan, const g
     if (araim)
         CU_RET(cudaMemcpyAsync(aout, sc.d_araim, (size_t) cfg->nfix * sizeof(gpsb200_araim_t), cudaMemcpyDeviceToHost,
                                s));
+    if (coarse) {
+        CU_RET(cudaMemcpyAsync(cout, sc.d_coarse, (size_t) cfg->nfix * sizeof(gpsb200_coarse_t), cudaMemcpyDeviceToHost,
+                               s));
+        if (ms)
+            CU_RET(cudaMemcpyAsync(ms, sc.d_ms, (size_t) cfg->nfix * nchan * sizeof(int64_t), cudaMemcpyDeviceToHost, s));
+    }
     CU_RET(cudaStreamSynchronize(s));
     sc.have_last = true;
     return cudaSuccess;

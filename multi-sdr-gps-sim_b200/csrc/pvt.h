@@ -17,11 +17,13 @@ static_assert(sizeof(gpsb200_raim_config_t) == 32, "gpsb200_raim_config_t layout
 static_assert(sizeof(gpsb200_raim_t) == 48, "gpsb200_raim_t layout");
 static_assert(sizeof(gpsb200_araim_config_t) == 96, "gpsb200_araim_config_t layout");
 static_assert(sizeof(gpsb200_araim_t) == 64, "gpsb200_araim_t layout");
+static_assert(sizeof(gpsb200_coarse_config_t) == 48, "gpsb200_coarse_config_t layout");
+static_assert(sizeof(gpsb200_coarse_t) == 32, "gpsb200_coarse_t layout");
 
-// Empty when the call is well-formed (see the header). raim and araim may be NULL; at most one is not.
+// Empty when the call is well-formed (see the header). raim, araim and coarse may be NULL; at most one is not.
 std::string check(const gpsb200_pvt_chan_t *chans, int nchan, const gpsb200_track_epoch_t *epochs, const int32_t *nepochs,
                   int max_epochs, const gpsb200_pvt_config_t *cfg, const gpsb200_raim_config_t *raim,
-                  const gpsb200_araim_config_t *araim);
+                  const gpsb200_araim_config_t *araim, const gpsb200_coarse_config_t *coarse = nullptr);
 
 // The RAIM tables of gpsb200_raim_thresholds (raim_thresholds.cpp); false when p_fa or p_md is outside 1e-12..0.5.
 bool raim_thresholds(double p_fa, double p_md, double *T, double *lambda);
@@ -56,16 +58,26 @@ struct Scratch {
     gpsb200_araim_t *d_araim = nullptr;          // [nfix]
     size_t araim_cap = 0;
     double kfa_h[GPSB200_RAIM_MAX_DOF] = {}, kfa_v[GPSB200_RAIM_MAX_DOF] = {};
+    // the coarse-time call of the previous call (gpsb200_pvt_coarse)
+    bool coarse = false, want_ms = false;
+    gpsb200_coarse_config_t coarse_cfg{};
+    gpsb200_coarse_t *d_coarse = nullptr;        // [nfix]
+    size_t coarse_cap = 0;
+    int64_t *d_ms = nullptr;                     // [nfix][nchan]
+    size_t ms_cap = 0;
 };
 
 void scratch_free(Scratch &sc);
 // Upload, run k_pvt on s and download the fixes (and residuals when not NULL); waits for the results. With raim
 // (not NULL) the kernel's RAIM instantiation runs and out [nfix] receives its records; with araim (not NULL) the ARAIM
-// instantiation and aout [nfix]. At most one of raim and araim is not NULL.
+// instantiation and aout [nfix]; with coarse (not NULL) k_pvt_coarse, cout [nfix] and ms [nfix][nchan] (may be NULL).
+// At most one of raim, araim and coarse is not NULL.
 cudaError_t run(Scratch &sc, const gpsb200_pvt_chan_t *chans, int nchan, const gpsb200_track_epoch_t *epochs,
                 const int32_t *nepochs, int max_epochs, const gpsb200_pvt_config_t *cfg,
                 const gpsb200_raim_config_t *raim, gpsb200_fix_t *fixes, double *residuals, gpsb200_raim_t *out,
-                cudaStream_t s, const gpsb200_araim_config_t *araim = nullptr, gpsb200_araim_t *aout = nullptr);
+                cudaStream_t s, const gpsb200_araim_config_t *araim = nullptr, gpsb200_araim_t *aout = nullptr,
+                const gpsb200_coarse_config_t *coarse = nullptr, gpsb200_coarse_t *cout = nullptr,
+                int64_t *ms = nullptr);
 // Enqueue k_pvt again on the previous call's device-resident inputs.
 cudaError_t replay(Scratch &sc, cudaStream_t s);
 

@@ -1365,4 +1365,60 @@ int gpsb200_almanac_read(const char *path, gpsb200_almanac_record_t rec[32], int
     return GPSB200_OK;
 }
 
+int gpsb200_rinex_ephemeris(const char *path, int rinex3, int32_t week, double sow, gpsb200_ephemeris_t eph[32]) {
+    if (!path || !eph || (rinex3 != 0 && rinex3 != 1) || week < 0 || !(sow >= 0.0 && sow < kSecWeek))
+        return GPSB200_ERR_ARG;
+    std::vector<Eph> sets((size_t) kEphSets * kMaxSat);
+    Eph (*tab)[kMaxSat] = reinterpret_cast<Eph (*)[kMaxSat]>(sets.data());
+    IonoUtc io;
+    const int n = rinex3 ? read_rinex3(path, tab, io) : read_rinex2(path, tab, io);
+    if (n < 0) return GPSB200_ERR_ARG;
+    GpsTime t;
+    t.week = week;
+    t.sec = sow;
+    for (int sv = 0; sv < kMaxSat; sv++) {
+        const Eph *best = nullptr;
+        double best_d = 0.0;
+        for (int k = 0; k < n; k++) {
+            const Eph &e = tab[k][sv];
+            const double d = fabs(gps_diff(e.toe, t));
+            if (e.valid && d <= 7200.0 && (!best || d < best_d)) {
+                best = &e;
+                best_d = d;
+            }
+        }
+        gpsb200_ephemeris_t &o = eph[sv];
+        o = gpsb200_ephemeris_t{};
+        if (!best) continue;
+        const Eph &e = *best;
+        o.valid = 1;
+        o.week = e.toe.week % 1024;
+        o.iodc = e.iodc;
+        o.iode = e.iode;
+        o.health = e.svh;
+        o.toc = e.toc.sec;
+        o.af0 = e.af0;
+        o.af1 = e.af1;
+        o.af2 = e.af2;
+        o.tgd = e.tgd;
+        o.toe = e.toe.sec;
+        o.m0 = e.m0;
+        o.deltan = e.deltan;
+        o.ecc = e.ecc;
+        o.sqrta = e.sqrta;
+        o.omg0 = e.omg0;
+        o.inc0 = e.inc0;
+        o.aop = e.aop;
+        o.omgdot = e.omgdot;
+        o.idot = e.idot;
+        o.cuc = e.cuc;
+        o.cus = e.cus;
+        o.crc = e.crc;
+        o.crs = e.crs;
+        o.cic = e.cic;
+        o.cis = e.cis;
+    }
+    return GPSB200_OK;
+}
+
 }  // extern "C"

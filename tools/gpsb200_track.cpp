@@ -11,6 +11,10 @@
 // the RAIM verdict, the PRNs it excluded ("-" for none) and HPL/VPL in metres (DESIGN §11.1). With --araim they come
 // from gpsb200_pvt_araim and each line gains the ARAIM verdict, the excluded PRN, the PRNs below the elevation mask
 // ("-" for none), HPL/VPL and the EMT in metres (DESIGN §11.2).
+// With --assist the fixes are coarse-time fixes (gpsb200_pvt_coarse, DESIGN §11.3): nothing needs to be decoded. The
+// ephemeris comes from a RINEX navigation file (gpsb200_rinex_ephemeris, at the assist time), the a-priori position
+// from --assist-pos and the a-priori time from --assist-time, the GPS time of the first sample after --block /
+// --offset-ms; each line gains delta, the solved a-priori time error in seconds.
 #include <algorithm>
 #include <cmath>
 #include <cstdio>
@@ -33,7 +37,8 @@ static void usage() {
     fprintf(stderr,
             "gpsb200-track FILE [--iq16] [--block B] [--offset-ms N] [--ms K] [--prn LIST] [--threshold R] [--device D]\n"
             "              [--fix [--fix-every MS] [--iono a0,a1,a2,a3,b0,b1,b2,b3] [--raim SIGMA[,P_FA,P_MD[,MAX_EXCLUDE]]]\n"
-            "               [--araim MASK_DEG[,SIGMA_URA,SIGMA_URE,B_NOM,P_SAT]]]\n"
+            "               [--araim MASK_DEG[,SIGMA_URA,SIGMA_URE,B_NOM,P_SAT]]\n"
+            "               [--assist NAV_FILE[,3] --assist-pos LAT,LON,H --assist-time YYYY/MM/DD,hh:mm:ss[.s]]]\n"
             "  FILE              interleaved I,Q at 3 Msps, int8 (default) or int16 (--iq16)\n"
             "  --block B         start at 0.1 s block B (sample 300000 B); --offset-ms N adds N ms (3000 N samples)\n"
             "  --ms K            track K ms of signal from the start (default: to the end of the file)\n"
@@ -44,7 +49,9 @@ static void usage() {
             "  --raim            fault detection and exclusion with pseudorange sigma SIGMA m (P_FA 1e-5, P_MD 1e-3,\n"
             "                    MAX_EXCLUDE 1 by default): adds the verdict, the excluded PRNs and HPL/VPL to each fix\n"
             "  --araim           advanced RAIM with elevation mask MASK_DEG (the other fields: the header's defaults): adds\n"
-            "                    the verdict, the excluded PRN, the masked PRNs, HPL/VPL and the EMT to each fix\n",
+            "                    the verdict, the excluded PRN, the masked PRNs, HPL/VPL and the EMT to each fix\n"
+            "  --assist          coarse-time fixes without decoding: ephemeris from the RINEX file (,3: RINEX 3), a-priori\n"
+            "                    position (deg, deg, m) and GPS time of the first sample; adds delta (s) to each fix\n",
             kDefaultThreshold, kDefaultFixEvery);
     exit(2);
 }
@@ -52,13 +59,18 @@ static void usage() {
 static const char *const kVerdict[] = {"PASS", "EXCLUDED", "ALERT", "UNAVAILABLE"};
 
 // Fixes from `first` every `step` samples to the last epoch of the channels, one line per fix with status OK; with
-// raim (not NULL) from gpsb200_pvt_raim, with its three columns; with araim (not NULL) from gpsb200_pvt_araim, with its five.
+// raim (not NULL) from gpsb200_pvt_raim, with its three columns; with araim (not NULL) from gpsb200_pvt_araim, with its five;
+// with ap (not NULL) from gpsb200_pvt_coarse, with delta.
 static int print_fixes(gpsb200_ctx_t *ctx, const std::vector<gpsb200_pvt_chan_t> &chans, const std::vector<int> &of,
                        const std::vector<std::vector<gpsb200_track_epoch_t>> &eps, long long first, long long step,
                        gpsb200_pvt_config_t cfg, const gpsb200_raim_config_t *raim,
-                       const gpsb200_araim_config_t *araim) {
+                       const gpsb200_araim_config_t *araim, const gpsb200_coarse_config_t *ap) {
     const int n = (int) chans.size();
-    printf("# fixes: %d channel(s) with an ephemeris and a time anchor decoded, Klobuchar %s\n", n, cfg.iono ? "on" : "off");
+    if (ap)
+        printf("# coarse-time fixes: %d channel(s) with an assisted ephemeris, Klobuchar %s\n", n, cfg.iono ? "on" : "off");
+    else
+        printf("# fixes: %d channel(s) with an ephemeris and a time anchor decoded, Klobuchar %s\n", n,
+               cfg.iono ? "on" : "off");
     if (n == 0) return GPSB200_OK;
     size_t me = 1;
     long long end = 0;
@@ -79,14 +91,18 @@ static int print_fixes(gpsb200_ctx_t *ctx, const std::vector<gpsb200_pvt_chan_t>
     std::vector<gpsb200_fix_t> fx(cfg.nfix);
     std::vector<gpsb200_raim_t> rm(raim ? cfg.nfix : 0);
     std::vector<gpsb200_araim_t> am(araim ? cfg.nfix : 0);
-    const int rc = araim ? gpsb200_pvt_araim(ctx, chans.data(), n, all.data(), cnt.data(), (int) me, &cfg, araim,
+    std::vector<gpsb200_coarse_t> cm(ap ? cfg.nfix : 0);
+    const int rc = ap ? gpsb200_pvt_coarse(ctx, chans.data(), n, all.data(), cnt.data(), (int) me, &cfg, ap, fx.data(),
+                                           nullptr, cm.data(), nullptr)
+                   : araim ? gpsb200_pvt_araim(ctx, chans.data(), n, all.data(), cnt.data(), (int) me, &cfg, araim,
                                              fx.data(), nullptr, am.data())
                    : raim ? gpsb200_pvt_raim(ctx, chans.data(), n, all.data(), cnt.data(), (int) me, &cfg, raim, fx.data(),
                                              nullptr, rm.data())
                           : gpsb200_pvt(ctx, chans.data(), n, all.data(), cnt.data(), (int) me, &cfg, fx.data(), nullptr);
     if (rc != GPSB200_OK) return rc;
     printf("# sample  tow_s  lat_deg  lon_deg  height_m  clock_m  vx  vy  vz (ECEF m/s)  channels  pdop%s\n",
-           raim ? "  raim  excluded_prns  hpl/vpl_m" : (araim ? "  araim  excluded_prn  masked_prns  hpl/vpl_m  emt_m" : ""));
+           raim ? "  raim  excluded_prns  hpl/vpl_m"
+                : (araim ? "  araim  excluded_prn  masked_prns  hpl/vpl_m  emt_m" : (ap ? "  delta_s" : "")));
     for (int i = 0; i < cfg.nfix; i++) {
         const gpsb200_fix_t &f = fx[i];
         if (f.status != GPSB200_FIX_OK) continue;
@@ -107,9 +123,26 @@ static int print_fixes(gpsb200_ctx_t *ctx, const std::vector<gpsb200_pvt_chan_t>
             printf("  %s  %s  %s  %.2f/%.2f  %.2f", kVerdict[am[i].verdict], ex.empty() ? "-" : ex.c_str(),
                    mk.empty() ? "-" : mk.c_str(), am[i].hpl, am[i].vpl, am[i].emt);
         }
+        if (ap) printf("  %.9f", cm[i].delta);
         printf("\n");
     }
     return GPSB200_OK;
+}
+
+// GPS week and second of a calendar date and time (GPS time, no leap seconds): days since 1980-01-06.
+static bool gps_of_date(const char *text, int32_t &week, double &sow) {
+    int y, mo, d, hh, mm;
+    double sec;
+    if (sscanf(text, "%d/%d/%d,%d:%d:%lf", &y, &mo, &d, &hh, &mm, &sec) != 6 || y < 1980 || mo < 1 || mo > 12 || d < 1 ||
+        d > 31 || hh < 0 || hh > 23 || mm < 0 || mm > 59 || !(sec >= 0.0 && sec < 60.0))
+        return false;
+    const int a = (14 - mo) / 12, yy = y + 4800 - a, m = mo + 12 * a - 3;
+    const long jdn = d + (153 * m + 2) / 5 + 365L * yy + yy / 4 - yy / 100 + yy / 400 - 32045;
+    const long days = jdn - 2444245;                // 1980-01-06
+    if (days < 0) return false;
+    week = (int32_t) (days / 7);
+    sow = (double) (days % 7) * 86400.0 + hh * 3600.0 + mm * 60.0 + sec;
+    return true;
 }
 
 int main(int argc, char **argv) {
@@ -127,6 +160,11 @@ int main(int argc, char **argv) {
     bool araim = false;
     gpsb200_araim_config_t acfg;
     memset(&acfg, 0, sizeof acfg);
+    std::string assist;
+    int assist_v3 = 0;
+    bool assist_pos = false, assist_time = false;
+    gpsb200_coarse_config_t ap;
+    memset(&ap, 0, sizeof ap);
     gpsb200_acq_config_t cfg;
     memset(&cfg, 0, sizeof cfg);
     cfg.ms = kAcqMs;
@@ -174,12 +212,35 @@ int main(int argc, char **argv) {
                                    &acfg.b_nom, &acfg.p_sat);
             if (got != 1 && got != 5) usage();
             araim = true;
+        } else if (a == "--assist") {
+            assist = val();
+            const size_t k = assist.rfind(',');
+            if (k != std::string::npos) {
+                if (assist.substr(k + 1) != "3") usage();
+                assist_v3 = 1;
+                assist.resize(k);
+            }
+        } else if (a == "--assist-pos") {
+            double llh[3];
+            if (sscanf(val(), "%lf,%lf,%lf", &llh[0], &llh[1], &llh[2]) != 3) usage();
+            const double kA = 6378137.0, kE2 = 0.0818191908426 * 0.0818191908426;   // WGS-84
+            const double la = llh[0] * M_PI / 180.0, lo = llh[1] * M_PI / 180.0;
+            const double N = kA / sqrt(1.0 - kE2 * sin(la) * sin(la));
+            ap.x_a[0] = (N + llh[2]) * cos(la) * cos(lo);
+            ap.x_a[1] = (N + llh[2]) * cos(la) * sin(lo);
+            ap.x_a[2] = (N * (1.0 - kE2) + llh[2]) * sin(la);
+            assist_pos = true;
+        } else if (a == "--assist-time") {
+            if (!gps_of_date(val(), ap.week, ap.t_a)) usage();
+            assist_time = true;
         }
         else if (a[0] != '-' && !path) path = argv[i];
         else usage();
     }
+    const bool coarse = !assist.empty();
     if (!path || block < 0 || offset_ms < 0 || ms == 0 || ms < -1 || fix_every < 1 || ((raim || araim) && !fix) ||
-        (raim && araim))
+        (raim && araim) || (coarse && (!fix || raim || araim || !assist_pos || !assist_time)) ||
+        (!coarse && (assist_pos || assist_time)))
         usage();
     cfg.f_lo_hz = kAcqLo;
     cfg.step_hz = kAcqStep;
@@ -187,6 +248,12 @@ int main(int argc, char **argv) {
 
     const size_t elem = ss == GPSB200_SC16 ? 2 : 1;
     const long long s0 = block * GPSB200_BLOCK_SAMPLES + offset_ms * GPSB200_ACQ_CODE_SAMPLES;
+    ap.s_a = s0;
+    gpsb200_ephemeris_t assisted[32];
+    if (coarse && gpsb200_rinex_ephemeris(assist.c_str(), assist_v3, ap.week, ap.t_a, assisted) != GPSB200_OK) {
+        fprintf(stderr, "gpsb200-track: cannot read the ephemeris of %s\n", assist.c_str());
+        return 1;
+    }
     const long long need = (long long) GPSB200_ACQ_CODE_SAMPLES * cfg.ms + GPSB200_ACQ_CODE_SAMPLES - 1;
     const long long have = file_samples(path, elem);
     if (have < 0) {
@@ -262,7 +329,16 @@ int main(int argc, char **argv) {
         const double dopp = ne > 0 ? e.back().carr_step * 3e6 / 4294967296.0 : 0.0;
         printf("%5d  %6s  %10.1f  %9d  %8d  %5d  %9d\n", state[c].prn, locked ? "yes" : "no", dopp, sy.subframes,
                sy.words_ok, sy.nwords, sy.first_tow);
-        if (fix) {
+        if (fix && coarse) {
+            gpsb200_pvt_chan_t pc;
+            memset(&pc, 0, sizeof pc);
+            pc.eph = assisted[state[c].prn - 1];
+            pc.prn = state[c].prn;
+            if (pc.eph.valid) {
+                fix_chans.push_back(pc);
+                fix_of.push_back(c);
+            }
+        } else if (fix) {
             gpsb200_pvt_chan_t pc;
             memset(&pc, 0, sizeof pc);
             gpsb200_nav_ephemeris(words.data(), sy.nwords, &pc.eph, nullptr);
@@ -275,7 +351,7 @@ int main(int argc, char **argv) {
         }
     }
     if (fix) rc = print_fixes(ctx, fix_chans, fix_of, eps, s0 + kFixLead, fix_every * GPSB200_ACQ_CODE_SAMPLES, pcfg,
-                              raim ? &rcfg : nullptr, araim ? &acfg : nullptr);
+                              raim ? &rcfg : nullptr, araim ? &acfg : nullptr, coarse ? &ap : nullptr);
     if (rc != GPSB200_OK) fprintf(stderr, "gpsb200-track: %s\n", gpsb200_last_error(ctx));
     gpsb200_destroy(ctx);
     return rc == GPSB200_OK ? 0 : 1;

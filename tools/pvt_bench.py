@@ -18,8 +18,15 @@ two more arms alternate with them: the ARAIM stage (gpsb200_pvt_araim, DESIGN §
 on the fault-free epochs, and with channel --fault's satellite clock (af0) off by twice the smallest bias that the
 channel's own hypothesis detects (from the numpy model at the fix 1 s into the run), so that every fix excludes once.
 
+With --coarse the same run also times coarse-time fixes (gpsb200_pvt_coarse, DESIGN §11.3) on the same epochs, the
+a-priori position 50 km east and 1 km up of the truth and the a-priori time 10 s late, alternating with the plain
+kernel --rounds times. Reported beside the kernel times: the Gauss-Newton iterations per fix of both arms and the
+satellite evaluations (Kepler, orbit and clock) per channel and fix they imply -- 1 for gpsb200_pvt; 3 for the
+prediction, one per iteration and 3 for the ambiguity check for the coarse call -- and the largest difference of the
+coarse fixes from the numpy model (tests/coarse_model.py) over the --check sample.
+
     python tools/pvt_bench.py [--iters 5] [--warmup 1] [--check 64] [--seconds 600] [--raim SIGMA [--fault C]]
-                              [--araim MASK_DEG]
+                              [--araim MASK_DEG] [--coarse]
 """
 import argparse
 import importlib
@@ -40,6 +47,7 @@ import pvt_truth as PT   # noqa: E402
 
 LOC = (35.681298, 139.766247, 10.0)
 START = (2024, 1, 7, 2, 0, 0.0)
+START_SOW, START_WEEK = 7200.0, 2296     # START is Sunday 02:00 of GPS week 2296
 
 
 def card():
@@ -133,6 +141,48 @@ def raim_arms(ctx, stream, chans, packed, n, cfg, args):
     return out
 
 
+def coarse_arms(ctx, stream, chans, eps, packed, n, cfg, args):
+    """Kernel time of the plain and coarse arms, alternating; iterations, satellite evaluations and the model check."""
+    import coarse_model as CM
+    x0 = PM.llh_ecef(*LOC)
+    lat, lon, _ = PM.ecef_llh(x0)
+    east = np.array([-np.sin(lon), np.cos(lon), 0.0])
+    up = np.array([np.cos(lat) * np.cos(lon), np.cos(lat) * np.sin(lon), np.sin(lat)])
+    ap = gps.coarse_config(x0 + 50e3 * east + 1e3 * up, START_SOW + 10.0, 0, START_WEEK)
+    arms = {"plain": lambda: ctx.pvt(chans, packed, cfg, nepochs=n),
+            "coarse": lambda: ctx.pvt_coarse(chans, packed, cfg, ap, want_ms=True, nepochs=n)}
+    times = {k: [] for k in arms}
+    got = {}
+    for _ in range(args.rounds):
+        for k, call in arms.items():
+            got[k] = call()
+            times[k] += replay_ms(ctx, stream, args.iters)
+    plain = got["plain"]
+    fix, rec, ms = got["coarse"]
+    ok = fix["status"] == gps.FIX_OK
+    it_p, it_c = float(plain["iterations"].mean()), float(fix["iterations"][ok].mean())
+    worst = {f: 0.0 for f in ("x", "y", "z", "clock_m", "vx", "vy", "vz")}
+    worst["delta_s"] = 0.0
+    rng = np.random.default_rng(2)
+    for i in rng.choice(len(fix), size=min(args.check, len(fix)), replace=False):
+        one = gps.pvt_config(int(cfg["s0"]) + int(i) * int(cfg["step"]), 1, 1, (cfg["alpha"], cfg["beta"]))
+        want, wrec, _, wms = CM.coarse(chans, eps, one, ap)
+        assert int(want["status"][0]) == int(fix["status"][i]) and np.array_equal(wms[0], ms[i])
+        if fix["status"][i] == gps.FIX_OK:
+            for f in worst:
+                a, b = (rec["delta"][i], wrec["delta"][0]) if f == "delta_s" else (fix[f][i], want[f][0])
+                worst[f] = max(worst[f], abs(float(a) - float(b)))
+    out = {"apriori": "50 km east, 1 km up, +10 s", "rounds": args.rounds,
+           "status_counts": {int(k): int(v) for k, v in zip(*np.unique(fix["status"], return_counts=True))},
+           "iterations_mean": {"plain": round(it_p, 3), "coarse": round(it_c, 3)},
+           "satellite_evals_per_channel_fix": {"plain": 1, "coarse": round(3 + it_c + 3, 3)},
+           "max_abs_diff_vs_model": {k: float("%.3g" % v) for k, v in worst.items()}}
+    for k, t in times.items():
+        out[k + "_kernel_ms_median"] = round(float(np.median(t)), 3)
+        out[k + "_kernel_ms_min"] = round(float(np.min(t)), 3)
+    return out
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--iters", type=int, default=5)
@@ -143,6 +193,7 @@ def main():
     ap.add_argument("--fault", type=int, default=0)
     ap.add_argument("--rounds", type=int, default=3)
     ap.add_argument("--araim", type=float, default=None)
+    ap.add_argument("--coarse", action="store_true")
     args = ap.parse_args()
     import torch
     if not torch.cuda.is_available():
@@ -178,6 +229,7 @@ def main():
             b.synchronize()
             kern.append(a.elapsed_time(b))
         raim = raim_arms(ctx, stream, chans, packed, n, cfg, args) if args.raim is not None else None
+        coarse = coarse_arms(ctx, stream, chans, eps, packed, n, cfg, args) if args.coarse else None
     rng = np.random.default_rng(1)
     worst = {f: 0.0 for f in ("x", "y", "z", "clock_m", "vx", "vy", "vz")}
     for i in rng.choice(nfix, size=min(args.check, nfix), replace=False):
@@ -196,7 +248,8 @@ def main():
                       "iters": args.iters, "fixes_per_s_kernel": round(nfix / (t_kern * 1e-3)),
                       "status_counts": st, "checked": min(args.check, nfix),
                       "max_abs_diff_vs_model": {k: float("%.3g" % v) for k, v in worst.items()},
-                      **({"raim": raim} if raim is not None else {})}), flush=True)
+                      **({"raim": raim} if raim is not None else {}),
+                      **({"coarse": coarse} if coarse is not None else {})}), flush=True)
 
 
 if __name__ == "__main__":
