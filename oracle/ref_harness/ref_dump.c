@@ -142,7 +142,7 @@ int thread_to_core(int core_id) { (void) core_id; return 0; }
 static void usage(void) {
     fprintf(stderr,
             "ref_dump -e NAV -l lat,lon,h -d SEC [--iq16] [-m motion.csv] [-s y/m/d,h:m:s]\n"
-            "         [--iq FILE] [--crc FILE] [--params FILE] [-3] [--pluto-gain]\n");
+            "         [--iq FILE] [--crc FILE] [--params FILE] [-3] [--pluto-gain] [-I]\n");
     exit(2);
 }
 
@@ -175,6 +175,7 @@ int main(int argc, char **argv) {
         }
         else if (!strcmp(argv[i], "--iq16")) sim.sample_size = SC16;
         else if (!strcmp(argv[i], "-3")) sim.use_rinex3 = true;
+        else if (!strcmp(argv[i], "-I")) sim.ionosphere_enable = false;   /* as gps-sim.c's -I */
         else if (!strcmp(argv[i], "--pluto-gain")) sim.sdr_type = SDR_PLUTOSDR;
         else if (!strcmp(argv[i], "--iq") && i + 1 < argc) iq_name = argv[++i];
         else if (!strcmp(argv[i], "--params") && i + 1 < argc) par_name = argv[++i];
