@@ -20,35 +20,63 @@ def _d(s):
     return float(s.replace("D", "E"))
 
 
-def read_rinex(path):
-    """-> (records {prn: dict}, ion_alpha[4], ion_beta[4]) of a RINEX-2 navigation file as gen_rinex writes it (first set
-    of each PRN)."""
+def _sow(y, m, d, hh, mi, sec):
+    """GPS second of week of a record epoch (UTC taken as GPS time, as the reference's date2gps does)."""
+    import datetime
+    dt = datetime.datetime(y, m, d, hh, mi) - datetime.datetime(1980, 1, 6)
+    return (dt.days * 86400 + dt.seconds) % 604800 + sec
+
+
+def read_rinex_sets(path):
+    """-> ([{prn: record} per set], ion_alpha[4], ion_beta[4]) of a RINEX-2 or RINEX-3 navigation file as gen_rinex
+    writes it. A record holds every broadcast field by name (sva and svh as written, before the reader's +32), and toc,
+    the second of week of its epoch line. A set starts where the epoch passes the set's first by more than an hour, as the
+    reference groups them (gps.c:1380-1392)."""
     lines = open(path).read().splitlines()
+    v3 = float(lines[0][:9]) >= 3.0
     alpha = beta = None
     i = 0
     while "END OF HEADER" not in lines[i]:
-        if lines[i][60:].strip() == "ION ALPHA":
-            alpha = [_d(lines[i][2 + 12 * k:14 + 12 * k]) for k in range(4)]
-        if lines[i][60:].strip() == "ION BETA":
-            beta = [_d(lines[i][2 + 12 * k:14 + 12 * k]) for k in range(4)]
+        label, ln = lines[i][60:].strip(), lines[i]
+        if label == "ION ALPHA" or (label == "IONOSPHERIC CORR" and ln.startswith("GPSA")):
+            alpha = [_d(ln[(5 if v3 else 2) + 12 * k:(17 if v3 else 14) + 12 * k]) for k in range(4)]
+        if label == "ION BETA" or (label == "IONOSPHERIC CORR" and ln.startswith("GPSB")):
+            beta = [_d(ln[(5 if v3 else 2) + 12 * k:(17 if v3 else 14) + 12 * k]) for k in range(4)]
         i += 1
     i += 1
-    recs = {}
+    sets, first = [], None
     names = ["iode", "crs", "deltan", "m0", "cuc", "ecc", "cus", "sqrta", "toe", "cic", "omg0", "cis", "inc0", "crc",
              "aop", "omgdot", "idot", "codes", "week", "l2p", "sva", "svh", "tgd", "iodc", "ttx", "fit", "sp1", "sp2"]
+    c0 = 4 if v3 else 3
     while i + 7 < len(lines) + 1 and i < len(lines):
         head = lines[i]
-        prn = int(head[0:2])
-        r = dict(af0=_d(head[22:41]), af1=_d(head[41:60]), af2=_d(head[60:79]))
+        if v3:
+            prn, y, m, d, hh, mi, sec = (int(head[1:3]), int(head[4:8]), int(head[9:11]), int(head[12:14]),
+                                         int(head[15:17]), int(head[18:20]), float(head[21:23]))
+            c = 23
+        else:
+            prn, y, m, d, hh, mi, sec = (int(head[0:2]), 2000 + int(head[3:5]), int(head[6:8]), int(head[9:11]),
+                                         int(head[12:14]), int(head[15:17]), float(head[17:22]))
+            c = 22
+        r = dict(af0=_d(head[c:c + 19]), af1=_d(head[c + 19:c + 38]), af2=_d(head[c + 38:c + 57]))
         vals = []
         for k in range(1, 8):
             ln = lines[i + k]
-            vals += [_d(ln[3 + 19 * j:22 + 19 * j]) for j in range(4)]
+            vals += [_d(ln[c0 + 19 * j:c0 + 19 + 19 * j]) for j in range(4)]
         r.update(zip(names, vals))
-        r["toc"] = r["toe"]
-        recs.setdefault(prn, r)
+        r["toc"] = _sow(y, m, d, hh, mi, sec)
+        if first is None or r["toc"] - first > 3600.0:
+            first = r["toc"]
+            sets.append({})
+        sets[-1].setdefault(prn, r)
         i += 8
-    return recs, np.array(alpha), np.array(beta)
+    return sets, np.array(alpha), np.array(beta)
+
+
+def read_rinex(path):
+    """-> (records {prn: dict}, ion_alpha[4], ion_beta[4]) of the first set of a navigation file (read_rinex_sets)."""
+    sets, alpha, beta = read_rinex_sets(path)
+    return sets[0], alpha, beta
 
 
 # integer field of eph2sbf (gps.c:662-684: truncation toward zero) and its scale; x pi for semicircles

@@ -184,9 +184,10 @@ def test_a_wrong_integer_cannot_be_seen_with_five_channels(tmp_path):
 
 
 def test_rinex_ephemeris_equals_the_file(tmp_path):
-    """gpsb200_rinex_ephemeris on gen_rinex's file: every field of each PRN's record is read_rinex's value; the RINEX-3
-    file of the same sky gives the same records; PRNs the file lacks, and times more than 2 h from every toe, give
-    valid 0."""
+    """gpsb200_rinex_ephemeris on gen_rinex's file: every field of each PRN's record is read_rinex's value, toc the
+    second of week of the record's epoch line and toe the orbit field; the RINEX-3 file of the same sky gives the same
+    records; PRNs the file lacks, and times more than 2 h from every toe, give valid 0. (tests/test_ephemeris_terms.py
+    reads files whose toc and toe differ.)"""
     nav = make_nav(tmp_path, 12)
     recs, _, _ = PT.read_rinex(nav)
     toe = next(iter(recs.values()))["toe"]
