@@ -808,6 +808,88 @@ int gpsb200_pvt_coarse(gpsb200_ctx_t *ctx, const gpsb200_pvt_chan_t *chans, int 
                        const gpsb200_pvt_config_t *cfg, const gpsb200_coarse_config_t *apriori, gpsb200_fix_t *fixes,
                        double *residuals, gpsb200_coarse_t *out, int64_t *ms);
 
+/* ---- position search: coarse-time fixes with no a-priori position (DESIGN §11.4; tests/search_model.py states it in
+ * numpy). gpsb200_pvt_coarse's assistance without x_a: the ephemeris, an a-priori GPS time t_a (s of week, week `week`)
+ * at stream sample s_a, and a grid of `nodes` = N candidate positions over the whole Earth. Per fix instant s:
+ *   1. Grid. Node i (0 <= i < N) is the Fibonacci lattice point z_i = 1 - (2 i + 1) / N, geodetic latitude asin(z_i),
+ *      longitude 2 pi frac(i g) (g the double nearest (3 - sqrt(5)) / 2 = 0x1.8722191a02d61p-2), height 0 on WGS-84:
+ *      x = (N_e cos lat cos lon, N_e cos lat sin lon, N_e (1 - e^2) sin lat), N_e = a / sqrt(1 - e^2 sin^2 lat).
+ *      gpsb200_search_nodes returns them.
+ *   2. Used channels: gpsb200_pvt_coarse step 2 (period, locks, eph.valid, health, |t_a(s) - toe| <= 7200 s); they do not
+ *      depend on the node. Fewer than GPSB200_SEARCH_MIN_CHANNELS: status GPSB200_FIX_FEW and nothing is searched (with 5
+ *      channels the coarse solve fits any integers exactly, so every node would return its own OK fix).
+ *   3. Visibility prune: each used channel's satellite position p at GPS time t_a(s) - 0.075 s (gpsb200_pvt's satellite,
+ *      unrotated). Node i is searched only if every used channel has (up_i . (p - x_i)) / |p - x_i| >=
+ *      sin(GPSB200_SEARCH_MIN_ELEV_DEG), up_i the unit vector at the node's latitude / longitude. A channel is tracked
+ *      only while its satellite is above the receiver's horizon (re-checked every 30 s), and a node within 50 km of the
+ *      receiver sees it at most about half a degree lower.
+ *   4. Per searched node: gpsb200_pvt_coarse steps 1 and 3-9 with x_a = the node and the same t_a, s_a and week. The
+ *      node is OK when that returns GPSB200_FIX_OK.
+ *   5. Winner: the OK node with the smallest floor(1000 rms) (post-fit rms in whole mm), the lowest node on ties. Nodes
+ *      that converge to one solution leave rms values that differ by rounding only (below 1 nm), so an exact comparison
+ *      would choose among them by rounding noise. The fix record, residuals, ms, delta, pdop, ref, week and changed are
+ *      the winner's coarse solve (its status replaced as below).
+ *   6. Uniqueness: support = the OK nodes whose fix lies within GPSB200_SEARCH_DISTINCT of the winner's (the winner
+ *      included). An OK node whose fix lies farther is a distinct solution; alt_rms / alt_dist are the rms and distance
+ *      from the winner of the distinct solution that step 5's ordering puts first. Any distinct solution: status
+ *      GPSB200_FIX_AMBIGUOUS, the records still the winner's. No OK node: GPSB200_FIX_NO_CONVERGENCE. More than
+ *      GPSB200_SEARCH_MAX_OK(N) OK nodes (the device keeps a list of that many per instant): GPSB200_FIX_AMBIGUOUS with
+ *      no winner, `ok` still the exact count. The nodes that converge to one fix cover a region of fixed area, so their
+ *      number grows in proportion to N: on the model a unique fix had at most 147 of 262 144 (1 in 1 783, 7 channels),
+ *      and the list holds 1 in 256 (at least 64), seven times that. So this outcome means many OK nodes that cannot be
+ *      one fix's, as at 6 channels (about 1 200 on the default grid).
+ *      Strict on purpose. On the model, 7 or more channels gave no distinct solution over the default grid, while 6
+ *      channels gave about a thousand wrong-integer fixes with rms of metres: a 6-channel search is AMBIGUOUS.
+ * Guarantee: the default grid's covering radius is 33.99 km on a sphere of the WGS-84 equatorial radius (the largest
+ * circumradius of its convex hull's facets). For a receiver at a height of 0-50 km some node lies within
+ * gpsb200_pvt_coarse's 50 km, and with t_a within 10 s that node's integers are right (2 x 34 km + 19 km is far below
+ * the 150 km limit). The winner is a different node only if that node also finds an OK fix. N = 131072 gives 48.06 km,
+ * too close to 50 km.
+ * Records without a winner: fix status, sample, nused and mask set, iterations 0, every double NaN; residuals NaN, ms
+ * -1, delta / pdop NaN, ref -1, week -1, changed 0. */
+#define GPSB200_SEARCH_NODES 262144          /* the default grid */
+#define GPSB200_SEARCH_MIN_NODES 64
+#define GPSB200_SEARCH_MAX_NODES 4194304     /* 2^22 */
+#define GPSB200_SEARCH_MIN_ELEV_DEG (-5.0)
+#define GPSB200_SEARCH_MIN_CHANNELS 6
+#define GPSB200_SEARCH_DISTINCT 1000.0       /* m */
+#define GPSB200_SEARCH_MAX_OK(n) ((n) / 256 > 64 ? (n) / 256 : 64)   /* OK-list length per instant, N nodes */
+#define GPSB200_SEARCH_HIT_BYTES_PER_OK 40
+#define GPSB200_SEARCH_HIT_BYTES (256ll << 20)   /* the device's OK lists of one pass over the instants */
+typedef struct gpsb200_search_config {
+    double t_a;            /* a-priori GPS time at sample s_a, s of week: 0 <= t_a < 604800 */
+    int64_t s_a;           /* stream sample of t_a: 0..2^62 */
+    int32_t week;          /* GPS week of t_a: >= 0 */
+    int32_t nodes;         /* grid nodes N: GPSB200_SEARCH_MIN_NODES..GPSB200_SEARCH_MAX_NODES */
+    int64_t reserved;      /* 0 */
+} gpsb200_search_config_t; /* 32 bytes */
+typedef struct gpsb200_search {
+    int32_t winner;        /* the winning node; -1 when there is none */
+    int32_t searched;      /* nodes that passed the visibility prune */
+    int32_t ok;            /* of those, nodes whose coarse solve was OK */
+    int32_t support;       /* OK nodes within GPSB200_SEARCH_DISTINCT of the winner's fix */
+    double alt_rms;        /* the first distinct solution's rms (step 6), m; NaN when there is none */
+    double alt_dist;       /* its distance from the winner's fix, m; NaN when there is none */
+    double delta, pdop;    /* the winner's (gpsb200_coarse_t) */
+    int32_t ref, week;     /* the winner's (gpsb200_coarse_t) */
+    uint32_t changed;      /* the winner's (gpsb200_coarse_t) */
+    int32_t reserved;
+} gpsb200_search_t;        /* 64 bytes */
+/* Host: xyz [n][3], the ECEF positions (m) of the n-node grid of step 1. GPSB200_ERR_ARG unless
+ * GPSB200_SEARCH_MIN_NODES <= n <= GPSB200_SEARCH_MAX_NODES and xyz is not NULL. */
+int gpsb200_search_nodes(int n, double *xyz);
+/* Searches: gpsb200_pvt_coarse's arguments with the search config in place of the a-priori one (GPSB200_ERR_ARG unless
+ * 0 <= t_a < 604800, 0 <= s_a <= 2^62, week >= 0, nodes in range and reserved 0; anchors are neither read nor checked),
+ * out [nfix] records, ms [nfix][nchan] and node_rms [nfix][nodes] (NULL: not wanted): the rms of each OK node, NaN where
+ * a node was pruned or not OK. Device scratch: 780 bytes per instant, plus one pass's OK lists, at most
+ * GPSB200_SEARCH_HIT_BYTES (the instants run in passes of as many as that holds, 40 bytes per list entry: 6 553 on
+ * the default grid, 409 at 2^22 nodes), never nfix x nodes; node_rms, when wanted, takes nfix x nodes doubles. Results do not depend on the order the device runs in. gpsb200_pvt_replay
+ * re-runs it when it ran last. */
+int gpsb200_pvt_search(gpsb200_ctx_t *ctx, const gpsb200_pvt_chan_t *chans, int nchan,
+                       const gpsb200_track_epoch_t *epochs, const int32_t *nepochs, int max_epochs,
+                       const gpsb200_pvt_config_t *cfg, const gpsb200_search_config_t *search, gpsb200_fix_t *fixes,
+                       double *residuals, gpsb200_search_t *out, int64_t *ms, double *node_rms);
+
 /* ---- scenario engine: the reference's host path outside the sample loop -------------
  * RINEX-2/3 navigation file (plain or gzip-compressed, read through zlib like the reference, gps.c:1147) +
  * location/motion -> the gpsb200_chan_t records and NAV frames the

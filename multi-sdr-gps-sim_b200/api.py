@@ -263,6 +263,32 @@ def coarse_config(x_a, t_a, s_a=0, week=0):
     return c
 
 
+# gpsb200_search_config_t / gpsb200_search_t (DESIGN §11.4)
+SEARCH_CONFIG_DTYPE = np.dtype([("t_a", "<f8"), ("s_a", "<i8"), ("week", "<i4"), ("nodes", "<i4"), ("reserved", "<i8")])
+SEARCH_DTYPE = np.dtype([("winner", "<i4"), ("searched", "<i4"), ("ok", "<i4"), ("support", "<i4"), ("alt_rms", "<f8"),
+                         ("alt_dist", "<f8"), ("delta", "<f8"), ("pdop", "<f8"), ("ref", "<i4"), ("week", "<i4"),
+                         ("changed", "<u4"), ("reserved", "<i4")])
+assert (SEARCH_CONFIG_DTYPE.itemsize, SEARCH_DTYPE.itemsize) == (32, 64)
+SEARCH_NODES = 262144
+
+
+def search_config(t_a, s_a=0, week=0, nodes=SEARCH_NODES):
+    """A SEARCH_CONFIG_DTYPE record: a-priori GPS time t_a (s of week `week`) at stream sample s_a, and the grid's node
+    count."""
+    c = np.zeros(1, SEARCH_CONFIG_DTYPE)[0]
+    c["t_a"], c["s_a"], c["week"], c["nodes"] = float(t_a), int(s_a), int(week), int(nodes)
+    return c
+
+
+def search_nodes(n=SEARCH_NODES):
+    """gpsb200_search_nodes: the ECEF positions float64[n, 3] of the n-node search grid."""
+    xyz = np.zeros((max(1, int(n)), 3))
+    rc = lib().gpsb200_search_nodes(int(n), xyz.ctypes.data)
+    if rc:
+        raise GpsB200Error(rc, "gpsb200_search_nodes")
+    return xyz
+
+
 def rinex_ephemeris(path, week, sow, rinex3=False):
     """gpsb200_rinex_ephemeris: EPHEMERIS_DTYPE[32], entry prn - 1 the PRN's record of the RINEX navigation file whose
     toe is nearest to GPS time (week, sow), within 2 h (valid 0 where there is none)."""
@@ -343,7 +369,7 @@ EXPORTS = ["gpsb200_create", "gpsb200_destroy", "gpsb200_last_error", "gpsb200_v
            "gpsb200_codegen", "gpsb200_acquire", "gpsb200_acquire_device", "gpsb200_track_start", "gpsb200_track",
            "gpsb200_track_device", "gpsb200_nav_decode", "gpsb200_nav_word_check", "gpsb200_nav_parity",
            "gpsb200_nav_ephemeris", "gpsb200_nav_time_anchor", "gpsb200_pvt", "gpsb200_pvt_replay",
-           "gpsb200_pvt_raim", "gpsb200_raim_thresholds", "gpsb200_pvt_araim", "gpsb200_araim_kfa", "gpsb200_pvt_coarse", "gpsb200_rinex_ephemeris", "gpsb200_bind_numa", "gpsb200_span_chain_host", "gpsb200_lanes_model_block",
+           "gpsb200_pvt_raim", "gpsb200_raim_thresholds", "gpsb200_pvt_araim", "gpsb200_araim_kfa", "gpsb200_pvt_coarse", "gpsb200_pvt_search", "gpsb200_search_nodes", "gpsb200_rinex_ephemeris", "gpsb200_bind_numa", "gpsb200_span_chain_host", "gpsb200_lanes_model_block",
            "gpsb200_lanes_window_band_host", "gpsb200_slice_prepare", "gpsb200_slice_probe",
            "gpsb200_slice_finish", "gpsb200_slice_finish_cb", "gpsb200_slice_wait", "gpsb200_link_apply", "gpsb200_slice_link_host", "gpsb200_debug_corrupt_chain", "gpsb200_synth_kernel_name",
            "gpsb200_debug_run_checkpoints", "gpsb200_checkpoint_segments_host",
@@ -454,6 +480,8 @@ def lib():
         L.gpsb200_pvt_araim.argtypes = L.gpsb200_pvt_raim.argtypes
         L.gpsb200_araim_kfa.argtypes = [C.c_double, C.c_double, C.c_void_p, C.c_void_p]
         L.gpsb200_pvt_coarse.argtypes = L.gpsb200_pvt_raim.argtypes + [C.c_void_p]
+        L.gpsb200_pvt_search.argtypes = L.gpsb200_pvt_coarse.argtypes + [C.c_void_p]
+        L.gpsb200_search_nodes.argtypes = [C.c_int, C.c_void_p]
         L.gpsb200_rinex_ephemeris.argtypes = [C.c_char_p, C.c_int, C.c_int32, C.c_double, C.c_void_p]
         _lib = L
     return _lib
@@ -1039,6 +1067,27 @@ class Context:
                                              None if res is None else res.ctypes.data, out.ctypes.data,
                                              None if ms is None else ms.ctypes.data))
         return (fixes, out) + ((res,) if want_residuals else ()) + ((ms,) if want_ms else ())
+
+    def pvt_search(self, chans, epochs, cfg, search, want_residuals=False, want_ms=False, want_node_rms=False,
+                   nepochs=None):
+        """Position search with no a-priori position (gpsb200_pvt_search; DESIGN §11.4): coarse-time fixes from every
+        node of a global grid. The arguments of pvt (anchors unread), plus search: SEARCH_CONFIG_DTYPE record
+        (search_config).
+        -> (fixes FIX_DTYPE[nfix], SEARCH_DTYPE[nfix]), then the residuals float64[nfix, nchan] with want_residuals, the
+        resolved ms of week int64[nfix, nchan] (-1 where not used) with want_ms, and every node's rms float64[nfix,
+        nodes] (NaN where pruned or not OK) with want_node_rms."""
+        ch, nchan, ep, n, me, cf, fixes, res = self._pvt_args(chans, epochs, cfg, want_residuals, nepochs)
+        sc = np.array(search, dtype=SEARCH_CONFIG_DTYPE).reshape(1)
+        out = np.zeros(fixes.size, SEARCH_DTYPE)
+        ms = np.zeros((fixes.size, max(1, nchan)), np.int64) if want_ms else None
+        nr = np.zeros((fixes.size, max(1, int(sc[0]["nodes"]))), np.float64) if want_node_rms else None
+        self._check(lib().gpsb200_pvt_search(self._h, ch.ctypes.data, nchan, ep.ctypes.data, n.ctypes.data, me,
+                                             cf.ctypes.data, sc.ctypes.data, fixes.ctypes.data,
+                                             None if res is None else res.ctypes.data, out.ctypes.data,
+                                             None if ms is None else ms.ctypes.data,
+                                             None if nr is None else nr.ctypes.data))
+        return ((fixes, out) + ((res,) if want_residuals else ()) + ((ms,) if want_ms else ())
+                + ((nr,) if want_node_rms else ()))
 
     @staticmethod
     def _pvt_args(chans, epochs, cfg, want_residuals, nepochs):

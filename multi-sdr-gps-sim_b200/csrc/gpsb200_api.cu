@@ -1140,20 +1140,22 @@ int track(gpsb200_ctx *ctx, const void *iq, int64_t nsamples, int sample_size, i
 }
 
 // Position fixes (pvt.cu), with the RAIM stage when raim is not NULL, the ARAIM stage when araim is not NULL, coarse-time
-// fixes when coarse is not NULL. Everything is checked before anything is enqueued.
+// fixes when coarse is not NULL, searches when search is not NULL. Everything is checked before anything is enqueued.
 int pvt_fix(gpsb200_ctx *ctx, const char *fn, const gpsb200_pvt_chan_t *chans, int nchan,
             const gpsb200_track_epoch_t *epochs, const int32_t *nepochs, int max_epochs, const gpsb200_pvt_config_t *cfg,
             const gpsb200_raim_config_t *raim, gpsb200_fix_t *fixes, double *residuals, gpsb200_raim_t *out,
             const gpsb200_araim_config_t *araim = nullptr, gpsb200_araim_t *aout = nullptr,
-            const gpsb200_coarse_config_t *coarse = nullptr, gpsb200_coarse_t *cout = nullptr, int64_t *ms = nullptr) {
+            const gpsb200_coarse_config_t *coarse = nullptr, gpsb200_coarse_t *cout = nullptr, int64_t *ms = nullptr,
+            const gpsb200_search_config_t *search = nullptr, gpsb200_search_t *sout = nullptr,
+            double *node_rms = nullptr) {
     const std::string at = std::string(fn) + ": ";
     if (!fixes) return fail(ctx, GPSB200_ERR_ARG, at + "NULL fixes");
-    const std::string bad = pvt::check(chans, nchan, epochs, nepochs, max_epochs, cfg, raim, araim, coarse);
+    const std::string bad = pvt::check(chans, nchan, epochs, nepochs, max_epochs, cfg, raim, araim, coarse, search);
     if (!bad.empty()) return fail(ctx, GPSB200_ERR_ARG, at + bad);
     const int rc = check_entry(ctx);
     if (rc) return rc;
     CU(pvt::run(ctx->pvt, chans, nchan, epochs, nepochs, max_epochs, cfg, raim, fixes, residuals, out, ctx->s_compute,
-                araim, aout, coarse, cout, ms));
+                araim, aout, coarse, cout, ms, search, sout, node_rms));
     return GPSB200_OK;
 }
 
@@ -1765,6 +1767,24 @@ int gpsb200_pvt_coarse(gpsb200_ctx_t *ctx, const gpsb200_pvt_chan_t *chans, int 
         return settle(ctx, nullptr, fail(ctx, GPSB200_ERR_ARG, "gpsb200_pvt_coarse: NULL apriori or out"));
     return settle(ctx, nullptr, pvt_fix(ctx, "gpsb200_pvt_coarse", chans, nchan, epochs, nepochs, max_epochs, cfg, nullptr,
                                         fixes, residuals, nullptr, nullptr, nullptr, apriori, out, ms));
+}
+
+int gpsb200_pvt_search(gpsb200_ctx_t *ctx, const gpsb200_pvt_chan_t *chans, int nchan,
+                       const gpsb200_track_epoch_t *epochs, const int32_t *nepochs, int max_epochs,
+                       const gpsb200_pvt_config_t *cfg, const gpsb200_search_config_t *search, gpsb200_fix_t *fixes,
+                       double *residuals, gpsb200_search_t *out, int64_t *ms, double *node_rms) {
+    if (!ctx) return GPSB200_ERR_ARG;
+    if (!search || !out)
+        return settle(ctx, nullptr, fail(ctx, GPSB200_ERR_ARG, "gpsb200_pvt_search: NULL search or out"));
+    return settle(ctx, nullptr, pvt_fix(ctx, "gpsb200_pvt_search", chans, nchan, epochs, nepochs, max_epochs, cfg, nullptr,
+                                        fixes, residuals, nullptr, nullptr, nullptr, nullptr, nullptr, ms, search, out,
+                                        node_rms));
+}
+
+int gpsb200_search_nodes(int n, double *xyz) {
+    if (!xyz || n < GPSB200_SEARCH_MIN_NODES || n > GPSB200_SEARCH_MAX_NODES) return GPSB200_ERR_ARG;
+    pvt::search_nodes(n, xyz);
+    return GPSB200_OK;
 }
 
 int gpsb200_araim_kfa(double p_fa_vert, double p_fa_horz, double *kfa_h, double *kfa_v) {

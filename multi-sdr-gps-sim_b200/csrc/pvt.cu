@@ -6,6 +6,7 @@
 // and the Klobuchar delay per lane and sums the normal equations over the warp with an XOR butterfly: both lanes of a
 // pair add the same two values, so every lane ends with the same bits and solves the 4 x 4 system identically. No
 // atomics, no shared memory; the kernel is bound by FP64 arithmetic (the trigonometry of the orbit and the iterations).
+#include <algorithm>
 #include <cmath>
 #include <cstring>
 #include <type_traits>
@@ -1161,6 +1162,450 @@ __global__ void __launch_bounds__(kWarps * 32, kCoarseMinBlocks) k_pvt_coarse(co
     if (a.ms && lane < a.nchan) a.ms[fi * a.nchan + lane] = has ? Nw : -1;
 }
 
+// ---- position search: coarse-time fixes from every node of a global grid (DESIGN §11.4) -----------------------------
+// An OK node's solution, appended to its fix instant's list (SearchArgs::hits) in whatever order the warps finish; only
+// order-free reductions read the list, so the results do not depend on scheduling.
+struct SearchHit {
+    double rms, x, y, z;
+    int32_t node, reserved;
+};
+static_assert(sizeof(SearchHit) == 5 * sizeof(double), "Scratch::d_hits holds SearchHit records as 5 doubles");
+static_assert(sizeof(SearchHit) == GPSB200_SEARCH_HIT_BYTES_PER_OK, "the header states the list's size");
+
+// Instants per pass of k_pvt_search and k_search_pick: as many as one GPSB200_SEARCH_HIT_BYTES list holds, at most 65535
+// (blockIdx.y).
+inline int search_pass(int nodes) {
+    const int64_t per = (int64_t) GPSB200_SEARCH_MAX_OK(nodes) * (int64_t) sizeof(SearchHit);
+    return (int) std::max<int64_t>(1, std::min<int64_t>(65535, (int64_t) GPSB200_SEARCH_HIT_BYTES / per));
+}
+struct SearchArgs : Args {
+    gpsb200_search_config_t sc;
+    double sin_min;            // sin(GPSB200_SEARCH_MIN_ELEV_DEG)
+    double *sat;               // [nfix][32][3]: each channel's satellite at t_a(s) - 0.075 s, unrotated
+    uint32_t *used;            // [nfix]: the used channels (header step 2)
+    int32_t *searched, *nok;   // [nfix]: nodes searched, OK nodes (also counts those the list could not hold)
+    SearchHit *hits;           // [instants of this pass][max_ok]
+    double *node_rms;          // [nfix][nodes] or NULL
+    gpsb200_search_t *out;
+    int64_t *ms;
+    int f0, nf;                // the instants f0 .. f0 + nf - 1 of this pass (k_pvt_search, k_search_pick)
+    int max_ok;                // the list's length per instant: GPSB200_SEARCH_MAX_OK(nodes)
+};
+
+// Node i of the n-node grid (header step 1): ECEF position x and the up vector at its geodetic latitude / longitude.
+__host__ __device__ inline void search_node(int64_t i, int n, double *x, double *up) {
+    constexpr double kGolden = 0x1.8722191a02d61p-2;   // the double nearest (3 - sqrt(5)) / 2
+    const double z = 1.0 - (2.0 * (double) i + 1.0) / (double) n;
+    const double t = (double) i * kGolden;
+    const double lat = asin(z), lon = 2.0 * M_PI * (t - floor(t));
+    const double sla = sin(lat), cla = cos(lat), slo = sin(lon), clo = cos(lon);
+    const double N = kWgsA / sqrt(1.0 - kWgsE * kWgsE * sla * sla);
+    x[0] = N * cla * clo;
+    x[1] = N * cla * slo;
+    x[2] = N * (1.0 - kWgsE * kWgsE) * sla;
+    up[0] = cla * clo;
+    up[1] = cla * slo;
+    up[2] = sla;
+}
+
+// k_pvt_coarse's header steps 1-9 from the a-priori config ap, restated rather than shared: moving k_pvt_coarse's body
+// into a function changes its register allocation. The fix and coarse records come out uniform over the warp; resid,
+// Nw and has are this lane's (channel's).
+__device__ __forceinline__ void search_solve(const Args &a, const gpsb200_coarse_config_t &ap, int64_t s, int lane,
+                                             gpsb200_fix_t &f, gpsb200_coarse_t &o, double &resid, int64_t &Nw,
+                                             bool &has) {
+    const double nan = __longlong_as_double(0x7ff8000000000000ll);
+    // header step 1
+    const int64_t ds = s - ap.s_a;
+    const int64_t q = floor_div(ds, 3000), m = ds - 3000 * q;
+    const double u = ap.t_a + (double) ds / 3e6;
+    const double kw = floor(u / 604800.0);
+    const double tas = u - 604800.0 * kw;
+    const double W = floor(ap.t_a), F = ap.t_a - W;
+    const double sub = F * 1000.0 + (double) m / 3000.0;   // ms
+
+    // header steps 2-4: measurement, prediction at x_a, reference channel
+    bool use = false;
+    double frac = 0.0, pred = 0.0, sel = -2.0;
+    const gpsb200_ephemeris_t *eph = nullptr;
+    double up[3];
+    {
+        double lat, lon, hgt, sla, cla, slo, clo;
+        ecef_llh(ap.x_a, lat, lon, hgt);
+        sincos(lat, &sla, &cla);
+        sincos(lon, &slo, &clo);
+        up[0] = cla * clo;
+        up[1] = cla * slo;
+        up[2] = sla;
+    }
+    double rate = 0.0;
+    if (lane < a.nchan) {
+        const gpsb200_pvt_chan_t &c = a.ch[lane];
+        const gpsb200_track_epoch_t *e = a.ep + (size_t) lane * a.max_epochs;
+        const int k = c.eph.valid && c.eph.health == 0 ? find_period(e, a.n[lane], s) : -1;
+        if (k >= 1 && e[k - 1].lock && e[k].lock && fabs(wrap_half_week(tas - c.eph.toe)) <= 7200.0) {
+            use = true;
+            eph = &c.eph;
+            const uint64_t phi = (uint64_t) e[k - 1].code_phase + (uint64_t) (s - e[k].sample) * e[k - 1].code_step;
+            frac = (double) phi / kCodeMod;
+            rate = -kLambda * ((double) e[k - 1].carr_step * kStepHz);
+            pred = predict(*eph, ap.x_a, tas, up, sel);
+        }
+    }
+    has = use;
+    const unsigned mask = __ballot_sync(kFull, use);
+    const int nused = __popc(mask);
+    double key = use ? sel : -2.0;
+    int r = lane;
+    warp_argmax(key, r);
+    const int ref = nused ? r : -1;
+    const double pred_r = __shfl_sync(kFull, pred, r), frac_r = __shfl_sync(kFull, frac, r);
+    // header step 5
+    const int64_t Nr = (int64_t) round_half_up(pred_r - frac_r);
+    const int64_t dN = (int64_t) round_half_up((pred - pred_r) - (frac - frac_r));
+    Nw = (((Nr + dN) % kWeekMs) + kWeekMs) % kWeekMs;
+    // header step 6
+    double rho = 0.0, tsv = 0.0;
+    if (has) {
+        int64_t D = ((int64_t) W * 1000 + q - Nw) % kWeekMs;
+        D = D >= kWeekMs / 2 ? D - kWeekMs : (D < -kWeekMs / 2 ? D + kWeekMs : D);
+        rho = (double) D * kCms + (sub - frac) * kCms;
+        tsv = (double) Nw * 1e-3 + frac * 1e-3;
+    }
+
+    f.sample = s;
+    f.nused = nused;
+    f.mask = mask;
+    f.iterations = 0;
+    f.status = nused < 5 ? GPSB200_FIX_FEW : GPSB200_FIX_NO_CONVERGENCE;
+    f.x = f.y = f.z = f.clock_m = f.t_rx = f.vx = f.vy = f.vz = f.drift = nan;
+    f.lat_deg = f.lon_deg = f.height = f.pdop = f.rms = nan;
+    o.delta = o.pdop = nan;
+    o.ref = ref;
+    o.week = -1;
+    o.changed = 0;
+    o.reserved = 0;
+    resid = nan;
+    if (nused >= 5) {
+        double X[5] = {ap.x_a[0], ap.x_a[1], ap.x_a[2], 0.0, 0.0};
+        double h[4] = {0, 0, 0, 0}, rr = 0.0, pr_v[3] = {0, 0, 0}, ddtsv = 0.0;
+        Chol5 ch;
+        bool ok = false;
+        double dX[5] = {0, 0, 0, 0, 0};
+#pragma unroll 1
+        for (int j = 0; j < GPSB200_PVT_MAX_ITER; j++) {
+            const double rad = sqrt(X[0] * X[0] + X[1] * X[1] + X[2] * X[2]);
+            const bool iono = a.cfg.iono && rad >= kIonoMinRadius;
+            double lat = 0.0, lon = 0.0, hgt = 0.0, sla = 0.0, cla = 0.0, slo = 0.0, clo = 0.0;
+            if (iono) {
+                ecef_llh(X, lat, lon, hgt);
+                sincos(lat, &sla, &cla);
+                sincos(lon, &slo, &clo);
+            }
+            h[0] = h[1] = h[2] = h[3] = 0.0;
+            rr = 0.0;
+            if (has) {
+                const gpsb200_ephemeris_t &e = *eph;
+                const double t = tsv + X[4];
+                const double d0 = wrap_half_week(t - e.toc);
+                const double tt = t - (e.af0 + d0 * (e.af1 + d0 * e.af2));
+                double p[3], v[3], dtsv;
+                satellite(e, tt, p, v, dtsv, ddtsv);
+                const double g0 = p[0] - X[0], g1 = p[1] - X[1], g2 = p[2] - X[2];
+                const double tau = sqrt(g0 * g0 + g1 * g1 + g2 * g2) / kC;
+                double sth, cth;
+                sincos(kOmegaE * tau, &sth, &cth);
+                const double px = p[0] * cth + p[1] * sth, py = p[1] * cth - p[0] * sth;
+                pr_v[0] = v[0] * cth + v[1] * sth;
+                pr_v[1] = v[1] * cth - v[0] * sth;
+                pr_v[2] = v[2];
+                const double l0 = px - X[0], l1 = py - X[1], l2 = p[2] - X[2];
+                const double R = sqrt(l0 * l0 + l1 * l1 + l2 * l2);
+                double I = 0.0;
+                if (iono) {
+                    const double nn = -sla * clo * l0 - sla * slo * l1 + cla * l2;
+                    const double ee = -slo * l0 + clo * l1;
+                    const double uu = cla * clo * l0 + cla * slo * l1 + sla * l2;
+                    double az = atan2(ee, nn);
+                    if (az < 0.0) az += 2.0 * kPi;
+                    const double el = atan2(uu, sqrt(nn * nn + ee * ee));
+                    I = klobuchar(a.cfg, lat, lon, az, el, tas + X[4] - X[3] / kC);
+                }
+                rr = rho - (R + X[3] - kC * dtsv + I);
+                h[0] = -l0 / R;
+                h[1] = -l1 / R;
+                h[2] = -l2 / R;
+                h[3] = (l0 * pr_v[0] + l1 * pr_v[1] + l2 * pr_v[2]) / R - kC * ddtsv;
+            }
+            const double N[15] = {warp_sum(h[0] * h[0]), warp_sum(h[0] * h[1]), warp_sum(h[0] * h[2]), warp_sum(h[0]),
+                                  warp_sum(h[0] * h[3]), warp_sum(h[1] * h[1]), warp_sum(h[1] * h[2]), warp_sum(h[1]),
+                                  warp_sum(h[1] * h[3]), warp_sum(h[2] * h[2]), warp_sum(h[2]), warp_sum(h[2] * h[3]),
+                                  (double) nused, warp_sum(h[3]), warp_sum(h[3] * h[3])};
+            const double b[5] = {warp_sum(h[0] * rr), warp_sum(h[1] * rr), warp_sum(h[2] * rr), warp_sum(rr),
+                                 warp_sum(h[3] * rr)};
+            f.iterations = j + 1;
+            if (!ch.factor(N)) break;
+            ch.solve<5>(b, dX);
+#pragma unroll
+            for (int i = 0; i < 5; i++) X[i] += dX[i];
+            if (sqrt(X[0] * X[0] + X[1] * X[1] + X[2] * X[2]) > kRunaway) break;
+            if (sqrt(dX[0] * dX[0] + dX[1] * dX[1] + dX[2] * dX[2]) < kConverged) {
+                ok = true;
+                break;
+            }
+        }
+        if (ok) {
+            // header step 8, at the fix, with the same reference channel
+            const double trx = tas + X[4] - X[3] / kC;
+            double dummy, pred2 = 0.0;
+            if (has) pred2 = predict(*eph, X, trx, up, dummy);
+            const double pred2_r = __shfl_sync(kFull, pred2, r);
+            const bool moved = has && (int64_t) round_half_up((pred2 - pred2_r) - (frac - frac_r)) != dN;
+            o.changed = __ballot_sync(kFull, moved);
+            if (has) resid = rr - (h[0] * dX[0] + h[1] * dX[1] + h[2] * dX[2] + dX[3] + h[3] * dX[4]);
+            if (o.changed || __any_sync(kFull, has && !(fabs(resid) <= GPSB200_COARSE_MAX_RESIDUAL))) {
+                f.status = GPSB200_FIX_AMBIGUOUS;
+                resid = nan;
+            } else {
+                // velocity and drift on the rows' first four columns, 5-state PDOP
+                const double y = has ? rate + kC * ddtsv + (h[0] * pr_v[0] + h[1] * pr_v[1] + h[2] * pr_v[2]) : 0.0;
+                const double bv[4] = {warp_sum(h[0] * y), warp_sum(h[1] * y), warp_sum(h[2] * y), warp_sum(y)};
+                double V[4];
+                ch.solve<4>(bv, V);
+                const double ss = warp_sum(has ? resid * resid : 0.0);
+                double Q[3];
+#pragma unroll
+                for (int i = 0; i < 3; i++) {
+                    double ei[5] = {0, 0, 0, 0, 0}, xi[5];
+                    ei[i] = 1.0;
+                    ch.solve<5>(ei, xi);
+                    Q[i] = xi[i];
+                }
+                f.status = GPSB200_FIX_OK;
+                f.x = X[0];
+                f.y = X[1];
+                f.z = X[2];
+                f.clock_m = X[3];
+                double t = trx, wk = kw;
+                if (t < 0.0) {
+                    t += 604800.0;
+                    wk -= 1.0;
+                } else if (t >= 604800.0) {
+                    t -= 604800.0;
+                    wk += 1.0;
+                }
+                f.t_rx = t;
+                f.vx = V[0];
+                f.vy = V[1];
+                f.vz = V[2];
+                f.drift = V[3];
+                double lat, lon, hgt;
+                ecef_llh(X, lat, lon, hgt);
+                f.lat_deg = lat * (180.0 / M_PI);
+                f.lon_deg = lon * (180.0 / M_PI);
+                f.height = hgt;
+                f.pdop = sqrt(Q[0] + Q[1] + Q[2]);
+                f.rms = sqrt(ss / (double) nused);
+                o.delta = X[4];
+                o.pdop = f.pdop;
+                o.week = ap.week + (int) wk;
+            }
+        }
+    }
+}
+
+// Per fix instant (one warp, lane = channel): header step 2's used channels and step 3's satellite positions; clears the
+// instant's counters.
+__global__ void __launch_bounds__(kWarps * 32) k_search_sats(const SearchArgs a) {
+    const int lane = threadIdx.x & 31;
+    const int64_t fi = (int64_t) blockIdx.x * kWarps + (threadIdx.x >> 5);
+    if (fi >= a.cfg.nfix) return;
+    const int64_t s = a.cfg.s0 + fi * a.cfg.step;
+    const int64_t ds = s - a.sc.s_a;
+    const double u = a.sc.t_a + (double) ds / 3e6;
+    const double tas = u - 604800.0 * floor(u / 604800.0);
+    bool use = false;
+    double p[3] = {0.0, 0.0, 0.0};
+    if (lane < a.nchan) {
+        const gpsb200_pvt_chan_t &c = a.ch[lane];
+        const gpsb200_track_epoch_t *e = a.ep + (size_t) lane * a.max_epochs;
+        const int k = c.eph.valid && c.eph.health == 0 ? find_period(e, a.n[lane], s) : -1;
+        if (k >= 1 && e[k - 1].lock && e[k].lock && fabs(wrap_half_week(tas - c.eph.toe)) <= 7200.0) {
+            use = true;
+            double v[3], dt, ddt;
+            satellite(c.eph, tas - 0.075, p, v, dt, ddt);
+        }
+    }
+    for (int i = 0; i < 3; i++) a.sat[(fi * 32 + lane) * 3 + i] = p[i];
+    const unsigned mask = __ballot_sync(kFull, use);
+    if (lane == 0) {
+        a.used[fi] = mask;
+        a.searched[fi] = 0;
+        a.nok[fi] = 0;
+    }
+}
+
+// Header steps 3-4 over the grid: one warp per 32 nodes of one fix instant (blockIdx.y). Each lane tests its own node's
+// visibility; the warp then solves the visible nodes one after another, lane = channel, and appends the OK ones to the
+// instant's list. Testing 32 nodes per warp keeps the warps busy although most nodes fail the test.
+constexpr int kSearchMinBlocks = 4;
+__global__ void __launch_bounds__(kWarps * 32, kSearchMinBlocks) k_pvt_search(const SearchArgs a) {
+    const int lane = threadIdx.x & 31;
+    const int64_t fi = (int64_t) a.f0 + blockIdx.y;
+    const int64_t base = ((int64_t) blockIdx.x * kWarps + (threadIdx.x >> 5)) * 32;
+    const int n = a.sc.nodes;
+    if (base >= n) return;
+    const unsigned used = a.used[fi];
+    const double nan = __longlong_as_double(0x7ff8000000000000ll);
+    const int64_t node = base + lane;
+    double x[3], up[3];
+    search_node(node, n, x, up);
+    bool vis = node < n;
+    // too few channels: nothing is searched (every node's rms stays NaN)
+    for (unsigned m = __popc(used) >= GPSB200_SEARCH_MIN_CHANNELS ? used : 0u; m; m &= m - 1) {
+        const double *p = a.sat + (fi * 32 + __ffs(m) - 1) * 3;
+        const double l0 = p[0] - x[0], l1 = p[1] - x[1], l2 = p[2] - x[2];
+        vis &= (up[0] * l0 + up[1] * l1 + up[2] * l2) / sqrt(l0 * l0 + l1 * l1 + l2 * l2) >= a.sin_min;
+    }
+    unsigned todo = __ballot_sync(kFull, vis && __popc(used) >= GPSB200_SEARCH_MIN_CHANNELS);
+    if (lane == 0 && todo) atomicAdd(a.searched + fi, __popc(todo));
+    double my_rms = nan;
+    const int64_t s = a.cfg.s0 + fi * a.cfg.step;
+    gpsb200_coarse_config_t ap;
+    ap.t_a = a.sc.t_a;
+    ap.s_a = a.sc.s_a;
+    ap.week = a.sc.week;
+    ap.reserved = 0;
+    for (; todo; todo &= todo - 1) {
+        const int j = __ffs(todo) - 1;
+        for (int i = 0; i < 3; i++) ap.x_a[i] = __shfl_sync(kFull, x[i], j);
+        gpsb200_fix_t f;
+        gpsb200_coarse_t o;
+        double resid;
+        int64_t Nw;
+        bool has;
+        search_solve(a, ap, s, lane, f, o, resid, Nw, has);
+        if (f.status != GPSB200_FIX_OK) continue;
+        if (lane == j) my_rms = f.rms;
+        if (lane == 0) {
+            const int k = atomicAdd(a.nok + fi, 1);
+            if (k < a.max_ok) a.hits[(fi - a.f0) * a.max_ok + k] = SearchHit{f.rms, f.x, f.y, f.z,
+                                                                                              (int32_t) (base + j), 0};
+        }
+    }
+    if (a.node_rms && node < n) a.node_rms[fi * n + node] = my_rms;
+}
+
+// The winner's ordering key (header step 5): rms in whole millimetres, rounded down.
+__device__ inline double rms_key(double rms) { return floor(rms * 1000.0); }
+
+// (key, node) lexicographic minimum over the warp, carrying the list index k; every lane ends with the same triple.
+__device__ inline void warp_argmin_hit(double &key, int &node, int &k) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+        const double okey = __shfl_xor_sync(kFull, key, o);
+        const int onode = __shfl_xor_sync(kFull, node, o), ok = __shfl_xor_sync(kFull, k, o);
+        if (okey < key || (okey == key && onode < node)) {
+            key = okey;
+            node = onode;
+            k = ok;
+        }
+    }
+}
+
+// Header steps 5-6 per fix instant (one warp, lane = channel): the winner and its support from the list, then the
+// winner's coarse solve again for the records. br / ar hold rms_key values.
+__global__ void __launch_bounds__(kWarps * 32) k_search_pick(const SearchArgs a) {
+    const int lane = threadIdx.x & 31;
+    const int64_t local = (int64_t) blockIdx.x * kWarps + (threadIdx.x >> 5);
+    if (local >= a.nf) return;
+    const int64_t fi = a.f0 + local;
+    const double nan = __longlong_as_double(0x7ff8000000000000ll), inf = __longlong_as_double(0x7ff0000000000000ll);
+    const int64_t s = a.cfg.s0 + fi * a.cfg.step;
+    const unsigned used = a.used[fi];
+    const int nused = __popc(used), nok = a.nok[fi];
+    gpsb200_search_t r;
+    r.winner = -1;
+    r.searched = a.searched[fi];
+    r.ok = nok;
+    r.support = 0;
+    r.alt_rms = r.alt_dist = nan;
+    r.reserved = 0;
+    if (nused >= GPSB200_SEARCH_MIN_CHANNELS && nok >= 1 && nok <= a.max_ok) {
+        const SearchHit *h = a.hits + (fi - a.f0) * a.max_ok;
+        double br = inf;
+        int bn = 0x7fffffff, bk = -1;
+        for (int k = lane; k < nok; k += 32)
+            if (rms_key(h[k].rms) < br || (rms_key(h[k].rms) == br && h[k].node < bn)) {
+                br = rms_key(h[k].rms);
+                bn = h[k].node;
+                bk = k;
+            }
+        warp_argmin_hit(br, bn, bk);
+        const double wx = h[bk].x, wy = h[bk].y, wz = h[bk].z;
+        double ar = inf;
+        int an = 0x7fffffff, ak = -1, near = 0;
+        for (int k = lane; k < nok; k += 32) {
+            const double dx = h[k].x - wx, dy = h[k].y - wy, dz = h[k].z - wz;
+            if (sqrt(dx * dx + dy * dy + dz * dz) <= GPSB200_SEARCH_DISTINCT) near++;
+            else if (rms_key(h[k].rms) < ar || (rms_key(h[k].rms) == ar && h[k].node < an)) {
+                ar = rms_key(h[k].rms);
+                an = h[k].node;
+                ak = k;
+            }
+        }
+        warp_argmin_hit(ar, an, ak);
+        r.winner = bn;
+        r.support = __reduce_add_sync(kFull, near);
+        if (ak >= 0) {
+            const double dx = h[ak].x - wx, dy = h[ak].y - wy, dz = h[ak].z - wz;
+            r.alt_rms = h[ak].rms;
+            r.alt_dist = sqrt(dx * dx + dy * dy + dz * dz);
+        }
+    }
+    gpsb200_fix_t f;
+    gpsb200_coarse_t o;
+    double resid = nan;
+    int64_t Nw = -1;
+    bool has = false;
+    if (r.winner >= 0) {
+        gpsb200_coarse_config_t ap;
+        double up[3];
+        search_node(r.winner, a.sc.nodes, ap.x_a, up);
+        ap.t_a = a.sc.t_a;
+        ap.s_a = a.sc.s_a;
+        ap.week = a.sc.week;
+        ap.reserved = 0;
+        search_solve(a, ap, s, lane, f, o, resid, Nw, has);
+        if (!isnan(r.alt_rms)) f.status = GPSB200_FIX_AMBIGUOUS;
+    } else {
+        f.sample = s;
+        f.status = nused < GPSB200_SEARCH_MIN_CHANNELS ? GPSB200_FIX_FEW
+                   : nok > a.max_ok                   ? GPSB200_FIX_AMBIGUOUS
+                                                      : GPSB200_FIX_NO_CONVERGENCE;
+        f.nused = nused;
+        f.mask = used;
+        f.iterations = 0;
+        f.x = f.y = f.z = f.clock_m = f.t_rx = f.vx = f.vy = f.vz = f.drift = nan;
+        f.lat_deg = f.lon_deg = f.height = f.pdop = f.rms = nan;
+        o.delta = o.pdop = nan;
+        o.ref = -1;
+        o.week = -1;
+        o.changed = 0;
+    }
+    r.delta = o.delta;
+    r.pdop = o.pdop;
+    r.ref = o.ref;
+    r.week = o.week;
+    r.changed = o.changed;
+    if (lane == 0) {
+        a.fixes[fi] = f;
+        a.out[fi] = r;
+    }
+    if (a.res && lane < a.nchan) a.res[fi * a.nchan + lane] = has ? resid : nan;
+    if (a.ms && lane < a.nchan) a.ms[fi * a.nchan + lane] = has ? Nw : -1;
+}
+
 template <bool kRaim> void fill(KernelArgs<kRaim> &a, const Scratch &sc);
 template <> void fill<false>(Args &a, const Scratch &sc) {
     a.ep = sc.d_epochs;
@@ -1191,7 +1636,37 @@ template <bool kRaim> cudaError_t launch_as(const Scratch &sc, cudaStream_t s) {
     return cudaGetLastError();
 }
 
+// gpsb200_pvt_search: the satellite table, then the grid and the pick in passes of search_pass(nodes) instants, each
+// pass reusing one OK list of GPSB200_SEARCH_HIT_BYTES at most.
+cudaError_t launch_search(const Scratch &sc, cudaStream_t s) {
+    SearchArgs a;
+    fill<false>(a, sc);
+    a.sc = sc.search_cfg;
+    a.sin_min = std::sin(GPSB200_SEARCH_MIN_ELEV_DEG * (M_PI / 180.0));
+    a.sat = sc.d_sat;
+    a.used = sc.d_used;
+    a.searched = sc.d_searched;
+    a.nok = sc.d_nok;
+    a.hits = reinterpret_cast<SearchHit *>(sc.d_hits);
+    a.node_rms = sc.want_node_rms ? sc.d_node_rms : nullptr;
+    a.out = sc.d_search;
+    a.ms = sc.want_ms ? sc.d_ms : nullptr;
+    a.max_ok = GPSB200_SEARCH_MAX_OK(a.sc.nodes);
+    const unsigned fix_blocks = (unsigned) (((int64_t) sc.cfg.nfix + kWarps - 1) / kWarps);
+    k_search_sats<<<fix_blocks, kWarps * 32, 0, s>>>(a);
+    const unsigned node_blocks = (unsigned) ((a.sc.nodes + kWarps * 32 - 1) / (kWarps * 32));
+    const int per_pass = search_pass(a.sc.nodes);
+    for (int f0 = 0; f0 < sc.cfg.nfix; f0 += per_pass) {
+        a.f0 = f0;
+        a.nf = std::min(per_pass, sc.cfg.nfix - f0);
+        k_pvt_search<<<dim3(node_blocks, (unsigned) a.nf), kWarps * 32, 0, s>>>(a);
+        k_search_pick<<<(unsigned) ((a.nf + kWarps - 1) / kWarps), kWarps * 32, 0, s>>>(a);
+    }
+    return cudaGetLastError();
+}
+
 cudaError_t launch(const Scratch &sc, cudaStream_t s) {
+    if (sc.search) return launch_search(sc, s);
     if (sc.coarse) {
         CoarseArgs a;
         fill<false>(a, sc);
@@ -1220,8 +1695,18 @@ cudaError_t launch(const Scratch &sc, cudaStream_t s) {
 
 std::string check(const gpsb200_pvt_chan_t *chans, int nchan, const gpsb200_track_epoch_t *epochs, const int32_t *nepochs,
                   int max_epochs, const gpsb200_pvt_config_t *cfg, const gpsb200_raim_config_t *raim,
-                  const gpsb200_araim_config_t *araim, const gpsb200_coarse_config_t *coarse) {
+                  const gpsb200_araim_config_t *araim, const gpsb200_coarse_config_t *coarse,
+                  const gpsb200_search_config_t *search) {
     if (!chans || !epochs || !nepochs || !cfg) return "NULL chans, epochs, nepochs or cfg";
+    if (search) {
+        const gpsb200_search_config_t &c = *search;
+        if (!(c.t_a >= 0.0 && c.t_a < 604800.0)) return "search t_a must lie in 0 <= t_a < 604800";
+        if (c.s_a < 0 || c.s_a > (1ll << 62)) return "search s_a outside 0..2^62";
+        if (c.week < 0) return "search week must be >= 0";
+        if (c.nodes < GPSB200_SEARCH_MIN_NODES || c.nodes > GPSB200_SEARCH_MAX_NODES)
+            return "search nodes outside 64..4194304";
+        if (c.reserved != 0) return "search reserved must be 0";
+    }
     if (coarse) {
         const gpsb200_coarse_config_t &c = *coarse;
         for (int i = 0; i < 3; i++)
@@ -1267,7 +1752,7 @@ std::string check(const gpsb200_pvt_chan_t *chans, int nchan, const gpsb200_trac
         const std::string at = "channel " + std::to_string(c) + ": ";
         if (nepochs[c] < 0 || nepochs[c] > max_epochs) return at + "nepochs outside 0..max_epochs";
         if (ch.eph.valid != 0 && ch.eph.valid != 1) return at + "eph.valid must be 0 or 1";
-        if (!ch.eph.valid || coarse) continue;   // never used, or a coarse-time call: its anchor is not read
+        if (!ch.eph.valid || coarse || search) continue;   // never used, or a coarse-time call: no anchor read
         if (ch.anchor_epoch < 0 || ch.anchor_epoch >= nepochs[c]) return at + "anchor_epoch outside the channel's epochs";
         if (ch.anchor_ms < 0 || ch.anchor_ms >= kWeekMs) return at + "anchor_ms outside 0..604799999";
         if (araim && (ch.eph.ura < 0 || ch.eph.ura > 15)) return at + "eph.ura outside 0..15";
@@ -1285,6 +1770,13 @@ void scratch_free(Scratch &sc) {
     cudaFree(sc.d_araim);
     cudaFree(sc.d_coarse);
     cudaFree(sc.d_ms);
+    cudaFree(sc.d_search);
+    cudaFree(sc.d_sat);
+    cudaFree(sc.d_used);
+    cudaFree(sc.d_searched);
+    cudaFree(sc.d_nok);
+    cudaFree(sc.d_hits);
+    cudaFree(sc.d_node_rms);
     sc = Scratch();
 }
 
@@ -1292,7 +1784,8 @@ cudaError_t run(Scratch &sc, const gpsb200_pvt_chan_t *chans, int nchan, const g
                 const int32_t *nepochs, int max_epochs, const gpsb200_pvt_config_t *cfg,
                 const gpsb200_raim_config_t *raim, gpsb200_fix_t *fixes, double *residuals, gpsb200_raim_t *out,
                 cudaStream_t s, const gpsb200_araim_config_t *araim, gpsb200_araim_t *aout,
-                const gpsb200_coarse_config_t *coarse, gpsb200_coarse_t *cout, int64_t *ms) {
+                const gpsb200_coarse_config_t *coarse, gpsb200_coarse_t *cout, int64_t *ms,
+                const gpsb200_search_config_t *search, gpsb200_search_t *sout, double *node_rms) {
     sc.have_last = false;
     if (!sc.d_chans) {
         CU_RET(cudaMalloc(&sc.d_chans, GPSB200_TRK_MAX_CHAN * sizeof(gpsb200_pvt_chan_t)));
@@ -1324,10 +1817,25 @@ cudaError_t run(Scratch &sc, const gpsb200_pvt_chan_t *chans, int nchan, const g
         if (ms) CU_RET(grow(sc.d_ms, sc.ms_cap, (size_t) cfg->nfix * nchan));
         sc.coarse_cfg = *coarse;
     }
+    sc.search = search != nullptr;
+    sc.want_node_rms = node_rms != nullptr;
+    if (search) {
+        const size_t nf = (size_t) cfg->nfix;
+        CU_RET(grow(sc.d_search, sc.search_cap, nf));
+        CU_RET(grow(sc.d_sat, sc.sat_cap, nf * 32 * 3));
+        CU_RET(grow(sc.d_used, sc.used_cap, nf));
+        CU_RET(grow(sc.d_searched, sc.searched_cap, nf));
+        CU_RET(grow(sc.d_nok, sc.nok_cap, nf));
+        const size_t pass = (size_t) std::min<int64_t>(search_pass(search->nodes), cfg->nfix);
+        CU_RET(grow(sc.d_hits, sc.hits_cap, pass * GPSB200_SEARCH_MAX_OK(search->nodes) * sizeof(SearchHit) / sizeof(double)));
+        if (ms) CU_RET(grow(sc.d_ms, sc.ms_cap, nf * nchan));
+        if (node_rms) CU_RET(grow(sc.d_node_rms, sc.node_rms_cap, nf * search->nodes));
+        sc.search_cfg = *search;
+    }
     // the reference channel of the nominal receive time: the lowest with a valid, healthy ephemeris (a coarse-time call
     // has no anchors and no nominal receive time)
     sc.ref = -1;
-    for (int c = 0; c < nchan && sc.ref < 0 && !coarse; c++)
+    for (int c = 0; c < nchan && sc.ref < 0 && !coarse && !search; c++)
         if (chans[c].eph.valid && chans[c].eph.health == 0) sc.ref = c;
     sc.ref_sample = sc.ref >= 0 ? epochs[(size_t) sc.ref * max_epochs + chans[sc.ref].anchor_epoch].sample : 0;
     sc.ref_ms = sc.ref >= 0 ? chans[sc.ref].anchor_ms : 0;
@@ -1354,12 +1862,28 @@ cudaError_t run(Scratch &sc, const gpsb200_pvt_chan_t *chans, int nchan, const g
         if (ms)
             CU_RET(cudaMemcpyAsync(ms, sc.d_ms, (size_t) cfg->nfix * nchan * sizeof(int64_t), cudaMemcpyDeviceToHost, s));
     }
+    if (search) {
+        CU_RET(cudaMemcpyAsync(sout, sc.d_search, (size_t) cfg->nfix * sizeof(gpsb200_search_t), cudaMemcpyDeviceToHost,
+                               s));
+        if (ms)
+            CU_RET(cudaMemcpyAsync(ms, sc.d_ms, (size_t) cfg->nfix * nchan * sizeof(int64_t), cudaMemcpyDeviceToHost, s));
+        if (node_rms)
+            CU_RET(cudaMemcpyAsync(node_rms, sc.d_node_rms, (size_t) cfg->nfix * search->nodes * sizeof(double),
+                                   cudaMemcpyDeviceToHost, s));
+    }
     CU_RET(cudaStreamSynchronize(s));
     sc.have_last = true;
     return cudaSuccess;
 }
 
 cudaError_t replay(Scratch &sc, cudaStream_t s) { return launch(sc, s); }
+
+void search_nodes(int n, double *xyz) {
+    for (int i = 0; i < n; i++) {
+        double up[3];
+        search_node(i, n, xyz + 3 * (size_t) i, up);
+    }
+}
 
 }  // namespace pvt
 }  // namespace gpsb200

@@ -19,11 +19,14 @@ static_assert(sizeof(gpsb200_araim_config_t) == 96, "gpsb200_araim_config_t layo
 static_assert(sizeof(gpsb200_araim_t) == 64, "gpsb200_araim_t layout");
 static_assert(sizeof(gpsb200_coarse_config_t) == 48, "gpsb200_coarse_config_t layout");
 static_assert(sizeof(gpsb200_coarse_t) == 32, "gpsb200_coarse_t layout");
+static_assert(sizeof(gpsb200_search_config_t) == 32, "gpsb200_search_config_t layout");
+static_assert(sizeof(gpsb200_search_t) == 64, "gpsb200_search_t layout");
 
-// Empty when the call is well-formed (see the header). raim, araim and coarse may be NULL; at most one is not.
+// Empty when the call is well-formed (see the header). raim, araim, coarse and search may be NULL; at most one is not.
 std::string check(const gpsb200_pvt_chan_t *chans, int nchan, const gpsb200_track_epoch_t *epochs, const int32_t *nepochs,
                   int max_epochs, const gpsb200_pvt_config_t *cfg, const gpsb200_raim_config_t *raim,
-                  const gpsb200_araim_config_t *araim, const gpsb200_coarse_config_t *coarse = nullptr);
+                  const gpsb200_araim_config_t *araim, const gpsb200_coarse_config_t *coarse = nullptr,
+                  const gpsb200_search_config_t *search = nullptr);
 
 // The RAIM tables of gpsb200_raim_thresholds (raim_thresholds.cpp); false when p_fa or p_md is outside 1e-12..0.5.
 bool raim_thresholds(double p_fa, double p_md, double *T, double *lambda);
@@ -65,21 +68,40 @@ struct Scratch {
     size_t coarse_cap = 0;
     int64_t *d_ms = nullptr;                     // [nfix][nchan]
     size_t ms_cap = 0;
+    // the search of the previous call (gpsb200_pvt_search): records, and the per-instant scratch of pvt.cu's kernels
+    bool search = false, want_node_rms = false;
+    gpsb200_search_config_t search_cfg{};
+    gpsb200_search_t *d_search = nullptr;        // [nfix]
+    size_t search_cap = 0;
+    double *d_sat = nullptr;                     // [nfix][32][3]
+    size_t sat_cap = 0;
+    uint32_t *d_used = nullptr;                  // [nfix]
+    size_t used_cap = 0;
+    int32_t *d_searched = nullptr, *d_nok = nullptr;   // [nfix]
+    size_t searched_cap = 0, nok_cap = 0;
+    double *d_hits = nullptr;                    // one pass's OK-node lists (pvt.cu: SearchHit, search_pass)
+    size_t hits_cap = 0;
+    double *d_node_rms = nullptr;                // [nfix][nodes], only when the caller asks for it
+    size_t node_rms_cap = 0;
 };
 
 void scratch_free(Scratch &sc);
 // Upload, run k_pvt on s and download the fixes (and residuals when not NULL); waits for the results. With raim
 // (not NULL) the kernel's RAIM instantiation runs and out [nfix] receives its records; with araim (not NULL) the ARAIM
 // instantiation and aout [nfix]; with coarse (not NULL) k_pvt_coarse, cout [nfix] and ms [nfix][nchan] (may be NULL).
-// At most one of raim, araim and coarse is not NULL.
+// With search (not NULL) the search kernels, sout [nfix], ms and node_rms [nfix][nodes] (may be NULL). At most one of
+// raim, araim, coarse and search is not NULL.
 cudaError_t run(Scratch &sc, const gpsb200_pvt_chan_t *chans, int nchan, const gpsb200_track_epoch_t *epochs,
                 const int32_t *nepochs, int max_epochs, const gpsb200_pvt_config_t *cfg,
                 const gpsb200_raim_config_t *raim, gpsb200_fix_t *fixes, double *residuals, gpsb200_raim_t *out,
                 cudaStream_t s, const gpsb200_araim_config_t *araim = nullptr, gpsb200_araim_t *aout = nullptr,
                 const gpsb200_coarse_config_t *coarse = nullptr, gpsb200_coarse_t *cout = nullptr,
-                int64_t *ms = nullptr);
+                int64_t *ms = nullptr, const gpsb200_search_config_t *search = nullptr,
+                gpsb200_search_t *sout = nullptr, double *node_rms = nullptr);
 // Enqueue k_pvt again on the previous call's device-resident inputs.
 cudaError_t replay(Scratch &sc, cudaStream_t s);
+// gpsb200_search_nodes: xyz [n][3], the ECEF positions of the n-node search grid.
+void search_nodes(int n, double *xyz);
 
 }  // namespace pvt
 }  // namespace gpsb200

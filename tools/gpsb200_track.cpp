@@ -14,7 +14,9 @@
 // With --assist the fixes are coarse-time fixes (gpsb200_pvt_coarse, DESIGN §11.3): nothing needs to be decoded. The
 // ephemeris comes from a RINEX navigation file (gpsb200_rinex_ephemeris, at the assist time), the a-priori position
 // from --assist-pos and the a-priori time from --assist-time, the GPS time of the first sample after --block /
-// --offset-ms; each line gains delta, the solved a-priori time error in seconds.
+// --offset-ms; each line gains delta, the solved a-priori time error in seconds. With --assist-pos search there is no
+// a-priori position: the fixes come from gpsb200_pvt_search over the default global grid (DESIGN §11.4) and each line
+// gains delta and then support, the number of grid nodes whose solve agreed with the fix.
 #include <algorithm>
 #include <cmath>
 #include <cstdio>
@@ -38,7 +40,7 @@ static void usage() {
             "gpsb200-track FILE [--iq16] [--block B] [--offset-ms N] [--ms K] [--prn LIST] [--threshold R] [--device D]\n"
             "              [--fix [--fix-every MS] [--iono a0,a1,a2,a3,b0,b1,b2,b3] [--raim SIGMA[,P_FA,P_MD[,MAX_EXCLUDE]]]\n"
             "               [--araim MASK_DEG[,SIGMA_URA,SIGMA_URE,B_NOM,P_SAT]]\n"
-            "               [--assist NAV_FILE[,3] --assist-pos LAT,LON,H --assist-time YYYY/MM/DD,hh:mm:ss[.s]]]\n"
+            "               [--assist NAV_FILE[,3] --assist-pos LAT,LON,H|search --assist-time YYYY/MM/DD,hh:mm:ss[.s]]]\n"
             "  FILE              interleaved I,Q at 3 Msps, int8 (default) or int16 (--iq16)\n"
             "  --block B         start at 0.1 s block B (sample 300000 B); --offset-ms N adds N ms (3000 N samples)\n"
             "  --ms K            track K ms of signal from the start (default: to the end of the file)\n"
@@ -51,7 +53,9 @@ static void usage() {
             "  --araim           advanced RAIM with elevation mask MASK_DEG (the other fields: the header's defaults): adds\n"
             "                    the verdict, the excluded PRN, the masked PRNs, HPL/VPL and the EMT to each fix\n"
             "  --assist          coarse-time fixes without decoding: ephemeris from the RINEX file (,3: RINEX 3), a-priori\n"
-            "                    position (deg, deg, m) and GPS time of the first sample; adds delta (s) to each fix\n",
+            "                    position (deg, deg, m) and GPS time of the first sample; adds delta (s) to each fix.\n"
+            "                    --assist-pos search: no a-priori position, a search over a global grid; adds delta (s)\n"
+            "                    and support\n",
             kDefaultThreshold, kDefaultFixEvery);
     exit(2);
 }
@@ -60,13 +64,17 @@ static const char *const kVerdict[] = {"PASS", "EXCLUDED", "ALERT", "UNAVAILABLE
 
 // Fixes from `first` every `step` samples to the last epoch of the channels, one line per fix with status OK; with
 // raim (not NULL) from gpsb200_pvt_raim, with its three columns; with araim (not NULL) from gpsb200_pvt_araim, with its five;
-// with ap (not NULL) from gpsb200_pvt_coarse, with delta.
+// with ap (not NULL) from gpsb200_pvt_coarse, with delta, or with search also set from gpsb200_pvt_search over the default
+// grid (ap's position unused), with delta and support.
 static int print_fixes(gpsb200_ctx_t *ctx, const std::vector<gpsb200_pvt_chan_t> &chans, const std::vector<int> &of,
                        const std::vector<std::vector<gpsb200_track_epoch_t>> &eps, long long first, long long step,
                        gpsb200_pvt_config_t cfg, const gpsb200_raim_config_t *raim,
-                       const gpsb200_araim_config_t *araim, const gpsb200_coarse_config_t *ap) {
+                       const gpsb200_araim_config_t *araim, const gpsb200_coarse_config_t *ap, bool search) {
     const int n = (int) chans.size();
-    if (ap)
+    if (ap && search)
+        printf("# position-search fixes (no a-priori position, %d-node grid): %d channel(s) with an assisted ephemeris, "
+               "Klobuchar %s\n", GPSB200_SEARCH_NODES, n, cfg.iono ? "on" : "off");
+    else if (ap)
         printf("# coarse-time fixes: %d channel(s) with an assisted ephemeris, Klobuchar %s\n", n, cfg.iono ? "on" : "off");
     else
         printf("# fixes: %d channel(s) with an ephemeris and a time anchor decoded, Klobuchar %s\n", n,
@@ -91,8 +99,19 @@ static int print_fixes(gpsb200_ctx_t *ctx, const std::vector<gpsb200_pvt_chan_t>
     std::vector<gpsb200_fix_t> fx(cfg.nfix);
     std::vector<gpsb200_raim_t> rm(raim ? cfg.nfix : 0);
     std::vector<gpsb200_araim_t> am(araim ? cfg.nfix : 0);
-    std::vector<gpsb200_coarse_t> cm(ap ? cfg.nfix : 0);
-    const int rc = ap ? gpsb200_pvt_coarse(ctx, chans.data(), n, all.data(), cnt.data(), (int) me, &cfg, ap, fx.data(),
+    std::vector<gpsb200_coarse_t> cm(ap && !search ? cfg.nfix : 0);
+    std::vector<gpsb200_search_t> sm(ap && search ? cfg.nfix : 0);
+    gpsb200_search_config_t sc;
+    memset(&sc, 0, sizeof sc);
+    if (ap) {
+        sc.t_a = ap->t_a;
+        sc.s_a = ap->s_a;
+        sc.week = ap->week;
+        sc.nodes = GPSB200_SEARCH_NODES;
+    }
+    const int rc = ap && search ? gpsb200_pvt_search(ctx, chans.data(), n, all.data(), cnt.data(), (int) me, &cfg, &sc,
+                                                     fx.data(), nullptr, sm.data(), nullptr, nullptr)
+                   : ap ? gpsb200_pvt_coarse(ctx, chans.data(), n, all.data(), cnt.data(), (int) me, &cfg, ap, fx.data(),
                                            nullptr, cm.data(), nullptr)
                    : araim ? gpsb200_pvt_araim(ctx, chans.data(), n, all.data(), cnt.data(), (int) me, &cfg, araim,
                                              fx.data(), nullptr, am.data())
@@ -102,7 +121,8 @@ static int print_fixes(gpsb200_ctx_t *ctx, const std::vector<gpsb200_pvt_chan_t>
     if (rc != GPSB200_OK) return rc;
     printf("# sample  tow_s  lat_deg  lon_deg  height_m  clock_m  vx  vy  vz (ECEF m/s)  channels  pdop%s\n",
            raim ? "  raim  excluded_prns  hpl/vpl_m"
-                : (araim ? "  araim  excluded_prn  masked_prns  hpl/vpl_m  emt_m" : (ap ? "  delta_s" : "")));
+                : (araim ? "  araim  excluded_prn  masked_prns  hpl/vpl_m  emt_m"
+                         : (ap ? (search ? "  delta_s  support" : "  delta_s") : "")));
     for (int i = 0; i < cfg.nfix; i++) {
         const gpsb200_fix_t &f = fx[i];
         if (f.status != GPSB200_FIX_OK) continue;
@@ -123,7 +143,8 @@ static int print_fixes(gpsb200_ctx_t *ctx, const std::vector<gpsb200_pvt_chan_t>
             printf("  %s  %s  %s  %.2f/%.2f  %.2f", kVerdict[am[i].verdict], ex.empty() ? "-" : ex.c_str(),
                    mk.empty() ? "-" : mk.c_str(), am[i].hpl, am[i].vpl, am[i].emt);
         }
-        if (ap) printf("  %.9f", cm[i].delta);
+        if (ap && search) printf("  %.9f  %d", sm[i].delta, sm[i].support);
+        else if (ap) printf("  %.9f", cm[i].delta);
         printf("\n");
     }
     return GPSB200_OK;
@@ -162,7 +183,7 @@ int main(int argc, char **argv) {
     memset(&acfg, 0, sizeof acfg);
     std::string assist;
     int assist_v3 = 0;
-    bool assist_pos = false, assist_time = false;
+    bool assist_pos = false, assist_time = false, assist_search = false;
     gpsb200_coarse_config_t ap;
     memset(&ap, 0, sizeof ap);
     gpsb200_acq_config_t cfg;
@@ -220,6 +241,9 @@ int main(int argc, char **argv) {
                 assist_v3 = 1;
                 assist.resize(k);
             }
+        } else if (a == "--assist-pos" && i + 1 < argc && std::string(argv[i + 1]) == "search") {
+            i++;
+            assist_pos = assist_search = true;
         } else if (a == "--assist-pos") {
             double llh[3];
             if (sscanf(val(), "%lf,%lf,%lf", &llh[0], &llh[1], &llh[2]) != 3) usage();
@@ -351,7 +375,7 @@ int main(int argc, char **argv) {
         }
     }
     if (fix) rc = print_fixes(ctx, fix_chans, fix_of, eps, s0 + kFixLead, fix_every * GPSB200_ACQ_CODE_SAMPLES, pcfg,
-                              raim ? &rcfg : nullptr, araim ? &acfg : nullptr, coarse ? &ap : nullptr);
+                              raim ? &rcfg : nullptr, araim ? &acfg : nullptr, coarse ? &ap : nullptr, assist_search);
     if (rc != GPSB200_OK) fprintf(stderr, "gpsb200-track: %s\n", gpsb200_last_error(ctx));
     gpsb200_destroy(ctx);
     return rc == GPSB200_OK ? 0 : 1;

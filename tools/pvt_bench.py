@@ -25,8 +25,14 @@ satellite evaluations (Kepler, orbit and clock) per channel and fix they imply -
 prediction, one per iteration and 3 for the ambiguity check for the coarse call -- and the largest difference of the
 coarse fixes from the numpy model (tests/coarse_model.py) over the --check sample.
 
+With --search the same run also times position searches (gpsb200_pvt_search, DESIGN §11.4) on the default grid, at
+2 000 fix instants spread over the run, on the 12 channels with the most epochs and on all 32, the a-priori time 10 s
+late; each alternates with gpsb200_pvt_coarse at the same instants (a-priori position 50 km east, 1 km up) --rounds
+times. Reported: kernel time per fix instant of both arms, the mean nodes searched and OK per instant, the status
+counts, and the largest difference from the numpy model (tests/search_model.py) over --search-check seeded instants.
+
     python tools/pvt_bench.py [--iters 5] [--warmup 1] [--check 64] [--seconds 600] [--raim SIGMA [--fault C]]
-                              [--araim MASK_DEG] [--coarse]
+                              [--araim MASK_DEG] [--coarse] [--search [--search-check 2]]
 """
 import argparse
 import importlib
@@ -183,6 +189,65 @@ def coarse_arms(ctx, stream, chans, eps, packed, n, cfg, args):
     return out
 
 
+def search_arms(ctx, stream, chans, eps, packed, n, iono, args):
+    """Per channel count: kernel time per instant of the coarse and search arms, alternating; counts; model check."""
+    import search_model as SM
+    x0 = PM.llh_ecef(*LOC)
+    lat, lon, _ = PM.ecef_llh(x0)
+    east = np.array([-np.sin(lon), np.cos(lon), 0.0])
+    up = np.array([np.cos(lat) * np.cos(lon), np.cos(lat) * np.sin(lon), np.sin(lat)])
+    ap = gps.coarse_config(x0 + 50e3 * east + 1e3 * up, START_SOW + 10.0, 0, START_WEEK)
+    sc = gps.search_config(START_SOW + 10.0, 0, START_WEEK, gps.SEARCH_NODES)
+    nfix = 2000
+    step = (args.seconds * 3000000 - 6000) // nfix
+    out = {"instants": nfix, "nodes": int(sc["nodes"]), "rounds": args.rounds}
+    for nch in (12, 32):
+        keep = np.sort(np.argsort(-n, kind="stable")[:nch])
+        ch, pk, nn = chans[keep], np.ascontiguousarray(packed[keep]), n[keep]
+        ev = [eps[k] for k in keep]
+        c = gps.pvt_config(3000, step, nfix, iono)
+        arms = {"coarse": lambda: ctx.pvt_coarse(ch, pk, c, ap, nepochs=nn),
+                "search": lambda: ctx.pvt_search(ch, pk, c, sc, want_residuals=True, want_ms=True, nepochs=nn)}
+        times = {k: [] for k in arms}
+        got = {}
+        for _ in range(args.rounds):
+            for k, call in arms.items():
+                got[k] = call()
+                times[k] += replay_ms(ctx, stream, args.iters)
+        fix, rec, res, ms = got["search"]
+        worst = {f: 0.0 for f in ("x", "y", "z", "clock_m", "vx", "vy", "vz", "rms")}
+        worst["delta_s"] = 0.0
+        differ = set()
+        rng = np.random.default_rng(3)
+        for i in rng.choice(nfix, size=min(args.search_check, nfix), replace=False):
+            one = gps.pvt_config(int(c["s0"]) + int(i) * step, 1, 1, iono)
+            want, wrec, _, wms = SM.search(ch, ev, one, sc)
+            if int(want["status"][0]) != int(fix["status"][i]):
+                differ.add("status")
+            if not np.array_equal(wms[0], ms[i]):
+                differ.add("ms")
+            for f in ("winner", "searched", "ok", "support"):
+                if int(wrec[f][0]) != int(rec[f][i]):
+                    differ.add("%s %d/%d" % (f, int(rec[f][i]), int(wrec[f][0])))
+            if rec["winner"][i] >= 0:
+                for f in worst:
+                    a, b = (rec["delta"][i], wrec["delta"][0]) if f == "delta_s" else (fix[f][i], want[f][0])
+                    worst[f] = max(worst[f], abs(float(a) - float(b)))
+        err = np.linalg.norm(np.stack([fix["x"], fix["y"], fix["z"]], 1) - x0, axis=1)
+        t_c, t_s = float(np.median(times["coarse"])), float(np.median(times["search"]))
+        out["ch%d" % nch] = {
+            "coarse_kernel_ms_median": round(t_c, 3), "search_kernel_ms_median": round(t_s, 3),
+            "search_kernel_ms_min": round(float(np.min(times["search"])), 3),
+            "coarse_us_per_instant": round(1e3 * t_c / nfix, 3), "search_ms_per_instant": round(t_s / nfix, 4),
+            "searched_mean": round(float(rec["searched"].mean()), 1), "ok_mean": round(float(rec["ok"].mean()), 2),
+            "ok_max": int(rec["ok"].max()), "support_mean": round(float(rec["support"].mean()), 2),
+            "status_counts": {int(k): int(v) for k, v in zip(*np.unique(fix["status"], return_counts=True))},
+            "max_err_vs_truth_m": round(float(np.nanmax(err)), 4),
+            "checked": min(args.search_check, nfix), "counts_differing_from_model": sorted(differ),
+            "max_abs_diff_vs_model": {k: float("%.3g" % v) for k, v in worst.items()}}
+    return out
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--iters", type=int, default=5)
@@ -194,6 +259,8 @@ def main():
     ap.add_argument("--rounds", type=int, default=3)
     ap.add_argument("--araim", type=float, default=None)
     ap.add_argument("--coarse", action="store_true")
+    ap.add_argument("--search", action="store_true")
+    ap.add_argument("--search-check", type=int, default=2)
     args = ap.parse_args()
     import torch
     if not torch.cuda.is_available():
@@ -230,6 +297,7 @@ def main():
             kern.append(a.elapsed_time(b))
         raim = raim_arms(ctx, stream, chans, packed, n, cfg, args) if args.raim is not None else None
         coarse = coarse_arms(ctx, stream, chans, eps, packed, n, cfg, args) if args.coarse else None
+        search = search_arms(ctx, stream, chans, eps, packed, n, iono, args) if args.search else None
     rng = np.random.default_rng(1)
     worst = {f: 0.0 for f in ("x", "y", "z", "clock_m", "vx", "vy", "vz")}
     for i in rng.choice(nfix, size=min(args.check, nfix), replace=False):
@@ -249,7 +317,8 @@ def main():
                       "status_counts": st, "checked": min(args.check, nfix),
                       "max_abs_diff_vs_model": {k: float("%.3g" % v) for k, v in worst.items()},
                       **({"raim": raim} if raim is not None else {}),
-                      **({"coarse": coarse} if coarse is not None else {})}), flush=True)
+                      **({"coarse": coarse} if coarse is not None else {}),
+                      **({"search": search} if search is not None else {})}), flush=True)
 
 
 if __name__ == "__main__":
