@@ -1139,23 +1139,18 @@ int track(gpsb200_ctx *ctx, const void *iq, int64_t nsamples, int sample_size, i
     return GPSB200_OK;
 }
 
-// Position fixes (pvt.cu), with the RAIM stage when raim is not NULL, the ARAIM stage when araim is not NULL, coarse-time
-// fixes when coarse is not NULL, searches when search is not NULL. Everything is checked before anything is enqueued.
+// Position fixes (pvt.cu), with the stage st names (none: plain fixes). Everything is checked before anything is
+// enqueued.
 int pvt_fix(gpsb200_ctx *ctx, const char *fn, const gpsb200_pvt_chan_t *chans, int nchan,
             const gpsb200_track_epoch_t *epochs, const int32_t *nepochs, int max_epochs, const gpsb200_pvt_config_t *cfg,
-            const gpsb200_raim_config_t *raim, gpsb200_fix_t *fixes, double *residuals, gpsb200_raim_t *out,
-            const gpsb200_araim_config_t *araim = nullptr, gpsb200_araim_t *aout = nullptr,
-            const gpsb200_coarse_config_t *coarse = nullptr, gpsb200_coarse_t *cout = nullptr, int64_t *ms = nullptr,
-            const gpsb200_search_config_t *search = nullptr, gpsb200_search_t *sout = nullptr,
-            double *node_rms = nullptr) {
+            gpsb200_fix_t *fixes, double *residuals, const pvt::Stage &st) {
     const std::string at = std::string(fn) + ": ";
     if (!fixes) return fail(ctx, GPSB200_ERR_ARG, at + "NULL fixes");
-    const std::string bad = pvt::check(chans, nchan, epochs, nepochs, max_epochs, cfg, raim, araim, coarse, search);
+    const std::string bad = pvt::check(chans, nchan, epochs, nepochs, max_epochs, cfg, st);
     if (!bad.empty()) return fail(ctx, GPSB200_ERR_ARG, at + bad);
     const int rc = check_entry(ctx);
     if (rc) return rc;
-    CU(pvt::run(ctx->pvt, chans, nchan, epochs, nepochs, max_epochs, cfg, raim, fixes, residuals, out, ctx->s_compute,
-                araim, aout, coarse, cout, ms, search, sout, node_rms));
+    CU(pvt::run(ctx->pvt, chans, nchan, epochs, nepochs, max_epochs, cfg, fixes, residuals, st, ctx->s_compute));
     return GPSB200_OK;
 }
 
@@ -1735,8 +1730,8 @@ int gpsb200_pvt(gpsb200_ctx_t *ctx, const gpsb200_pvt_chan_t *chans, int nchan, 
                 const int32_t *nepochs, int max_epochs, const gpsb200_pvt_config_t *cfg, gpsb200_fix_t *fixes,
                 double *residuals) {
     if (!ctx) return GPSB200_ERR_ARG;
-    return settle(ctx, nullptr, pvt_fix(ctx, "gpsb200_pvt", chans, nchan, epochs, nepochs, max_epochs, cfg, nullptr, fixes,
-                                        residuals, nullptr));
+    return settle(ctx, nullptr, pvt_fix(ctx, "gpsb200_pvt", chans, nchan, epochs, nepochs, max_epochs, cfg, fixes,
+                                        residuals, pvt::Stage()));
 }
 
 int gpsb200_pvt_raim(gpsb200_ctx_t *ctx, const gpsb200_pvt_chan_t *chans, int nchan, const gpsb200_track_epoch_t *epochs,
@@ -1744,8 +1739,11 @@ int gpsb200_pvt_raim(gpsb200_ctx_t *ctx, const gpsb200_pvt_chan_t *chans, int nc
                      const gpsb200_raim_config_t *raim, gpsb200_fix_t *fixes, double *residuals, gpsb200_raim_t *out) {
     if (!ctx) return GPSB200_ERR_ARG;
     if (!raim || !out) return settle(ctx, nullptr, fail(ctx, GPSB200_ERR_ARG, "gpsb200_pvt_raim: NULL raim or out"));
-    return settle(ctx, nullptr, pvt_fix(ctx, "gpsb200_pvt_raim", chans, nchan, epochs, nepochs, max_epochs, cfg, raim,
-                                        fixes, residuals, out));
+    pvt::Stage st;
+    st.raim = raim;
+    st.raim_out = out;
+    return settle(ctx, nullptr, pvt_fix(ctx, "gpsb200_pvt_raim", chans, nchan, epochs, nepochs, max_epochs, cfg, fixes,
+                                        residuals, st));
 }
 
 int gpsb200_pvt_araim(gpsb200_ctx_t *ctx, const gpsb200_pvt_chan_t *chans, int nchan, const gpsb200_track_epoch_t *epochs,
@@ -1754,8 +1752,11 @@ int gpsb200_pvt_araim(gpsb200_ctx_t *ctx, const gpsb200_pvt_chan_t *chans, int n
                       gpsb200_araim_t *out) {
     if (!ctx) return GPSB200_ERR_ARG;
     if (!araim || !out) return settle(ctx, nullptr, fail(ctx, GPSB200_ERR_ARG, "gpsb200_pvt_araim: NULL araim or out"));
-    return settle(ctx, nullptr, pvt_fix(ctx, "gpsb200_pvt_araim", chans, nchan, epochs, nepochs, max_epochs, cfg, nullptr,
-                                        fixes, residuals, nullptr, araim, out));
+    pvt::Stage st;
+    st.araim = araim;
+    st.araim_out = out;
+    return settle(ctx, nullptr, pvt_fix(ctx, "gpsb200_pvt_araim", chans, nchan, epochs, nepochs, max_epochs, cfg, fixes,
+                                        residuals, st));
 }
 
 int gpsb200_pvt_coarse(gpsb200_ctx_t *ctx, const gpsb200_pvt_chan_t *chans, int nchan,
@@ -1765,8 +1766,12 @@ int gpsb200_pvt_coarse(gpsb200_ctx_t *ctx, const gpsb200_pvt_chan_t *chans, int 
     if (!ctx) return GPSB200_ERR_ARG;
     if (!apriori || !out)
         return settle(ctx, nullptr, fail(ctx, GPSB200_ERR_ARG, "gpsb200_pvt_coarse: NULL apriori or out"));
-    return settle(ctx, nullptr, pvt_fix(ctx, "gpsb200_pvt_coarse", chans, nchan, epochs, nepochs, max_epochs, cfg, nullptr,
-                                        fixes, residuals, nullptr, nullptr, nullptr, apriori, out, ms));
+    pvt::Stage st;
+    st.coarse = apriori;
+    st.coarse_out = out;
+    st.ms = ms;
+    return settle(ctx, nullptr, pvt_fix(ctx, "gpsb200_pvt_coarse", chans, nchan, epochs, nepochs, max_epochs, cfg, fixes,
+                                        residuals, st));
 }
 
 int gpsb200_pvt_search(gpsb200_ctx_t *ctx, const gpsb200_pvt_chan_t *chans, int nchan,
@@ -1776,9 +1781,13 @@ int gpsb200_pvt_search(gpsb200_ctx_t *ctx, const gpsb200_pvt_chan_t *chans, int 
     if (!ctx) return GPSB200_ERR_ARG;
     if (!search || !out)
         return settle(ctx, nullptr, fail(ctx, GPSB200_ERR_ARG, "gpsb200_pvt_search: NULL search or out"));
-    return settle(ctx, nullptr, pvt_fix(ctx, "gpsb200_pvt_search", chans, nchan, epochs, nepochs, max_epochs, cfg, nullptr,
-                                        fixes, residuals, nullptr, nullptr, nullptr, nullptr, nullptr, ms, search, out,
-                                        node_rms));
+    pvt::Stage st;
+    st.search = search;
+    st.search_out = out;
+    st.ms = ms;
+    st.node_rms = node_rms;
+    return settle(ctx, nullptr, pvt_fix(ctx, "gpsb200_pvt_search", chans, nchan, epochs, nepochs, max_epochs, cfg, fixes,
+                                        residuals, st));
 }
 
 int gpsb200_search_nodes(int n, double *xyz) {

@@ -92,22 +92,36 @@ __device__ inline void warp_argmax(double &v, int &j) {
     }
 }
 
-// Cholesky solve of the symmetric 4 x 4 system N x = b, N packed as n00 n01 n02 n03 n11 n12 n13 n22 n23 n33.
-// false when N is not positive definite.
-struct Chol {
-    double l[4][4];
-    __device__ bool factor(const double *N) {
-        const double a[4][4] = {{N[0], N[1], N[2], N[3]}, {N[1], N[4], N[5], N[6]}, {N[2], N[5], N[7], N[8]},
-                                {N[3], N[6], N[8], N[9]}};
+// Cholesky solve of the symmetric N x N system, packed as its upper triangle row by row (N = 4: n00 n01 n02 n03 n11 n12
+// n13 n22 n23 n33). factor is false when the system is not positive definite. solve<n> uses the leading n x n block,
+// whose factor is the leading block of the whole factor.
+template <int N> struct Chol {
+    double l[N][N];
+    __device__ bool factor(const double *P) {
+        double a[N][N];
+        if constexpr (N == 4) {
+            // Loaded by the loop below, the 4 x 4 system moved the register allocation of k_pvt's RAIM instantiation:
+            // 17.62-17.74 ms against 17.46-17.57 ms (tools/pvt_bench.py --raim, H100 80GB HBM3, 700 W).
+            const double b[4][4] = {{P[0], P[1], P[2], P[3]}, {P[1], P[4], P[5], P[6]}, {P[2], P[5], P[7], P[8]},
+                                    {P[3], P[6], P[8], P[9]}};
+            for (int i = 0; i < 4; i++)
+                for (int j = 0; j < 4; j++) a[i][j] = b[i][j];
+        } else {
+            int t = 0;
 #pragma unroll
-        for (int j = 0; j < 4; j++) {
+            for (int i = 0; i < N; i++)
+#pragma unroll
+                for (int j = i; j < N; j++) a[i][j] = a[j][i] = P[t++];
+        }
+#pragma unroll
+        for (int j = 0; j < N; j++) {
             double d = a[j][j];
 #pragma unroll
             for (int k = 0; k < j; k++) d -= l[j][k] * l[j][k];
             if (!(d > 0.0)) return false;
             l[j][j] = sqrt(d);
 #pragma unroll
-            for (int i = j + 1; i < 4; i++) {
+            for (int i = j + 1; i < N; i++) {
                 double v = a[i][j];
 #pragma unroll
                 for (int k = 0; k < j; k++) v -= l[i][k] * l[j][k];
@@ -116,20 +130,20 @@ struct Chol {
         }
         return true;
     }
-    __device__ void solve(const double *b, double *x) const {
-        double y[4];
+    template <int n = N> __device__ void solve(const double *b, double *x) const {
+        double y[n];
 #pragma unroll
-        for (int i = 0; i < 4; i++) {
+        for (int i = 0; i < n; i++) {
             double v = b[i];
 #pragma unroll
             for (int k = 0; k < i; k++) v -= l[i][k] * y[k];
             y[i] = v / l[i][i];
         }
 #pragma unroll
-        for (int i = 3; i >= 0; i--) {
+        for (int i = n - 1; i >= 0; i--) {
             double v = y[i];
 #pragma unroll
-            for (int k = i + 1; k < 4; k++) v -= l[k][i] * x[k];
+            for (int k = i + 1; k < n; k++) v -= l[k][i] * x[k];
             x[i] = v / l[i][i];
         }
     }
@@ -258,6 +272,134 @@ __device__ int find_period(const gpsb200_track_epoch_t *e, int n, int64_t s) {
     return -1;
 }
 
+// The eligibility test of a lane's channel at sample s: a valid, healthy ephemeris and a code period k >= 1 holding s
+// whose two epochs are locked. Returns k, with the code phase at s (frac, ms) and the range rate (m/s) of that period;
+// -1 when the channel fails the test.
+__device__ __forceinline__ int locked_period(const Args &a, int lane, int64_t s, double &frac, double &rate) {
+    const gpsb200_pvt_chan_t &c = a.ch[lane];
+    const gpsb200_track_epoch_t *e = a.ep + (size_t) lane * a.max_epochs;
+    const int k = c.eph.valid && c.eph.health == 0 ? find_period(e, a.n[lane], s) : -1;
+    if (!(k >= 1 && e[k - 1].lock && e[k].lock)) return -1;
+    const uint64_t phi = (uint64_t) e[k - 1].code_phase + (uint64_t) (s - e[k].sample) * e[k - 1].code_step;
+    frac = (double) phi / kCodeMod;
+    rate = -kLambda * ((double) e[k - 1].carr_step * kStepHz);
+    return k;
+}
+
+// The measurement of a lane's channel at sample s for a fix with the time anchor (DESIGN §11): q whole ms and m samples
+// after the reference channel's anchor, the pseudorange rho, the range rate and the satellite (position, velocity,
+// clock offset and drift) at its transmit time. false, with nothing written, when the channel fails locked_period (or,
+// with ura, has URA index 15) or the transmit time lies more than 2 h from toe.
+__device__ __forceinline__ bool measure(const Args &a, int lane, int64_t s, int64_t q, int64_t m, bool ura, double &rho,
+                                        double &rate, double *p, double *v, double &dtsv, double &ddtsv) {
+    if (lane >= a.nchan || a.ref < 0) return false;
+    const gpsb200_pvt_chan_t &c = a.ch[lane];
+    if (ura && !(c.eph.ura >= 0 && c.eph.ura < 15)) return false;
+    double frac, rt;
+    const int k = locked_period(a, lane, s, frac, rt);
+    if (k < 1) return false;
+    const int64_t T = (((c.anchor_ms + k - c.anchor_epoch) % kWeekMs) + kWeekMs) % kWeekMs;
+    const double tsv = (double) T * 1e-3 + frac * 1e-3;
+    if (!(fabs(wrap_half_week(tsv - c.eph.toe)) <= 7200.0)) return false;
+    int64_t D = (a.ref_ms + 75 + q - T) % kWeekMs;
+    D = D >= kWeekMs / 2 ? D - kWeekMs : (D < -kWeekMs / 2 ? D + kWeekMs : D);
+    rho = (double) D * kCms + ((double) m / 3000.0 - frac) * kCms;
+    rate = rt;
+    const double d0 = wrap_half_week(tsv - c.eph.toc);
+    const double tt = tsv - (c.eph.af0 + d0 * (c.eph.af1 + d0 * c.eph.af2));
+    satellite(c.eph, tt, p, v, dtsv, ddtsv);
+    return true;
+}
+
+// The geodetic frame at an ECEF point: latitude and longitude (rad) and their sines and cosines; all 0 until set.
+struct Geo {
+    double lat = 0.0, lon = 0.0, sla = 0.0, cla = 0.0, slo = 0.0, clo = 0.0;
+    __device__ void set(const double *x) {
+        double hgt;
+        ecef_llh(x, lat, lon, hgt);
+        sincos(lat, &sla, &cla);
+        sincos(lon, &slo, &clo);
+    }
+};
+
+// A lane's row at the estimate X: the satellite at p, v (ECEF at its transmit time) turned by the Earth's rotation over
+// the flight time. Gives the line of sight l, its length R and the turned velocity pv; with enu, also l's azimuth and
+// elevation in the frame g (az and el are left as they are without).
+__device__ __forceinline__ void sight(const double *p, const double *v, const double *X, const Geo &g, bool enu,
+                                      double *l, double &R, double *pv, double &az, double &el) {
+    const double g0 = p[0] - X[0], g1 = p[1] - X[1], g2 = p[2] - X[2];
+    const double tau = sqrt(g0 * g0 + g1 * g1 + g2 * g2) / kC;
+    double sth, cth;
+    sincos(kOmegaE * tau, &sth, &cth);
+    const double px = p[0] * cth + p[1] * sth, py = p[1] * cth - p[0] * sth;
+    pv[0] = v[0] * cth + v[1] * sth;
+    pv[1] = v[1] * cth - v[0] * sth;
+    pv[2] = v[2];
+    l[0] = px - X[0];
+    l[1] = py - X[1];
+    l[2] = p[2] - X[2];
+    R = sqrt(l[0] * l[0] + l[1] * l[1] + l[2] * l[2]);
+    if (enu) {
+        const double nn = -g.sla * g.clo * l[0] - g.sla * g.slo * l[1] + g.cla * l[2];
+        const double ee = -g.slo * l[0] + g.clo * l[1];
+        const double uu = g.cla * g.clo * l[0] + g.cla * g.slo * l[1] + g.sla * l[2];
+        az = atan2(ee, nn);
+        if (az < 0.0) az += 2.0 * kPi;
+        el = atan2(uu, sqrt(nn * nn + ee * ee));
+    }
+}
+
+// The record of a fix instant before its solve, and of one without a fix: NaN fields, the status and the channels used.
+__device__ inline void no_fix(gpsb200_fix_t &f, int64_t s, int nused, unsigned mask, int status) {
+    const double nan = __longlong_as_double(0x7ff8000000000000ll);
+    f.sample = s;
+    f.nused = nused;
+    f.mask = mask;
+    f.iterations = 0;
+    f.status = status;
+    f.x = f.y = f.z = f.clock_m = f.t_rx = f.vx = f.vy = f.vz = f.drift = nan;
+    f.lat_deg = f.lon_deg = f.height = f.pdop = f.rms = nan;
+}
+
+// The record of a converged fix X (position and clock first), ch the factor of its last iteration and trx its receive
+// time before the fold into the week: velocity and drift on the rows h of the lanes in use, y weighted by wy; PDOP; the
+// rms of the post-fit residuals resid; latitude / longitude (also returned, rad) and height.
+template <int N>
+__device__ __forceinline__ void finish(const Chol<N> &ch, const double *X, double trx, bool use, const double *h,
+                                       const double *pv, double rate, double ddtsv, double wy, double resid, int nused,
+                                       gpsb200_fix_t &f, double &lat, double &lon) {
+    const double y = use ? (rate + kC * ddtsv + (h[0] * pv[0] + h[1] * pv[1] + h[2] * pv[2])) * wy : 0.0;
+    const double bv[4] = {warp_sum(h[0] * y), warp_sum(h[1] * y), warp_sum(h[2] * y), warp_sum(y)};
+    double V[4];
+    ch.template solve<4>(bv, V);
+    const double ss = warp_sum(use ? resid * resid : 0.0);
+    double Q[3];
+#pragma unroll
+    for (int i = 0; i < 3; i++) {
+        double ei[N] = {}, xi[N];
+        ei[i] = 1.0;
+        ch.solve(ei, xi);
+        Q[i] = xi[i];
+    }
+    f.status = GPSB200_FIX_OK;
+    f.x = X[0];
+    f.y = X[1];
+    f.z = X[2];
+    f.clock_m = X[3];
+    f.t_rx = trx < 0.0 ? trx + 604800.0 : (trx >= 604800.0 ? trx - 604800.0 : trx);
+    f.vx = V[0];
+    f.vy = V[1];
+    f.vz = V[2];
+    f.drift = V[3];
+    double hgt;
+    ecef_llh(X, lat, lon, hgt);
+    f.lat_deg = lat * (180.0 / M_PI);
+    f.lon_deg = lon * (180.0 / M_PI);
+    f.height = hgt;
+    f.pdop = sqrt(Q[0] + Q[1] + Q[2]);
+    f.rms = sqrt(ss / (double) nused);
+}
+
 // ---- ARAIM (DESIGN §11.2) --------------------------------------------------------------------------------------------
 __device__ inline double q_tail(double x) { return 0.5 * erfc(x / M_SQRT2); }          // the standard normal upper tail
 __device__ inline double q_inv(double p) { return M_SQRT2 * erfcinv(2.0 * p); }
@@ -276,18 +418,17 @@ struct Ss {
 // subset solutions come from N_k = N - w_k g_k g_k^T, which each lane factors itself; the sums over the other channels'
 // rows run in one loop over the lanes (__shfl_sync), O(n^2) per fix. Returns sigma_acc,U.
 __device__ double mhss(const AraimArgs &a, bool use, int n, const double *h, double sw, double r, double acc2,
-                       const double *N, const Chol &ch, const double *X, Ss &o) {
+                       const double *N, const Chol<4> &ch, const double *X, Ss &o) {
     const int lane = threadIdx.x & 31;
-    double lat, lon, hgt, sla, cla, slo, clo;
-    ecef_llh(X, lat, lon, hgt);
-    sincos(lat, &sla, &cla);
-    sincos(lon, &slo, &clo);
-    const double u[3][3] = {{-slo, clo, 0.0}, {-sla * clo, -sla * slo, cla}, {cla * clo, cla * slo, sla}};
+    Geo g;
+    g.set(X);
+    const double u[3][3] = {{-g.slo, g.clo, 0.0}, {-g.sla * g.clo, -g.sla * g.slo, g.cla},
+                            {g.cla * g.clo, g.cla * g.slo, g.sla}};
     // the normal matrix less this lane's row
     const double w0 = use ? h[0] * sw : 0.0, w1 = use ? h[1] * sw : 0.0, w2 = use ? h[2] * sw : 0.0, wc = use ? sw : 0.0;
     const double Nk[10] = {N[0] - w0 * w0, N[1] - w0 * w1, N[2] - w0 * w2, N[3] - w0 * wc, N[4] - w1 * w1,
                            N[5] - w1 * w2, N[6] - w1 * wc, N[7] - w2 * w2, N[8] - w2 * wc, N[9] - wc * wc};
-    Chol ck;
+    Chol<4> ck;
     const bool fk = use && ck.factor(Nk);
     o.pd = !use || fk;
     double z[3][4], z0[3][4];   // N_k^-1 u_q and N^-1 u_q
@@ -374,7 +515,7 @@ __device__ double p_not_monitored(double p, int n) {
 // measurement) and `use` (in the solve). An excluded lane still evaluates its row every iteration, with weight 0, so the
 // same warp sums serve every pass, and its residual against the final fix comes out of the same formula. The RAIM
 // instantiation is held to 128 registers (4 CTAs per SM, as the plain one) at the price of some spills: at its natural
-// 160 it ran 3 CTAs per SM and 15 % slower. The plain one keeps its bounds and instructions (DESIGN §11.1).
+// 160 it ran 3 CTAs per SM and 15 % slower (DESIGN §11.1).
 template <bool kRaim>
 __global__ void __launch_bounds__(kWarps * 32, kRaim ? 4 : 0) k_pvt(const KernelArgs<kRaim> a) {
     const int lane = threadIdx.x & 31;
@@ -384,44 +525,17 @@ __global__ void __launch_bounds__(kWarps * 32, kRaim ? 4 : 0) k_pvt(const Kernel
     const double nan = __longlong_as_double(0x7ff8000000000000ll);
 
     // ---- the measurement of this lane's channel (integers), its satellite (FP64) ----
-    bool use = false;
     double rho = 0.0, rate = 0.0, dtsv = 0.0, ddtsv = 0.0, p[3] = {0, 0, 0}, v[3] = {0, 0, 0};
     // the nominal receive time: whole ms of week and the sub-ms sample offset from the reference channel's anchor
     const int64_t ds = s - a.ref_sample;
     const int64_t q = floor_div(ds, 3000), m = ds - 3000 * q;
     const int64_t nom_ms = (((a.ref_ms + 75 + q) % kWeekMs) + kWeekMs) % kWeekMs;
-    if (lane < a.nchan && a.ref >= 0) {
-        const gpsb200_pvt_chan_t &c = a.ch[lane];
-        const gpsb200_track_epoch_t *e = a.ep + (size_t) lane * a.max_epochs;
-        const int k = c.eph.valid && c.eph.health == 0 ? find_period(e, a.n[lane], s) : -1;
-        if (k >= 1 && e[k - 1].lock && e[k].lock) {
-            const uint64_t phi = (uint64_t) e[k - 1].code_phase + (uint64_t) (s - e[k].sample) * e[k - 1].code_step;
-            const int64_t T = (((c.anchor_ms + k - c.anchor_epoch) % kWeekMs) + kWeekMs) % kWeekMs;
-            const double frac = (double) phi / kCodeMod;               // ms
-            const double tsv = (double) T * 1e-3 + frac * 1e-3;
-            if (fabs(wrap_half_week(tsv - c.eph.toe)) <= 7200.0) {
-                use = true;
-                int64_t D = (a.ref_ms + 75 + q - T) % kWeekMs;
-                D = D >= kWeekMs / 2 ? D - kWeekMs : (D < -kWeekMs / 2 ? D + kWeekMs : D);
-                rho = (double) D * kCms + ((double) m / 3000.0 - frac) * kCms;
-                rate = -kLambda * ((double) e[k - 1].carr_step * kStepHz);
-                const double d0 = wrap_half_week(tsv - c.eph.toc);
-                const double tt = tsv - (c.eph.af0 + d0 * (c.eph.af1 + d0 * c.eph.af2));
-                satellite(c.eph, tt, p, v, dtsv, ddtsv);
-            }
-        }
-    }
+    bool use = measure(a, lane, s, q, m, false, rho, rate, p, v, dtsv, ddtsv);
     const bool has = use;
     unsigned mask = __ballot_sync(kFull, use);
     int nused = __popc(mask);
     gpsb200_fix_t f;
-    f.sample = s;
-    f.nused = nused;
-    f.mask = mask;
-    f.iterations = 0;
-    f.status = nused < 4 ? GPSB200_FIX_FEW : GPSB200_FIX_NO_CONVERGENCE;
-    f.x = f.y = f.z = f.clock_m = f.t_rx = f.vx = f.vy = f.vz = f.drift = nan;
-    f.lat_deg = f.lon_deg = f.height = f.pdop = f.rms = nan;
+    no_fix(f, s, nused, mask, nused < 4 ? GPSB200_FIX_FEW : GPSB200_FIX_NO_CONVERGENCE);
     double resid = nan;
     // RAIM: the record, and this lane's N^-1 g (position part) and 1 - h_jj of the last pass
     int verdict = GPSB200_RAIM_UNAVAILABLE, dof = 0;
@@ -430,7 +544,7 @@ __global__ void __launch_bounds__(kWarps * 32, kRaim ? 4 : 0) k_pvt(const Kernel
     if (nused >= 4) {
         double X[4] = {0.0, 0.0, 0.0, 0.0};
         double h[3] = {0, 0, 0}, r = 0.0, pr_v[3] = {0, 0, 0};
-        Chol ch;
+        Chol<4> ch;
         bool ok = false;
         double dX[4] = {0, 0, 0, 0};
         int it0 = 0;   // iterations of the earlier passes
@@ -440,40 +554,19 @@ __global__ void __launch_bounds__(kWarps * 32, kRaim ? 4 : 0) k_pvt(const Kernel
         for (int j = 0; j < GPSB200_PVT_MAX_ITER; j++) {
             const double rad = sqrt(X[0] * X[0] + X[1] * X[1] + X[2] * X[2]);
             const bool iono = a.cfg.iono && rad >= kIonoMinRadius;
-            double lat = 0.0, lon = 0.0, hgt = 0.0, sla = 0.0, cla = 0.0, slo = 0.0, clo = 0.0;
-            if (iono) {
-                ecef_llh(X, lat, lon, hgt);
-                sincos(lat, &sla, &cla);
-                sincos(lon, &slo, &clo);
-            }
+            Geo g;
+            if (iono) g.set(X);
             h[0] = h[1] = h[2] = 0.0;
             r = 0.0;
             if (has) {
-                const double g0 = p[0] - X[0], g1 = p[1] - X[1], g2 = p[2] - X[2];
-                const double tau = sqrt(g0 * g0 + g1 * g1 + g2 * g2) / kC;
-                double sth, cth;
-                sincos(kOmegaE * tau, &sth, &cth);
-                const double px = p[0] * cth + p[1] * sth, py = p[1] * cth - p[0] * sth;
-                pr_v[0] = v[0] * cth + v[1] * sth;
-                pr_v[1] = v[1] * cth - v[0] * sth;
-                pr_v[2] = v[2];
-                const double l0 = px - X[0], l1 = py - X[1], l2 = p[2] - X[2];
-                const double R = sqrt(l0 * l0 + l1 * l1 + l2 * l2);
-                double I = 0.0;
-                if (iono) {
-                    const double nn = -sla * clo * l0 - sla * slo * l1 + cla * l2;
-                    const double ee = -slo * l0 + clo * l1;
-                    const double uu = cla * clo * l0 + cla * slo * l1 + sla * l2;
-                    double az = atan2(ee, nn);
-                    if (az < 0.0) az += 2.0 * kPi;
-                    const double el = atan2(uu, sqrt(nn * nn + ee * ee));
-                    const double trx = (double) nom_ms * 1e-3 + (double) m / 3e6 - X[3] / kC;
-                    I = klobuchar(a.cfg, lat, lon, az, el, trx);
-                }
+                double l[3], R, az = 0.0, el = 0.0, I = 0.0;
+                sight(p, v, X, g, iono, l, R, pr_v, az, el);
+                if (iono)
+                    I = klobuchar(a.cfg, g.lat, g.lon, az, el, (double) nom_ms * 1e-3 + (double) m / 3e6 - X[3] / kC);
                 r = rho - (R + X[3] - kC * dtsv + I);
-                h[0] = -l0 / R;
-                h[1] = -l1 / R;
-                h[2] = -l2 / R;
+                h[0] = -l[0] / R;
+                h[1] = -l[1] / R;
+                h[2] = -l[2] / R;
             }
             // an excluded lane's row enters with weight 0
             const double w0 = kRaim && !use ? 0.0 : h[0], w1 = kRaim && !use ? 0.0 : h[1], w2 = kRaim && !use ? 0.0 : h[2];
@@ -535,37 +628,9 @@ __global__ void __launch_bounds__(kWarps * 32, kRaim ? 4 : 0) k_pvt(const Kernel
         if (ok) {
             // post-fit residuals of the last iteration, velocity and drift on the same rows
             if (has) resid = r - (h[0] * dX[0] + h[1] * dX[1] + h[2] * dX[2] + dX[3]);
-            const double y = use ? rate + kC * ddtsv + (h[0] * pr_v[0] + h[1] * pr_v[1] + h[2] * pr_v[2]) : 0.0;
-            const double bv[4] = {warp_sum(h[0] * y), warp_sum(h[1] * y), warp_sum(h[2] * y), warp_sum(y)};
-            double V[4];
-            ch.solve(bv, V);
-            const double ss = warp_sum(use ? resid * resid : 0.0);
-            double Q[3];
-#pragma unroll
-            for (int i = 0; i < 3; i++) {
-                double ei[4] = {0, 0, 0, 0}, xi[4];
-                ei[i] = 1.0;
-                ch.solve(ei, xi);
-                Q[i] = xi[i];
-            }
-            f.status = GPSB200_FIX_OK;
-            f.x = X[0];
-            f.y = X[1];
-            f.z = X[2];
-            f.clock_m = X[3];
-            double trx = (double) nom_ms * 1e-3 + ((double) m / 3e6 - X[3] / kC);
-            f.t_rx = trx < 0.0 ? trx + 604800.0 : (trx >= 604800.0 ? trx - 604800.0 : trx);
-            f.vx = V[0];
-            f.vy = V[1];
-            f.vz = V[2];
-            f.drift = V[3];
-            double lat, lon, hgt;
-            ecef_llh(X, lat, lon, hgt);
-            f.lat_deg = lat * (180.0 / M_PI);
-            f.lon_deg = lon * (180.0 / M_PI);
-            f.height = hgt;
-            f.pdop = sqrt(Q[0] + Q[1] + Q[2]);
-            f.rms = sqrt(ss / (double) nused);
+            double lat, lon;
+            finish(ch, X, (double) nom_ms * 1e-3 + ((double) m / 3e6 - X[3] / kC), use, h, pr_v, rate, ddtsv, 1.0,
+                   resid, nused, f, lat, lon);
             if constexpr (kRaim) {
                 if (verdict != GPSB200_RAIM_UNAVAILABLE) {
                     // Brown's slopes: N^-1 g in east / north / up at the fix
@@ -604,11 +669,11 @@ __global__ void __launch_bounds__(kWarps * 32, kRaim ? 4 : 0) k_pvt(const Kernel
     }
 }
 
-// k_pvt_araim: gpsb200_pvt_araim (DESIGN §11.2). The measurement and the Gauss-Newton pass are k_pvt's, restated here
-// with the weights so that k_pvt's two instantiations keep their instructions; `use` is the set, so a masked or
-// excluded lane's row enters with weight 0. Rows and residuals are scaled by sw = 1 / sigma_int, computed per iteration
-// at the estimate's elevation. Solution separation and the protection levels run where the test of a set is final,
-// inside the pass loop, so that nothing of them stays live across a re-solve. kAraimMinBlocks: DESIGN §11.2.
+// k_pvt_araim: gpsb200_pvt_araim (DESIGN §11.2). The measurement and the Gauss-Newton pass are k_pvt's with the
+// weights; `use` is the set, so a masked or excluded lane's row enters with weight 0. Rows and residuals are scaled by
+// sw = 1 / sigma_int, computed per iteration at the estimate's elevation. Solution separation and the protection levels
+// run where the test of a set is final, inside the pass loop, so that nothing of them stays live across a re-solve.
+// kAraimMinBlocks: DESIGN §11.2.
 constexpr int kAraimMinBlocks = 4;
 __global__ void __launch_bounds__(kWarps * 32, kAraimMinBlocks) k_pvt_araim(const AraimArgs a) {
     const int lane = threadIdx.x & 31;
@@ -618,49 +683,24 @@ __global__ void __launch_bounds__(kWarps * 32, kAraimMinBlocks) k_pvt_araim(cons
     const double nan = __longlong_as_double(0x7ff8000000000000ll);
 
     // ---- the measurement of this lane's channel (integers), its satellite (FP64), its URA sigmas ----
-    bool use = false;
     double rho = 0.0, rate = 0.0, dtsv = 0.0, ddtsv = 0.0, p[3] = {0, 0, 0}, v[3] = {0, 0, 0};
     double sura2 = 0.0, sure2 = 0.0;
     const int64_t ds = s - a.ref_sample;
     const int64_t q = floor_div(ds, 3000), m = ds - 3000 * q;
     const int64_t nom_ms = (((a.ref_ms + 75 + q) % kWeekMs) + kWeekMs) % kWeekMs;
-    if (lane < a.nchan && a.ref >= 0) {
-        const gpsb200_pvt_chan_t &c = a.ch[lane];
-        const gpsb200_track_epoch_t *e = a.ep + (size_t) lane * a.max_epochs;
-        const bool ura_ok = c.eph.ura >= 0 && c.eph.ura < 15;   // header step 1: URA index 15 never enters the set
-        const int k = ura_ok && c.eph.valid && c.eph.health == 0 ? find_period(e, a.n[lane], s) : -1;
-        if (k >= 1 && e[k - 1].lock && e[k].lock) {
-            const uint64_t phi = (uint64_t) e[k - 1].code_phase + (uint64_t) (s - e[k].sample) * e[k - 1].code_step;
-            const int64_t T = (((c.anchor_ms + k - c.anchor_epoch) % kWeekMs) + kWeekMs) % kWeekMs;
-            const double frac = (double) phi / kCodeMod;
-            const double tsv = (double) T * 1e-3 + frac * 1e-3;
-            if (fabs(wrap_half_week(tsv - c.eph.toe)) <= 7200.0) {
-                use = true;
-                int64_t D = (a.ref_ms + 75 + q - T) % kWeekMs;
-                D = D >= kWeekMs / 2 ? D - kWeekMs : (D < -kWeekMs / 2 ? D + kWeekMs : D);
-                rho = (double) D * kCms + ((double) m / 3000.0 - frac) * kCms;
-                rate = -kLambda * ((double) e[k - 1].carr_step * kStepHz);
-                const double d0 = wrap_half_week(tsv - c.eph.toc);
-                const double tt = tsv - (c.eph.af0 + d0 * (c.eph.af1 + d0 * c.eph.af2));
-                satellite(c.eph, tt, p, v, dtsv, ddtsv);
-                const double sura = fmax(a.araim.sigma_ura, kUraNom[c.eph.ura]);
-                const double sure = sura * a.araim.sigma_ure / a.araim.sigma_ura;
-                sura2 = sura * sura;
-                sure2 = sure * sure;
-            }
-        }
+    // header step 1: URA index 15 never enters the set
+    bool use = measure(a, lane, s, q, m, true, rho, rate, p, v, dtsv, ddtsv);
+    if (use) {
+        const double sura = fmax(a.araim.sigma_ura, kUraNom[a.ch[lane].eph.ura]);
+        const double sure = sura * a.araim.sigma_ure / a.araim.sigma_ura;
+        sura2 = sura * sura;
+        sure2 = sure * sure;
     }
     const bool has = use;
     unsigned mask = __ballot_sync(kFull, use);
     int nused = __popc(mask);
     gpsb200_fix_t f;
-    f.sample = s;
-    f.nused = nused;
-    f.mask = mask;
-    f.iterations = 0;
-    f.status = nused < 4 ? GPSB200_FIX_FEW : GPSB200_FIX_NO_CONVERGENCE;
-    f.x = f.y = f.z = f.clock_m = f.t_rx = f.vx = f.vy = f.vz = f.drift = nan;
-    f.lat_deg = f.lon_deg = f.height = f.pdop = f.rms = nan;
+    no_fix(f, s, nused, mask, nused < 4 ? GPSB200_FIX_FEW : GPSB200_FIX_NO_CONVERGENCE);
     double resid = nan;
     // the record; this lane's 1 / sigma_int, elevation and sigma^2 other than URA / URE of the last iteration
     int verdict = GPSB200_RAIM_UNAVAILABLE;
@@ -672,7 +712,7 @@ __global__ void __launch_bounds__(kWarps * 32, kAraimMinBlocks) k_pvt_araim(cons
         double X[4] = {0.0, 0.0, 0.0, 0.0};
         double h[3] = {0, 0, 0}, r = 0.0, pr_v[3] = {0, 0, 0};
         double N[10];   // the weighted normal matrix of the last iteration
-        Chol ch;
+        Chol<4> ch;
         bool ok = false;
         double dX[4] = {0, 0, 0, 0};
         int it0 = 0;   // iterations of the earlier passes
@@ -682,43 +722,21 @@ __global__ void __launch_bounds__(kWarps * 32, kAraimMinBlocks) k_pvt_araim(cons
             for (int j = 0; j < GPSB200_PVT_MAX_ITER; j++) {
                 const double rad = sqrt(X[0] * X[0] + X[1] * X[1] + X[2] * X[2]);
                 const bool near = rad >= kIonoMinRadius, iono = a.cfg.iono && near;
-                double lat = 0.0, lon = 0.0, hgt = 0.0, sla = 0.0, cla = 0.0, slo = 0.0, clo = 0.0;
-                if (near) {   // the elevation weighs with or without the Klobuchar term
-                    ecef_llh(X, lat, lon, hgt);
-                    sincos(lat, &sla, &cla);
-                    sincos(lon, &slo, &clo);
-                }
+                Geo g;
+                if (near) g.set(X);   // the elevation weighs with or without the Klobuchar term
                 h[0] = h[1] = h[2] = 0.0;
                 r = 0.0;
                 if (has) {
-                    const double g0 = p[0] - X[0], g1 = p[1] - X[1], g2 = p[2] - X[2];
-                    const double tau = sqrt(g0 * g0 + g1 * g1 + g2 * g2) / kC;
-                    double sth, cth;
-                    sincos(kOmegaE * tau, &sth, &cth);
-                    const double px = p[0] * cth + p[1] * sth, py = p[1] * cth - p[0] * sth;
-                    pr_v[0] = v[0] * cth + v[1] * sth;
-                    pr_v[1] = v[1] * cth - v[0] * sth;
-                    pr_v[2] = v[2];
-                    const double l0 = px - X[0], l1 = py - X[1], l2 = p[2] - X[2];
-                    const double R = sqrt(l0 * l0 + l1 * l1 + l2 * l2);
-                    double I = 0.0, Fm[2] = {1.0, 0.0};
+                    double l[3], R, az = 0.0, I = 0.0, Fm[2] = {1.0, 0.0};
                     el = 0.5 * M_PI;
-                    if (near) {
-                        const double nn = -sla * clo * l0 - sla * slo * l1 + cla * l2;
-                        const double ee = -slo * l0 + clo * l1;
-                        const double uu = cla * clo * l0 + cla * slo * l1 + sla * l2;
-                        double az = atan2(ee, nn);
-                        if (az < 0.0) az += 2.0 * kPi;
-                        el = atan2(uu, sqrt(nn * nn + ee * ee));
-                        if (iono) {
-                            const double trx = (double) nom_ms * 1e-3 + (double) m / 3e6 - X[3] / kC;
-                            I = klobuchar(a.cfg, lat, lon, az, el, trx, Fm);
-                        }
-                    }
+                    sight(p, v, X, g, near, l, R, pr_v, az, el);
+                    if (iono)
+                        I = klobuchar(a.cfg, g.lat, g.lon, az, el, (double) nom_ms * 1e-3 + (double) m / 3e6 - X[3] / kC,
+                                      Fm);
                     r = rho - (R + X[3] - kC * dtsv + I);
-                    h[0] = -l0 / R;
-                    h[1] = -l1 / R;
-                    h[2] = -l2 / R;
+                    h[0] = -l[0] / R;
+                    h[1] = -l[1] / R;
+                    h[2] = -l[2] / R;
                     // header step 2
                     const double se = sin(el);
                     const double st = 0.12 * 1.001 / sqrt(0.002001 + se * se);
@@ -817,37 +835,9 @@ __global__ void __launch_bounds__(kWarps * 32, kAraimMinBlocks) k_pvt_araim(cons
         if (ok) {
             // post-fit residuals of the last iteration; velocity and drift on its weighted rows
             if (has) resid = r - (h[0] * dX[0] + h[1] * dX[1] + h[2] * dX[2] + dX[3]);
-            const double y = use ? (rate + kC * ddtsv + (h[0] * pr_v[0] + h[1] * pr_v[1] + h[2] * pr_v[2])) * (sw * sw) : 0.0;
-            const double bv[4] = {warp_sum(h[0] * y), warp_sum(h[1] * y), warp_sum(h[2] * y), warp_sum(y)};
-            double V[4];
-            ch.solve(bv, V);
-            const double ss = warp_sum(use ? resid * resid : 0.0);
-            double Q[3];
-#pragma unroll
-            for (int i = 0; i < 3; i++) {
-                double ei[4] = {0, 0, 0, 0}, xi[4];
-                ei[i] = 1.0;
-                ch.solve(ei, xi);
-                Q[i] = xi[i];
-            }
-            f.status = GPSB200_FIX_OK;
-            f.x = X[0];
-            f.y = X[1];
-            f.z = X[2];
-            f.clock_m = X[3];
-            double trx = (double) nom_ms * 1e-3 + ((double) m / 3e6 - X[3] / kC);
-            f.t_rx = trx < 0.0 ? trx + 604800.0 : (trx >= 604800.0 ? trx - 604800.0 : trx);
-            f.vx = V[0];
-            f.vy = V[1];
-            f.vz = V[2];
-            f.drift = V[3];
-            double lat, lon, hgt;
-            ecef_llh(X, lat, lon, hgt);
-            f.lat_deg = lat * (180.0 / M_PI);
-            f.lon_deg = lon * (180.0 / M_PI);
-            f.height = hgt;
-            f.pdop = sqrt(Q[0] + Q[1] + Q[2]);
-            f.rms = sqrt(ss / (double) nused);
+            double lat, lon;
+            finish(ch, X, (double) nom_ms * 1e-3 + ((double) m / 3e6 - X[3] / kC), use, h, pr_v, rate, ddtsv, sw * sw,
+                   resid, nused, f, lat, lon);
         }
     }
     if (lane == 0) {
@@ -875,53 +865,6 @@ struct CoarseArgs : Args {
     int64_t *ms;
 };
 
-// Cholesky solve of the symmetric 5 x 5 system, N packed as its upper triangle row by row (15 values). solve<n> uses
-// the leading n x n block, whose factor is the leading block of the whole factor.
-struct Chol5 {
-    double l[5][5];
-    __device__ bool factor(const double *N) {
-        double a[5][5];
-        int t = 0;
-#pragma unroll
-        for (int i = 0; i < 5; i++)
-#pragma unroll
-            for (int j = i; j < 5; j++) a[i][j] = a[j][i] = N[t++];
-#pragma unroll
-        for (int j = 0; j < 5; j++) {
-            double d = a[j][j];
-#pragma unroll
-            for (int k = 0; k < j; k++) d -= l[j][k] * l[j][k];
-            if (!(d > 0.0)) return false;
-            l[j][j] = sqrt(d);
-#pragma unroll
-            for (int i = j + 1; i < 5; i++) {
-                double v = a[i][j];
-#pragma unroll
-                for (int k = 0; k < j; k++) v -= l[i][k] * l[j][k];
-                l[i][j] = v / l[j][j];
-            }
-        }
-        return true;
-    }
-    template <int n> __device__ void solve(const double *b, double *x) const {
-        double y[n];
-#pragma unroll
-        for (int i = 0; i < n; i++) {
-            double v = b[i];
-#pragma unroll
-            for (int k = 0; k < i; k++) v -= l[i][k] * y[k];
-            y[i] = v / l[i][i];
-        }
-#pragma unroll
-        for (int i = n - 1; i >= 0; i--) {
-            double v = y[i];
-#pragma unroll
-            for (int k = i + 1; k < n; k++) v -= l[k][i] * x[k];
-            x[i] = v / l[i][i];
-        }
-    }
-};
-
 // Header step 3: the predicted transmit time (ms, satellite time) of a satellite at position x and receive time t, and
 // sin(elevation) seen along the up vector `up` (unit, ECEF).
 __device__ double predict(const gpsb200_ephemeris_t &e, const double *x, double t, const double *up, double &sel) {
@@ -943,42 +886,39 @@ __device__ double predict(const gpsb200_ephemeris_t &e, const double *x, double 
 
 __device__ inline double round_half_up(double v) { return floor(v + 0.5); }
 
-// k_pvt_coarse: gpsb200_pvt_coarse (DESIGN §11.3). One warp per fix, lane = channel, as k_pvt; a kernel of its own so
-// that k_pvt's and k_pvt_araim's instructions stay as they are. The satellite is evaluated in every iteration, at the
-// transmit time moved by the current delta. kCoarseMinBlocks: held to 128 registers (some spills) it ran 10 % faster
-// than at its natural 168 with 3 CTAs per SM (DESIGN §11.3).
-constexpr int kCoarseMinBlocks = 4;
-__global__ void __launch_bounds__(kWarps * 32, kCoarseMinBlocks) k_pvt_coarse(const CoarseArgs a) {
-    const int lane = threadIdx.x & 31;
-    const int64_t fi = (int64_t) blockIdx.x * kWarps + (threadIdx.x >> 5);
-    if (fi >= a.cfg.nfix) return;   // the whole warp leaves together
-    const int64_t s = a.cfg.s0 + fi * a.cfg.step;
-    const double nan = __longlong_as_double(0x7ff8000000000000ll);
+// The coarse record of an instant without a coarse-time fix.
+__device__ inline void no_coarse(gpsb200_coarse_t &o, int ref) {
+    o.delta = o.pdop = __longlong_as_double(0x7ff8000000000000ll);
+    o.ref = ref;
+    o.week = -1;
+    o.changed = 0;
+    o.reserved = 0;
+}
 
+// gpsb200_pvt_coarse's header steps 1-9 at sample s from the a-priori config ap: one warp, lane = channel, as k_pvt. The satellite is evaluated in every iteration, at the transmit time moved by the current delta. The fix and
+// coarse records come out uniform over the warp; resid, Nw and has are this lane's (channel's).
+__device__ __forceinline__ void coarse_solve(const Args &a, const gpsb200_coarse_config_t &ap, int64_t s, int lane,
+                                             gpsb200_fix_t &f, gpsb200_coarse_t &o, double &resid, int64_t &Nw,
+                                             bool &has) {
+    const double nan = __longlong_as_double(0x7ff8000000000000ll);
     // header step 1
-    const int64_t ds = s - a.ap.s_a;
+    const int64_t ds = s - ap.s_a;
     const int64_t q = floor_div(ds, 3000), m = ds - 3000 * q;
-    const double u = a.ap.t_a + (double) ds / 3e6;
+    const double u = ap.t_a + (double) ds / 3e6;
     const double kw = floor(u / 604800.0);
     const double tas = u - 604800.0 * kw;
-    const double W = floor(a.ap.t_a), F = a.ap.t_a - W;
+    const double W = floor(ap.t_a), F = ap.t_a - W;
     const double sub = F * 1000.0 + (double) m / 3000.0;   // ms
 
     // header steps 2-4: measurement, prediction at x_a, reference channel
     bool use = false;
-    double frac = 0.0, pred = 0.0, sel = -2.0;
+    double frac = 0.0, rate = 0.0, pred = 0.0, sel = -2.0;
     const gpsb200_ephemeris_t *eph = nullptr;
-    double up[3];
-    {
-        double lat, lon, hgt, sla, cla, slo, clo;
-        ecef_llh(a.ap.x_a, lat, lon, hgt);
-        sincos(lat, &sla, &cla);
-        sincos(lon, &slo, &clo);
-        up[0] = cla * clo;
-        up[1] = cla * slo;
-        up[2] = sla;
-    }
-    double rate = 0.0;
+    Geo ga;
+    ga.set(ap.x_a);
+    const double up[3] = {ga.cla * ga.clo, ga.cla * ga.slo, ga.sla};
+    // locked_period, restated: calling it here made k_pvt_coarse take 25.55-25.60 ms against 25.22-25.48 ms and the
+    // 12-channel search 8 094 ms against 8 078 ms (tools/pvt_bench.py --coarse / --search, H100 80GB HBM3, 700 W).
     if (lane < a.nchan) {
         const gpsb200_pvt_chan_t &c = a.ch[lane];
         const gpsb200_track_epoch_t *e = a.ep + (size_t) lane * a.max_epochs;
@@ -989,10 +929,10 @@ __global__ void __launch_bounds__(kWarps * 32, kCoarseMinBlocks) k_pvt_coarse(co
             const uint64_t phi = (uint64_t) e[k - 1].code_phase + (uint64_t) (s - e[k].sample) * e[k - 1].code_step;
             frac = (double) phi / kCodeMod;
             rate = -kLambda * ((double) e[k - 1].carr_step * kStepHz);
-            pred = predict(*eph, a.ap.x_a, tas, up, sel);
+            pred = predict(*eph, ap.x_a, tas, up, sel);
         }
     }
-    const bool has = use;
+    has = use;
     const unsigned mask = __ballot_sync(kFull, use);
     const int nused = __popc(mask);
     double key = use ? sel : -2.0;
@@ -1003,7 +943,7 @@ __global__ void __launch_bounds__(kWarps * 32, kCoarseMinBlocks) k_pvt_coarse(co
     // header step 5
     const int64_t Nr = (int64_t) round_half_up(pred_r - frac_r);
     const int64_t dN = (int64_t) round_half_up((pred - pred_r) - (frac - frac_r));
-    const int64_t Nw = (((Nr + dN) % kWeekMs) + kWeekMs) % kWeekMs;
+    Nw = (((Nr + dN) % kWeekMs) + kWeekMs) % kWeekMs;
     // header step 6
     double rho = 0.0, tsv = 0.0;
     if (has) {
@@ -1013,37 +953,21 @@ __global__ void __launch_bounds__(kWarps * 32, kCoarseMinBlocks) k_pvt_coarse(co
         tsv = (double) Nw * 1e-3 + frac * 1e-3;
     }
 
-    gpsb200_fix_t f;
-    f.sample = s;
-    f.nused = nused;
-    f.mask = mask;
-    f.iterations = 0;
-    f.status = nused < 5 ? GPSB200_FIX_FEW : GPSB200_FIX_NO_CONVERGENCE;
-    f.x = f.y = f.z = f.clock_m = f.t_rx = f.vx = f.vy = f.vz = f.drift = nan;
-    f.lat_deg = f.lon_deg = f.height = f.pdop = f.rms = nan;
-    gpsb200_coarse_t o;
-    o.delta = o.pdop = nan;
-    o.ref = ref;
-    o.week = -1;
-    o.changed = 0;
-    o.reserved = 0;
-    double resid = nan;
+    no_fix(f, s, nused, mask, nused < 5 ? GPSB200_FIX_FEW : GPSB200_FIX_NO_CONVERGENCE);
+    no_coarse(o, ref);
+    resid = nan;
     if (nused >= 5) {
-        double X[5] = {a.ap.x_a[0], a.ap.x_a[1], a.ap.x_a[2], 0.0, 0.0};
+        double X[5] = {ap.x_a[0], ap.x_a[1], ap.x_a[2], 0.0, 0.0};
         double h[4] = {0, 0, 0, 0}, rr = 0.0, pr_v[3] = {0, 0, 0}, ddtsv = 0.0;
-        Chol5 ch;
+        Chol<5> ch;
         bool ok = false;
         double dX[5] = {0, 0, 0, 0, 0};
 #pragma unroll 1
         for (int j = 0; j < GPSB200_PVT_MAX_ITER; j++) {
             const double rad = sqrt(X[0] * X[0] + X[1] * X[1] + X[2] * X[2]);
             const bool iono = a.cfg.iono && rad >= kIonoMinRadius;
-            double lat = 0.0, lon = 0.0, hgt = 0.0, sla = 0.0, cla = 0.0, slo = 0.0, clo = 0.0;
-            if (iono) {
-                ecef_llh(X, lat, lon, hgt);
-                sincos(lat, &sla, &cla);
-                sincos(lon, &slo, &clo);
-            }
+            Geo g;
+            if (iono) g.set(X);
             h[0] = h[1] = h[2] = h[3] = 0.0;
             rr = 0.0;
             if (has) {
@@ -1051,33 +975,15 @@ __global__ void __launch_bounds__(kWarps * 32, kCoarseMinBlocks) k_pvt_coarse(co
                 const double t = tsv + X[4];
                 const double d0 = wrap_half_week(t - e.toc);
                 const double tt = t - (e.af0 + d0 * (e.af1 + d0 * e.af2));
-                double p[3], v[3], dtsv;
+                double p[3], v[3], dtsv, l[3], R, az = 0.0, el = 0.0, I = 0.0;
                 satellite(e, tt, p, v, dtsv, ddtsv);
-                const double g0 = p[0] - X[0], g1 = p[1] - X[1], g2 = p[2] - X[2];
-                const double tau = sqrt(g0 * g0 + g1 * g1 + g2 * g2) / kC;
-                double sth, cth;
-                sincos(kOmegaE * tau, &sth, &cth);
-                const double px = p[0] * cth + p[1] * sth, py = p[1] * cth - p[0] * sth;
-                pr_v[0] = v[0] * cth + v[1] * sth;
-                pr_v[1] = v[1] * cth - v[0] * sth;
-                pr_v[2] = v[2];
-                const double l0 = px - X[0], l1 = py - X[1], l2 = p[2] - X[2];
-                const double R = sqrt(l0 * l0 + l1 * l1 + l2 * l2);
-                double I = 0.0;
-                if (iono) {
-                    const double nn = -sla * clo * l0 - sla * slo * l1 + cla * l2;
-                    const double ee = -slo * l0 + clo * l1;
-                    const double uu = cla * clo * l0 + cla * slo * l1 + sla * l2;
-                    double az = atan2(ee, nn);
-                    if (az < 0.0) az += 2.0 * kPi;
-                    const double el = atan2(uu, sqrt(nn * nn + ee * ee));
-                    I = klobuchar(a.cfg, lat, lon, az, el, tas + X[4] - X[3] / kC);
-                }
+                sight(p, v, X, g, iono, l, R, pr_v, az, el);
+                if (iono) I = klobuchar(a.cfg, g.lat, g.lon, az, el, tas + X[4] - X[3] / kC);
                 rr = rho - (R + X[3] - kC * dtsv + I);
-                h[0] = -l0 / R;
-                h[1] = -l1 / R;
-                h[2] = -l2 / R;
-                h[3] = (l0 * pr_v[0] + l1 * pr_v[1] + l2 * pr_v[2]) / R - kC * ddtsv;
+                h[0] = -l[0] / R;
+                h[1] = -l[1] / R;
+                h[2] = -l[2] / R;
+                h[3] = (l[0] * pr_v[0] + l[1] * pr_v[1] + l[2] * pr_v[2]) / R - kC * ddtsv;
             }
             const double N[15] = {warp_sum(h[0] * h[0]), warp_sum(h[0] * h[1]), warp_sum(h[0] * h[2]), warp_sum(h[0]),
                                   warp_sum(h[0] * h[3]), warp_sum(h[1] * h[1]), warp_sum(h[1] * h[2]), warp_sum(h[1]),
@@ -1087,7 +993,7 @@ __global__ void __launch_bounds__(kWarps * 32, kCoarseMinBlocks) k_pvt_coarse(co
                                  warp_sum(h[3] * rr)};
             f.iterations = j + 1;
             if (!ch.factor(N)) break;
-            ch.solve<5>(b, dX);
+            ch.solve(b, dX);
 #pragma unroll
             for (int i = 0; i < 5; i++) X[i] += dX[i];
             if (sqrt(X[0] * X[0] + X[1] * X[1] + X[2] * X[2]) > kRunaway) break;
@@ -1109,51 +1015,31 @@ __global__ void __launch_bounds__(kWarps * 32, kCoarseMinBlocks) k_pvt_coarse(co
                 f.status = GPSB200_FIX_AMBIGUOUS;
                 resid = nan;
             } else {
-                // velocity and drift on the rows' first four columns, 5-state PDOP
-                const double y = has ? rate + kC * ddtsv + (h[0] * pr_v[0] + h[1] * pr_v[1] + h[2] * pr_v[2]) : 0.0;
-                const double bv[4] = {warp_sum(h[0] * y), warp_sum(h[1] * y), warp_sum(h[2] * y), warp_sum(y)};
-                double V[4];
-                ch.solve<4>(bv, V);
-                const double ss = warp_sum(has ? resid * resid : 0.0);
-                double Q[3];
-#pragma unroll
-                for (int i = 0; i < 3; i++) {
-                    double ei[5] = {0, 0, 0, 0, 0}, xi[5];
-                    ei[i] = 1.0;
-                    ch.solve<5>(ei, xi);
-                    Q[i] = xi[i];
-                }
-                f.status = GPSB200_FIX_OK;
-                f.x = X[0];
-                f.y = X[1];
-                f.z = X[2];
-                f.clock_m = X[3];
-                double t = trx, wk = kw;
-                if (t < 0.0) {
-                    t += 604800.0;
-                    wk -= 1.0;
-                } else if (t >= 604800.0) {
-                    t -= 604800.0;
-                    wk += 1.0;
-                }
-                f.t_rx = t;
-                f.vx = V[0];
-                f.vy = V[1];
-                f.vz = V[2];
-                f.drift = V[3];
-                double lat, lon, hgt;
-                ecef_llh(X, lat, lon, hgt);
-                f.lat_deg = lat * (180.0 / M_PI);
-                f.lon_deg = lon * (180.0 / M_PI);
-                f.height = hgt;
-                f.pdop = sqrt(Q[0] + Q[1] + Q[2]);
-                f.rms = sqrt(ss / (double) nused);
+                // velocity and drift on the rows' first four columns, 5-state PDOP; t_rx's fold carries into the week
+                double lat, lon;
+                finish(ch, X, trx, has, h, pr_v, rate, ddtsv, 1.0, resid, nused, f, lat, lon);
                 o.delta = X[4];
                 o.pdop = f.pdop;
-                o.week = a.ap.week + (int) wk;
+                o.week = ap.week + (int) (trx < 0.0 ? kw - 1.0 : (trx >= 604800.0 ? kw + 1.0 : kw));
             }
         }
     }
+}
+
+// k_pvt_coarse: gpsb200_pvt_coarse (DESIGN §11.3), one warp per fix. kCoarseMinBlocks: held to 128 registers (some
+// spills) it ran 10 % faster than at its natural 168 with 3 CTAs per SM (DESIGN §11.3).
+constexpr int kCoarseMinBlocks = 4;
+__global__ void __launch_bounds__(kWarps * 32, kCoarseMinBlocks) k_pvt_coarse(const CoarseArgs a) {
+    const int lane = threadIdx.x & 31;
+    const int64_t fi = (int64_t) blockIdx.x * kWarps + (threadIdx.x >> 5);
+    if (fi >= a.cfg.nfix) return;   // the whole warp leaves together
+    const double nan = __longlong_as_double(0x7ff8000000000000ll);
+    gpsb200_fix_t f;
+    gpsb200_coarse_t o;
+    double resid;
+    int64_t Nw;
+    bool has;
+    coarse_solve(a, a.ap, a.cfg.s0 + fi * a.cfg.step, lane, f, o, resid, Nw, has);
     if (lane == 0) {
         a.fixes[fi] = f;
         a.out[fi] = o;
@@ -1208,212 +1094,6 @@ __host__ __device__ inline void search_node(int64_t i, int n, double *x, double 
     up[2] = sla;
 }
 
-// k_pvt_coarse's header steps 1-9 from the a-priori config ap, restated rather than shared: moving k_pvt_coarse's body
-// into a function changes its register allocation. The fix and coarse records come out uniform over the warp; resid,
-// Nw and has are this lane's (channel's).
-__device__ __forceinline__ void search_solve(const Args &a, const gpsb200_coarse_config_t &ap, int64_t s, int lane,
-                                             gpsb200_fix_t &f, gpsb200_coarse_t &o, double &resid, int64_t &Nw,
-                                             bool &has) {
-    const double nan = __longlong_as_double(0x7ff8000000000000ll);
-    // header step 1
-    const int64_t ds = s - ap.s_a;
-    const int64_t q = floor_div(ds, 3000), m = ds - 3000 * q;
-    const double u = ap.t_a + (double) ds / 3e6;
-    const double kw = floor(u / 604800.0);
-    const double tas = u - 604800.0 * kw;
-    const double W = floor(ap.t_a), F = ap.t_a - W;
-    const double sub = F * 1000.0 + (double) m / 3000.0;   // ms
-
-    // header steps 2-4: measurement, prediction at x_a, reference channel
-    bool use = false;
-    double frac = 0.0, pred = 0.0, sel = -2.0;
-    const gpsb200_ephemeris_t *eph = nullptr;
-    double up[3];
-    {
-        double lat, lon, hgt, sla, cla, slo, clo;
-        ecef_llh(ap.x_a, lat, lon, hgt);
-        sincos(lat, &sla, &cla);
-        sincos(lon, &slo, &clo);
-        up[0] = cla * clo;
-        up[1] = cla * slo;
-        up[2] = sla;
-    }
-    double rate = 0.0;
-    if (lane < a.nchan) {
-        const gpsb200_pvt_chan_t &c = a.ch[lane];
-        const gpsb200_track_epoch_t *e = a.ep + (size_t) lane * a.max_epochs;
-        const int k = c.eph.valid && c.eph.health == 0 ? find_period(e, a.n[lane], s) : -1;
-        if (k >= 1 && e[k - 1].lock && e[k].lock && fabs(wrap_half_week(tas - c.eph.toe)) <= 7200.0) {
-            use = true;
-            eph = &c.eph;
-            const uint64_t phi = (uint64_t) e[k - 1].code_phase + (uint64_t) (s - e[k].sample) * e[k - 1].code_step;
-            frac = (double) phi / kCodeMod;
-            rate = -kLambda * ((double) e[k - 1].carr_step * kStepHz);
-            pred = predict(*eph, ap.x_a, tas, up, sel);
-        }
-    }
-    has = use;
-    const unsigned mask = __ballot_sync(kFull, use);
-    const int nused = __popc(mask);
-    double key = use ? sel : -2.0;
-    int r = lane;
-    warp_argmax(key, r);
-    const int ref = nused ? r : -1;
-    const double pred_r = __shfl_sync(kFull, pred, r), frac_r = __shfl_sync(kFull, frac, r);
-    // header step 5
-    const int64_t Nr = (int64_t) round_half_up(pred_r - frac_r);
-    const int64_t dN = (int64_t) round_half_up((pred - pred_r) - (frac - frac_r));
-    Nw = (((Nr + dN) % kWeekMs) + kWeekMs) % kWeekMs;
-    // header step 6
-    double rho = 0.0, tsv = 0.0;
-    if (has) {
-        int64_t D = ((int64_t) W * 1000 + q - Nw) % kWeekMs;
-        D = D >= kWeekMs / 2 ? D - kWeekMs : (D < -kWeekMs / 2 ? D + kWeekMs : D);
-        rho = (double) D * kCms + (sub - frac) * kCms;
-        tsv = (double) Nw * 1e-3 + frac * 1e-3;
-    }
-
-    f.sample = s;
-    f.nused = nused;
-    f.mask = mask;
-    f.iterations = 0;
-    f.status = nused < 5 ? GPSB200_FIX_FEW : GPSB200_FIX_NO_CONVERGENCE;
-    f.x = f.y = f.z = f.clock_m = f.t_rx = f.vx = f.vy = f.vz = f.drift = nan;
-    f.lat_deg = f.lon_deg = f.height = f.pdop = f.rms = nan;
-    o.delta = o.pdop = nan;
-    o.ref = ref;
-    o.week = -1;
-    o.changed = 0;
-    o.reserved = 0;
-    resid = nan;
-    if (nused >= 5) {
-        double X[5] = {ap.x_a[0], ap.x_a[1], ap.x_a[2], 0.0, 0.0};
-        double h[4] = {0, 0, 0, 0}, rr = 0.0, pr_v[3] = {0, 0, 0}, ddtsv = 0.0;
-        Chol5 ch;
-        bool ok = false;
-        double dX[5] = {0, 0, 0, 0, 0};
-#pragma unroll 1
-        for (int j = 0; j < GPSB200_PVT_MAX_ITER; j++) {
-            const double rad = sqrt(X[0] * X[0] + X[1] * X[1] + X[2] * X[2]);
-            const bool iono = a.cfg.iono && rad >= kIonoMinRadius;
-            double lat = 0.0, lon = 0.0, hgt = 0.0, sla = 0.0, cla = 0.0, slo = 0.0, clo = 0.0;
-            if (iono) {
-                ecef_llh(X, lat, lon, hgt);
-                sincos(lat, &sla, &cla);
-                sincos(lon, &slo, &clo);
-            }
-            h[0] = h[1] = h[2] = h[3] = 0.0;
-            rr = 0.0;
-            if (has) {
-                const gpsb200_ephemeris_t &e = *eph;
-                const double t = tsv + X[4];
-                const double d0 = wrap_half_week(t - e.toc);
-                const double tt = t - (e.af0 + d0 * (e.af1 + d0 * e.af2));
-                double p[3], v[3], dtsv;
-                satellite(e, tt, p, v, dtsv, ddtsv);
-                const double g0 = p[0] - X[0], g1 = p[1] - X[1], g2 = p[2] - X[2];
-                const double tau = sqrt(g0 * g0 + g1 * g1 + g2 * g2) / kC;
-                double sth, cth;
-                sincos(kOmegaE * tau, &sth, &cth);
-                const double px = p[0] * cth + p[1] * sth, py = p[1] * cth - p[0] * sth;
-                pr_v[0] = v[0] * cth + v[1] * sth;
-                pr_v[1] = v[1] * cth - v[0] * sth;
-                pr_v[2] = v[2];
-                const double l0 = px - X[0], l1 = py - X[1], l2 = p[2] - X[2];
-                const double R = sqrt(l0 * l0 + l1 * l1 + l2 * l2);
-                double I = 0.0;
-                if (iono) {
-                    const double nn = -sla * clo * l0 - sla * slo * l1 + cla * l2;
-                    const double ee = -slo * l0 + clo * l1;
-                    const double uu = cla * clo * l0 + cla * slo * l1 + sla * l2;
-                    double az = atan2(ee, nn);
-                    if (az < 0.0) az += 2.0 * kPi;
-                    const double el = atan2(uu, sqrt(nn * nn + ee * ee));
-                    I = klobuchar(a.cfg, lat, lon, az, el, tas + X[4] - X[3] / kC);
-                }
-                rr = rho - (R + X[3] - kC * dtsv + I);
-                h[0] = -l0 / R;
-                h[1] = -l1 / R;
-                h[2] = -l2 / R;
-                h[3] = (l0 * pr_v[0] + l1 * pr_v[1] + l2 * pr_v[2]) / R - kC * ddtsv;
-            }
-            const double N[15] = {warp_sum(h[0] * h[0]), warp_sum(h[0] * h[1]), warp_sum(h[0] * h[2]), warp_sum(h[0]),
-                                  warp_sum(h[0] * h[3]), warp_sum(h[1] * h[1]), warp_sum(h[1] * h[2]), warp_sum(h[1]),
-                                  warp_sum(h[1] * h[3]), warp_sum(h[2] * h[2]), warp_sum(h[2]), warp_sum(h[2] * h[3]),
-                                  (double) nused, warp_sum(h[3]), warp_sum(h[3] * h[3])};
-            const double b[5] = {warp_sum(h[0] * rr), warp_sum(h[1] * rr), warp_sum(h[2] * rr), warp_sum(rr),
-                                 warp_sum(h[3] * rr)};
-            f.iterations = j + 1;
-            if (!ch.factor(N)) break;
-            ch.solve<5>(b, dX);
-#pragma unroll
-            for (int i = 0; i < 5; i++) X[i] += dX[i];
-            if (sqrt(X[0] * X[0] + X[1] * X[1] + X[2] * X[2]) > kRunaway) break;
-            if (sqrt(dX[0] * dX[0] + dX[1] * dX[1] + dX[2] * dX[2]) < kConverged) {
-                ok = true;
-                break;
-            }
-        }
-        if (ok) {
-            // header step 8, at the fix, with the same reference channel
-            const double trx = tas + X[4] - X[3] / kC;
-            double dummy, pred2 = 0.0;
-            if (has) pred2 = predict(*eph, X, trx, up, dummy);
-            const double pred2_r = __shfl_sync(kFull, pred2, r);
-            const bool moved = has && (int64_t) round_half_up((pred2 - pred2_r) - (frac - frac_r)) != dN;
-            o.changed = __ballot_sync(kFull, moved);
-            if (has) resid = rr - (h[0] * dX[0] + h[1] * dX[1] + h[2] * dX[2] + dX[3] + h[3] * dX[4]);
-            if (o.changed || __any_sync(kFull, has && !(fabs(resid) <= GPSB200_COARSE_MAX_RESIDUAL))) {
-                f.status = GPSB200_FIX_AMBIGUOUS;
-                resid = nan;
-            } else {
-                // velocity and drift on the rows' first four columns, 5-state PDOP
-                const double y = has ? rate + kC * ddtsv + (h[0] * pr_v[0] + h[1] * pr_v[1] + h[2] * pr_v[2]) : 0.0;
-                const double bv[4] = {warp_sum(h[0] * y), warp_sum(h[1] * y), warp_sum(h[2] * y), warp_sum(y)};
-                double V[4];
-                ch.solve<4>(bv, V);
-                const double ss = warp_sum(has ? resid * resid : 0.0);
-                double Q[3];
-#pragma unroll
-                for (int i = 0; i < 3; i++) {
-                    double ei[5] = {0, 0, 0, 0, 0}, xi[5];
-                    ei[i] = 1.0;
-                    ch.solve<5>(ei, xi);
-                    Q[i] = xi[i];
-                }
-                f.status = GPSB200_FIX_OK;
-                f.x = X[0];
-                f.y = X[1];
-                f.z = X[2];
-                f.clock_m = X[3];
-                double t = trx, wk = kw;
-                if (t < 0.0) {
-                    t += 604800.0;
-                    wk -= 1.0;
-                } else if (t >= 604800.0) {
-                    t -= 604800.0;
-                    wk += 1.0;
-                }
-                f.t_rx = t;
-                f.vx = V[0];
-                f.vy = V[1];
-                f.vz = V[2];
-                f.drift = V[3];
-                double lat, lon, hgt;
-                ecef_llh(X, lat, lon, hgt);
-                f.lat_deg = lat * (180.0 / M_PI);
-                f.lon_deg = lon * (180.0 / M_PI);
-                f.height = hgt;
-                f.pdop = sqrt(Q[0] + Q[1] + Q[2]);
-                f.rms = sqrt(ss / (double) nused);
-                o.delta = X[4];
-                o.pdop = f.pdop;
-                o.week = ap.week + (int) wk;
-            }
-        }
-    }
-}
-
 // Per fix instant (one warp, lane = channel): header step 2's used channels and step 3's satellite positions; clears the
 // instant's counters.
 __global__ void __launch_bounds__(kWarps * 32) k_search_sats(const SearchArgs a) {
@@ -1427,13 +1107,12 @@ __global__ void __launch_bounds__(kWarps * 32) k_search_sats(const SearchArgs a)
     bool use = false;
     double p[3] = {0.0, 0.0, 0.0};
     if (lane < a.nchan) {
-        const gpsb200_pvt_chan_t &c = a.ch[lane];
-        const gpsb200_track_epoch_t *e = a.ep + (size_t) lane * a.max_epochs;
-        const int k = c.eph.valid && c.eph.health == 0 ? find_period(e, a.n[lane], s) : -1;
-        if (k >= 1 && e[k - 1].lock && e[k].lock && fabs(wrap_half_week(tas - c.eph.toe)) <= 7200.0) {
+        const gpsb200_ephemeris_t &eph = a.ch[lane].eph;
+        double frac, rate;
+        if (locked_period(a, lane, s, frac, rate) >= 1 && fabs(wrap_half_week(tas - eph.toe)) <= 7200.0) {
             use = true;
             double v[3], dt, ddt;
-            satellite(c.eph, tas - 0.075, p, v, dt, ddt);
+            satellite(eph, tas - 0.075, p, v, dt, ddt);
         }
     }
     for (int i = 0; i < 3; i++) a.sat[(fi * 32 + lane) * 3 + i] = p[i];
@@ -1484,7 +1163,7 @@ __global__ void __launch_bounds__(kWarps * 32, kSearchMinBlocks) k_pvt_search(co
         double resid;
         int64_t Nw;
         bool has;
-        search_solve(a, ap, s, lane, f, o, resid, Nw, has);
+        coarse_solve(a, ap, s, lane, f, o, resid, Nw, has);
         if (f.status != GPSB200_FIX_OK) continue;
         if (lane == j) my_rms = f.rms;
         if (lane == 0) {
@@ -1576,22 +1255,14 @@ __global__ void __launch_bounds__(kWarps * 32) k_search_pick(const SearchArgs a)
         ap.s_a = a.sc.s_a;
         ap.week = a.sc.week;
         ap.reserved = 0;
-        search_solve(a, ap, s, lane, f, o, resid, Nw, has);
+        coarse_solve(a, ap, s, lane, f, o, resid, Nw, has);
         if (!isnan(r.alt_rms)) f.status = GPSB200_FIX_AMBIGUOUS;
     } else {
-        f.sample = s;
-        f.status = nused < GPSB200_SEARCH_MIN_CHANNELS ? GPSB200_FIX_FEW
-                   : nok > a.max_ok                   ? GPSB200_FIX_AMBIGUOUS
-                                                      : GPSB200_FIX_NO_CONVERGENCE;
-        f.nused = nused;
-        f.mask = used;
-        f.iterations = 0;
-        f.x = f.y = f.z = f.clock_m = f.t_rx = f.vx = f.vy = f.vz = f.drift = nan;
-        f.lat_deg = f.lon_deg = f.height = f.pdop = f.rms = nan;
-        o.delta = o.pdop = nan;
-        o.ref = -1;
-        o.week = -1;
-        o.changed = 0;
+        no_fix(f, s, nused, used,
+               nused < GPSB200_SEARCH_MIN_CHANNELS ? GPSB200_FIX_FEW
+               : nok > a.max_ok                    ? GPSB200_FIX_AMBIGUOUS
+                                                   : GPSB200_FIX_NO_CONVERGENCE);
+        no_coarse(o, -1);
     }
     r.delta = o.delta;
     r.pdop = o.pdop;
@@ -1606,8 +1277,7 @@ __global__ void __launch_bounds__(kWarps * 32) k_search_pick(const SearchArgs a)
     if (a.ms && lane < a.nchan) a.ms[fi * a.nchan + lane] = has ? Nw : -1;
 }
 
-template <bool kRaim> void fill(KernelArgs<kRaim> &a, const Scratch &sc);
-template <> void fill<false>(Args &a, const Scratch &sc) {
+void fill(Args &a, const Scratch &sc) {
     a.ep = sc.d_epochs;
     a.ch = sc.d_chans;
     a.n = sc.d_n;
@@ -1620,27 +1290,12 @@ template <> void fill<false>(Args &a, const Scratch &sc) {
     a.fixes = sc.d_fixes;
     a.res = sc.want_res ? sc.d_res : nullptr;
 }
-template <> void fill<true>(RaimArgs &a, const Scratch &sc) {
-    fill<false>(a, sc);
-    a.raim = sc.raim_cfg;
-    memcpy(a.T, sc.tab_T, sizeof a.T);
-    memcpy(a.lambda, sc.tab_lambda, sizeof a.lambda);
-    a.out = sc.d_raim;
-}
-
-template <bool kRaim> cudaError_t launch_as(const Scratch &sc, cudaStream_t s) {
-    KernelArgs<kRaim> a;
-    fill<kRaim>(a, sc);
-    const int64_t blocks = ((int64_t) sc.cfg.nfix + kWarps - 1) / kWarps;
-    k_pvt<kRaim><<<(unsigned) blocks, kWarps * 32, 0, s>>>(a);
-    return cudaGetLastError();
-}
 
 // gpsb200_pvt_search: the satellite table, then the grid and the pick in passes of search_pass(nodes) instants, each
 // pass reusing one OK list of GPSB200_SEARCH_HIT_BYTES at most.
 cudaError_t launch_search(const Scratch &sc, cudaStream_t s) {
     SearchArgs a;
-    fill<false>(a, sc);
+    fill(a, sc);
     a.sc = sc.search_cfg;
     a.sin_min = std::sin(GPSB200_SEARCH_MIN_ELEV_DEG * (M_PI / 180.0));
     a.sat = sc.d_sat;
@@ -1666,37 +1321,57 @@ cudaError_t launch_search(const Scratch &sc, cudaStream_t s) {
 }
 
 cudaError_t launch(const Scratch &sc, cudaStream_t s) {
-    if (sc.search) return launch_search(sc, s);
-    if (sc.coarse) {
-        CoarseArgs a;
-        fill<false>(a, sc);
-        a.ap = sc.coarse_cfg;
-        a.out = sc.d_coarse;
-        a.ms = sc.want_ms ? sc.d_ms : nullptr;
-        const int64_t blocks = ((int64_t) sc.cfg.nfix + kWarps - 1) / kWarps;
-        k_pvt_coarse<<<(unsigned) blocks, kWarps * 32, 0, s>>>(a);
-        return cudaGetLastError();
+    const unsigned blocks = (unsigned) (((int64_t) sc.cfg.nfix + kWarps - 1) / kWarps);
+    switch (sc.mode) {
+    case Mode::plain: {
+        Args a;
+        fill(a, sc);
+        k_pvt<false><<<blocks, kWarps * 32, 0, s>>>(a);
+        break;
     }
-    if (sc.araim) {
+    case Mode::raim: {
+        RaimArgs a;
+        fill(a, sc);
+        a.raim = sc.raim_cfg;
+        memcpy(a.T, sc.tab_T, sizeof a.T);
+        memcpy(a.lambda, sc.tab_lambda, sizeof a.lambda);
+        a.out = sc.d_raim;
+        k_pvt<true><<<blocks, kWarps * 32, 0, s>>>(a);
+        break;
+    }
+    case Mode::araim: {
         AraimArgs a;
-        fill<false>(a, sc);
+        fill(a, sc);
         a.araim = sc.araim_cfg;
         memcpy(a.kh, sc.kfa_h, sizeof a.kh);
         memcpy(a.kv, sc.kfa_v, sizeof a.kv);
         a.out = sc.d_araim;
-        const int64_t blocks = ((int64_t) sc.cfg.nfix + kWarps - 1) / kWarps;
-        k_pvt_araim<<<(unsigned) blocks, kWarps * 32, 0, s>>>(a);
-        return cudaGetLastError();
+        k_pvt_araim<<<blocks, kWarps * 32, 0, s>>>(a);
+        break;
     }
-    return sc.raim ? launch_as<true>(sc, s) : launch_as<false>(sc, s);
+    case Mode::coarse: {
+        CoarseArgs a;
+        fill(a, sc);
+        a.ap = sc.coarse_cfg;
+        a.out = sc.d_coarse;
+        a.ms = sc.want_ms ? sc.d_ms : nullptr;
+        k_pvt_coarse<<<blocks, kWarps * 32, 0, s>>>(a);
+        break;
+    }
+    case Mode::search:
+        return launch_search(sc, s);
+    }
+    return cudaGetLastError();
 }
 
 }  // namespace
 
 std::string check(const gpsb200_pvt_chan_t *chans, int nchan, const gpsb200_track_epoch_t *epochs, const int32_t *nepochs,
-                  int max_epochs, const gpsb200_pvt_config_t *cfg, const gpsb200_raim_config_t *raim,
-                  const gpsb200_araim_config_t *araim, const gpsb200_coarse_config_t *coarse,
-                  const gpsb200_search_config_t *search) {
+                  int max_epochs, const gpsb200_pvt_config_t *cfg, const Stage &st) {
+    const gpsb200_raim_config_t *raim = st.raim;
+    const gpsb200_araim_config_t *araim = st.araim;
+    const gpsb200_coarse_config_t *coarse = st.coarse;
+    const gpsb200_search_config_t *search = st.search;
     if (!chans || !epochs || !nepochs || !cfg) return "NULL chans, epochs, nepochs or cfg";
     if (search) {
         const gpsb200_search_config_t &c = *search;
@@ -1781,61 +1456,55 @@ void scratch_free(Scratch &sc) {
 }
 
 cudaError_t run(Scratch &sc, const gpsb200_pvt_chan_t *chans, int nchan, const gpsb200_track_epoch_t *epochs,
-                const int32_t *nepochs, int max_epochs, const gpsb200_pvt_config_t *cfg,
-                const gpsb200_raim_config_t *raim, gpsb200_fix_t *fixes, double *residuals, gpsb200_raim_t *out,
-                cudaStream_t s, const gpsb200_araim_config_t *araim, gpsb200_araim_t *aout,
-                const gpsb200_coarse_config_t *coarse, gpsb200_coarse_t *cout, int64_t *ms,
-                const gpsb200_search_config_t *search, gpsb200_search_t *sout, double *node_rms) {
+                const int32_t *nepochs, int max_epochs, const gpsb200_pvt_config_t *cfg, gpsb200_fix_t *fixes,
+                double *residuals, const Stage &st, cudaStream_t s) {
+    const size_t nf = (size_t) cfg->nfix;
     sc.have_last = false;
     if (!sc.d_chans) {
         CU_RET(cudaMalloc(&sc.d_chans, GPSB200_TRK_MAX_CHAN * sizeof(gpsb200_pvt_chan_t)));
         CU_RET(cudaMalloc(&sc.d_n, GPSB200_TRK_MAX_CHAN * sizeof(int32_t)));
     }
     CU_RET(grow(sc.d_epochs, sc.epoch_cap, (size_t) nchan * max_epochs));
-    CU_RET(grow(sc.d_fixes, sc.fix_cap, (size_t) cfg->nfix));
-    if (residuals) CU_RET(grow(sc.d_res, sc.res_cap, (size_t) cfg->nfix * nchan));
-    sc.raim = raim != nullptr;
-    if (raim) {
-        CU_RET(grow(sc.d_raim, sc.raim_cap, (size_t) cfg->nfix));
-        sc.raim_cfg = *raim;
-        if (raim->p_fa != sc.tab_p_fa || raim->p_md != sc.tab_p_md) {   // the tables take 20-80 ms of host time
-            raim_thresholds(raim->p_fa, raim->p_md, sc.tab_T, sc.tab_lambda);
-            sc.tab_p_fa = raim->p_fa;
-            sc.tab_p_md = raim->p_md;
+    CU_RET(grow(sc.d_fixes, sc.fix_cap, nf));
+    if (residuals) CU_RET(grow(sc.d_res, sc.res_cap, nf * nchan));
+    if (st.ms) CU_RET(grow(sc.d_ms, sc.ms_cap, nf * nchan));
+    sc.mode = st.mode();
+    if (st.raim) {
+        CU_RET(grow(sc.d_raim, sc.raim_cap, nf));
+        sc.raim_cfg = *st.raim;
+        if (st.raim->p_fa != sc.tab_p_fa || st.raim->p_md != sc.tab_p_md) {   // the tables take 20-80 ms of host time
+            raim_thresholds(st.raim->p_fa, st.raim->p_md, sc.tab_T, sc.tab_lambda);
+            sc.tab_p_fa = st.raim->p_fa;
+            sc.tab_p_md = st.raim->p_md;
         }
     }
-    sc.araim = araim != nullptr;
-    if (araim) {
-        CU_RET(grow(sc.d_araim, sc.araim_cap, (size_t) cfg->nfix));
-        sc.araim_cfg = *araim;
-        araim_kfa(araim->p_fa_vert, araim->p_fa_horz, sc.kfa_h, sc.kfa_v);
+    if (st.araim) {
+        CU_RET(grow(sc.d_araim, sc.araim_cap, nf));
+        sc.araim_cfg = *st.araim;
+        araim_kfa(st.araim->p_fa_vert, st.araim->p_fa_horz, sc.kfa_h, sc.kfa_v);
     }
-    sc.coarse = coarse != nullptr;
-    sc.want_ms = ms != nullptr;
-    if (coarse) {
-        CU_RET(grow(sc.d_coarse, sc.coarse_cap, (size_t) cfg->nfix));
-        if (ms) CU_RET(grow(sc.d_ms, sc.ms_cap, (size_t) cfg->nfix * nchan));
-        sc.coarse_cfg = *coarse;
+    if (st.coarse) {
+        CU_RET(grow(sc.d_coarse, sc.coarse_cap, nf));
+        sc.coarse_cfg = *st.coarse;
     }
-    sc.search = search != nullptr;
-    sc.want_node_rms = node_rms != nullptr;
-    if (search) {
-        const size_t nf = (size_t) cfg->nfix;
+    if (st.search) {
+        const int nodes = st.search->nodes;
         CU_RET(grow(sc.d_search, sc.search_cap, nf));
         CU_RET(grow(sc.d_sat, sc.sat_cap, nf * 32 * 3));
         CU_RET(grow(sc.d_used, sc.used_cap, nf));
         CU_RET(grow(sc.d_searched, sc.searched_cap, nf));
         CU_RET(grow(sc.d_nok, sc.nok_cap, nf));
-        const size_t pass = (size_t) std::min<int64_t>(search_pass(search->nodes), cfg->nfix);
-        CU_RET(grow(sc.d_hits, sc.hits_cap, pass * GPSB200_SEARCH_MAX_OK(search->nodes) * sizeof(SearchHit) / sizeof(double)));
-        if (ms) CU_RET(grow(sc.d_ms, sc.ms_cap, nf * nchan));
-        if (node_rms) CU_RET(grow(sc.d_node_rms, sc.node_rms_cap, nf * search->nodes));
-        sc.search_cfg = *search;
+        const size_t pass = (size_t) std::min<int64_t>(search_pass(nodes), cfg->nfix);
+        CU_RET(grow(sc.d_hits, sc.hits_cap, pass * GPSB200_SEARCH_MAX_OK(nodes) * sizeof(SearchHit) / sizeof(double)));
+        if (st.node_rms) CU_RET(grow(sc.d_node_rms, sc.node_rms_cap, nf * nodes));
+        sc.search_cfg = *st.search;
     }
+    sc.want_ms = st.ms != nullptr;
+    sc.want_node_rms = st.node_rms != nullptr;
     // the reference channel of the nominal receive time: the lowest with a valid, healthy ephemeris (a coarse-time call
     // has no anchors and no nominal receive time)
     sc.ref = -1;
-    for (int c = 0; c < nchan && sc.ref < 0 && !coarse && !search; c++)
+    for (int c = 0; c < nchan && sc.ref < 0 && !st.coarse && !st.search; c++)
         if (chans[c].eph.valid && chans[c].eph.health == 0) sc.ref = c;
     sc.ref_sample = sc.ref >= 0 ? epochs[(size_t) sc.ref * max_epochs + chans[sc.ref].anchor_epoch].sample : 0;
     sc.ref_ms = sc.ref >= 0 ? chans[sc.ref].anchor_ms : 0;
@@ -1848,29 +1517,17 @@ cudaError_t run(Scratch &sc, const gpsb200_pvt_chan_t *chans, int nchan, const g
     CU_RET(cudaMemcpyAsync(sc.d_chans, chans, nchan * sizeof(gpsb200_pvt_chan_t), cudaMemcpyHostToDevice, s));
     CU_RET(cudaMemcpyAsync(sc.d_n, nepochs, nchan * sizeof(int32_t), cudaMemcpyHostToDevice, s));
     CU_RET(launch(sc, s));
-    CU_RET(cudaMemcpyAsync(fixes, sc.d_fixes, (size_t) cfg->nfix * sizeof(gpsb200_fix_t), cudaMemcpyDeviceToHost, s));
-    if (residuals)
-        CU_RET(cudaMemcpyAsync(residuals, sc.d_res, (size_t) cfg->nfix * nchan * sizeof(double), cudaMemcpyDeviceToHost, s));
-    if (raim)
-        CU_RET(cudaMemcpyAsync(out, sc.d_raim, (size_t) cfg->nfix * sizeof(gpsb200_raim_t), cudaMemcpyDeviceToHost, s));
-    if (araim)
-        CU_RET(cudaMemcpyAsync(aout, sc.d_araim, (size_t) cfg->nfix * sizeof(gpsb200_araim_t), cudaMemcpyDeviceToHost,
-                               s));
-    if (coarse) {
-        CU_RET(cudaMemcpyAsync(cout, sc.d_coarse, (size_t) cfg->nfix * sizeof(gpsb200_coarse_t), cudaMemcpyDeviceToHost,
-                               s));
-        if (ms)
-            CU_RET(cudaMemcpyAsync(ms, sc.d_ms, (size_t) cfg->nfix * nchan * sizeof(int64_t), cudaMemcpyDeviceToHost, s));
-    }
-    if (search) {
-        CU_RET(cudaMemcpyAsync(sout, sc.d_search, (size_t) cfg->nfix * sizeof(gpsb200_search_t), cudaMemcpyDeviceToHost,
-                               s));
-        if (ms)
-            CU_RET(cudaMemcpyAsync(ms, sc.d_ms, (size_t) cfg->nfix * nchan * sizeof(int64_t), cudaMemcpyDeviceToHost, s));
-        if (node_rms)
-            CU_RET(cudaMemcpyAsync(node_rms, sc.d_node_rms, (size_t) cfg->nfix * search->nodes * sizeof(double),
-                                   cudaMemcpyDeviceToHost, s));
-    }
+    const auto down = [&](void *dst, const void *src, size_t bytes) {
+        return cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, s);
+    };
+    CU_RET(down(fixes, sc.d_fixes, nf * sizeof(gpsb200_fix_t)));
+    if (residuals) CU_RET(down(residuals, sc.d_res, nf * nchan * sizeof(double)));
+    if (st.raim) CU_RET(down(st.raim_out, sc.d_raim, nf * sizeof(gpsb200_raim_t)));
+    if (st.araim) CU_RET(down(st.araim_out, sc.d_araim, nf * sizeof(gpsb200_araim_t)));
+    if (st.coarse) CU_RET(down(st.coarse_out, sc.d_coarse, nf * sizeof(gpsb200_coarse_t)));
+    if (st.search) CU_RET(down(st.search_out, sc.d_search, nf * sizeof(gpsb200_search_t)));
+    if (st.ms) CU_RET(down(st.ms, sc.d_ms, nf * nchan * sizeof(int64_t)));
+    if (st.node_rms) CU_RET(down(st.node_rms, sc.d_node_rms, nf * st.search->nodes * sizeof(double)));
     CU_RET(cudaStreamSynchronize(s));
     sc.have_last = true;
     return cudaSuccess;

@@ -22,11 +22,30 @@ static_assert(sizeof(gpsb200_coarse_t) == 32, "gpsb200_coarse_t layout");
 static_assert(sizeof(gpsb200_search_config_t) == 32, "gpsb200_search_config_t layout");
 static_assert(sizeof(gpsb200_search_t) == 64, "gpsb200_search_t layout");
 
-// Empty when the call is well-formed (see the header). raim, araim, coarse and search may be NULL; at most one is not.
+// What a fix call runs beside the fixes: nothing (gpsb200_pvt), the RAIM or ARAIM stage, coarse-time fixes or searches.
+enum class Mode { plain, raim, araim, coarse, search };
+
+// A fix call's stage: at most one of raim, araim, coarse and search is set, each with the records [nfix] it fills.
+// ms [nfix][nchan] (coarse, search) and node_rms [nfix][nodes] (search) may stay NULL.
+struct Stage {
+    const gpsb200_raim_config_t *raim = nullptr;
+    gpsb200_raim_t *raim_out = nullptr;
+    const gpsb200_araim_config_t *araim = nullptr;
+    gpsb200_araim_t *araim_out = nullptr;
+    const gpsb200_coarse_config_t *coarse = nullptr;
+    gpsb200_coarse_t *coarse_out = nullptr;
+    const gpsb200_search_config_t *search = nullptr;
+    gpsb200_search_t *search_out = nullptr;
+    int64_t *ms = nullptr;
+    double *node_rms = nullptr;
+    Mode mode() const {
+        return raim ? Mode::raim : araim ? Mode::araim : coarse ? Mode::coarse : search ? Mode::search : Mode::plain;
+    }
+};
+
+// Empty when the call is well-formed (see the header).
 std::string check(const gpsb200_pvt_chan_t *chans, int nchan, const gpsb200_track_epoch_t *epochs, const int32_t *nepochs,
-                  int max_epochs, const gpsb200_pvt_config_t *cfg, const gpsb200_raim_config_t *raim,
-                  const gpsb200_araim_config_t *araim, const gpsb200_coarse_config_t *coarse = nullptr,
-                  const gpsb200_search_config_t *search = nullptr);
+                  int max_epochs, const gpsb200_pvt_config_t *cfg, const Stage &st);
 
 // The RAIM tables of gpsb200_raim_thresholds (raim_thresholds.cpp); false when p_fa or p_md is outside 1e-12..0.5.
 bool raim_thresholds(double p_fa, double p_md, double *T, double *lambda);
@@ -48,28 +67,27 @@ struct Scratch {
     int64_t ref_sample = 0, ref_ms = 0;
     gpsb200_pvt_config_t cfg{};
     bool want_res = false;
+    Mode mode = Mode::plain;
     // the RAIM stage of the previous call (gpsb200_pvt_raim), and the tables of the last p_fa / p_md seen
-    bool raim = false;
     gpsb200_raim_config_t raim_cfg{};
     gpsb200_raim_t *d_raim = nullptr;            // [nfix]
     size_t raim_cap = 0;
     double tab_p_fa = 0.0, tab_p_md = 0.0;       // 0: no tables yet
     double tab_T[GPSB200_RAIM_MAX_DOF] = {}, tab_lambda[GPSB200_RAIM_MAX_DOF] = {};
     // the ARAIM stage of the previous call (gpsb200_pvt_araim)
-    bool araim = false;
     gpsb200_araim_config_t araim_cfg{};
     gpsb200_araim_t *d_araim = nullptr;          // [nfix]
     size_t araim_cap = 0;
     double kfa_h[GPSB200_RAIM_MAX_DOF] = {}, kfa_v[GPSB200_RAIM_MAX_DOF] = {};
     // the coarse-time call of the previous call (gpsb200_pvt_coarse)
-    bool coarse = false, want_ms = false;
+    bool want_ms = false;
     gpsb200_coarse_config_t coarse_cfg{};
     gpsb200_coarse_t *d_coarse = nullptr;        // [nfix]
     size_t coarse_cap = 0;
     int64_t *d_ms = nullptr;                     // [nfix][nchan]
     size_t ms_cap = 0;
     // the search of the previous call (gpsb200_pvt_search): records, and the per-instant scratch of pvt.cu's kernels
-    bool search = false, want_node_rms = false;
+    bool want_node_rms = false;
     gpsb200_search_config_t search_cfg{};
     gpsb200_search_t *d_search = nullptr;        // [nfix]
     size_t search_cap = 0;
@@ -86,19 +104,12 @@ struct Scratch {
 };
 
 void scratch_free(Scratch &sc);
-// Upload, run k_pvt on s and download the fixes (and residuals when not NULL); waits for the results. With raim
-// (not NULL) the kernel's RAIM instantiation runs and out [nfix] receives its records; with araim (not NULL) the ARAIM
-// instantiation and aout [nfix]; with coarse (not NULL) k_pvt_coarse, cout [nfix] and ms [nfix][nchan] (may be NULL).
-// With search (not NULL) the search kernels, sout [nfix], ms and node_rms [nfix][nodes] (may be NULL). At most one of
-// raim, araim, coarse and search is not NULL.
+// Upload, run the kernels of st's stage on s and download the fixes [nfix], the residuals [nfix][nchan] (when not NULL)
+// and the stage's outputs; waits for the results.
 cudaError_t run(Scratch &sc, const gpsb200_pvt_chan_t *chans, int nchan, const gpsb200_track_epoch_t *epochs,
-                const int32_t *nepochs, int max_epochs, const gpsb200_pvt_config_t *cfg,
-                const gpsb200_raim_config_t *raim, gpsb200_fix_t *fixes, double *residuals, gpsb200_raim_t *out,
-                cudaStream_t s, const gpsb200_araim_config_t *araim = nullptr, gpsb200_araim_t *aout = nullptr,
-                const gpsb200_coarse_config_t *coarse = nullptr, gpsb200_coarse_t *cout = nullptr,
-                int64_t *ms = nullptr, const gpsb200_search_config_t *search = nullptr,
-                gpsb200_search_t *sout = nullptr, double *node_rms = nullptr);
-// Enqueue k_pvt again on the previous call's device-resident inputs.
+                const int32_t *nepochs, int max_epochs, const gpsb200_pvt_config_t *cfg, gpsb200_fix_t *fixes,
+                double *residuals, const Stage &st, cudaStream_t s);
+// Enqueue the previous call's kernels again on its device-resident inputs.
 cudaError_t replay(Scratch &sc, cudaStream_t s);
 // gpsb200_search_nodes: xyz [n][3], the ECEF positions of the n-node search grid.
 void search_nodes(int n, double *xyz);

@@ -177,7 +177,8 @@ def test_bad_configs_are_refused_before_anything_runs(tmp_path):
 
 
 def test_winner_equals_the_coarse_kernel_from_its_node(tmp_path):
-    """The search restates k_pvt_coarse's solve: from the winner node, gpsb200_pvt_coarse gives the same bytes."""
+    """The search runs k_pvt_coarse's solve (coarse_solve): from the winner node, gpsb200_pvt_coarse gives the same
+    bytes."""
     chans, eps, iono = sky12(tmp_path)
     ch = unanchored(chans)
     cfg = gps.pvt_config(30000, 2999993, 3, iono)
