@@ -358,6 +358,25 @@ int gpsb200_acquire(gpsb200_ctx_t *ctx, const void *iq, int64_t nsamples, int sa
  * the synthesis of that buffer -- and the call returns when the results (and grid, in host memory) are in. */
 int gpsb200_acquire_device(gpsb200_ctx_t *ctx, const void *iq_device, int64_t nsamples, int sample_size,
                            const gpsb200_acq_config_t *cfg, gpsb200_acq_result_t *res, uint64_t *grid, void *stream);
+/* ---- per-PRN Doppler windows: the search above with a bin grid of each PRN's own (DESIGN §9.1) ----------------------
+ * A warm start (gpsb200_almanac_predict) knows each visible PRN's Doppler to a few hundred Hz and searches a few bins
+ * around it instead of the whole grid. The arguments are gpsb200_acquire's plus f_lo_prn[cfg->nprn]:
+ *   bins       bin j of the p-th requested PRN (cfg->prn[p]) is f_{p,j} = f_lo_prn[p] + j * cfg->step_hz, j < cfg->nbins;
+ *              cfg->f_lo_hz is ignored; every f_lo_prn[p] finite and every bin within +-1.5 MHz
+ *   the rest   samples, window, u_{p,j} = (uint32) llround(f_{p,j} * 2^32 / 3e6), tables, replica, K, P, the argmax with
+ *              its tie rules and p2: as above, per PRN over its own bins; res[p].doppler_hz = f_{p,j1}
+ * So row p of the result (and of the grid) equals gpsb200_acquire run with prn = {cfg->prn[p]} and f_lo_hz = f_lo_prn[p],
+ * bit for bit. Every argument is checked before anything is enqueued (GPSB200_ERR_ARG; f_lo_prn NULL included). */
+int gpsb200_acquire_windows(gpsb200_ctx_t *ctx, const void *iq, int64_t nsamples, int sample_size,
+                            const gpsb200_acq_config_t *cfg, const double *f_lo_prn, gpsb200_acq_result_t *res,
+                            uint64_t *grid);
+/* Test hook: the CTAs per (bin, PRN) row of a search of nprn x nbins rows on this context's device (1, 2, 3, 4 or 6; a
+ * split search gives the same results, DESIGN §9.1). force 0 restores the automatic choice, 1, 2, 3, 4 or 6 fixes every
+ * later search of the context to that split, -1 leaves the setting; GPSB200_ERR_ARG otherwise. Enqueues nothing. */
+int gpsb200_debug_acq_split(gpsb200_ctx_t *ctx, int force, int nprn, int nbins);
+int gpsb200_acquire_windows_device(gpsb200_ctx_t *ctx, const void *iq_device, int64_t nsamples, int sample_size,
+                                   const gpsb200_acq_config_t *cfg, const double *f_lo_prn, gpsb200_acq_result_t *res,
+                                   uint64_t *grid, void *stream);
 
 /* ---- tracking: code and carrier loops over an I/Q stream, one coherent period per C/A code epoch ---------------------
  * A closed loop per channel, sequential in time, in exact integer arithmetic so that it is reproducible bit for bit
@@ -1005,6 +1024,55 @@ typedef struct gpsb200_almanac_record {
 /* Parse a SEM file into rec[0..31] (indexed by svid - 1); *valid = 1 when at least one record is complete. Returns
  * GPSB200_ERR_ARG when the file cannot be opened. For tests (the parser against the reference's, field by field). */
 int gpsb200_almanac_read(const char *path, gpsb200_almanac_record_t rec[32], int32_t *valid);
+
+/* ---- almanac from decoded words (host; csrc/navdecode.cpp) ----------------------------------------------------------
+ * Input: word records of one channel, as for gpsb200_nav_ephemeris; a subframe counts when its 10 words are in sequence
+ * and all pass parity. Pages read (IS-GPS-200 20.3.3.5.1.2), all with data ID 1 (bits 23-22 of word 3's data):
+ *   almanac    subframe 4 or 5 with SV ID (bits 21-16 of word 3) 1..32 -- subframe 5 pages 1-24, subframe 4 pages 2-5
+ *              and 7-10. Fields, two's complement where signed, times exact powers of two, in the units of
+ *              gpsb200_almanac_read (angles in semicircles): e (w3 bits 15-0, 2^-21), toa (w4 23-16, 2^12 s), delta_i
+ *              (w4 15-0, 2^-19), OMEGADOT (w5 23-8, 2^-38), health (w5 7-0), sqrt A (w6, 2^-11), OMEGA0 (w7, 2^-23),
+ *              omega (w8, 2^-23), M0 (w9, 2^-23), af0 (11 bits: w10 23-16 above w10 4-2, 2^-20), af1 (w10 15-5, 2^-38).
+ *              The last such page of an SV in the words wins; rec[svid - 1] gets svid and valid = 1; svn, ura and
+ *              config_code are not broadcast and stay 0. SV ID 0 (a dummy page) decodes to nothing.
+ *   WNa        subframe 5 page 25 (SV ID 51): toa (bits 15-8) and WNa (bits 7-0); the last one wins. *wna_out = WNa, or
+ *              -1 when no such page was read. Every decoded record's toa_week is WNa resolved to the full week within
+ *              -128..127 of `week` (the meaning gpsb200_almanac_read gives it), -1 when there is no WNa.
+ * Subframe 4 page 18 (ionosphere and UTC) is gpsb200_nav_ephemeris's. Records not decoded are all 0.
+ * What the scenario engine sends, and so what a decode of its stream gives:
+ *   - every page's health is 0 (the reference writes 000);
+ *   - a SEM record cut short by the end of the file is sent in subframe 5 with the fields that were read;
+ *   - the engine scales OMEGADOT, af1 (2^-38) and OMEGA0, omega, M0 (2^-23) by decimal literals that are not exactly
+ *     powers of two (3.63797880709171e-12, 1.19209289550781e-07), so its integer is trunc(SEM / literal), which can
+ *     differ by one LSB from trunc(SEM / 2^-k); decoded here with 2^-k, such a field is within one LSB of the SEM value.
+ * GPSB200_ERR_ARG on a bad argument (NULL rec, n < 0, words NULL with n > 0). */
+int gpsb200_nav_almanac(const gpsb200_nav_word_t *words, int64_t n, int32_t week, gpsb200_almanac_record_t rec[32],
+                        int32_t *wna_out);
+
+/* ---- where each satellite is in the sky, from an almanac (host; csrc/almanac.cpp; tests/almanac_model.py) -----------
+ * For rec[i] (svid i + 1) with valid != 0, svid != 0 and toa_week >= 0, at GPS time (week, sow) of a receiver at ECEF
+ * x_a (m), static. FP64, pi = 3.1415926535898 for semicircles, the constants of gps.h (GM, OMEGA_E, c, lambda_L1):
+ *   orbit(t)   IS-GPS-200's almanac orbit: t_k = (week_t - toa_week) 604800 + sow_t - toa_sec; A = sqrt_A^2,
+ *              n = sqrt(GM / A^3), M = M0 + n t_k; E by Newton from E = M until |dE| <= 1e-14 (at most 10 steps);
+ *              i = 0.30 + delta_i (semicircles); no harmonic terms, no delta n, no IDOT; OMEGA = OMEGA0 +
+ *              (OMEGADOT - OMEGA_E) t_k - OMEGA_E toa_sec; position and velocity as the ephemeris orbit's (DESIGN §11)
+ *              with those terms zero; clock dt = af0 + af1 t_k
+ *   transmit   tau1 = |orbit(t).p - x_a| / c; the satellite is orbit(t - tau1)
+ *   sight      as §11's: tau = |p - x_a| / c, p and v turned about z by OMEGA_E tau; l = p' - x_a, R = |l|; azimuth and
+ *              elevation of l in the frame at x_a's geodetic latitude / longitude (six fixed-point steps, as ecef_llh)
+ *   out        el_deg, az_deg (0..360) in degrees; range_m = R - c dt; range rate r = l . v' / R;
+ *              doppler_hz = -(r - c af1) / lambda_L1, the sign of the scenario's f_carr, where the acquisition peaks
+ * out[i].prn = i + 1; out[i].valid = 0 (the rest 0) for records not predicted. GPSB200_ERR_ARG for a NULL argument, a
+ * non-finite sow or x_a. */
+typedef struct gpsb200_sky {
+    int32_t prn;
+    int32_t valid;
+    double el_deg, az_deg;
+    double range_m;
+    double doppler_hz;
+} gpsb200_sky_t;           /* 40 bytes */
+int gpsb200_almanac_predict(const gpsb200_almanac_record_t rec[32], int32_t week, double sow, const double x_a[3],
+                            gpsb200_sky_t out[32]);
 /* Assistance data for gpsb200_pvt_coarse: the ephemeris of a RINEX-2 (rinex3 = 0) or RINEX-3 (rinex3 = 1) navigation
  * file, read by the scenario engine's readers. eph[prn - 1] is the PRN's record whose toe (week and second) is nearest
  * to GPS time (week, sow), the first such record on ties, among those within 7200 s; valid = 0 where there is none. The

@@ -19,6 +19,7 @@ from .api import (  # noqa: F401
     RAIM_MAX_EXCLUDE, raim_config, raim_thresholds, ARAIM_CONFIG_DTYPE, ARAIM_DTYPE, araim_config, araim_kfa,
     COARSE_CONFIG_DTYPE, COARSE_DTYPE, FIX_AMBIGUOUS, coarse_config, rinex_ephemeris,
     SEARCH_CONFIG_DTYPE, SEARCH_DTYPE, SEARCH_NODES, search_config, search_nodes,
+    SKY_DTYPE, nav_almanac, almanac_predict,
 )
 from .synthetic import synthetic_chans  # noqa: F401,E402
 from . import sharding  # noqa: F401,E402

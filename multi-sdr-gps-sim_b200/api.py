@@ -75,6 +75,7 @@ class SteerState(C.Structure):
 
 assert C.sizeof(SteerState) == 64
 
+ERR_ARG = -1
 ERR_END = -6
 # the keys of the reference's interactive mode (gui.h:25-32, gps-sim.c:336-401)
 KEYS = "adwseqtgxX"
@@ -336,6 +337,38 @@ def nav_ephemeris(words):
     return eph[0], iono[0]
 
 
+def nav_almanac(words, week):
+    """gpsb200_nav_almanac: the almanac of the subframe 4 / 5 pages in the word records (NAV_WORD_DTYPE, in order), WNa
+    resolved to the full week within -128..127 of `week`. -> (ALMANAC_RECORD_DTYPE[32] indexed by svid - 1, WNa or -1)."""
+    w = np.ascontiguousarray(words, dtype=NAV_WORD_DTYPE)
+    rec = np.zeros(32, ALMANAC_RECORD_DTYPE)
+    wna = C.c_int32(0)
+    rc = lib().gpsb200_nav_almanac(w.ctypes.data if w.size else None, w.size, int(week), rec.ctypes.data, C.byref(wna))
+    if rc:
+        raise GpsB200Error(rc, "gpsb200_nav_almanac")
+    return rec, int(wna.value)
+
+
+# gpsb200_sky_t: one row per PRN 1..32
+SKY_DTYPE = np.dtype([("prn", "<i4"), ("valid", "<i4"), ("el_deg", "<f8"), ("az_deg", "<f8"), ("range_m", "<f8"),
+                      ("doppler_hz", "<f8")])
+assert SKY_DTYPE.itemsize == 40
+
+
+def almanac_predict(rec, week, sow, x_a):
+    """gpsb200_almanac_predict: elevation, azimuth, range and the Doppler the acquisition peaks at of every almanac
+    record (ALMANAC_RECORD_DTYPE[32], e.g. from nav_almanac or almanac_read) at GPS time (week, sow) for a static
+    receiver at ECEF x_a (m). -> SKY_DTYPE[32]; rows with valid 0 were not predicted."""
+    r = np.ascontiguousarray(rec, dtype=ALMANAC_RECORD_DTYPE)
+    assert r.size == 32
+    x = np.ascontiguousarray(x_a, dtype=np.float64).reshape(3)
+    out = np.zeros(32, SKY_DTYPE)
+    rc = lib().gpsb200_almanac_predict(r.ctypes.data, int(week), float(sow), x.ctypes.data, out.ctypes.data)
+    if rc:
+        raise GpsB200Error(rc, "gpsb200_almanac_predict")
+    return out
+
+
 def nav_time_anchor(words, sync):
     """gpsb200_nav_time_anchor: (anchor_epoch, anchor_ms) of a tracked channel from the words and sync nav_decode
     returned for its epochs; anchor_epoch is -1 when no HOW passed parity."""
@@ -366,7 +399,9 @@ _lib = None
 EXPORTS = ["gpsb200_create", "gpsb200_destroy", "gpsb200_last_error", "gpsb200_version", "gpsb200_set_nav",
            "gpsb200_synth_blocks", "gpsb200_synth_blocks_scatter", "gpsb200_synth_blocks_device", "gpsb200_replay_device",
            "gpsb200_carrier_advance", "gpsb200_carrier_chain", "gpsb200_carrier_chain_device", "gpsb200_carrier_probe_fixup",
-           "gpsb200_codegen", "gpsb200_acquire", "gpsb200_acquire_device", "gpsb200_track_start", "gpsb200_track",
+           "gpsb200_codegen", "gpsb200_acquire", "gpsb200_acquire_device", "gpsb200_acquire_windows",
+           "gpsb200_acquire_windows_device", "gpsb200_debug_acq_split", "gpsb200_nav_almanac", "gpsb200_almanac_predict", "gpsb200_track_start",
+           "gpsb200_track",
            "gpsb200_track_device", "gpsb200_nav_decode", "gpsb200_nav_word_check", "gpsb200_nav_parity",
            "gpsb200_nav_ephemeris", "gpsb200_nav_time_anchor", "gpsb200_pvt", "gpsb200_pvt_replay",
            "gpsb200_pvt_raim", "gpsb200_raim_thresholds", "gpsb200_pvt_araim", "gpsb200_araim_kfa", "gpsb200_pvt_coarse", "gpsb200_pvt_search", "gpsb200_search_nodes", "gpsb200_rinex_ephemeris", "gpsb200_bind_numa", "gpsb200_span_chain_host", "gpsb200_lanes_model_block",
@@ -459,6 +494,13 @@ def lib():
                                       C.c_void_p]
         L.gpsb200_acquire_device.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.POINTER(AcqConfig),
                                              C.c_void_p, C.c_void_p, C.c_void_p]
+        L.gpsb200_acquire_windows.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.POINTER(AcqConfig),
+                                              C.c_void_p, C.c_void_p, C.c_void_p]
+        L.gpsb200_acquire_windows_device.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.POINTER(AcqConfig),
+                                                     C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+        L.gpsb200_debug_acq_split.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int]
+        L.gpsb200_nav_almanac.argtypes = [C.c_void_p, C.c_int64, C.c_int32, C.c_void_p, C.POINTER(C.c_int32)]
+        L.gpsb200_almanac_predict.argtypes = [C.c_void_p, C.c_int32, C.c_double, C.c_void_p, C.c_void_p]
         L.gpsb200_track_start.argtypes = [C.c_int, C.c_double, C.c_int64, C.c_void_p]
         L.gpsb200_track.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_int64, C.c_void_p, C.c_int, C.c_int,
                                     C.c_void_p, C.c_void_p]
@@ -986,6 +1028,46 @@ class Context:
             rc = lib().gpsb200_acquire(self._h, a.ctypes.data, n, int(sample_size), C.byref(cfg), res.ctypes.data, gp)
         self._check(rc)
         return (res, grid) if want_grid else res
+
+    def acquire_windows(self, iq=None, sample_size=SC08, prns=(), f_lo_prn=(), step=250.0, nbins=5, ms=10, s0=0,
+                        want_grid=False, device_ptr=None, nsamples=None, stream=0):
+        """The acquisition search with a Doppler window per PRN (gpsb200_acquire_windows; DESIGN §9.1): bin j of
+        prns[p] is f_lo_prn[p] + j * step, j < nbins; everything else as acquire, whose arguments these are. Row p
+        equals acquire(prns=[prns[p]], f_lo=f_lo_prn[p], ...) bit for bit.
+        -> results ACQ_RESULT_DTYPE[nprn], and with want_grid also the power grid uint64[nprn, nbins, 3000]."""
+        prns = [int(p) for p in prns]
+        flo = np.ascontiguousarray(f_lo_prn, dtype=np.float64).reshape(-1)
+        if flo.size != len(prns):
+            raise GpsB200Error(ERR_ARG, "acquire_windows: %d first bins for %d PRNs" % (flo.size, len(prns)))
+        cfg = AcqConfig()
+        cfg.s0, cfg.ms, cfg.nprn = int(s0), int(ms), len(prns)
+        for i, p in enumerate(prns[:32]):   # more than 32 is rejected by the library with the other argument checks
+            cfg.prn[i] = p
+        cfg.f_lo_hz, cfg.step_hz, cfg.nbins = 0.0, float(step), int(nbins)
+        res = np.zeros(max(1, min(len(prns), 32)), ACQ_RESULT_DTYPE)
+        grid = np.zeros((max(1, len(prns)), max(1, int(nbins)), ACQ_CODE_SAMPLES), np.uint64) if want_grid else None
+        gp = None if grid is None else grid.ctypes.data
+        fp = flo.ctypes.data if flo.size else None
+        if device_ptr is not None:
+            assert iq is None and nsamples is not None
+            rc = lib().gpsb200_acquire_windows_device(self._h, C.c_void_p(device_ptr), int(nsamples), int(sample_size),
+                                                      C.byref(cfg), fp, res.ctypes.data, gp, C.c_void_p(stream))
+        else:
+            a = np.ascontiguousarray(iq)
+            n = a.size // 2 if nsamples is None else int(nsamples)
+            assert n <= a.size // 2
+            rc = lib().gpsb200_acquire_windows(self._h, a.ctypes.data, n, int(sample_size), C.byref(cfg), fp,
+                                               res.ctypes.data, gp)
+        self._check(rc)
+        return (res, grid) if want_grid else res
+
+    def debug_acq_split(self, nprn, nbins, force=-1):
+        """gpsb200_debug_acq_split: the CTAs per row a search of nprn x nbins rows uses on this context; force 0
+        restores the automatic choice, 1/2/3/4/6 fixes it for every later search, -1 leaves it."""
+        rc = lib().gpsb200_debug_acq_split(self._h, int(force), int(nprn), int(nbins))
+        if rc < 0:
+            self._check(rc)
+        return rc
 
     def track(self, states, iq=None, sample_size=SC08, base=0, max_epochs=None, device_ptr=None, nsamples=None, stream=0):
         """Code and carrier tracking (gpsb200_track; DESIGN §10) of the channels `states` (TRACK_STATE_DTYPE[nchan], e.g.

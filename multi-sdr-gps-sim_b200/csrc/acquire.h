@@ -23,30 +23,41 @@ constexpr int kExclude = 3;                    // P2 excludes delays within +-3 
 struct Scratch {
     int16_t *d_edges = nullptr;        // [33][kMaxEdges] sign-change positions of every PRN's replica, row 0 unused
     int32_t *d_nedges = nullptr;       // [33]
-    uint64_t *d_grid = nullptr;        // [nprn][nbins][3000] when the caller wants the grid
+    uint64_t *d_grid = nullptr;        // [nprn][nbins][3000] when the caller wants the grid or the search is split
     size_t grid_cap = 0;
     uint64_t *d_rows = nullptr;        // [nprn][nbins][3]: P1, P2, tau1 of every row
     size_t rows_cap = 0;
     gpsb200_acq_result_t *d_res = nullptr, *h_res = nullptr;   // [32]
-    uint32_t *d_u = nullptr;           // [nbins] phase steps
+    uint32_t *d_u = nullptr;           // [nbins] phase steps; with per-PRN windows [nprn][nbins]
     size_t u_cap = 0;
     int32_t *d_prn = nullptr;          // [32]
+    double *d_flo = nullptr;           // [32] first bin of each PRN's window (gpsb200_acquire_windows)
+    int sms = 0;                       // SM count of the device (the split rule)
+    int force_split = 0;               // 0: the split rule; else the split of every search (a test hook)
 };
 
 // Empty when the search is well-formed: PRNs 1..32, 1 <= K <= 100, 1 <= nbins <= GPSB200_ACQ_MAX_BINS, every bin within
-// +-1.5 MHz, sample size SC08/SC16, a window [s0, s0 + 3000 K + 2999) inside a buffer of nsamples samples.
-std::string check(const gpsb200_acq_config_t *cfg, int64_t nsamples, int sample_size);
+// +-1.5 MHz, sample size SC08/SC16, a window [s0, s0 + 3000 K + 2999) inside a buffer of nsamples samples. With
+// windows, the bins are f_lo_prn[p] + j step_hz (f_lo_prn not NULL) and cfg->f_lo_hz is not looked at.
+std::string check(const gpsb200_acq_config_t *cfg, int64_t nsamples, int sample_size, bool windows = false,
+                  const double *f_lo_prn = nullptr);
+// The CTAs per row of a search of `rows` = nprn x nbins rows on `sms` SMs: of 1, 2, 3, 4, 6 the one with the least
+// per-SM work when the CTAs spread evenly, ceil(rows split / sms) / split, the smallest on ties; split_of applies a
+// forced split instead when one is set. split_allowed: whether a split is one of those.
+int split_for(int rows, int sms);
+int split_of(const Scratch &sc, int nprn, int nbins);
+bool split_allowed(int split);
 // Samples the search reads from s0 on: 3000 K + 2999.
 int64_t window_samples(const gpsb200_acq_config_t *cfg);
 // Phase step of bin j: (uint32) llround(f_j * 2^32 / 3e6).
 uint32_t phase_step(double f_hz);
 
-cudaError_t scratch_reserve(Scratch &sc, const gpsb200_acq_config_t *cfg, bool want_grid);
+cudaError_t scratch_reserve(Scratch &sc, const gpsb200_acq_config_t *cfg, bool windows, bool want_grid);
 void scratch_free(Scratch &sc);
 // Enqueue the search of the samples at `window` (the first sample is s0) on s; results land in sc.h_res after a
-// synchronize of s, the grid (want_grid) in sc.d_grid.
-cudaError_t launch(Scratch &sc, const void *window, int sample_size, const gpsb200_acq_config_t *cfg, bool want_grid,
-                   cudaStream_t s);
+// synchronize of s, the grid (want_grid) in sc.d_grid. f_lo_prn (NULL: cfg->f_lo_hz for every PRN): per-PRN windows.
+cudaError_t launch(Scratch &sc, const void *window, int sample_size, const gpsb200_acq_config_t *cfg,
+                   const double *f_lo_prn, bool want_grid, cudaStream_t s);
 
 }  // namespace acq
 }  // namespace gpsb200

@@ -1094,24 +1094,29 @@ int carrier_chain_device(gpsb200_ctx *ctx, const gpsb200_chan_t *chans, int nblk
 }
 
 
-// The acquisition search of both entry points (acquire.cu). Everything is checked before anything is enqueued; a device
-// source is searched in place on the caller's stream, a host source's window is copied up first.
+// The acquisition search of the four entry points (acquire.cu): the standard one, and with `windows` the per-PRN Doppler
+// windows starting at f_lo_prn. Everything is checked before anything is enqueued; a device source is searched in place
+// on the caller's stream, a host source's window is copied up first.
 int acquire(gpsb200_ctx *ctx, const void *iq, int64_t nsamples, int sample_size, const gpsb200_acq_config_t *cfg,
-            gpsb200_acq_result_t *res, uint64_t *grid, bool device, cudaStream_t s) {
-    if (!iq || !res) return fail(ctx, GPSB200_ERR_ARG, "gpsb200_acquire: NULL source or result array");
-    const std::string bad = acq::check(cfg, nsamples, sample_size);
-    if (!bad.empty()) return fail(ctx, GPSB200_ERR_ARG, "gpsb200_acquire: " + bad);
-    int rc = device ? check_aligned(ctx, iq, "gpsb200_acquire_device", "iq_device") : GPSB200_OK;
+            bool windows, const double *f_lo_prn, gpsb200_acq_result_t *res, uint64_t *grid, bool device,
+            cudaStream_t s) {
+    const char *name = windows ? "gpsb200_acquire_windows" : "gpsb200_acquire";
+    if (!iq || !res) return fail(ctx, GPSB200_ERR_ARG, std::string(name) + ": NULL source or result array");
+    const std::string bad = acq::check(cfg, nsamples, sample_size, windows, f_lo_prn);
+    if (!bad.empty()) return fail(ctx, GPSB200_ERR_ARG, std::string(name) + ": " + bad);
+    int rc = device ? check_aligned(ctx, iq, windows ? "gpsb200_acquire_windows_device" : "gpsb200_acquire_device",
+                                    "iq_device")
+                    : GPSB200_OK;
     if (!rc) rc = check_entry(ctx);
     if (rc) return rc;
-    CU(acq::scratch_reserve(ctx->acq, cfg, grid != nullptr));
+    CU(acq::scratch_reserve(ctx->acq, cfg, windows, grid != nullptr));
     const size_t elem = sample_size == GPSB200_SC16 ? 2 : 1;
     const void *window = static_cast<const char *>(iq) + (size_t) cfg->s0 * 2 * elem;
     if (!device) {
         rc = stage_rx_source(ctx, window, (size_t) acq::window_samples(cfg) * 2 * elem, s, &window);
         if (rc) return rc;
     }
-    CU(acq::launch(ctx->acq, window, sample_size, cfg, grid != nullptr, s));
+    CU(acq::launch(ctx->acq, window, sample_size, cfg, windows ? f_lo_prn : nullptr, grid != nullptr, s));
     if (grid)
         CU(cudaMemcpy(grid, ctx->acq.d_grid, (size_t) cfg->nprn * cfg->nbins * acq::kCode * sizeof(uint64_t),
                       cudaMemcpyDeviceToHost));
@@ -1686,14 +1691,43 @@ int gpsb200_synth_blocks(gpsb200_ctx_t *ctx, const gpsb200_chan_t *chans, int nb
 int gpsb200_acquire(gpsb200_ctx_t *ctx, const void *iq, int64_t nsamples, int sample_size, const gpsb200_acq_config_t *cfg,
                     gpsb200_acq_result_t *res, uint64_t *grid) {
     if (!ctx) return GPSB200_ERR_ARG;
-    return settle(ctx, nullptr, acquire(ctx, iq, nsamples, sample_size, cfg, res, grid, false, ctx->s_compute));
+    return settle(ctx, nullptr, acquire(ctx, iq, nsamples, sample_size, cfg, false, nullptr, res, grid, false,
+                                        ctx->s_compute));
 }
 
 int gpsb200_acquire_device(gpsb200_ctx_t *ctx, const void *iq_device, int64_t nsamples, int sample_size,
                            const gpsb200_acq_config_t *cfg, gpsb200_acq_result_t *res, uint64_t *grid, void *stream_) {
     if (!ctx) return GPSB200_ERR_ARG;
     cudaStream_t s = stream_ ? (cudaStream_t) stream_ : ctx->s_compute;
-    return settle(ctx, s, acquire(ctx, iq_device, nsamples, sample_size, cfg, res, grid, true, s));
+    return settle(ctx, s, acquire(ctx, iq_device, nsamples, sample_size, cfg, false, nullptr, res, grid, true, s));
+}
+
+int gpsb200_acquire_windows(gpsb200_ctx_t *ctx, const void *iq, int64_t nsamples, int sample_size,
+                            const gpsb200_acq_config_t *cfg, const double *f_lo_prn, gpsb200_acq_result_t *res,
+                            uint64_t *grid) {
+    if (!ctx) return GPSB200_ERR_ARG;
+    return settle(ctx, nullptr, acquire(ctx, iq, nsamples, sample_size, cfg, true, f_lo_prn, res, grid, false,
+                                        ctx->s_compute));
+}
+
+int gpsb200_acquire_windows_device(gpsb200_ctx_t *ctx, const void *iq_device, int64_t nsamples, int sample_size,
+                                   const gpsb200_acq_config_t *cfg, const double *f_lo_prn, gpsb200_acq_result_t *res,
+                                   uint64_t *grid, void *stream_) {
+    if (!ctx) return GPSB200_ERR_ARG;
+    cudaStream_t s = stream_ ? (cudaStream_t) stream_ : ctx->s_compute;
+    return settle(ctx, s, acquire(ctx, iq_device, nsamples, sample_size, cfg, true, f_lo_prn, res, grid, true, s));
+}
+
+int gpsb200_debug_acq_split(gpsb200_ctx_t *ctx, int force, int nprn, int nbins) {
+    if (!ctx || !(force == -1 || force == 0 || acq::split_allowed(force)) || nprn < 1 || nprn > 32 || nbins < 1 ||
+        nbins > GPSB200_ACQ_MAX_BINS)
+        return GPSB200_ERR_ARG;
+    if (force >= 0) ctx->acq.force_split = force;
+    if (!ctx->acq.sms) {
+        if (!ctx->s_compute) return fail(ctx, GPSB200_ERR_CUDA, "context has no CUDA device");
+        CU(cudaDeviceGetAttribute(&ctx->acq.sms, cudaDevAttrMultiProcessorCount, ctx->cfg.device));
+    }
+    return acq::split_of(ctx->acq, nprn, nbins);
 }
 
 int gpsb200_track_start(int prn, double doppler_hz, int64_t sample, gpsb200_track_state_t *st) {

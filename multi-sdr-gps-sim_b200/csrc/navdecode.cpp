@@ -1,6 +1,7 @@
 // Bit sync, frame sync and word decoding of the 50 bit/s navigation message from the epochs of one tracked channel
 // (include/gpsb200.h: gpsb200_nav_decode; DESIGN §10), and the ephemeris, Klobuchar terms and transmit-time anchor the
-// words carry (gpsb200_nav_ephemeris, gpsb200_nav_time_anchor; DESIGN §11). Cheap and sequential: host code, shared by
+// words carry (gpsb200_nav_ephemeris, gpsb200_nav_time_anchor; DESIGN §11), and the almanac of subframes 4 and 5
+// (gpsb200_nav_almanac; DESIGN §9.1). Cheap and sequential: host code, shared by
 // the CLI and Python.
 #include <stdint.h>
 
@@ -40,6 +41,15 @@ double sext(uint32_t v, int bits) {
 
 // A 32-bit field split 8 + 24 over two words: the low 8 data bits of `hi`, all 24 of `lo`.
 int32_t split32(uint32_t hi, uint32_t lo) { return (int32_t) (((hi & 0xFFu) << 24) | (lo & 0xFFFFFFu)); }
+
+// Subframe starts: a TLM (index a multiple of 10) with its 9 successors in sequence and all 10 with good parity.
+// Returns the subframe id of the HOW, 0 when words[i] starts no such subframe.
+int subframe_id(const gpsb200_nav_word_t *words, int64_t n, int64_t i) {
+    if (i < 0 || i + 10 > n || words[i].index % 10 != 0) return 0;
+    for (int j = 0; j < 10; j++)
+        if (words[i + j].index != words[i].index + j || !words[i + j].parity_ok) return 0;
+    return (int) ((words[i + 1].data >> 2) & 7u);
+}
 
 // IS-GPS-200 scale factors; semicircles are turned into radians with the reference's pi (kPi).
 const double kP2m5 = 0.03125, kP2m19 = 1.0 / 524288.0, kP2m29 = 1.0 / 536870912.0, kP2m31 = 1.0 / 2147483648.0,
@@ -140,13 +150,7 @@ int gpsb200_nav_ephemeris(const gpsb200_nav_word_t *words, int64_t n, gpsb200_ep
     if (!eph || n < 0 || (n > 0 && !words)) return GPSB200_ERR_ARG;
     memset(eph, 0, sizeof *eph);
     if (iono) memset(iono, 0, sizeof *iono);
-    // subframe starts: a TLM (index a multiple of 10) with its 9 successors in sequence and all 10 with good parity
-    auto good_subframe = [&](int64_t i) -> int {
-        if (i < 0 || i + 10 > n || words[i].index % 10 != 0) return 0;
-        for (int j = 0; j < 10; j++)
-            if (words[i + j].index != words[i].index + j || !words[i + j].parity_ok) return 0;
-        return (int) ((words[i + 1].data >> 2) & 7u);
-    };
+    auto good_subframe = [&](int64_t i) { return subframe_id(words, n, i); };
     for (int64_t i = n - 30; i >= 0; i--) {
         if (good_subframe(i) != 1 || good_subframe(i + 10) != 2 || good_subframe(i + 20) != 3) continue;
         const gpsb200_nav_word_t *s1 = words + i, *s2 = words + i + 10, *s3 = words + i + 20;
@@ -199,6 +203,45 @@ int gpsb200_nav_ephemeris(const gpsb200_nav_word_t *words, int64_t n, gpsb200_ep
             iono->valid = 1;
             break;
         }
+    return GPSB200_OK;
+}
+
+int gpsb200_nav_almanac(const gpsb200_nav_word_t *words, int64_t n, int32_t week, gpsb200_almanac_record_t rec[32],
+                        int32_t *wna_out) {
+    if (!rec || n < 0 || (n > 0 && !words)) return GPSB200_ERR_ARG;
+    memset(rec, 0, 32 * sizeof *rec);
+    int32_t wna = -1;
+    for (int64_t i = 0; i + 10 <= n; i++) {
+        const int sf = subframe_id(words, n, i);
+        if (sf != 4 && sf != 5) continue;
+        const gpsb200_nav_word_t *s = words + i;
+        if (((s[2].data >> 22) & 3u) != 1u) continue;
+        const int svid = (int) ((s[2].data >> 16) & 0x3Fu);
+        if (sf == 5 && svid == 51) {
+            wna = (int32_t) (s[2].data & 0xFFu);
+            continue;
+        }
+        if (svid < 1 || svid > 32) continue;
+        gpsb200_almanac_record_t &r = rec[svid - 1];
+        r.svid = svid;
+        r.valid = 1;
+        r.e = (double) (s[2].data & 0xFFFFu) * std::ldexp(1.0, -21);
+        r.toa_sec = (double) ((s[3].data >> 16) & 0xFFu) * 4096.0;
+        r.delta_i = sext(s[3].data, 16) * std::ldexp(1.0, -19);
+        r.omegadot = sext(s[4].data >> 8, 16) * std::ldexp(1.0, -38);
+        r.health = (int32_t) (s[4].data & 0xFFu);
+        r.sqrta = (double) (s[5].data & 0xFFFFFFu) * std::ldexp(1.0, -11);
+        r.omega0 = sext(s[6].data, 24) * std::ldexp(1.0, -23);
+        r.aop = sext(s[7].data, 24) * std::ldexp(1.0, -23);
+        r.m0 = sext(s[8].data, 24) * std::ldexp(1.0, -23);
+        r.af0 = sext((((s[9].data >> 16) & 0xFFu) << 3) | ((s[9].data >> 2) & 7u), 11) * std::ldexp(1.0, -20);
+        r.af1 = sext(s[9].data >> 5, 11) * std::ldexp(1.0, -38);
+    }
+    // WNa (8 bits) to the full week nearest the caller's: within -128..127 of it
+    const int32_t full = wna < 0 ? -1 : week + (int32_t) ((((wna - week) % 256 + 256 + 128) % 256) - 128);
+    for (int sv = 0; sv < 32; sv++)
+        if (rec[sv].svid) rec[sv].toa_week = full;
+    if (wna_out) *wna_out = wna;
     return GPSB200_OK;
 }
 

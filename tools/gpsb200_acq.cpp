@@ -3,6 +3,12 @@
 // 3000 K + 2999 samples from the start offset -- and runs gpsb200_acquire on it; prints one line per PRN: best Doppler
 // bin, code delay (samples from the window start to the code's chip 0, and in chips), P1/P2 and whether P1/P2 reaches
 // the threshold. The search and its arithmetic are those of include/gpsb200.h (DESIGN §9).
+//
+// Warm start (--almanac, DESIGN §9.1): with a SEM almanac, an a-priori position and the GPS time of the window's first
+// sample, gpsb200_almanac_predict gives each PRN's elevation and Doppler; only the PRNs predicted at or above the mask
+// are searched, each over 2h + 1 bins of the --doppler step around its prediction (h = ceil(window / step)), starting
+// at step * round(f / step) - h * step so that the bins lie on the cold search's grid (gpsb200_acquire_windows). Each
+// line then also shows the predicted Doppler and elevation.
 #include <cmath>
 #include <cstdio>
 #include <cstdlib>
@@ -16,18 +22,28 @@
 // P1/P2 at or above which a PRN counts as acquired. Without noise, absent PRNs of the project's streams stay below 1.6
 // and present ones are far above 3 (tests/test_acquire.py fixes the bounds of both from the model).
 static const double kDefaultThreshold = 2.5;
+// Warm start: half-width of each PRN's Doppler window and the elevation mask. The almanac predicts the Doppler of the
+// project's streams to within 146 Hz (tests/test_almanac_decode.py), so +-500 Hz (5 bins at 250 Hz) holds it with room
+// for an a-priori a few tens of km and seconds off.
+static const double kDefaultWindow = 500.0, kDefaultMask = -5.0;
 
 static void usage() {
     fprintf(stderr,
             "gpsb200-acq FILE [--iq16] [--block B] [--offset-ms N] [--ms K] [--doppler LO,HI,STEP] [--prn LIST]\n"
             "            [--threshold R] [--device D]\n"
+            "            [--almanac FILE.sem --assist-pos LAT,LON,H --assist-time YYYY/MM/DD,hh:mm:ss[.s]\n"
+            "             [--window HZ] [--mask DEG]]\n"
             "  FILE              interleaved I,Q at 3 Msps, int8 (default) or int16 (--iq16)\n"
             "  --block B         start at 0.1 s block B (sample 300000 B); --offset-ms N adds N ms (3000 N samples)\n"
             "  --ms K            coherent 1 ms periods summed, 1..100 (default 10)\n"
             "  --doppler L,H,S   Doppler bins L, L+S, .. up to H, in Hz (default -5000,5000,250)\n"
             "  --prn LIST        e.g. 1-32 (default), 3,7,12-15\n"
-            "  --threshold R     P1/P2 at or above R counts as acquired (default %.1f)\n",
-            kDefaultThreshold);
+            "  --threshold R     P1/P2 at or above R counts as acquired (default %.1f)\n"
+            "  --almanac         warm start: search the PRNs of --prn predicted at or above the mask from the SEM file\n"
+            "                    at --assist-pos / --assist-time (GPS time of the window's first sample), each over\n"
+            "                    the bins of the --doppler step within --window Hz of its prediction (default %.0f)\n"
+            "  --mask DEG        elevation mask of the warm start (default %.0f)\n",
+            kDefaultThreshold, kDefaultWindow, kDefaultMask);
     exit(2);
 }
 
@@ -39,6 +55,10 @@ int main(int argc, char **argv) {
     gpsb200_acq_config_t cfg;
     memset(&cfg, 0, sizeof cfg);
     cfg.ms = 10;
+    const char *almanac = nullptr;
+    double x_a[3] = {0.0, 0.0, 0.0}, sow = 0.0, window = kDefaultWindow, mask = kDefaultMask;
+    int32_t week = 0;
+    bool have_pos = false, have_time = false;
     parse_prns("1-32", &cfg);
     for (int i = 1; i < argc; i++) {
         std::string a = argv[i];
@@ -56,13 +76,52 @@ int main(int argc, char **argv) {
             if (!parse_prns(val(), &cfg)) usage();
         } else if (a == "--threshold") threshold = atof(val());
         else if (a == "--device") device = atoi(val());
+        else if (a == "--almanac") almanac = val();
+        else if (a == "--assist-pos") {
+            if (!ecef_of_llh(val(), x_a)) usage();
+            have_pos = true;
+        } else if (a == "--assist-time") {
+            if (!gps_of_date(val(), week, sow)) usage();
+            have_time = true;
+        } else if (a == "--window") {
+            window = atof(val());
+            if (!(window >= 0.0)) usage();
+        } else if (a == "--mask") mask = atof(val());
         else if (a[0] != '-' && !path) path = argv[i];
         else usage();
     }
-    if (!path || block < 0 || offset_ms < 0) usage();
+    if (!path || block < 0 || offset_ms < 0 || (almanac && (!have_pos || !have_time)) ||
+        (!almanac && (have_pos || have_time)))
+        usage();
     cfg.f_lo_hz = lo;
     cfg.step_hz = step;
     cfg.nbins = (int) std::floor((hi - lo) / step + 1e-9) + 1;
+    // warm start: the PRNs of the list predicted at or above the mask, each with its own first bin
+    std::vector<double> f_lo_prn;
+    gpsb200_sky_t sky[32];
+    if (almanac) {
+        gpsb200_almanac_record_t rec[32];
+        int32_t valid = 0;
+        if (gpsb200_almanac_read(almanac, rec, &valid) != GPSB200_OK ||
+            gpsb200_almanac_predict(rec, week, sow, x_a, sky) != GPSB200_OK) {
+            fprintf(stderr, "gpsb200-acq: cannot read the almanac of %s\n", almanac);
+            return 1;
+        }
+        const int h = (int) std::ceil(window / step - 1e-9);
+        int n = 0;
+        for (int i = 0; i < cfg.nprn; i++) {
+            const gpsb200_sky_t &k = sky[cfg.prn[i] - 1];
+            if (!k.valid || !(k.el_deg >= mask)) continue;
+            cfg.prn[n++] = cfg.prn[i];
+            f_lo_prn.push_back(step * std::round(k.doppler_hz / step) - h * step);
+        }
+        cfg.nprn = n;
+        cfg.nbins = 2 * h + 1;
+        if (n == 0) {
+            printf("# %s: no PRN of the list is predicted at or above %.1f deg\n", path, mask);
+            return 0;
+        }
+    }
 
     const size_t elem = ss == GPSB200_SC16 ? 2 : 1;
     const long long s0 = block * GPSB200_BLOCK_SAMPLES + offset_ms * GPSB200_ACQ_CODE_SAMPLES;
@@ -88,22 +147,33 @@ int main(int argc, char **argv) {
     gpsb200_ctx_t *ctx = nullptr;
     int rc = create_rx_context(device, &ctx);
     std::vector<gpsb200_acq_result_t> res(cfg.nprn);
-    if (rc == GPSB200_OK) rc = gpsb200_acquire(ctx, buf.data(), need, ss, &cfg, res.data(), nullptr);
+    if (rc == GPSB200_OK)
+        rc = almanac ? gpsb200_acquire_windows(ctx, buf.data(), need, ss, &cfg, f_lo_prn.data(), res.data(), nullptr)
+                     : gpsb200_acquire(ctx, buf.data(), need, ss, &cfg, res.data(), nullptr);
     if (rc != GPSB200_OK) {
         fprintf(stderr, "gpsb200-acq: %s\n", ctx ? gpsb200_last_error(ctx) : "cannot create a context");
         gpsb200_destroy(ctx);
         return 1;
     }
     gpsb200_destroy(ctx);
-    printf("# %s: sample %lld, %d ms, %d bins %.1f .. %.1f Hz, threshold P1/P2 >= %.2f\n", path, s0, cfg.ms, cfg.nbins, lo,
-           lo + (cfg.nbins - 1) * step, threshold);
-    printf("# PRN  doppler_hz  delay_samples  delay_chips  P1/P2  acquired\n");
+    if (almanac) {
+        printf("# %s: sample %lld, %d ms, warm start from %s: %d PRN(s) at or above %.1f deg, %d bins of %.1f Hz "
+               "around each prediction, threshold P1/P2 >= %.2f\n",
+               path, s0, cfg.ms, almanac, cfg.nprn, mask, cfg.nbins, step, threshold);
+        printf("# PRN  doppler_hz  delay_samples  delay_chips  P1/P2  acquired  predicted_hz  elevation_deg\n");
+    } else {
+        printf("# %s: sample %lld, %d ms, %d bins %.1f .. %.1f Hz, threshold P1/P2 >= %.2f\n", path, s0, cfg.ms,
+               cfg.nbins, lo, lo + (cfg.nbins - 1) * step, threshold);
+        printf("# PRN  doppler_hz  delay_samples  delay_chips  P1/P2  acquired\n");
+    }
     int nacq = 0;
     for (const auto &r : res) {
         const bool acq = r.ratio >= threshold;
         nacq += acq;
-        printf("%5d  %10.1f  %13d  %11.3f  %8.3f  %s\n", r.prn, r.doppler_hz, r.delay, r.delay_chips, r.ratio,
+        printf("%5d  %10.1f  %13d  %11.3f  %8.3f  %s", r.prn, r.doppler_hz, r.delay, r.delay_chips, r.ratio,
                acq ? "yes" : "no");
+        if (almanac) printf("  %12.1f  %13.2f", sky[r.prn - 1].doppler_hz, sky[r.prn - 1].el_deg);
+        printf("\n");
     }
     printf("# %d of %d acquired\n", nacq, cfg.nprn);
     return 0;

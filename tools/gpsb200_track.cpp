@@ -150,22 +150,6 @@ static int print_fixes(gpsb200_ctx_t *ctx, const std::vector<gpsb200_pvt_chan_t>
     return GPSB200_OK;
 }
 
-// GPS week and second of a calendar date and time (GPS time, no leap seconds): days since 1980-01-06.
-static bool gps_of_date(const char *text, int32_t &week, double &sow) {
-    int y, mo, d, hh, mm;
-    double sec;
-    if (sscanf(text, "%d/%d/%d,%d:%d:%lf", &y, &mo, &d, &hh, &mm, &sec) != 6 || y < 1980 || mo < 1 || mo > 12 || d < 1 ||
-        d > 31 || hh < 0 || hh > 23 || mm < 0 || mm > 59 || !(sec >= 0.0 && sec < 60.0))
-        return false;
-    const int a = (14 - mo) / 12, yy = y + 4800 - a, m = mo + 12 * a - 3;
-    const long jdn = d + (153 * m + 2) / 5 + 365L * yy + yy / 4 - yy / 100 + yy / 400 - 32045;
-    const long days = jdn - 2444245;                // 1980-01-06
-    if (days < 0) return false;
-    week = (int32_t) (days / 7);
-    sow = (double) (days % 7) * 86400.0 + hh * 3600.0 + mm * 60.0 + sec;
-    return true;
-}
-
 int main(int argc, char **argv) {
     const char *path = nullptr;
     int ss = GPSB200_SC08, device = 0;
@@ -245,14 +229,7 @@ int main(int argc, char **argv) {
             i++;
             assist_pos = assist_search = true;
         } else if (a == "--assist-pos") {
-            double llh[3];
-            if (sscanf(val(), "%lf,%lf,%lf", &llh[0], &llh[1], &llh[2]) != 3) usage();
-            const double kA = 6378137.0, kE2 = 0.0818191908426 * 0.0818191908426;   // WGS-84
-            const double la = llh[0] * M_PI / 180.0, lo = llh[1] * M_PI / 180.0;
-            const double N = kA / sqrt(1.0 - kE2 * sin(la) * sin(la));
-            ap.x_a[0] = (N + llh[2]) * cos(la) * cos(lo);
-            ap.x_a[1] = (N + llh[2]) * cos(la) * sin(lo);
-            ap.x_a[2] = (N * (1.0 - kE2) + llh[2]) * sin(la);
+            if (!ecef_of_llh(val(), ap.x_a)) usage();
             assist_pos = true;
         } else if (a == "--assist-time") {
             if (!gps_of_date(val(), ap.week, ap.t_a)) usage();
