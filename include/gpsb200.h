@@ -909,6 +909,84 @@ int gpsb200_pvt_search(gpsb200_ctx_t *ctx, const gpsb200_pvt_chan_t *chans, int 
                        const gpsb200_pvt_config_t *cfg, const gpsb200_search_config_t *search, gpsb200_fix_t *fixes,
                        double *residuals, gpsb200_search_t *out, int64_t *ms, double *node_rms);
 
+/* ---- snapshot measurement: a fine code phase and carrier step from an acquisition, without tracking (DESIGN §11.5;
+ * tests/snapshot_model.py states it in numpy). An acquisition peak is quantised to one sample (99.9 m of range) and one
+ * Doppler bin; this refines each acquired PRN, over the window the search ran on, to a measurement the coarse-time fix
+ * can use. Exact integer arithmetic, with the tracker's pieces (samples, tables, wipe-off, replica c(x) = 2 ca[x >> 32]
+ * - 1, M = 1023 * 2^32, H = 2^31, angle(), "/" truncating, ">>" floor; the gpsb200_track header). For each PRN p of the
+ * search (res[p], K = acq->ms, window samples m = 0 .. 3000 K - 1 after s0, chunk k = samples 3000 k .. 3000 k + 2999):
+ *   0. Weak: unless res[p].ratio >= cfg->min_ratio the record is the seed of step 1 with status GPSB200_SNAP_WEAK,
+ *      iterations 0, last_step 0 and power 0: it is never refined.
+ *   1. Seed (as gpsb200_track_start): w = (int32) llround(doppler_hz * 2^32 / 3e6), u = clamp(NOM + w / 1540, MIN, MAX),
+ *      phi = (M - (delay * u) mod M) mod M: the prompt phase at s0 that wraps at s0 + delay.
+ *   2. Frequency pass at (phi, u, w): prompt sums P_I,k, P_Q,k (int32) with the replica at (phi + m u) mod M and the
+ *      carrier index ((uint32) (m w)) >> 23, continuous over the window. power = sum_k P_I,k^2 + P_Q,k^2. With K >= 2:
+ *      per pair (k, k + 1) cross = P_I,k P_Q,k+1 - P_Q,k P_I,k+1, dot = P_I,k P_I,k+1 + P_Q,k P_Q,k+1, both negated
+ *      when dot < 0 (data bits drop out, as in the FLL); d = angle(sum dot, sum cross) in 2^-32 turns per 3000 samples;
+ *      w += d / 3000, u = clamp(NOM + w / 1540). K = 1 leaves w and u.
+ *   3. Code: `iterations` passes at the current phi and the fixed u, w, each with the early ((p + H) mod M), late
+ *      ((p - H) mod M) and prompt replicas: E = sum_k E_I,k^2 + E_Q,k^2, L and power likewise (int64); E and L shifted
+ *      right by max(0, bitlen(E + L) - 40); D = ((E - L) * 2^14) / (E + L) (0 when E + L = 0); phi = (phi + D *
+ *      GPSB200_SNAP_GAIN) mod M. On the ideal triangle D ~ -4 delta 2^14 for a replica delta chips ahead, so the step
+ *      is half a Newton step: the full step limit-cycles on the sampled correlation. last_step = the last D.
+ *   4. Status GPSB200_SNAP_NO_CONVERGENCE when iterations >= 1 and |last_step| > GPSB200_SNAP_MAX_LAST_D (a step above a
+ *      thousandth of a chip), else GPSB200_SNAP_OK.
+ * Bounds: |I_d|, |Q_d| <= 2 * 128 * 250, so a chunk sum is at most 3000 * 64000 = 1.92e8 < 2^31 in magnitude; |(I_d,
+ * Q_d)| <= 181.02 * 250.46 (the tables' largest modulus), so a chunk's squared magnitude is at most 1.85e16 and E, L,
+ * power <= K * 1.85e16, E + L <= 3.7e18 < 2^63 for K <= 100; |cross|, dot <= 1.85e16 per pair, sums <= 99 * 1.85e16. */
+#define GPSB200_SNAP_MAX_ITER   16
+#define GPSB200_SNAP_ITERATIONS 12            /* the default */
+#define GPSB200_SNAP_GAIN       32768         /* 2^15: the step in 2^-32 chips per unit of D */
+#define GPSB200_SNAP_MAX_LAST_D 131           /* 131 * 2^15 < 2^32 / 1000 */
+enum { GPSB200_SNAP_OK = 0, GPSB200_SNAP_WEAK = 1, GPSB200_SNAP_NO_CONVERGENCE = 2 };
+typedef struct gpsb200_snapshot_config {
+    double min_ratio;      /* refined when res.ratio >= min_ratio (gpsb200-acq's threshold: 2.5); finite, >= 0 */
+    int32_t iterations;    /* code passes: 0..GPSB200_SNAP_MAX_ITER */
+    int32_t reserved;      /* 0 */
+} gpsb200_snapshot_config_t;   /* 16 bytes */
+typedef struct gpsb200_snapshot {
+    int32_t prn;
+    int32_t status;        /* GPSB200_SNAP_* */
+    int64_t sample;        /* s0: the instant the measurement holds at */
+    uint64_t code_phase;   /* prompt code phase at `sample`, 2^-32 chips, < 1023 * 2^32 */
+    uint32_t code_step;    /* u, 2^-32 chips per sample */
+    int32_t carr_step;     /* w, 3e6 / 2^32 Hz */
+    int32_t iterations;    /* code passes run */
+    int32_t last_step;     /* D of the last code pass (0 with none) */
+    uint64_t power;        /* prompt power of the last pass */
+    double ratio;          /* res.ratio */
+} gpsb200_snapshot_t;      /* 56 bytes */
+/* Refine the results res [acq->nprn] of a search run with acq on nsamples samples of host memory (the search's
+ * arguments: the same window must lie in the buffer) into out [acq->nprn], in the order of acq->prn. acq may be the
+ * config of gpsb200_acquire or of gpsb200_acquire_windows: its bins (f_lo_hz, step_hz, nbins) are neither read nor
+ * checked. Every argument is checked before anything is enqueued (GPSB200_ERR_ARG: s0, ms, nprn, prn and the window
+ * as gpsb200_acquire checks them, res[p].prn == acq->prn[p], delays 0..2999, |doppler_hz| <= 10 kHz -- the seed is
+ * gpsb200_track_start's, with its range, which keeps w and the refined w far inside int32 -- the config in
+ * range). Blocking. */
+int gpsb200_snapshot_measure(gpsb200_ctx_t *ctx, const void *iq, int64_t nsamples, int sample_size,
+                             const gpsb200_acq_config_t *acq, const gpsb200_acq_result_t *res,
+                             const gpsb200_snapshot_config_t *cfg, gpsb200_snapshot_t *out);
+/* Same for a source in device memory (16-byte aligned), measured in place on `stream` (0 = the context's own stream)
+ * behind whatever it holds; returns when the records are in host memory. */
+int gpsb200_snapshot_measure_device(gpsb200_ctx_t *ctx, const void *iq_device, int64_t nsamples, int sample_size,
+                                    const gpsb200_acq_config_t *acq, const gpsb200_acq_result_t *res,
+                                    const gpsb200_snapshot_config_t *cfg, gpsb200_snapshot_t *out, void *stream);
+/* ---- fixes from snapshot records (DESIGN §11.5): gpsb200_pvt_coarse and gpsb200_pvt_search with meas [nsnap][nchan]
+ * in place of the epochs. Snapshot i's fix instant is its records' common `sample` (all nchan records of a row must hold
+ * the same sample, 0..2^62; else GPSB200_ERR_ARG); cfg->nfix is nsnap (>= 1); cfg->iono, alpha and beta apply; cfg->s0
+ * and cfg->step are not read. Channel c is used at snapshot i when meas[i][c].status is GPSB200_SNAP_OK, meas[i][c].prn
+ * equals chans[c].prn, eph.valid, eph.health == 0 and |t_a(s) - toe| <= 7200 s; its measurement is frac =
+ * code_phase / (1023 2^32) ms and rate = -lambda carr_step 3e6 / 2^32. Everything else is gpsb200_pvt_coarse's
+ * (gpsb200_pvt_search's) procedure, records and checks, unchanged; anchors are not read. gpsb200_pvt_replay re-runs the
+ * call when it ran last. */
+int gpsb200_pvt_snapshot(gpsb200_ctx_t *ctx, const gpsb200_pvt_chan_t *chans, int nchan, const gpsb200_snapshot_t *meas,
+                         const gpsb200_pvt_config_t *cfg, const gpsb200_coarse_config_t *apriori, gpsb200_fix_t *fixes,
+                         double *residuals, gpsb200_coarse_t *out, int64_t *ms);
+int gpsb200_pvt_snapshot_search(gpsb200_ctx_t *ctx, const gpsb200_pvt_chan_t *chans, int nchan,
+                                const gpsb200_snapshot_t *meas, const gpsb200_pvt_config_t *cfg,
+                                const gpsb200_search_config_t *search, gpsb200_fix_t *fixes, double *residuals,
+                                gpsb200_search_t *out, int64_t *ms, double *node_rms);
+
 /* ---- scenario engine: the reference's host path outside the sample loop -------------
  * RINEX-2/3 navigation file (plain or gzip-compressed, read through zlib like the reference, gps.c:1147) +
  * location/motion -> the gpsb200_chan_t records and NAV frames the

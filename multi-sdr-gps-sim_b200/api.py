@@ -281,6 +281,23 @@ def search_config(t_a, s_a=0, week=0, nodes=SEARCH_NODES):
     return c
 
 
+# gpsb200_snapshot_config_t / gpsb200_snapshot_t (DESIGN §11.5)
+SNAPSHOT_CONFIG_DTYPE = np.dtype([("min_ratio", "<f8"), ("iterations", "<i4"), ("reserved", "<i4")])
+SNAPSHOT_DTYPE = np.dtype([("prn", "<i4"), ("status", "<i4"), ("sample", "<i8"), ("code_phase", "<u8"),
+                           ("code_step", "<u4"), ("carr_step", "<i4"), ("iterations", "<i4"), ("last_step", "<i4"),
+                           ("power", "<u8"), ("ratio", "<f8")])
+assert (SNAPSHOT_CONFIG_DTYPE.itemsize, SNAPSHOT_DTYPE.itemsize) == (16, 56)
+SNAP_OK, SNAP_WEAK, SNAP_NO_CONVERGENCE = 0, 1, 2
+SNAP_ITERATIONS, SNAP_MAX_ITER = 12, 16
+
+
+def snapshot_config(min_ratio=2.5, iterations=SNAP_ITERATIONS):
+    """A SNAPSHOT_CONFIG_DTYPE record: the acquisition ratio a PRN needs to be refined, and the code iterations."""
+    c = np.zeros(1, SNAPSHOT_CONFIG_DTYPE)[0]
+    c["min_ratio"], c["iterations"] = float(min_ratio), int(iterations)
+    return c
+
+
 def search_nodes(n=SEARCH_NODES):
     """gpsb200_search_nodes: the ECEF positions float64[n, 3] of the n-node search grid."""
     xyz = np.zeros((max(1, int(n)), 3))
@@ -404,7 +421,7 @@ EXPORTS = ["gpsb200_create", "gpsb200_destroy", "gpsb200_last_error", "gpsb200_v
            "gpsb200_track",
            "gpsb200_track_device", "gpsb200_nav_decode", "gpsb200_nav_word_check", "gpsb200_nav_parity",
            "gpsb200_nav_ephemeris", "gpsb200_nav_time_anchor", "gpsb200_pvt", "gpsb200_pvt_replay",
-           "gpsb200_pvt_raim", "gpsb200_raim_thresholds", "gpsb200_pvt_araim", "gpsb200_araim_kfa", "gpsb200_pvt_coarse", "gpsb200_pvt_search", "gpsb200_search_nodes", "gpsb200_rinex_ephemeris", "gpsb200_bind_numa", "gpsb200_span_chain_host", "gpsb200_lanes_model_block",
+           "gpsb200_pvt_raim", "gpsb200_raim_thresholds", "gpsb200_pvt_araim", "gpsb200_araim_kfa", "gpsb200_pvt_coarse", "gpsb200_pvt_search", "gpsb200_search_nodes", "gpsb200_snapshot_measure", "gpsb200_snapshot_measure_device", "gpsb200_pvt_snapshot", "gpsb200_pvt_snapshot_search", "gpsb200_rinex_ephemeris", "gpsb200_bind_numa", "gpsb200_span_chain_host", "gpsb200_lanes_model_block",
            "gpsb200_lanes_window_band_host", "gpsb200_slice_prepare", "gpsb200_slice_probe",
            "gpsb200_slice_finish", "gpsb200_slice_finish_cb", "gpsb200_slice_wait", "gpsb200_link_apply", "gpsb200_slice_link_host", "gpsb200_debug_corrupt_chain", "gpsb200_synth_kernel_name",
            "gpsb200_debug_run_checkpoints", "gpsb200_checkpoint_segments_host",
@@ -524,6 +541,12 @@ def lib():
         L.gpsb200_pvt_coarse.argtypes = L.gpsb200_pvt_raim.argtypes + [C.c_void_p]
         L.gpsb200_pvt_search.argtypes = L.gpsb200_pvt_coarse.argtypes + [C.c_void_p]
         L.gpsb200_search_nodes.argtypes = [C.c_int, C.c_void_p]
+        L.gpsb200_snapshot_measure.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.POINTER(AcqConfig),
+                                               C.c_void_p, C.c_void_p, C.c_void_p]
+        L.gpsb200_snapshot_measure_device.argtypes = L.gpsb200_snapshot_measure.argtypes + [C.c_void_p]
+        L.gpsb200_pvt_snapshot.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
+                                           C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+        L.gpsb200_pvt_snapshot_search.argtypes = L.gpsb200_pvt_snapshot.argtypes + [C.c_void_p]
         L.gpsb200_rinex_ephemeris.argtypes = [C.c_char_p, C.c_int, C.c_int32, C.c_double, C.c_void_p]
         _lib = L
     return _lib
@@ -1168,6 +1191,81 @@ class Context:
                                              None if res is None else res.ctypes.data, out.ctypes.data,
                                              None if ms is None else ms.ctypes.data,
                                              None if nr is None else nr.ctypes.data))
+        return ((fixes, out) + ((res,) if want_residuals else ()) + ((ms,) if want_ms else ())
+                + ((nr,) if want_node_rms else ()))
+
+    def snapshot_measure(self, res, iq=None, sample_size=SC08, ms=10, s0=0, prns=None, f_lo=-5000.0, step=250.0,
+                         nbins=41, cfg=None, device_ptr=None, nsamples=None, stream=0):
+        """Refine acquisition results to snapshot measurements (gpsb200_snapshot_measure; DESIGN §11.5). res: the
+        ACQ_RESULT_DTYPE rows a search returned; ms, s0, prns (default res["prn"]), f_lo, step and nbins: the search's
+        arguments (acquire's); cfg: SNAPSHOT_CONFIG_DTYPE record (snapshot_config(), the default). Source as acquire.
+        -> SNAPSHOT_DTYPE[nprn] in the order of res."""
+        r = np.ascontiguousarray(res, dtype=ACQ_RESULT_DTYPE).reshape(-1)
+        prns = [int(p) for p in (r["prn"] if prns is None else prns)]
+        acq = AcqConfig()
+        acq.s0, acq.ms, acq.nprn = int(s0), int(ms), len(prns)
+        for i, p in enumerate(prns[:32]):
+            acq.prn[i] = p
+        acq.f_lo_hz, acq.step_hz, acq.nbins = float(f_lo), float(step), int(nbins)
+        sc = np.array(snapshot_config() if cfg is None else cfg, dtype=SNAPSHOT_CONFIG_DTYPE).reshape(1)
+        if r.size < len(prns):
+            raise GpsB200Error(ERR_ARG, "snapshot_measure: %d results for %d PRNs" % (r.size, len(prns)))
+        out = np.zeros(max(1, len(prns)), SNAPSHOT_DTYPE)
+        if device_ptr is not None:
+            assert iq is None and nsamples is not None
+            rc = lib().gpsb200_snapshot_measure_device(self._h, C.c_void_p(device_ptr), int(nsamples), int(sample_size),
+                                                       C.byref(acq), r.ctypes.data, sc.ctypes.data, out.ctypes.data,
+                                                       C.c_void_p(stream))
+        else:
+            a = np.ascontiguousarray(iq)
+            n = a.size // 2 if nsamples is None else int(nsamples)
+            assert n <= a.size // 2
+            rc = lib().gpsb200_snapshot_measure(self._h, a.ctypes.data, n, int(sample_size), C.byref(acq), r.ctypes.data,
+                                                sc.ctypes.data, out.ctypes.data)
+        self._check(rc)
+        return out[:len(prns)]
+
+    @staticmethod
+    def _snapshot_args(chans, meas, cfg, want_residuals):
+        ch = np.ascontiguousarray(chans, dtype=PVT_CHAN_DTYPE).reshape(-1)
+        m = np.ascontiguousarray(meas, dtype=SNAPSHOT_DTYPE)
+        if m.ndim == 1:
+            m = m.reshape(1, -1)
+        assert m.ndim == 2 and m.shape[0] >= 1 and m.shape[1] == ch.size, (m.shape, ch.size)
+        cf = np.array(cfg, dtype=PVT_CONFIG_DTYPE).reshape(1).copy()
+        cf[0]["nfix"] = m.shape[0]
+        fixes = np.zeros(max(1, m.shape[0]), FIX_DTYPE)
+        res = np.zeros((fixes.size, max(1, ch.size))) if want_residuals else None
+        return ch, m, cf, fixes, res
+
+    def pvt_snapshot(self, chans, meas, cfg, apriori, want_residuals=False, want_ms=False):
+        """Coarse-time fixes from snapshot records (gpsb200_pvt_snapshot; DESIGN §11.5). meas: SNAPSHOT_DTYPE
+        [nsnap, nchan], row i the records of snapshot i with column c for chans[c] (a 1-D array is one snapshot); cfg:
+        PVT_CONFIG_DTYPE record whose iono terms apply (nfix is set to nsnap, s0 and step are not read); apriori:
+        COARSE_CONFIG_DTYPE record. -> pvt_coarse's tuple."""
+        ch, m, cf, fixes, res = self._snapshot_args(chans, meas, cfg, want_residuals)
+        ap = np.array(apriori, dtype=COARSE_CONFIG_DTYPE).reshape(1)
+        out = np.zeros(fixes.size, COARSE_DTYPE)
+        ms = np.zeros((fixes.size, max(1, ch.size)), np.int64) if want_ms else None
+        self._check(lib().gpsb200_pvt_snapshot(self._h, ch.ctypes.data, ch.size, m.ctypes.data, cf.ctypes.data,
+                                               ap.ctypes.data, fixes.ctypes.data,
+                                               None if res is None else res.ctypes.data, out.ctypes.data,
+                                               None if ms is None else ms.ctypes.data))
+        return (fixes, out) + ((res,) if want_residuals else ()) + ((ms,) if want_ms else ())
+
+    def pvt_snapshot_search(self, chans, meas, cfg, search, want_residuals=False, want_ms=False, want_node_rms=False):
+        """Position searches from snapshot records (gpsb200_pvt_snapshot_search; DESIGN §11.5): pvt_snapshot's
+        arguments with search (SEARCH_CONFIG_DTYPE record) in place of apriori. -> pvt_search's tuple."""
+        ch, m, cf, fixes, res = self._snapshot_args(chans, meas, cfg, want_residuals)
+        sc = np.array(search, dtype=SEARCH_CONFIG_DTYPE).reshape(1)
+        out = np.zeros(fixes.size, SEARCH_DTYPE)
+        ms = np.zeros((fixes.size, max(1, ch.size)), np.int64) if want_ms else None
+        nr = np.zeros((fixes.size, max(1, int(sc[0]["nodes"]))), np.float64) if want_node_rms else None
+        self._check(lib().gpsb200_pvt_snapshot_search(self._h, ch.ctypes.data, ch.size, m.ctypes.data, cf.ctypes.data,
+                                                      sc.ctypes.data, fixes.ctypes.data,
+                                                      None if res is None else res.ctypes.data, out.ctypes.data,
+                                                      None if ms is None else ms.ctypes.data,
+                                                      None if nr is None else nr.ctypes.data))
         return ((fixes, out) + ((res,) if want_residuals else ()) + ((ms,) if want_ms else ())
                 + ((nr,) if want_node_rms else ()))
 

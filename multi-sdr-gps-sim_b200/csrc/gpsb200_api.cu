@@ -29,6 +29,7 @@
 
 #include "../../include/gpsb200.h"
 #include "acquire.h"
+#include "snapshot.h"
 #include "device_buffer.h"
 #include "track.h"
 #include "pvt.h"
@@ -214,6 +215,7 @@ struct gpsb200_ctx {
     acq::Scratch acq;                      // acquisition searches (acquire.cu), allocated by the first one
     trk::Scratch trk;                      // tracking calls (track.cu), allocated by the first one
     pvt::Scratch pvt;                      // position fixes (pvt.cu), allocated by the first one
+    snap::Scratch snap;                    // snapshot measurements (snapshot.cu), allocated by the first one
     std::string err;
 };
 
@@ -1144,6 +1146,30 @@ int track(gpsb200_ctx *ctx, const void *iq, int64_t nsamples, int sample_size, i
     return GPSB200_OK;
 }
 
+// The snapshot measurement of both entry points (snapshot.cu). Everything is checked before anything is enqueued; a
+// device source is measured in place on the caller's stream, a host source's window is copied up first.
+int snapshot_measure(gpsb200_ctx *ctx, const void *iq, int64_t nsamples, int sample_size, const gpsb200_acq_config_t *acq,
+                     const gpsb200_acq_result_t *res, const gpsb200_snapshot_config_t *cfg, gpsb200_snapshot_t *out,
+                     bool device, cudaStream_t s) {
+    const char *name = device ? "gpsb200_snapshot_measure_device" : "gpsb200_snapshot_measure";
+    if (!iq || !out) return fail(ctx, GPSB200_ERR_ARG, std::string(name) + ": NULL source or output");
+    const std::string bad = snap::check(acq, nsamples, sample_size, res, cfg);
+    if (!bad.empty()) return fail(ctx, GPSB200_ERR_ARG, std::string(name) + ": " + bad);
+    int rc = device ? check_aligned(ctx, iq, name, "iq_device") : GPSB200_OK;
+    if (!rc) rc = check_entry(ctx);
+    if (rc) return rc;
+    CU(trk::scratch_reserve(ctx->trk, 1, 1));   // the +-1 chips of every PRN
+    const size_t elem = sample_size == GPSB200_SC16 ? 2 : 1;
+    const void *window = static_cast<const char *>(iq) + (size_t) acq->s0 * 2 * elem;
+    if (!device) {
+        rc = stage_rx_source(ctx, window, (size_t) acq::window_samples(acq) * 2 * elem, s, &window);
+        if (rc) return rc;
+    }
+    snap::seed(acq, res, cfg, out);
+    CU(snap::launch(ctx->snap, window, sample_size, acq->ms, acq->nprn, ctx->trk.d_codes, cfg->iterations, out, s));
+    return GPSB200_OK;
+}
+
 // Position fixes (pvt.cu), with the stage st names (none: plain fixes). Everything is checked before anything is
 // enqueued.
 int pvt_fix(gpsb200_ctx *ctx, const char *fn, const gpsb200_pvt_chan_t *chans, int nchan,
@@ -1474,6 +1500,7 @@ void gpsb200_destroy(gpsb200_ctx_t *ctx) {
     cudaFreeHost(ctx->h_seg_end);
     acq::scratch_free(ctx->acq);
     trk::scratch_free(ctx->trk);
+    snap::scratch_free(ctx->snap);
     pvt::scratch_free(ctx->pvt);
     if (ctx->s_compute) cudaStreamDestroy(ctx->s_compute);
     if (ctx->s_copy) cudaStreamDestroy(ctx->s_copy);
@@ -1821,6 +1848,54 @@ int gpsb200_pvt_search(gpsb200_ctx_t *ctx, const gpsb200_pvt_chan_t *chans, int 
     st.ms = ms;
     st.node_rms = node_rms;
     return settle(ctx, nullptr, pvt_fix(ctx, "gpsb200_pvt_search", chans, nchan, epochs, nepochs, max_epochs, cfg, fixes,
+                                        residuals, st));
+}
+
+int gpsb200_snapshot_measure(gpsb200_ctx_t *ctx, const void *iq, int64_t nsamples, int sample_size,
+                             const gpsb200_acq_config_t *acq, const gpsb200_acq_result_t *res,
+                             const gpsb200_snapshot_config_t *cfg, gpsb200_snapshot_t *out) {
+    if (!ctx) return GPSB200_ERR_ARG;
+    return settle(ctx, nullptr, snapshot_measure(ctx, iq, nsamples, sample_size, acq, res, cfg, out, false,
+                                                 ctx->s_compute));
+}
+
+int gpsb200_snapshot_measure_device(gpsb200_ctx_t *ctx, const void *iq_device, int64_t nsamples, int sample_size,
+                                    const gpsb200_acq_config_t *acq, const gpsb200_acq_result_t *res,
+                                    const gpsb200_snapshot_config_t *cfg, gpsb200_snapshot_t *out, void *stream_) {
+    if (!ctx) return GPSB200_ERR_ARG;
+    cudaStream_t s = stream_ ? (cudaStream_t) stream_ : ctx->s_compute;
+    return settle(ctx, s, snapshot_measure(ctx, iq_device, nsamples, sample_size, acq, res, cfg, out, true, s));
+}
+
+int gpsb200_pvt_snapshot(gpsb200_ctx_t *ctx, const gpsb200_pvt_chan_t *chans, int nchan, const gpsb200_snapshot_t *meas,
+                         const gpsb200_pvt_config_t *cfg, const gpsb200_coarse_config_t *apriori, gpsb200_fix_t *fixes,
+                         double *residuals, gpsb200_coarse_t *out, int64_t *ms) {
+    if (!ctx) return GPSB200_ERR_ARG;
+    if (!apriori || !out || !meas)
+        return settle(ctx, nullptr, fail(ctx, GPSB200_ERR_ARG, "gpsb200_pvt_snapshot: NULL meas, apriori or out"));
+    pvt::Stage st;
+    st.coarse = apriori;
+    st.coarse_out = out;
+    st.ms = ms;
+    st.meas = meas;
+    return settle(ctx, nullptr, pvt_fix(ctx, "gpsb200_pvt_snapshot", chans, nchan, nullptr, nullptr, 1, cfg, fixes,
+                                        residuals, st));
+}
+
+int gpsb200_pvt_snapshot_search(gpsb200_ctx_t *ctx, const gpsb200_pvt_chan_t *chans, int nchan,
+                                const gpsb200_snapshot_t *meas, const gpsb200_pvt_config_t *cfg,
+                                const gpsb200_search_config_t *search, gpsb200_fix_t *fixes, double *residuals,
+                                gpsb200_search_t *out, int64_t *ms, double *node_rms) {
+    if (!ctx) return GPSB200_ERR_ARG;
+    if (!search || !out || !meas)
+        return settle(ctx, nullptr, fail(ctx, GPSB200_ERR_ARG, "gpsb200_pvt_snapshot_search: NULL meas, search or out"));
+    pvt::Stage st;
+    st.search = search;
+    st.search_out = out;
+    st.ms = ms;
+    st.node_rms = node_rms;
+    st.meas = meas;
+    return settle(ctx, nullptr, pvt_fix(ctx, "gpsb200_pvt_snapshot_search", chans, nchan, nullptr, nullptr, 1, cfg, fixes,
                                         residuals, st));
 }
 

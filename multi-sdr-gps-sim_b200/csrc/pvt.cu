@@ -864,6 +864,10 @@ struct CoarseArgs : Args {
     gpsb200_coarse_t *out;
     int64_t *ms;
 };
+// Fixes from snapshot records (DESIGN §11.5): the records [nfix][nchan] in place of the epochs.
+struct SnapCoarseArgs : CoarseArgs {
+    const gpsb200_snapshot_t *meas;
+};
 
 // Header step 3: the predicted transmit time (ms, satellite time) of a satellite at position x and receive time t, and
 // sin(elevation) seen along the up vector `up` (unit, ECEF).
@@ -895,11 +899,69 @@ __device__ inline void no_coarse(gpsb200_coarse_t &o, int ref) {
     o.reserved = 0;
 }
 
+// The two measurements of the coarse-time solve (header step 2 of gpsb200_pvt_coarse). Each gives a fix's instant
+// and, per lane: used, whether the channel is used at sample s and a-priori time tas; take, for a used channel, use =
+// true, its ephemeris, code phase (frac, ms), range rate (m/s) and the prediction of step 3 at x_a (pred, sel), and
+// nothing for the others. The body of take sits in each measurement so that the tracked one compiles as it did before
+// the snapshot one existed.
+// From tracked epochs at the instants s0 + i step.
+struct FromEpochs {
+    __device__ __forceinline__ int64_t instant(const Args &a, int64_t fi) const { return a.cfg.s0 + fi * a.cfg.step; }
+    __device__ __forceinline__ bool used(const Args &a, int lane, int64_t s, double tas,
+                                         const gpsb200_ephemeris_t &eph) const {
+        double frac, rate;
+        return locked_period(a, lane, s, frac, rate) >= 1 && fabs(wrap_half_week(tas - eph.toe)) <= 7200.0;
+    }
+    // locked_period, restated: calling it here made k_pvt_coarse take 25.55-25.60 ms against 25.22-25.48 ms and the
+    // 12-channel search 8 094 ms against 8 078 ms (tools/pvt_bench.py --coarse / --search, H100 80GB HBM3, 700 W).
+    __device__ __forceinline__ void take(const Args &a, int lane, int64_t s, double tas, const double *x_a,
+                                         const double *up, bool &use, const gpsb200_ephemeris_t *&eph, double &frac,
+                                         double &rate, double &pred, double &sel) const {
+        if (lane < a.nchan) {
+            const gpsb200_pvt_chan_t &c = a.ch[lane];
+            const gpsb200_track_epoch_t *e = a.ep + (size_t) lane * a.max_epochs;
+            const int k = c.eph.valid && c.eph.health == 0 ? find_period(e, a.n[lane], s) : -1;
+            if (k >= 1 && e[k - 1].lock && e[k].lock && fabs(wrap_half_week(tas - c.eph.toe)) <= 7200.0) {
+                use = true;
+                eph = &c.eph;
+                const uint64_t phi = (uint64_t) e[k - 1].code_phase + (uint64_t) (s - e[k].sample) * e[k - 1].code_step;
+                frac = (double) phi / kCodeMod;
+                rate = -kLambda * ((double) e[k - 1].carr_step * kStepHz);
+                pred = predict(*eph, x_a, tas, up, sel);
+            }
+        }
+    }
+};
+// From the snapshot records of one fix instant (row: the instant's nchan records); the instant is their sample.
+struct FromSnapshots {
+    const gpsb200_snapshot_t *row;
+    __device__ __forceinline__ int64_t instant(const Args &, int64_t) const { return row[0].sample; }
+    __device__ __forceinline__ bool used(const Args &a, int lane, int64_t, double tas,
+                                         const gpsb200_ephemeris_t &eph) const {
+        const gpsb200_snapshot_t &r = row[lane];
+        return r.status == GPSB200_SNAP_OK && r.prn == a.ch[lane].prn && eph.valid && eph.health == 0 &&
+               fabs(wrap_half_week(tas - eph.toe)) <= 7200.0;
+    }
+    __device__ __forceinline__ void take(const Args &a, int lane, int64_t s, double tas, const double *x_a,
+                                         const double *up, bool &use, const gpsb200_ephemeris_t *&eph, double &frac,
+                                         double &rate, double &pred, double &sel) const {
+        if (lane < a.nchan && used(a, lane, s, tas, a.ch[lane].eph)) {
+            use = true;
+            eph = &a.ch[lane].eph;
+            frac = (double) row[lane].code_phase / kCodeMod;
+            rate = -kLambda * ((double) row[lane].carr_step * kStepHz);
+            pred = predict(*eph, x_a, tas, up, sel);
+        }
+    }
+};
+
 // gpsb200_pvt_coarse's header steps 1-9 at sample s from the a-priori config ap: one warp, lane = channel, as k_pvt. The satellite is evaluated in every iteration, at the transmit time moved by the current delta. The fix and
-// coarse records come out uniform over the warp; resid, Nw and has are this lane's (channel's).
-__device__ __forceinline__ void coarse_solve(const Args &a, const gpsb200_coarse_config_t &ap, int64_t s, int lane,
-                                             gpsb200_fix_t &f, gpsb200_coarse_t &o, double &resid, int64_t &Nw,
-                                             bool &has) {
+// coarse records come out uniform over the warp; resid, Nw and has are this lane's (channel's). meas: the measurement
+// of step 2 (FromEpochs or FromSnapshots).
+template <class Meas>
+__device__ __forceinline__ void coarse_solve(const Args &a, const Meas &meas, const gpsb200_coarse_config_t &ap,
+                                             int64_t s, int lane, gpsb200_fix_t &f, gpsb200_coarse_t &o, double &resid,
+                                             int64_t &Nw, bool &has) {
     const double nan = __longlong_as_double(0x7ff8000000000000ll);
     // header step 1
     const int64_t ds = s - ap.s_a;
@@ -917,21 +979,7 @@ __device__ __forceinline__ void coarse_solve(const Args &a, const gpsb200_coarse
     Geo ga;
     ga.set(ap.x_a);
     const double up[3] = {ga.cla * ga.clo, ga.cla * ga.slo, ga.sla};
-    // locked_period, restated: calling it here made k_pvt_coarse take 25.55-25.60 ms against 25.22-25.48 ms and the
-    // 12-channel search 8 094 ms against 8 078 ms (tools/pvt_bench.py --coarse / --search, H100 80GB HBM3, 700 W).
-    if (lane < a.nchan) {
-        const gpsb200_pvt_chan_t &c = a.ch[lane];
-        const gpsb200_track_epoch_t *e = a.ep + (size_t) lane * a.max_epochs;
-        const int k = c.eph.valid && c.eph.health == 0 ? find_period(e, a.n[lane], s) : -1;
-        if (k >= 1 && e[k - 1].lock && e[k].lock && fabs(wrap_half_week(tas - c.eph.toe)) <= 7200.0) {
-            use = true;
-            eph = &c.eph;
-            const uint64_t phi = (uint64_t) e[k - 1].code_phase + (uint64_t) (s - e[k].sample) * e[k - 1].code_step;
-            frac = (double) phi / kCodeMod;
-            rate = -kLambda * ((double) e[k - 1].carr_step * kStepHz);
-            pred = predict(*eph, ap.x_a, tas, up, sel);
-        }
-    }
+    meas.take(a, lane, s, tas, ap.x_a, up, use, eph, frac, rate, pred, sel);
     has = use;
     const unsigned mask = __ballot_sync(kFull, use);
     const int nused = __popc(mask);
@@ -1029,23 +1077,34 @@ __device__ __forceinline__ void coarse_solve(const Args &a, const gpsb200_coarse
 // k_pvt_coarse: gpsb200_pvt_coarse (DESIGN §11.3), one warp per fix. kCoarseMinBlocks: held to 128 registers (some
 // spills) it ran 10 % faster than at its natural 168 with 3 CTAs per SM (DESIGN §11.3).
 constexpr int kCoarseMinBlocks = 4;
-__global__ void __launch_bounds__(kWarps * 32, kCoarseMinBlocks) k_pvt_coarse(const CoarseArgs a) {
-    const int lane = threadIdx.x & 31;
-    const int64_t fi = (int64_t) blockIdx.x * kWarps + (threadIdx.x >> 5);
-    if (fi >= a.cfg.nfix) return;   // the whole warp leaves together
+template <class Meas>
+__device__ __forceinline__ void coarse_fix(const CoarseArgs &a, const Meas &meas, int64_t fi, int lane) {
     const double nan = __longlong_as_double(0x7ff8000000000000ll);
     gpsb200_fix_t f;
     gpsb200_coarse_t o;
     double resid;
     int64_t Nw;
     bool has;
-    coarse_solve(a, a.ap, a.cfg.s0 + fi * a.cfg.step, lane, f, o, resid, Nw, has);
+    coarse_solve(a, meas, a.ap, meas.instant(a, fi), lane, f, o, resid, Nw, has);
     if (lane == 0) {
         a.fixes[fi] = f;
         a.out[fi] = o;
     }
     if (a.res && lane < a.nchan) a.res[fi * a.nchan + lane] = has ? resid : nan;
     if (a.ms && lane < a.nchan) a.ms[fi * a.nchan + lane] = has ? Nw : -1;
+}
+__global__ void __launch_bounds__(kWarps * 32, kCoarseMinBlocks) k_pvt_coarse(const CoarseArgs a) {
+    const int lane = threadIdx.x & 31;
+    const int64_t fi = (int64_t) blockIdx.x * kWarps + (threadIdx.x >> 5);
+    if (fi >= a.cfg.nfix) return;   // the whole warp leaves together
+    coarse_fix(a, FromEpochs(), fi, lane);
+}
+// gpsb200_pvt_snapshot: the same fixes from snapshot records.
+__global__ void __launch_bounds__(kWarps * 32, kCoarseMinBlocks) k_pvt_snapshot(const SnapCoarseArgs a) {
+    const int lane = threadIdx.x & 31;
+    const int64_t fi = (int64_t) blockIdx.x * kWarps + (threadIdx.x >> 5);
+    if (fi >= a.cfg.nfix) return;
+    coarse_fix(a, FromSnapshots{a.meas + fi * a.nchan}, fi, lane);
 }
 
 // ---- position search: coarse-time fixes from every node of a global grid (DESIGN §11.4) -----------------------------
@@ -1077,6 +1136,9 @@ struct SearchArgs : Args {
     int f0, nf;                // the instants f0 .. f0 + nf - 1 of this pass (k_pvt_search, k_search_pick)
     int max_ok;                // the list's length per instant: GPSB200_SEARCH_MAX_OK(nodes)
 };
+struct SnapSearchArgs : SearchArgs {
+    const gpsb200_snapshot_t *meas;   // [nfix][nchan]
+};
 
 // Node i of the n-node grid (header step 1): ECEF position x and the up vector at its geodetic latitude / longitude.
 __host__ __device__ inline void search_node(int64_t i, int n, double *x, double *up) {
@@ -1096,11 +1158,9 @@ __host__ __device__ inline void search_node(int64_t i, int n, double *x, double 
 
 // Per fix instant (one warp, lane = channel): header step 2's used channels and step 3's satellite positions; clears the
 // instant's counters.
-__global__ void __launch_bounds__(kWarps * 32) k_search_sats(const SearchArgs a) {
-    const int lane = threadIdx.x & 31;
-    const int64_t fi = (int64_t) blockIdx.x * kWarps + (threadIdx.x >> 5);
-    if (fi >= a.cfg.nfix) return;
-    const int64_t s = a.cfg.s0 + fi * a.cfg.step;
+template <class Meas>
+__device__ __forceinline__ void search_sats(const SearchArgs &a, const Meas &meas, int64_t fi, int lane) {
+    const int64_t s = meas.instant(a, fi);
     const int64_t ds = s - a.sc.s_a;
     const double u = a.sc.t_a + (double) ds / 3e6;
     const double tas = u - 604800.0 * floor(u / 604800.0);
@@ -1108,8 +1168,7 @@ __global__ void __launch_bounds__(kWarps * 32) k_search_sats(const SearchArgs a)
     double p[3] = {0.0, 0.0, 0.0};
     if (lane < a.nchan) {
         const gpsb200_ephemeris_t &eph = a.ch[lane].eph;
-        double frac, rate;
-        if (locked_period(a, lane, s, frac, rate) >= 1 && fabs(wrap_half_week(tas - eph.toe)) <= 7200.0) {
+        if (meas.used(a, lane, s, tas, eph)) {
             use = true;
             double v[3], dt, ddt;
             satellite(eph, tas - 0.075, p, v, dt, ddt);
@@ -1123,14 +1182,25 @@ __global__ void __launch_bounds__(kWarps * 32) k_search_sats(const SearchArgs a)
         a.nok[fi] = 0;
     }
 }
+__global__ void __launch_bounds__(kWarps * 32) k_search_sats(const SearchArgs a) {
+    const int lane = threadIdx.x & 31;
+    const int64_t fi = (int64_t) blockIdx.x * kWarps + (threadIdx.x >> 5);
+    if (fi >= a.cfg.nfix) return;
+    search_sats(a, FromEpochs(), fi, lane);
+}
+__global__ void __launch_bounds__(kWarps * 32) k_snapshot_sats(const SnapSearchArgs a) {
+    const int lane = threadIdx.x & 31;
+    const int64_t fi = (int64_t) blockIdx.x * kWarps + (threadIdx.x >> 5);
+    if (fi >= a.cfg.nfix) return;
+    search_sats(a, FromSnapshots{a.meas + fi * a.nchan}, fi, lane);
+}
 
 // Header steps 3-4 over the grid: one warp per 32 nodes of one fix instant (blockIdx.y). Each lane tests its own node's
 // visibility; the warp then solves the visible nodes one after another, lane = channel, and appends the OK ones to the
 // instant's list. Testing 32 nodes per warp keeps the warps busy although most nodes fail the test.
 constexpr int kSearchMinBlocks = 4;
-__global__ void __launch_bounds__(kWarps * 32, kSearchMinBlocks) k_pvt_search(const SearchArgs a) {
-    const int lane = threadIdx.x & 31;
-    const int64_t fi = (int64_t) a.f0 + blockIdx.y;
+template <class Meas>
+__device__ __forceinline__ void search_nodes_of(const SearchArgs &a, const Meas &meas, int64_t fi, int lane) {
     const int64_t base = ((int64_t) blockIdx.x * kWarps + (threadIdx.x >> 5)) * 32;
     const int n = a.sc.nodes;
     if (base >= n) return;
@@ -1149,7 +1219,7 @@ __global__ void __launch_bounds__(kWarps * 32, kSearchMinBlocks) k_pvt_search(co
     unsigned todo = __ballot_sync(kFull, vis && __popc(used) >= GPSB200_SEARCH_MIN_CHANNELS);
     if (lane == 0 && todo) atomicAdd(a.searched + fi, __popc(todo));
     double my_rms = nan;
-    const int64_t s = a.cfg.s0 + fi * a.cfg.step;
+    const int64_t s = meas.instant(a, fi);
     gpsb200_coarse_config_t ap;
     ap.t_a = a.sc.t_a;
     ap.s_a = a.sc.s_a;
@@ -1163,7 +1233,7 @@ __global__ void __launch_bounds__(kWarps * 32, kSearchMinBlocks) k_pvt_search(co
         double resid;
         int64_t Nw;
         bool has;
-        coarse_solve(a, ap, s, lane, f, o, resid, Nw, has);
+        coarse_solve(a, meas, ap, s, lane, f, o, resid, Nw, has);
         if (f.status != GPSB200_FIX_OK) continue;
         if (lane == j) my_rms = f.rms;
         if (lane == 0) {
@@ -1173,6 +1243,14 @@ __global__ void __launch_bounds__(kWarps * 32, kSearchMinBlocks) k_pvt_search(co
         }
     }
     if (a.node_rms && node < n) a.node_rms[fi * n + node] = my_rms;
+}
+__global__ void __launch_bounds__(kWarps * 32, kSearchMinBlocks) k_pvt_search(const SearchArgs a) {
+    const int64_t fi = (int64_t) a.f0 + blockIdx.y;
+    search_nodes_of(a, FromEpochs(), fi, threadIdx.x & 31);
+}
+__global__ void __launch_bounds__(kWarps * 32, kSearchMinBlocks) k_snapshot_search(const SnapSearchArgs a) {
+    const int64_t fi = (int64_t) a.f0 + blockIdx.y;
+    search_nodes_of(a, FromSnapshots{a.meas + fi * a.nchan}, fi, threadIdx.x & 31);
 }
 
 // The winner's ordering key (header step 5): rms in whole millimetres, rounded down.
@@ -1194,13 +1272,10 @@ __device__ inline void warp_argmin_hit(double &key, int &node, int &k) {
 
 // Header steps 5-6 per fix instant (one warp, lane = channel): the winner and its support from the list, then the
 // winner's coarse solve again for the records. br / ar hold rms_key values.
-__global__ void __launch_bounds__(kWarps * 32) k_search_pick(const SearchArgs a) {
-    const int lane = threadIdx.x & 31;
-    const int64_t local = (int64_t) blockIdx.x * kWarps + (threadIdx.x >> 5);
-    if (local >= a.nf) return;
-    const int64_t fi = a.f0 + local;
+template <class Meas>
+__device__ __forceinline__ void search_pick(const SearchArgs &a, const Meas &meas, int64_t fi, int lane) {
     const double nan = __longlong_as_double(0x7ff8000000000000ll), inf = __longlong_as_double(0x7ff0000000000000ll);
-    const int64_t s = a.cfg.s0 + fi * a.cfg.step;
+    const int64_t s = meas.instant(a, fi);
     const unsigned used = a.used[fi];
     const int nused = __popc(used), nok = a.nok[fi];
     gpsb200_search_t r;
@@ -1255,7 +1330,7 @@ __global__ void __launch_bounds__(kWarps * 32) k_search_pick(const SearchArgs a)
         ap.s_a = a.sc.s_a;
         ap.week = a.sc.week;
         ap.reserved = 0;
-        coarse_solve(a, ap, s, lane, f, o, resid, Nw, has);
+        coarse_solve(a, meas, ap, s, lane, f, o, resid, Nw, has);
         if (!isnan(r.alt_rms)) f.status = GPSB200_FIX_AMBIGUOUS;
     } else {
         no_fix(f, s, nused, used,
@@ -1276,6 +1351,17 @@ __global__ void __launch_bounds__(kWarps * 32) k_search_pick(const SearchArgs a)
     if (a.res && lane < a.nchan) a.res[fi * a.nchan + lane] = has ? resid : nan;
     if (a.ms && lane < a.nchan) a.ms[fi * a.nchan + lane] = has ? Nw : -1;
 }
+__global__ void __launch_bounds__(kWarps * 32) k_search_pick(const SearchArgs a) {
+    const int64_t local = (int64_t) blockIdx.x * kWarps + (threadIdx.x >> 5);
+    if (local >= a.nf) return;
+    search_pick(a, FromEpochs(), a.f0 + local, threadIdx.x & 31);
+}
+__global__ void __launch_bounds__(kWarps * 32) k_snapshot_pick(const SnapSearchArgs a) {
+    const int64_t local = (int64_t) blockIdx.x * kWarps + (threadIdx.x >> 5);
+    if (local >= a.nf) return;
+    const int64_t fi = a.f0 + local;
+    search_pick(a, FromSnapshots{a.meas + fi * a.nchan}, fi, threadIdx.x & 31);
+}
 
 void fill(Args &a, const Scratch &sc) {
     a.ep = sc.d_epochs;
@@ -1293,9 +1379,11 @@ void fill(Args &a, const Scratch &sc) {
 
 // gpsb200_pvt_search: the satellite table, then the grid and the pick in passes of search_pass(nodes) instants, each
 // pass reusing one OK list of GPSB200_SEARCH_HIT_BYTES at most.
+template <bool kSnap>
 cudaError_t launch_search(const Scratch &sc, cudaStream_t s) {
-    SearchArgs a;
+    typename std::conditional<kSnap, SnapSearchArgs, SearchArgs>::type a;
     fill(a, sc);
+    if constexpr (kSnap) a.meas = sc.d_meas;
     a.sc = sc.search_cfg;
     a.sin_min = std::sin(GPSB200_SEARCH_MIN_ELEV_DEG * (M_PI / 180.0));
     a.sat = sc.d_sat;
@@ -1308,14 +1396,21 @@ cudaError_t launch_search(const Scratch &sc, cudaStream_t s) {
     a.ms = sc.want_ms ? sc.d_ms : nullptr;
     a.max_ok = GPSB200_SEARCH_MAX_OK(a.sc.nodes);
     const unsigned fix_blocks = (unsigned) (((int64_t) sc.cfg.nfix + kWarps - 1) / kWarps);
-    k_search_sats<<<fix_blocks, kWarps * 32, 0, s>>>(a);
+    if constexpr (kSnap) k_snapshot_sats<<<fix_blocks, kWarps * 32, 0, s>>>(a);
+    else k_search_sats<<<fix_blocks, kWarps * 32, 0, s>>>(a);
     const unsigned node_blocks = (unsigned) ((a.sc.nodes + kWarps * 32 - 1) / (kWarps * 32));
     const int per_pass = search_pass(a.sc.nodes);
     for (int f0 = 0; f0 < sc.cfg.nfix; f0 += per_pass) {
         a.f0 = f0;
         a.nf = std::min(per_pass, sc.cfg.nfix - f0);
-        k_pvt_search<<<dim3(node_blocks, (unsigned) a.nf), kWarps * 32, 0, s>>>(a);
-        k_search_pick<<<(unsigned) ((a.nf + kWarps - 1) / kWarps), kWarps * 32, 0, s>>>(a);
+        const unsigned pick_blocks = (unsigned) ((a.nf + kWarps - 1) / kWarps);
+        if constexpr (kSnap) {
+            k_snapshot_search<<<dim3(node_blocks, (unsigned) a.nf), kWarps * 32, 0, s>>>(a);
+            k_snapshot_pick<<<pick_blocks, kWarps * 32, 0, s>>>(a);
+        } else {
+            k_pvt_search<<<dim3(node_blocks, (unsigned) a.nf), kWarps * 32, 0, s>>>(a);
+            k_search_pick<<<pick_blocks, kWarps * 32, 0, s>>>(a);
+        }
     }
     return cudaGetLastError();
 }
@@ -1358,8 +1453,20 @@ cudaError_t launch(const Scratch &sc, cudaStream_t s) {
         k_pvt_coarse<<<blocks, kWarps * 32, 0, s>>>(a);
         break;
     }
+    case Mode::snapshot: {
+        SnapCoarseArgs a;
+        fill(a, sc);
+        a.ap = sc.coarse_cfg;
+        a.out = sc.d_coarse;
+        a.ms = sc.want_ms ? sc.d_ms : nullptr;
+        a.meas = sc.d_meas;
+        k_pvt_snapshot<<<blocks, kWarps * 32, 0, s>>>(a);
+        break;
+    }
     case Mode::search:
-        return launch_search(sc, s);
+        return launch_search<false>(sc, s);
+    case Mode::snapshot_search:
+        return launch_search<true>(sc, s);
     }
     return cudaGetLastError();
 }
@@ -1372,7 +1479,11 @@ std::string check(const gpsb200_pvt_chan_t *chans, int nchan, const gpsb200_trac
     const gpsb200_araim_config_t *araim = st.araim;
     const gpsb200_coarse_config_t *coarse = st.coarse;
     const gpsb200_search_config_t *search = st.search;
-    if (!chans || !epochs || !nepochs || !cfg) return "NULL chans, epochs, nepochs or cfg";
+    if (st.meas) {
+        if (!chans || !cfg) return "NULL chans, meas or cfg";
+    } else if (!chans || !epochs || !nepochs || !cfg) {
+        return "NULL chans, epochs, nepochs or cfg";
+    }
     if (search) {
         const gpsb200_search_config_t &c = *search;
         if (!(c.t_a >= 0.0 && c.t_a < 604800.0)) return "search t_a must lie in 0 <= t_a < 604800";
@@ -1415,17 +1526,26 @@ std::string check(const gpsb200_pvt_chan_t *chans, int nchan, const gpsb200_trac
     if (nchan < 1 || nchan > GPSB200_TRK_MAX_CHAN) return "nchan must be 1..32";
     if (max_epochs < 1) return "max_epochs must be >= 1";
     if (cfg->nfix < 1) return "nfix must be >= 1";
-    if (cfg->step < 1) return "step must be >= 1";
+    if (!st.meas && cfg->step < 1) return "step must be >= 1";
     if (cfg->iono != 0 && cfg->iono != 1) return "iono must be 0 or 1";
     const int64_t kLast = 1ll << 62;   // fix instants stay far from int64 overflow
-    if (cfg->s0 < 0 || cfg->s0 > kLast || (int64_t) (cfg->nfix - 1) > (kLast - cfg->s0) / cfg->step)
+    if (!st.meas && (cfg->s0 < 0 || cfg->s0 > kLast || (int64_t) (cfg->nfix - 1) > (kLast - cfg->s0) / cfg->step))
         return "fix instants outside 0..2^62";
+    if (st.meas) {   // snapshot records: each row's common sample is its fix instant
+        for (int64_t i = 0; i < cfg->nfix; i++) {
+            const gpsb200_snapshot_t *row = st.meas + i * nchan;
+            const std::string at = "snapshot " + std::to_string(i) + ": ";
+            if (row[0].sample < 0 || row[0].sample > kLast) return at + "sample outside 0..2^62";
+            for (int c = 1; c < nchan; c++)
+                if (row[c].sample != row[0].sample) return at + "records of different samples";
+        }
+    }
     for (int i = 0; i < 4; i++)
         if (!std::isfinite(cfg->alpha[i]) || !std::isfinite(cfg->beta[i])) return "alpha / beta must be finite";
     for (int c = 0; c < nchan; c++) {
         const gpsb200_pvt_chan_t &ch = chans[c];
         const std::string at = "channel " + std::to_string(c) + ": ";
-        if (nepochs[c] < 0 || nepochs[c] > max_epochs) return at + "nepochs outside 0..max_epochs";
+        if (!st.meas && (nepochs[c] < 0 || nepochs[c] > max_epochs)) return at + "nepochs outside 0..max_epochs";
         if (ch.eph.valid != 0 && ch.eph.valid != 1) return at + "eph.valid must be 0 or 1";
         if (!ch.eph.valid || coarse || search) continue;   // never used, or a coarse-time call: no anchor read
         if (ch.anchor_epoch < 0 || ch.anchor_epoch >= nepochs[c]) return at + "anchor_epoch outside the channel's epochs";
@@ -1452,6 +1572,7 @@ void scratch_free(Scratch &sc) {
     cudaFree(sc.d_nok);
     cudaFree(sc.d_hits);
     cudaFree(sc.d_node_rms);
+    cudaFree(sc.d_meas);
     sc = Scratch();
 }
 
@@ -1464,7 +1585,8 @@ cudaError_t run(Scratch &sc, const gpsb200_pvt_chan_t *chans, int nchan, const g
         CU_RET(cudaMalloc(&sc.d_chans, GPSB200_TRK_MAX_CHAN * sizeof(gpsb200_pvt_chan_t)));
         CU_RET(cudaMalloc(&sc.d_n, GPSB200_TRK_MAX_CHAN * sizeof(int32_t)));
     }
-    CU_RET(grow(sc.d_epochs, sc.epoch_cap, (size_t) nchan * max_epochs));
+    if (st.meas) CU_RET(grow(sc.d_meas, sc.meas_cap, nf * nchan));
+    else CU_RET(grow(sc.d_epochs, sc.epoch_cap, (size_t) nchan * max_epochs));
     CU_RET(grow(sc.d_fixes, sc.fix_cap, nf));
     if (residuals) CU_RET(grow(sc.d_res, sc.res_cap, nf * nchan));
     if (st.ms) CU_RET(grow(sc.d_ms, sc.ms_cap, nf * nchan));
@@ -1512,10 +1634,14 @@ cudaError_t run(Scratch &sc, const gpsb200_pvt_chan_t *chans, int nchan, const g
     sc.max_epochs = max_epochs;
     sc.cfg = *cfg;
     sc.want_res = residuals != nullptr;
-    CU_RET(cudaMemcpyAsync(sc.d_epochs, epochs, (size_t) nchan * max_epochs * sizeof(gpsb200_track_epoch_t),
-                           cudaMemcpyHostToDevice, s));
+    if (st.meas) {
+        CU_RET(cudaMemcpyAsync(sc.d_meas, st.meas, nf * nchan * sizeof(gpsb200_snapshot_t), cudaMemcpyHostToDevice, s));
+    } else {
+        CU_RET(cudaMemcpyAsync(sc.d_epochs, epochs, (size_t) nchan * max_epochs * sizeof(gpsb200_track_epoch_t),
+                               cudaMemcpyHostToDevice, s));
+        CU_RET(cudaMemcpyAsync(sc.d_n, nepochs, nchan * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+    }
     CU_RET(cudaMemcpyAsync(sc.d_chans, chans, nchan * sizeof(gpsb200_pvt_chan_t), cudaMemcpyHostToDevice, s));
-    CU_RET(cudaMemcpyAsync(sc.d_n, nepochs, nchan * sizeof(int32_t), cudaMemcpyHostToDevice, s));
     CU_RET(launch(sc, s));
     const auto down = [&](void *dst, const void *src, size_t bytes) {
         return cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, s);

@@ -21,12 +21,16 @@ static_assert(sizeof(gpsb200_coarse_config_t) == 48, "gpsb200_coarse_config_t la
 static_assert(sizeof(gpsb200_coarse_t) == 32, "gpsb200_coarse_t layout");
 static_assert(sizeof(gpsb200_search_config_t) == 32, "gpsb200_search_config_t layout");
 static_assert(sizeof(gpsb200_search_t) == 64, "gpsb200_search_t layout");
+static_assert(sizeof(gpsb200_snapshot_config_t) == 16, "gpsb200_snapshot_config_t layout");
+static_assert(sizeof(gpsb200_snapshot_t) == 56, "gpsb200_snapshot_t layout");
 
-// What a fix call runs beside the fixes: nothing (gpsb200_pvt), the RAIM or ARAIM stage, coarse-time fixes or searches.
-enum class Mode { plain, raim, araim, coarse, search };
+// What a fix call runs beside the fixes: nothing (gpsb200_pvt), the RAIM or ARAIM stage, coarse-time fixes or searches,
+// from tracked epochs or (snapshot, snapshot_search) from snapshot records.
+enum class Mode { plain, raim, araim, coarse, search, snapshot, snapshot_search };
 
 // A fix call's stage: at most one of raim, araim, coarse and search is set, each with the records [nfix] it fills.
-// ms [nfix][nchan] (coarse, search) and node_rms [nfix][nodes] (search) may stay NULL.
+// ms [nfix][nchan] (coarse, search) and node_rms [nfix][nodes] (search) may stay NULL. meas [nfix][nchan] (coarse or
+// search only): the measurements are these snapshot records, and the epochs are neither read nor checked.
 struct Stage {
     const gpsb200_raim_config_t *raim = nullptr;
     gpsb200_raim_t *raim_out = nullptr;
@@ -38,8 +42,13 @@ struct Stage {
     gpsb200_search_t *search_out = nullptr;
     int64_t *ms = nullptr;
     double *node_rms = nullptr;
+    const gpsb200_snapshot_t *meas = nullptr;
     Mode mode() const {
-        return raim ? Mode::raim : araim ? Mode::araim : coarse ? Mode::coarse : search ? Mode::search : Mode::plain;
+        return raim     ? Mode::raim
+               : araim  ? Mode::araim
+               : coarse ? (meas ? Mode::snapshot : Mode::coarse)
+               : search ? (meas ? Mode::snapshot_search : Mode::search)
+                        : Mode::plain;
     }
 };
 
@@ -101,6 +110,8 @@ struct Scratch {
     size_t hits_cap = 0;
     double *d_node_rms = nullptr;                // [nfix][nodes], only when the caller asks for it
     size_t node_rms_cap = 0;
+    gpsb200_snapshot_t *d_meas = nullptr;        // [nfix][nchan]: the snapshot records of a snapshot call
+    size_t meas_cap = 0;
 };
 
 void scratch_free(Scratch &sc);

@@ -1,0 +1,263 @@
+// Snapshot measurement (include/gpsb200.h: gpsb200_snapshot_measure; DESIGN §11.5).
+//
+// k_snapshot: one CTA per PRN, 256 threads. A pass correlates the K chunks of 3000 samples from s0: every thread wipes
+// off samples j = tid + 256 r (r < 12, j < 3000) of each chunk against the prompt replica (and, in the code passes, the
+// early and late ones), the sums are reduced per chunk with warp shuffles into shared memory, then summed over the 8
+// warps by one thread per chunk. Warp 0 reduces the chunks' int64 powers and thread 0 runs the header's update. Every
+// sum is an exact integer sum, so its value does not depend on the order; there are no atomics. Pass 0 is the frequency
+// pass (prompt only, at the seed), then one code pass per iteration.
+#include <cstring>
+#include <cmath>
+
+#include "acquire.h"
+#include "device_buffer.h"
+#include "rx_samples.cuh"
+#include "snapshot.h"
+#include "track.h"
+
+namespace gpsb200 {
+namespace snap {
+
+namespace {
+
+using rx::load_iq;
+using rx::sine512;
+using trk::kHalf;
+using trk::kM;
+
+constexpr int kWarps = kThreads / 32;
+constexpr unsigned kFull = 0xffffffffu;
+
+struct Smem {
+    int2 tab[512];                                  // (cos, sin)
+    int8_t ca[1024];                                // the PRN's chips as +-1
+    int32_t part[GPSB200_ACQ_MAX_MS][kWarps][6];    // warp partials per chunk: E_I, E_Q, L_I, L_Q, P_I, P_Q
+    int32_t p[GPSB200_ACQ_MAX_MS][2];               // the chunks' prompt sums (frequency pass)
+    int64_t sq[GPSB200_ACQ_MAX_MS][3];              // the chunks' early, late and prompt powers (code passes)
+    gpsb200_snapshot_t rec;                         // owned by thread 0
+};
+
+__device__ __forceinline__ uint32_t clamp_u(int32_t w) {
+    int64_t u = (int64_t) GPSB200_TRK_CODE_STEP_NOM + trk::tdiv(w, 1540);
+    u = u < (int64_t) GPSB200_TRK_CODE_STEP_MIN ? (int64_t) GPSB200_TRK_CODE_STEP_MIN
+                                                 : (u > (int64_t) GPSB200_TRK_CODE_STEP_MAX ? (int64_t) GPSB200_TRK_CODE_STEP_MAX : u);
+    return (uint32_t) u;
+}
+
+// One pass over the K chunks with the replica at phi + m u (mod M) and the wipe-off at m w: the warp partials of every
+// chunk into sm.part (prompt only unless kCode).
+template <typename T, bool kCode>
+__device__ __forceinline__ void correlate(Smem &sm, const T *__restrict__ iq, int K, uint64_t phi, uint32_t u, uint32_t w) {
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    constexpr int kSums = kCode ? 6 : 2;
+#pragma unroll 1
+    for (int k = 0; k < K; k++) {
+        const uint64_t base = (phi + (uint64_t) (kChunk * k) * u) % kM;
+        int a[kSums];
+#pragma unroll
+        for (int j = 0; j < kSums; j++) a[j] = 0;
+#pragma unroll
+        for (int r = 0; r < kPerThread; r++) {
+            const int j = tid + kThreads * r;
+            if (j < kChunk) {
+                const int m = kChunk * k + j;
+                int I, Q;
+                load_iq<T>(iq, m, I, Q);
+                const int2 cs = sm.tab[((uint32_t) m * w) >> 23];
+                const int dI = I * cs.x + Q * cs.y, dQ = Q * cs.x - I * cs.y;
+                uint64_t p = base + (uint64_t) j * u;   // base < M and j u <= 2999 u_max <= M: one fold
+                if (p >= kM) p -= kM;
+                const int cp = sm.ca[p >> 32];
+                a[kSums - 2] += cp * dI;
+                a[kSums - 1] += cp * dQ;
+                if (kCode) {
+                    uint64_t e = p + kHalf;
+                    if (e >= kM) e -= kM;
+                    const uint64_t l = p >= kHalf ? p - kHalf : p + kM - kHalf;
+                    const int ce = sm.ca[e >> 32], cl = sm.ca[l >> 32];
+                    a[0] += ce * dI;
+                    a[1] += ce * dQ;
+                    a[2] += cl * dI;
+                    a[3] += cl * dQ;
+                }
+            }
+        }
+#pragma unroll
+        for (int j = 0; j < kSums; j++)
+#pragma unroll
+            for (int o = 16; o > 0; o >>= 1) a[j] += __shfl_xor_sync(kFull, a[j], o);
+        if (lane == 0)
+#pragma unroll
+            for (int j = 0; j < kSums; j++) sm.part[k][warp][6 - kSums + j] = a[j];
+    }
+}
+
+// The chunk sum of quantity j (0..5 as in Smem::part) of chunk k over the warps.
+__device__ __forceinline__ int64_t chunk_sum(const Smem &sm, int k, int j) {
+    int v = 0;
+#pragma unroll
+    for (int q = 0; q < kWarps; q++) v += sm.part[k][q][j];
+    return v;
+}
+
+template <typename T>
+__global__ void __launch_bounds__(kThreads) k_snapshot(const T *__restrict__ iq, int K, const int8_t *__restrict__ codes,
+                                                       int iterations, gpsb200_snapshot_t *__restrict__ recs) {
+    __shared__ Smem sm;
+    const int tid = threadIdx.x, lane = tid & 31;
+    for (int i = tid; i < 512; i += kThreads) sm.tab[i] = make_int2(sine512(i + 128), sine512(i));
+    if (tid == 0) sm.rec = recs[blockIdx.x];
+    __syncthreads();
+    if (sm.rec.status != GPSB200_SNAP_OK) return;   // WEAK: the seed record stays (the whole CTA leaves)
+    for (int i = tid; i < GPSB200_CA_LEN; i += kThreads) sm.ca[i] = codes[sm.rec.prn * GPSB200_CA_LEN + i];
+    __syncthreads();
+
+    // header step 2: the frequency pass at the seed
+    correlate<T, false>(sm, iq, K, sm.rec.code_phase, sm.rec.code_step, (uint32_t) sm.rec.carr_step);
+    __syncthreads();
+    if (tid < K) {
+        sm.p[tid][0] = (int32_t) chunk_sum(sm, tid, 4);
+        sm.p[tid][1] = (int32_t) chunk_sum(sm, tid, 5);
+    }
+    __syncthreads();
+    if (tid == 0) {
+        int64_t pw = 0, sc = 0, sd = 0;
+        for (int k = 0; k < K; k++) {
+            const int64_t pi = sm.p[k][0], pq = sm.p[k][1];
+            pw += pi * pi + pq * pq;
+            if (k + 1 < K) {
+                const int64_t ni = sm.p[k + 1][0], nq = sm.p[k + 1][1];
+                int64_t cross = pi * nq - pq * ni, dot = pi * ni + pq * nq;
+                if (dot < 0) {
+                    dot = -dot;
+                    cross = -cross;
+                }
+                sc += cross;
+                sd += dot;
+            }
+        }
+        sm.rec.power = (uint64_t) pw;
+        if (K >= 2) {
+            sm.rec.carr_step += (int32_t) trk::tdiv(trk::angle(sd, sc), 3000);
+            sm.rec.code_step = clamp_u(sm.rec.carr_step);
+        }
+    }
+    __syncthreads();
+
+    // header step 3: the code iterations at w1, u1
+#pragma unroll 1
+    for (int it = 0; it < iterations; it++) {
+        correlate<T, true>(sm, iq, K, sm.rec.code_phase, sm.rec.code_step, (uint32_t) sm.rec.carr_step);
+        __syncthreads();
+        if (tid < K) {
+            int64_t v[6];
+#pragma unroll
+            for (int j = 0; j < 6; j++) v[j] = chunk_sum(sm, tid, j);
+            sm.sq[tid][0] = v[0] * v[0] + v[1] * v[1];
+            sm.sq[tid][1] = v[2] * v[2] + v[3] * v[3];
+            sm.sq[tid][2] = v[4] * v[4] + v[5] * v[5];
+        }
+        __syncthreads();
+        if (tid < 32) {
+            int64_t E = 0, L = 0, P = 0;
+            for (int k = lane; k < K; k += 32) {
+                E += sm.sq[k][0];
+                L += sm.sq[k][1];
+                P += sm.sq[k][2];
+            }
+#pragma unroll
+            for (int o = 16; o > 0; o >>= 1) {
+                E += __shfl_xor_sync(kFull, E, o);
+                L += __shfl_xor_sync(kFull, L, o);
+                P += __shfl_xor_sync(kFull, P, o);
+            }
+            if (tid == 0) {
+                const int bl = trk::bitlen64((uint64_t) (E + L));
+                const int s = bl > 40 ? bl - 40 : 0;
+                E >>= s;
+                L >>= s;
+                const int64_t D = (E + L) == 0 ? 0 : trk::tdiv((E - L) * 16384, E + L);
+                int64_t phi = (int64_t) sm.rec.code_phase + D * GPSB200_SNAP_GAIN;
+                phi = phi < 0 ? phi + (int64_t) kM : (phi >= (int64_t) kM ? phi - (int64_t) kM : phi);
+                sm.rec.code_phase = (uint64_t) phi;
+                sm.rec.last_step = (int32_t) D;
+                sm.rec.power = (uint64_t) P;
+            }
+        }
+        __syncthreads();
+    }
+    if (tid == 0) {
+        gpsb200_snapshot_t r = sm.rec;
+        r.iterations = iterations;
+        if (iterations > 0 && (r.last_step > GPSB200_SNAP_MAX_LAST_D || r.last_step < -GPSB200_SNAP_MAX_LAST_D))
+            r.status = GPSB200_SNAP_NO_CONVERGENCE;
+        recs[blockIdx.x] = r;
+    }
+}
+
+}  // namespace
+
+std::string check(const gpsb200_acq_config_t *acq, int64_t nsamples, int sample_size, const gpsb200_acq_result_t *res,
+                  const gpsb200_snapshot_config_t *cfg) {
+    if (!acq || !res || !cfg) return "NULL acquisition config, results or snapshot config";
+    // the measurement reads s0, K, the PRNs and the window, never the bins: check the config with one neutral bin, so
+    // that the config of a per-PRN window search (gpsb200_acquire_windows) is accepted as it stands
+    gpsb200_acq_config_t one = *acq;
+    one.f_lo_hz = 0.0;
+    one.step_hz = 0.0;
+    one.nbins = 1;
+    const std::string bad = acq::check(&one, nsamples, sample_size);
+    if (!bad.empty()) return bad;
+    if (!(cfg->min_ratio >= 0.0) || !std::isfinite(cfg->min_ratio)) return "min_ratio must be finite and >= 0";
+    if (cfg->iterations < 0 || cfg->iterations > GPSB200_SNAP_MAX_ITER) return "iterations must be 0..16";
+    if (cfg->reserved != 0) return "snapshot config reserved must be 0";
+    for (int p = 0; p < acq->nprn; p++) {
+        const gpsb200_acq_result_t &r = res[p];
+        const std::string at = "result " + std::to_string(p) + ": ";
+        if (r.prn != acq->prn[p]) return at + "prn differs from the search's PRN list";
+        if (r.delay < 0 || r.delay >= kChunk) return at + "delay outside 0..2999";
+        if (!(std::fabs(r.doppler_hz) <= 10000.0)) return at + "|doppler_hz| above 10 kHz";
+    }
+    return std::string();
+}
+
+void seed(const gpsb200_acq_config_t *acq, const gpsb200_acq_result_t *res, const gpsb200_snapshot_config_t *cfg,
+          gpsb200_snapshot_t *out) {
+    for (int p = 0; p < acq->nprn; p++) {
+        const gpsb200_acq_result_t &r = res[p];
+        gpsb200_snapshot_t &o = out[p];
+        memset(&o, 0, sizeof o);
+        o.prn = r.prn;
+        o.sample = acq->s0;
+        o.carr_step = (int32_t) acq::phase_step(r.doppler_hz);
+        int64_t u = (int64_t) GPSB200_TRK_CODE_STEP_NOM + trk::tdiv(o.carr_step, 1540);
+        u = u < (int64_t) GPSB200_TRK_CODE_STEP_MIN ? (int64_t) GPSB200_TRK_CODE_STEP_MIN
+                                                     : (u > (int64_t) GPSB200_TRK_CODE_STEP_MAX ? (int64_t) GPSB200_TRK_CODE_STEP_MAX : u);
+        o.code_step = (uint32_t) u;
+        o.code_phase = (kM - ((uint64_t) r.delay * o.code_step) % kM) % kM;
+        o.ratio = r.ratio;
+        o.status = r.ratio >= cfg->min_ratio ? GPSB200_SNAP_OK : GPSB200_SNAP_WEAK;
+    }
+}
+
+void scratch_free(Scratch &sc) {
+    cudaFree(sc.d_rec);
+    sc = Scratch();
+}
+
+cudaError_t launch(Scratch &sc, const void *window, int sample_size, int K, int nprn, const int8_t *codes, int iterations,
+                   gpsb200_snapshot_t *rec, cudaStream_t s) {
+    if (!sc.d_rec) CU_RET(cudaMalloc(&sc.d_rec, 32 * sizeof(gpsb200_snapshot_t)));
+    CU_RET(cudaMemcpyAsync(sc.d_rec, rec, nprn * sizeof(gpsb200_snapshot_t), cudaMemcpyHostToDevice, s));
+    if (sample_size == GPSB200_SC08)
+        k_snapshot<int8_t><<<nprn, kThreads, 0, s>>>(static_cast<const int8_t *>(window), K, codes, iterations, sc.d_rec);
+    else
+        k_snapshot<int16_t><<<nprn, kThreads, 0, s>>>(static_cast<const int16_t *>(window), K, codes, iterations,
+                                                      sc.d_rec);
+    CU_RET(cudaGetLastError());
+    CU_RET(cudaMemcpyAsync(rec, sc.d_rec, nprn * sizeof(gpsb200_snapshot_t), cudaMemcpyDeviceToHost, s));
+    return cudaStreamSynchronize(s);
+}
+
+}  // namespace snap
+}  // namespace gpsb200

@@ -1,0 +1,36 @@
+// Snapshot measurement (include/gpsb200.h: gpsb200_snapshot_measure; DESIGN §11.5): each acquired peak refined, over
+// the searched window, to a code phase in 2^-32 chips and a carrier step in 3e6/2^32 Hz, in exact integer arithmetic.
+#pragma once
+#include <cuda_runtime.h>
+#include <stdint.h>
+
+#include <string>
+
+#include "../../include/gpsb200.h"
+
+namespace gpsb200 {
+namespace snap {
+
+constexpr int kChunk = 3000;                   // samples per chunk (one nominal C/A period)
+constexpr int kThreads = 256;                  // threads of k_snapshot
+constexpr int kPerThread = (kChunk + kThreads - 1) / kThreads;   // 12 samples per thread and chunk
+
+// Empty when the call is well-formed: the search config as gpsb200_acquire checks it, res [nprn] in its PRN order with
+// delays 0..2999 and |doppler_hz| <= 10 kHz, and the snapshot config in range.
+std::string check(const gpsb200_acq_config_t *acq, int64_t nsamples, int sample_size, const gpsb200_acq_result_t *res,
+                  const gpsb200_snapshot_config_t *cfg);
+// Header step 1 and the WEAK rule, on the host: the records the kernel starts from (and leaves as they are when WEAK).
+void seed(const gpsb200_acq_config_t *acq, const gpsb200_acq_result_t *res, const gpsb200_snapshot_config_t *cfg,
+          gpsb200_snapshot_t *out);
+
+struct Scratch {
+    gpsb200_snapshot_t *d_rec = nullptr;   // [32]
+};
+void scratch_free(Scratch &sc);
+// Enqueue the refinement of rec [nprn] (seeded) over the window at `window` (stream sample s0 first) on s and wait for
+// the records. codes: [33][1023] chips as +-1 (trk::Scratch::d_codes).
+cudaError_t launch(Scratch &sc, const void *window, int sample_size, int K, int nprn, const int8_t *codes, int iterations,
+                   gpsb200_snapshot_t *rec, cudaStream_t s);
+
+}  // namespace snap
+}  // namespace gpsb200

@@ -9,6 +9,14 @@
 // are searched, each over 2h + 1 bins of the --doppler step around its prediction (h = ceil(window / step)), starting
 // at step * round(f / step) - h * step so that the bins lie on the cold search's grid (gpsb200_acquire_windows). Each
 // line then also shows the predicted Doppler and elevation.
+//
+// Snapshot fixes (--fix, DESIGN §11.5): with a RINEX navigation file (--assist), the GPS time of the first window's
+// first sample (--assist-time) and an a-priori position (--assist-pos LAT,LON,H) or none (--assist-pos search), every
+// --every ms from the start offset (--count windows) the search runs on its window, gpsb200_snapshot_measure refines
+// the PRNs at or above the threshold, and gpsb200_pvt_snapshot (gpsb200_pvt_snapshot_search over the default global
+// grid with search) fixes from them, with the ephemeris valid at the assist time. One line per snapshot: sample,
+// status, position, clock, velocity, channels used, PDOP and delta (the solved a-priori time error), plus support with
+// search. No tracking, no navigation message: each fix comes from its K ms window alone.
 #include <cmath>
 #include <cstdio>
 #include <cstdlib>
@@ -33,6 +41,8 @@ static void usage() {
             "            [--threshold R] [--device D]\n"
             "            [--almanac FILE.sem --assist-pos LAT,LON,H --assist-time YYYY/MM/DD,hh:mm:ss[.s]\n"
             "             [--window HZ] [--mask DEG]]\n"
+            "            [--fix --assist NAV_FILE[,3] --assist-pos LAT,LON,H|search --assist-time YYYY/MM/DD,hh:mm:ss[.s]\n"
+            "             [--every MS] [--count N] [--iono a0,a1,a2,a3,b0,b1,b2,b3]]\n"
             "  FILE              interleaved I,Q at 3 Msps, int8 (default) or int16 (--iq16)\n"
             "  --block B         start at 0.1 s block B (sample 300000 B); --offset-ms N adds N ms (3000 N samples)\n"
             "  --ms K            coherent 1 ms periods summed, 1..100 (default 10)\n"
@@ -42,9 +52,111 @@ static void usage() {
             "  --almanac         warm start: search the PRNs of --prn predicted at or above the mask from the SEM file\n"
             "                    at --assist-pos / --assist-time (GPS time of the window's first sample), each over\n"
             "                    the bins of the --doppler step within --window Hz of its prediction (default %.0f)\n"
-            "  --mask DEG        elevation mask of the warm start (default %.0f)\n",
+            "  --mask DEG        elevation mask of the warm start (default %.0f)\n"
+            "  --fix             snapshot fixes from the window alone: the acquired PRNs refined (gpsb200_snapshot_measure),\n"
+            "                    then a coarse-time fix from --assist-pos, or a search over a global grid with 'search';\n"
+            "                    ephemeris from the RINEX file of --assist (,3: RINEX 3) at --assist-time, the GPS time\n"
+            "                    of the first window's first sample; one window every --every ms (default 100), --count\n"
+            "                    windows (default 1); --iono: the Klobuchar alpha / beta to apply\n",
             kDefaultThreshold, kDefaultWindow, kDefaultMask);
     exit(2);
+}
+
+// --fix: count windows every every_ms from sample s0, each searched on the standard grid, measured and fixed alone.
+static int snapshot_fixes(const char *path, int ss, int device, long long s0, gpsb200_acq_config_t cfg, double lo,
+                          double hi, double step, double threshold, const char *nav, int nav_v3, const double *x_a,
+                          int32_t week, double sow, long long every_ms, long long count, gpsb200_pvt_config_t pcfg) {
+    cfg.f_lo_hz = lo;
+    cfg.step_hz = step;
+    cfg.nbins = (int) std::floor((hi - lo) / step + 1e-9) + 1;
+    gpsb200_ephemeris_t eph[32];
+    if (gpsb200_rinex_ephemeris(nav, nav_v3, week, sow, eph) != GPSB200_OK) {
+        fprintf(stderr, "gpsb200-acq: cannot read the ephemeris of %s\n", nav);
+        return 1;
+    }
+    const size_t elem = ss == GPSB200_SC16 ? 2 : 1;
+    const long long need = (long long) GPSB200_ACQ_CODE_SAMPLES * cfg.ms + GPSB200_ACQ_CODE_SAMPLES - 1;
+    const long long have = file_samples(path, elem);
+    FILE *f = fopen(path, "rb");
+    if (have < 0 || !f) {
+        fprintf(stderr, "gpsb200-acq: cannot open %s\n", path);
+        return 1;
+    }
+    gpsb200_ctx_t *ctx = nullptr;
+    if (create_rx_context(device, &ctx) != GPSB200_OK) {
+        fprintf(stderr, "gpsb200-acq: cannot create a context\n");
+        fclose(f);
+        return 1;
+    }
+    gpsb200_snapshot_config_t scfg;
+    memset(&scfg, 0, sizeof scfg);
+    scfg.min_ratio = threshold;
+    scfg.iterations = GPSB200_SNAP_ITERATIONS;
+    gpsb200_coarse_config_t ap;
+    memset(&ap, 0, sizeof ap);
+    if (x_a) memcpy(ap.x_a, x_a, sizeof ap.x_a);
+    ap.t_a = sow;
+    ap.s_a = s0;
+    ap.week = week;
+    gpsb200_search_config_t sc;
+    memset(&sc, 0, sizeof sc);
+    sc.t_a = sow;
+    sc.s_a = s0;
+    sc.week = week;
+    sc.nodes = GPSB200_SEARCH_NODES;
+    pcfg.nfix = 1;
+    pcfg.step = 1;
+    printf("# %s: snapshot fixes, %lld window(s) of %d ms every %lld ms from sample %lld, %s, Klobuchar %s\n", path,
+           count, cfg.ms, every_ms, s0, x_a ? "coarse-time fix from the a-priori position" : "search over a global grid",
+           pcfg.iono ? "on" : "off");
+    printf("# sample  status  lat_deg  lon_deg  height_m  clock_m  vx  vy  vz (ECEF m/s)  channels  pdop  delta_s%s\n",
+           x_a ? "" : "  support");
+    static const char *const kStatus[] = {"OK", "FEW", "NO_CONVERGENCE", "AMBIGUOUS"};
+    int rc = GPSB200_OK;
+    std::vector<char> buf;
+    for (long long i = 0; i < count && rc == GPSB200_OK; i++) {
+        const long long s = s0 + i * every_ms * GPSB200_ACQ_CODE_SAMPLES;
+        if (s + need > have || !read_at(f, s, need, elem, buf)) break;
+        cfg.s0 = 0;
+        std::vector<gpsb200_acq_result_t> res(cfg.nprn);
+        std::vector<gpsb200_snapshot_t> meas(cfg.nprn);
+        rc = gpsb200_acquire(ctx, buf.data(), need, ss, &cfg, res.data(), nullptr);
+        if (rc == GPSB200_OK) rc = gpsb200_snapshot_measure(ctx, buf.data(), need, ss, &cfg, res.data(), &scfg, meas.data());
+        if (rc != GPSB200_OK) break;
+        // the channels: the measured PRNs with an ephemeris valid at the assist time
+        std::vector<gpsb200_pvt_chan_t> chans;
+        std::vector<gpsb200_snapshot_t> row;
+        for (auto &m : meas) {
+            if (m.status != GPSB200_SNAP_OK || !eph[m.prn - 1].valid) continue;
+            gpsb200_pvt_chan_t pc;
+            memset(&pc, 0, sizeof pc);
+            pc.eph = eph[m.prn - 1];
+            pc.prn = m.prn;
+            chans.push_back(pc);
+            m.sample = s;
+            row.push_back(m);
+        }
+        gpsb200_fix_t fx;
+        gpsb200_coarse_t co;
+        gpsb200_search_t sr;
+        if (chans.empty()) {
+            printf("%lld  FEW\n", s);
+            continue;
+        }
+        rc = x_a ? gpsb200_pvt_snapshot(ctx, chans.data(), (int) chans.size(), row.data(), &pcfg, &ap, &fx, nullptr, &co,
+                                        nullptr)
+                 : gpsb200_pvt_snapshot_search(ctx, chans.data(), (int) chans.size(), row.data(), &pcfg, &sc, &fx, nullptr,
+                                               &sr, nullptr, nullptr);
+        if (rc != GPSB200_OK) break;
+        printf("%lld  %s  %.8f  %.8f  %.3f  %.3f  %.3f  %.3f  %.3f  %d  %.2f  %.9f", s, kStatus[fx.status], fx.lat_deg,
+               fx.lon_deg, fx.height, fx.clock_m, fx.vx, fx.vy, fx.vz, fx.nused, fx.pdop, x_a ? co.delta : sr.delta);
+        if (!x_a) printf("  %d", sr.support);
+        printf("\n");
+    }
+    fclose(f);
+    if (rc != GPSB200_OK) fprintf(stderr, "gpsb200-acq: %s\n", gpsb200_last_error(ctx));
+    gpsb200_destroy(ctx);
+    return rc == GPSB200_OK ? 0 : 1;
 }
 
 int main(int argc, char **argv) {
@@ -59,6 +171,12 @@ int main(int argc, char **argv) {
     double x_a[3] = {0.0, 0.0, 0.0}, sow = 0.0, window = kDefaultWindow, mask = kDefaultMask;
     int32_t week = 0;
     bool have_pos = false, have_time = false;
+    bool fix = false, pos_search = false;
+    std::string assist;
+    int assist_v3 = 0;
+    long long every_ms = 100, count = 1;
+    gpsb200_pvt_config_t pcfg;
+    memset(&pcfg, 0, sizeof pcfg);
     parse_prns("1-32", &cfg);
     for (int i = 1; i < argc; i++) {
         std::string a = argv[i];
@@ -77,7 +195,10 @@ int main(int argc, char **argv) {
         } else if (a == "--threshold") threshold = atof(val());
         else if (a == "--device") device = atoi(val());
         else if (a == "--almanac") almanac = val();
-        else if (a == "--assist-pos") {
+        else if (a == "--assist-pos" && i + 1 < argc && std::string(argv[i + 1]) == "search") {
+            i++;
+            have_pos = pos_search = true;
+        } else if (a == "--assist-pos") {
             if (!ecef_of_llh(val(), x_a)) usage();
             have_pos = true;
         } else if (a == "--assist-time") {
@@ -87,12 +208,34 @@ int main(int argc, char **argv) {
             window = atof(val());
             if (!(window >= 0.0)) usage();
         } else if (a == "--mask") mask = atof(val());
+        else if (a == "--fix") fix = true;
+        else if (a == "--assist") {
+            assist = val();
+            const size_t k = assist.rfind(',');
+            if (k != std::string::npos) {
+                if (assist.substr(k + 1) != "3") usage();
+                assist_v3 = 1;
+                assist.resize(k);
+            }
+        } else if (a == "--every") every_ms = atoll(val());
+        else if (a == "--count") count = atoll(val());
+        else if (a == "--iono") {
+            double *ab = pcfg.alpha;
+            double *bb = pcfg.beta;
+            if (sscanf(val(), "%lf,%lf,%lf,%lf,%lf,%lf,%lf,%lf", ab, ab + 1, ab + 2, ab + 3, bb, bb + 1, bb + 2, bb + 3) != 8)
+                usage();
+            pcfg.iono = 1;
+        }
         else if (a[0] != '-' && !path) path = argv[i];
         else usage();
     }
-    if (!path || block < 0 || offset_ms < 0 || (almanac && (!have_pos || !have_time)) ||
-        (!almanac && (have_pos || have_time)))
+    if (!path || block < 0 || offset_ms < 0 || (almanac && (!have_pos || !have_time || pos_search || fix)) ||
+        (!almanac && !fix && (have_pos || have_time)) || (fix && (assist.empty() || !have_pos || !have_time)) ||
+        (!fix && (!assist.empty() || pcfg.iono)) || every_ms < 1 || count < 1)
         usage();
+    if (fix) return snapshot_fixes(path, ss, device, block * GPSB200_BLOCK_SAMPLES + offset_ms * GPSB200_ACQ_CODE_SAMPLES,
+                                   cfg, lo, hi, step, threshold, assist.c_str(), assist_v3, pos_search ? nullptr : x_a,
+                                   week, sow, every_ms, count, pcfg);
     cfg.f_lo_hz = lo;
     cfg.step_hz = step;
     cfg.nbins = (int) std::floor((hi - lo) / step + 1e-9) + 1;
