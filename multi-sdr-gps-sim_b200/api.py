@@ -1031,26 +1031,8 @@ class Context:
         on `stream` behind the work it holds.
         -> results ACQ_RESULT_DTYPE[nprn] (prn, bin, delay, doppler_hz, delay_chips, p1, p2, ratio), and with want_grid
         also the whole power grid uint64[nprn, nbins, 3000]."""
-        prns = [int(p) for p in prns]
-        cfg = AcqConfig()
-        cfg.s0, cfg.ms, cfg.nprn = int(s0), int(ms), len(prns)
-        for i, p in enumerate(prns[:32]):   # more than 32 is rejected by the library with the other argument checks
-            cfg.prn[i] = p
-        cfg.f_lo_hz, cfg.step_hz, cfg.nbins = float(f_lo), float(step), int(nbins)
-        res = np.zeros(max(1, min(len(prns), 32)), ACQ_RESULT_DTYPE)
-        grid = np.zeros((max(1, len(prns)), max(1, int(nbins)), ACQ_CODE_SAMPLES), np.uint64) if want_grid else None
-        gp = None if grid is None else grid.ctypes.data
-        if device_ptr is not None:
-            assert iq is None and nsamples is not None
-            rc = lib().gpsb200_acquire_device(self._h, C.c_void_p(device_ptr), int(nsamples), int(sample_size), C.byref(cfg),
-                                              res.ctypes.data, gp, C.c_void_p(stream))
-        else:
-            a = np.ascontiguousarray(iq)
-            n = a.size // 2 if nsamples is None else int(nsamples)
-            assert n <= a.size // 2
-            rc = lib().gpsb200_acquire(self._h, a.ctypes.data, n, int(sample_size), C.byref(cfg), res.ctypes.data, gp)
-        self._check(rc)
-        return (res, grid) if want_grid else res
+        return self._acquire(None, iq, sample_size, [int(p) for p in prns], ms, s0, f_lo, step, nbins, want_grid,
+                             device_ptr, nsamples, stream)
 
     def acquire_windows(self, iq=None, sample_size=SC08, prns=(), f_lo_prn=(), step=250.0, nbins=5, ms=10, s0=0,
                         want_grid=False, device_ptr=None, nsamples=None, stream=0):
@@ -1062,27 +1044,47 @@ class Context:
         flo = np.ascontiguousarray(f_lo_prn, dtype=np.float64).reshape(-1)
         if flo.size != len(prns):
             raise GpsB200Error(ERR_ARG, "acquire_windows: %d first bins for %d PRNs" % (flo.size, len(prns)))
+        return self._acquire(flo, iq, sample_size, prns, ms, s0, 0.0, step, nbins, want_grid, device_ptr, nsamples,
+                             stream)
+
+    def _acquire(self, f_lo_prn, iq, sample_size, prns, ms, s0, f_lo, step, nbins, want_grid, device_ptr, nsamples,
+                 stream):
+        """acquire, or with f_lo_prn (float64[nprn], the first bins) acquire_windows."""
+        cfg = self._acq_config(prns, ms, s0, f_lo, step, nbins)
+        res = np.zeros(max(1, min(len(prns), 32)), ACQ_RESULT_DTYPE)
+        grid = np.zeros((max(1, len(prns)), max(1, int(nbins)), ACQ_CODE_SAMPLES), np.uint64) if want_grid else None
+        gp = None if grid is None else grid.ctypes.data
+        src, n, dev = self._rx_source(iq, device_ptr, nsamples, stream)
+        if f_lo_prn is None:
+            fn, fp = lib().gpsb200_acquire_device if dev else lib().gpsb200_acquire, ()
+        else:
+            fn = lib().gpsb200_acquire_windows_device if dev else lib().gpsb200_acquire_windows
+            fp = (f_lo_prn.ctypes.data if f_lo_prn.size else None,)
+        self._check(fn(self._h, src, n, int(sample_size), C.byref(cfg), *fp, res.ctypes.data, gp, *dev))
+        return (res, grid) if want_grid else res
+
+    @staticmethod
+    def _acq_config(prns, ms, s0, f_lo, step, nbins):
+        """The AcqConfig of a search of the PRNs `prns` (a list of ints) with acquire's other arguments."""
         cfg = AcqConfig()
         cfg.s0, cfg.ms, cfg.nprn = int(s0), int(ms), len(prns)
         for i, p in enumerate(prns[:32]):   # more than 32 is rejected by the library with the other argument checks
             cfg.prn[i] = p
-        cfg.f_lo_hz, cfg.step_hz, cfg.nbins = 0.0, float(step), int(nbins)
-        res = np.zeros(max(1, min(len(prns), 32)), ACQ_RESULT_DTYPE)
-        grid = np.zeros((max(1, len(prns)), max(1, int(nbins)), ACQ_CODE_SAMPLES), np.uint64) if want_grid else None
-        gp = None if grid is None else grid.ctypes.data
-        fp = flo.ctypes.data if flo.size else None
+        cfg.f_lo_hz, cfg.step_hz, cfg.nbins = float(f_lo), float(step), int(nbins)
+        return cfg
+
+    @staticmethod
+    def _rx_source(iq, device_ptr, nsamples, stream):
+        """The source of a receiver call: nsamples samples at device_ptr, or the numpy array iq (its first nsamples,
+        default all). -> (pointer, nsamples, the arguments the _device entry point takes after its others: (stream,)
+        for a device source, () for a host one)."""
         if device_ptr is not None:
             assert iq is None and nsamples is not None
-            rc = lib().gpsb200_acquire_windows_device(self._h, C.c_void_p(device_ptr), int(nsamples), int(sample_size),
-                                                      C.byref(cfg), fp, res.ctypes.data, gp, C.c_void_p(stream))
-        else:
-            a = np.ascontiguousarray(iq)
-            n = a.size // 2 if nsamples is None else int(nsamples)
-            assert n <= a.size // 2
-            rc = lib().gpsb200_acquire_windows(self._h, a.ctypes.data, n, int(sample_size), C.byref(cfg), fp,
-                                               res.ctypes.data, gp)
-        self._check(rc)
-        return (res, grid) if want_grid else res
+            return C.c_void_p(device_ptr), int(nsamples), (C.c_void_p(stream),)
+        a = np.ascontiguousarray(iq)
+        n = a.size // 2 if nsamples is None else int(nsamples)
+        assert n <= a.size // 2
+        return a.ctypes, n, ()   # a.ctypes converts to the array's address and keeps the array alive
 
     def debug_acq_split(self, nprn, nbins, force=-1):
         """gpsb200_debug_acq_split: the CTAs per row a search of nprn x nbins rows uses on this context; force 0
@@ -1100,23 +1102,13 @@ class Context:
         -> (epochs: a list of TRACK_EPOCH_DTYPE arrays, one per channel, states after the call)."""
         st = np.array(states, dtype=TRACK_STATE_DTYPE).reshape(-1).copy()
         nchan = st.size
-        if device_ptr is not None:
-            assert iq is None and nsamples is not None
-            n = int(nsamples)
-        else:
-            a = np.ascontiguousarray(iq)
-            n = a.size // 2 if nsamples is None else int(nsamples)
-            assert n <= a.size // 2
+        src, n, dev = self._rx_source(iq, device_ptr, nsamples, stream)
         me = int(max_epochs) if max_epochs is not None else n // 2999 + 1
         out = np.zeros((max(1, nchan), max(1, me)), TRACK_EPOCH_DTYPE)
         cnt = np.zeros(max(1, nchan), np.int32)
-        if device_ptr is not None:
-            rc = lib().gpsb200_track_device(self._h, C.c_void_p(device_ptr), n, int(sample_size), int(base),
-                                            st.ctypes.data, nchan, me, out.ctypes.data, cnt.ctypes.data, C.c_void_p(stream))
-        else:
-            rc = lib().gpsb200_track(self._h, a.ctypes.data, n, int(sample_size), int(base), st.ctypes.data, nchan, me,
-                                     out.ctypes.data, cnt.ctypes.data)
-        self._check(rc)
+        fn = lib().gpsb200_track_device if dev else lib().gpsb200_track
+        self._check(fn(self._h, src, n, int(sample_size), int(base), st.ctypes.data, nchan, me, out.ctypes.data,
+                       cnt.ctypes.data, *dev))
         return [out[c, :cnt[c]].copy() for c in range(nchan)], st
 
     def pvt(self, chans, epochs, cfg, want_residuals=False, nepochs=None):
@@ -1202,27 +1194,15 @@ class Context:
         -> SNAPSHOT_DTYPE[nprn] in the order of res."""
         r = np.ascontiguousarray(res, dtype=ACQ_RESULT_DTYPE).reshape(-1)
         prns = [int(p) for p in (r["prn"] if prns is None else prns)]
-        acq = AcqConfig()
-        acq.s0, acq.ms, acq.nprn = int(s0), int(ms), len(prns)
-        for i, p in enumerate(prns[:32]):
-            acq.prn[i] = p
-        acq.f_lo_hz, acq.step_hz, acq.nbins = float(f_lo), float(step), int(nbins)
+        acq = self._acq_config(prns, ms, s0, f_lo, step, nbins)
         sc = np.array(snapshot_config() if cfg is None else cfg, dtype=SNAPSHOT_CONFIG_DTYPE).reshape(1)
         if r.size < len(prns):
             raise GpsB200Error(ERR_ARG, "snapshot_measure: %d results for %d PRNs" % (r.size, len(prns)))
         out = np.zeros(max(1, len(prns)), SNAPSHOT_DTYPE)
-        if device_ptr is not None:
-            assert iq is None and nsamples is not None
-            rc = lib().gpsb200_snapshot_measure_device(self._h, C.c_void_p(device_ptr), int(nsamples), int(sample_size),
-                                                       C.byref(acq), r.ctypes.data, sc.ctypes.data, out.ctypes.data,
-                                                       C.c_void_p(stream))
-        else:
-            a = np.ascontiguousarray(iq)
-            n = a.size // 2 if nsamples is None else int(nsamples)
-            assert n <= a.size // 2
-            rc = lib().gpsb200_snapshot_measure(self._h, a.ctypes.data, n, int(sample_size), C.byref(acq), r.ctypes.data,
-                                                sc.ctypes.data, out.ctypes.data)
-        self._check(rc)
+        src, n, dev = self._rx_source(iq, device_ptr, nsamples, stream)
+        fn = lib().gpsb200_snapshot_measure_device if dev else lib().gpsb200_snapshot_measure
+        self._check(fn(self._h, src, n, int(sample_size), C.byref(acq), r.ctypes.data, sc.ctypes.data, out.ctypes.data,
+                       *dev))
         return out[:len(prns)]
 
     @staticmethod

@@ -35,7 +35,6 @@ namespace acq {
 namespace {
 
 using rx::load_iq;
-using rx::sine512;
 
 struct Best {
     uint64_t v;
@@ -139,7 +138,7 @@ k_acq_grid(const T *__restrict__ iq, const int16_t *__restrict__ edges_all, cons
     const int prn = prns[p];
     const int ne = nedges_all[prn];
     const uint32_t u = u_bins[kWindows ? p * nbins + j : j];
-    for (int i = tid; i < 512; i += kThreads) sm.tab[i] = make_int2(sine512(i + 128), sine512(i));
+    rx::fill_carrier_table(sm.tab, kThreads);
     for (int i = tid; i < ne; i += kThreads) sm.edges[i] = edges_all[prn * kMaxEdges + i];
     if (tid == 0) sm.S[0] = make_int2(0, 0);
 
@@ -160,10 +159,9 @@ k_acq_grid(const T *__restrict__ iq, const int16_t *__restrict__ edges_all, cons
             if (tau0 + m < 2 * kCode - 1) {   // the window's 3000 K + 2999 samples; beyond: zeros (delays >= 3000 only)
                 int I, Q;
                 load_iq<T>(iq, base + m, I, Q);
-                const uint32_t ph = (uint32_t) (base + m) * u;
-                const int2 cs = sm.tab[ph >> 23];
-                dI = I * cs.x + Q * cs.y;
-                dQ = Q * cs.x - I * cs.y;
+                const int2 d = rx::wipe_off(sm.tab, (uint32_t) (base + m) * u, I, Q);
+                dI = d.x;
+                dQ = d.y;
             }
             sI += dI;
             sQ += dQ;

@@ -208,6 +208,7 @@ struct gpsb200_ctx {
     size_t out_bytes = 0;
     uint8_t *d_rx = nullptr;               // receiver staging of host sources (acquisition window, tracking buffer)
     size_t rx_bytes = 0;
+    int8_t *d_rx_chips = nullptr;          // chips as +-1 of tracking and snapshots (trk::chips_upload), built once
     bool nav_dirty = true;
     std::unique_ptr<WorkerPool> pool;      // host passes (guesses, fix-up scan)
     SynthArgs last{};                      // replay state
@@ -601,11 +602,20 @@ int ensure_staging(gpsb200_ctx *ctx, int sample_size) {
     return GPSB200_OK;
 }
 
-// A receiver call's host source is copied up on s into the context's receiver staging buffer, *dev points there.
-// Acquisition and tracking both wait for their results, so they never hold the buffer at the same time.
-int stage_rx_source(gpsb200_ctx *ctx, const void *src, size_t bytes, cudaStream_t s, const void **dev) {
-    CU(grow(ctx->d_rx, ctx->rx_bytes, bytes));
-    if (bytes) CU(cudaMemcpyAsync(ctx->d_rx, src, bytes, cudaMemcpyHostToDevice, s));
+// The source of a receiver call (entry point fn), after the call's own contract check: a device source is checked for
+// alignment and read in place; of a host source, samples first .. first + count - 1 are copied up on s into the
+// context's receiver staging buffer (every receiver call waits for its results, so no two hold it at the same time).
+// *dev: the device address of sample `first`.
+int rx_source(gpsb200_ctx *ctx, const char *fn, const void *iq, int64_t first, int64_t count, int sample_size,
+              bool device, cudaStream_t s, const void **dev) {
+    int rc = device ? check_aligned(ctx, iq, fn, "iq_device") : GPSB200_OK;
+    if (!rc) rc = check_entry(ctx);
+    if (rc) return rc;
+    const size_t elem = sample_size == GPSB200_SC16 ? 4 : 2;
+    *dev = static_cast<const char *>(iq) + (size_t) first * elem;
+    if (device) return GPSB200_OK;
+    CU(grow(ctx->d_rx, ctx->rx_bytes, (size_t) count * elem));
+    if (count) CU(cudaMemcpyAsync(ctx->d_rx, *dev, (size_t) count * elem, cudaMemcpyHostToDevice, s));
     *dev = ctx->d_rx;
     return GPSB200_OK;
 }
@@ -623,6 +633,11 @@ int settle(gpsb200_ctx *ctx, cudaStream_t caller, int rc) {
     cudaStreamSynchronize(ctx->s_ck);
     cudaStreamSynchronize(ctx->s_copy);
     return rc;
+}
+
+// The stream of an entry point that takes the caller's: stream_, or the context's compute stream when it is NULL.
+cudaStream_t caller_stream(gpsb200_ctx *ctx, void *stream_) {
+    return stream_ ? (cudaStream_t) stream_ : ctx->s_compute;
 }
 
 // ---- the steps of a call --------------------------------------------------------------------------------------------
@@ -1097,8 +1112,7 @@ int carrier_chain_device(gpsb200_ctx *ctx, const gpsb200_chan_t *chans, int nblk
 
 
 // The acquisition search of the four entry points (acquire.cu): the standard one, and with `windows` the per-PRN Doppler
-// windows starting at f_lo_prn. Everything is checked before anything is enqueued; a device source is searched in place
-// on the caller's stream, a host source's window is copied up first.
+// windows starting at f_lo_prn. Everything is checked before anything is enqueued; the source is rx_source's.
 int acquire(gpsb200_ctx *ctx, const void *iq, int64_t nsamples, int sample_size, const gpsb200_acq_config_t *cfg,
             bool windows, const double *f_lo_prn, gpsb200_acq_result_t *res, uint64_t *grid, bool device,
             cudaStream_t s) {
@@ -1106,18 +1120,11 @@ int acquire(gpsb200_ctx *ctx, const void *iq, int64_t nsamples, int sample_size,
     if (!iq || !res) return fail(ctx, GPSB200_ERR_ARG, std::string(name) + ": NULL source or result array");
     const std::string bad = acq::check(cfg, nsamples, sample_size, windows, f_lo_prn);
     if (!bad.empty()) return fail(ctx, GPSB200_ERR_ARG, std::string(name) + ": " + bad);
-    int rc = device ? check_aligned(ctx, iq, windows ? "gpsb200_acquire_windows_device" : "gpsb200_acquire_device",
-                                    "iq_device")
-                    : GPSB200_OK;
-    if (!rc) rc = check_entry(ctx);
+    const void *window;
+    const int rc = rx_source(ctx, windows ? "gpsb200_acquire_windows_device" : "gpsb200_acquire_device", iq, cfg->s0,
+                             acq::window_samples(cfg), sample_size, device, s, &window);
     if (rc) return rc;
     CU(acq::scratch_reserve(ctx->acq, cfg, windows, grid != nullptr));
-    const size_t elem = sample_size == GPSB200_SC16 ? 2 : 1;
-    const void *window = static_cast<const char *>(iq) + (size_t) cfg->s0 * 2 * elem;
-    if (!device) {
-        rc = stage_rx_source(ctx, window, (size_t) acq::window_samples(cfg) * 2 * elem, s, &window);
-        if (rc) return rc;
-    }
     CU(acq::launch(ctx->acq, window, sample_size, cfg, windows ? f_lo_prn : nullptr, grid != nullptr, s));
     if (grid)
         CU(cudaMemcpy(grid, ctx->acq.d_grid, (size_t) cfg->nprn * cfg->nbins * acq::kCode * sizeof(uint64_t),
@@ -1126,28 +1133,23 @@ int acquire(gpsb200_ctx *ctx, const void *iq, int64_t nsamples, int sample_size,
     return GPSB200_OK;
 }
 
-// The tracking of both entry points (track.cu). Everything is checked before anything is enqueued; a device source is
-// tracked in place on the caller's stream, a host source is copied up first.
+// The tracking of both entry points (track.cu). Everything is checked before anything is enqueued.
 int track(gpsb200_ctx *ctx, const void *iq, int64_t nsamples, int sample_size, int64_t base, gpsb200_track_state_t *state,
           int nchan, int max_epochs, gpsb200_track_epoch_t *epochs, int32_t *nepochs, bool device, cudaStream_t s) {
     if (!iq || !epochs || !nepochs) return fail(ctx, GPSB200_ERR_ARG, "gpsb200_track: NULL source, epochs or nepochs");
     const std::string bad = trk::check(state, nchan, max_epochs, nsamples, base, sample_size);
     if (!bad.empty()) return fail(ctx, GPSB200_ERR_ARG, "gpsb200_track: " + bad);
-    int rc = device ? check_aligned(ctx, iq, "gpsb200_track_device", "iq_device") : GPSB200_OK;
-    if (!rc) rc = check_entry(ctx);
+    const void *src;
+    const int rc = rx_source(ctx, "gpsb200_track_device", iq, 0, nsamples, sample_size, device, s, &src);
     if (rc) return rc;
+    if (!ctx->d_rx_chips) CU(trk::chips_upload(&ctx->d_rx_chips));
     CU(trk::scratch_reserve(ctx->trk, nchan, max_epochs));
-    const void *src = iq;
-    if (!device) {
-        rc = stage_rx_source(ctx, iq, (size_t) nsamples * 2 * (sample_size == GPSB200_SC16 ? 2 : 1), s, &src);
-        if (rc) return rc;
-    }
-    CU(trk::launch(ctx->trk, src, nsamples, sample_size, base, state, nchan, max_epochs, epochs, nepochs, s));
+    CU(trk::launch(ctx->trk, ctx->d_rx_chips, src, nsamples, sample_size, base, state, nchan, max_epochs, epochs,
+                   nepochs, s));
     return GPSB200_OK;
 }
 
-// The snapshot measurement of both entry points (snapshot.cu). Everything is checked before anything is enqueued; a
-// device source is measured in place on the caller's stream, a host source's window is copied up first.
+// The snapshot measurement of both entry points (snapshot.cu). Everything is checked before anything is enqueued.
 int snapshot_measure(gpsb200_ctx *ctx, const void *iq, int64_t nsamples, int sample_size, const gpsb200_acq_config_t *acq,
                      const gpsb200_acq_result_t *res, const gpsb200_snapshot_config_t *cfg, gpsb200_snapshot_t *out,
                      bool device, cudaStream_t s) {
@@ -1155,18 +1157,12 @@ int snapshot_measure(gpsb200_ctx *ctx, const void *iq, int64_t nsamples, int sam
     if (!iq || !out) return fail(ctx, GPSB200_ERR_ARG, std::string(name) + ": NULL source or output");
     const std::string bad = snap::check(acq, nsamples, sample_size, res, cfg);
     if (!bad.empty()) return fail(ctx, GPSB200_ERR_ARG, std::string(name) + ": " + bad);
-    int rc = device ? check_aligned(ctx, iq, name, "iq_device") : GPSB200_OK;
-    if (!rc) rc = check_entry(ctx);
+    const void *window;
+    const int rc = rx_source(ctx, name, iq, acq->s0, acq::window_samples(acq), sample_size, device, s, &window);
     if (rc) return rc;
-    CU(trk::scratch_reserve(ctx->trk, 1, 1));   // the +-1 chips of every PRN
-    const size_t elem = sample_size == GPSB200_SC16 ? 2 : 1;
-    const void *window = static_cast<const char *>(iq) + (size_t) acq->s0 * 2 * elem;
-    if (!device) {
-        rc = stage_rx_source(ctx, window, (size_t) acq::window_samples(acq) * 2 * elem, s, &window);
-        if (rc) return rc;
-    }
+    if (!ctx->d_rx_chips) CU(trk::chips_upload(&ctx->d_rx_chips));
     snap::seed(acq, res, cfg, out);
-    CU(snap::launch(ctx->snap, window, sample_size, acq->ms, acq->nprn, ctx->trk.d_codes, cfg->iterations, out, s));
+    CU(snap::launch(ctx->snap, window, sample_size, acq->ms, acq->nprn, ctx->d_rx_chips, cfg->iterations, out, s));
     return GPSB200_OK;
 }
 
@@ -1491,6 +1487,7 @@ void gpsb200_destroy(gpsb200_ctx_t *ctx) {
     cudaFree(ctx->d_chips);
     cudaFree(ctx->d_out);
     cudaFree(ctx->d_rx);
+    cudaFree(ctx->d_rx_chips);
     for (auto &e : ctx->ev)
         if (e) cudaEventDestroy(e);
     for (auto &e : ctx->ev_done)
@@ -1522,7 +1519,7 @@ int gpsb200_synth_blocks_device(gpsb200_ctx_t *ctx, const gpsb200_chan_t *chans,
                                 int sample_size, void *dst_device, void *stream_, double *carr_phase_out,
                                 gpsb200_stats_t *stats) {
     if (!ctx) return GPSB200_ERR_ARG;
-    cudaStream_t s = stream_ ? (cudaStream_t) stream_ : ctx->s_compute;
+    cudaStream_t s = caller_stream(ctx, stream_);
     int rc = check_call(ctx, chans, nblk, nchan, sample_size, dst_device);
     if (!rc) rc = check_aligned(ctx, dst_device, "gpsb200_synth_blocks_device", "dst_device");
     if (!rc) {
@@ -1536,7 +1533,7 @@ int gpsb200_synth_blocks_device(gpsb200_ctx_t *ctx, const gpsb200_chan_t *chans,
 int gpsb200_slice_prepare(gpsb200_ctx_t *ctx, const gpsb200_chan_t *chans, int nblk, int nchan, int sample_size,
                           void *dst_device, void *dst_host, void *stream_, gpsb200_slice_link_t *link) {
     if (!ctx) return GPSB200_ERR_ARG;
-    cudaStream_t s = stream_ ? (cudaStream_t) stream_ : ctx->s_compute;
+    cudaStream_t s = caller_stream(ctx, stream_);
     return settle(ctx, s, slice_prepare(ctx, chans, nblk, nchan, sample_size, dst_device, dst_host, s, link));
 }
 
@@ -1690,7 +1687,7 @@ int gpsb200_replay_device(gpsb200_ctx_t *ctx, void *dst_device, void *stream_, i
     const int rc = check_aligned(ctx, dst_device, "gpsb200_replay_device", "dst_device");
     if (rc) return rc;
     CU(cudaSetDevice(ctx->cfg.device));
-    cudaStream_t s = stream_ ? (cudaStream_t) stream_ : ctx->s_compute;
+    cudaStream_t s = caller_stream(ctx, stream_);
     SynthArgs a = ctx->last;
     if (dst_device) a.out = dst_device;
     if (kernel_mask & 8) CU(launch_tables(a, s));
@@ -1725,7 +1722,7 @@ int gpsb200_acquire(gpsb200_ctx_t *ctx, const void *iq, int64_t nsamples, int sa
 int gpsb200_acquire_device(gpsb200_ctx_t *ctx, const void *iq_device, int64_t nsamples, int sample_size,
                            const gpsb200_acq_config_t *cfg, gpsb200_acq_result_t *res, uint64_t *grid, void *stream_) {
     if (!ctx) return GPSB200_ERR_ARG;
-    cudaStream_t s = stream_ ? (cudaStream_t) stream_ : ctx->s_compute;
+    cudaStream_t s = caller_stream(ctx, stream_);
     return settle(ctx, s, acquire(ctx, iq_device, nsamples, sample_size, cfg, false, nullptr, res, grid, true, s));
 }
 
@@ -1741,7 +1738,7 @@ int gpsb200_acquire_windows_device(gpsb200_ctx_t *ctx, const void *iq_device, in
                                    const gpsb200_acq_config_t *cfg, const double *f_lo_prn, gpsb200_acq_result_t *res,
                                    uint64_t *grid, void *stream_) {
     if (!ctx) return GPSB200_ERR_ARG;
-    cudaStream_t s = stream_ ? (cudaStream_t) stream_ : ctx->s_compute;
+    cudaStream_t s = caller_stream(ctx, stream_);
     return settle(ctx, s, acquire(ctx, iq_device, nsamples, sample_size, cfg, true, f_lo_prn, res, grid, true, s));
 }
 
@@ -1762,11 +1759,8 @@ int gpsb200_track_start(int prn, double doppler_hz, int64_t sample, gpsb200_trac
     memset(st, 0, sizeof *st);
     st->prn = prn;
     st->sample = sample;
-    st->carr_step = (int32_t) acq::phase_step(doppler_hz);
+    trk::start_steps(doppler_hz, st->carr_step, st->code_step);
     st->carr_freq = (int64_t) st->carr_step * 1024;
-    int64_t u = (int64_t) GPSB200_TRK_CODE_STEP_NOM + trk::tdiv(st->carr_step, 1540);
-    u = std::min<int64_t>(std::max<int64_t>(u, GPSB200_TRK_CODE_STEP_MIN), GPSB200_TRK_CODE_STEP_MAX);
-    st->code_step = (uint32_t) u;
     return GPSB200_OK;
 }
 
@@ -1782,7 +1776,7 @@ int gpsb200_track_device(gpsb200_ctx_t *ctx, const void *iq_device, int64_t nsam
                          gpsb200_track_state_t *state, int nchan, int max_epochs, gpsb200_track_epoch_t *epochs,
                          int32_t *nepochs, void *stream_) {
     if (!ctx) return GPSB200_ERR_ARG;
-    cudaStream_t s = stream_ ? (cudaStream_t) stream_ : ctx->s_compute;
+    cudaStream_t s = caller_stream(ctx, stream_);
     return settle(ctx, s, track(ctx, iq_device, nsamples, sample_size, base, state, nchan, max_epochs, epochs, nepochs,
                                 true, s));
 }
@@ -1863,7 +1857,7 @@ int gpsb200_snapshot_measure_device(gpsb200_ctx_t *ctx, const void *iq_device, i
                                     const gpsb200_acq_config_t *acq, const gpsb200_acq_result_t *res,
                                     const gpsb200_snapshot_config_t *cfg, gpsb200_snapshot_t *out, void *stream_) {
     if (!ctx) return GPSB200_ERR_ARG;
-    cudaStream_t s = stream_ ? (cudaStream_t) stream_ : ctx->s_compute;
+    cudaStream_t s = caller_stream(ctx, stream_);
     return settle(ctx, s, snapshot_measure(ctx, iq_device, nsamples, sample_size, acq, res, cfg, out, true, s));
 }
 
@@ -1917,7 +1911,7 @@ int gpsb200_raim_thresholds(double p_fa, double p_md, double *T, double *lambda)
 
 int gpsb200_pvt_replay(gpsb200_ctx_t *ctx, void *stream_) {
     if (!ctx) return GPSB200_ERR_ARG;
-    cudaStream_t s = stream_ ? (cudaStream_t) stream_ : ctx->s_compute;
+    cudaStream_t s = caller_stream(ctx, stream_);
     return settle(ctx, s, pvt_replay(ctx, s));
 }
 

@@ -21,12 +21,9 @@ namespace snap {
 namespace {
 
 using rx::load_iq;
-using rx::sine512;
-using trk::kHalf;
 using trk::kM;
 
 constexpr int kWarps = kThreads / 32;
-constexpr unsigned kFull = 0xffffffffu;
 
 struct Smem {
     int2 tab[512];                                  // (cos, sin)
@@ -37,18 +34,11 @@ struct Smem {
     gpsb200_snapshot_t rec;                         // owned by thread 0
 };
 
-__device__ __forceinline__ uint32_t clamp_u(int32_t w) {
-    int64_t u = (int64_t) GPSB200_TRK_CODE_STEP_NOM + trk::tdiv(w, 1540);
-    u = u < (int64_t) GPSB200_TRK_CODE_STEP_MIN ? (int64_t) GPSB200_TRK_CODE_STEP_MIN
-                                                 : (u > (int64_t) GPSB200_TRK_CODE_STEP_MAX ? (int64_t) GPSB200_TRK_CODE_STEP_MAX : u);
-    return (uint32_t) u;
-}
-
 // One pass over the K chunks with the replica at phi + m u (mod M) and the wipe-off at m w: the warp partials of every
 // chunk into sm.part (prompt only unless kCode).
 template <typename T, bool kCode>
 __device__ __forceinline__ void correlate(Smem &sm, const T *__restrict__ iq, int K, uint64_t phi, uint32_t u, uint32_t w) {
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int tid = threadIdx.x, warp = tid >> 5;
     constexpr int kSums = kCode ? 6 : 2;
 #pragma unroll 1
     for (int k = 0; k < K; k++) {
@@ -63,61 +53,43 @@ __device__ __forceinline__ void correlate(Smem &sm, const T *__restrict__ iq, in
                 const int m = kChunk * k + j;
                 int I, Q;
                 load_iq<T>(iq, m, I, Q);
-                const int2 cs = sm.tab[((uint32_t) m * w) >> 23];
-                const int dI = I * cs.x + Q * cs.y, dQ = Q * cs.x - I * cs.y;
+                const int2 d = rx::wipe_off(sm.tab, (uint32_t) m * w, I, Q);
                 uint64_t p = base + (uint64_t) j * u;   // base < M and j u <= 2999 u_max <= M: one fold
                 if (p >= kM) p -= kM;
-                const int cp = sm.ca[p >> 32];
-                a[kSums - 2] += cp * dI;
-                a[kSums - 1] += cp * dQ;
+                int ce, cp, cl;   // the early and late chips are not read in the frequency pass
+                rx::epl_chips(sm.ca, p, ce, cp, cl);
+                a[kSums - 2] += cp * d.x;
+                a[kSums - 1] += cp * d.y;
                 if (kCode) {
-                    uint64_t e = p + kHalf;
-                    if (e >= kM) e -= kM;
-                    const uint64_t l = p >= kHalf ? p - kHalf : p + kM - kHalf;
-                    const int ce = sm.ca[e >> 32], cl = sm.ca[l >> 32];
-                    a[0] += ce * dI;
-                    a[1] += ce * dQ;
-                    a[2] += cl * dI;
-                    a[3] += cl * dQ;
+                    a[0] += ce * d.x;
+                    a[1] += ce * d.y;
+                    a[2] += cl * d.x;
+                    a[3] += cl * d.y;
                 }
             }
         }
-#pragma unroll
-        for (int j = 0; j < kSums; j++)
-#pragma unroll
-            for (int o = 16; o > 0; o >>= 1) a[j] += __shfl_xor_sync(kFull, a[j], o);
-        if (lane == 0)
-#pragma unroll
-            for (int j = 0; j < kSums; j++) sm.part[k][warp][6 - kSums + j] = a[j];
+        rx::warp_partials(a, &sm.part[k][warp][6 - kSums]);
     }
 }
 
-// The chunk sum of quantity j (0..5 as in Smem::part) of chunk k over the warps.
-__device__ __forceinline__ int64_t chunk_sum(const Smem &sm, int k, int j) {
-    int v = 0;
-#pragma unroll
-    for (int q = 0; q < kWarps; q++) v += sm.part[k][q][j];
-    return v;
-}
-
 template <typename T>
-__global__ void __launch_bounds__(kThreads) k_snapshot(const T *__restrict__ iq, int K, const int8_t *__restrict__ codes,
+__global__ void __launch_bounds__(kThreads) k_snapshot(const T *__restrict__ iq, int K, const int8_t *__restrict__ chips,
                                                        int iterations, gpsb200_snapshot_t *__restrict__ recs) {
     __shared__ Smem sm;
     const int tid = threadIdx.x, lane = tid & 31;
-    for (int i = tid; i < 512; i += kThreads) sm.tab[i] = make_int2(sine512(i + 128), sine512(i));
+    rx::fill_carrier_table(sm.tab, kThreads);
     if (tid == 0) sm.rec = recs[blockIdx.x];
     __syncthreads();
     if (sm.rec.status != GPSB200_SNAP_OK) return;   // WEAK: the seed record stays (the whole CTA leaves)
-    for (int i = tid; i < GPSB200_CA_LEN; i += kThreads) sm.ca[i] = codes[sm.rec.prn * GPSB200_CA_LEN + i];
+    for (int i = tid; i < GPSB200_CA_LEN; i += kThreads) sm.ca[i] = chips[sm.rec.prn * GPSB200_CA_LEN + i];
     __syncthreads();
 
     // header step 2: the frequency pass at the seed
     correlate<T, false>(sm, iq, K, sm.rec.code_phase, sm.rec.code_step, (uint32_t) sm.rec.carr_step);
     __syncthreads();
     if (tid < K) {
-        sm.p[tid][0] = (int32_t) chunk_sum(sm, tid, 4);
-        sm.p[tid][1] = (int32_t) chunk_sum(sm, tid, 5);
+        sm.p[tid][0] = rx::warps_sum<kWarps>(sm.part[tid], 4);
+        sm.p[tid][1] = rx::warps_sum<kWarps>(sm.part[tid], 5);
     }
     __syncthreads();
     if (tid == 0) {
@@ -126,20 +98,15 @@ __global__ void __launch_bounds__(kThreads) k_snapshot(const T *__restrict__ iq,
             const int64_t pi = sm.p[k][0], pq = sm.p[k][1];
             pw += pi * pi + pq * pq;
             if (k + 1 < K) {
-                const int64_t ni = sm.p[k + 1][0], nq = sm.p[k + 1][1];
-                int64_t cross = pi * nq - pq * ni, dot = pi * ni + pq * nq;
-                if (dot < 0) {
-                    dot = -dot;
-                    cross = -cross;
-                }
-                sc += cross;
-                sd += dot;
+                const trk::CrossDot f = trk::fll(pi, pq, sm.p[k + 1][0], sm.p[k + 1][1]);
+                sc += f.cross;
+                sd += f.dot;
             }
         }
         sm.rec.power = (uint64_t) pw;
         if (K >= 2) {
             sm.rec.carr_step += (int32_t) trk::tdiv(trk::angle(sd, sc), 3000);
-            sm.rec.code_step = clamp_u(sm.rec.carr_step);
+            sm.rec.code_step = trk::code_step(sm.rec.carr_step);
         }
     }
     __syncthreads();
@@ -152,7 +119,7 @@ __global__ void __launch_bounds__(kThreads) k_snapshot(const T *__restrict__ iq,
         if (tid < K) {
             int64_t v[6];
 #pragma unroll
-            for (int j = 0; j < 6; j++) v[j] = chunk_sum(sm, tid, j);
+            for (int j = 0; j < 6; j++) v[j] = rx::warps_sum<kWarps>(sm.part[tid], j);
             sm.sq[tid][0] = v[0] * v[0] + v[1] * v[1];
             sm.sq[tid][1] = v[2] * v[2] + v[3] * v[3];
             sm.sq[tid][2] = v[4] * v[4] + v[5] * v[5];
@@ -167,16 +134,12 @@ __global__ void __launch_bounds__(kThreads) k_snapshot(const T *__restrict__ iq,
             }
 #pragma unroll
             for (int o = 16; o > 0; o >>= 1) {
-                E += __shfl_xor_sync(kFull, E, o);
-                L += __shfl_xor_sync(kFull, L, o);
-                P += __shfl_xor_sync(kFull, P, o);
+                E += __shfl_xor_sync(0xffffffffu, E, o);
+                L += __shfl_xor_sync(0xffffffffu, L, o);
+                P += __shfl_xor_sync(0xffffffffu, P, o);
             }
             if (tid == 0) {
-                const int bl = trk::bitlen64((uint64_t) (E + L));
-                const int s = bl > 40 ? bl - 40 : 0;
-                E >>= s;
-                L >>= s;
-                const int64_t D = (E + L) == 0 ? 0 : trk::tdiv((E - L) * 16384, E + L);
+                const int64_t D = trk::dll(E, L);
                 int64_t phi = (int64_t) sm.rec.code_phase + D * GPSB200_SNAP_GAIN;
                 phi = phi < 0 ? phi + (int64_t) kM : (phi >= (int64_t) kM ? phi - (int64_t) kM : phi);
                 sm.rec.code_phase = (uint64_t) phi;
@@ -229,11 +192,7 @@ void seed(const gpsb200_acq_config_t *acq, const gpsb200_acq_result_t *res, cons
         memset(&o, 0, sizeof o);
         o.prn = r.prn;
         o.sample = acq->s0;
-        o.carr_step = (int32_t) acq::phase_step(r.doppler_hz);
-        int64_t u = (int64_t) GPSB200_TRK_CODE_STEP_NOM + trk::tdiv(o.carr_step, 1540);
-        u = u < (int64_t) GPSB200_TRK_CODE_STEP_MIN ? (int64_t) GPSB200_TRK_CODE_STEP_MIN
-                                                     : (u > (int64_t) GPSB200_TRK_CODE_STEP_MAX ? (int64_t) GPSB200_TRK_CODE_STEP_MAX : u);
-        o.code_step = (uint32_t) u;
+        trk::start_steps(r.doppler_hz, o.carr_step, o.code_step);
         o.code_phase = (kM - ((uint64_t) r.delay * o.code_step) % kM) % kM;
         o.ratio = r.ratio;
         o.status = r.ratio >= cfg->min_ratio ? GPSB200_SNAP_OK : GPSB200_SNAP_WEAK;
@@ -245,14 +204,14 @@ void scratch_free(Scratch &sc) {
     sc = Scratch();
 }
 
-cudaError_t launch(Scratch &sc, const void *window, int sample_size, int K, int nprn, const int8_t *codes, int iterations,
+cudaError_t launch(Scratch &sc, const void *window, int sample_size, int K, int nprn, const int8_t *chips, int iterations,
                    gpsb200_snapshot_t *rec, cudaStream_t s) {
     if (!sc.d_rec) CU_RET(cudaMalloc(&sc.d_rec, 32 * sizeof(gpsb200_snapshot_t)));
     CU_RET(cudaMemcpyAsync(sc.d_rec, rec, nprn * sizeof(gpsb200_snapshot_t), cudaMemcpyHostToDevice, s));
     if (sample_size == GPSB200_SC08)
-        k_snapshot<int8_t><<<nprn, kThreads, 0, s>>>(static_cast<const int8_t *>(window), K, codes, iterations, sc.d_rec);
+        k_snapshot<int8_t><<<nprn, kThreads, 0, s>>>(static_cast<const int8_t *>(window), K, chips, iterations, sc.d_rec);
     else
-        k_snapshot<int16_t><<<nprn, kThreads, 0, s>>>(static_cast<const int16_t *>(window), K, codes, iterations,
+        k_snapshot<int16_t><<<nprn, kThreads, 0, s>>>(static_cast<const int16_t *>(window), K, chips, iterations,
                                                       sc.d_rec);
     CU_RET(cudaGetLastError());
     CU_RET(cudaMemcpyAsync(rec, sc.d_rec, nprn * sizeof(gpsb200_snapshot_t), cudaMemcpyDeviceToHost, s));

@@ -28,8 +28,8 @@ struct Scratch {
 };
 void scratch_free(Scratch &sc);
 // Enqueue the refinement of rec [nprn] (seeded) over the window at `window` (stream sample s0 first) on s and wait for
-// the records. codes: [33][1023] chips as +-1 (trk::Scratch::d_codes).
-cudaError_t launch(Scratch &sc, const void *window, int sample_size, int K, int nprn, const int8_t *codes, int iterations,
+// the records. chips: [33][1023] chips as +-1 (trk::chips_upload).
+cudaError_t launch(Scratch &sc, const void *window, int sample_size, int K, int nprn, const int8_t *chips, int iterations,
                    gpsb200_snapshot_t *rec, cudaStream_t s);
 
 }  // namespace snap

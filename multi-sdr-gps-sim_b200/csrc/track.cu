@@ -8,6 +8,7 @@
 #include <cstring>
 #include <vector>
 
+#include "acquire.h"
 #include "device_buffer.h"
 #include "rx_samples.cuh"
 #include "synth_tables.h"
@@ -19,7 +20,6 @@ namespace trk {
 namespace {
 
 using rx::load_iq;
-using rx::sine512;
 
 constexpr int kWarps = kThreads / 32;
 
@@ -33,16 +33,16 @@ struct Smem {
 
 template <typename T>
 __global__ void __launch_bounds__(kThreads)
-k_track(const T *__restrict__ iq, int64_t nsamples, int64_t base, const int8_t *__restrict__ codes,
+k_track(const T *__restrict__ iq, int64_t nsamples, int64_t base, const int8_t *__restrict__ chips,
         gpsb200_track_state_t *__restrict__ states, int max_epochs, gpsb200_track_epoch_t *__restrict__ epochs,
         int32_t *__restrict__ nepochs) {
     __shared__ Smem sm;
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int tid = threadIdx.x, warp = tid >> 5;
     const int ch = blockIdx.x;
-    for (int i = tid; i < 512; i += kThreads) sm.tab[i] = make_int2(sine512(i + 128), sine512(i));
+    rx::fill_carrier_table(sm.tab, kThreads);
     if (tid == 0) sm.st = states[ch];
     __syncthreads();
-    for (int i = tid; i < GPSB200_CA_LEN; i += kThreads) sm.ca[i] = codes[sm.st.prn * GPSB200_CA_LEN + i];
+    for (int i = tid; i < GPSB200_CA_LEN; i += kThreads) sm.ca[i] = chips[sm.st.prn * GPSB200_CA_LEN + i];
     const int64_t end = base + nsamples;
     gpsb200_track_epoch_t *out = epochs + (size_t) ch * max_epochs;
     int k = 0;
@@ -64,36 +64,22 @@ k_track(const T *__restrict__ iq, int64_t nsamples, int64_t base, const int8_t *
             if (m < L) {
                 int I, Q;
                 load_iq<T>(iq, s + m, I, Q);
-                const int2 cs = sm.tab[(theta + (uint32_t) m * w) >> 23];
-                const int dI = I * cs.x + Q * cs.y, dQ = Q * cs.x - I * cs.y;
-                const uint64_t p = phi + (uint64_t) m * u;
-                uint64_t e = p + kHalf;
-                if (e >= kM) e -= kM;
-                const uint64_t l = p >= kHalf ? p - kHalf : p + kM - kHalf;
-                const int ce = sm.ca[e >> 32], cp = sm.ca[p >> 32], cl = sm.ca[l >> 32];
-                a[0] += ce * dI;
-                a[1] += ce * dQ;
-                a[2] += cp * dI;
-                a[3] += cp * dQ;
-                a[4] += cl * dI;
-                a[5] += cl * dQ;
+                const int2 d = rx::wipe_off(sm.tab, theta + (uint32_t) m * w, I, Q);
+                int ce, cp, cl;
+                rx::epl_chips(sm.ca, phi + (uint64_t) m * u, ce, cp, cl);
+                a[0] += ce * d.x;
+                a[1] += ce * d.y;
+                a[2] += cp * d.x;
+                a[3] += cp * d.y;
+                a[4] += cl * d.x;
+                a[5] += cl * d.y;
             }
         }
-#pragma unroll
-        for (int j = 0; j < 6; j++)
-#pragma unroll
-            for (int o = 16; o > 0; o >>= 1) a[j] += __shfl_xor_sync(0xffffffffu, a[j], o);
-        if (lane == 0)
-#pragma unroll
-            for (int j = 0; j < 6; j++) sm.part[warp][j] = a[j];
+        rx::warp_partials(a, sm.part[warp]);
         __syncthreads();
         if (tid == 0) {
             int32_t c[6];
-            for (int j = 0; j < 6; j++) {
-                int v = 0;
-                for (int q = 0; q < kWarps; q++) v += sm.part[q][j];
-                c[j] = v;
-            }
+            for (int j = 0; j < 6; j++) c[j] = rx::warps_sum<kWarps>(sm.part, j);
             gpsb200_track_state_t st = sm.st;
             const int64_t s_abs = st.sample;
             st.sample += L;
@@ -148,16 +134,24 @@ std::string check(const gpsb200_track_state_t *st, int nchan, int max_epochs, in
     return std::string();
 }
 
+void start_steps(double doppler_hz, int32_t &w, uint32_t &u) {
+    w = (int32_t) acq::phase_step(doppler_hz);
+    u = code_step(w);
+}
+
+cudaError_t chips_upload(int8_t **d) {
+    std::vector<int8_t> c((size_t) 33 * GPSB200_CA_LEN, 0);
+    for (int prn = 1; prn <= 32; prn++) {
+        uint8_t ca[GPSB200_CA_LEN];
+        ca_code(prn, ca);
+        for (int i = 0; i < GPSB200_CA_LEN; i++) c[(size_t) prn * GPSB200_CA_LEN + i] = (int8_t) (2 * ca[i] - 1);
+    }
+    CU_RET(cudaMalloc(d, c.size()));
+    return cudaMemcpy(*d, c.data(), c.size(), cudaMemcpyHostToDevice);
+}
+
 cudaError_t scratch_reserve(Scratch &sc, int nchan, int max_epochs) {
-    if (!sc.d_codes) {
-        std::vector<int8_t> c((size_t) 33 * GPSB200_CA_LEN, 0);
-        for (int prn = 1; prn <= 32; prn++) {
-            uint8_t ca[GPSB200_CA_LEN];
-            ca_code(prn, ca);
-            for (int i = 0; i < GPSB200_CA_LEN; i++) c[(size_t) prn * GPSB200_CA_LEN + i] = (int8_t) (2 * ca[i] - 1);
-        }
-        CU_RET(cudaMalloc(&sc.d_codes, c.size()));
-        CU_RET(cudaMemcpy(sc.d_codes, c.data(), c.size(), cudaMemcpyHostToDevice));
+    if (!sc.d_state) {
         CU_RET(cudaMalloc(&sc.d_state, GPSB200_TRK_MAX_CHAN * sizeof(gpsb200_track_state_t)));
         CU_RET(cudaMalloc(&sc.d_n, GPSB200_TRK_MAX_CHAN * sizeof(int32_t)));
     }
@@ -165,22 +159,21 @@ cudaError_t scratch_reserve(Scratch &sc, int nchan, int max_epochs) {
 }
 
 void scratch_free(Scratch &sc) {
-    cudaFree(sc.d_codes);
     cudaFree(sc.d_state);
     cudaFree(sc.d_epochs);
     cudaFree(sc.d_n);
     sc = Scratch();
 }
 
-cudaError_t launch(Scratch &sc, const void *src, int64_t nsamples, int sample_size, int64_t base,
+cudaError_t launch(Scratch &sc, const int8_t *chips, const void *src, int64_t nsamples, int sample_size, int64_t base,
                    gpsb200_track_state_t *state, int nchan, int max_epochs, gpsb200_track_epoch_t *epochs,
                    int32_t *nepochs, cudaStream_t s) {
     CU_RET(cudaMemcpyAsync(sc.d_state, state, nchan * sizeof(gpsb200_track_state_t), cudaMemcpyHostToDevice, s));
     if (sample_size == GPSB200_SC08)
-        k_track<int8_t><<<nchan, kThreads, 0, s>>>(static_cast<const int8_t *>(src), nsamples, base, sc.d_codes,
+        k_track<int8_t><<<nchan, kThreads, 0, s>>>(static_cast<const int8_t *>(src), nsamples, base, chips,
                                                    sc.d_state, max_epochs, sc.d_epochs, sc.d_n);
     else
-        k_track<int16_t><<<nchan, kThreads, 0, s>>>(static_cast<const int16_t *>(src), nsamples, base, sc.d_codes,
+        k_track<int16_t><<<nchan, kThreads, 0, s>>>(static_cast<const int16_t *>(src), nsamples, base, chips,
                                                     sc.d_state, max_epochs, sc.d_epochs, sc.d_n);
     CU_RET(cudaGetLastError());
     CU_RET(cudaMemcpyAsync(nepochs, sc.d_n, nchan * sizeof(int32_t), cudaMemcpyDeviceToHost, s));

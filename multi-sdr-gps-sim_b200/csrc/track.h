@@ -58,6 +58,38 @@ __host__ __device__ inline int32_t angle(int64_t x, int64_t y) {
     return (int32_t) z;
 }
 
+// The code step at carrier step w and DLL discriminator D: NOM + w / 1540 + 2048 D / 3000 (carrier aided), clamped to
+// GPSB200_TRK_CODE_STEP_MIN..MAX. A start state and the snapshot measurement take D = 0.
+__host__ __device__ inline uint32_t code_step(int32_t w, int64_t D = 0) {
+    int64_t u = (int64_t) GPSB200_TRK_CODE_STEP_NOM + tdiv(w, 1540) + tdiv(2048 * D, 3000);
+    u = u < (int64_t) GPSB200_TRK_CODE_STEP_MIN ? (int64_t) GPSB200_TRK_CODE_STEP_MIN
+                                                 : (u > (int64_t) GPSB200_TRK_CODE_STEP_MAX ? (int64_t) GPSB200_TRK_CODE_STEP_MAX : u);
+    return (uint32_t) u;
+}
+
+// DLL discriminator of early and late powers E, L >= 0: both shifted to at most 40 bits, then (E - L) 2^14 / (E + L).
+__host__ __device__ inline int64_t dll(int64_t E, int64_t L) {
+    const int bl = bitlen64((uint64_t) (E + L));
+    const int s = bl > 40 ? bl - 40 : 0;
+    E >>= s;
+    L >>= s;
+    return (E + L) == 0 ? 0 : tdiv((E - L) * 16384, E + L);
+}
+
+// FLL terms of the prompt sums (i0, q0) and the next ones (i1, q1): cross and dot, both negated when dot < 0 (a data
+// bit flipped between them). The loop takes the angle of one pair, the snapshot the angle of the sums over its chunks.
+struct CrossDot {
+    int64_t cross, dot;
+};
+__host__ __device__ inline CrossDot fll(int64_t i0, int64_t q0, int64_t i1, int64_t q1) {
+    const int64_t cross = i0 * q1 - q0 * i1, dot = i0 * i1 + q0 * q1;
+    return dot < 0 ? CrossDot{-cross, -dot} : CrossDot{cross, dot};
+}
+
+// The carrier step w = acq::phase_step(doppler_hz) and code step u = code_step(w) a channel starts from at an
+// acquisition's Doppler (gpsb200_track_start, the snapshot measurement's seed).
+void start_steps(double doppler_hz, int32_t &w, uint32_t &u);
+
 // One loop update after a period with sums c[6] = E_I, E_Q, P_I, P_Q, L_I, L_Q. Updates carr_freq, carr_step, code_step,
 // prev_*, lock_*, lock and epochs of st (the phases and sample are advanced by the caller).
 __host__ __device__ inline void loop_update(gpsb200_track_state_t &st, const int32_t c[6]) {
@@ -67,13 +99,8 @@ __host__ __device__ inline void loop_update(gpsb200_track_state_t &st, const int
     int64_t F = st.carr_freq;
     // FLL assist during pull-in
     if (st.epochs >= 1 && st.epochs < GPSB200_TRK_FLL_EPOCHS) {
-        int64_t cross = (int64_t) st.prev_i * pq - (int64_t) st.prev_q * pi;
-        int64_t dot = (int64_t) st.prev_i * pi + (int64_t) st.prev_q * pq;
-        if (dot < 0) {
-            dot = -dot;
-            cross = -cross;
-        }
-        F += tdiv(64 * (int64_t) angle(dot, cross), 3000);
+        const CrossDot f = fll(st.prev_i, st.prev_q, pi, pq);
+        F += tdiv(64 * (int64_t) angle(f.dot, f.cross), 3000);
     }
     F += (int64_t) (e >> 12);
     F = F > kFreqClamp ? kFreqClamp : (F < -kFreqClamp ? -kFreqClamp : F);
@@ -81,17 +108,8 @@ __host__ __device__ inline void loop_update(gpsb200_track_state_t &st, const int
     const int32_t w = (int32_t) ((F >> 10) + (int64_t) (e >> 16));
     st.carr_step = w;
     // DLL: normalised early-minus-late power, carrier aided
-    int64_t E = (int64_t) c[0] * c[0] + (int64_t) c[1] * c[1];
-    int64_t L = (int64_t) c[4] * c[4] + (int64_t) c[5] * c[5];
-    const int bl = bitlen64((uint64_t) (E + L));
-    const int s = bl > 40 ? bl - 40 : 0;
-    E >>= s;
-    L >>= s;
-    const int64_t D = (E + L) == 0 ? 0 : tdiv((E - L) * 16384, E + L);
-    int64_t u = (int64_t) GPSB200_TRK_CODE_STEP_NOM + tdiv(w, 1540) + tdiv(2048 * D, 3000);
-    u = u < (int64_t) GPSB200_TRK_CODE_STEP_MIN ? (int64_t) GPSB200_TRK_CODE_STEP_MIN
-                                                 : (u > (int64_t) GPSB200_TRK_CODE_STEP_MAX ? (int64_t) GPSB200_TRK_CODE_STEP_MAX : u);
-    st.code_step = (uint32_t) u;
+    const int64_t D = dll((int64_t) c[0] * c[0] + (int64_t) c[1] * c[1], (int64_t) c[4] * c[4] + (int64_t) c[5] * c[5]);
+    st.code_step = code_step(w, D);
     // narrow-band lock indicator
     const int32_t api = (int32_t) (pi < 0 ? -pi : pi), apq = (int32_t) (pq < 0 ? -pq : pq);
     st.lock_i += (api - st.lock_i) >> 4;
@@ -109,9 +127,11 @@ __host__ __device__ inline int period_len(uint64_t phi, uint32_t u) { return (in
 std::string check(const gpsb200_track_state_t *st, int nchan, int max_epochs, int64_t nsamples, int64_t base,
                   int sample_size);
 
+// The [33][1023] C/A chips as +-1 (row 0 unused) that k_track and k_snapshot read, in a new device buffer *d.
+cudaError_t chips_upload(int8_t **d);
+
 // Device scratch of the tracking calls of one context, grown as needed.
 struct Scratch {
-    int8_t *d_codes = nullptr;                   // [33][1023] chips as +-1, row 0 unused
     gpsb200_track_state_t *d_state = nullptr;    // [GPSB200_TRK_MAX_CHAN]
     gpsb200_track_epoch_t *d_epochs = nullptr;   // [nchan][max_epochs]
     size_t epoch_cap = 0;
@@ -121,7 +141,8 @@ struct Scratch {
 cudaError_t scratch_reserve(Scratch &sc, int nchan, int max_epochs);
 void scratch_free(Scratch &sc);
 // Enqueue the tracking of the samples at `src` (stream sample `base` first) on s and wait for the results.
-cudaError_t launch(Scratch &sc, const void *src, int64_t nsamples, int sample_size, int64_t base,
+// chips: chips_upload's table.
+cudaError_t launch(Scratch &sc, const int8_t *chips, const void *src, int64_t nsamples, int sample_size, int64_t base,
                    gpsb200_track_state_t *state, int nchan, int max_epochs, gpsb200_track_epoch_t *epochs,
                    int32_t *nepochs, cudaStream_t s);
 

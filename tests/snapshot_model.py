@@ -2,8 +2,8 @@
 fixes from snapshot records (gpsb200_pvt_snapshot / gpsb200_pvt_snapshot_search): the tests' reference.
 
 It shares no code with the library: samples, carrier tables, phase-step rounding and C/A codes come from acq_model, the
-CORDIC angle, truncating division and bit lengths from track_model. Everything runs in int64 (Python ints where a
-product could leave it). The fixes restate only the measurement step; the solve is coarse_model's, run at each
+CORDIC angle, truncating division, the code-step rule and the DLL discriminator from track_model. Everything runs in
+int64 (Python ints where a product could leave it). The fixes restate only the measurement step; the solve is coarse_model's, run at each
 snapshot's instant with its measurement step replaced by the one below."""
 import numpy as np
 
@@ -22,15 +22,11 @@ SNAPSHOT_DTYPE = np.dtype([("prn", "<i4"), ("status", "<i4"), ("sample", "<i8"),
 assert SNAPSHOT_DTYPE.itemsize == 56
 
 
-def clamp_u(w):
-    return int(np.clip(T.CODE_STEP_NOM + int(T.tdiv(np.int64(w), 1540)), T.CODE_STEP_MIN, T.CODE_STEP_MAX))
-
-
 def seed(res_row, s0):
     """Step 1: (w0, u0, phi0) of one acquisition result."""
     w = A.phase_step(float(res_row["doppler_hz"]))
     w = w - (1 << 32) if w >= 1 << 31 else w
-    u = clamp_u(w)
+    u = int(T.code_step_of(np.int64(w)))
     phi = (-int(res_row["delay"]) * u) % M
     return w, u, phi
 
@@ -79,11 +75,7 @@ def dll(ei, eq, li, lq):
     E = sum(int(a) * int(a) + int(b) * int(b) for a, b in zip(ei, eq))
     L = sum(int(a) * int(a) + int(b) * int(b) for a, b in zip(li, lq))
     assert E + L < 2 ** 63
-    s = max(0, (E + L).bit_length() - 40)
-    E, L = E >> s, L >> s
-    if E + L == 0:
-        return 0
-    return int(T.tdiv(np.int64((E - L) * 16384), np.int64(E + L)))
+    return int(T.dll(E, L))
 
 
 def power(pi, pq):
@@ -111,7 +103,7 @@ def measure(iq, sample_size, s0, K, res, min_ratio=2.5, iterations=12, trace=Non
         pw = power(f["pi"], f["pq"])
         if K >= 2:
             w = w + freq_step(f["pi"], f["pq"])
-            u = clamp_u(w)
+            u = int(T.code_step_of(np.int64(w)))
         D = 0
         ds = []
         for _ in range(iterations):

@@ -162,6 +162,18 @@ def test_model_truncating_division():
     assert list(T.tdiv(np.array([7, -7, 7, -7]), np.array([2, 2, -2, -2]))) == [3, -3, -3, 3]
 
 
+def test_track_start_is_the_model():
+    """gpsb200_track_start (the library's start steps, which the snapshot measurement also seeds from) equals the
+    model's start state at Dopplers across +-10 kHz: whole and fractional Hz, both signs, the range's ends."""
+    rng = np.random.default_rng(11)
+    dopplers = np.concatenate([np.linspace(-10000.0, 10000.0, 801), rng.uniform(-10000.0, 10000.0, 400),
+                               [-0.4, 0.4, -1e-9, 0.0]])
+    for i, f in enumerate(dopplers):
+        prn, sample = 1 + i % 32, 7919 * i
+        got, want = gps.track_start(prn, f, sample), T.start(prn, f, sample)
+        assert all(got[k] == want[k] for k in T.STATE_DTYPE.names), (f, got, want)
+
+
 def model_run(name, nblk):
     g = scenario.load_golden(name)
     ch = golden_rows(g, range(nblk))

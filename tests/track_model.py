@@ -63,8 +63,19 @@ def angle(x, y):
     return z
 
 
-def code_step_of(w, D):
-    return np.clip(CODE_STEP_NOM + tdiv(w, 1540) + tdiv(2048 * D, 3000), CODE_STEP_MIN, CODE_STEP_MAX)
+def code_step_of(w, D=0):
+    """The code step at carrier step w and DLL discriminator D (D = 0: a start state and the snapshot measurement)."""
+    return np.clip(CODE_STEP_NOM + tdiv(w, 1540) + tdiv(2048 * np.asarray(D, np.int64), 3000), CODE_STEP_MIN,
+                   CODE_STEP_MAX)
+
+
+def dll(E, L):
+    """DLL discriminator of early and late powers E, L >= 0: both shifted to 40 bits, then (E - L) 2^14 / (E + L)."""
+    E, L = np.asarray(E, np.int64), np.asarray(L, np.int64)
+    s = excess_bits(E + L, 40)
+    E, L = E >> s, L >> s
+    tot = E + L
+    return np.where(tot == 0, 0, tdiv((E - L) * 16384, np.where(tot == 0, 1, tot)))
 
 
 def start(prn, doppler_hz, sample):
@@ -73,7 +84,7 @@ def start(prn, doppler_hz, sample):
     w = A.phase_step(doppler_hz)
     w = w - (1 << 32) if w >= 1 << 31 else w
     st["prn"], st["sample"], st["carr_step"], st["carr_freq"] = prn, sample, w, w * 1024
-    st["code_step"] = int(code_step_of(np.int64(w), np.int64(0)))
+    st["code_step"] = int(code_step_of(np.int64(w)))
     return st
 
 
@@ -93,13 +104,7 @@ def loop_update(S, c):
     S["carr_freq"] = F
     w = (F >> 10) + (e >> 16)
     S["carr_step"] = w
-    E = c[0] * c[0] + c[1] * c[1]
-    L = c[4] * c[4] + c[5] * c[5]
-    s = excess_bits(E + L, 40)
-    E, L = E >> s, L >> s
-    tot = E + L
-    D = np.where(tot == 0, 0, tdiv((E - L) * 16384, np.where(tot == 0, 1, tot)))
-    S["code_step"] = code_step_of(w, D)
+    S["code_step"] = code_step_of(w, dll(c[0] * c[0] + c[1] * c[1], c[4] * c[4] + c[5] * c[5]))
     S["lock_i"] = S["lock_i"] + ((np.abs(pi) - S["lock_i"]) >> 4)
     S["lock_q"] = S["lock_q"] + ((np.abs(pq) - S["lock_q"]) >> 4)
     S["lock"] = (3 * S["lock_q"] < S["lock_i"]).astype(np.int64)
