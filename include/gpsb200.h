@@ -971,6 +971,36 @@ int gpsb200_snapshot_measure(gpsb200_ctx_t *ctx, const void *iq, int64_t nsample
 int gpsb200_snapshot_measure_device(gpsb200_ctx_t *ctx, const void *iq_device, int64_t nsamples, int sample_size,
                                     const gpsb200_acq_config_t *acq, const gpsb200_acq_result_t *res,
                                     const gpsb200_snapshot_config_t *cfg, gpsb200_snapshot_t *out, void *stream);
+/* ---- snapshot batch: the search and the measurement above over many windows of one source in one call (DESIGN §11.6)
+ * Window w (0 <= w < nwin) starts at sample s0[w]; windows may overlap, repeat and come in any order. acq->s0 is not
+ * read; K, the PRN list, the bins and cfg are shared by every window. Row w of res [nwin][acq->nprn] and of out
+ * [nwin][acq->nprn] is, bit for bit, what these single calls give:
+ *   search     gpsb200_acquire with acq->s0 = s0[w] (f_lo NULL: the standard grid from acq->f_lo_hz), or
+ *              gpsb200_acquire_windows with acq->s0 = s0[w] and f_lo_prn = f_lo + w * acq->nprn (f_lo [nwin][nprn]);
+ *   measure    gpsb200_snapshot_measure with acq->s0 = s0[w] on those results, with cfg.
+ * Every argument is checked before anything is enqueued (GPSB200_ERR_ARG): nwin >= 1, s0 and the other pointers not
+ * NULL, cfg as gpsb200_snapshot_measure checks it, and every window as its single search checks it (the window inside
+ * the buffer, each f_lo row finite with its bins within +-1.5 MHz). The measurement's check of the results (|doppler_hz|
+ * <= 10 kHz) can only be made after the search: a window that fails it ends the call with GPSB200_ERR_ARG before its
+ * pass is measured. The search grid is not offered. Blocking.
+ * Passes: the windows run in consecutive passes of P = max(1, floor(GPSB200_SNAP_BATCH_SCRATCH / B)) windows (the last
+ * may hold fewer), B = nprn nbins 24028 + nprn 128 + 8 + (3000 K + 2999) 2 sample_size bytes: the device scratch one window
+ * may take (the split search's powers, its rows and phase steps, the per-pair tables, records and the staged window), so
+ * a pass of two windows or more stays within the cap, and its (window, PRN) pairs far below the grid's y limit. The
+ * search of a pass with fewer (window, PRN, bin) rows than a full wave (3 CTAs on every SM) splits them as one search of
+ * that many rows would; a larger pass runs unsplit; gpsb200_debug_acq_split forces a split for batches as for single
+ * searches. Neither the passes nor the split change a result. Between the search and the measurement of a pass, the
+ * results come down once and the seeded records go up once. Of a host source only the windows go up, packed. */
+#define GPSB200_SNAP_BATCH_SCRATCH (256LL << 20)
+int gpsb200_snapshot_batch(gpsb200_ctx_t *ctx, const void *iq, int64_t nsamples, int sample_size,
+                           const gpsb200_acq_config_t *acq, int nwin, const int64_t *s0, const double *f_lo,
+                           const gpsb200_snapshot_config_t *cfg, gpsb200_acq_result_t *res, gpsb200_snapshot_t *out);
+/* Same for a source in device memory (16-byte aligned), searched and measured in place on `stream` (0 = the context's
+ * own stream) behind whatever it holds; returns when the results and records are in host memory. */
+int gpsb200_snapshot_batch_device(gpsb200_ctx_t *ctx, const void *iq_device, int64_t nsamples, int sample_size,
+                                  const gpsb200_acq_config_t *acq, int nwin, const int64_t *s0, const double *f_lo,
+                                  const gpsb200_snapshot_config_t *cfg, gpsb200_acq_result_t *res,
+                                  gpsb200_snapshot_t *out, void *stream);
 /* ---- fixes from snapshot records (DESIGN §11.5): gpsb200_pvt_coarse and gpsb200_pvt_search with meas [nsnap][nchan]
  * in place of the epochs. Snapshot i's fix instant is its records' common `sample` (all nchan records of a row must hold
  * the same sample, 0..2^62; else GPSB200_ERR_ARG); cfg->nfix is nsnap (>= 1); cfg->iono, alpha and beta apply; cfg->s0

@@ -21,7 +21,7 @@ from .api import (  # noqa: F401
     SEARCH_CONFIG_DTYPE, SEARCH_DTYPE, SEARCH_NODES, search_config, search_nodes,
     SKY_DTYPE, nav_almanac, almanac_predict,
     SNAPSHOT_CONFIG_DTYPE, SNAPSHOT_DTYPE, SNAP_OK, SNAP_WEAK, SNAP_NO_CONVERGENCE, SNAP_ITERATIONS, SNAP_MAX_ITER,
-    snapshot_config,
+    snapshot_config, SNAP_BATCH_SCRATCH, snapshot_batch_pass,
 )
 from .synthetic import synthetic_chans  # noqa: F401,E402
 from . import sharding  # noqa: F401,E402

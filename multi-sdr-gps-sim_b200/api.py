@@ -289,6 +289,14 @@ SNAPSHOT_DTYPE = np.dtype([("prn", "<i4"), ("status", "<i4"), ("sample", "<i8"),
 assert (SNAPSHOT_CONFIG_DTYPE.itemsize, SNAPSHOT_DTYPE.itemsize) == (16, 56)
 SNAP_OK, SNAP_WEAK, SNAP_NO_CONVERGENCE = 0, 1, 2
 SNAP_ITERATIONS, SNAP_MAX_ITER = 12, 16
+SNAP_BATCH_SCRATCH = 256 << 20   # GPSB200_SNAP_BATCH_SCRATCH: the device-scratch cap of a batch pass, bytes
+
+
+def snapshot_batch_pass(nprn, nbins, ms, sample_size=SC08):
+    """The windows of one pass of gpsb200_snapshot_batch (at least one): how many fit the scratch cap, as the header
+    states it."""
+    b = nprn * nbins * 24028 + nprn * 128 + 8 + acq_window_samples(ms) * 2 * int(sample_size)
+    return max(1, SNAP_BATCH_SCRATCH // b)
 
 
 def snapshot_config(min_ratio=2.5, iterations=SNAP_ITERATIONS):
@@ -421,7 +429,7 @@ EXPORTS = ["gpsb200_create", "gpsb200_destroy", "gpsb200_last_error", "gpsb200_v
            "gpsb200_track",
            "gpsb200_track_device", "gpsb200_nav_decode", "gpsb200_nav_word_check", "gpsb200_nav_parity",
            "gpsb200_nav_ephemeris", "gpsb200_nav_time_anchor", "gpsb200_pvt", "gpsb200_pvt_replay",
-           "gpsb200_pvt_raim", "gpsb200_raim_thresholds", "gpsb200_pvt_araim", "gpsb200_araim_kfa", "gpsb200_pvt_coarse", "gpsb200_pvt_search", "gpsb200_search_nodes", "gpsb200_snapshot_measure", "gpsb200_snapshot_measure_device", "gpsb200_pvt_snapshot", "gpsb200_pvt_snapshot_search", "gpsb200_rinex_ephemeris", "gpsb200_bind_numa", "gpsb200_span_chain_host", "gpsb200_lanes_model_block",
+           "gpsb200_pvt_raim", "gpsb200_raim_thresholds", "gpsb200_pvt_araim", "gpsb200_araim_kfa", "gpsb200_pvt_coarse", "gpsb200_pvt_search", "gpsb200_search_nodes", "gpsb200_snapshot_measure", "gpsb200_snapshot_measure_device", "gpsb200_snapshot_batch", "gpsb200_snapshot_batch_device", "gpsb200_pvt_snapshot", "gpsb200_pvt_snapshot_search", "gpsb200_rinex_ephemeris", "gpsb200_bind_numa", "gpsb200_span_chain_host", "gpsb200_lanes_model_block",
            "gpsb200_lanes_window_band_host", "gpsb200_slice_prepare", "gpsb200_slice_probe",
            "gpsb200_slice_finish", "gpsb200_slice_finish_cb", "gpsb200_slice_wait", "gpsb200_link_apply", "gpsb200_slice_link_host", "gpsb200_debug_corrupt_chain", "gpsb200_synth_kernel_name",
            "gpsb200_debug_run_checkpoints", "gpsb200_checkpoint_segments_host",
@@ -544,6 +552,9 @@ def lib():
         L.gpsb200_snapshot_measure.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.POINTER(AcqConfig),
                                                C.c_void_p, C.c_void_p, C.c_void_p]
         L.gpsb200_snapshot_measure_device.argtypes = L.gpsb200_snapshot_measure.argtypes + [C.c_void_p]
+        L.gpsb200_snapshot_batch.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.POINTER(AcqConfig), C.c_int,
+                                             C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+        L.gpsb200_snapshot_batch_device.argtypes = L.gpsb200_snapshot_batch.argtypes + [C.c_void_p]
         L.gpsb200_pvt_snapshot.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
                                            C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
         L.gpsb200_pvt_snapshot_search.argtypes = L.gpsb200_pvt_snapshot.argtypes + [C.c_void_p]
@@ -1204,6 +1215,36 @@ class Context:
         self._check(fn(self._h, src, n, int(sample_size), C.byref(acq), r.ctypes.data, sc.ctypes.data, out.ctypes.data,
                        *dev))
         return out[:len(prns)]
+
+    def snapshot_batch(self, s0, iq=None, sample_size=SC08, prns=range(1, 33), ms=10, f_lo=-5000.0, step=250.0,
+                       nbins=41, f_lo_prn=None, cfg=None, device_ptr=None, nsamples=None, stream=0):
+        """The search and the snapshot measurement of many windows in one call (gpsb200_snapshot_batch; DESIGN §11.6):
+        window w starts at sample s0[w] (windows may overlap, repeat and come in any order). Without f_lo_prn every
+        window searches the standard grid f_lo + j * step, as acquire; with f_lo_prn (float64[nwin, nprn]) window w
+        searches PRN prns[p] from f_lo_prn[w, p], as acquire_windows. cfg: SNAPSHOT_CONFIG_DTYPE record (snapshot_config(),
+        the default). Source as acquire.
+        -> (results ACQ_RESULT_DTYPE[nwin, nprn], SNAPSHOT_DTYPE[nwin, nprn]): row w equals acquire (or
+        acquire_windows) with s0=s0[w] and snapshot_measure on its results, bit for bit."""
+        prns = [int(p) for p in prns]
+        s = np.ascontiguousarray(s0, dtype=np.int64).reshape(-1)
+        nwin = s.size
+        flo = None
+        if f_lo_prn is not None:
+            flo = np.ascontiguousarray(f_lo_prn, dtype=np.float64)
+            if flo.shape != (nwin, len(prns)):
+                raise GpsB200Error(ERR_ARG, "snapshot_batch: f_lo_prn of shape %s for %d windows of %d PRNs"
+                                   % (flo.shape, nwin, len(prns)))
+        acq = self._acq_config(prns, ms, 0, f_lo, step, nbins)
+        sc = np.array(snapshot_config() if cfg is None else cfg, dtype=SNAPSHOT_CONFIG_DTYPE).reshape(1)
+        shape = (max(1, nwin), max(1, min(len(prns), 32)))
+        res = np.zeros(shape, ACQ_RESULT_DTYPE)
+        out = np.zeros(shape, SNAPSHOT_DTYPE)
+        src, n, dev = self._rx_source(iq, device_ptr, nsamples, stream)
+        fn = lib().gpsb200_snapshot_batch_device if dev else lib().gpsb200_snapshot_batch
+        self._check(fn(self._h, src, n, int(sample_size), C.byref(acq), nwin, s.ctypes.data if nwin else None,
+                       None if flo is None else flo.ctypes.data, sc.ctypes.data, res.ctypes.data, out.ctypes.data,
+                       *dev))
+        return res, out
 
     @staticmethod
     def _snapshot_args(chans, meas, cfg, want_residuals):

@@ -20,6 +20,8 @@
 // each row's 3072 delays over kSplit CTAs (grid z): each slice builds the prefix sums its delays read and writes its
 // powers to device scratch, and k_acq_reduce applies the row's argmax, tie and P2 rules, with no atomics. The split
 // comes from nprn x nbins and the SM count (split_for), never from the caller; the results are the same bits either way.
+// A batch (DESIGN §11.6) splits only a pass of fewer rows than one full wave (batch_split): on 8 windows of the standard
+// grid split_for picks 3 slices, whose prefix sums cost twice a row's, and the pass ran 17 % slower than unsplit.
 #include <cmath>
 #include <cstring>
 #include <vector>
@@ -123,11 +125,12 @@ __device__ __forceinline__ void reduce_row(const uint64_t (&pw)[kTausPerThread],
 // kWindows: phase steps from a [nprn][nbins] table. kSplit > 1: CTA (j, p, z) computes slice z of row (p, j) and writes
 // its powers to grid (scratch of [nprn][nbins][3000], required); k_acq_reduce reduces the rows. The prefix sums start at
 // tau0 instead of 0: C takes differences of S only (its coefficients sum to zero), so C is the same integer.
+// The body of k_acq_grid and k_acq_batch, which differ only in where a CTA's samples start.
 template <typename T, bool kWindows, int kSplit>
-__global__ void __launch_bounds__(kThreads, 3)
-k_acq_grid(const T *__restrict__ iq, const int16_t *__restrict__ edges_all, const int32_t *__restrict__ nedges_all,
-           const int32_t *__restrict__ prns, const uint32_t *__restrict__ u_bins, int K, int nbins,
-           uint64_t *__restrict__ grid, uint64_t *__restrict__ rows) {
+__device__ __forceinline__ void grid_row(const T *__restrict__ iq, const int16_t *__restrict__ edges_all,
+                                         const int32_t *__restrict__ nedges_all, const int32_t *__restrict__ prns,
+                                         const uint32_t *__restrict__ u_bins, int K, int nbins,
+                                         uint64_t *__restrict__ grid, uint64_t *__restrict__ rows) {
     using Sh = Slice<kSplit>;
     constexpr int kPer = Sh::kPer, kR = Sh::kR;
     extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -232,6 +235,27 @@ k_acq_grid(const T *__restrict__ iq, const int16_t *__restrict__ edges_all, cons
     }
 }
 
+template <typename T, bool kWindows, int kSplit>
+__global__ void __launch_bounds__(kThreads, kCtasPerSm)
+k_acq_grid(const T *__restrict__ iq, const int16_t *__restrict__ edges_all, const int32_t *__restrict__ nedges_all,
+           const int32_t *__restrict__ prns, const uint32_t *__restrict__ u_bins, int K, int nbins,
+           uint64_t *__restrict__ grid, uint64_t *__restrict__ rows) {
+    grid_row<T, kWindows, kSplit>(iq, edges_all, nedges_all, prns, u_bins, K, nbins, grid, rows);
+}
+
+// A batch of windows (gpsb200_snapshot_batch; DESIGN §11.6): the per-PRN window search with row p = w nprn + q of grid
+// y the (window w, PRN q) pair. prns and u_bins hold one row per pair; window w's samples start win_off[w] samples
+// from iq.
+template <typename T, int kSplit>
+__global__ void __launch_bounds__(kThreads, kCtasPerSm)
+k_acq_batch(const T *__restrict__ iq, const int64_t *__restrict__ win_off, int nprn,
+            const int16_t *__restrict__ edges_all, const int32_t *__restrict__ nedges_all,
+            const int32_t *__restrict__ prns, const uint32_t *__restrict__ u_bins, int K, int nbins,
+            uint64_t *__restrict__ grid, uint64_t *__restrict__ rows) {
+    const T *w = iq + 2 * win_off[blockIdx.y / nprn];
+    grid_row<T, true, kSplit>(w, edges_all, nedges_all, prns, u_bins, K, nbins, grid, rows);
+}
+
 // The rows of a split search: one CTA per (bin, PRN) reduces the powers its slices wrote to grid, as k_acq_grid does.
 __global__ void __launch_bounds__(kThreads) k_acq_reduce(const uint64_t *__restrict__ grid, int nbins,
                                                          uint64_t *__restrict__ rows) {
@@ -295,6 +319,10 @@ template <typename T, bool kWin>
 const GridKernel kGrid[] = {(GridKernel) k_acq_grid<T, kWin, 1>, (GridKernel) k_acq_grid<T, kWin, 2>,
                                 (GridKernel) k_acq_grid<T, kWin, 3>, (GridKernel) k_acq_grid<T, kWin, 4>,
                                 (GridKernel) k_acq_grid<T, kWin, 6>};
+template <typename T>
+const GridKernel kBatch[] = {(GridKernel) k_acq_batch<T, 1>, (GridKernel) k_acq_batch<T, 2>,
+                             (GridKernel) k_acq_batch<T, 3>, (GridKernel) k_acq_batch<T, 4>,
+                             (GridKernel) k_acq_batch<T, 6>};
 constexpr int kSplits[] = {1, 2, 3, 4, 6};
 constexpr int kNumSplits = sizeof(kSplits) / sizeof(kSplits[0]);
 
@@ -303,6 +331,21 @@ GridKernel grid_kernel(int sample_size, bool windows, int split) {
     while (kSplits[i] != split) i++;
     if (sample_size == GPSB200_SC08) return windows ? kGrid<int8_t, true>[i] : kGrid<int8_t, false>[i];
     return windows ? kGrid<int16_t, true>[i] : kGrid<int16_t, false>[i];
+}
+
+GridKernel batch_kernel(int sample_size, int split) {
+    int i = 0;
+    while (kSplits[i] != split) i++;
+    return sample_size == GPSB200_SC08 ? kBatch<int8_t>[i] : kBatch<int16_t>[i];
+}
+
+// The phase steps of rows p < nrow from their first bins f_lo[p] (NULL: cfg->f_lo_hz for one row), [nrow][nbins].
+std::vector<uint32_t> phase_steps(const gpsb200_acq_config_t *cfg, int nrow, const double *f_lo) {
+    std::vector<uint32_t> u((size_t) nrow * cfg->nbins);
+    for (int p = 0; p < nrow; p++)
+        for (int j = 0; j < cfg->nbins; j++)
+            u[(size_t) p * cfg->nbins + j] = phase_step((f_lo ? f_lo[p] : cfg->f_lo_hz) + (double) j * cfg->step_hz);
+    return u;
 }
 
 }  // namespace
@@ -331,6 +374,12 @@ int split_for(int rows, int sms) {
 
 int split_of(const Scratch &sc, int nprn, int nbins) {
     return sc.force_split ? sc.force_split : split_for(nprn * nbins, sc.sms);
+}
+
+int batch_split(const Scratch &sc, int npair, int nbins) {
+    const int64_t rows = (int64_t) npair * nbins;
+    if (sc.force_split || rows < (int64_t) kCtasPerSm * sc.sms) return split_of(sc, npair, nbins);
+    return 1;
 }
 
 int64_t window_samples(const gpsb200_acq_config_t *cfg) { return (int64_t) kCode * cfg->ms + (kCode - 1); }
@@ -382,7 +431,7 @@ cudaError_t scratch_reserve(Scratch &sc, const gpsb200_acq_config_t *cfg, bool w
         CU_RET(cudaMalloc(&sc.d_flo, 32 * sizeof(double)));
         for (int i = 0; i < kNumSplits; i++)
             for (GridKernel k : {kGrid<int8_t, false>[i], kGrid<int16_t, false>[i], kGrid<int8_t, true>[i],
-                                 kGrid<int16_t, true>[i]})
+                                 kGrid<int16_t, true>[i], kBatch<int8_t>[i], kBatch<int16_t>[i]})
                 CU_RET(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, sizeof(Smem)));
         int dev = 0;
         CU_RET(cudaGetDevice(&dev));
@@ -395,7 +444,24 @@ cudaError_t scratch_reserve(Scratch &sc, const gpsb200_acq_config_t *cfg, bool w
     return cudaSuccess;
 }
 
+cudaError_t batch_reserve(Scratch &sc, const gpsb200_acq_config_t *cfg, int nwin) {
+    const size_t npair = (size_t) nwin * cfg->nprn;
+    CU_RET(scratch_reserve(sc, cfg, true, false));
+    CU_RET(grow(sc.d_rows, sc.rows_cap, npair * cfg->nbins * 3));
+    CU_RET(grow(sc.d_u, sc.u_cap, npair * cfg->nbins));
+    CU_RET(grow(sc.d_boff, sc.boff_cap, (size_t) nwin));
+    CU_RET(grow(sc.d_bprn, sc.bprn_cap, npair));
+    CU_RET(grow(sc.d_bflo, sc.bflo_cap, npair));
+    CU_RET(grow(sc.d_bres, sc.bres_cap, npair));
+    if (batch_split(sc, (int) npair, cfg->nbins) > 1) CU_RET(grow(sc.d_grid, sc.grid_cap, npair * cfg->nbins * kCode));
+    return cudaSuccess;
+}
+
 void scratch_free(Scratch &sc) {
+    cudaFree(sc.d_boff);
+    cudaFree(sc.d_bprn);
+    cudaFree(sc.d_bflo);
+    cudaFree(sc.d_bres);
     cudaFree(sc.d_edges);
     cudaFree(sc.d_nedges);
     cudaFree(sc.d_grid);
@@ -413,12 +479,7 @@ void scratch_free(Scratch &sc) {
 cudaError_t launch(Scratch &sc, const void *window, int sample_size, const gpsb200_acq_config_t *cfg,
                    const double *f_lo_prn, bool want_grid, cudaStream_t s) {
     // the small parameter arrays go up by value in the stream order (the host copies are on this call's stack)
-    const int nrow = f_lo_prn ? cfg->nprn : 1;
-    std::vector<uint32_t> u((size_t) nrow * cfg->nbins);
-    for (int p = 0; p < nrow; p++)
-        for (int j = 0; j < cfg->nbins; j++)
-            u[(size_t) p * cfg->nbins + j] =
-                phase_step((f_lo_prn ? f_lo_prn[p] : cfg->f_lo_hz) + (double) j * cfg->step_hz);
+    const std::vector<uint32_t> u = phase_steps(cfg, f_lo_prn ? cfg->nprn : 1, f_lo_prn);
     CU_RET(cudaMemcpyAsync(sc.d_u, u.data(), u.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, s));
     CU_RET(cudaMemcpyAsync(sc.d_prn, cfg->prn, cfg->nprn * sizeof(int32_t), cudaMemcpyHostToDevice, s));
     if (f_lo_prn) CU_RET(cudaMemcpyAsync(sc.d_flo, f_lo_prn, cfg->nprn * sizeof(double), cudaMemcpyHostToDevice, s));
@@ -439,6 +500,35 @@ cudaError_t launch(Scratch &sc, const void *window, int sample_size, const gpsb2
     CU_RET(cudaGetLastError());
     CU_RET(cudaMemcpyAsync(sc.h_res, sc.d_res, cfg->nprn * sizeof(gpsb200_acq_result_t), cudaMemcpyDeviceToHost, s));
     // pageable sources of the two uploads must outlive them: wait here (the search is blocking anyway)
+    return cudaStreamSynchronize(s);
+}
+
+cudaError_t launch_batch(Scratch &sc, const void *src, int sample_size, const gpsb200_acq_config_t *cfg, int nwin,
+                         const int64_t *win_off, const double *f_lo, gpsb200_acq_result_t *res, cudaStream_t s) {
+    const int npair = nwin * cfg->nprn;
+    std::vector<int32_t> prn((size_t) npair);
+    for (int i = 0; i < npair; i++) prn[i] = cfg->prn[i % cfg->nprn];
+    const std::vector<uint32_t> u = phase_steps(cfg, npair, f_lo);
+    CU_RET(cudaMemcpyAsync(sc.d_u, u.data(), u.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, s));
+    CU_RET(cudaMemcpyAsync(sc.d_bprn, prn.data(), prn.size() * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+    CU_RET(cudaMemcpyAsync(sc.d_bflo, f_lo, npair * sizeof(double), cudaMemcpyHostToDevice, s));
+    CU_RET(cudaMemcpyAsync(sc.d_boff, win_off, nwin * sizeof(int64_t), cudaMemcpyHostToDevice, s));
+    const int split = batch_split(sc, npair, cfg->nbins);
+    uint64_t *g = split > 1 ? sc.d_grid : nullptr;
+    const void *p = src;
+    int nprn = cfg->nprn;
+    void *args[] = {(void *) &p, (void *) &sc.d_boff, (void *) &nprn, (void *) &sc.d_edges, (void *) &sc.d_nedges,
+                    (void *) &sc.d_bprn, (void *) &sc.d_u, (void *) &cfg->ms, (void *) &cfg->nbins, (void *) &g,
+                    (void *) &sc.d_rows};
+    CU_RET(cudaLaunchKernel(batch_kernel(sample_size, split), dim3(cfg->nbins, npair, split), dim3(kThreads), args,
+                            sizeof(Smem), s));
+    if (split > 1) {
+        k_acq_reduce<<<dim3(cfg->nbins, npair), kThreads, 0, s>>>(sc.d_grid, cfg->nbins, sc.d_rows);
+        CU_RET(cudaGetLastError());
+    }
+    k_acq_pick<<<npair, 32, 0, s>>>(sc.d_rows, sc.d_bprn, cfg->nbins, cfg->f_lo_hz, sc.d_bflo, cfg->step_hz, sc.d_bres);
+    CU_RET(cudaGetLastError());
+    CU_RET(cudaMemcpyAsync(res, sc.d_bres, npair * sizeof(gpsb200_acq_result_t), cudaMemcpyDeviceToHost, s));
     return cudaStreamSynchronize(s);
 }
 

@@ -13,6 +13,7 @@ namespace acq {
 
 constexpr int kCode = 3000;                    // samples per C/A period at 3 Msps
 constexpr int kThreads = 256;                  // threads of k_acq_grid
+constexpr int kCtasPerSm = 3;                  // its launch bound: CTAs per SM
 constexpr int kTausPerThread = 12;             // delays per thread: 256 x 12 = 3072 >= 3000 (the last 72 are discarded)
 constexpr int kTaus = kThreads * kTausPerThread;
 constexpr int kPrefix = 6144;                  // prefix sums S[0..6144] of one window (needs 3072 + 3000 - 1 <= 6143)
@@ -32,6 +33,14 @@ struct Scratch {
     size_t u_cap = 0;
     int32_t *d_prn = nullptr;          // [32]
     double *d_flo = nullptr;           // [32] first bin of each PRN's window (gpsb200_acquire_windows)
+    int64_t *d_boff = nullptr;         // batches (gpsb200_snapshot_batch): [nwin] window offsets in samples,
+    size_t boff_cap = 0;
+    int32_t *d_bprn = nullptr;         // [nwin][nprn] PRN,
+    size_t bprn_cap = 0;
+    double *d_bflo = nullptr;          // [nwin][nprn] first bin
+    size_t bflo_cap = 0;
+    gpsb200_acq_result_t *d_bres = nullptr;   // and [nwin][nprn] results of every (window, PRN) pair
+    size_t bres_cap = 0;
     int sms = 0;                       // SM count of the device (the split rule)
     int force_split = 0;               // 0: the split rule; else the split of every search (a test hook)
 };
@@ -47,17 +56,28 @@ std::string check(const gpsb200_acq_config_t *cfg, int64_t nsamples, int sample_
 int split_for(int rows, int sms);
 int split_of(const Scratch &sc, int nprn, int nbins);
 bool split_allowed(int split);
+// The split of a batch pass of npair (window, PRN) pairs: split_of while its rows npair x nbins are fewer than a full
+// wave (kCtasPerSm CTAs on every SM) or a split is forced, else 1: a split only pays while SMs would idle.
+int batch_split(const Scratch &sc, int npair, int nbins);
 // Samples the search reads from s0 on: 3000 K + 2999.
 int64_t window_samples(const gpsb200_acq_config_t *cfg);
 // Phase step of bin j: (uint32) llround(f_j * 2^32 / 3e6).
 uint32_t phase_step(double f_hz);
 
 cudaError_t scratch_reserve(Scratch &sc, const gpsb200_acq_config_t *cfg, bool windows, bool want_grid);
+// Scratch of a batch pass of nwin windows (launch_batch).
+cudaError_t batch_reserve(Scratch &sc, const gpsb200_acq_config_t *cfg, int nwin);
 void scratch_free(Scratch &sc);
 // Enqueue the search of the samples at `window` (the first sample is s0) on s; results land in sc.h_res after a
 // synchronize of s, the grid (want_grid) in sc.d_grid. f_lo_prn (NULL: cfg->f_lo_hz for every PRN): per-PRN windows.
 cudaError_t launch(Scratch &sc, const void *window, int sample_size, const gpsb200_acq_config_t *cfg,
                    const double *f_lo_prn, bool want_grid, cudaStream_t s);
+
+// Enqueue the per-PRN window search of nwin windows on s and wait for it: window w starts win_off[w] samples from src,
+// pair (w, q) searches PRN cfg->prn[q] from first bin f_lo[w nprn + q]; res [nwin][nprn] (host) as gpsb200_acquire_windows
+// run on each window gives it (with f_lo[..] = cfg->f_lo_hz, as gpsb200_acquire gives it). nwin nprn <= 65535.
+cudaError_t launch_batch(Scratch &sc, const void *src, int sample_size, const gpsb200_acq_config_t *cfg, int nwin,
+                         const int64_t *win_off, const double *f_lo, gpsb200_acq_result_t *res, cudaStream_t s);
 
 }  // namespace acq
 }  // namespace gpsb200

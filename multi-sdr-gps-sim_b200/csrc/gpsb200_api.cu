@@ -1166,6 +1166,66 @@ int snapshot_measure(gpsb200_ctx *ctx, const void *iq, int64_t nsamples, int sam
     return GPSB200_OK;
 }
 
+// The snapshot batch of both entry points (acquire.cu, snapshot.cu; DESIGN §11.6). Every argument of every window is
+// checked before anything is enqueued. The windows then run in passes of snap::batch_pass: the search of the pass, one
+// download of its results, the measurement's checks and seed on the host (snap::seed), one upload and the measurement.
+// A host source goes up one window after another, packed; a device source is read in place.
+int snapshot_batch(gpsb200_ctx *ctx, const void *iq, int64_t nsamples, int sample_size, const gpsb200_acq_config_t *acq,
+                   int nwin, const int64_t *s0, const double *f_lo, const gpsb200_snapshot_config_t *cfg,
+                   gpsb200_acq_result_t *res, gpsb200_snapshot_t *out, bool device, cudaStream_t s) {
+    const char *name = device ? "gpsb200_snapshot_batch_device" : "gpsb200_snapshot_batch";
+    const std::string at = std::string(name) + ": ";
+    if (!iq || !acq || !s0 || !cfg || !res || !out)
+        return fail(ctx, GPSB200_ERR_ARG, at + "NULL source, search config, s0, snapshot config, results or output");
+    if (nwin < 1) return fail(ctx, GPSB200_ERR_ARG, at + "nwin must be >= 1");
+    std::string bad = snap::check_config(cfg);
+    if (!bad.empty()) return fail(ctx, GPSB200_ERR_ARG, at + bad);
+    gpsb200_acq_config_t one = *acq;
+    for (int w = 0; w < nwin; w++) {
+        one.s0 = s0[w];
+        bad = acq::check(&one, nsamples, sample_size, f_lo != nullptr, f_lo ? f_lo + (size_t) w * acq->nprn : nullptr);
+        if (!bad.empty()) return fail(ctx, GPSB200_ERR_ARG, at + "window " + std::to_string(w) + ": " + bad);
+    }
+    int rc = device ? check_aligned(ctx, iq, name, "iq_device") : GPSB200_OK;
+    if (!rc) rc = check_entry(ctx);
+    if (rc) return rc;
+    if (!ctx->d_rx_chips) CU(trk::chips_upload(&ctx->d_rx_chips));
+    const int nprn = acq->nprn, per = snap::batch_pass(acq, sample_size, nwin);
+    const int64_t span = acq::window_samples(acq);
+    const size_t elem = sample_size == GPSB200_SC16 ? 4 : 2;
+    std::vector<int64_t> off((size_t) per);
+    std::vector<double> flo(f_lo ? 0 : (size_t) per * nprn, acq->f_lo_hz);   // the standard grid: f_lo_hz every row
+    for (int w0 = 0; w0 < nwin; w0 += per) {
+        const int n = std::min(per, nwin - w0);
+        CU(acq::batch_reserve(ctx->acq, acq, n));
+        const void *src = iq;
+        if (device) {
+            for (int i = 0; i < n; i++) off[i] = s0[w0 + i];
+        } else {
+            CU(grow(ctx->d_rx, ctx->rx_bytes, (size_t) n * span * elem));
+            for (int i = 0; i < n; i++) {
+                off[i] = (int64_t) i * span;
+                CU(cudaMemcpyAsync(ctx->d_rx + (size_t) off[i] * elem, static_cast<const char *>(iq) + s0[w0 + i] * elem,
+                                   (size_t) span * elem, cudaMemcpyHostToDevice, s));
+            }
+            src = ctx->d_rx;
+        }
+        gpsb200_acq_result_t *r = res + (size_t) w0 * nprn;
+        gpsb200_snapshot_t *o = out + (size_t) w0 * nprn;
+        CU(acq::launch_batch(ctx->acq, src, sample_size, acq, n, off.data(),
+                             f_lo ? f_lo + (size_t) w0 * nprn : flo.data(), r, s));
+        for (int i = 0; i < n; i++) {
+            one.s0 = s0[w0 + i];
+            bad = snap::check(&one, nsamples, sample_size, r + (size_t) i * nprn, cfg);
+            if (!bad.empty()) return fail(ctx, GPSB200_ERR_ARG, at + "window " + std::to_string(w0 + i) + ": " + bad);
+            snap::seed(&one, r + (size_t) i * nprn, cfg, o + (size_t) i * nprn);
+        }
+        CU(snap::launch_batch(ctx->snap, src, sample_size, acq->ms, n, nprn, ctx->acq.d_boff, ctx->d_rx_chips,
+                              cfg->iterations, o, s));
+    }
+    return GPSB200_OK;
+}
+
 // Position fixes (pvt.cu), with the stage st names (none: plain fixes). Everything is checked before anything is
 // enqueued.
 int pvt_fix(gpsb200_ctx *ctx, const char *fn, const gpsb200_pvt_chan_t *chans, int nchan,
@@ -1859,6 +1919,24 @@ int gpsb200_snapshot_measure_device(gpsb200_ctx_t *ctx, const void *iq_device, i
     if (!ctx) return GPSB200_ERR_ARG;
     cudaStream_t s = caller_stream(ctx, stream_);
     return settle(ctx, s, snapshot_measure(ctx, iq_device, nsamples, sample_size, acq, res, cfg, out, true, s));
+}
+
+int gpsb200_snapshot_batch(gpsb200_ctx_t *ctx, const void *iq, int64_t nsamples, int sample_size,
+                           const gpsb200_acq_config_t *acq, int nwin, const int64_t *s0, const double *f_lo,
+                           const gpsb200_snapshot_config_t *cfg, gpsb200_acq_result_t *res, gpsb200_snapshot_t *out) {
+    if (!ctx) return GPSB200_ERR_ARG;
+    return settle(ctx, nullptr, snapshot_batch(ctx, iq, nsamples, sample_size, acq, nwin, s0, f_lo, cfg, res, out, false,
+                                               ctx->s_compute));
+}
+
+int gpsb200_snapshot_batch_device(gpsb200_ctx_t *ctx, const void *iq_device, int64_t nsamples, int sample_size,
+                                  const gpsb200_acq_config_t *acq, int nwin, const int64_t *s0, const double *f_lo,
+                                  const gpsb200_snapshot_config_t *cfg, gpsb200_acq_result_t *res,
+                                  gpsb200_snapshot_t *out, void *stream_) {
+    if (!ctx) return GPSB200_ERR_ARG;
+    cudaStream_t s = caller_stream(ctx, stream_);
+    return settle(ctx, s, snapshot_batch(ctx, iq_device, nsamples, sample_size, acq, nwin, s0, f_lo, cfg, res, out, true,
+                                         s));
 }
 
 int gpsb200_pvt_snapshot(gpsb200_ctx_t *ctx, const gpsb200_pvt_chan_t *chans, int nchan, const gpsb200_snapshot_t *meas,

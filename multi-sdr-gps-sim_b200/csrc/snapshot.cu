@@ -6,8 +6,9 @@
 // warps by one thread per chunk. Warp 0 reduces the chunks' int64 powers and thread 0 runs the header's update. Every
 // sum is an exact integer sum, so its value does not depend on the order; there are no atomics. Pass 0 is the frequency
 // pass (prompt only, at the seed), then one code pass per iteration.
-#include <cstring>
+#include <algorithm>
 #include <cmath>
+#include <cstring>
 
 #include "acquire.h"
 #include "device_buffer.h"
@@ -72,10 +73,10 @@ __device__ __forceinline__ void correlate(Smem &sm, const T *__restrict__ iq, in
     }
 }
 
+// The body of k_snapshot and k_snapshot_batch, which differ only in where a CTA's samples start: record blockIdx.x.
 template <typename T>
-__global__ void __launch_bounds__(kThreads) k_snapshot(const T *__restrict__ iq, int K, const int8_t *__restrict__ chips,
-                                                       int iterations, gpsb200_snapshot_t *__restrict__ recs) {
-    __shared__ Smem sm;
+__device__ __forceinline__ void measure(Smem &sm, const T *__restrict__ iq, int K, const int8_t *__restrict__ chips,
+                                        int iterations, gpsb200_snapshot_t *__restrict__ recs) {
     const int tid = threadIdx.x, lane = tid & 31;
     rx::fill_carrier_table(sm.tab, kThreads);
     if (tid == 0) sm.rec = recs[blockIdx.x];
@@ -158,7 +159,31 @@ __global__ void __launch_bounds__(kThreads) k_snapshot(const T *__restrict__ iq,
     }
 }
 
+template <typename T>
+__global__ void __launch_bounds__(kThreads) k_snapshot(const T *__restrict__ iq, int K, const int8_t *__restrict__ chips,
+                                                       int iterations, gpsb200_snapshot_t *__restrict__ recs) {
+    __shared__ Smem sm;
+    measure<T>(sm, iq, K, chips, iterations, recs);
+}
+
+// A batch of windows (gpsb200_snapshot_batch; DESIGN §11.6): record blockIdx.x = w nprn + q, window w's samples start
+// win_off[w] samples from iq.
+template <typename T>
+__global__ void __launch_bounds__(kThreads)
+k_snapshot_batch(const T *__restrict__ iq, const int64_t *__restrict__ win_off, int nprn, int K,
+                 const int8_t *__restrict__ chips, int iterations, gpsb200_snapshot_t *__restrict__ recs) {
+    __shared__ Smem sm;
+    measure<T>(sm, iq + 2 * win_off[blockIdx.x / nprn], K, chips, iterations, recs);
+}
+
 }  // namespace
+
+std::string check_config(const gpsb200_snapshot_config_t *cfg) {
+    if (!(cfg->min_ratio >= 0.0) || !std::isfinite(cfg->min_ratio)) return "min_ratio must be finite and >= 0";
+    if (cfg->iterations < 0 || cfg->iterations > GPSB200_SNAP_MAX_ITER) return "iterations must be 0..16";
+    if (cfg->reserved != 0) return "snapshot config reserved must be 0";
+    return std::string();
+}
 
 std::string check(const gpsb200_acq_config_t *acq, int64_t nsamples, int sample_size, const gpsb200_acq_result_t *res,
                   const gpsb200_snapshot_config_t *cfg) {
@@ -171,9 +196,8 @@ std::string check(const gpsb200_acq_config_t *acq, int64_t nsamples, int sample_
     one.nbins = 1;
     const std::string bad = acq::check(&one, nsamples, sample_size);
     if (!bad.empty()) return bad;
-    if (!(cfg->min_ratio >= 0.0) || !std::isfinite(cfg->min_ratio)) return "min_ratio must be finite and >= 0";
-    if (cfg->iterations < 0 || cfg->iterations > GPSB200_SNAP_MAX_ITER) return "iterations must be 0..16";
-    if (cfg->reserved != 0) return "snapshot config reserved must be 0";
+    const std::string bad_cfg = check_config(cfg);
+    if (!bad_cfg.empty()) return bad_cfg;
     for (int p = 0; p < acq->nprn; p++) {
         const gpsb200_acq_result_t &r = res[p];
         const std::string at = "result " + std::to_string(p) + ": ";
@@ -199,8 +223,24 @@ void seed(const gpsb200_acq_config_t *acq, const gpsb200_acq_result_t *res, cons
     }
 }
 
+int64_t batch_window_bytes(const gpsb200_acq_config_t *acq, int sample_size) {
+    const int64_t rows = (int64_t) acq->nprn * acq->nbins;
+    // a pair's PRN, first bin, result and record: 4 + 8 + 56 + 56 = 124 bytes, rounded up as the header states it
+    const int64_t pair = 128;
+    static_assert(sizeof(int32_t) + sizeof(double) + sizeof(gpsb200_acq_result_t) + sizeof(gpsb200_snapshot_t) <= 128,
+                  "a pair's scratch");
+    return rows * ((int64_t) acq::kCode * 8 + 3 * 8 + 4) + acq->nprn * pair + 8 +
+           acq::window_samples(acq) * (sample_size == GPSB200_SC16 ? 4 : 2);
+}
+
+int batch_pass(const gpsb200_acq_config_t *acq, int sample_size, int nwin) {
+    const int64_t w = GPSB200_SNAP_BATCH_SCRATCH / batch_window_bytes(acq, sample_size);
+    return (int) std::max<int64_t>(1, std::min<int64_t>(w, nwin));
+}
+
 void scratch_free(Scratch &sc) {
     cudaFree(sc.d_rec);
+    cudaFree(sc.d_brec);
     sc = Scratch();
 }
 
@@ -215,6 +255,23 @@ cudaError_t launch(Scratch &sc, const void *window, int sample_size, int K, int 
                                                       sc.d_rec);
     CU_RET(cudaGetLastError());
     CU_RET(cudaMemcpyAsync(rec, sc.d_rec, nprn * sizeof(gpsb200_snapshot_t), cudaMemcpyDeviceToHost, s));
+    return cudaStreamSynchronize(s);
+}
+
+cudaError_t launch_batch(Scratch &sc, const void *src, int sample_size, int K, int nwin, int nprn,
+                         const int64_t *d_win_off, const int8_t *chips, int iterations, gpsb200_snapshot_t *rec,
+                         cudaStream_t s) {
+    const int n = nwin * nprn;
+    CU_RET(grow(sc.d_brec, sc.brec_cap, (size_t) n));
+    CU_RET(cudaMemcpyAsync(sc.d_brec, rec, n * sizeof(gpsb200_snapshot_t), cudaMemcpyHostToDevice, s));
+    if (sample_size == GPSB200_SC08)
+        k_snapshot_batch<int8_t><<<n, kThreads, 0, s>>>(static_cast<const int8_t *>(src), d_win_off, nprn, K, chips,
+                                                        iterations, sc.d_brec);
+    else
+        k_snapshot_batch<int16_t><<<n, kThreads, 0, s>>>(static_cast<const int16_t *>(src), d_win_off, nprn, K, chips,
+                                                         iterations, sc.d_brec);
+    CU_RET(cudaGetLastError());
+    CU_RET(cudaMemcpyAsync(rec, sc.d_brec, n * sizeof(gpsb200_snapshot_t), cudaMemcpyDeviceToHost, s));
     return cudaStreamSynchronize(s);
 }
 

@@ -16,7 +16,12 @@
 // the PRNs at or above the threshold, and gpsb200_pvt_snapshot (gpsb200_pvt_snapshot_search over the default global
 // grid with search) fixes from them, with the ephemeris valid at the assist time. One line per snapshot: sample,
 // status, position, clock, velocity, channels used, PDOP and delta (the solved a-priori time error), plus support with
-// search. No tracking, no navigation message: each fix comes from its K ms window alone.
+// search. No tracking, no navigation message: each fix comes from its K ms window alone. The windows are read, searched
+// and measured up to 100 at a time (gpsb200_snapshot_batch, DESIGN §11.6); the fixes stay one call per window. With
+// --almanac and an a-priori position the windows are warm started: each window's sky is predicted at its own time (the
+// assist time plus its offset from the first window), every window of a chunk searches the PRNs predicted at or above
+// the mask in any of them, each over the warm start's bins around that window's own prediction.
+#include <algorithm>
 #include <cmath>
 #include <cstdio>
 #include <cstdlib>
@@ -42,7 +47,8 @@ static void usage() {
             "            [--almanac FILE.sem --assist-pos LAT,LON,H --assist-time YYYY/MM/DD,hh:mm:ss[.s]\n"
             "             [--window HZ] [--mask DEG]]\n"
             "            [--fix --assist NAV_FILE[,3] --assist-pos LAT,LON,H|search --assist-time YYYY/MM/DD,hh:mm:ss[.s]\n"
-            "             [--every MS] [--count N] [--iono a0,a1,a2,a3,b0,b1,b2,b3]]\n"
+            "             [--every MS] [--count N] [--iono a0,a1,a2,a3,b0,b1,b2,b3]\n"
+            "             [--almanac FILE.sem [--window HZ] [--mask DEG]]]\n"
             "  FILE              interleaved I,Q at 3 Msps, int8 (default) or int16 (--iq16)\n"
             "  --block B         start at 0.1 s block B (sample 300000 B); --offset-ms N adds N ms (3000 N samples)\n"
             "  --ms K            coherent 1 ms periods summed, 1..100 (default 10)\n"
@@ -57,15 +63,53 @@ static void usage() {
             "                    then a coarse-time fix from --assist-pos, or a search over a global grid with 'search';\n"
             "                    ephemeris from the RINEX file of --assist (,3: RINEX 3) at --assist-time, the GPS time\n"
             "                    of the first window's first sample; one window every --every ms (default 100), --count\n"
-            "                    windows (default 1); --iono: the Klobuchar alpha / beta to apply\n",
+            "                    windows (default 1); --iono: the Klobuchar alpha / beta to apply; --almanac (with\n"
+            "                    LAT,LON,H only): warm start every window from its own predicted sky\n",
             kDefaultThreshold, kDefaultWindow, kDefaultMask);
     exit(2);
 }
 
-// --fix: count windows every every_ms from sample s0, each searched on the standard grid, measured and fixed alone.
+// --fix: windows of a chunk go up packed and are searched and measured in one gpsb200_snapshot_batch call, at most
+// kChunk at a time; each is then fixed alone. A batch call ends at a window whose Doppler result lies beyond the
+// measurement's +-10 kHz before its pass is measured, where the single calls end at that window: with bins beyond
+// +-10 kHz the windows go one per call, so that the lines printed before such a failure stay those of the single calls.
+static const int kChunk = 100;
+
+// The PRNs of the chunk's warm start: of the list, those predicted at or above the mask in any window of the chunk (the
+// window at sample s[w] predicted at assist time sow + (s[w] - s0) / 3 MHz), each window with its own first bins f_lo
+// [n][nprn] on the standard grid. false when the almanac cannot be predicted.
+static bool warm_chunk(const gpsb200_almanac_record_t *alm, int32_t week, double sow, const double *x_a, long long s0,
+                       const std::vector<long long> &s, double step, double window, double mask,
+                       gpsb200_acq_config_t &cfg, std::vector<double> &f_lo) {
+    const int n = (int) s.size(), h = (int) std::ceil(window / step - 1e-9);
+    std::vector<gpsb200_sky_t> sky((size_t) n * 32);
+    for (int w = 0; w < n; w++)
+        if (gpsb200_almanac_predict(alm, week, sow + (double) (s[w] - s0) / 3e6, x_a, &sky[(size_t) w * 32]) != GPSB200_OK)
+            return false;
+    int np = 0;
+    for (int i = 0; i < cfg.nprn; i++) {
+        bool up = false;
+        for (int w = 0; w < n; w++) {
+            const gpsb200_sky_t &k = sky[(size_t) w * 32 + cfg.prn[i] - 1];
+            up = up || (k.valid && k.el_deg >= mask);
+        }
+        if (up) cfg.prn[np++] = cfg.prn[i];
+    }
+    cfg.nprn = np;
+    cfg.nbins = 2 * h + 1;
+    f_lo.resize((size_t) n * np);
+    for (int w = 0; w < n; w++)
+        for (int q = 0; q < np; q++)
+            f_lo[(size_t) w * np + q] = step * std::round(sky[(size_t) w * 32 + cfg.prn[q] - 1].doppler_hz / step) - h * step;
+    return true;
+}
+
+// --fix: count windows every every_ms from sample s0, each searched on the standard grid (or, with an almanac, warm
+// started), measured and fixed alone.
 static int snapshot_fixes(const char *path, int ss, int device, long long s0, gpsb200_acq_config_t cfg, double lo,
                           double hi, double step, double threshold, const char *nav, int nav_v3, const double *x_a,
-                          int32_t week, double sow, long long every_ms, long long count, gpsb200_pvt_config_t pcfg) {
+                          int32_t week, double sow, long long every_ms, long long count, gpsb200_pvt_config_t pcfg,
+                          const gpsb200_almanac_record_t *alm, const char *almanac, double window, double mask) {
     cfg.f_lo_hz = lo;
     cfg.step_hz = step;
     cfg.nbins = (int) std::floor((hi - lo) / step + 1e-9) + 1;
@@ -109,49 +153,87 @@ static int snapshot_fixes(const char *path, int ss, int device, long long s0, gp
     printf("# %s: snapshot fixes, %lld window(s) of %d ms every %lld ms from sample %lld, %s, Klobuchar %s\n", path,
            count, cfg.ms, every_ms, s0, x_a ? "coarse-time fix from the a-priori position" : "search over a global grid",
            pcfg.iono ? "on" : "off");
+    if (alm)
+        printf("# warm start from %s: the PRNs predicted at or above %.1f deg in a chunk's windows, %d bins of %.1f Hz "
+               "around each window's prediction\n", almanac, mask, 2 * (int) std::ceil(window / step - 1e-9) + 1, step);
     printf("# sample  status  lat_deg  lon_deg  height_m  clock_m  vx  vy  vz (ECEF m/s)  channels  pdop  delta_s%s\n",
            x_a ? "" : "  support");
     static const char *const kStatus[] = {"OK", "FEW", "NO_CONVERGENCE", "AMBIGUOUS"};
     int rc = GPSB200_OK;
-    std::vector<char> buf;
-    for (long long i = 0; i < count && rc == GPSB200_OK; i++) {
-        const long long s = s0 + i * every_ms * GPSB200_ACQ_CODE_SAMPLES;
-        if (s + need > have || !read_at(f, s, need, elem, buf)) break;
-        cfg.s0 = 0;
-        std::vector<gpsb200_acq_result_t> res(cfg.nprn);
-        std::vector<gpsb200_snapshot_t> meas(cfg.nprn);
-        rc = gpsb200_acquire(ctx, buf.data(), need, ss, &cfg, res.data(), nullptr);
-        if (rc == GPSB200_OK) rc = gpsb200_snapshot_measure(ctx, buf.data(), need, ss, &cfg, res.data(), &scfg, meas.data());
-        if (rc != GPSB200_OK) break;
-        // the channels: the measured PRNs with an ephemeris valid at the assist time
-        std::vector<gpsb200_pvt_chan_t> chans;
-        std::vector<gpsb200_snapshot_t> row;
-        for (auto &m : meas) {
-            if (m.status != GPSB200_SNAP_OK || !eph[m.prn - 1].valid) continue;
-            gpsb200_pvt_chan_t pc;
-            memset(&pc, 0, sizeof pc);
-            pc.eph = eph[m.prn - 1];
-            pc.prn = m.prn;
-            chans.push_back(pc);
-            m.sample = s;
-            row.push_back(m);
+    std::vector<char> buf, one;
+    bool inside = true;   // every window so far inside the file
+    for (long long i = 0; i < count && inside && rc == GPSB200_OK;) {
+        // the chunk: up to kChunk windows, packed, up to the first one not inside the file
+        std::vector<long long> s;
+        buf.clear();
+        for (; i < count && (int) s.size() < kChunk; i++) {
+            const long long si = s0 + i * every_ms * GPSB200_ACQ_CODE_SAMPLES;
+            if (si + need > have || !read_at(f, si, need, elem, one)) {
+                inside = false;
+                break;
+            }
+            buf.insert(buf.end(), one.begin(), one.end());
+            s.push_back(si);
         }
-        gpsb200_fix_t fx;
-        gpsb200_coarse_t co;
-        gpsb200_search_t sr;
-        if (chans.empty()) {
-            printf("%lld  FEW\n", s);
-            continue;
+        const int n = (int) s.size();
+        gpsb200_acq_config_t c = cfg;
+        std::vector<double> f_lo;   // empty: the standard grid
+        if (alm && !warm_chunk(alm, week, sow, x_a, s0, s, step, window, mask, c, f_lo)) {
+            fprintf(stderr, "gpsb200-acq: cannot predict the almanac of %s\n", almanac);
+            fclose(f);
+            gpsb200_destroy(ctx);
+            return 1;
         }
-        rc = x_a ? gpsb200_pvt_snapshot(ctx, chans.data(), (int) chans.size(), row.data(), &pcfg, &ap, &fx, nullptr, &co,
-                                        nullptr)
-                 : gpsb200_pvt_snapshot_search(ctx, chans.data(), (int) chans.size(), row.data(), &pcfg, &sc, &fx, nullptr,
-                                               &sr, nullptr, nullptr);
-        if (rc != GPSB200_OK) break;
-        printf("%lld  %s  %.8f  %.8f  %.3f  %.3f  %.3f  %.3f  %.3f  %d  %.2f  %.9f", s, kStatus[fx.status], fx.lat_deg,
-               fx.lon_deg, fx.height, fx.clock_m, fx.vx, fx.vy, fx.vz, fx.nused, fx.pdop, x_a ? co.delta : sr.delta);
-        if (!x_a) printf("  %d", sr.support);
-        printf("\n");
+        std::vector<int64_t> off(n);
+        for (int w = 0; w < n; w++) off[w] = (int64_t) w * need;
+        bool doppler_inside = true;   // every bin within the measurement's +-10 kHz
+        for (size_t r = 0; r < (f_lo.empty() ? 1 : f_lo.size()); r++) {
+            const double b0 = f_lo.empty() ? c.f_lo_hz : f_lo[r], b1 = b0 + (c.nbins - 1) * c.step_hz;
+            doppler_inside = doppler_inside && std::fabs(b0) <= 10000.0 && std::fabs(b1) <= 10000.0;
+        }
+        const int per = doppler_inside ? std::max(n, 1) : 1, np = c.nprn;
+        std::vector<gpsb200_acq_result_t> res((size_t) n * np);
+        std::vector<gpsb200_snapshot_t> meas((size_t) n * np);
+        for (int w0 = 0; w0 < n && rc == GPSB200_OK; w0 += per) {
+            const int m = std::min(per, n - w0);
+            if (np > 0)
+                rc = gpsb200_snapshot_batch(ctx, buf.data(), (int64_t) n * need, ss, &c, m, off.data() + w0,
+                                            f_lo.empty() ? nullptr : f_lo.data() + (size_t) w0 * np, &scfg,
+                                            res.data() + (size_t) w0 * np, meas.data() + (size_t) w0 * np);
+            for (int w = w0; w < w0 + m && rc == GPSB200_OK; w++) {
+                // the channels: the measured PRNs with an ephemeris valid at the assist time
+                std::vector<gpsb200_pvt_chan_t> chans;
+                std::vector<gpsb200_snapshot_t> row;
+                for (int q = 0; q < np; q++) {
+                    gpsb200_snapshot_t mq = meas[(size_t) w * np + q];
+                    if (mq.status != GPSB200_SNAP_OK || !eph[mq.prn - 1].valid) continue;
+                    gpsb200_pvt_chan_t pc;
+                    memset(&pc, 0, sizeof pc);
+                    pc.eph = eph[mq.prn - 1];
+                    pc.prn = mq.prn;
+                    chans.push_back(pc);
+                    mq.sample = s[w];
+                    row.push_back(mq);
+                }
+                gpsb200_fix_t fx;
+                gpsb200_coarse_t co;
+                gpsb200_search_t sr;
+                if (chans.empty()) {
+                    printf("%lld  FEW\n", s[w]);
+                    continue;
+                }
+                rc = x_a ? gpsb200_pvt_snapshot(ctx, chans.data(), (int) chans.size(), row.data(), &pcfg, &ap, &fx,
+                                                nullptr, &co, nullptr)
+                         : gpsb200_pvt_snapshot_search(ctx, chans.data(), (int) chans.size(), row.data(), &pcfg, &sc,
+                                                       &fx, nullptr, &sr, nullptr, nullptr);
+                if (rc != GPSB200_OK) break;
+                printf("%lld  %s  %.8f  %.8f  %.3f  %.3f  %.3f  %.3f  %.3f  %d  %.2f  %.9f", s[w], kStatus[fx.status],
+                       fx.lat_deg, fx.lon_deg, fx.height, fx.clock_m, fx.vx, fx.vy, fx.vz, fx.nused, fx.pdop,
+                       x_a ? co.delta : sr.delta);
+                if (!x_a) printf("  %d", sr.support);
+                printf("\n");
+            }
+        }
     }
     fclose(f);
     if (rc != GPSB200_OK) fprintf(stderr, "gpsb200-acq: %s\n", gpsb200_last_error(ctx));
@@ -229,13 +311,21 @@ int main(int argc, char **argv) {
         else if (a[0] != '-' && !path) path = argv[i];
         else usage();
     }
-    if (!path || block < 0 || offset_ms < 0 || (almanac && (!have_pos || !have_time || pos_search || fix)) ||
+    if (!path || block < 0 || offset_ms < 0 || (almanac && (!have_pos || !have_time || pos_search)) ||
         (!almanac && !fix && (have_pos || have_time)) || (fix && (assist.empty() || !have_pos || !have_time)) ||
         (!fix && (!assist.empty() || pcfg.iono)) || every_ms < 1 || count < 1)
         usage();
-    if (fix) return snapshot_fixes(path, ss, device, block * GPSB200_BLOCK_SAMPLES + offset_ms * GPSB200_ACQ_CODE_SAMPLES,
-                                   cfg, lo, hi, step, threshold, assist.c_str(), assist_v3, pos_search ? nullptr : x_a,
-                                   week, sow, every_ms, count, pcfg);
+    if (fix) {
+        gpsb200_almanac_record_t rec[32];
+        int32_t valid = 0;
+        if (almanac && gpsb200_almanac_read(almanac, rec, &valid) != GPSB200_OK) {
+            fprintf(stderr, "gpsb200-acq: cannot read the almanac of %s\n", almanac);
+            return 1;
+        }
+        return snapshot_fixes(path, ss, device, block * GPSB200_BLOCK_SAMPLES + offset_ms * GPSB200_ACQ_CODE_SAMPLES, cfg,
+                              lo, hi, step, threshold, assist.c_str(), assist_v3, pos_search ? nullptr : x_a, week, sow,
+                              every_ms, count, pcfg, almanac ? rec : nullptr, almanac, window, mask);
+    }
     cfg.f_lo_hz = lo;
     cfg.step_hz = step;
     cfg.nbins = (int) std::floor((hi - lo) / step + 1e-9) + 1;
