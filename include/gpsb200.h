@@ -1017,6 +1017,99 @@ int gpsb200_pvt_snapshot_search(gpsb200_ctx_t *ctx, const gpsb200_pvt_chan_t *ch
                                 const gpsb200_search_config_t *search, gpsb200_fix_t *fixes, double *residuals,
                                 gpsb200_search_t *out, int64_t *ms, double *node_rms);
 
+/* ---- collective detection: a position from satellites too weak to acquire alone (DESIGN §11.7;
+ * tests/collective_model.py states it in numpy). Axelrad et al., "Collective Detection and Direct Positioning Using
+ * Multiple GNSS Satellites", NAVIGATION 58(4), 2011. Each PRN's whole power grid P_p(j, tau) of one search is scored
+ * against a lattice of candidate receiver positions and time offsets around the a-priori ones: a candidate predicts
+ * every satellite's code delay and Doppler bin, and the grids' powers at those cells are added up for every common
+ * receiver clock shift. The best candidate seeds the PRNs; gpsb200_snapshot_measure and gpsb200_pvt_snapshot finish.
+ * Arguments: the search (acq, f_lo_prn: NULL for gpsb200_acquire's standard grid, else gpsb200_acquire_windows'
+ * per-PRN first bins), eph[32] indexed by PRN - 1 (as gpsb200_rinex_ephemeris returns it), the a-priori config ap
+ * (gpsb200_pvt_coarse's) and the lattice config cfg. s0 = acq->s0; "/" on integers floors.
+ *   1. Search: gpsb200_acquire (gpsb200_acquire_windows) on the window, unchanged; res [nprn] is its results, bit for bit.
+ *   2. Used: searched PRN p (acq->prn[p]) is used when eph[prn - 1] is valid with health 0, |t0 - toe| <= 7200 s
+ *      (week-wrapped) for t0 = ap->t_a + (s0 - ap->s_a) / 3e6, its sin(elevation) from gpsb200_pvt_coarse's step 3
+ *      prediction at ap->x_a, t0 (up vector at x_a) is >= sin(cfg->mask_deg pi / 180), and mu_p > 0 (step 3). Fewer than
+ *      GPSB200_CD_MIN_USED used PRNs: status GPSB200_CD_FEW and nothing is scored.
+ *   3. Normalise: mu_p = floor(sum_{j,tau} P_p(j, tau) / (nbins 3000)), the sum exact (128 bits: it reaches 2.3e25);
+ *      q_p(j, tau) = min(floor(2^GPSB200_CD_Q_SHIFT P_p(j, tau) / mu_p), GPSB200_CD_Q_CAP) (uint16). The cap keeps one
+ *      strong satellite from outvoting the others.
+ *   4. Lattice: hypothesis h = ((i_t n_u + i_u) n_n + i_n) n_e + i_e, i_a < n_a; offset o_a = (i_a - (n_a - 1) / 2)
+ *      step_a (real halves; 0 when n_a = 1) along east, north, up (m) and time (s); position x_h = x_a + o_e E + o_n N +
+ *      o_u U (E, N, U: the unit vectors at x_a's WGS-84 latitude / longitude, gpsb200_pvt's conversion), time t_h =
+ *      t0 + o_t.
+ *   5. Predict, per (h, used p): pred = step 3 of gpsb200_pvt_coarse at x_h, t_h (ms, satellite time); delay d =
+ *      round(3000 (1 - frac(pred))) mod 3000 (round(v) = floor(v + 0.5)), the sample after s0 where chip 0 starts;
+ *      Doppler f = -(e . v_rot - c drift) / lambda_L1 with e, v_rot and drift of the prediction's last step and a static
+ *      receiver (the sign of a channel's f_carr, where the acquisition peaks); bin j = round((f - f_lo_p) / step_hz),
+ *      j = 0 when nbins = 1. A PRN whose j lies outside 0..nbins-1 adds nothing at h.
+ *   6. Score: S(h, b) = sum_p q_p(j_p(h), (d_p(h) + b) mod 3000) for every clock shift b < 3000 (uint32: at most
+ *      32 GPSB200_CD_Q_CAP = 2^18); S_h = max_b S(h, b) and b_h its lowest b.
+ *   7. Pick: the winner h* has the largest S_h, the lowest h on ties. The runner-up has the largest S_h among the h
+ *      whose lattice distance sqrt((o_e - o_e*)^2 + (o_n - o_n*)^2 + (o_u - o_u*)^2) exceeds cfg->distinct_m, the lowest
+ *      h on ties. Status GPSB200_CD_AMBIGUOUS when 100 S_runner >= GPSB200_CD_AMBIGUOUS_PCT S_h*, else GPSB200_CD_OK.
+ *   8. Seeds [nprn]: for a PRN with a cell at h* (used, j in range), res[p] as if its argmax had been forced there: bin
+ *      j_p(h*), delay (d_p(h*) + b*) mod 3000, doppler_hz = f_lo_p + j step_hz, delay_chips = delay 1023 / 3000,
+ *      p1 = P_p(j, delay), p2 = the largest P_p(j, tau) more than 3 samples (circular) from delay, ratio = p1 / p2
+ *      (infinity when p2 is 0). Every other PRN (and every PRN when FEW): res[p] with ratio -1. So the seeds go
+ *      straight into gpsb200_snapshot_measure with min_ratio 0, which refines the PRNs with a cell and leaves the others
+ *      WEAK; (x*, ap->t_a + o_t*) at ap->s_a is the a-priori config of gpsb200_pvt_snapshot.
+ * out: the record below; records without a winner (FEW) have winner, runner and shift -1, scores 0 and NaN doubles, a
+ * winner without a runner-up has runner -1, runner_score 0 and runner_dist NaN. scores (NULL: not wanted) [nhyp]: S_h,
+ * b_h (every 0 when FEW). table (NULL: not wanted) [nhyp][nprn]: (j, d) of step 5, bin -1 where j lies outside the grid,
+ * both -1 for unused PRNs (every -1 when FEW).
+ * Checks (GPSB200_ERR_ARG, before anything is enqueued): acq and f_lo_prn as the search checks them, eph, ap, cfg, res,
+ * seed and out not NULL, ap as gpsb200_pvt_coarse checks it, every n_a >= 1 with n_e n_n n_u n_t <= GPSB200_CD_MAX_HYP,
+ * step_a finite and > 0 where n_a > 1, mask_deg and distinct_m finite, reserved 0.
+ * Device scratch beyond the search's (which keeps its grid): nprn nbins (6072 x 2 + 16) bytes of normalised rows and row
+ * sums, 8 nhyp bytes of per-hypothesis scores (128 MiB at GPSB200_CD_MAX_HYP), and 8 nhyp nprn bytes when the table
+ * is wanted. Results do not depend on the order the device runs in. Blocking. */
+#define GPSB200_CD_MAX_HYP    (1 << 24)
+#define GPSB200_CD_MIN_USED   4
+#define GPSB200_CD_Q_SHIFT    8
+#define GPSB200_CD_Q_CAP      8192
+#define GPSB200_CD_AMBIGUOUS_PCT 90
+enum { GPSB200_CD_OK = 0, GPSB200_CD_FEW = 1, GPSB200_CD_AMBIGUOUS = 2 };
+typedef struct gpsb200_collective_config {
+    int32_t n[4];          /* lattice points along east, north, up, time: >= 1 each */
+    double step[4];        /* their spacing: m, m, m, s; finite and > 0 where n > 1 */
+    double mask_deg;       /* elevation mask of the used PRNs at x_a, degrees: finite */
+    double distinct_m;     /* the runner-up lies farther than this from the winner, m: finite */
+    int64_t reserved;      /* 0 */
+} gpsb200_collective_config_t;   /* 72 bytes */
+typedef struct gpsb200_collective {
+    int32_t status;        /* GPSB200_CD_* */
+    int32_t nused;         /* used PRNs (step 2) */
+    uint32_t used;         /* bit p: acq->prn[p] is used */
+    int32_t shift;         /* b*: the winner's clock shift, samples; -1 without a winner */
+    int32_t winner, runner;    /* hypotheses h* and the runner-up's; -1 when there is none */
+    uint32_t score, runner_score;  /* their S_h; 0 when there is none */
+    double o_t;            /* the winner's time offset, s */
+    double x[3];           /* the winner's ECEF position x_h*, m */
+    double lat_deg, lon_deg, height;   /* and its WGS-84 latitude, longitude and height (gpsb200_pvt's conversion) */
+    double runner_dist;    /* the runner-up's lattice distance from the winner, m */
+} gpsb200_collective_t;    /* 96 bytes */
+typedef struct gpsb200_cd_score {
+    uint32_t score;        /* S_h */
+    int32_t shift;         /* b_h */
+} gpsb200_cd_score_t;      /* 8 bytes */
+typedef struct gpsb200_cd_cell {
+    int32_t bin;           /* j_p(h); -1 outside the grid or unused */
+    int32_t delay;         /* d_p(h); -1 unused */
+} gpsb200_cd_cell_t;       /* 8 bytes */
+int gpsb200_collective(gpsb200_ctx_t *ctx, const void *iq, int64_t nsamples, int sample_size,
+                       const gpsb200_acq_config_t *acq, const double *f_lo_prn, const gpsb200_ephemeris_t *eph,
+                       const gpsb200_coarse_config_t *ap, const gpsb200_collective_config_t *cfg,
+                       gpsb200_acq_result_t *res, gpsb200_acq_result_t *seed, gpsb200_collective_t *out,
+                       gpsb200_cd_score_t *scores, gpsb200_cd_cell_t *table);
+/* Same for a source in device memory (16-byte aligned), searched and scored in place on `stream` (0 = the context's
+ * own stream) behind whatever it holds; returns when the outputs are in host memory. */
+int gpsb200_collective_device(gpsb200_ctx_t *ctx, const void *iq_device, int64_t nsamples, int sample_size,
+                              const gpsb200_acq_config_t *acq, const double *f_lo_prn, const gpsb200_ephemeris_t *eph,
+                              const gpsb200_coarse_config_t *ap, const gpsb200_collective_config_t *cfg,
+                              gpsb200_acq_result_t *res, gpsb200_acq_result_t *seed, gpsb200_collective_t *out,
+                              gpsb200_cd_score_t *scores, gpsb200_cd_cell_t *table, void *stream);
+
 /* ---- scenario engine: the reference's host path outside the sample loop -------------
  * RINEX-2/3 navigation file (plain or gzip-compressed, read through zlib like the reference, gps.c:1147) +
  * location/motion -> the gpsb200_chan_t records and NAV frames the

@@ -22,6 +22,8 @@ from .api import (  # noqa: F401
     SKY_DTYPE, nav_almanac, almanac_predict,
     SNAPSHOT_CONFIG_DTYPE, SNAPSHOT_DTYPE, SNAP_OK, SNAP_WEAK, SNAP_NO_CONVERGENCE, SNAP_ITERATIONS, SNAP_MAX_ITER,
     snapshot_config, SNAP_BATCH_SCRATCH, snapshot_batch_pass,
+    COLLECTIVE_CONFIG_DTYPE, COLLECTIVE_DTYPE, CD_SCORE_DTYPE, CD_CELL_DTYPE, CD_OK, CD_FEW, CD_AMBIGUOUS, CD_MAX_HYP,
+    CD_MIN_USED, CD_Q_SHIFT, CD_Q_CAP, CD_AMBIGUOUS_PCT, collective_config,
 )
 from .synthetic import synthetic_chans  # noqa: F401,E402
 from . import sharding  # noqa: F401,E402

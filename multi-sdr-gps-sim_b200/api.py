@@ -306,6 +306,34 @@ def snapshot_config(min_ratio=2.5, iterations=SNAP_ITERATIONS):
     return c
 
 
+# gpsb200_collective_config_t / gpsb200_collective_t / gpsb200_cd_score_t / gpsb200_cd_cell_t (DESIGN §11.7)
+COLLECTIVE_CONFIG_DTYPE = np.dtype([("n", "<i4", 4), ("step", "<f8", 4), ("mask_deg", "<f8"), ("distinct_m", "<f8"),
+                                    ("reserved", "<i8")])
+COLLECTIVE_DTYPE = np.dtype([("status", "<i4"), ("nused", "<i4"), ("used", "<u4"), ("shift", "<i4"), ("winner", "<i4"),
+                             ("runner", "<i4"), ("score", "<u4"), ("runner_score", "<u4"), ("o_t", "<f8"),
+                             ("x", "<f8", 3), ("lat_deg", "<f8"), ("lon_deg", "<f8"), ("height", "<f8"),
+                             ("runner_dist", "<f8")])
+CD_SCORE_DTYPE = np.dtype([("score", "<u4"), ("shift", "<i4")])
+CD_CELL_DTYPE = np.dtype([("bin", "<i4"), ("delay", "<i4")])
+assert (COLLECTIVE_CONFIG_DTYPE.itemsize, COLLECTIVE_DTYPE.itemsize) == (72, 96)
+CD_OK, CD_FEW, CD_AMBIGUOUS = 0, 1, 2
+CD_MAX_HYP, CD_MIN_USED, CD_Q_SHIFT, CD_Q_CAP, CD_AMBIGUOUS_PCT = 1 << 24, 4, 8, 8192, 90
+
+
+def collective_config(ext_m, step_m, ext_s=0.0, step_s=1.0, up_ext_m=0.0, up_step_m=1.0, mask_deg=5.0,
+                      distinct_m=None):
+    """A COLLECTIVE_CONFIG_DTYPE record for a lattice of +-ext_m east and north at step_m, +-up_ext_m up at up_step_m
+    and +-ext_s in time at step_s: n = 2 floor(ext / step) + 1 points per axis (one where ext is 0). distinct_m
+    defaults to two horizontal steps."""
+    c = np.zeros(1, COLLECTIVE_CONFIG_DTYPE)[0]
+    for a, (e, st) in enumerate(((ext_m, step_m), (ext_m, step_m), (up_ext_m, up_step_m), (ext_s, step_s))):
+        c["n"][a] = 2 * int(np.floor(float(e) / float(st) + 1e-9)) + 1 if e > 0 else 1
+        c["step"][a] = float(st)
+    c["mask_deg"] = float(mask_deg)
+    c["distinct_m"] = 2.0 * float(step_m) if distinct_m is None else float(distinct_m)
+    return c
+
+
 def search_nodes(n=SEARCH_NODES):
     """gpsb200_search_nodes: the ECEF positions float64[n, 3] of the n-node search grid."""
     xyz = np.zeros((max(1, int(n)), 3))
@@ -429,7 +457,7 @@ EXPORTS = ["gpsb200_create", "gpsb200_destroy", "gpsb200_last_error", "gpsb200_v
            "gpsb200_track",
            "gpsb200_track_device", "gpsb200_nav_decode", "gpsb200_nav_word_check", "gpsb200_nav_parity",
            "gpsb200_nav_ephemeris", "gpsb200_nav_time_anchor", "gpsb200_pvt", "gpsb200_pvt_replay",
-           "gpsb200_pvt_raim", "gpsb200_raim_thresholds", "gpsb200_pvt_araim", "gpsb200_araim_kfa", "gpsb200_pvt_coarse", "gpsb200_pvt_search", "gpsb200_search_nodes", "gpsb200_snapshot_measure", "gpsb200_snapshot_measure_device", "gpsb200_snapshot_batch", "gpsb200_snapshot_batch_device", "gpsb200_pvt_snapshot", "gpsb200_pvt_snapshot_search", "gpsb200_rinex_ephemeris", "gpsb200_bind_numa", "gpsb200_span_chain_host", "gpsb200_lanes_model_block",
+           "gpsb200_pvt_raim", "gpsb200_raim_thresholds", "gpsb200_pvt_araim", "gpsb200_araim_kfa", "gpsb200_pvt_coarse", "gpsb200_pvt_search", "gpsb200_search_nodes", "gpsb200_snapshot_measure", "gpsb200_snapshot_measure_device", "gpsb200_snapshot_batch", "gpsb200_snapshot_batch_device", "gpsb200_pvt_snapshot", "gpsb200_pvt_snapshot_search", "gpsb200_collective", "gpsb200_collective_device", "gpsb200_rinex_ephemeris", "gpsb200_bind_numa", "gpsb200_span_chain_host", "gpsb200_lanes_model_block",
            "gpsb200_lanes_window_band_host", "gpsb200_slice_prepare", "gpsb200_slice_probe",
            "gpsb200_slice_finish", "gpsb200_slice_finish_cb", "gpsb200_slice_wait", "gpsb200_link_apply", "gpsb200_slice_link_host", "gpsb200_debug_corrupt_chain", "gpsb200_synth_kernel_name",
            "gpsb200_debug_run_checkpoints", "gpsb200_checkpoint_segments_host",
@@ -558,6 +586,10 @@ def lib():
         L.gpsb200_pvt_snapshot.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
                                            C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
         L.gpsb200_pvt_snapshot_search.argtypes = L.gpsb200_pvt_snapshot.argtypes + [C.c_void_p]
+        L.gpsb200_collective.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.POINTER(AcqConfig), C.c_void_p,
+                                         C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                         C.c_void_p, C.c_void_p]
+        L.gpsb200_collective_device.argtypes = L.gpsb200_collective.argtypes + [C.c_void_p]
         L.gpsb200_rinex_ephemeris.argtypes = [C.c_char_p, C.c_int, C.c_int32, C.c_double, C.c_void_p]
         _lib = L
     return _lib
@@ -1245,6 +1277,41 @@ class Context:
                        None if flo is None else flo.ctypes.data, sc.ctypes.data, res.ctypes.data, out.ctypes.data,
                        *dev))
         return res, out
+
+    def collective(self, eph, apriori, cfg, iq=None, sample_size=SC08, prns=range(1, 33), ms=10, s0=0, f_lo=-5000.0,
+                   step=250.0, nbins=41, f_lo_prn=None, want_scores=False, want_table=False, device_ptr=None,
+                   nsamples=None, stream=0):
+        """Collective detection (gpsb200_collective; DESIGN §11.7): the search of acquire (or, with f_lo_prn
+        float64[nprn], of acquire_windows) over its arguments, then a lattice of receiver positions and time offsets
+        around apriori (COARSE_CONFIG_DTYPE) scored against the power grids. eph: EPHEMERIS_DTYPE[32] indexed by PRN - 1
+        (rinex_ephemeris); cfg: COLLECTIVE_CONFIG_DTYPE record (collective_config). Source as acquire.
+        -> (results ACQ_RESULT_DTYPE[nprn], seeds ACQ_RESULT_DTYPE[nprn], COLLECTIVE_DTYPE record), then with
+        want_scores CD_SCORE_DTYPE[nhyp] and with want_table CD_CELL_DTYPE[nhyp, nprn]."""
+        prns = [int(p) for p in prns]
+        flo = None
+        if f_lo_prn is not None:
+            flo = np.ascontiguousarray(f_lo_prn, dtype=np.float64).reshape(-1)
+            if flo.size != len(prns):
+                raise GpsB200Error(ERR_ARG, "collective: %d first bins for %d PRNs" % (flo.size, len(prns)))
+        acq = self._acq_config(prns, ms, s0, f_lo, step, nbins)
+        e = np.ascontiguousarray(eph, dtype=EPHEMERIS_DTYPE).reshape(-1)
+        if e.size != 32:
+            raise GpsB200Error(ERR_ARG, "collective: %d ephemeris records, not 32" % e.size)
+        ap = np.array(apriori, dtype=COARSE_CONFIG_DTYPE).reshape(1)
+        cf = np.array(cfg, dtype=COLLECTIVE_CONFIG_DTYPE).reshape(1)
+        nhyp = max(1, int(np.prod(cf[0]["n"].astype(np.int64)))) if (cf[0]["n"] >= 1).all() else 1
+        n = max(1, min(len(prns), 32))
+        res, seed = np.zeros(n, ACQ_RESULT_DTYPE), np.zeros(n, ACQ_RESULT_DTYPE)
+        rec = np.zeros(1, COLLECTIVE_DTYPE)
+        sc = np.zeros(nhyp, CD_SCORE_DTYPE) if want_scores else None
+        tb = np.zeros((nhyp, n), CD_CELL_DTYPE) if want_table else None
+        src, ns, dev = self._rx_source(iq, device_ptr, nsamples, stream)
+        fn = lib().gpsb200_collective_device if dev else lib().gpsb200_collective
+        self._check(fn(self._h, src, ns, int(sample_size), C.byref(acq), None if flo is None else flo.ctypes.data,
+                       e.ctypes.data, ap.ctypes.data, cf.ctypes.data, res.ctypes.data, seed.ctypes.data,
+                       rec.ctypes.data, None if sc is None else sc.ctypes.data,
+                       None if tb is None else tb.ctypes.data, *dev))
+        return (res, seed, rec[0]) + ((sc,) if want_scores else ()) + ((tb,) if want_table else ())
 
     @staticmethod
     def _snapshot_args(chans, meas, cfg, want_residuals):

@@ -30,6 +30,7 @@
 #include "../../include/gpsb200.h"
 #include "acquire.h"
 #include "snapshot.h"
+#include "collective.h"
 #include "device_buffer.h"
 #include "track.h"
 #include "pvt.h"
@@ -217,6 +218,7 @@ struct gpsb200_ctx {
     trk::Scratch trk;                      // tracking calls (track.cu), allocated by the first one
     pvt::Scratch pvt;                      // position fixes (pvt.cu), allocated by the first one
     snap::Scratch snap;                    // snapshot measurements (snapshot.cu), allocated by the first one
+    cd::Scratch cd;                        // collective detection (collective.cu), allocated by the first one
     std::string err;
 };
 
@@ -1166,6 +1168,31 @@ int snapshot_measure(gpsb200_ctx *ctx, const void *iq, int64_t nsamples, int sam
     return GPSB200_OK;
 }
 
+// Collective detection of both entry points (acquire.cu, collective.cu; DESIGN §11.7): the search with its grid kept on
+// the device, then the lattice scored against it. Everything is checked before anything is enqueued.
+int collective(gpsb200_ctx *ctx, const void *iq, int64_t nsamples, int sample_size, const gpsb200_acq_config_t *acq,
+               const double *f_lo_prn, const gpsb200_ephemeris_t *eph, const gpsb200_coarse_config_t *ap,
+               const gpsb200_collective_config_t *cfg, gpsb200_acq_result_t *res, gpsb200_acq_result_t *seed,
+               gpsb200_collective_t *out, gpsb200_cd_score_t *scores, gpsb200_cd_cell_t *table, bool device,
+               cudaStream_t s) {
+    const char *name = device ? "gpsb200_collective_device" : "gpsb200_collective";
+    const std::string at = std::string(name) + ": ";
+    if (!iq || !eph || !ap || !cfg || !res || !seed || !out)
+        return fail(ctx, GPSB200_ERR_ARG, at + "NULL source, ephemeris, a-priori or lattice config, results, seeds or record");
+    std::string bad = acq::check(acq, nsamples, sample_size, f_lo_prn != nullptr, f_lo_prn);
+    if (bad.empty()) bad = pvt::check_coarse(*ap);
+    if (bad.empty()) bad = cd::check(cfg);
+    if (!bad.empty()) return fail(ctx, GPSB200_ERR_ARG, at + bad);
+    const void *window;
+    const int rc = rx_source(ctx, name, iq, acq->s0, acq::window_samples(acq), sample_size, device, s, &window);
+    if (rc) return rc;
+    CU(acq::scratch_reserve(ctx->acq, acq, f_lo_prn != nullptr, true));
+    CU(acq::launch(ctx->acq, window, sample_size, acq, f_lo_prn, true, s));
+    memcpy(res, ctx->acq.h_res, (size_t) acq->nprn * sizeof(gpsb200_acq_result_t));
+    CU(cd::launch(ctx->cd, ctx->acq.d_grid, ctx->acq.d_res, acq, f_lo_prn, eph, ap, cfg, seed, out, scores, table, s));
+    return GPSB200_OK;
+}
+
 // The snapshot batch of both entry points (acquire.cu, snapshot.cu; DESIGN §11.6). Every argument of every window is
 // checked before anything is enqueued. The windows then run in passes of snap::batch_pass: the search of the pass, one
 // download of its results, the measurement's checks and seed on the host (snap::seed), one upload and the measurement.
@@ -1558,6 +1585,7 @@ void gpsb200_destroy(gpsb200_ctx_t *ctx) {
     acq::scratch_free(ctx->acq);
     trk::scratch_free(ctx->trk);
     snap::scratch_free(ctx->snap);
+    cd::scratch_free(ctx->cd);
     pvt::scratch_free(ctx->pvt);
     if (ctx->s_compute) cudaStreamDestroy(ctx->s_compute);
     if (ctx->s_copy) cudaStreamDestroy(ctx->s_copy);
@@ -1937,6 +1965,27 @@ int gpsb200_snapshot_batch_device(gpsb200_ctx_t *ctx, const void *iq_device, int
     cudaStream_t s = caller_stream(ctx, stream_);
     return settle(ctx, s, snapshot_batch(ctx, iq_device, nsamples, sample_size, acq, nwin, s0, f_lo, cfg, res, out, true,
                                          s));
+}
+
+int gpsb200_collective(gpsb200_ctx_t *ctx, const void *iq, int64_t nsamples, int sample_size,
+                       const gpsb200_acq_config_t *acq, const double *f_lo_prn, const gpsb200_ephemeris_t *eph,
+                       const gpsb200_coarse_config_t *ap, const gpsb200_collective_config_t *cfg,
+                       gpsb200_acq_result_t *res, gpsb200_acq_result_t *seed, gpsb200_collective_t *out,
+                       gpsb200_cd_score_t *scores, gpsb200_cd_cell_t *table) {
+    if (!ctx) return GPSB200_ERR_ARG;
+    return settle(ctx, nullptr, collective(ctx, iq, nsamples, sample_size, acq, f_lo_prn, eph, ap, cfg, res, seed, out,
+                                           scores, table, false, ctx->s_compute));
+}
+
+int gpsb200_collective_device(gpsb200_ctx_t *ctx, const void *iq_device, int64_t nsamples, int sample_size,
+                              const gpsb200_acq_config_t *acq, const double *f_lo_prn, const gpsb200_ephemeris_t *eph,
+                              const gpsb200_coarse_config_t *ap, const gpsb200_collective_config_t *cfg,
+                              gpsb200_acq_result_t *res, gpsb200_acq_result_t *seed, gpsb200_collective_t *out,
+                              gpsb200_cd_score_t *scores, gpsb200_cd_cell_t *table, void *stream_) {
+    if (!ctx) return GPSB200_ERR_ARG;
+    cudaStream_t s = caller_stream(ctx, stream_);
+    return settle(ctx, s, collective(ctx, iq_device, nsamples, sample_size, acq, f_lo_prn, eph, ap, cfg, res, seed, out,
+                                     scores, table, true, s));
 }
 
 int gpsb200_pvt_snapshot(gpsb200_ctx_t *ctx, const gpsb200_pvt_chan_t *chans, int nchan, const gpsb200_snapshot_t *meas,

@@ -13,6 +13,7 @@
 #include <vector>
 
 #include "device_buffer.h"
+#include "orbit.cuh"
 #include "pvt.h"
 #include "synth_tables.h"
 
@@ -22,7 +23,6 @@ namespace pvt {
 namespace {
 
 constexpr double kCms = 2.99792458e5;             // metres per ms of light time
-constexpr double kRelF = -4.442807633e-10;        // relativistic clock term, s / m^1/2
 constexpr double kCodeMod = 1023.0 * 4294967296.0;   // 2^-32 chips per code period
 constexpr double kStepHz = 3e6 / 4294967296.0;    // carrier step unit, Hz
 constexpr double kIonoMinRadius = 6e6;            // the Klobuchar term needs an estimate near the surface
@@ -59,8 +59,6 @@ template <bool kRaim> using KernelArgs = typename std::conditional<kRaim, RaimAr
 __constant__ double kUraNom[15] = {2.0, 2.8, 4.0, 5.7, 8.0, 11.3, 16.0, 32.0, 64.0, 128.0, 256.0, 512.0, 1024.0, 2048.0,
                                    4096.0};
 constexpr double kTenDeg = 10.0 * M_PI / 180.0;
-
-__device__ inline double wrap_half_week(double d) { return d > 302400.0 ? d - 604800.0 : (d < -302400.0 ? d + 604800.0 : d); }
 
 __device__ inline int64_t floor_div(int64_t a, int64_t b) {
     const int64_t q = a / b;
@@ -149,25 +147,6 @@ template <int N> struct Chol {
     }
 };
 
-// WGS-84 latitude, longitude (rad) and height of an ECEF point: six fixed-point steps of
-// lat = atan2(z + e^2 N(lat) sin lat, p) from lat = atan2(z, p (1 - e^2)).
-__device__ void ecef_llh(const double *x, double &lat, double &lon, double &h) {
-    const double e2 = kWgsE * kWgsE;
-    const double p = sqrt(x[0] * x[0] + x[1] * x[1]);
-    lon = atan2(x[1], x[0]);
-    lat = atan2(x[2], p * (1.0 - e2));
-    double N = kWgsA;
-#pragma unroll 1
-    for (int it = 0; it < 6; it++) {
-        const double sl = sin(lat);
-        N = kWgsA / sqrt(1.0 - e2 * sl * sl);
-        lat = atan2(x[2] + e2 * N * sl, p);
-    }
-    double sl, cl;
-    sincos(lat, &sl, &cl);
-    h = p * cl + x[2] * sl - kWgsA * sqrt(1.0 - e2 * sl * sl);
-}
-
 // The Klobuchar delay in metres (the reference's ionosphericDelay, gps.c:1893-1964, with a valid alpha / beta set).
 // Fm (not NULL): receives the obliquity factor F and the geomagnetic latitude phi_m (semicircles) as well.
 __device__ double klobuchar(const gpsb200_pvt_config_t &cfg, double lat, double lon, double az, double el, double t,
@@ -197,57 +176,6 @@ __device__ double klobuchar(const gpsb200_pvt_config_t &cfg, double lat, double 
         return F * (5.0e-9 + amp * (1.0 - X2 / 2.0 + X2 * X2 / 24.0)) * kC;
     }
     return F * 5.0e-9 * kC;
-}
-
-// Satellite position, velocity (ECEF) at GPS time t and clock offset / drift (IS-GPS-200 20.3.3.3.3, 20.3.3.4.3).
-__device__ void satellite(const gpsb200_ephemeris_t &e, double t, double *p, double *v, double &dt, double &ddt) {
-    const double tk = wrap_half_week(t - e.toe);
-    const double A = e.sqrta * e.sqrta;
-    const double n = sqrt(kGM / (A * A * A)) + e.deltan;
-    const double M = e.m0 + n * tk;
-    double E = M;
-#pragma unroll 1
-    for (int it = 0; it < 10; it++) {
-        double sE, cE;
-        sincos(E, &sE, &cE);
-        const double dE = (M - E + e.ecc * sE) / (1.0 - e.ecc * cE);
-        E += dE;
-        if (fabs(dE) <= 1e-14) break;
-    }
-    double sE, cE;
-    sincos(E, &sE, &cE);
-    const double om = 1.0 - e.ecc * cE;
-    const double Edot = n / om;
-    const double sq = sqrt(1.0 - e.ecc * e.ecc);
-    const double pk = atan2(sq * sE, cE - e.ecc) + e.aop;
-    const double pkdot = sq * Edot / om;
-    double s2, c2;
-    sincos(2.0 * pk, &s2, &c2);
-    const double uk = pk + e.cus * s2 + e.cuc * c2;
-    const double ukdot = pkdot * (1.0 + 2.0 * (e.cus * c2 - e.cuc * s2));
-    const double rk = A * om + e.crc * c2 + e.crs * s2;
-    const double rkdot = A * e.ecc * sE * Edot + 2.0 * pkdot * (e.crs * c2 - e.crc * s2);
-    const double ik = e.inc0 + e.idot * tk + e.cic * c2 + e.cis * s2;
-    const double ikdot = e.idot + 2.0 * pkdot * (e.cis * c2 - e.cic * s2);
-    double su, cu, si, ci;
-    sincos(uk, &su, &cu);
-    sincos(ik, &si, &ci);
-    const double xp = rk * cu, yp = rk * su;
-    const double xpdot = rkdot * cu - yp * ukdot, ypdot = rkdot * su + xp * ukdot;
-    const double odot = e.omgdot - kOmegaE;
-    const double ok = e.omg0 + tk * odot - kOmegaE * e.toe;
-    double so, co;
-    sincos(ok, &so, &co);
-    p[0] = xp * co - yp * ci * so;
-    p[1] = xp * so + yp * ci * co;
-    p[2] = yp * si;
-    const double tmp = ypdot * ci - yp * si * ikdot;
-    v[0] = -odot * p[1] + xpdot * co - tmp * so;
-    v[1] = odot * p[0] + xpdot * so + tmp * co;
-    v[2] = yp * ci * ikdot + ypdot * si;
-    const double d = wrap_half_week(t - e.toc);
-    dt = e.af0 + d * (e.af1 + d * e.af2) + kRelF * e.ecc * e.sqrta * sE - e.tgd;
-    ddt = e.af1 + 2.0 * d * e.af2;
 }
 
 // The code period k >= 1 of a channel holding sample s (epochs[k].sample <= s < epochs[k + 1].sample), -1 if none.
@@ -310,17 +238,6 @@ __device__ __forceinline__ bool measure(const Args &a, int lane, int64_t s, int6
     satellite(c.eph, tt, p, v, dtsv, ddtsv);
     return true;
 }
-
-// The geodetic frame at an ECEF point: latitude and longitude (rad) and their sines and cosines; all 0 until set.
-struct Geo {
-    double lat = 0.0, lon = 0.0, sla = 0.0, cla = 0.0, slo = 0.0, clo = 0.0;
-    __device__ void set(const double *x) {
-        double hgt;
-        ecef_llh(x, lat, lon, hgt);
-        sincos(lat, &sla, &cla);
-        sincos(lon, &slo, &clo);
-    }
-};
 
 // A lane's row at the estimate X: the satellite at p, v (ECEF at its transmit time) turned by the Earth's rotation over
 // the flight time. Gives the line of sight l, its length R and the turned velocity pv; with enu, also l's azimuth and
@@ -868,27 +785,6 @@ struct CoarseArgs : Args {
 struct SnapCoarseArgs : CoarseArgs {
     const gpsb200_snapshot_t *meas;
 };
-
-// Header step 3: the predicted transmit time (ms, satellite time) of a satellite at position x and receive time t, and
-// sin(elevation) seen along the up vector `up` (unit, ECEF).
-__device__ double predict(const gpsb200_ephemeris_t &e, const double *x, double t, const double *up, double &sel) {
-    double tau = 0.075, p[3], v[3], dt = 0.0, ddt;
-    double l0 = 0.0, l1 = 0.0, l2 = 0.0;
-#pragma unroll 1
-    for (int i = 0; i < 3; i++) {
-        satellite(e, t - tau, p, v, dt, ddt);
-        double sth, cth;
-        sincos(kOmegaE * tau, &sth, &cth);
-        l0 = p[0] * cth + p[1] * sth - x[0];
-        l1 = p[1] * cth - p[0] * sth - x[1];
-        l2 = p[2] - x[2];
-        tau = sqrt(l0 * l0 + l1 * l1 + l2 * l2) / kC;
-    }
-    sel = (up[0] * l0 + up[1] * l1 + up[2] * l2) / (tau * kC);
-    return 1000.0 * (t - tau + dt);
-}
-
-__device__ inline double round_half_up(double v) { return floor(v + 0.5); }
 
 // The coarse record of an instant without a coarse-time fix.
 __device__ inline void no_coarse(gpsb200_coarse_t &o, int ref) {
@@ -1473,6 +1369,16 @@ cudaError_t launch(const Scratch &sc, cudaStream_t s) {
 
 }  // namespace
 
+std::string check_coarse(const gpsb200_coarse_config_t &c) {
+    for (int i = 0; i < 3; i++)
+        if (!std::isfinite(c.x_a[i])) return "coarse x_a must be finite";
+    if (!(c.t_a >= 0.0 && c.t_a < 604800.0)) return "coarse t_a must lie in 0 <= t_a < 604800";
+    if (c.s_a < 0 || c.s_a > (1ll << 62)) return "coarse s_a outside 0..2^62";
+    if (c.week < 0) return "coarse week must be >= 0";
+    if (c.reserved != 0) return "coarse reserved must be 0";
+    return std::string();
+}
+
 std::string check(const gpsb200_pvt_chan_t *chans, int nchan, const gpsb200_track_epoch_t *epochs, const int32_t *nepochs,
                   int max_epochs, const gpsb200_pvt_config_t *cfg, const Stage &st) {
     const gpsb200_raim_config_t *raim = st.raim;
@@ -1494,13 +1400,8 @@ std::string check(const gpsb200_pvt_chan_t *chans, int nchan, const gpsb200_trac
         if (c.reserved != 0) return "search reserved must be 0";
     }
     if (coarse) {
-        const gpsb200_coarse_config_t &c = *coarse;
-        for (int i = 0; i < 3; i++)
-            if (!std::isfinite(c.x_a[i])) return "coarse x_a must be finite";
-        if (!(c.t_a >= 0.0 && c.t_a < 604800.0)) return "coarse t_a must lie in 0 <= t_a < 604800";
-        if (c.s_a < 0 || c.s_a > (1ll << 62)) return "coarse s_a outside 0..2^62";
-        if (c.week < 0) return "coarse week must be >= 0";
-        if (c.reserved != 0) return "coarse reserved must be 0";
+        const std::string bad = check_coarse(*coarse);
+        if (!bad.empty()) return bad;
     }
     if (araim) {
         const gpsb200_araim_config_t &r = *araim;

@@ -56,6 +56,9 @@ struct Stage {
 std::string check(const gpsb200_pvt_chan_t *chans, int nchan, const gpsb200_track_epoch_t *epochs, const int32_t *nepochs,
                   int max_epochs, const gpsb200_pvt_config_t *cfg, const Stage &st);
 
+// The a-priori config's part of check (gpsb200_pvt_coarse), also collective detection's.
+std::string check_coarse(const gpsb200_coarse_config_t &c);
+
 // The RAIM tables of gpsb200_raim_thresholds (raim_thresholds.cpp); false when p_fa or p_md is outside 1e-12..0.5.
 bool raim_thresholds(double p_fa, double p_md, double *T, double *lambda);
 // The ARAIM test multipliers of gpsb200_araim_kfa (raim_thresholds.cpp); false when a probability is outside 1e-12..0.5.

@@ -21,6 +21,11 @@
 // --almanac and an a-priori position the windows are warm started: each window's sky is predicted at its own time (the
 // assist time plus its offset from the first window), every window of a chunk searches the PRNs predicted at or above
 // the mask in any of them, each over the warm start's bins around that window's own prediction.
+// Collective detection (--fix --collective, DESIGN §11.7): with an a-priori position, per window one
+// gpsb200_collective call scores a lattice of positions and time offsets around the a-priori against the powers of all
+// searched PRNs, so that satellites below the threshold still count; the seeds at the winner's cells are refined
+// (gpsb200_snapshot_measure, min_ratio 0) and fixed from the winner (gpsb200_pvt_snapshot). Without --collective the
+// output is unchanged.
 #include <algorithm>
 #include <cmath>
 #include <cstdio>
@@ -39,6 +44,9 @@ static const double kDefaultThreshold = 2.5;
 // project's streams to within 146 Hz (tests/test_almanac_decode.py), so +-500 Hz (5 bins at 250 Hz) holds it with room
 // for an a-priori a few tens of km and seconds off.
 static const double kDefaultWindow = 500.0, kDefaultMask = -5.0;
+// --collective: the runner-up lies farther than this (or two lattice steps) from the winner. On the model a clean
+// winner's neighbours within 1 km keep most of its score (DESIGN §11.7).
+static const double kDistinct = 1000.0;
 
 static void usage() {
     fprintf(stderr,
@@ -48,7 +56,8 @@ static void usage() {
             "             [--window HZ] [--mask DEG]]\n"
             "            [--fix --assist NAV_FILE[,3] --assist-pos LAT,LON,H|search --assist-time YYYY/MM/DD,hh:mm:ss[.s]\n"
             "             [--every MS] [--count N] [--iono a0,a1,a2,a3,b0,b1,b2,b3]\n"
-            "             [--almanac FILE.sem [--window HZ] [--mask DEG]]]\n"
+            "             [--almanac FILE.sem [--window HZ] [--mask DEG]]\n"
+            "             [--collective EXT_M,STEP_M[,EXT_S,STEP_S] [--mask DEG]]]\n"
             "  FILE              interleaved I,Q at 3 Msps, int8 (default) or int16 (--iq16)\n"
             "  --block B         start at 0.1 s block B (sample 300000 B); --offset-ms N adds N ms (3000 N samples)\n"
             "  --ms K            coherent 1 ms periods summed, 1..100 (default 10)\n"
@@ -64,7 +73,13 @@ static void usage() {
             "                    ephemeris from the RINEX file of --assist (,3: RINEX 3) at --assist-time, the GPS time\n"
             "                    of the first window's first sample; one window every --every ms (default 100), --count\n"
             "                    windows (default 1); --iono: the Klobuchar alpha / beta to apply; --almanac (with\n"
-            "                    LAT,LON,H only): warm start every window from its own predicted sky\n",
+            "                    LAT,LON,H only): warm start every window from its own predicted sky\n"
+            "  --collective      (with --fix and LAT,LON,H) collective detection per window: a lattice of +-EXT_M at\n"
+            "                    STEP_M east and north and +-EXT_S at STEP_S in time (default 0: none) around the\n"
+            "                    a-priori, scored over every PRN of the search (used: ephemeris valid, elevation at or\n"
+            "                    above --mask); its seeds refined and fixed from the winner; the line adds the lattice\n"
+            "                    status, runner-up / winner score, clock shift, time offset, used PRNs and how many of\n"
+            "                    them passed --threshold alone\n",
             kDefaultThreshold, kDefaultWindow, kDefaultMask);
     exit(2);
 }
@@ -241,6 +256,124 @@ static int snapshot_fixes(const char *path, int ss, int device, long long s0, gp
     return rc == GPSB200_OK ? 0 : 1;
 }
 
+// --collective: count windows every every_ms from sample s0, each searched on the standard grid and scored against a
+// lattice around the a-priori position and time (gpsb200_collective, DESIGN §11.7), one call per window; the seeds are
+// measured with min_ratio 0 (gpsb200_snapshot_measure) and fixed from the winner (gpsb200_pvt_snapshot). lat: the
+// lattice's sizes and steps (the a-priori time is that of the first window's first sample).
+static int collective_fixes(const char *path, int ss, int device, long long s0, gpsb200_acq_config_t cfg, double lo,
+                            double hi, double step, double threshold, const char *nav, int nav_v3, const double *x_a,
+                            int32_t week, double sow, long long every_ms, long long count, gpsb200_pvt_config_t pcfg,
+                            const gpsb200_collective_config_t &lat) {
+    cfg.f_lo_hz = lo;
+    cfg.step_hz = step;
+    cfg.nbins = (int) std::floor((hi - lo) / step + 1e-9) + 1;
+    cfg.s0 = 0;
+    gpsb200_ephemeris_t eph[32];
+    if (gpsb200_rinex_ephemeris(nav, nav_v3, week, sow, eph) != GPSB200_OK) {
+        fprintf(stderr, "gpsb200-acq: cannot read the ephemeris of %s\n", nav);
+        return 1;
+    }
+    const size_t elem = ss == GPSB200_SC16 ? 2 : 1;
+    const long long need = (long long) GPSB200_ACQ_CODE_SAMPLES * cfg.ms + GPSB200_ACQ_CODE_SAMPLES - 1;
+    const long long have = file_samples(path, elem);
+    FILE *f = fopen(path, "rb");
+    if (have < 0 || !f) {
+        fprintf(stderr, "gpsb200-acq: cannot open %s\n", path);
+        return 1;
+    }
+    gpsb200_ctx_t *ctx = nullptr;
+    if (create_rx_context(device, &ctx) != GPSB200_OK) {
+        fprintf(stderr, "gpsb200-acq: cannot create a context\n");
+        fclose(f);
+        return 1;
+    }
+    gpsb200_snapshot_config_t scfg;
+    memset(&scfg, 0, sizeof scfg);
+    scfg.iterations = GPSB200_SNAP_ITERATIONS;   // min_ratio 0: every seeded PRN, none of the others (ratio -1)
+    pcfg.nfix = 1;
+    pcfg.step = 1;
+    printf("# %s: collective detection and snapshot fixes, %lld window(s) of %d ms every %lld ms from sample %lld, "
+           "lattice %d x %d x %d x %d (east, north, up at %.1f m, time at %.3f s), mask %.1f deg, Klobuchar %s\n", path,
+           count, cfg.ms, every_ms, s0, lat.n[0], lat.n[1], lat.n[2], lat.n[3], lat.step[0], lat.step[3], lat.mask_deg,
+           pcfg.iono ? "on" : "off");
+    printf("# sample  status  lat_deg  lon_deg  height_m  clock_m  vx  vy  vz (ECEF m/s)  channels  pdop  delta_s  "
+           "collective  score_ratio  shift  o_t_s  used_prns  alone\n");
+    static const char *const kStatus[] = {"OK", "FEW", "NO_CONVERGENCE", "AMBIGUOUS"};
+    static const char *const kCd[] = {"OK", "FEW", "AMBIGUOUS"};
+    const int np = cfg.nprn;
+    std::vector<gpsb200_acq_result_t> res(np), seed(np);
+    std::vector<gpsb200_snapshot_t> meas(np);
+    std::vector<char> one;
+    int rc = GPSB200_OK;
+    for (long long i = 0; i < count && rc == GPSB200_OK; i++) {
+        const long long si = s0 + i * every_ms * GPSB200_ACQ_CODE_SAMPLES;
+        if (si + need > have || !read_at(f, si, need, elem, one)) break;
+        // the a-priori time at this window's first sample, in the window's own sample numbers
+        gpsb200_coarse_config_t ap;
+        memset(&ap, 0, sizeof ap);
+        memcpy(ap.x_a, x_a, sizeof ap.x_a);
+        const double t = sow + (double) (si - s0) / 3e6;
+        const double kw = std::floor(t / 604800.0);
+        ap.t_a = t - 604800.0 * kw;
+        ap.week = week + (int32_t) kw;
+        gpsb200_collective_t cd;
+        rc = gpsb200_collective(ctx, one.data(), need, ss, &cfg, nullptr, eph, &ap, &lat, res.data(), seed.data(), &cd,
+                                nullptr, nullptr);
+        if (rc != GPSB200_OK) break;
+        int alone = 0;
+        std::string used;
+        for (int q = 0; q < np; q++) {
+            alone += (cd.used >> q & 1) && res[q].ratio >= threshold;
+            if (cd.used >> q & 1) used += (used.empty() ? "" : ",") + std::to_string(cfg.prn[q]);
+        }
+        if (used.empty()) used = "-";
+        char tail[256];
+        snprintf(tail, sizeof tail, "  %s  %.4f  %d  %.3f  %s  %d", kCd[cd.status],
+                 cd.score ? (double) cd.runner_score / (double) cd.score : 0.0, cd.shift, cd.o_t, used.c_str(), alone);
+        if (cd.winner < 0) {
+            printf("%lld  FEW%s\n", si, tail);
+            continue;
+        }
+        rc = gpsb200_snapshot_measure(ctx, one.data(), need, ss, &cfg, seed.data(), &scfg, meas.data());
+        if (rc != GPSB200_OK) break;
+        std::vector<gpsb200_pvt_chan_t> chans;
+        std::vector<gpsb200_snapshot_t> row;
+        for (int q = 0; q < np; q++) {
+            gpsb200_snapshot_t mq = meas[q];
+            if (mq.status != GPSB200_SNAP_OK || !eph[mq.prn - 1].valid) continue;
+            gpsb200_pvt_chan_t pc;
+            memset(&pc, 0, sizeof pc);
+            pc.eph = eph[mq.prn - 1];
+            pc.prn = mq.prn;
+            chans.push_back(pc);
+            mq.sample = si;
+            row.push_back(mq);
+        }
+        if (chans.empty()) {
+            printf("%lld  FEW%s\n", si, tail);
+            continue;
+        }
+        // the winner as the a-priori of the coarse-time fix, at this window's first sample
+        gpsb200_coarse_config_t wp = ap;
+        memcpy(wp.x_a, cd.x, sizeof wp.x_a);
+        const double tw = ap.t_a + cd.o_t, kt = std::floor(tw / 604800.0);
+        wp.t_a = tw - 604800.0 * kt;
+        wp.week = ap.week + (int32_t) kt;
+        wp.s_a = si;
+        gpsb200_fix_t fx;
+        gpsb200_coarse_t co;
+        rc = gpsb200_pvt_snapshot(ctx, chans.data(), (int) chans.size(), row.data(), &pcfg, &wp, &fx, nullptr, &co,
+                                  nullptr);
+        if (rc != GPSB200_OK) break;
+        printf("%lld  %s  %.8f  %.8f  %.3f  %.3f  %.3f  %.3f  %.3f  %d  %.2f  %.9f%s\n", si, kStatus[fx.status],
+               fx.lat_deg, fx.lon_deg, fx.height, fx.clock_m, fx.vx, fx.vy, fx.vz, fx.nused, fx.pdop, co.delta, tail);
+    }
+    fclose(f);
+    if (rc != GPSB200_OK) fprintf(stderr, "gpsb200-acq: %s\n", gpsb200_last_error(ctx));
+    gpsb200_destroy(ctx);
+    return rc == GPSB200_OK ? 0 : 1;
+}
+
 int main(int argc, char **argv) {
     const char *path = nullptr;
     int ss = GPSB200_SC08, device = 0;
@@ -253,7 +386,9 @@ int main(int argc, char **argv) {
     double x_a[3] = {0.0, 0.0, 0.0}, sow = 0.0, window = kDefaultWindow, mask = kDefaultMask;
     int32_t week = 0;
     bool have_pos = false, have_time = false;
-    bool fix = false, pos_search = false;
+    bool fix = false, pos_search = false, collective = false;
+    gpsb200_collective_config_t lattice;
+    memset(&lattice, 0, sizeof lattice);
     std::string assist;
     int assist_v3 = 0;
     long long every_ms = 100, count = 1;
@@ -291,6 +426,18 @@ int main(int argc, char **argv) {
             if (!(window >= 0.0)) usage();
         } else if (a == "--mask") mask = atof(val());
         else if (a == "--fix") fix = true;
+        else if (a == "--collective") {
+            double ext = 0.0, st = 0.0, ext_s = 0.0, st_s = 1.0;
+            const int k = sscanf(val(), "%lf,%lf,%lf,%lf", &ext, &st, &ext_s, &st_s);
+            if ((k != 2 && k != 4) || !(ext >= 0.0) || !(st > 0.0) || !(ext_s >= 0.0) || !(st_s > 0.0)) usage();
+            const double ext_a[4] = {ext, ext, 0.0, ext_s}, st_a[4] = {st, st, 1.0, st_s};
+            for (int ax = 0; ax < 4; ax++) {
+                lattice.n[ax] = 2 * (int) std::floor(ext_a[ax] / st_a[ax] + 1e-9) + 1;
+                lattice.step[ax] = st_a[ax];
+            }
+            lattice.distinct_m = std::max(kDistinct, 2.0 * st);
+            collective = true;
+        }
         else if (a == "--assist") {
             assist = val();
             const size_t k = assist.rfind(',');
@@ -313,8 +460,15 @@ int main(int argc, char **argv) {
     }
     if (!path || block < 0 || offset_ms < 0 || (almanac && (!have_pos || !have_time || pos_search)) ||
         (!almanac && !fix && (have_pos || have_time)) || (fix && (assist.empty() || !have_pos || !have_time)) ||
-        (!fix && (!assist.empty() || pcfg.iono)) || every_ms < 1 || count < 1)
+        (!fix && (!assist.empty() || pcfg.iono)) || every_ms < 1 || count < 1 ||
+        (collective && (!fix || pos_search || almanac)))
         usage();
+    if (collective) {
+        lattice.mask_deg = mask;
+        return collective_fixes(path, ss, device, block * GPSB200_BLOCK_SAMPLES + offset_ms * GPSB200_ACQ_CODE_SAMPLES,
+                                cfg, lo, hi, step, threshold, assist.c_str(), assist_v3, x_a, week, sow, every_ms, count,
+                                pcfg, lattice);
+    }
     if (fix) {
         gpsb200_almanac_record_t rec[32];
         int32_t valid = 0;
