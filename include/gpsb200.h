@@ -393,7 +393,9 @@ int gpsb200_acquire_windows_device(gpsb200_ctx_t *ctx, const void *iq_device, in
  *   sums       E_I = sum_{m<L} c(early) I_d, E_Q, P_I, P_Q, L_I, L_Q likewise: int32 (|.| <= 3001 * 64000 < 2^31)
  *   angle(x,y) for x >= 0: both shifted right by max(0, bitlen(max(|x|, |y|)) - 30), then 24 CORDIC vectoring steps
  *              i = 0..23: y > 0 ? (x + (y >> i), y - (x >> i), z + A_i) : (x - (y >> i), y + (x >> i), z - A_i) from
- *              z = 0; A_i = round(atan(2^-i) / 2 pi * 2^32) (listed in csrc/track.h); z in 2^-32 turns
+ *              z = 0; A_i = round(atan(2^-i) / 2 pi * 2^32) (listed in csrc/track.h); z in 2^-32 turns. angle(0, 0) = 0
+ *              (the steps would give -0.277 turn): a period or window of zeros steers nothing. Small vectors keep
+ *              the steps' error, at most 1/r turn + 90 units at magnitude r (0.056 turn at r = 2; DESIGN §10)
  *   PLL        (x, y) = (P_I, P_Q), negated when P_I < 0 (Costas: data bits do not matter); e = angle(x, y)
  *   FLL        for 1 <= epochs < GPSB200_TRK_FLL_EPOCHS: cross = I' P_Q - Q' P_I, dot = I' P_I + Q' P_Q (int64, I', Q'
  *              the previous prompt), both negated when dot < 0; d = angle(dot, cross); F += (64 d) / 3000

@@ -34,8 +34,10 @@ __host__ __device__ inline int bitlen64(uint64_t v) {
 #endif
 }
 
-// Angle of (x, y), x >= 0, in 2^-32 turns: normalised to 30 bits, then 24 CORDIC vectoring steps.
+// Angle of (x, y), x >= 0, in 2^-32 turns: normalised to 30 bits, then 24 CORDIC vectoring steps. The zero vector has
+// angle 0 (the steps alone would give -0.277 turn), so that a period or window of zeros steers no loop.
 __host__ __device__ inline int32_t angle(int64_t x, int64_t y) {
+    if (x == 0 && y == 0) return 0;
     const int32_t A[kCordicSteps] = {GPSB200_TRK_ATAN};
     const uint64_t ay = y < 0 ? (uint64_t) (-y) : (uint64_t) y;
     const uint64_t mx = (uint64_t) x > ay ? (uint64_t) x : ay;

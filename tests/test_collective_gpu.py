@@ -41,9 +41,9 @@ def sky(tmp_path_factory):
     return eph, eph32, iono
 
 
-def check_against_model(ctx, iq, ss, prns, eph, ap, cfg, f_lo_prn=None, nbins=41, step=250.0, f_lo=-5000.0):
+def check_against_model(ctx, iq, ss, prns, eph, ap, cfg, f_lo_prn=None, nbins=41, step=250.0, f_lo=-5000.0, ms=K):
     """One call with scores and table, checked against acquire and the model; -> (res, seed, rec)."""
-    kw = dict(iq=iq, sample_size=ss, prns=prns, ms=K, s0=S0, nbins=nbins, step=step)
+    kw = dict(iq=iq, sample_size=ss, prns=prns, ms=ms, s0=S0, nbins=nbins, step=step)
     if f_lo_prn is None:
         res0, P = ctx.acquire(f_lo=f_lo, want_grid=True, **kw)
         flo = np.full(len(prns), f_lo)

@@ -167,7 +167,7 @@ def period_len(st):
     return (T.M - st["code_phase"].astype(object) + st["code_step"].astype(object) - 1) // st["code_step"].astype(object)
 
 
-@pytest.mark.parametrize("nch", [1, 7, 32])
+@pytest.mark.parametrize("nch", [1, 4, 7, 12, 20, 32])
 @pytest.mark.parametrize("kind", ["int8", "int16", "full", "signal"])
 def test_track_limit_states(kind, nch):
     """States at the limits (tests/test_receiver_edges.py: limit_states) stepped through 300 periods: one uncut call,
@@ -177,7 +177,9 @@ def test_track_limit_states(kind, nch):
     buffer's last sample (and not tracked one sample short), channels past the end with 0 epochs and their state kept.
     On the full-scale input the last channel tracks the signal coherently (coherent_state), which drives bitlen(E + L)
     past 52 and |P_I| past 2^26, towards the int32 bound of the sums; with one channel that is the only channel, and it
-    stays near its 1 kHz carrier, so carr_freq reaches its clamp in the other eleven runs only."""
+    stays near its 1 kHz carrier, so carr_freq reaches its clamp in the other runs only. Channel 3 (kind 3: 199 epochs,
+    no previous prompt) runs its last FLL update on cross = dot = 0, whose angle is 0: its first carrier step is the
+    PLL's alone (with four channels on the full-scale input that channel is the coherent one instead)."""
     iq, ss, prns = track_input(kind)
     base = 17
     st0 = limit_states([prns[c % len(prns)] for c in range(nch)], base, nch)
@@ -192,6 +194,13 @@ def test_track_limit_states(kind, nch):
         if kind == "full":
             bits, p_i = coherent_reach(eps1[-1])
             assert bits >= 52 and p_i > 2 ** 26, (bits, p_i)
+        if nch > 4 or (nch == 4 and kind != "full"):
+            z, ep = st0[3], eps1[3][0]
+            assert z["epochs"] == T.FLL_EPOCHS - 1 and z["prev_i"] == 0 and z["prev_q"] == 0
+            pi, pq = int(ep["p_i"]), int(ep["p_q"])
+            e = int(T.angle(np.int64(abs(pi)), np.int64(-pq if pi < 0 else pq)))
+            F = min(max(int(z["carr_freq"]) + (e >> 12), -T.FREQ_CLAMP), T.FREQ_CLAMP)
+            assert int(ep["carr_step"]) == (F >> 10) + (e >> 16)
 
         def call(s, lo, hi, me):
             buf = iq[2 * (lo - base):2 * (hi - base)]

@@ -51,8 +51,9 @@ def excess_bits(v, keep):
 
 
 def angle(x, y):
-    """Angle of (x, y), x >= 0, in 2^-32 turns: both shifted to 30 bits, 24 CORDIC vectoring steps."""
+    """Angle of (x, y), x >= 0, in 2^-32 turns: both shifted to 30 bits, 24 CORDIC vectoring steps; 0 for (0, 0)."""
     x, y = np.asarray(x, np.int64).copy(), np.asarray(y, np.int64).copy()
+    zero = (x == 0) & (y == 0)
     s = excess_bits(np.maximum(x, np.abs(y)), 30)
     x, y = x >> s, y >> s
     z = np.zeros(x.shape, np.int64)
@@ -60,7 +61,7 @@ def angle(x, y):
         xs, ys = x >> i, y >> i
         pos = y > 0
         x, y, z = np.where(pos, x + ys, x - ys), np.where(pos, y - xs, y + xs), np.where(pos, z + a, z - a)
-    return z
+    return np.where(zero, 0, z)
 
 
 def code_step_of(w, D=0):
