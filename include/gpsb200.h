@@ -1112,6 +1112,129 @@ int gpsb200_collective_device(gpsb200_ctx_t *ctx, const void *iq_device, int64_t
                               gpsb200_acq_result_t *res, gpsb200_acq_result_t *seed, gpsb200_collective_t *out,
                               gpsb200_cd_score_t *scores, gpsb200_cd_cell_t *table, void *stream);
 
+/* ---- vector tracking: every channel's NCOs commanded by one navigation filter (DESIGN §10.1; tests/vtrack_model.py
+ * states it in numpy). Spilker 1996; Lashley, Bevly & Hung, IEEE J-STSP 3(4), 2009. A channel needs no acquisition and
+ * no loop of its own: the filter predicts its code phase and Doppler, and its discriminators feed back only a correction.
+ * Constants: C = 299792458 m/s, FS = 3e6, lambda_chip = C / 1.023e6, lambda = C / 1575.42e6, OMEGA_E as gpsb200_pvt;
+ * integer pieces (samples, tables, wipe-off, replicas, M, H, angle(), dll(), code_step(), "/" truncating) are the
+ * gpsb200_track header's.
+ *   seed       gpsb200_vtrack_seed: filter state X = (x, y, z, vx, vy, vz, b, d) (ECEF m, m/s, clock bias m, drift m/s)
+ *              at stream sample s0 whose true receive time is t_rx; t0 = t_rx + b / C (receive time by the receiver
+ *              clock); P = diag(sp^2, sp^2, sp^2, sv^2, sv^2, sv^2, sb^2, sd^2) from the config; channels unseeded.
+ *   predict    channel c at stream sample s (s >= s0) from X at filter sample t_f (FP64, this order): dt = (s - t_f) / FS,
+ *              r = X[0..2] + X[3..5] dt, b = X[6] + X[7] dt; q = floor((s - s0) / 3000), m = s - s0 - 3000 q,
+ *              t = t0 + q / 1000 + m / FS - b / C; tau = 0.075, three times: satellite(eph, t - tau) (gpsb200_pvt's,
+ *              position p, velocity v, clock dt_sv, drift ddt), p and v turned about z by OMEGA_E tau, l = p_rot - r,
+ *              tau = |l| / C. Code phase phi (chips) = 1023 frac(F0 + m / 3000 + 1000 (dt_sv - tau - b / C)),
+ *              F0 = frac(1000 t0), frac(x) = x - floor(x); unit vector e = l / |l|; range rate
+ *              rr = e . (v_rot - X[3..5]) - C ddt + X[7]; Doppler f = -rr / lambda.
+ *   command    from X at a channel's period start s with NCO code phase phi' (2^-32 chips): w = (int32) llround(f 2^32 /
+ *              FS), f clamped to +-10 kHz; err = phi 2^32 - phi' wrapped into [-M/2, M/2), llround to int64; u =
+ *              clamp(NOM + w / 1540 + err / (3000 N), MIN, MAX). The code correction goes only through u, so every
+ *              period keeps 2999..3001 samples and the epochs run on without a jump.
+ *   first      an unseeded call starts each channel at s0 from X: w as above, u = code_step(w), phi0 = llround(phi 2^32)
+ *              mod M; its first period starts where the code wraps: s0 + ceil((M - phi0) / u) with phi' = phi0 + that
+ *              many u - M (s0 and phi0 itself when phi0 = 0); theta = 0. The filter sample t_f = s0.
+ *   periods    per channel exactly gpsb200_track's (sums E_I..L_Q, L, theta, phi, the epoch record) with u and w held
+ *              for the whole interval; the record's lock is 1 when the channel was used at the last update. Also
+ *              S = sum_{m<L} I^2 + Q^2 of the reduced samples (int32: <= 3001 * 32768).
+ *   interval   N periods per channel. Sums over them (int64, exact): E = sum E_I^2 + E_Q^2, L likewise, P = sum P_I^2
+ *              + P_Q^2, S = sum S; over the N - 1 pairs of consecutive prompts inside the interval, dot and cross as
+ *              gpsb200_track's FLL forms and folds them. Bounds (N <= 100): E, L, P <= 100 * 1.85e16; S <= 9.9e9;
+ *              |dot|, |cross| <= 99 * 1.85e16; all below 2^63.
+ *   update     once every channel has N periods (the call stops instead when some channel's next period leaves the
+ *              buffer first, or max_updates updates ran). t_f' = the largest channel end sample; time update to t_f'
+ *              with F (r += v dt, b += d dt) and the constant-velocity / two-state clock process noise, per axis
+ *              [[qa dt^3/3, qa dt^2/2], [qa dt^2/2, qa dt]], clock [[qb dt + qd dt^3/3, qd dt^2/2], [qd dt^2/2, qd dt]]:
+ *              P = F P F^T + Q. Per channel c at its end sample s_c, with predict at that X: power ratio
+ *              q = P / (GPSB200_VTRK_NOISE_SCALE S) (0 when S = 0; about 1 + C/N0 x 1 ms); used when q >= q_min;
+ *              D = dll(E, L); du = u - code_step(w); code residual r = wrap_[-511.5, 511.5)(phi'/2^32 + D / 65536 -
+ *              du n / 2^33 - phi) chips (n = the interval's samples; D / 65536 chips is the signal's mean lead on
+ *              the replica, du n / 2 what the correction added by the end); innovation y_c = -lambda_chip r,
+ *              row (-e, 0, 0, 0, 1, 0); a = angle(dot, cross), f_m = w FS / 2^32 + a 1000 / 2^32 Hz, innovation
+ *              y_r = -lambda f_m - rr, row (0, 0, 0, -e, 0, 1); variances sc^2 / ((q - 1) N) and sr^2 / ((q - 1) N).
+ *              Sequential scalar updates at the used channels in channel order, code before rate: y' = y - row .
+ *              (X - X_prior), g = P row^T, s = row . g + var, K = g / s, X += K y', P -= K g^T (every sum in index
+ *              order). Then every channel is commanded from the new X at its end sample; its sums restart.
+ *   outputs    per update a gpsb200_fix_t (sample t_f'; status OK with 4 or more used channels, else FEW; iterations
+ *              1; the position, velocity and clock are the filter's, also when FEW: unlike gpsb200_pvt's record, a FEW
+ *              vector fix holds the state the filter coasts on, not NaN; t_rx = t0 + (t_f' - s0) / FS - b / C; PDOP from
+ *              the used code rows as gpsb200_pvt's, NaN when FEW; rms of the post-fit code residuals y_c - row .
+ *              (X - X_prior) of the used channels) and a gpsb200_vtrack_chan_t per channel.
+ * The state carries everything, so any cut of a run into calls gives the run of one call bit for bit. */
+#define GPSB200_VTRK_MAX_PERIODS 100
+#define GPSB200_VTRK_NOISE_SCALE 62500.0     /* 250^2: the carrier table's nominal squared modulus */
+typedef struct gpsb200_vtrack_config {
+    int32_t periods;       /* N: 1..GPSB200_VTRK_MAX_PERIODS */
+    int32_t reserved;      /* 0 */
+    double sigma_code_m;   /* sc > 0: sigma of a code measurement at q - 1 = 1 and N = 1 */
+    double sigma_rate_mps; /* sr > 0 */
+    double q_min;          /* > 1 */
+    double accel_psd;      /* qa >= 0, m^2/s^3 per axis */
+    double bias_psd;       /* qb >= 0, m^2/s */
+    double drift_psd;      /* qd >= 0, m^2/s^3 */
+    double sigma_pos, sigma_vel, sigma_bias, sigma_drift;   /* sp, sv, sb, sd > 0: the seed's P */
+} gpsb200_vtrack_config_t; /* 88 bytes */
+typedef struct gpsb200_vtrack_chan_state {
+    gpsb200_track_state_t nco;   /* prn, sample (next period), code / carrier NCO, code_step u, carr_step w, epochs */
+    int64_t start;         /* first sample of the interval */
+    int64_t e, l, p, s, dot, cross;   /* the interval's sums so far */
+    int32_t k;             /* periods of the interval so far, 0..N */
+    int32_t used;          /* used at the last update */
+} gpsb200_vtrack_chan_state_t;  /* 128 bytes */
+typedef struct gpsb200_vtrack_state {
+    int64_t s0;            /* the seed's sample */
+    double t0;             /* receive time by the receiver clock at s0, s of week */
+    int32_t nchan;         /* 1..GPSB200_TRK_MAX_CHAN */
+    int32_t seeded;        /* 0 until the first call starts the channels */
+    int32_t updates;       /* filter updates so far */
+    int32_t reserved;
+    int64_t t_f;           /* the sample X holds at */
+    double x[8];
+    double P[64];          /* row major */
+    gpsb200_vtrack_chan_state_t ch[GPSB200_TRK_MAX_CHAN];
+} gpsb200_vtrack_state_t;  /* 4712 bytes */
+typedef struct gpsb200_vtrack_chan {
+    int64_t sample;        /* the channel's end sample s_c of the interval */
+    int64_t e, l, p, s, dot, cross;   /* the interval's sums */
+    int32_t prn;
+    int32_t used;
+    uint32_t code_step;    /* u commanded for the next interval */
+    int32_t carr_step;     /* w commanded for the next interval */
+    double q;              /* power ratio */
+    double code_res_m;     /* innovation y_c (m) */
+    double rate_res_mps;   /* innovation y_r (m/s) */
+    double sigma_code_m;   /* sqrt of the variances (inf when not used) */
+    double sigma_rate_mps;
+} gpsb200_vtrack_chan_t;   /* 112 bytes */
+/* Fill the config with the defaults (N 20, sc 50 m, sr 10 m/s, q_min 1.2, qa 1, qb 0.1, qd 0.01, sp 100 m, sv 1 m/s,
+ * sb 10 m, sd 1 m/s). */
+void gpsb200_vtrack_config_default(gpsb200_vtrack_config_t *cfg);
+/* The seed (see above): x8 = X, t_rx at stream sample s0 (>= 0), nchan PRNs (1..32). GPSB200_ERR_ARG on a bad argument
+ * (NULL pointers, nchan out of range, a non-finite X or t_rx outside [0, 604800), the config's sigmas). Host only. */
+int gpsb200_vtrack_seed(const gpsb200_vtrack_config_t *cfg, const double *x8, double t_rx, int64_t s0,
+                        const int32_t *prn, int nchan, gpsb200_vtrack_state_t *state);
+/* Vector-track state->nchan channels over nsamples samples of host memory (int8 / int16 I,Q interleaved; stream sample
+ * `base` first; s0 and every channel's sample >= base). chans [nchan]: the ephemeris of each channel (chans[c].prn must
+ * be the channel's PRN, eph.valid; anchors not read). state in and out. fixes [max_updates] and out [max_updates][nchan]
+ * get the updates (*nupdates of them, max_updates >= 1). epochs (NULL: not wanted) [nchan][max_epochs] and nepochs
+ * [nchan] get each channel's period records; max_epochs >= (max_updates + 1) N. Every argument is checked before
+ * anything is enqueued (GPSB200_ERR_ARG). Blocking. */
+int gpsb200_vtrack(gpsb200_ctx_t *ctx, const void *iq, int64_t nsamples, int sample_size, int64_t base,
+                   const gpsb200_pvt_chan_t *chans, const gpsb200_vtrack_config_t *cfg, gpsb200_vtrack_state_t *state,
+                   int max_updates, gpsb200_fix_t *fixes, gpsb200_vtrack_chan_t *out, int32_t *nupdates,
+                   gpsb200_track_epoch_t *epochs, int max_epochs, int32_t *nepochs);
+/* Same for a source in device memory (16-byte aligned), tracked in place on `stream` (0 = the context's own stream)
+ * behind whatever it holds; returns when the outputs are in host memory. */
+int gpsb200_vtrack_device(gpsb200_ctx_t *ctx, const void *iq_device, int64_t nsamples, int sample_size, int64_t base,
+                          const gpsb200_pvt_chan_t *chans, const gpsb200_vtrack_config_t *cfg,
+                          gpsb200_vtrack_state_t *state, int max_updates, gpsb200_fix_t *fixes,
+                          gpsb200_vtrack_chan_t *out, int32_t *nupdates, gpsb200_track_epoch_t *epochs, int max_epochs,
+                          int32_t *nepochs, void *stream);
+/* Test hook: the cluster size (CTAs, 1..16) of later vector-tracking calls of this context; 0 restores the automatic
+ * choice (min(nchan, 8)). Channel c runs on CTA c mod K; no choice changes a result. GPSB200_ERR_ARG otherwise. */
+int gpsb200_debug_vtrack_cluster(gpsb200_ctx_t *ctx, int ctas);
+
 /* ---- scenario engine: the reference's host path outside the sample loop -------------
  * RINEX-2/3 navigation file (plain or gzip-compressed, read through zlib like the reference, gps.c:1147) +
  * location/motion -> the gpsb200_chan_t records and NAV frames the

@@ -24,6 +24,7 @@ from .api import (  # noqa: F401
     snapshot_config, SNAP_BATCH_SCRATCH, snapshot_batch_pass,
     COLLECTIVE_CONFIG_DTYPE, COLLECTIVE_DTYPE, CD_SCORE_DTYPE, CD_CELL_DTYPE, CD_OK, CD_FEW, CD_AMBIGUOUS, CD_MAX_HYP,
     CD_MIN_USED, CD_Q_SHIFT, CD_Q_CAP, CD_AMBIGUOUS_PCT, collective_config,
+    VTRACK_CONFIG_DTYPE, VTRACK_CHAN_STATE_DTYPE, VTRACK_STATE_DTYPE, VTRACK_CHAN_DTYPE, vtrack_config, vtrack_seed,
 )
 from .synthetic import synthetic_chans  # noqa: F401,E402
 from . import sharding  # noqa: F401,E402

@@ -139,6 +139,29 @@ NAV_SYNC_DTYPE = np.dtype([("bit_edge", "<i4"), ("nbits", "<i4"), ("frame_bit", 
 assert NAV_BIT_DTYPE.itemsize == 24 and NAV_WORD_DTYPE.itemsize == 32 and NAV_SYNC_DTYPE.itemsize == 32
 
 
+def vtrack_config(**kw):
+    """gpsb200_vtrack_config_default with the fields of kw replaced. -> VTRACK_CONFIG_DTYPE record."""
+    c = np.zeros(1, VTRACK_CONFIG_DTYPE)
+    lib().gpsb200_vtrack_config_default(c.ctypes.data)
+    for k, v in kw.items():
+        c[0][k] = v
+    return c[0]
+
+
+def vtrack_seed(cfg, x8, t_rx, s0, prns):
+    """gpsb200_vtrack_seed: the state of a run from X = (x, y, z, vx, vy, vz, b, d) at stream sample s0 whose true
+    receive time is t_rx (s of week), one channel per PRN. -> VTRACK_STATE_DTYPE record."""
+    st = np.zeros(1, VTRACK_STATE_DTYPE)
+    cf = np.array(cfg, dtype=VTRACK_CONFIG_DTYPE).reshape(1)
+    x = np.ascontiguousarray(x8, np.float64)
+    p = np.ascontiguousarray(prns, np.int32)
+    rc = lib().gpsb200_vtrack_seed(cf.ctypes.data, x.ctypes.data, float(t_rx), int(s0), p.ctypes.data, p.size,
+                                   st.ctypes.data)
+    if rc:
+        raise GpsB200Error(rc, "gpsb200_vtrack_seed")
+    return st[0]
+
+
 def track_start(prn, doppler_hz, sample):
     """gpsb200_track_start: the tracking state of a channel from an acquisition (prn, Doppler, the sample where the
     code's chip 0 starts: s0 + delay). -> TRACK_STATE_DTYPE record."""
@@ -195,6 +218,22 @@ FIX_DTYPE = np.dtype([("sample", "<i8"), ("status", "<i4"), ("nused", "<i4"), ("
 assert (EPHEMERIS_DTYPE.itemsize, IONO_DTYPE.itemsize, PVT_CHAN_DTYPE.itemsize, PVT_CONFIG_DTYPE.itemsize,
         FIX_DTYPE.itemsize) == (200, 72, 216, 88, 136)
 FIX_OK, FIX_FEW, FIX_NO_CONVERGENCE = 0, 1, 2
+VTRACK_CONFIG_DTYPE = np.dtype([("periods", "<i4"), ("reserved", "<i4"), ("sigma_code_m", "<f8"),
+                                ("sigma_rate_mps", "<f8"), ("q_min", "<f8"), ("accel_psd", "<f8"), ("bias_psd", "<f8"),
+                                ("drift_psd", "<f8"), ("sigma_pos", "<f8"), ("sigma_vel", "<f8"), ("sigma_bias", "<f8"),
+                                ("sigma_drift", "<f8")])
+VTRACK_CHAN_STATE_DTYPE = np.dtype([("nco", TRACK_STATE_DTYPE), ("start", "<i8"), ("e", "<i8"), ("l", "<i8"),
+                                    ("p", "<i8"), ("s", "<i8"), ("dot", "<i8"), ("cross", "<i8"), ("k", "<i4"),
+                                    ("used", "<i4")])
+VTRACK_STATE_DTYPE = np.dtype([("s0", "<i8"), ("t0", "<f8"), ("nchan", "<i4"), ("seeded", "<i4"), ("updates", "<i4"),
+                               ("reserved", "<i4"), ("t_f", "<i8"), ("x", "<f8", 8), ("P", "<f8", (8, 8)),
+                               ("ch", VTRACK_CHAN_STATE_DTYPE, 32)])
+VTRACK_CHAN_DTYPE = np.dtype([("sample", "<i8"), ("e", "<i8"), ("l", "<i8"), ("p", "<i8"), ("s", "<i8"),
+                              ("dot", "<i8"), ("cross", "<i8"), ("prn", "<i4"), ("used", "<i4"), ("code_step", "<u4"),
+                              ("carr_step", "<i4"), ("q", "<f8"), ("code_res_m", "<f8"), ("rate_res_mps", "<f8"),
+                              ("sigma_code_m", "<f8"), ("sigma_rate_mps", "<f8")])
+assert (VTRACK_CONFIG_DTYPE.itemsize, VTRACK_CHAN_STATE_DTYPE.itemsize, VTRACK_STATE_DTYPE.itemsize,
+        VTRACK_CHAN_DTYPE.itemsize) == (88, 128, 4712, 112)
 PVT_MAX_ITER = 12
 
 # gpsb200_raim_config_t / gpsb200_raim_t (DESIGN §11.1)
@@ -457,7 +496,7 @@ EXPORTS = ["gpsb200_create", "gpsb200_destroy", "gpsb200_last_error", "gpsb200_v
            "gpsb200_track",
            "gpsb200_track_device", "gpsb200_nav_decode", "gpsb200_nav_word_check", "gpsb200_nav_parity",
            "gpsb200_nav_ephemeris", "gpsb200_nav_time_anchor", "gpsb200_pvt", "gpsb200_pvt_replay",
-           "gpsb200_pvt_raim", "gpsb200_raim_thresholds", "gpsb200_pvt_araim", "gpsb200_araim_kfa", "gpsb200_pvt_coarse", "gpsb200_pvt_search", "gpsb200_search_nodes", "gpsb200_snapshot_measure", "gpsb200_snapshot_measure_device", "gpsb200_snapshot_batch", "gpsb200_snapshot_batch_device", "gpsb200_pvt_snapshot", "gpsb200_pvt_snapshot_search", "gpsb200_collective", "gpsb200_collective_device", "gpsb200_rinex_ephemeris", "gpsb200_bind_numa", "gpsb200_span_chain_host", "gpsb200_lanes_model_block",
+           "gpsb200_pvt_raim", "gpsb200_raim_thresholds", "gpsb200_pvt_araim", "gpsb200_araim_kfa", "gpsb200_pvt_coarse", "gpsb200_pvt_search", "gpsb200_search_nodes", "gpsb200_snapshot_measure", "gpsb200_snapshot_measure_device", "gpsb200_snapshot_batch", "gpsb200_snapshot_batch_device", "gpsb200_pvt_snapshot", "gpsb200_pvt_snapshot_search", "gpsb200_collective", "gpsb200_collective_device", "gpsb200_vtrack_config_default", "gpsb200_vtrack_seed", "gpsb200_vtrack", "gpsb200_vtrack_device", "gpsb200_debug_vtrack_cluster", "gpsb200_rinex_ephemeris", "gpsb200_bind_numa", "gpsb200_span_chain_host", "gpsb200_lanes_model_block",
            "gpsb200_lanes_window_band_host", "gpsb200_slice_prepare", "gpsb200_slice_probe",
            "gpsb200_slice_finish", "gpsb200_slice_finish_cb", "gpsb200_slice_wait", "gpsb200_link_apply", "gpsb200_slice_link_host", "gpsb200_debug_corrupt_chain", "gpsb200_synth_kernel_name",
            "gpsb200_debug_run_checkpoints", "gpsb200_checkpoint_segments_host",
@@ -590,6 +629,14 @@ def lib():
                                          C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                          C.c_void_p, C.c_void_p]
         L.gpsb200_collective_device.argtypes = L.gpsb200_collective.argtypes + [C.c_void_p]
+        L.gpsb200_vtrack_config_default.argtypes = [C.c_void_p]
+        L.gpsb200_vtrack_config_default.restype = None
+        L.gpsb200_vtrack_seed.argtypes = [C.c_void_p, C.c_void_p, C.c_double, C.c_int64, C.c_void_p, C.c_int, C.c_void_p]
+        L.gpsb200_vtrack.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_int64, C.c_void_p, C.c_void_p,
+                                     C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int,
+                                     C.c_void_p]
+        L.gpsb200_vtrack_device.argtypes = L.gpsb200_vtrack.argtypes + [C.c_void_p]
+        L.gpsb200_debug_vtrack_cluster.argtypes = [C.c_void_p, C.c_int]
         L.gpsb200_rinex_ephemeris.argtypes = [C.c_char_p, C.c_int, C.c_int32, C.c_double, C.c_void_p]
         _lib = L
     return _lib
@@ -1153,6 +1200,37 @@ class Context:
         self._check(fn(self._h, src, n, int(sample_size), int(base), st.ctypes.data, nchan, me, out.ctypes.data,
                        cnt.ctypes.data, *dev))
         return [out[c, :cnt[c]].copy() for c in range(nchan)], st
+
+    def vtrack(self, chans, cfg, state, max_updates, iq=None, sample_size=SC08, base=0, want_epochs=False,
+               device_ptr=None, nsamples=None, stream=0):
+        """Vector tracking (gpsb200_vtrack; DESIGN §10.1) of the channels of `state` (VTRACK_STATE_DTYPE, e.g. from
+        vtrack_seed) with the ephemerides chans (PVT_CHAN_DTYPE[nchan]) and the config cfg (vtrack_config), over a
+        buffer whose first sample is the stream's sample `base` (source as for track), at most max_updates filter
+        updates. -> (fixes FIX_DTYPE[n], VTRACK_CHAN_DTYPE[n][nchan], epochs (a list of TRACK_EPOCH_DTYPE arrays per
+        channel, or None), state after the call)."""
+        st = np.array(state, dtype=VTRACK_STATE_DTYPE).reshape(()).copy()
+        ch = np.ascontiguousarray(chans, dtype=PVT_CHAN_DTYPE)
+        cf = np.array(cfg, dtype=VTRACK_CONFIG_DTYPE).reshape(()).copy()
+        nchan = int(st["nchan"])
+        src, n, dev = self._rx_source(iq, device_ptr, nsamples, stream)
+        mu = int(max_updates)
+        fixes = np.zeros(max(1, mu), FIX_DTYPE)
+        out = np.zeros((max(1, mu), max(1, nchan)), VTRACK_CHAN_DTYPE)
+        nu = np.zeros(1, np.int32)
+        me = (mu + 1) * int(cf["periods"]) if want_epochs else 0
+        ep = np.zeros((max(1, nchan), max(1, me)), TRACK_EPOCH_DTYPE) if want_epochs else None
+        cnt = np.zeros(max(1, nchan), np.int32)
+        fn = lib().gpsb200_vtrack_device if dev else lib().gpsb200_vtrack
+        self._check(fn(self._h, src, n, int(sample_size), int(base), ch.ctypes.data, cf.ctypes.data, st.ctypes.data, mu,
+                       fixes.ctypes.data, out.ctypes.data, nu.ctypes.data, ep.ctypes.data if want_epochs else None, me,
+                       cnt.ctypes.data, *dev))
+        k = int(nu[0])
+        eps = [ep[c, :cnt[c]].copy() for c in range(nchan)] if want_epochs else None
+        return fixes[:k].copy(), out[:k, :nchan].copy(), eps, st
+
+    def debug_vtrack_cluster(self, ctas):
+        """gpsb200_debug_vtrack_cluster: the CTAs of the cluster of later vector-tracking calls (0: automatic)."""
+        self._check(lib().gpsb200_debug_vtrack_cluster(self._h, int(ctas)))
 
     def pvt(self, chans, epochs, cfg, want_residuals=False, nepochs=None):
         """Position, velocity and time fixes (gpsb200_pvt; DESIGN §11). chans: PVT_CHAN_DTYPE[nchan] (ephemeris and time

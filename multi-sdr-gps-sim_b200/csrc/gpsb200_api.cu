@@ -33,6 +33,7 @@
 #include "collective.h"
 #include "device_buffer.h"
 #include "track.h"
+#include "vtrack.h"
 #include "pvt.h"
 #include "nco_exact.h"
 #include "synth_kernels.h"
@@ -219,6 +220,8 @@ struct gpsb200_ctx {
     pvt::Scratch pvt;                      // position fixes (pvt.cu), allocated by the first one
     snap::Scratch snap;                    // snapshot measurements (snapshot.cu), allocated by the first one
     cd::Scratch cd;                        // collective detection (collective.cu), allocated by the first one
+    vtk::Scratch vtk;                      // vector tracking (vtrack.cu), allocated by the first one
+    int vtk_ctas = 0;                      // gpsb200_debug_vtrack_cluster (0: automatic)
     std::string err;
 };
 
@@ -1151,6 +1154,27 @@ int track(gpsb200_ctx *ctx, const void *iq, int64_t nsamples, int sample_size, i
     return GPSB200_OK;
 }
 
+// The vector tracking of both entry points (vtrack.cu). Everything is checked before anything is enqueued.
+int vtrack(gpsb200_ctx *ctx, const void *iq, int64_t nsamples, int sample_size, int64_t base,
+           const gpsb200_pvt_chan_t *chans, const gpsb200_vtrack_config_t *cfg, gpsb200_vtrack_state_t *state,
+           int max_updates, gpsb200_fix_t *fixes, gpsb200_vtrack_chan_t *out, int32_t *nupdates,
+           gpsb200_track_epoch_t *epochs, int max_epochs, int32_t *nepochs, bool device, cudaStream_t s) {
+    const char *name = device ? "gpsb200_vtrack_device" : "gpsb200_vtrack";
+    if (!iq || !fixes || !out || !nupdates || (epochs && !nepochs))
+        return fail(ctx, GPSB200_ERR_ARG, std::string(name) + ": NULL source, fixes, out, nupdates or nepochs");
+    const std::string bad = vtk::check(state, chans, cfg, max_updates, epochs != nullptr, max_epochs, nsamples, base,
+                                       sample_size);
+    if (!bad.empty()) return fail(ctx, GPSB200_ERR_ARG, std::string(name) + ": " + bad);
+    const void *src;
+    const int rc = rx_source(ctx, name, iq, 0, nsamples, sample_size, device, s, &src);
+    if (rc) return rc;
+    if (!ctx->d_rx_chips) CU(trk::chips_upload(&ctx->d_rx_chips));
+    CU(vtk::scratch_reserve(ctx->vtk, state->nchan, max_updates, epochs ? max_epochs : 0));
+    CU(vtk::launch(ctx->vtk, ctx->d_rx_chips, src, nsamples, sample_size, base, chans, cfg, state, max_updates, fixes,
+                   out, nupdates, epochs, max_epochs, nepochs, ctx->vtk_ctas, s));
+    return GPSB200_OK;
+}
+
 // The snapshot measurement of both entry points (snapshot.cu). Everything is checked before anything is enqueued.
 int snapshot_measure(gpsb200_ctx *ctx, const void *iq, int64_t nsamples, int sample_size, const gpsb200_acq_config_t *acq,
                      const gpsb200_acq_result_t *res, const gpsb200_snapshot_config_t *cfg, gpsb200_snapshot_t *out,
@@ -1586,6 +1610,7 @@ void gpsb200_destroy(gpsb200_ctx_t *ctx) {
     trk::scratch_free(ctx->trk);
     snap::scratch_free(ctx->snap);
     cd::scratch_free(ctx->cd);
+    vtk::scratch_free(ctx->vtk);
     pvt::scratch_free(ctx->pvt);
     if (ctx->s_compute) cudaStreamDestroy(ctx->s_compute);
     if (ctx->s_copy) cudaStreamDestroy(ctx->s_copy);
@@ -1867,6 +1892,70 @@ int gpsb200_track_device(gpsb200_ctx_t *ctx, const void *iq_device, int64_t nsam
     cudaStream_t s = caller_stream(ctx, stream_);
     return settle(ctx, s, track(ctx, iq_device, nsamples, sample_size, base, state, nchan, max_epochs, epochs, nepochs,
                                 true, s));
+}
+
+void gpsb200_vtrack_config_default(gpsb200_vtrack_config_t *cfg) {
+    if (!cfg) return;
+    memset(cfg, 0, sizeof *cfg);
+    cfg->periods = 20;
+    cfg->sigma_code_m = 50.0;
+    cfg->sigma_rate_mps = 10.0;
+    cfg->q_min = 1.2;
+    cfg->accel_psd = 1.0;
+    cfg->bias_psd = 0.1;
+    cfg->drift_psd = 0.01;
+    cfg->sigma_pos = 100.0;
+    cfg->sigma_vel = 1.0;
+    cfg->sigma_bias = 10.0;
+    cfg->sigma_drift = 1.0;
+}
+
+int gpsb200_vtrack_seed(const gpsb200_vtrack_config_t *cfg, const double *x8, double t_rx, int64_t s0,
+                        const int32_t *prn, int nchan, gpsb200_vtrack_state_t *st) {
+    if (!x8 || !prn || !st || nchan < 1 || nchan > GPSB200_TRK_MAX_CHAN || s0 < 0 || !(t_rx >= 0.0 && t_rx < 604800.0))
+        return GPSB200_ERR_ARG;
+    if (!vtk::check_config(cfg).empty()) return GPSB200_ERR_ARG;
+    for (int i = 0; i < 8; i++)
+        if (!std::isfinite(x8[i])) return GPSB200_ERR_ARG;
+    for (int c = 0; c < nchan; c++)
+        if (prn[c] < 1 || prn[c] > 32) return GPSB200_ERR_ARG;
+    memset(st, 0, sizeof *st);
+    st->s0 = s0;
+    st->t_f = s0;
+    st->nchan = nchan;
+    st->t0 = t_rx + x8[6] / 2.99792458e8;
+    for (int i = 0; i < 8; i++) st->x[i] = x8[i];
+    const double sd[8] = {cfg->sigma_pos, cfg->sigma_pos, cfg->sigma_pos, cfg->sigma_vel,
+                          cfg->sigma_vel, cfg->sigma_vel, cfg->sigma_bias, cfg->sigma_drift};
+    for (int i = 0; i < 8; i++) st->P[i * 9] = sd[i] * sd[i];
+    for (int c = 0; c < nchan; c++) st->ch[c].nco.prn = prn[c];
+    return GPSB200_OK;
+}
+
+int gpsb200_vtrack(gpsb200_ctx_t *ctx, const void *iq, int64_t nsamples, int sample_size, int64_t base,
+                   const gpsb200_pvt_chan_t *chans, const gpsb200_vtrack_config_t *cfg, gpsb200_vtrack_state_t *state,
+                   int max_updates, gpsb200_fix_t *fixes, gpsb200_vtrack_chan_t *out, int32_t *nupdates,
+                   gpsb200_track_epoch_t *epochs, int max_epochs, int32_t *nepochs) {
+    if (!ctx) return GPSB200_ERR_ARG;
+    return settle(ctx, nullptr, vtrack(ctx, iq, nsamples, sample_size, base, chans, cfg, state, max_updates, fixes, out,
+                                       nupdates, epochs, max_epochs, nepochs, false, ctx->s_compute));
+}
+
+int gpsb200_vtrack_device(gpsb200_ctx_t *ctx, const void *iq_device, int64_t nsamples, int sample_size, int64_t base,
+                          const gpsb200_pvt_chan_t *chans, const gpsb200_vtrack_config_t *cfg,
+                          gpsb200_vtrack_state_t *state, int max_updates, gpsb200_fix_t *fixes,
+                          gpsb200_vtrack_chan_t *out, int32_t *nupdates, gpsb200_track_epoch_t *epochs, int max_epochs,
+                          int32_t *nepochs, void *stream_) {
+    if (!ctx) return GPSB200_ERR_ARG;
+    cudaStream_t s = caller_stream(ctx, stream_);
+    return settle(ctx, s, vtrack(ctx, iq_device, nsamples, sample_size, base, chans, cfg, state, max_updates, fixes, out,
+                                 nupdates, epochs, max_epochs, nepochs, true, s));
+}
+
+int gpsb200_debug_vtrack_cluster(gpsb200_ctx_t *ctx, int ctas) {
+    if (!ctx || ctas < 0 || ctas > vtk::kMaxCluster) return GPSB200_ERR_ARG;
+    ctx->vtk_ctas = ctas;
+    return GPSB200_OK;
 }
 
 int gpsb200_pvt(gpsb200_ctx_t *ctx, const gpsb200_pvt_chan_t *chans, int nchan, const gpsb200_track_epoch_t *epochs,
