@@ -417,18 +417,18 @@ std::string check(const gpsb200_acq_config_t *cfg, int64_t nsamples, int sample_
 }
 
 cudaError_t scratch_reserve(Scratch &sc, const gpsb200_acq_config_t *cfg, bool windows, bool want_grid) {
-    if (!sc.d_edges) {
+    CU_RET(sc.d_edges.grow((size_t) 33 * kMaxEdges));
+    CU_RET(sc.d_nedges.grow(33));
+    CU_RET(sc.d_res.grow(32));
+    CU_RET(sc.h_res.grow(32));
+    CU_RET(sc.d_prn.grow(32));
+    CU_RET(sc.d_flo.grow(32));
+    if (!sc.ready) {
         std::vector<int16_t> e((size_t) 33 * kMaxEdges, 0);
         std::vector<int32_t> n(33, 0);
         for (int prn = 1; prn <= 32; prn++) n[prn] = replica_edges(prn, e.data() + (size_t) prn * kMaxEdges);
-        CU_RET(cudaMalloc(&sc.d_edges, e.size() * sizeof(int16_t)));
-        CU_RET(cudaMemcpy(sc.d_edges, e.data(), e.size() * sizeof(int16_t), cudaMemcpyHostToDevice));
-        CU_RET(cudaMalloc(&sc.d_nedges, n.size() * sizeof(int32_t)));
-        CU_RET(cudaMemcpy(sc.d_nedges, n.data(), n.size() * sizeof(int32_t), cudaMemcpyHostToDevice));
-        CU_RET(cudaMalloc(&sc.d_res, 32 * sizeof(gpsb200_acq_result_t)));
-        CU_RET(cudaHostAlloc(&sc.h_res, 32 * sizeof(gpsb200_acq_result_t), cudaHostAllocDefault));
-        CU_RET(cudaMalloc(&sc.d_prn, 32 * sizeof(int32_t)));
-        CU_RET(cudaMalloc(&sc.d_flo, 32 * sizeof(double)));
+        CU_RET(cudaMemcpy(sc.d_edges.get(), e.data(), e.size() * sizeof(int16_t), cudaMemcpyHostToDevice));
+        CU_RET(cudaMemcpy(sc.d_nedges.get(), n.data(), n.size() * sizeof(int32_t), cudaMemcpyHostToDevice));
         for (int i = 0; i < kNumSplits; i++)
             for (GridKernel k : {kGrid<int8_t, false>[i], kGrid<int16_t, false>[i], kGrid<int8_t, true>[i],
                                  kGrid<int16_t, true>[i], kBatch<int8_t>[i], kBatch<int16_t>[i]})
@@ -436,69 +436,58 @@ cudaError_t scratch_reserve(Scratch &sc, const gpsb200_acq_config_t *cfg, bool w
         int dev = 0;
         CU_RET(cudaGetDevice(&dev));
         CU_RET(cudaDeviceGetAttribute(&sc.sms, cudaDevAttrMultiProcessorCount, dev));
+        sc.ready = true;
     }
-    CU_RET(grow(sc.d_rows, sc.rows_cap, (size_t) 32 * cfg->nbins * 3));
-    CU_RET(grow(sc.d_u, sc.u_cap, (size_t) (windows ? cfg->nprn : 1) * cfg->nbins));
+    CU_RET(sc.d_rows.grow((size_t) 32 * cfg->nbins * 3));
+    CU_RET(sc.d_u.grow((size_t) (windows ? cfg->nprn : 1) * cfg->nbins));
     if (want_grid || split_of(sc, cfg->nprn, cfg->nbins) > 1)
-        CU_RET(grow(sc.d_grid, sc.grid_cap, (size_t) cfg->nprn * cfg->nbins * kCode));
+        CU_RET(sc.d_grid.grow((size_t) cfg->nprn * cfg->nbins * kCode));
     return cudaSuccess;
 }
 
 cudaError_t batch_reserve(Scratch &sc, const gpsb200_acq_config_t *cfg, int nwin) {
     const size_t npair = (size_t) nwin * cfg->nprn;
     CU_RET(scratch_reserve(sc, cfg, true, false));
-    CU_RET(grow(sc.d_rows, sc.rows_cap, npair * cfg->nbins * 3));
-    CU_RET(grow(sc.d_u, sc.u_cap, npair * cfg->nbins));
-    CU_RET(grow(sc.d_boff, sc.boff_cap, (size_t) nwin));
-    CU_RET(grow(sc.d_bprn, sc.bprn_cap, npair));
-    CU_RET(grow(sc.d_bflo, sc.bflo_cap, npair));
-    CU_RET(grow(sc.d_bres, sc.bres_cap, npair));
-    if (batch_split(sc, (int) npair, cfg->nbins) > 1) CU_RET(grow(sc.d_grid, sc.grid_cap, npair * cfg->nbins * kCode));
+    CU_RET(sc.d_rows.grow(npair * cfg->nbins * 3));
+    CU_RET(sc.d_u.grow(npair * cfg->nbins));
+    CU_RET(sc.d_boff.grow((size_t) nwin));
+    CU_RET(sc.d_bprn.grow(npair));
+    CU_RET(sc.d_bflo.grow(npair));
+    CU_RET(sc.d_bres.grow(npair));
+    if (batch_split(sc, (int) npair, cfg->nbins) > 1) CU_RET(sc.d_grid.grow(npair * cfg->nbins * kCode));
     return cudaSuccess;
-}
-
-void scratch_free(Scratch &sc) {
-    cudaFree(sc.d_boff);
-    cudaFree(sc.d_bprn);
-    cudaFree(sc.d_bflo);
-    cudaFree(sc.d_bres);
-    cudaFree(sc.d_edges);
-    cudaFree(sc.d_nedges);
-    cudaFree(sc.d_grid);
-    cudaFree(sc.d_rows);
-    cudaFree(sc.d_res);
-    cudaFreeHost(sc.h_res);
-    cudaFree(sc.d_u);
-    cudaFree(sc.d_prn);
-    cudaFree(sc.d_flo);
-    const int force = sc.force_split;
-    sc = Scratch();
-    sc.force_split = force;
 }
 
 cudaError_t launch(Scratch &sc, const void *window, int sample_size, const gpsb200_acq_config_t *cfg,
                    const double *f_lo_prn, bool want_grid, cudaStream_t s) {
     // the small parameter arrays go up by value in the stream order (the host copies are on this call's stack)
     const std::vector<uint32_t> u = phase_steps(cfg, f_lo_prn ? cfg->nprn : 1, f_lo_prn);
-    CU_RET(cudaMemcpyAsync(sc.d_u, u.data(), u.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, s));
-    CU_RET(cudaMemcpyAsync(sc.d_prn, cfg->prn, cfg->nprn * sizeof(int32_t), cudaMemcpyHostToDevice, s));
-    if (f_lo_prn) CU_RET(cudaMemcpyAsync(sc.d_flo, f_lo_prn, cfg->nprn * sizeof(double), cudaMemcpyHostToDevice, s));
+    CU_RET(cudaMemcpyAsync(sc.d_u.get(), u.data(), u.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, s));
+    CU_RET(cudaMemcpyAsync(sc.d_prn.get(), cfg->prn, cfg->nprn * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+    if (f_lo_prn)
+        CU_RET(cudaMemcpyAsync(sc.d_flo.get(), f_lo_prn, cfg->nprn * sizeof(double), cudaMemcpyHostToDevice, s));
     const int split = split_of(sc, cfg->nprn, cfg->nbins);
     const dim3 grid(cfg->nbins, cfg->nprn, split);
-    uint64_t *g = want_grid || split > 1 ? sc.d_grid : nullptr;
+    uint64_t *g = want_grid || split > 1 ? sc.d_grid.get() : nullptr;
     const GridKernel kernel = grid_kernel(sample_size, f_lo_prn != nullptr, split);
+    // cudaLaunchKernel reads each argument at the address given: these local pointer copies, never an owning array
     const void *src = window;   // either sample type: the kernels take the pointer as is
-    void *args[] = {(void *) &src, (void *) &sc.d_edges, (void *) &sc.d_nedges, (void *) &sc.d_prn, (void *) &sc.d_u,
-                    (void *) &cfg->ms, (void *) &cfg->nbins, (void *) &g, (void *) &sc.d_rows};
+    const int16_t *edges = sc.d_edges.get();
+    const int32_t *nedges = sc.d_nedges.get(), *prn = sc.d_prn.get();
+    const uint32_t *u_dev = sc.d_u.get();
+    uint64_t *rows = sc.d_rows.get();
+    void *args[] = {(void *) &src, (void *) &edges, (void *) &nedges, (void *) &prn, (void *) &u_dev,
+                    (void *) &cfg->ms, (void *) &cfg->nbins, (void *) &g, (void *) &rows};
     CU_RET(cudaLaunchKernel(kernel, grid, dim3(kThreads), args, sizeof(Smem), s));
     if (split > 1) {
-        k_acq_reduce<<<dim3(cfg->nbins, cfg->nprn), kThreads, 0, s>>>(sc.d_grid, cfg->nbins, sc.d_rows);
+        k_acq_reduce<<<dim3(cfg->nbins, cfg->nprn), kThreads, 0, s>>>(sc.d_grid.get(), cfg->nbins, rows);
         CU_RET(cudaGetLastError());
     }
-    k_acq_pick<<<cfg->nprn, 32, 0, s>>>(sc.d_rows, sc.d_prn, cfg->nbins, cfg->f_lo_hz, f_lo_prn ? sc.d_flo : nullptr,
-                                        cfg->step_hz, sc.d_res);
+    k_acq_pick<<<cfg->nprn, 32, 0, s>>>(rows, sc.d_prn.get(), cfg->nbins, cfg->f_lo_hz,
+                                        f_lo_prn ? sc.d_flo.get() : nullptr, cfg->step_hz, sc.d_res.get());
     CU_RET(cudaGetLastError());
-    CU_RET(cudaMemcpyAsync(sc.h_res, sc.d_res, cfg->nprn * sizeof(gpsb200_acq_result_t), cudaMemcpyDeviceToHost, s));
+    CU_RET(cudaMemcpyAsync(sc.h_res.get(), sc.d_res.get(), cfg->nprn * sizeof(gpsb200_acq_result_t),
+                           cudaMemcpyDeviceToHost, s));
     // pageable sources of the two uploads must outlive them: wait here (the search is blocking anyway)
     return cudaStreamSynchronize(s);
 }
@@ -509,26 +498,33 @@ cudaError_t launch_batch(Scratch &sc, const void *src, int sample_size, const gp
     std::vector<int32_t> prn((size_t) npair);
     for (int i = 0; i < npair; i++) prn[i] = cfg->prn[i % cfg->nprn];
     const std::vector<uint32_t> u = phase_steps(cfg, npair, f_lo);
-    CU_RET(cudaMemcpyAsync(sc.d_u, u.data(), u.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, s));
-    CU_RET(cudaMemcpyAsync(sc.d_bprn, prn.data(), prn.size() * sizeof(int32_t), cudaMemcpyHostToDevice, s));
-    CU_RET(cudaMemcpyAsync(sc.d_bflo, f_lo, npair * sizeof(double), cudaMemcpyHostToDevice, s));
-    CU_RET(cudaMemcpyAsync(sc.d_boff, win_off, nwin * sizeof(int64_t), cudaMemcpyHostToDevice, s));
+    CU_RET(cudaMemcpyAsync(sc.d_u.get(), u.data(), u.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, s));
+    CU_RET(cudaMemcpyAsync(sc.d_bprn.get(), prn.data(), prn.size() * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+    CU_RET(cudaMemcpyAsync(sc.d_bflo.get(), f_lo, npair * sizeof(double), cudaMemcpyHostToDevice, s));
+    CU_RET(cudaMemcpyAsync(sc.d_boff.get(), win_off, nwin * sizeof(int64_t), cudaMemcpyHostToDevice, s));
     const int split = batch_split(sc, npair, cfg->nbins);
-    uint64_t *g = split > 1 ? sc.d_grid : nullptr;
+    uint64_t *g = split > 1 ? sc.d_grid.get() : nullptr;
+    // the arguments by address, of local pointer copies as in launch
     const void *p = src;
     int nprn = cfg->nprn;
-    void *args[] = {(void *) &p, (void *) &sc.d_boff, (void *) &nprn, (void *) &sc.d_edges, (void *) &sc.d_nedges,
-                    (void *) &sc.d_bprn, (void *) &sc.d_u, (void *) &cfg->ms, (void *) &cfg->nbins, (void *) &g,
-                    (void *) &sc.d_rows};
+    const int64_t *boff = sc.d_boff.get();
+    const int16_t *edges = sc.d_edges.get();
+    const int32_t *nedges = sc.d_nedges.get(), *bprn = sc.d_bprn.get();
+    const uint32_t *u_dev = sc.d_u.get();
+    uint64_t *rows = sc.d_rows.get();
+    void *args[] = {(void *) &p, (void *) &boff, (void *) &nprn, (void *) &edges, (void *) &nedges,
+                    (void *) &bprn, (void *) &u_dev, (void *) &cfg->ms, (void *) &cfg->nbins, (void *) &g,
+                    (void *) &rows};
     CU_RET(cudaLaunchKernel(batch_kernel(sample_size, split), dim3(cfg->nbins, npair, split), dim3(kThreads), args,
                             sizeof(Smem), s));
     if (split > 1) {
-        k_acq_reduce<<<dim3(cfg->nbins, npair), kThreads, 0, s>>>(sc.d_grid, cfg->nbins, sc.d_rows);
+        k_acq_reduce<<<dim3(cfg->nbins, npair), kThreads, 0, s>>>(sc.d_grid.get(), cfg->nbins, rows);
         CU_RET(cudaGetLastError());
     }
-    k_acq_pick<<<npair, 32, 0, s>>>(sc.d_rows, sc.d_bprn, cfg->nbins, cfg->f_lo_hz, sc.d_bflo, cfg->step_hz, sc.d_bres);
+    k_acq_pick<<<npair, 32, 0, s>>>(rows, bprn, cfg->nbins, cfg->f_lo_hz, sc.d_bflo.get(), cfg->step_hz,
+                                    sc.d_bres.get());
     CU_RET(cudaGetLastError());
-    CU_RET(cudaMemcpyAsync(res, sc.d_bres, npair * sizeof(gpsb200_acq_result_t), cudaMemcpyDeviceToHost, s));
+    CU_RET(cudaMemcpyAsync(res, sc.d_bres.get(), npair * sizeof(gpsb200_acq_result_t), cudaMemcpyDeviceToHost, s));
     return cudaStreamSynchronize(s);
 }
 

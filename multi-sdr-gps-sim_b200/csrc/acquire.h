@@ -7,6 +7,7 @@
 #include <string>
 
 #include "../../include/gpsb200.h"
+#include "device_buffer.h"
 
 namespace gpsb200 {
 namespace acq {
@@ -22,25 +23,20 @@ constexpr int kExclude = 3;                    // P2 excludes delays within +-3 
 
 // Device scratch of the searches of one context, grown as needed.
 struct Scratch {
-    int16_t *d_edges = nullptr;        // [33][kMaxEdges] sign-change positions of every PRN's replica, row 0 unused
-    int32_t *d_nedges = nullptr;       // [33]
-    uint64_t *d_grid = nullptr;        // [nprn][nbins][3000] when the caller wants the grid or the search is split
-    size_t grid_cap = 0;
-    uint64_t *d_rows = nullptr;        // [nprn][nbins][3]: P1, P2, tau1 of every row
-    size_t rows_cap = 0;
-    gpsb200_acq_result_t *d_res = nullptr, *h_res = nullptr;   // [32]
-    uint32_t *d_u = nullptr;           // [nbins] phase steps; with per-PRN windows [nprn][nbins]
-    size_t u_cap = 0;
-    int32_t *d_prn = nullptr;          // [32]
-    double *d_flo = nullptr;           // [32] first bin of each PRN's window (gpsb200_acquire_windows)
-    int64_t *d_boff = nullptr;         // batches (gpsb200_snapshot_batch): [nwin] window offsets in samples,
-    size_t boff_cap = 0;
-    int32_t *d_bprn = nullptr;         // [nwin][nprn] PRN,
-    size_t bprn_cap = 0;
-    double *d_bflo = nullptr;          // [nwin][nprn] first bin
-    size_t bflo_cap = 0;
-    gpsb200_acq_result_t *d_bres = nullptr;   // and [nwin][nprn] results of every (window, PRN) pair
-    size_t bres_cap = 0;
+    DeviceArray<int16_t> d_edges;      // [33][kMaxEdges] sign-change positions of every PRN's replica, row 0 unused
+    DeviceArray<int32_t> d_nedges;     // [33]
+    DeviceArray<uint64_t> d_grid;      // [nprn][nbins][3000] when the caller wants the grid or the search is split
+    DeviceArray<uint64_t> d_rows;      // [nprn][nbins][3]: P1, P2, tau1 of every row
+    DeviceArray<gpsb200_acq_result_t> d_res;   // [32]
+    PinnedArray<gpsb200_acq_result_t> h_res;   // [32]
+    DeviceArray<uint32_t> d_u;         // [nbins] phase steps; with per-PRN windows [nprn][nbins]
+    DeviceArray<int32_t> d_prn;        // [32]
+    DeviceArray<double> d_flo;         // [32] first bin of each PRN's window (gpsb200_acquire_windows)
+    DeviceArray<int64_t> d_boff;       // batches (gpsb200_snapshot_batch): [nwin] window offsets in samples,
+    DeviceArray<int32_t> d_bprn;       // [nwin][nprn] PRN,
+    DeviceArray<double> d_bflo;        // [nwin][nprn] first bin
+    DeviceArray<gpsb200_acq_result_t> d_bres;   // and [nwin][nprn] results of every (window, PRN) pair
+    bool ready = false;                // d_edges / d_nedges uploaded, kernel attributes set, sms read
     int sms = 0;                       // SM count of the device (the split rule)
     int force_split = 0;               // 0: the split rule; else the split of every search (a test hook)
 };
@@ -67,7 +63,6 @@ uint32_t phase_step(double f_hz);
 cudaError_t scratch_reserve(Scratch &sc, const gpsb200_acq_config_t *cfg, bool windows, bool want_grid);
 // Scratch of a batch pass of nwin windows (launch_batch).
 cudaError_t batch_reserve(Scratch &sc, const gpsb200_acq_config_t *cfg, int nwin);
-void scratch_free(Scratch &sc);
 // Enqueue the search of the samples at `window` (the first sample is s0) on s; results land in sc.h_res after a
 // synchronize of s, the grid (want_grid) in sc.d_grid. f_lo_prn (NULL: cfg->f_lo_hz for every PRN): per-PRN windows.
 cudaError_t launch(Scratch &sc, const void *window, int sample_size, const gpsb200_acq_config_t *cfg,

@@ -424,18 +424,6 @@ int64_t hypotheses(const gpsb200_collective_config_t *cfg) {
     return (int64_t) cfg->n[0] * cfg->n[1] * cfg->n[2] * cfg->n[3];
 }
 
-void scratch_free(Scratch &sc) {
-    cudaFree(sc.d_rowsum);
-    cudaFree(sc.d_q);
-    cudaFree(sc.d_scores);
-    cudaFree(sc.d_table);
-    cudaFree(sc.d_eph);
-    cudaFree(sc.d_setup);
-    cudaFree(sc.d_rec);
-    cudaFree(sc.d_seed);
-    sc = Scratch();
-}
-
 cudaError_t launch(Scratch &sc, const uint64_t *d_grid, const gpsb200_acq_result_t *d_res,
                    const gpsb200_acq_config_t *acq, const double *f_lo_prn, const gpsb200_ephemeris_t *eph,
                    const gpsb200_coarse_config_t *ap, const gpsb200_collective_config_t *cfg,
@@ -443,27 +431,25 @@ cudaError_t launch(Scratch &sc, const uint64_t *d_grid, const gpsb200_acq_result
                    gpsb200_cd_cell_t *table, cudaStream_t s) {
     const int nprn = acq->nprn, nbins = acq->nbins;
     const int64_t nhyp = hypotheses(cfg);
-    if (!sc.d_eph) {
-        CU_RET(cudaMalloc(&sc.d_eph, 32 * sizeof(gpsb200_ephemeris_t)));
-        CU_RET(cudaMalloc(&sc.d_setup, sizeof(Setup)));
-        CU_RET(cudaMalloc(&sc.d_rec, sizeof(gpsb200_collective_t)));
-        CU_RET(cudaMalloc(&sc.d_seed, 32 * sizeof(gpsb200_acq_result_t)));
-    }
-    CU_RET(grow(sc.d_rowsum, sc.rowsum_cap, (size_t) nprn * nbins * 2));
-    CU_RET(grow(sc.d_q, sc.q_cap, (size_t) nprn * nbins * kRow));
-    CU_RET(grow(sc.d_scores, sc.scores_cap, (size_t) nhyp));
-    if (table) CU_RET(grow(sc.d_table, sc.table_cap, (size_t) nhyp * nprn));
+    CU_RET(sc.d_eph.grow(32));
+    CU_RET(sc.d_setup.grow(1));
+    CU_RET(sc.d_rec.grow(1));
+    CU_RET(sc.d_seed.grow(32));
+    CU_RET(sc.d_rowsum.grow((size_t) nprn * nbins * 2));
+    CU_RET(sc.d_q.grow((size_t) nprn * nbins * kRow));
+    CU_RET(sc.d_scores.grow((size_t) nhyp));
+    if (table) CU_RET(sc.d_table.grow((size_t) nhyp * nprn));
     Args a{};
     a.grid = d_grid;
-    a.rowsum = sc.d_rowsum;
-    a.q = sc.d_q;
-    a.eph = sc.d_eph;
-    a.setup = sc.d_setup;
-    a.scores = sc.d_scores;
-    a.table = table ? sc.d_table : nullptr;
-    a.rec = sc.d_rec;
+    a.rowsum = sc.d_rowsum.get();
+    a.q = sc.d_q.get();
+    a.eph = sc.d_eph.get();
+    a.setup = sc.d_setup.get();
+    a.scores = sc.d_scores.get();
+    a.table = table ? sc.d_table.get() : nullptr;
+    a.rec = sc.d_rec.get();
     a.res = d_res;
-    a.seed = sc.d_seed;
+    a.seed = sc.d_seed.get();
     a.s0 = acq->s0;
     a.nprn = nprn;
     a.nbins = nbins;
@@ -476,7 +462,7 @@ cudaError_t launch(Scratch &sc, const uint64_t *d_grid, const gpsb200_acq_result
     a.ap = *ap;
     a.cfg = *cfg;
     // eph is the caller's memory: wait for the copy before returning (every path below synchronizes s)
-    CU_RET(cudaMemcpyAsync(sc.d_eph, eph, 32 * sizeof(gpsb200_ephemeris_t), cudaMemcpyHostToDevice, s));
+    CU_RET(cudaMemcpyAsync(sc.d_eph.get(), eph, 32 * sizeof(gpsb200_ephemeris_t), cudaMemcpyHostToDevice, s));
     k_cd_rowsum<<<dim3(nbins, nprn), kThreads, 0, s>>>(a);
     CU_RET(cudaGetLastError());
     k_cd_q<<<dim3(nbins, nprn), kThreads, 0, s>>>(a);
@@ -484,7 +470,7 @@ cudaError_t launch(Scratch &sc, const uint64_t *d_grid, const gpsb200_acq_result
     k_cd_setup<<<1, 32, 0, s>>>(a);
     CU_RET(cudaGetLastError());
     int nused = 0;
-    CU_RET(cudaMemcpyAsync(&nused, &sc.d_setup->nused, sizeof(int), cudaMemcpyDeviceToHost, s));
+    CU_RET(cudaMemcpyAsync(&nused, &sc.d_setup.get()->nused, sizeof(int), cudaMemcpyDeviceToHost, s));
     CU_RET(cudaStreamSynchronize(s));
     const bool scored = nused >= GPSB200_CD_MIN_USED;
     if (scored) {
@@ -495,18 +481,19 @@ cudaError_t launch(Scratch &sc, const uint64_t *d_grid, const gpsb200_acq_result
     }
     k_cd_seed<<<nprn, kThreads, 0, s>>>(a);
     CU_RET(cudaGetLastError());
-    CU_RET(cudaMemcpyAsync(out, sc.d_rec, sizeof(gpsb200_collective_t), cudaMemcpyDeviceToHost, s));
-    CU_RET(cudaMemcpyAsync(seed, sc.d_seed, nprn * sizeof(gpsb200_acq_result_t), cudaMemcpyDeviceToHost, s));
+    CU_RET(cudaMemcpyAsync(out, sc.d_rec.get(), sizeof(gpsb200_collective_t), cudaMemcpyDeviceToHost, s));
+    CU_RET(cudaMemcpyAsync(seed, sc.d_seed.get(), nprn * sizeof(gpsb200_acq_result_t), cudaMemcpyDeviceToHost, s));
     if (scores) {
         if (scored)
-            CU_RET(cudaMemcpyAsync(scores, sc.d_scores, nhyp * sizeof(gpsb200_cd_score_t), cudaMemcpyDeviceToHost, s));
+            CU_RET(cudaMemcpyAsync(scores, sc.d_scores.get(), nhyp * sizeof(gpsb200_cd_score_t), cudaMemcpyDeviceToHost,
+                                   s));
         else
             memset(scores, 0, nhyp * sizeof(gpsb200_cd_score_t));
     }
     if (table) {
         if (scored)
-            CU_RET(cudaMemcpyAsync(table, sc.d_table, nhyp * nprn * sizeof(gpsb200_cd_cell_t), cudaMemcpyDeviceToHost,
-                                   s));
+            CU_RET(cudaMemcpyAsync(table, sc.d_table.get(), nhyp * nprn * sizeof(gpsb200_cd_cell_t),
+                                   cudaMemcpyDeviceToHost, s));
         else
             memset(table, 0xff, nhyp * nprn * sizeof(gpsb200_cd_cell_t));
     }

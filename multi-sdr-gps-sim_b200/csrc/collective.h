@@ -7,6 +7,7 @@
 #include <string>
 
 #include "../../include/gpsb200.h"
+#include "device_buffer.h"
 
 namespace gpsb200 {
 namespace cd {
@@ -23,20 +24,15 @@ int64_t hypotheses(const gpsb200_collective_config_t *cfg);
 
 struct Setup;
 struct Scratch {
-    uint64_t *d_rowsum = nullptr;          // [nprn][nbins][2] 128-bit row sums (lo, hi)
-    size_t rowsum_cap = 0;
-    uint16_t *d_q = nullptr;               // [nprn][nbins][kRow]
-    size_t q_cap = 0;
-    gpsb200_cd_score_t *d_scores = nullptr;   // [nhyp]
-    size_t scores_cap = 0;
-    gpsb200_cd_cell_t *d_table = nullptr;  // [nhyp][nprn], only when the caller wants it
-    size_t table_cap = 0;
-    gpsb200_ephemeris_t *d_eph = nullptr;  // [32]
-    Setup *d_setup = nullptr;
-    gpsb200_collective_t *d_rec = nullptr;
-    gpsb200_acq_result_t *d_seed = nullptr;   // [32]
+    DeviceArray<uint64_t> d_rowsum;             // [nprn][nbins][2] 128-bit row sums (lo, hi)
+    DeviceArray<uint16_t> d_q;                  // [nprn][nbins][kRow]
+    DeviceArray<gpsb200_cd_score_t> d_scores;   // [nhyp]
+    DeviceArray<gpsb200_cd_cell_t> d_table;     // [nhyp][nprn], only when the caller wants it
+    DeviceArray<gpsb200_ephemeris_t> d_eph;     // [32]
+    DeviceArray<Setup> d_setup;                 // [1]
+    DeviceArray<gpsb200_collective_t> d_rec;    // [1]
+    DeviceArray<gpsb200_acq_result_t> d_seed;   // [32]
 };
-void scratch_free(Scratch &sc);
 
 // Steps 2-8 on the grid [nprn][nbins][3000] and results d_res [nprn] (device) a search with acq and f_lo_prn left, on s;
 // waits for seed [nprn], out and, when not NULL, scores [nhyp] and table [nhyp][nprn] (host).

@@ -179,38 +179,44 @@ struct gpsb200_ctx {
     cudaStream_t s_compute = nullptr, s_copy = nullptr, s_pre = nullptr, s_ck = nullptr;
     cudaEvent_t ev[kCallEvents]{};
     std::vector<cudaEvent_t> ev_done;      // one per synthesis chunk
-    BlockChanDev *d_bc = nullptr, *h_bc = nullptr;
-    RunCkpt *d_ck = nullptr, *h_ck = nullptr;          // h_ck: run checkpoints of small calls, computed on the host
-    uint32_t *d_nav = nullptr, *h_nav = nullptr;
-    uint32_t *d_chips = nullptr;
-    int32_t *d_atab = nullptr;             // per-block carrier tables (k_tables -> k_synth)
-    double *d_carr_end = nullptr;
-    int *d_chain_errors = nullptr, *h_chain_errors = nullptr;   // device self-check of the carrier chain
-    double *d_guess = nullptr, *h_guess = nullptr;     // speculative block-start phases
+    DeviceArray<BlockChanDev> d_bc;
+    PinnedArray<BlockChanDev> h_bc;
+    DeviceArray<RunCkpt> d_ck;
+    PinnedArray<RunCkpt> h_ck;                         // run checkpoints of small calls, computed on the host
+    DeviceArray<uint32_t> d_nav;
+    PinnedArray<uint32_t> h_nav;
+    DeviceArray<uint32_t> d_chips;
+    DeviceArray<int32_t> d_atab;           // per-block carrier tables (k_tables -> k_synth)
+    DeviceArray<double> d_carr_end;
+    DeviceArray<int> d_chain_errors;                   // device self-check of the carrier chain
+    PinnedArray<int> h_chain_errors;
+    DeviceArray<double> d_guess;                       // speculative block-start phases
+    PinnedArray<double> h_guess;
     std::vector<uint8_t> h_guess_abs;                  // relative-mode marker per (block, channel), see prepare_blocks
     std::vector<uint8_t> h_span_flags;                 // per (span, channel): 1 = every block idle, 2 = one satellite throughout
-    double *d_carr0 = nullptr, *h_carr0 = nullptr;     // exact block-start phases of host-resolved (irregular) spans
-    CarrierProbe *d_probe = nullptr;                   // block probes in HBM (k_chain reads them)
-    CarrierProbe *h_probe = nullptr, *d_probe_host = nullptr;   // ... and in mapped host memory (host fallback)
-    double *d_seg = nullptr;                           // [block][chan][kSegStates] probe states at checkpoint-segment starts
-    CarrierProbe *h_span_sum = nullptr, *d_span_sum = nullptr;  // span summaries, mapped host memory
-    SpanBlockState *d_spec = nullptr;                  // speculative block-start phases
+    DeviceArray<double> d_carr0;                       // exact block-start phases of host-resolved (irregular) spans
+    PinnedArray<double> h_carr0;
+    DeviceArray<CarrierProbe> d_probe;                 // block probes in HBM (k_chain reads them)
+    PinnedArray<CarrierProbe> h_probe;                 // ... and in mapped host memory (host fallback)
+    DeviceArray<double> d_seg;                         // [block][chan][kSegStates] probe states at checkpoint-segment starts
+    PinnedArray<CarrierProbe> h_span_sum;              // span summaries, mapped host memory
+    DeviceArray<SpanBlockState> d_spec;                // speculative block-start phases
     bool lanes_on = true;                              // GPSB200_LANES=0: always k_synth (lane = channel)
     bool lanes_veto = false;                           // a channel record outside k_synth_lanes' range was seen
-    SpanRes *d_span_res = nullptr, *h_span_res = nullptr;
+    DeviceArray<SpanRes> d_span_res;
+    PinnedArray<SpanRes> h_span_res;
     int max_spans = 0;
-    double *h_seg_end = nullptr, *d_seg_end = nullptr;   // mapped: device-walked end phases of every pipeline segment's last block
+    PinnedArray<double> h_seg_end;         // mapped: device-walked end phases of every pipeline segment's last block
     std::vector<double> seg_expect;        // what the chain says they must be
     std::vector<cudaEvent_t> ev_seg;       // probes of segment i complete
     int fault_inject_chain = 0;            // gpsb200_debug_corrupt_chain(): 1 = resolution, 2 = segment state
     bool trace_on = false;
     double trace_t0 = 0.0;
     Call call;                             // a slice call begun with gpsb200_slice_prepare (active until finished)
-    uint8_t *d_out = nullptr;              // synthesis staging of host destinations
-    size_t out_bytes = 0;
-    uint8_t *d_rx = nullptr;               // receiver staging of host sources (acquisition window, tracking buffer)
-    size_t rx_bytes = 0;
-    int8_t *d_rx_chips = nullptr;          // chips as +-1 of tracking and snapshots (trk::chips_upload), built once
+    DeviceArray<uint8_t> d_out;            // synthesis staging of host destinations
+    DeviceArray<uint8_t> d_rx;             // receiver staging of host sources (acquisition window, tracking buffer)
+    DeviceArray<int8_t> d_rx_chips;        // chips as +-1 of tracking and snapshots (trk::chips_upload), built once
+    bool rx_chips_ready = false;           // ... when d_rx_chips holds them
     bool nav_dirty = true;
     std::unique_ptr<WorkerPool> pool;      // host passes (guesses, fix-up scan)
     SynthArgs last{};                      // replay state
@@ -525,24 +531,24 @@ SynthArgs make_args(gpsb200_ctx *ctx, int blk0, int nblk, int nchan, int sample_
     // blk0 is a multiple of kSpanBlocks whenever the chain kernels are launched with these arguments
     SynthArgs a{};
     const size_t off = (size_t) blk0 * nchan;
-    a.bc = ctx->d_bc + off;
-    a.carr0 = ctx->d_carr0 + off;
-    a.guess = ctx->d_guess + off;
-    a.probe = ctx->d_probe + off;
-    a.probe_host = ctx->d_probe_host + off;
-    a.seg = ctx->d_seg + off * kSegStates;
-    a.spec = ctx->d_spec + off;
+    a.bc = ctx->d_bc.get() + off;
+    a.carr0 = ctx->d_carr0.get() + off;
+    a.guess = ctx->d_guess.get() + off;
+    a.probe = ctx->d_probe.get() + off;
+    a.probe_host = ctx->h_probe.dev() + off;
+    a.seg = ctx->d_seg.get() + off * kSegStates;
+    a.spec = ctx->d_spec.get() + off;
     a.span_blocks = kSpanBlocks;
     a.nspan = (nblk + kSpanBlocks - 1) / kSpanBlocks;
-    a.span_sum = ctx->d_span_sum + (size_t) (blk0 / kSpanBlocks) * nchan;
-    a.span_res = ctx->d_span_res + (size_t) (blk0 / kSpanBlocks) * nchan;
-    a.ck = ctx->d_ck + off * ctx->nruns;
-    a.nav = ctx->d_nav;
+    a.span_sum = ctx->h_span_sum.dev() + (size_t) (blk0 / kSpanBlocks) * nchan;
+    a.span_res = ctx->d_span_res.get() + (size_t) (blk0 / kSpanBlocks) * nchan;
+    a.ck = ctx->d_ck.get() + off * ctx->nruns;
+    a.nav = ctx->d_nav.get();
     a.nav_stride = ctx->cfg.max_chan;
-    a.chipbits = ctx->d_chips;
-    a.atab = ctx->d_atab + (size_t) blk0 * kAtabRows * 32;
-    a.carr_end = ctx->d_carr_end + off;
-    a.chain_errors = ctx->d_chain_errors;
+    a.chipbits = ctx->d_chips.get();
+    a.atab = ctx->d_atab.get() + (size_t) blk0 * kAtabRows * 32;
+    a.carr_end = ctx->d_carr_end.get() + off;
+    a.chain_errors = ctx->d_chain_errors.get();
     a.out = out;
     a.nblk = nblk;
     a.nchan = nchan;
@@ -570,7 +576,7 @@ SynthArgs call_args(gpsb200_ctx *ctx, const Call &call, int b0, int nb) {
 int upload_nav(gpsb200_ctx *ctx, cudaStream_t s) {
     if (!ctx->nav_dirty) return GPSB200_OK;
     const size_t bytes = (size_t) ctx->cfg.max_nav_frames * ctx->cfg.max_chan * GPSB200_NAV_WORDS * 4;
-    CU(cudaMemcpyAsync(ctx->d_nav, ctx->h_nav, bytes, cudaMemcpyHostToDevice, s));
+    CU(cudaMemcpyAsync(ctx->d_nav.get(), ctx->h_nav.get(), bytes, cudaMemcpyHostToDevice, s));
     ctx->nav_dirty = false;
     return GPSB200_OK;
 }
@@ -603,7 +609,7 @@ int check_aligned(gpsb200_ctx *ctx, const void *p, const char *fn, const char *a
 
 // Host destinations are staged in the context's own device buffer, sized for the context's largest call.
 int ensure_staging(gpsb200_ctx *ctx, int sample_size) {
-    CU(grow(ctx->d_out, ctx->out_bytes, (size_t) ctx->cfg.max_blocks * GPSB200_BLOCK_ELEMS * sample_size));
+    CU(ctx->d_out.grow((size_t) ctx->cfg.max_blocks * GPSB200_BLOCK_ELEMS * sample_size));
     return GPSB200_OK;
 }
 
@@ -619,10 +625,20 @@ int rx_source(gpsb200_ctx *ctx, const char *fn, const void *iq, int64_t first, i
     const size_t elem = sample_size == GPSB200_SC16 ? 4 : 2;
     *dev = static_cast<const char *>(iq) + (size_t) first * elem;
     if (device) return GPSB200_OK;
-    CU(grow(ctx->d_rx, ctx->rx_bytes, (size_t) count * elem));
-    if (count) CU(cudaMemcpyAsync(ctx->d_rx, *dev, (size_t) count * elem, cudaMemcpyHostToDevice, s));
-    *dev = ctx->d_rx;
+    CU(ctx->d_rx.grow((size_t) count * elem));
+    if (count) CU(cudaMemcpyAsync(ctx->d_rx.get(), *dev, (size_t) count * elem, cudaMemcpyHostToDevice, s));
+    *dev = ctx->d_rx.get();
     return GPSB200_OK;
+}
+
+// The chips as +-1 of tracking and snapshots in ctx->d_rx_chips, built by the first receiver call that needs them (and
+// again by the next one when a build fails part way).
+cudaError_t rx_chips(gpsb200_ctx *ctx) {
+    if (!ctx->rx_chips_ready) {
+        CU_RET(trk::chips_upload(ctx->d_rx_chips));
+        ctx->rx_chips_ready = true;
+    }
+    return cudaSuccess;
 }
 
 // The one error path of every entry point that enqueues work: on a non-OK return wait for everything this context
@@ -657,7 +673,7 @@ int call_open(gpsb200_ctx *ctx, const Call &call) {
     CU(cudaStreamWaitEvent(ctx->s_ck, ctx->ev[kEvCallStart], 0));
     const int rc = upload_nav(ctx, ctx->s_pre);
     if (rc) return rc;
-    CU(cudaMemsetAsync(ctx->d_chain_errors, 0, sizeof(int), ctx->s_pre));
+    CU(cudaMemsetAsync(ctx->d_chain_errors.get(), 0, sizeof(int), ctx->s_pre));
     return GPSB200_OK;
 }
 
@@ -672,7 +688,8 @@ int seg_params(gpsb200_ctx *ctx, Call &call, int b0, int b1, cudaStream_t sp, st
     const int rc = prepare_blocks(ctx, call.chans, b0, b1, call.nchan, guessed ? *guessed : call.chain, link, guessed);
     if (rc) return rc;
     call.st.host_chain_ms += now_ms() - t0;
-    CU(cudaMemcpyAsync(ctx->d_bc + off, ctx->h_bc + off, cnt * sizeof(BlockChanDev), cudaMemcpyHostToDevice, sp));
+    CU(cudaMemcpyAsync(ctx->d_bc.get() + off, ctx->h_bc.get() + off, cnt * sizeof(BlockChanDev), cudaMemcpyHostToDevice,
+                       sp));
     call.st.h2d_bytes += (int64_t) (cnt * sizeof(BlockChanDev));
     if (call.dst) {
         CU(launch_tables(call_args(ctx, call, b0, b1 - b0), sp));     // needs only the parameters: off the critical path
@@ -687,7 +704,8 @@ int seg_probe(gpsb200_ctx *ctx, Call &call, int b0, int b1, cudaStream_t sp) {
     const size_t off = (size_t) b0 * call.nchan, cnt = (size_t) (b1 - b0) * call.nchan;
     SynthArgs a = make_args(ctx, b0, b1 - b0, call.nchan, call.sample_size, nullptr);
     if (!call.dst) a.ck = nullptr;
-    CU(cudaMemcpyAsync(ctx->d_guess + off, ctx->h_guess + off, cnt * sizeof(double), cudaMemcpyHostToDevice, sp));
+    CU(cudaMemcpyAsync(ctx->d_guess.get() + off, ctx->h_guess.get() + off, cnt * sizeof(double), cudaMemcpyHostToDevice,
+                       sp));
     if (b0 == 0) CU(cudaEventRecord(ctx->ev[kEvProbeStart], sp));
     CU(launch_probe(a, sp));
     CU(launch_chain(a, sp));
@@ -738,10 +756,12 @@ int seg_commit(gpsb200_ctx *ctx, Call &call, int i0, int i1, cudaStream_t sp) {
     SynthArgs a = call_args(ctx, call, b0, b1 - b0);
     const size_t soff = (size_t) (b0 / kSpanBlocks) * nchan, scnt = (size_t) a.nspan * nchan;
     if (b0 == 0) CU(cudaEventRecord(ctx->ev[kEvCkptStart], sp));
-    CU(cudaMemcpyAsync(ctx->d_span_res + soff, ctx->h_span_res + soff, scnt * sizeof(SpanRes), cudaMemcpyHostToDevice, sp));
+    CU(cudaMemcpyAsync(ctx->d_span_res.get() + soff, ctx->h_span_res.get() + soff, scnt * sizeof(SpanRes),
+                       cudaMemcpyHostToDevice, sp));
     call.st.h2d_bytes += (int64_t) (scnt * sizeof(SpanRes));
     if (slow > 0) {                                  // rare: block start phases of the host-resolved spans
-        CU(cudaMemcpyAsync(ctx->d_carr0 + off, ctx->h_carr0 + off, cnt * sizeof(double), cudaMemcpyHostToDevice, sp));
+        CU(cudaMemcpyAsync(ctx->d_carr0.get() + off, ctx->h_carr0.get() + off, cnt * sizeof(double),
+                           cudaMemcpyHostToDevice, sp));
         call.st.h2d_bytes += (int64_t) (cnt * sizeof(double));
     }
     // test hook of the device self-check (gpsb200_debug_corrupt_chain mode 2): move the state that block b0 + 5's probe
@@ -749,7 +769,7 @@ int seg_commit(gpsb200_ctx *ctx, Call &call, int i0, int i1, cudaStream_t sp) {
     // are complete: the host scan waited for them); k_checkpoints must notice
     const int jm = ckpt_segments(ctx->nruns) / 2;
     if (ctx->fault_inject_chain == 2 && b1 - b0 > 6 && jm >= 1) {
-        double *p = ctx->d_seg + (size_t) (b0 + 5) * nchan * kSegStates, h[kSegStates];
+        double *p = ctx->d_seg.get() + (size_t) (b0 + 5) * nchan * kSegStates, h[kSegStates];
         CU(cudaMemcpyAsync(h, p, sizeof h, cudaMemcpyDeviceToHost, sp));
         CU(cudaStreamSynchronize(sp));
         h[jm - 1] += 0x1p-51;
@@ -758,7 +778,7 @@ int seg_commit(gpsb200_ctx *ctx, Call &call, int i0, int i1, cudaStream_t sp) {
         CU(cudaStreamSynchronize(sp));
     }
     SynthArgs ack = a;
-    ack.last_end_host = ctx->d_seg_end + (size_t) i0 * nchan;
+    ack.last_end_host = ctx->h_seg_end.dev() + (size_t) i0 * nchan;
     CU(launch_checkpoints(ack, sp));
     if (b0 == 0) CU(cudaEventRecord(ctx->ev[kEvCkptEnd], sp));
     call.st.launches += 1;
@@ -796,7 +816,7 @@ int seg_commit(gpsb200_ctx *ctx, Call &call, int i0, int i1, cudaStream_t sp) {
 // checkpoint launches on sp; the call's device state stays resident for gpsb200_replay_device.
 int call_close(gpsb200_ctx *ctx, const Call &call, cudaStream_t sp) {
     CU(cudaEventRecord(ctx->ev[kEvCallEnd], call.stream));
-    CU(cudaMemcpyAsync(ctx->h_chain_errors, ctx->d_chain_errors, sizeof(int), cudaMemcpyDeviceToHost, sp));
+    CU(cudaMemcpyAsync(ctx->h_chain_errors.get(), ctx->d_chain_errors.get(), sizeof(int), cudaMemcpyDeviceToHost, sp));
     ctx->last = call_args(ctx, call, 0, call.nblk);
     ctx->have_last = true;
     return GPSB200_OK;
@@ -805,7 +825,7 @@ int call_close(gpsb200_ctx *ctx, const Call &call, cudaStream_t sp) {
 // Verdict of the device self-check (the counter read by call_close must have arrived): the per-block comparisons inside
 // the checkpoint launches plus the comparisons at the end of every committed range.
 int call_verdict(gpsb200_ctx *ctx, const Call &call) {
-    int bad = *ctx->h_chain_errors;
+    int bad = ctx->h_chain_errors[0];
     for (int i = 0; i < call.rows; i++)
         for (int c = 0; c < call.nchan; c++) {
             const double want = ctx->seg_expect[(size_t) i * call.nchan + c];
@@ -844,7 +864,7 @@ int small_call(gpsb200_ctx *ctx, Call &call, double *carr_phase_out, gpsb200_sta
             ChainState stc = call.chain[c];
             for (int b = 0; b < nblk; b++) {
                 const BlockChanDev &p = ctx->h_bc[(size_t) b * nchan + c];
-                RunCkpt *ck = ctx->h_ck + (size_t) b * nruns * nchan + c;
+                RunCkpt *ck = ctx->h_ck.get() + (size_t) b * nruns * nchan + c;
                 if (p.prn <= 0) {
                     stc.prn = 0;
                     for (int r = 0; r < nruns; r++) ck[(size_t) r * nchan] = RunCkpt{0.0, 0.0, 0u, 0u};
@@ -872,8 +892,8 @@ int small_call(gpsb200_ctx *ctx, Call &call, double *carr_phase_out, gpsb200_sta
     if (rc) return rc;
     const size_t cnt = (size_t) nblk * nchan;
     CU(cudaEventRecord(ctx->ev[kEvCallStart], s));
-    CU(cudaMemcpyAsync(ctx->d_bc, ctx->h_bc, cnt * sizeof(BlockChanDev), cudaMemcpyHostToDevice, s));
-    CU(cudaMemcpyAsync(ctx->d_ck, ctx->h_ck, cnt * nruns * sizeof(RunCkpt), cudaMemcpyHostToDevice, s));
+    CU(cudaMemcpyAsync(ctx->d_bc.get(), ctx->h_bc.get(), cnt * sizeof(BlockChanDev), cudaMemcpyHostToDevice, s));
+    CU(cudaMemcpyAsync(ctx->d_ck.get(), ctx->h_ck.get(), cnt * nruns * sizeof(RunCkpt), cudaMemcpyHostToDevice, s));
     const SynthArgs a = call_args(ctx, call, 0, nblk);
     CU(launch_tables(a, s));
     CU(launch_synth(a, s));
@@ -982,7 +1002,7 @@ int slice_prepare(gpsb200_ctx *ctx, const gpsb200_chan_t *chans, int nblk, int n
     if (!dst_device) {                          // host destination only: stage in the context's own device buffer
         rc = ensure_staging(ctx, sample_size);
         if (rc) return rc;
-        dst_device = ctx->d_out;
+        dst_device = ctx->d_out.get();
     }
     if (!link) return fail(ctx, GPSB200_ERR_ARG, "gpsb200_slice_prepare: link is NULL");
     Call &call = ctx->call = Call(chans, nblk, nchan, sample_size, dst_device, dst_host, nullptr, s);
@@ -1085,7 +1105,7 @@ int synth_host(gpsb200_ctx *ctx, const gpsb200_chan_t *chans, int nblk, int ncha
     if (rc) return rc;
     rc = ensure_staging(ctx, sample_size);
     if (rc) return rc;
-    Call call(chans, nblk, nchan, sample_size, ctx->d_out, dst_host, scatter, ctx->s_compute);
+    Call call(chans, nblk, nchan, sample_size, ctx->d_out.get(), dst_host, scatter, ctx->s_compute);
     return run_pipeline(ctx, call, carr_phase_out, stats);
 }
 
@@ -1132,9 +1152,9 @@ int acquire(gpsb200_ctx *ctx, const void *iq, int64_t nsamples, int sample_size,
     CU(acq::scratch_reserve(ctx->acq, cfg, windows, grid != nullptr));
     CU(acq::launch(ctx->acq, window, sample_size, cfg, windows ? f_lo_prn : nullptr, grid != nullptr, s));
     if (grid)
-        CU(cudaMemcpy(grid, ctx->acq.d_grid, (size_t) cfg->nprn * cfg->nbins * acq::kCode * sizeof(uint64_t),
+        CU(cudaMemcpy(grid, ctx->acq.d_grid.get(), (size_t) cfg->nprn * cfg->nbins * acq::kCode * sizeof(uint64_t),
                       cudaMemcpyDeviceToHost));
-    memcpy(res, ctx->acq.h_res, (size_t) cfg->nprn * sizeof(gpsb200_acq_result_t));
+    memcpy(res, ctx->acq.h_res.get(), (size_t) cfg->nprn * sizeof(gpsb200_acq_result_t));
     return GPSB200_OK;
 }
 
@@ -1147,9 +1167,9 @@ int track(gpsb200_ctx *ctx, const void *iq, int64_t nsamples, int sample_size, i
     const void *src;
     const int rc = rx_source(ctx, "gpsb200_track_device", iq, 0, nsamples, sample_size, device, s, &src);
     if (rc) return rc;
-    if (!ctx->d_rx_chips) CU(trk::chips_upload(&ctx->d_rx_chips));
+    CU(rx_chips(ctx));
     CU(trk::scratch_reserve(ctx->trk, nchan, max_epochs));
-    CU(trk::launch(ctx->trk, ctx->d_rx_chips, src, nsamples, sample_size, base, state, nchan, max_epochs, epochs,
+    CU(trk::launch(ctx->trk, ctx->d_rx_chips.get(), src, nsamples, sample_size, base, state, nchan, max_epochs, epochs,
                    nepochs, s));
     return GPSB200_OK;
 }
@@ -1168,10 +1188,10 @@ int vtrack(gpsb200_ctx *ctx, const void *iq, int64_t nsamples, int sample_size, 
     const void *src;
     const int rc = rx_source(ctx, name, iq, 0, nsamples, sample_size, device, s, &src);
     if (rc) return rc;
-    if (!ctx->d_rx_chips) CU(trk::chips_upload(&ctx->d_rx_chips));
+    CU(rx_chips(ctx));
     CU(vtk::scratch_reserve(ctx->vtk, state->nchan, max_updates, epochs ? max_epochs : 0));
-    CU(vtk::launch(ctx->vtk, ctx->d_rx_chips, src, nsamples, sample_size, base, chans, cfg, state, max_updates, fixes,
-                   out, nupdates, epochs, max_epochs, nepochs, ctx->vtk_ctas, s));
+    CU(vtk::launch(ctx->vtk, ctx->d_rx_chips.get(), src, nsamples, sample_size, base, chans, cfg, state, max_updates,
+                   fixes, out, nupdates, epochs, max_epochs, nepochs, ctx->vtk_ctas, s));
     return GPSB200_OK;
 }
 
@@ -1186,9 +1206,10 @@ int snapshot_measure(gpsb200_ctx *ctx, const void *iq, int64_t nsamples, int sam
     const void *window;
     const int rc = rx_source(ctx, name, iq, acq->s0, acq::window_samples(acq), sample_size, device, s, &window);
     if (rc) return rc;
-    if (!ctx->d_rx_chips) CU(trk::chips_upload(&ctx->d_rx_chips));
+    CU(rx_chips(ctx));
     snap::seed(acq, res, cfg, out);
-    CU(snap::launch(ctx->snap, window, sample_size, acq->ms, acq->nprn, ctx->d_rx_chips, cfg->iterations, out, s));
+    CU(snap::launch(ctx->snap, window, sample_size, acq->ms, acq->nprn, ctx->d_rx_chips.get(), cfg->iterations, out,
+                    s));
     return GPSB200_OK;
 }
 
@@ -1212,8 +1233,9 @@ int collective(gpsb200_ctx *ctx, const void *iq, int64_t nsamples, int sample_si
     if (rc) return rc;
     CU(acq::scratch_reserve(ctx->acq, acq, f_lo_prn != nullptr, true));
     CU(acq::launch(ctx->acq, window, sample_size, acq, f_lo_prn, true, s));
-    memcpy(res, ctx->acq.h_res, (size_t) acq->nprn * sizeof(gpsb200_acq_result_t));
-    CU(cd::launch(ctx->cd, ctx->acq.d_grid, ctx->acq.d_res, acq, f_lo_prn, eph, ap, cfg, seed, out, scores, table, s));
+    memcpy(res, ctx->acq.h_res.get(), (size_t) acq->nprn * sizeof(gpsb200_acq_result_t));
+    CU(cd::launch(ctx->cd, ctx->acq.d_grid.get(), ctx->acq.d_res.get(), acq, f_lo_prn, eph, ap, cfg, seed, out, scores,
+                  table, s));
     return GPSB200_OK;
 }
 
@@ -1240,7 +1262,7 @@ int snapshot_batch(gpsb200_ctx *ctx, const void *iq, int64_t nsamples, int sampl
     int rc = device ? check_aligned(ctx, iq, name, "iq_device") : GPSB200_OK;
     if (!rc) rc = check_entry(ctx);
     if (rc) return rc;
-    if (!ctx->d_rx_chips) CU(trk::chips_upload(&ctx->d_rx_chips));
+    CU(rx_chips(ctx));
     const int nprn = acq->nprn, per = snap::batch_pass(acq, sample_size, nwin);
     const int64_t span = acq::window_samples(acq);
     const size_t elem = sample_size == GPSB200_SC16 ? 4 : 2;
@@ -1253,13 +1275,14 @@ int snapshot_batch(gpsb200_ctx *ctx, const void *iq, int64_t nsamples, int sampl
         if (device) {
             for (int i = 0; i < n; i++) off[i] = s0[w0 + i];
         } else {
-            CU(grow(ctx->d_rx, ctx->rx_bytes, (size_t) n * span * elem));
+            CU(ctx->d_rx.grow((size_t) n * span * elem));
             for (int i = 0; i < n; i++) {
                 off[i] = (int64_t) i * span;
-                CU(cudaMemcpyAsync(ctx->d_rx + (size_t) off[i] * elem, static_cast<const char *>(iq) + s0[w0 + i] * elem,
-                                   (size_t) span * elem, cudaMemcpyHostToDevice, s));
+                CU(cudaMemcpyAsync(ctx->d_rx.get() + (size_t) off[i] * elem,
+                                   static_cast<const char *>(iq) + s0[w0 + i] * elem, (size_t) span * elem,
+                                   cudaMemcpyHostToDevice, s));
             }
-            src = ctx->d_rx;
+            src = ctx->d_rx.get();
         }
         gpsb200_acq_result_t *r = res + (size_t) w0 * nprn;
         gpsb200_snapshot_t *o = out + (size_t) w0 * nprn;
@@ -1271,8 +1294,8 @@ int snapshot_batch(gpsb200_ctx *ctx, const void *iq, int64_t nsamples, int sampl
             if (!bad.empty()) return fail(ctx, GPSB200_ERR_ARG, at + "window " + std::to_string(w0 + i) + ": " + bad);
             snap::seed(&one, r + (size_t) i * nprn, cfg, o + (size_t) i * nprn);
         }
-        CU(snap::launch_batch(ctx->snap, src, sample_size, acq->ms, n, nprn, ctx->acq.d_boff, ctx->d_rx_chips,
-                              cfg->iterations, o, s));
+        CU(snap::launch_batch(ctx->snap, src, sample_size, acq->ms, n, nprn, ctx->acq.d_boff.get(),
+                              ctx->d_rx_chips.get(), cfg->iterations, o, s));
     }
     return GPSB200_OK;
 }
@@ -1514,45 +1537,41 @@ int gpsb200_create(const gpsb200_config_t *cfg, gpsb200_ctx_t **out) {
     const size_t max_segs = segments_of(c.max_blocks).size();     // every call's segments have their rows and events
     ctx->ev_seg.resize(max_segs);
     for (auto &e : ctx->ev_seg) CU(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-    CU(cudaHostAlloc(&ctx->h_seg_end, max_segs * c.max_chan * sizeof(double), cudaHostAllocMapped));
-    CU(cudaHostGetDevicePointer((void **) &ctx->d_seg_end, ctx->h_seg_end, 0));
+    CU(ctx->h_seg_end.grow(max_segs * c.max_chan, cudaHostAllocMapped));
     ctx->seg_expect.assign(max_segs * c.max_chan, -1.0);
     const size_t nbc = (size_t) c.max_blocks * c.max_chan;
-    CU(cudaMalloc(&ctx->d_bc, nbc * sizeof(BlockChanDev)));
-    CU(cudaHostAlloc(&ctx->h_bc, nbc * sizeof(BlockChanDev), cudaHostAllocDefault));
-    CU(cudaMalloc(&ctx->d_ck, nbc * ctx->nruns * sizeof(RunCkpt)));
-    CU(cudaHostAlloc(&ctx->h_ck, (size_t) std::min(c.max_blocks, kHostChainBlocks) * c.max_chan * ctx->nruns * sizeof(RunCkpt),
-                     cudaHostAllocDefault));
-    CU(cudaMalloc(&ctx->d_carr_end, nbc * sizeof(double)));
-    CU(cudaMalloc(&ctx->d_atab, (size_t) c.max_blocks * kAtabRows * 32 * sizeof(int32_t)));
-    CU(cudaMalloc(&ctx->d_chain_errors, sizeof(int)));
-    CU(cudaHostAlloc(&ctx->h_chain_errors, sizeof(int), cudaHostAllocDefault));
-    CU(cudaMalloc(&ctx->d_guess, nbc * sizeof(double)));
-    CU(cudaHostAlloc(&ctx->h_guess, nbc * sizeof(double), cudaHostAllocDefault));
+    CU(ctx->d_bc.grow(nbc));
+    CU(ctx->h_bc.grow(nbc));
+    CU(ctx->d_ck.grow(nbc * ctx->nruns));
+    CU(ctx->h_ck.grow((size_t) std::min(c.max_blocks, kHostChainBlocks) * c.max_chan * ctx->nruns));
+    CU(ctx->d_carr_end.grow(nbc));
+    CU(ctx->d_atab.grow((size_t) c.max_blocks * kAtabRows * 32));
+    CU(ctx->d_chain_errors.grow(1));
+    CU(ctx->h_chain_errors.grow(1));
+    CU(ctx->d_guess.grow(nbc));
+    CU(ctx->h_guess.grow(nbc));
     ctx->h_guess_abs.assign(nbc, 1);
     ctx->h_span_flags.assign((size_t) ((c.max_blocks + kSpanBlocks - 1) / kSpanBlocks + 1) * c.max_chan, 0);
-    CU(cudaMalloc(&ctx->d_carr0, nbc * sizeof(double)));
-    CU(cudaHostAlloc(&ctx->h_carr0, nbc * sizeof(double), cudaHostAllocDefault));
+    CU(ctx->d_carr0.grow(nbc));
+    CU(ctx->h_carr0.grow(nbc));
     // block probes: one copy in HBM (k_chain reads it), one written by the kernel straight into mapped
     // pinned host memory for the host's block-by-block fallback; span summaries only in mapped host memory
     // (a copy-engine download would queue behind the large result downloads of earlier segments)
-    CU(cudaMalloc(&ctx->d_probe, nbc * sizeof(CarrierProbe)));
-    CU(cudaHostAlloc(&ctx->h_probe, nbc * sizeof(CarrierProbe), cudaHostAllocMapped));
-    CU(cudaHostGetDevicePointer((void **) &ctx->d_probe_host, ctx->h_probe, 0));
-    CU(cudaMalloc(&ctx->d_seg, nbc * kSegStates * sizeof(double)));      // only k_checkpoints reads them: HBM only
+    CU(ctx->d_probe.grow(nbc));
+    CU(ctx->h_probe.grow(nbc, cudaHostAllocMapped));
+    CU(ctx->d_seg.grow(nbc * kSegStates));      // only k_checkpoints reads them: HBM only
     ctx->max_spans = (c.max_blocks + kSpanBlocks - 1) / kSpanBlocks + 1;
     const size_t nsc = (size_t) ctx->max_spans * c.max_chan;
-    CU(cudaHostAlloc(&ctx->h_span_sum, nsc * sizeof(CarrierProbe), cudaHostAllocMapped));
-    CU(cudaHostGetDevicePointer((void **) &ctx->d_span_sum, ctx->h_span_sum, 0));
-    CU(cudaMalloc(&ctx->d_spec, nbc * sizeof(SpanBlockState)));
+    CU(ctx->h_span_sum.grow(nsc, cudaHostAllocMapped));
+    CU(ctx->d_spec.grow(nbc));
     if (const char *ev = getenv("GPSB200_TRACE")) ctx->trace_on = atoi(ev) != 0;
     if (const char *ev = getenv("GPSB200_LANES")) ctx->lanes_on = atoi(ev) != 0;
-    CU(cudaMalloc(&ctx->d_span_res, nsc * sizeof(SpanRes)));
-    CU(cudaHostAlloc(&ctx->h_span_res, nsc * sizeof(SpanRes), cudaHostAllocDefault));
-    const size_t navb = (size_t) c.max_nav_frames * c.max_chan * GPSB200_NAV_WORDS * 4;
-    CU(cudaMalloc(&ctx->d_nav, navb));
-    CU(cudaHostAlloc(&ctx->h_nav, navb, cudaHostAllocDefault));
-    memset(ctx->h_nav, 0, navb);
+    CU(ctx->d_span_res.grow(nsc));
+    CU(ctx->h_span_res.grow(nsc));
+    const size_t navw = (size_t) c.max_nav_frames * c.max_chan * GPSB200_NAV_WORDS;
+    CU(ctx->d_nav.grow(navw));
+    CU(ctx->h_nav.grow(navw));
+    memset(ctx->h_nav.get(), 0, navw * sizeof(uint32_t));
     // packed C/A chips (ca[], gps.c:2817), periodically extended so that any 32-chip window
     // starting at chip 0..1022 is two consecutive words; row = prn
     std::vector<uint32_t> chips((size_t) 33 * kChipWords, 0);
@@ -1562,8 +1581,8 @@ int gpsb200_create(const gpsb200_config_t *cfg, gpsb200_ctx_t **out) {
         for (int n = 0; n < kChipWords * 32; n++)
             if (ca[n % GPSB200_CA_LEN]) chips[(size_t) prn * kChipWords + (n >> 5)] |= 1u << (n & 31);
     }
-    CU(cudaMalloc(&ctx->d_chips, chips.size() * 4));
-    CU(cudaMemcpy(ctx->d_chips, chips.data(), chips.size() * 4, cudaMemcpyHostToDevice));
+    CU(ctx->d_chips.grow(chips.size()));
+    CU(cudaMemcpy(ctx->d_chips.get(), chips.data(), chips.size() * 4, cudaMemcpyHostToDevice));
     return GPSB200_OK;
 }
 
@@ -1574,56 +1593,24 @@ void gpsb200_destroy(gpsb200_ctx_t *ctx) {
     if (ctx->s_copy) cudaStreamSynchronize(ctx->s_copy);
     if (ctx->s_pre) cudaStreamSynchronize(ctx->s_pre);
     if (ctx->s_ck) cudaStreamSynchronize(ctx->s_ck);
-    cudaFree(ctx->d_bc);
-    cudaFreeHost(ctx->h_bc);
-    cudaFree(ctx->d_ck);
-    cudaFreeHost(ctx->h_ck);
-    cudaFree(ctx->d_carr_end);
-    cudaFree(ctx->d_atab);
-    cudaFree(ctx->d_chain_errors);
-    cudaFreeHost(ctx->h_chain_errors);
-    cudaFree(ctx->d_guess);
-    cudaFreeHost(ctx->h_guess);
-    cudaFree(ctx->d_carr0);
-    cudaFreeHost(ctx->h_carr0);
-    cudaFreeHost(ctx->h_probe);
-    cudaFree(ctx->d_probe);
-    cudaFree(ctx->d_seg);
-    cudaFreeHost(ctx->h_span_sum);
-    cudaFree(ctx->d_spec);
-    cudaFree(ctx->d_span_res);
-    cudaFreeHost(ctx->h_span_res);
-    cudaFree(ctx->d_nav);
-    cudaFreeHost(ctx->h_nav);
-    cudaFree(ctx->d_chips);
-    cudaFree(ctx->d_out);
-    cudaFree(ctx->d_rx);
-    cudaFree(ctx->d_rx_chips);
     for (auto &e : ctx->ev)
         if (e) cudaEventDestroy(e);
     for (auto &e : ctx->ev_done)
         if (e) cudaEventDestroy(e);
     for (auto &e : ctx->ev_seg)
         if (e) cudaEventDestroy(e);
-    cudaFreeHost(ctx->h_seg_end);
-    acq::scratch_free(ctx->acq);
-    trk::scratch_free(ctx->trk);
-    snap::scratch_free(ctx->snap);
-    cd::scratch_free(ctx->cd);
-    vtk::scratch_free(ctx->vtk);
-    pvt::scratch_free(ctx->pvt);
     if (ctx->s_compute) cudaStreamDestroy(ctx->s_compute);
     if (ctx->s_copy) cudaStreamDestroy(ctx->s_copy);
     if (ctx->s_pre) cudaStreamDestroy(ctx->s_pre);
     if (ctx->s_ck) cudaStreamDestroy(ctx->s_ck);
-    delete ctx;
+    delete ctx;   // frees the buffers, on the device selected above
 }
 
 int gpsb200_set_nav(gpsb200_ctx_t *ctx, int frame, int chan, const uint32_t dwrd[GPSB200_NAV_WORDS]) {
     if (!ctx || !dwrd) return GPSB200_ERR_ARG;
     if (frame < 0 || frame >= ctx->cfg.max_nav_frames || chan < 0 || chan >= ctx->cfg.max_chan)
         return fail(ctx, GPSB200_ERR_ARG, "gpsb200_set_nav: frame/channel out of range");
-    memcpy(ctx->h_nav + ((size_t) frame * ctx->cfg.max_chan + chan) * GPSB200_NAV_WORDS, dwrd, GPSB200_NAV_WORDS * 4);
+    memcpy(&ctx->h_nav[((size_t) frame * ctx->cfg.max_chan + chan) * GPSB200_NAV_WORDS], dwrd, GPSB200_NAV_WORDS * 4);
     ctx->nav_dirty = true;
     return GPSB200_OK;
 }
@@ -1756,7 +1743,7 @@ int gpsb200_debug_run_checkpoints(gpsb200_ctx_t *ctx, int nblk, int nchan, void 
     if (!ctx->s_compute) return fail(ctx, GPSB200_ERR_CUDA, "context has no CUDA device");
     CU(cudaSetDevice(ctx->cfg.device));
     CU(cudaDeviceSynchronize());             // the call's streams may be the caller's
-    CU(cudaMemcpy(out, ctx->d_ck, (size_t) nblk * ctx->nruns * nchan * sizeof(RunCkpt), cudaMemcpyDeviceToHost));
+    CU(cudaMemcpy(out, ctx->d_ck.get(), (size_t) nblk * ctx->nruns * nchan * sizeof(RunCkpt), cudaMemcpyDeviceToHost));
     return GPSB200_OK;
 }
 
@@ -1768,9 +1755,9 @@ int gpsb200_debug_block_probes(gpsb200_ctx_t *ctx, int nblk, int nchan, void *pr
     CU(cudaSetDevice(ctx->cfg.device));
     CU(cudaDeviceSynchronize());             // the call's streams may be the caller's
     const size_t cnt = (size_t) nblk * nchan;
-    CU(cudaMemcpy(probes_out, ctx->d_probe, cnt * sizeof(CarrierProbe), cudaMemcpyDeviceToHost));
-    if (seg_out) CU(cudaMemcpy(seg_out, ctx->d_seg, cnt * kSegStates * sizeof(double), cudaMemcpyDeviceToHost));
-    if (guess_out) CU(cudaMemcpy(guess_out, ctx->d_guess, cnt * sizeof(double), cudaMemcpyDeviceToHost));
+    CU(cudaMemcpy(probes_out, ctx->d_probe.get(), cnt * sizeof(CarrierProbe), cudaMemcpyDeviceToHost));
+    if (seg_out) CU(cudaMemcpy(seg_out, ctx->d_seg.get(), cnt * kSegStates * sizeof(double), cudaMemcpyDeviceToHost));
+    if (guess_out) CU(cudaMemcpy(guess_out, ctx->d_guess.get(), cnt * sizeof(double), cudaMemcpyDeviceToHost));
     return GPSB200_OK;
 }
 

@@ -1260,17 +1260,17 @@ __global__ void __launch_bounds__(kWarps * 32) k_snapshot_pick(const SnapSearchA
 }
 
 void fill(Args &a, const Scratch &sc) {
-    a.ep = sc.d_epochs;
-    a.ch = sc.d_chans;
-    a.n = sc.d_n;
+    a.ep = sc.d_epochs.get();
+    a.ch = sc.d_chans.get();
+    a.n = sc.d_n.get();
     a.nchan = sc.nchan;
     a.max_epochs = sc.max_epochs;
     a.ref = sc.ref;
     a.ref_sample = sc.ref_sample;
     a.ref_ms = sc.ref_ms;
     a.cfg = sc.cfg;
-    a.fixes = sc.d_fixes;
-    a.res = sc.want_res ? sc.d_res : nullptr;
+    a.fixes = sc.d_fixes.get();
+    a.res = sc.want_res ? sc.d_res.get() : nullptr;
 }
 
 // gpsb200_pvt_search: the satellite table, then the grid and the pick in passes of search_pass(nodes) instants, each
@@ -1279,17 +1279,17 @@ template <bool kSnap>
 cudaError_t launch_search(const Scratch &sc, cudaStream_t s) {
     typename std::conditional<kSnap, SnapSearchArgs, SearchArgs>::type a;
     fill(a, sc);
-    if constexpr (kSnap) a.meas = sc.d_meas;
+    if constexpr (kSnap) a.meas = sc.d_meas.get();
     a.sc = sc.search_cfg;
     a.sin_min = std::sin(GPSB200_SEARCH_MIN_ELEV_DEG * (M_PI / 180.0));
-    a.sat = sc.d_sat;
-    a.used = sc.d_used;
-    a.searched = sc.d_searched;
-    a.nok = sc.d_nok;
-    a.hits = reinterpret_cast<SearchHit *>(sc.d_hits);
-    a.node_rms = sc.want_node_rms ? sc.d_node_rms : nullptr;
-    a.out = sc.d_search;
-    a.ms = sc.want_ms ? sc.d_ms : nullptr;
+    a.sat = sc.d_sat.get();
+    a.used = sc.d_used.get();
+    a.searched = sc.d_searched.get();
+    a.nok = sc.d_nok.get();
+    a.hits = reinterpret_cast<SearchHit *>(sc.d_hits.get());
+    a.node_rms = sc.want_node_rms ? sc.d_node_rms.get() : nullptr;
+    a.out = sc.d_search.get();
+    a.ms = sc.want_ms ? sc.d_ms.get() : nullptr;
     a.max_ok = GPSB200_SEARCH_MAX_OK(a.sc.nodes);
     const unsigned fix_blocks = (unsigned) (((int64_t) sc.cfg.nfix + kWarps - 1) / kWarps);
     if constexpr (kSnap) k_snapshot_sats<<<fix_blocks, kWarps * 32, 0, s>>>(a);
@@ -1326,7 +1326,7 @@ cudaError_t launch(const Scratch &sc, cudaStream_t s) {
         a.raim = sc.raim_cfg;
         memcpy(a.T, sc.tab_T, sizeof a.T);
         memcpy(a.lambda, sc.tab_lambda, sizeof a.lambda);
-        a.out = sc.d_raim;
+        a.out = sc.d_raim.get();
         k_pvt<true><<<blocks, kWarps * 32, 0, s>>>(a);
         break;
     }
@@ -1336,7 +1336,7 @@ cudaError_t launch(const Scratch &sc, cudaStream_t s) {
         a.araim = sc.araim_cfg;
         memcpy(a.kh, sc.kfa_h, sizeof a.kh);
         memcpy(a.kv, sc.kfa_v, sizeof a.kv);
-        a.out = sc.d_araim;
+        a.out = sc.d_araim.get();
         k_pvt_araim<<<blocks, kWarps * 32, 0, s>>>(a);
         break;
     }
@@ -1344,8 +1344,8 @@ cudaError_t launch(const Scratch &sc, cudaStream_t s) {
         CoarseArgs a;
         fill(a, sc);
         a.ap = sc.coarse_cfg;
-        a.out = sc.d_coarse;
-        a.ms = sc.want_ms ? sc.d_ms : nullptr;
+        a.out = sc.d_coarse.get();
+        a.ms = sc.want_ms ? sc.d_ms.get() : nullptr;
         k_pvt_coarse<<<blocks, kWarps * 32, 0, s>>>(a);
         break;
     }
@@ -1353,9 +1353,9 @@ cudaError_t launch(const Scratch &sc, cudaStream_t s) {
         SnapCoarseArgs a;
         fill(a, sc);
         a.ap = sc.coarse_cfg;
-        a.out = sc.d_coarse;
-        a.ms = sc.want_ms ? sc.d_ms : nullptr;
-        a.meas = sc.d_meas;
+        a.out = sc.d_coarse.get();
+        a.ms = sc.want_ms ? sc.d_ms.get() : nullptr;
+        a.meas = sc.d_meas.get();
         k_pvt_snapshot<<<blocks, kWarps * 32, 0, s>>>(a);
         break;
     }
@@ -1456,44 +1456,21 @@ std::string check(const gpsb200_pvt_chan_t *chans, int nchan, const gpsb200_trac
     return std::string();
 }
 
-void scratch_free(Scratch &sc) {
-    cudaFree(sc.d_epochs);
-    cudaFree(sc.d_chans);
-    cudaFree(sc.d_n);
-    cudaFree(sc.d_fixes);
-    cudaFree(sc.d_res);
-    cudaFree(sc.d_raim);
-    cudaFree(sc.d_araim);
-    cudaFree(sc.d_coarse);
-    cudaFree(sc.d_ms);
-    cudaFree(sc.d_search);
-    cudaFree(sc.d_sat);
-    cudaFree(sc.d_used);
-    cudaFree(sc.d_searched);
-    cudaFree(sc.d_nok);
-    cudaFree(sc.d_hits);
-    cudaFree(sc.d_node_rms);
-    cudaFree(sc.d_meas);
-    sc = Scratch();
-}
-
 cudaError_t run(Scratch &sc, const gpsb200_pvt_chan_t *chans, int nchan, const gpsb200_track_epoch_t *epochs,
                 const int32_t *nepochs, int max_epochs, const gpsb200_pvt_config_t *cfg, gpsb200_fix_t *fixes,
                 double *residuals, const Stage &st, cudaStream_t s) {
     const size_t nf = (size_t) cfg->nfix;
     sc.have_last = false;
-    if (!sc.d_chans) {
-        CU_RET(cudaMalloc(&sc.d_chans, GPSB200_TRK_MAX_CHAN * sizeof(gpsb200_pvt_chan_t)));
-        CU_RET(cudaMalloc(&sc.d_n, GPSB200_TRK_MAX_CHAN * sizeof(int32_t)));
-    }
-    if (st.meas) CU_RET(grow(sc.d_meas, sc.meas_cap, nf * nchan));
-    else CU_RET(grow(sc.d_epochs, sc.epoch_cap, (size_t) nchan * max_epochs));
-    CU_RET(grow(sc.d_fixes, sc.fix_cap, nf));
-    if (residuals) CU_RET(grow(sc.d_res, sc.res_cap, nf * nchan));
-    if (st.ms) CU_RET(grow(sc.d_ms, sc.ms_cap, nf * nchan));
+    CU_RET(sc.d_chans.grow(GPSB200_TRK_MAX_CHAN));
+    CU_RET(sc.d_n.grow(GPSB200_TRK_MAX_CHAN));
+    if (st.meas) CU_RET(sc.d_meas.grow(nf * nchan));
+    else CU_RET(sc.d_epochs.grow((size_t) nchan * max_epochs));
+    CU_RET(sc.d_fixes.grow(nf));
+    if (residuals) CU_RET(sc.d_res.grow(nf * nchan));
+    if (st.ms) CU_RET(sc.d_ms.grow(nf * nchan));
     sc.mode = st.mode();
     if (st.raim) {
-        CU_RET(grow(sc.d_raim, sc.raim_cap, nf));
+        CU_RET(sc.d_raim.grow(nf));
         sc.raim_cfg = *st.raim;
         if (st.raim->p_fa != sc.tab_p_fa || st.raim->p_md != sc.tab_p_md) {   // the tables take 20-80 ms of host time
             raim_thresholds(st.raim->p_fa, st.raim->p_md, sc.tab_T, sc.tab_lambda);
@@ -1502,24 +1479,24 @@ cudaError_t run(Scratch &sc, const gpsb200_pvt_chan_t *chans, int nchan, const g
         }
     }
     if (st.araim) {
-        CU_RET(grow(sc.d_araim, sc.araim_cap, nf));
+        CU_RET(sc.d_araim.grow(nf));
         sc.araim_cfg = *st.araim;
         araim_kfa(st.araim->p_fa_vert, st.araim->p_fa_horz, sc.kfa_h, sc.kfa_v);
     }
     if (st.coarse) {
-        CU_RET(grow(sc.d_coarse, sc.coarse_cap, nf));
+        CU_RET(sc.d_coarse.grow(nf));
         sc.coarse_cfg = *st.coarse;
     }
     if (st.search) {
         const int nodes = st.search->nodes;
-        CU_RET(grow(sc.d_search, sc.search_cap, nf));
-        CU_RET(grow(sc.d_sat, sc.sat_cap, nf * 32 * 3));
-        CU_RET(grow(sc.d_used, sc.used_cap, nf));
-        CU_RET(grow(sc.d_searched, sc.searched_cap, nf));
-        CU_RET(grow(sc.d_nok, sc.nok_cap, nf));
+        CU_RET(sc.d_search.grow(nf));
+        CU_RET(sc.d_sat.grow(nf * 32 * 3));
+        CU_RET(sc.d_used.grow(nf));
+        CU_RET(sc.d_searched.grow(nf));
+        CU_RET(sc.d_nok.grow(nf));
         const size_t pass = (size_t) std::min<int64_t>(search_pass(nodes), cfg->nfix);
-        CU_RET(grow(sc.d_hits, sc.hits_cap, pass * GPSB200_SEARCH_MAX_OK(nodes) * sizeof(SearchHit) / sizeof(double)));
-        if (st.node_rms) CU_RET(grow(sc.d_node_rms, sc.node_rms_cap, nf * nodes));
+        CU_RET(sc.d_hits.grow(pass * GPSB200_SEARCH_MAX_OK(nodes) * sizeof(SearchHit) / sizeof(double)));
+        if (st.node_rms) CU_RET(sc.d_node_rms.grow(nf * nodes));
         sc.search_cfg = *st.search;
     }
     sc.want_ms = st.ms != nullptr;
@@ -1536,25 +1513,26 @@ cudaError_t run(Scratch &sc, const gpsb200_pvt_chan_t *chans, int nchan, const g
     sc.cfg = *cfg;
     sc.want_res = residuals != nullptr;
     if (st.meas) {
-        CU_RET(cudaMemcpyAsync(sc.d_meas, st.meas, nf * nchan * sizeof(gpsb200_snapshot_t), cudaMemcpyHostToDevice, s));
-    } else {
-        CU_RET(cudaMemcpyAsync(sc.d_epochs, epochs, (size_t) nchan * max_epochs * sizeof(gpsb200_track_epoch_t),
+        CU_RET(cudaMemcpyAsync(sc.d_meas.get(), st.meas, nf * nchan * sizeof(gpsb200_snapshot_t),
                                cudaMemcpyHostToDevice, s));
-        CU_RET(cudaMemcpyAsync(sc.d_n, nepochs, nchan * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+    } else {
+        CU_RET(cudaMemcpyAsync(sc.d_epochs.get(), epochs, (size_t) nchan * max_epochs * sizeof(gpsb200_track_epoch_t),
+                               cudaMemcpyHostToDevice, s));
+        CU_RET(cudaMemcpyAsync(sc.d_n.get(), nepochs, nchan * sizeof(int32_t), cudaMemcpyHostToDevice, s));
     }
-    CU_RET(cudaMemcpyAsync(sc.d_chans, chans, nchan * sizeof(gpsb200_pvt_chan_t), cudaMemcpyHostToDevice, s));
+    CU_RET(cudaMemcpyAsync(sc.d_chans.get(), chans, nchan * sizeof(gpsb200_pvt_chan_t), cudaMemcpyHostToDevice, s));
     CU_RET(launch(sc, s));
     const auto down = [&](void *dst, const void *src, size_t bytes) {
         return cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, s);
     };
-    CU_RET(down(fixes, sc.d_fixes, nf * sizeof(gpsb200_fix_t)));
-    if (residuals) CU_RET(down(residuals, sc.d_res, nf * nchan * sizeof(double)));
-    if (st.raim) CU_RET(down(st.raim_out, sc.d_raim, nf * sizeof(gpsb200_raim_t)));
-    if (st.araim) CU_RET(down(st.araim_out, sc.d_araim, nf * sizeof(gpsb200_araim_t)));
-    if (st.coarse) CU_RET(down(st.coarse_out, sc.d_coarse, nf * sizeof(gpsb200_coarse_t)));
-    if (st.search) CU_RET(down(st.search_out, sc.d_search, nf * sizeof(gpsb200_search_t)));
-    if (st.ms) CU_RET(down(st.ms, sc.d_ms, nf * nchan * sizeof(int64_t)));
-    if (st.node_rms) CU_RET(down(st.node_rms, sc.d_node_rms, nf * st.search->nodes * sizeof(double)));
+    CU_RET(down(fixes, sc.d_fixes.get(), nf * sizeof(gpsb200_fix_t)));
+    if (residuals) CU_RET(down(residuals, sc.d_res.get(), nf * nchan * sizeof(double)));
+    if (st.raim) CU_RET(down(st.raim_out, sc.d_raim.get(), nf * sizeof(gpsb200_raim_t)));
+    if (st.araim) CU_RET(down(st.araim_out, sc.d_araim.get(), nf * sizeof(gpsb200_araim_t)));
+    if (st.coarse) CU_RET(down(st.coarse_out, sc.d_coarse.get(), nf * sizeof(gpsb200_coarse_t)));
+    if (st.search) CU_RET(down(st.search_out, sc.d_search.get(), nf * sizeof(gpsb200_search_t)));
+    if (st.ms) CU_RET(down(st.ms, sc.d_ms.get(), nf * nchan * sizeof(int64_t)));
+    if (st.node_rms) CU_RET(down(st.node_rms, sc.d_node_rms.get(), nf * st.search->nodes * sizeof(double)));
     CU_RET(cudaStreamSynchronize(s));
     sc.have_last = true;
     return cudaSuccess;

@@ -6,6 +6,7 @@
 #include <string>
 
 #include "../../include/gpsb200.h"
+#include "device_buffer.h"
 
 namespace gpsb200 {
 namespace pvt {
@@ -66,14 +67,11 @@ bool araim_kfa(double p_fa_vert, double p_fa_horz, double *kh, double *kv);
 
 // Device scratch of the fix calls of one context, grown as needed, and what gpsb200_pvt_replay re-runs.
 struct Scratch {
-    gpsb200_track_epoch_t *d_epochs = nullptr;   // [nchan][max_epochs]
-    size_t epoch_cap = 0;
-    gpsb200_pvt_chan_t *d_chans = nullptr;       // [GPSB200_TRK_MAX_CHAN]
-    int32_t *d_n = nullptr;                      // [GPSB200_TRK_MAX_CHAN]
-    gpsb200_fix_t *d_fixes = nullptr;            // [nfix]
-    size_t fix_cap = 0;
-    double *d_res = nullptr;                     // [nfix][nchan]
-    size_t res_cap = 0;
+    DeviceArray<gpsb200_track_epoch_t> d_epochs;  // [nchan][max_epochs]
+    DeviceArray<gpsb200_pvt_chan_t> d_chans;     // [GPSB200_TRK_MAX_CHAN]
+    DeviceArray<int32_t> d_n;                    // [GPSB200_TRK_MAX_CHAN]
+    DeviceArray<gpsb200_fix_t> d_fixes;          // [nfix]
+    DeviceArray<double> d_res;                   // [nfix][nchan]
     bool have_last = false;                      // the arguments of the previous call, for replay
     int nchan = 0, max_epochs = 0, ref = -1;
     int64_t ref_sample = 0, ref_ms = 0;
@@ -82,42 +80,30 @@ struct Scratch {
     Mode mode = Mode::plain;
     // the RAIM stage of the previous call (gpsb200_pvt_raim), and the tables of the last p_fa / p_md seen
     gpsb200_raim_config_t raim_cfg{};
-    gpsb200_raim_t *d_raim = nullptr;            // [nfix]
-    size_t raim_cap = 0;
+    DeviceArray<gpsb200_raim_t> d_raim;          // [nfix]
     double tab_p_fa = 0.0, tab_p_md = 0.0;       // 0: no tables yet
     double tab_T[GPSB200_RAIM_MAX_DOF] = {}, tab_lambda[GPSB200_RAIM_MAX_DOF] = {};
     // the ARAIM stage of the previous call (gpsb200_pvt_araim)
     gpsb200_araim_config_t araim_cfg{};
-    gpsb200_araim_t *d_araim = nullptr;          // [nfix]
-    size_t araim_cap = 0;
+    DeviceArray<gpsb200_araim_t> d_araim;        // [nfix]
     double kfa_h[GPSB200_RAIM_MAX_DOF] = {}, kfa_v[GPSB200_RAIM_MAX_DOF] = {};
     // the coarse-time call of the previous call (gpsb200_pvt_coarse)
     bool want_ms = false;
     gpsb200_coarse_config_t coarse_cfg{};
-    gpsb200_coarse_t *d_coarse = nullptr;        // [nfix]
-    size_t coarse_cap = 0;
-    int64_t *d_ms = nullptr;                     // [nfix][nchan]
-    size_t ms_cap = 0;
+    DeviceArray<gpsb200_coarse_t> d_coarse;      // [nfix]
+    DeviceArray<int64_t> d_ms;                   // [nfix][nchan]
     // the search of the previous call (gpsb200_pvt_search): records, and the per-instant scratch of pvt.cu's kernels
     bool want_node_rms = false;
     gpsb200_search_config_t search_cfg{};
-    gpsb200_search_t *d_search = nullptr;        // [nfix]
-    size_t search_cap = 0;
-    double *d_sat = nullptr;                     // [nfix][32][3]
-    size_t sat_cap = 0;
-    uint32_t *d_used = nullptr;                  // [nfix]
-    size_t used_cap = 0;
-    int32_t *d_searched = nullptr, *d_nok = nullptr;   // [nfix]
-    size_t searched_cap = 0, nok_cap = 0;
-    double *d_hits = nullptr;                    // one pass's OK-node lists (pvt.cu: SearchHit, search_pass)
-    size_t hits_cap = 0;
-    double *d_node_rms = nullptr;                // [nfix][nodes], only when the caller asks for it
-    size_t node_rms_cap = 0;
-    gpsb200_snapshot_t *d_meas = nullptr;        // [nfix][nchan]: the snapshot records of a snapshot call
-    size_t meas_cap = 0;
+    DeviceArray<gpsb200_search_t> d_search;      // [nfix]
+    DeviceArray<double> d_sat;                   // [nfix][32][3]
+    DeviceArray<uint32_t> d_used;                // [nfix]
+    DeviceArray<int32_t> d_searched, d_nok;      // [nfix]
+    DeviceArray<double> d_hits;                  // one pass's OK-node lists (pvt.cu: SearchHit, search_pass)
+    DeviceArray<double> d_node_rms;              // [nfix][nodes], only when the caller asks for it
+    DeviceArray<gpsb200_snapshot_t> d_meas;      // [nfix][nchan]: the snapshot records of a snapshot call
 };
 
-void scratch_free(Scratch &sc);
 // Upload, run the kernels of st's stage on s and download the fixes [nfix], the residuals [nfix][nchan] (when not NULL)
 // and the stage's outputs; waits for the results.
 cudaError_t run(Scratch &sc, const gpsb200_pvt_chan_t *chans, int nchan, const gpsb200_track_epoch_t *epochs,

@@ -238,23 +238,18 @@ int batch_pass(const gpsb200_acq_config_t *acq, int sample_size, int nwin) {
     return (int) std::max<int64_t>(1, std::min<int64_t>(w, nwin));
 }
 
-void scratch_free(Scratch &sc) {
-    cudaFree(sc.d_rec);
-    cudaFree(sc.d_brec);
-    sc = Scratch();
-}
-
 cudaError_t launch(Scratch &sc, const void *window, int sample_size, int K, int nprn, const int8_t *chips, int iterations,
                    gpsb200_snapshot_t *rec, cudaStream_t s) {
-    if (!sc.d_rec) CU_RET(cudaMalloc(&sc.d_rec, 32 * sizeof(gpsb200_snapshot_t)));
-    CU_RET(cudaMemcpyAsync(sc.d_rec, rec, nprn * sizeof(gpsb200_snapshot_t), cudaMemcpyHostToDevice, s));
+    CU_RET(sc.d_rec.grow(32));
+    CU_RET(cudaMemcpyAsync(sc.d_rec.get(), rec, nprn * sizeof(gpsb200_snapshot_t), cudaMemcpyHostToDevice, s));
     if (sample_size == GPSB200_SC08)
-        k_snapshot<int8_t><<<nprn, kThreads, 0, s>>>(static_cast<const int8_t *>(window), K, chips, iterations, sc.d_rec);
+        k_snapshot<int8_t><<<nprn, kThreads, 0, s>>>(static_cast<const int8_t *>(window), K, chips, iterations,
+                                                     sc.d_rec.get());
     else
         k_snapshot<int16_t><<<nprn, kThreads, 0, s>>>(static_cast<const int16_t *>(window), K, chips, iterations,
-                                                      sc.d_rec);
+                                                      sc.d_rec.get());
     CU_RET(cudaGetLastError());
-    CU_RET(cudaMemcpyAsync(rec, sc.d_rec, nprn * sizeof(gpsb200_snapshot_t), cudaMemcpyDeviceToHost, s));
+    CU_RET(cudaMemcpyAsync(rec, sc.d_rec.get(), nprn * sizeof(gpsb200_snapshot_t), cudaMemcpyDeviceToHost, s));
     return cudaStreamSynchronize(s);
 }
 
@@ -262,16 +257,16 @@ cudaError_t launch_batch(Scratch &sc, const void *src, int sample_size, int K, i
                          const int64_t *d_win_off, const int8_t *chips, int iterations, gpsb200_snapshot_t *rec,
                          cudaStream_t s) {
     const int n = nwin * nprn;
-    CU_RET(grow(sc.d_brec, sc.brec_cap, (size_t) n));
-    CU_RET(cudaMemcpyAsync(sc.d_brec, rec, n * sizeof(gpsb200_snapshot_t), cudaMemcpyHostToDevice, s));
+    CU_RET(sc.d_brec.grow((size_t) n));
+    CU_RET(cudaMemcpyAsync(sc.d_brec.get(), rec, n * sizeof(gpsb200_snapshot_t), cudaMemcpyHostToDevice, s));
     if (sample_size == GPSB200_SC08)
         k_snapshot_batch<int8_t><<<n, kThreads, 0, s>>>(static_cast<const int8_t *>(src), d_win_off, nprn, K, chips,
-                                                        iterations, sc.d_brec);
+                                                        iterations, sc.d_brec.get());
     else
         k_snapshot_batch<int16_t><<<n, kThreads, 0, s>>>(static_cast<const int16_t *>(src), d_win_off, nprn, K, chips,
-                                                         iterations, sc.d_brec);
+                                                         iterations, sc.d_brec.get());
     CU_RET(cudaGetLastError());
-    CU_RET(cudaMemcpyAsync(rec, sc.d_brec, n * sizeof(gpsb200_snapshot_t), cudaMemcpyDeviceToHost, s));
+    CU_RET(cudaMemcpyAsync(rec, sc.d_brec.get(), n * sizeof(gpsb200_snapshot_t), cudaMemcpyDeviceToHost, s));
     return cudaStreamSynchronize(s);
 }
 

@@ -7,6 +7,7 @@
 #include <string>
 
 #include "../../include/gpsb200.h"
+#include "device_buffer.h"
 
 namespace gpsb200 {
 namespace snap {
@@ -26,11 +27,9 @@ void seed(const gpsb200_acq_config_t *acq, const gpsb200_acq_result_t *res, cons
           gpsb200_snapshot_t *out);
 
 struct Scratch {
-    gpsb200_snapshot_t *d_rec = nullptr;   // [32]
-    gpsb200_snapshot_t *d_brec = nullptr;  // [nwin][nprn] of a batch pass
-    size_t brec_cap = 0;
+    DeviceArray<gpsb200_snapshot_t> d_rec;    // [32]
+    DeviceArray<gpsb200_snapshot_t> d_brec;   // [nwin][nprn] of a batch pass
 };
-void scratch_free(Scratch &sc);
 // Enqueue the refinement of rec [nprn] (seeded) over the window at `window` (stream sample s0 first) on s and wait for
 // the records. chips: [33][1023] chips as +-1 (trk::chips_upload).
 cudaError_t launch(Scratch &sc, const void *window, int sample_size, int K, int nprn, const int8_t *chips, int iterations,

@@ -139,50 +139,41 @@ void start_steps(double doppler_hz, int32_t &w, uint32_t &u) {
     u = code_step(w);
 }
 
-cudaError_t chips_upload(int8_t **d) {
+cudaError_t chips_upload(DeviceArray<int8_t> &d) {
     std::vector<int8_t> c((size_t) 33 * GPSB200_CA_LEN, 0);
     for (int prn = 1; prn <= 32; prn++) {
         uint8_t ca[GPSB200_CA_LEN];
         ca_code(prn, ca);
         for (int i = 0; i < GPSB200_CA_LEN; i++) c[(size_t) prn * GPSB200_CA_LEN + i] = (int8_t) (2 * ca[i] - 1);
     }
-    CU_RET(cudaMalloc(d, c.size()));
-    return cudaMemcpy(*d, c.data(), c.size(), cudaMemcpyHostToDevice);
+    CU_RET(d.grow(c.size()));
+    return cudaMemcpy(d.get(), c.data(), c.size(), cudaMemcpyHostToDevice);
 }
 
 cudaError_t scratch_reserve(Scratch &sc, int nchan, int max_epochs) {
-    if (!sc.d_state) {
-        CU_RET(cudaMalloc(&sc.d_state, GPSB200_TRK_MAX_CHAN * sizeof(gpsb200_track_state_t)));
-        CU_RET(cudaMalloc(&sc.d_n, GPSB200_TRK_MAX_CHAN * sizeof(int32_t)));
-    }
-    return grow(sc.d_epochs, sc.epoch_cap, (size_t) nchan * max_epochs);
-}
-
-void scratch_free(Scratch &sc) {
-    cudaFree(sc.d_state);
-    cudaFree(sc.d_epochs);
-    cudaFree(sc.d_n);
-    sc = Scratch();
+    CU_RET(sc.d_state.grow(GPSB200_TRK_MAX_CHAN));
+    CU_RET(sc.d_n.grow(GPSB200_TRK_MAX_CHAN));
+    return sc.d_epochs.grow((size_t) nchan * max_epochs);
 }
 
 cudaError_t launch(Scratch &sc, const int8_t *chips, const void *src, int64_t nsamples, int sample_size, int64_t base,
                    gpsb200_track_state_t *state, int nchan, int max_epochs, gpsb200_track_epoch_t *epochs,
                    int32_t *nepochs, cudaStream_t s) {
-    CU_RET(cudaMemcpyAsync(sc.d_state, state, nchan * sizeof(gpsb200_track_state_t), cudaMemcpyHostToDevice, s));
+    CU_RET(cudaMemcpyAsync(sc.d_state.get(), state, nchan * sizeof(gpsb200_track_state_t), cudaMemcpyHostToDevice, s));
     if (sample_size == GPSB200_SC08)
         k_track<int8_t><<<nchan, kThreads, 0, s>>>(static_cast<const int8_t *>(src), nsamples, base, chips,
-                                                   sc.d_state, max_epochs, sc.d_epochs, sc.d_n);
+                                                   sc.d_state.get(), max_epochs, sc.d_epochs.get(), sc.d_n.get());
     else
         k_track<int16_t><<<nchan, kThreads, 0, s>>>(static_cast<const int16_t *>(src), nsamples, base, chips,
-                                                    sc.d_state, max_epochs, sc.d_epochs, sc.d_n);
+                                                    sc.d_state.get(), max_epochs, sc.d_epochs.get(), sc.d_n.get());
     CU_RET(cudaGetLastError());
-    CU_RET(cudaMemcpyAsync(nepochs, sc.d_n, nchan * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
-    CU_RET(cudaMemcpyAsync(state, sc.d_state, nchan * sizeof(gpsb200_track_state_t), cudaMemcpyDeviceToHost, s));
+    CU_RET(cudaMemcpyAsync(nepochs, sc.d_n.get(), nchan * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+    CU_RET(cudaMemcpyAsync(state, sc.d_state.get(), nchan * sizeof(gpsb200_track_state_t), cudaMemcpyDeviceToHost, s));
     CU_RET(cudaStreamSynchronize(s));
     // the epochs of channel c sit at c * max_epochs; copy only the written ones
     for (int c = 0; c < nchan; c++)
         if (nepochs[c] > 0)
-            CU_RET(cudaMemcpyAsync(epochs + (size_t) c * max_epochs, sc.d_epochs + (size_t) c * max_epochs,
+            CU_RET(cudaMemcpyAsync(epochs + (size_t) c * max_epochs, sc.d_epochs.get() + (size_t) c * max_epochs,
                                    (size_t) nepochs[c] * sizeof(gpsb200_track_epoch_t), cudaMemcpyDeviceToHost, s));
     return cudaStreamSynchronize(s);
 }

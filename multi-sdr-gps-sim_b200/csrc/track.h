@@ -7,6 +7,7 @@
 #include <string>
 
 #include "../../include/gpsb200.h"
+#include "device_buffer.h"
 
 namespace gpsb200 {
 namespace trk {
@@ -129,19 +130,17 @@ __host__ __device__ inline int period_len(uint64_t phi, uint32_t u) { return (in
 std::string check(const gpsb200_track_state_t *st, int nchan, int max_epochs, int64_t nsamples, int64_t base,
                   int sample_size);
 
-// The [33][1023] C/A chips as +-1 (row 0 unused) that k_track and k_snapshot read, in a new device buffer *d.
-cudaError_t chips_upload(int8_t **d);
+// The [33][1023] C/A chips as +-1 (row 0 unused) that k_track and k_snapshot read, written into d.
+cudaError_t chips_upload(DeviceArray<int8_t> &d);
 
 // Device scratch of the tracking calls of one context, grown as needed.
 struct Scratch {
-    gpsb200_track_state_t *d_state = nullptr;    // [GPSB200_TRK_MAX_CHAN]
-    gpsb200_track_epoch_t *d_epochs = nullptr;   // [nchan][max_epochs]
-    size_t epoch_cap = 0;
-    int32_t *d_n = nullptr;                      // [GPSB200_TRK_MAX_CHAN]
+    DeviceArray<gpsb200_track_state_t> d_state;    // [GPSB200_TRK_MAX_CHAN]
+    DeviceArray<gpsb200_track_epoch_t> d_epochs;   // [nchan][max_epochs]
+    DeviceArray<int32_t> d_n;                      // [GPSB200_TRK_MAX_CHAN]
 };
 
 cudaError_t scratch_reserve(Scratch &sc, int nchan, int max_epochs);
-void scratch_free(Scratch &sc);
 // Enqueue the tracking of the samples at `src` (stream sample `base` first) on s and wait for the results.
 // chips: chips_upload's table.
 cudaError_t launch(Scratch &sc, const int8_t *chips, const void *src, int64_t nsamples, int sample_size, int64_t base,

@@ -596,25 +596,13 @@ std::string check(const gpsb200_vtrack_state_t *st, const gpsb200_pvt_chan_t *ch
 }
 
 cudaError_t scratch_reserve(Scratch &sc, int nchan, int max_updates, int max_epochs) {
-    if (!sc.d_state) {
-        CU_RET(cudaMalloc(&sc.d_state, sizeof(gpsb200_vtrack_state_t)));
-        CU_RET(cudaMalloc(&sc.d_chans, kMaxChan * sizeof(gpsb200_pvt_chan_t)));
-        CU_RET(cudaMalloc(&sc.d_n, (kMaxChan + 1) * sizeof(int32_t)));
-    }
-    CU_RET(grow(sc.d_fix, sc.upd_cap, (size_t) max_updates));
-    CU_RET(grow(sc.d_out, sc.out_cap, (size_t) max_updates * nchan));
-    if (max_epochs > 0) CU_RET(grow(sc.d_epochs, sc.epoch_cap, (size_t) nchan * max_epochs));
+    CU_RET(sc.d_state.grow(1));
+    CU_RET(sc.d_chans.grow(kMaxChan));
+    CU_RET(sc.d_n.grow(kMaxChan + 1));
+    CU_RET(sc.d_fix.grow((size_t) max_updates));
+    CU_RET(sc.d_out.grow((size_t) max_updates * nchan));
+    if (max_epochs > 0) CU_RET(sc.d_epochs.grow((size_t) nchan * max_epochs));
     return cudaSuccess;
-}
-
-void scratch_free(Scratch &sc) {
-    cudaFree(sc.d_state);
-    cudaFree(sc.d_chans);
-    cudaFree(sc.d_n);
-    cudaFree(sc.d_fix);
-    cudaFree(sc.d_out);
-    cudaFree(sc.d_epochs);
-    sc = Scratch();
 }
 
 cudaError_t launch(Scratch &sc, const int8_t *chips, const void *src, int64_t nsamples, int sample_size, int64_t base,
@@ -624,31 +612,34 @@ cudaError_t launch(Scratch &sc, const int8_t *chips, const void *src, int64_t ns
     const int nchan = state->nchan;
     const int K = ctas > 0 ? (ctas < nchan ? ctas : nchan) : (nchan < 8 ? nchan : 8);
     const size_t dyn = (size_t) ((nchan + K - 1) / K) * 1024;
-    CU_RET(cudaMemcpyAsync(sc.d_state, state, sizeof(gpsb200_vtrack_state_t), cudaMemcpyHostToDevice, s));
-    CU_RET(cudaMemcpyAsync(sc.d_chans, chans, nchan * sizeof(gpsb200_pvt_chan_t), cudaMemcpyHostToDevice, s));
-    CU_RET(cudaMemsetAsync(sc.d_n, 0, (kMaxChan + 1) * sizeof(int32_t), s));
-    gpsb200_track_epoch_t *dep = epochs ? sc.d_epochs : nullptr;
+    CU_RET(cudaMemcpyAsync(sc.d_state.get(), state, sizeof(gpsb200_vtrack_state_t), cudaMemcpyHostToDevice, s));
+    CU_RET(cudaMemcpyAsync(sc.d_chans.get(), chans, nchan * sizeof(gpsb200_pvt_chan_t), cudaMemcpyHostToDevice, s));
+    CU_RET(cudaMemsetAsync(sc.d_n.get(), 0, (kMaxChan + 1) * sizeof(int32_t), s));
+    gpsb200_track_epoch_t *dep = epochs ? sc.d_epochs.get() : nullptr;
     if (sample_size == GPSB200_SC08)
-        CU_RET(launch_k<int8_t>(K, dyn, s, static_cast<const int8_t *>(src), nsamples, base, chips, sc.d_chans, *cfg,
-                                sc.d_state, max_updates, sc.d_fix, sc.d_out, dep, max_epochs, sc.d_n));
+        CU_RET(launch_k<int8_t>(K, dyn, s, static_cast<const int8_t *>(src), nsamples, base, chips, sc.d_chans.get(),
+                                *cfg, sc.d_state.get(), max_updates, sc.d_fix.get(), sc.d_out.get(), dep, max_epochs,
+                                sc.d_n.get()));
     else
-        CU_RET(launch_k<int16_t>(K, dyn, s, static_cast<const int16_t *>(src), nsamples, base, chips, sc.d_chans, *cfg,
-                                 sc.d_state, max_updates, sc.d_fix, sc.d_out, dep, max_epochs, sc.d_n));
+        CU_RET(launch_k<int16_t>(K, dyn, s, static_cast<const int16_t *>(src), nsamples, base, chips, sc.d_chans.get(),
+                                 *cfg, sc.d_state.get(), max_updates, sc.d_fix.get(), sc.d_out.get(), dep, max_epochs,
+                                 sc.d_n.get()));
     int32_t n[kMaxChan + 1];
-    CU_RET(cudaMemcpyAsync(n, sc.d_n, sizeof n, cudaMemcpyDeviceToHost, s));
-    CU_RET(cudaMemcpyAsync(state, sc.d_state, sizeof(gpsb200_vtrack_state_t), cudaMemcpyDeviceToHost, s));
+    CU_RET(cudaMemcpyAsync(n, sc.d_n.get(), sizeof n, cudaMemcpyDeviceToHost, s));
+    CU_RET(cudaMemcpyAsync(state, sc.d_state.get(), sizeof(gpsb200_vtrack_state_t), cudaMemcpyDeviceToHost, s));
     CU_RET(cudaStreamSynchronize(s));
     *nupdates = n[kMaxChan];
     if (n[kMaxChan] > 0) {
-        CU_RET(cudaMemcpyAsync(fixes, sc.d_fix, (size_t) n[kMaxChan] * sizeof(gpsb200_fix_t), cudaMemcpyDeviceToHost, s));
-        CU_RET(cudaMemcpyAsync(out, sc.d_out, (size_t) n[kMaxChan] * nchan * sizeof(gpsb200_vtrack_chan_t),
+        CU_RET(cudaMemcpyAsync(fixes, sc.d_fix.get(), (size_t) n[kMaxChan] * sizeof(gpsb200_fix_t),
+                               cudaMemcpyDeviceToHost, s));
+        CU_RET(cudaMemcpyAsync(out, sc.d_out.get(), (size_t) n[kMaxChan] * nchan * sizeof(gpsb200_vtrack_chan_t),
                                cudaMemcpyDeviceToHost, s));
     }
     if (epochs)
         for (int c = 0; c < nchan; c++) {
             nepochs[c] = n[c];
             if (n[c] > 0)
-                CU_RET(cudaMemcpyAsync(epochs + (size_t) c * max_epochs, sc.d_epochs + (size_t) c * max_epochs,
+                CU_RET(cudaMemcpyAsync(epochs + (size_t) c * max_epochs, sc.d_epochs.get() + (size_t) c * max_epochs,
                                        (size_t) n[c] * sizeof(gpsb200_track_epoch_t), cudaMemcpyDeviceToHost, s));
         }
     return cudaStreamSynchronize(s);

@@ -7,6 +7,7 @@
 #include <string>
 
 #include "../../include/gpsb200.h"
+#include "device_buffer.h"
 
 namespace gpsb200 {
 namespace vtk {
@@ -20,18 +21,15 @@ std::string check_config(const gpsb200_vtrack_config_t *cfg);
 
 // Device scratch of the vector-tracking calls of one context, grown as needed.
 struct Scratch {
-    gpsb200_vtrack_state_t *d_state = nullptr;
-    gpsb200_pvt_chan_t *d_chans = nullptr;        // [GPSB200_TRK_MAX_CHAN]
-    int32_t *d_n = nullptr;                       // [GPSB200_TRK_MAX_CHAN + 1]: nepochs, then nupdates
-    gpsb200_fix_t *d_fix = nullptr;
-    gpsb200_vtrack_chan_t *d_out = nullptr;
-    size_t upd_cap = 0, out_cap = 0;
-    gpsb200_track_epoch_t *d_epochs = nullptr;
-    size_t epoch_cap = 0;
+    DeviceArray<gpsb200_vtrack_state_t> d_state;   // [1]
+    DeviceArray<gpsb200_pvt_chan_t> d_chans;       // [GPSB200_TRK_MAX_CHAN]
+    DeviceArray<int32_t> d_n;                      // [GPSB200_TRK_MAX_CHAN + 1]: nepochs, then nupdates
+    DeviceArray<gpsb200_fix_t> d_fix;              // [max_updates]
+    DeviceArray<gpsb200_vtrack_chan_t> d_out;      // [max_updates][nchan]
+    DeviceArray<gpsb200_track_epoch_t> d_epochs;   // [nchan][max_epochs]
 };
 
 cudaError_t scratch_reserve(Scratch &sc, int nchan, int max_updates, int max_epochs);
-void scratch_free(Scratch &sc);
 // Enqueue the call on s with a cluster of `ctas` CTAs (0: min(nchan, 8)) and wait for the results.
 cudaError_t launch(Scratch &sc, const int8_t *chips, const void *src, int64_t nsamples, int sample_size, int64_t base,
                    const gpsb200_pvt_chan_t *chans, const gpsb200_vtrack_config_t *cfg, gpsb200_vtrack_state_t *state,
