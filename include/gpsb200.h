@@ -1211,7 +1211,9 @@ typedef struct gpsb200_vtrack_chan {
  * sb 10 m, sd 1 m/s). */
 void gpsb200_vtrack_config_default(gpsb200_vtrack_config_t *cfg);
 /* The seed (see above): x8 = X, t_rx at stream sample s0 (>= 0), nchan PRNs (1..32). GPSB200_ERR_ARG on a bad argument
- * (NULL pointers, nchan out of range, a non-finite X or t_rx outside [0, 604800), the config's sigmas). Host only. */
+ * (NULL pointers, nchan out of range, a non-finite X or t_rx outside [0, 604800), the config's sigmas). Host only.
+ * A PRN may appear on one channel only (here and in the state gpsb200_vtrack reads): two channels on one satellite
+ * would enter the filter as independent measurements and make the PDOP's normal matrix singular. */
 int gpsb200_vtrack_seed(const gpsb200_vtrack_config_t *cfg, const double *x8, double t_rx, int64_t s0,
                         const int32_t *prn, int nchan, gpsb200_vtrack_state_t *state);
 /* Vector-track state->nchan channels over nsamples samples of host memory (int8 / int16 I,Q interleaved; stream sample

@@ -1904,8 +1904,11 @@ int gpsb200_vtrack_seed(const gpsb200_vtrack_config_t *cfg, const double *x8, do
     if (!vtk::check_config(cfg).empty()) return GPSB200_ERR_ARG;
     for (int i = 0; i < 8; i++)
         if (!std::isfinite(x8[i])) return GPSB200_ERR_ARG;
-    for (int c = 0; c < nchan; c++)
-        if (prn[c] < 1 || prn[c] > 32) return GPSB200_ERR_ARG;
+    uint32_t seen = 0;
+    for (int c = 0; c < nchan; c++) {
+        if (prn[c] < 1 || prn[c] > 32 || (seen >> (prn[c] - 1) & 1u)) return GPSB200_ERR_ARG;
+        seen |= 1u << (prn[c] - 1);
+    }
     memset(st, 0, sizeof *st);
     st->s0 = s0;
     st->t_f = s0;

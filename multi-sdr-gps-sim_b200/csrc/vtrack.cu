@@ -576,10 +576,13 @@ std::string check(const gpsb200_vtrack_state_t *st, const gpsb200_pvt_chan_t *ch
         if (!std::isfinite(st->x[i])) return "X is not finite";
     for (int i = 0; i < 64; i++)
         if (!std::isfinite(st->P[i])) return "P is not finite";
+    uint32_t seen = 0;   // a repeated PRN would count one satellite's measurements twice and make G singular
     for (int c = 0; c < st->nchan; c++) {
         const gpsb200_vtrack_chan_state_t &cs = st->ch[c];
         const std::string at = "channel " + std::to_string(c) + ": ";
         if (cs.nco.prn < 1 || cs.nco.prn > 32) return at + "PRN outside 1..32";
+        if (seen >> (cs.nco.prn - 1) & 1u) return at + "PRN already on an earlier channel";
+        seen |= 1u << (cs.nco.prn - 1);
         if (chans[c].prn != cs.nco.prn) return at + "chans[c].prn is not the channel's PRN";
         if (!chans[c].eph.valid) return at + "no valid ephemeris";
         if (cs.k < 0 || cs.k > cfg->periods) return at + "k outside 0..periods";

@@ -50,8 +50,10 @@ def seeded(ctx, chans, cfg, st):
     return s
 
 
-def check_model(iq, ss, chans, cfg, st, fixes, outs, eps, st_after):
-    mf, mo, me, mst = V.run(iq, ss, 0, st, chans, cfg, len(fixes) + 1, replay=outs)
+def check_model(iq, ss, chans, cfg, st, fixes, outs, eps, st_after, base=0, max_updates=None):
+    """max_updates: that of a kernel call that stopped by it (None: the call ran to its buffer's end)."""
+    mu = len(fixes) + 1 if max_updates is None else max_updates
+    mf, mo, me, mst = V.run(iq, ss, base, st, chans, cfg, mu, replay=outs)
     assert len(mf) == len(fixes)
     for f in ("sample", "e", "l", "p", "s", "dot", "cross", "prn", "used", "q"):
         assert np.array_equal(mo[f], outs[f]), f
@@ -75,6 +77,52 @@ def check_model(iq, ss, chans, cfg, st, fixes, outs, eps, st_after):
     assert np.abs(mo["rate_res_mps"] - outs["rate_res_mps"]).max() <= 1e-6
     assert np.array_equal(fixes["mask"], [f["mask"] for f in mf])
     assert mst["ch"].tobytes() == st_after["ch"].tobytes()
+    check_fix_fields(fixes, outs, mf, mo, st, mst, st_after)
+
+
+FIX_REFS_MAX = 200        # fixes checked against the 50-digit references per call (evenly spaced)
+
+
+def check_fix_fields(fixes, outs, mf, mo, st, mst, st_after):
+    """The rest of the fix record, the channel records and the state after the call against the model's, and t_rx and
+    the geodetic coordinates against 50-digit references computed from the kernel's own outputs."""
+    from test_vtrack_edges import geodetic_exact, t_rx_exact
+    for f in ("sample", "status", "nused"):
+        assert np.array_equal(fixes[f], [m[f] for m in mf]), f
+    assert (fixes["iterations"] == 1).all()
+    rms = np.array([m["rms"] for m in mf])
+    assert np.array_equal(np.isnan(fixes["rms"]), np.isnan(rms)) and np.array_equal(np.isnan(rms), fixes["nused"] == 0)
+    assert np.nan_to_num(np.abs(fixes["rms"] - rms)).max(initial=0.0) <= 1e-6
+    pdop = np.array([m["pdop"] for m in mf])
+    few = fixes["status"] == gps.FIX_FEW
+    assert np.array_equal(np.isnan(fixes["pdop"]), few) and np.array_equal(np.isnan(pdop), few)
+    # X agrees within 1e-6 m, so the lines of sight differ by ~5e-14 and the inverse of G by its condition number
+    # (about nused PDOP^2) times that: 1e-9 on a good geometry, more on the near-singular ones of a few channels on noise
+    tol = 1e-9 + 1e-12 * fixes["nused"] * np.nan_to_num(pdop) ** 2
+    rel = np.nan_to_num(np.abs(fixes["pdop"] / pdop - 1))
+    assert (rel <= tol).all(), (rel.max(), pdop[np.argmax(rel / tol)], fixes["nused"][np.argmax(rel / tol)])
+    for f in ("sigma_code_m", "sigma_rate_mps"):
+        assert np.array_equal(outs[f], mo[f]), f
+        assert np.array_equal(np.isinf(outs[f]), outs["used"] == 0), f
+    for f in ("t_f", "updates", "seeded"):
+        assert int(st_after[f]) == int(mst[f]), (f, st_after[f], mst[f])
+    assert np.abs(st_after["x"] - mst["x"]).max() <= 1e-6
+    P, Pm = st_after["P"], mst["P"]
+    d = np.sqrt(np.abs(np.diag(Pm)))
+    assert (np.abs(P - Pm) <= 1e-9 * np.outer(d, d)).all(), np.abs(P - Pm).max()
+    for k in np.unique(np.linspace(0, len(fixes) - 1, min(len(fixes), FIX_REFS_MAX)).astype(int)):
+        f = fixes[k]
+        assert abs(f["t_rx"] - t_rx_exact(st, f)) <= 1.2e-10, (k, f["t_rx"] - t_rx_exact(st, f))
+        lat, lon, h = geodetic_exact([f["x"], f["y"], f["z"]])
+        assert abs(f["lat_deg"] - lat) <= 1e-10 and abs(f["lon_deg"] - lon) <= 1e-10 and abs(f["height"] - h) <= 1e-5, k
+
+
+def check_covariance(st):
+    """The filter's P after a long run: symmetric within 1e-9 relative and positive definite (a Cholesky factor)."""
+    P = st["P"]
+    d = np.sqrt(np.diag(P))
+    assert (np.abs(P - P.T) <= 1e-9 * np.outer(d, d)).all()
+    np.linalg.cholesky(P)
 
 
 def test_correlators_and_filter_equal_the_model(ctx, sky12):
@@ -180,10 +228,11 @@ def test_30s_across_the_frame_roll(ctx, tmp_path):
     prns = [int(p) for p in ch[0]["prn"] if p > 0]
     chans = chans_of(tmp_path, 12, prns)
     cfg = gps.vtrack_config()
-    fixes, outs, eps, _ = ctx.vtrack(chans, cfg, state0(prns, cfg), 100000, iq=iq, want_epochs=True)
+    fixes, outs, eps, st = ctx.vtrack(chans, cfg, state0(prns, cfg), 100000, iq=iq, want_epochs=True)
     assert len(fixes) >= 1495
     late = fixes["sample"] >= SETTLE * 3e6
     assert (fixes["nused"][late] == 12).all()
+    check_covariance(st)
     xyz = np.stack([fixes["x"], fixes["y"], fixes["z"]], 1)
     x0 = PM.llh_ecef(*LOC)
     check_truth(ch, prns, eps, xyz, fixes["sample"], lambda s: np.broadcast_to(x0, (s.size, 3)))
@@ -212,8 +261,9 @@ def test_moving_receiver_on_the_circle(ctx, tmp_path):
     cfg = gps.vtrack_config(accel_psd=10.0)
     x_true, v_true = PT.truth_xyz(rows, np.array([0]))
     st = gps.vtrack_seed(cfg, seed_x(x_true[0], v_true[0]), START_SOW, 0, prns)
-    fixes, outs, eps, _ = ctx.vtrack(chans, cfg, st, 100000, iq=iq, sample_size=gps.SC16, want_epochs=True)
+    fixes, outs, eps, st = ctx.vtrack(chans, cfg, st, 100000, iq=iq, sample_size=gps.SC16, want_epochs=True)
     assert len(fixes) >= 2990
+    check_covariance(st)
     late = fixes["sample"] >= SETTLE * 3e6
     assert (fixes["status"][late] == gps.FIX_OK).all()
     xyz = np.stack([fixes["x"], fixes["y"], fixes["z"]], 1)
@@ -299,5 +349,14 @@ def test_bad_arguments_are_refused(ctx, sky12):
         ctx.vtrack(chans, cfg, late, 10, iq=iq[:600000])
     with pytest.raises(gps.GpsB200Error):
         ctx.debug_vtrack_cluster(17)
+    # a repeated PRN: refused by the seed, and in a state edited to hold one
+    with pytest.raises(gps.GpsB200Error):
+        gps.vtrack_seed(cfg, seed_x(PM.llh_ecef(*LOC)), START_SOW, 0, [5, 5, 6, 7])
+    twice = np.array([st], st.dtype)[0]
+    twice["ch"][3]["nco"]["prn"] = twice["ch"][1]["nco"]["prn"]
+    twice_chans = chans.copy()
+    twice_chans[3] = chans[1]
+    with pytest.raises(gps.GpsB200Error):
+        ctx.vtrack(twice_chans, cfg, twice, 10, iq=iq[:600000])
     f, o, _, _ = ctx.vtrack(chans, cfg, st, 10, iq=iq[:600000])
     assert len(f) == 4 and (f["status"] == gps.FIX_OK).all()
